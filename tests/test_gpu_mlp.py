@@ -5,11 +5,19 @@ import networkx as nx
 import pytest
 import torch
 
+import kernel_oracles as ko
 from nn_distributed_training_b200.models import FourierNet
 from nn_distributed_training_b200.parallel.arena import FlatLayout, NodeArena
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _fp32_references():
+    """The fp32 autograd comparisons in this module mean fp32, not TF32."""
+    with ko.fp32_references():
+        yield
 
 
 def _arena(shape, scale, L, seed=0):
@@ -212,3 +220,175 @@ def test_rl_problem_runs_fused_mlp_kernels_on_cuda():
     DiNNOPPO(pr, torch.device(DEV), conf).train()
     for m in pr.models.values():
         assert all(torch.isfinite(p).all() for p in m.parameters())
+
+
+# ---- tensor-core density kernels against the bf16-faithful fp64 oracle ------------------------------------------------
+LOSS_NAME = {"BCELoss": "BCE", "MSELoss": "MSE", "L1Loss": "L1"}
+
+
+def _fused_density(L, B, M, h1=256, loss="BCE", net="fourier", seed=0):
+    """A fused density problem of L nodes with M rows each and a different network per node."""
+    from nn_distributed_training_b200.data.shards import Shard
+    from nn_distributed_training_b200.models.relu_nn import FFReLUNet
+    from nn_distributed_training_b200.problems import DistDensityProblem
+    g = torch.Generator().manual_seed(seed)
+    span = 1200.0 if net == "fourier" else 2.0          # the ReLU net takes normalised coordinates
+    shards = [Shard((torch.rand(M, 2, generator=g) - 0.5) * span, (torch.rand(M, generator=g) < 0.3).float())
+              for _ in range(L)]
+    conf = {"problem_name": "d", "train_batch_size": B, "val_batch_size": 200,
+            "metrics": ["forward_pass_count", "validation_loss", "consensus_error", "current_epoch"],
+            "metrics_config": {"evaluate_frequency": 100}, "optimizer_config": {}}
+    torch.manual_seed(seed)
+    shape = [2, h1, 64, 64, 64, 1]
+    base = FourierNet(shape, scale=0.05) if net == "fourier" else FFReLUNet(shape)
+    lossf = {"BCE": torch.nn.BCELoss(), "MSE": torch.nn.MSELoss(), "L1": torch.nn.L1Loss()}[loss]
+    pr = DistDensityProblem(nx.cycle_graph(L), base, lossf, shards, shards[0], DEV, conf, backend="fused", seed=3)
+    assert pr.backend == "fused"
+    for l in range(L):
+        pr.arena.theta[l] *= 1.0 + 0.03 * l
+    return pr
+
+
+def _oracle(pr, l, call, rounding=True, cache=None):
+    rows = ko.batch_rows(pr.shards.sizes, pr.train_batch_size, pr.seed, l, call, pr.placement.lo).to(DEV)
+    return ko.mlp_bf16_faithful(pr.arena.theta[l], pr.base_model.spec, pr.shards.x[rows], pr.shards.y[rows],
+                                LOSS_NAME[type(pr.base_loss).__name__], rounding=rounding, cache=cache)
+
+
+def _assert_grad_row(got, gf, ge, spec):
+    """Kernel gradient row against the faithful oracle ``gf`` with yardstick ``ge``.  The output-bias gradient
+    mean(dL/dz) is a single number that the bf16 roundings barely touch (for L1 on the ReLU net, or on saturated BCE
+    rows, it is the same number in both oracles), so it has no yardstick error to scale: it is held to fp32 accuracy
+    on its own, every other tensor to the yardstick."""
+    o9 = ko.slots(spec)[9][0]
+    got = got.double().clone()
+    torch.testing.assert_close(got[o9], gf[o9], rtol=1e-4, atol=1e-6)
+    got[o9] = gf[o9]
+    return ko.assert_close_to_oracle(got, gf, ge, ko.MLP_FRAC, spec=spec)
+
+
+def _check_train_step(pr, tag):
+    """One fused compute_grads() of every node against the faithful oracle on the rows it drew: gradient error at most
+    MLP_FRAC x the faithful reference's own error against exact fp64, per tensor and per 16 x 8 block; same loss."""
+    calls = pr.calls.copy()
+    loss = pr.fused.compute_grads().clone()
+    worst = 0.0
+    for l in range(pr.placement.L):
+        lf, gf, _ = _oracle(pr, l, int(calls[l]))
+        ge = _oracle(pr, l, int(calls[l]), rounding=False)[1]
+        rat = _assert_grad_row(pr.arena.grad[l], gf, ge, pr.base_model.spec)
+        worst = max(worst, *(max(v) for v in rat.values()))
+        torch.testing.assert_close(loss[l].double(), lf, rtol=1e-4, atol=1e-6)
+    print(f"\nRATIO mlp_train {tag} call {int(calls[0])}: {worst:.2e}")
+
+
+@pytest.mark.parametrize("h1", [64, 128, 256])
+@pytest.mark.parametrize("L,B", [(4, 12500), (2, 20000)])
+def test_train_kernel_production_partition_matches_oracle(L, B, h1):
+    """dist_online_dense_PAPER's batch sizes: L x ceil(B / 128) tiles exceed the SMs, so a CTA accumulates several
+    tiles (acc_store add), crosses node boundaries (flush + next slot), and in the partial second batch the CTAs whose
+    tiles all lie past its end write zeros (!have_acc)."""
+    pr = _fused_density(L, B, M=B + B // 2 + 1, h1=h1)
+    assert pr.fused.G < L * -(-B // 128)
+    for _ in range(2):
+        _check_train_step(pr, f"L={L} B={B} h1={h1}")
+
+
+@pytest.mark.parametrize("B", [1, 127, 128, 129, 1000])
+def test_train_kernel_any_cta_count_matches_oracle(B):
+    """The static (node, tile) partition over G CTAs, G from one CTA walking every tile of every node to more CTAs
+    than tiles: the summed gradients agree across G up to fp32 reassociation and each matches the oracle.  CTAs never
+    wait on each other, so every G is a valid launch."""
+    L = 3
+    pr = _fused_density(L, B, M=B + B // 2 + 1, h1=128)
+    fz, spec = pr.fused, pr.base_model.spec
+    I = L * -(-B // 128)
+    Gs = sorted({1, 2, 7, I - 1, I, 132} - {0})
+    for call in (0, 1):
+        got = {}
+        for G in Gs:
+            S = -(-G // L) + 1
+            gp = torch.zeros(L, S, fz.n_pad, device=DEV)
+            lp = torch.zeros(L, S, device=DEV)
+            fz.calls.fill_(call)
+            fz.ext.MlpOp(dict(fz.base, train_ctas=G, S=S, grad_part=gp.data_ptr(), loss_part=lp.data_ptr())).train()
+            got[G] = (gp.sum(1), lp.sum(1))
+        for l in range(L):
+            lf, gf, _ = _oracle(pr, l, call)
+            ge = _oracle(pr, l, call, rounding=False)[1]
+            g1 = got[Gs[0]][0][l]
+            for G in Gs:
+                g = got[G][0][l]
+                for o, s in ko.slots(spec):
+                    n = int(torch.tensor(s).prod())
+                    torch.testing.assert_close(g[o: o + n], g1[o: o + n], rtol=1e-5,
+                                               atol=1e-5 * g1[o: o + n].abs().max().item(), msg=f"G={G} slot {o}")
+                _assert_grad_row(g, gf, ge, spec)
+                torch.testing.assert_close(got[G][1][l].double(), lf, rtol=1e-4, atol=1e-6)
+
+
+@pytest.mark.parametrize("L", [1, 3, 8])
+@pytest.mark.parametrize("M", [1, 127, 129, 10000, 50000])
+def test_forward_kernel_matches_faithful_forward(M, L):
+    """MlpForward over M rows: a partial last tile, one row, and more tiles than CTAs (the grid-stride loop).  The
+    output's error against the faithful forward pass, as an RMS over all rows, is at most MLP_FRAC x the faithful
+    pass's own error against exact fp64, and at most 0.5x in every 128-row tile (measured: 0.33 at worst, where one
+    tile holds a few one-ulp bf16 rounding differences; a wrong tile is off by the size of the output).  The yardstick
+    is measured on 8192 rows of the same input distribution, so it does not depend on M."""
+    from nn_distributed_training_b200.ops.mlp_fused import MlpForward
+    arena, _, spec = _arena([2, 256, 64, 64, 64, 1], 0.05, L)
+    g = torch.Generator(device=DEV).manual_seed(M)
+    x = (torch.rand(M, 2, device=DEV, generator=g) - 0.5) * 1500
+    xc = (torch.rand(8192, 2, device=DEV, generator=g) - 0.5) * 1500
+    fwd = MlpForward(arena, spec, L, torch.device(DEV))
+    out = fwd(x).double()
+    worst = 0.0
+    for l in range(L):
+        th = arena.theta[l]
+        pf = ko.mlp_bf16_faithful(th, spec, x, torch.zeros(M, device=DEV), "MSE")[2]
+        cal = (ko.mlp_bf16_faithful(th, spec, xc, xc[:, 0], "MSE", rounding=False)[2]
+               - ko.mlp_bf16_faithful(th, spec, xc, xc[:, 0], "MSE")[2])
+        yard = cal.pow(2).mean().sqrt()
+        tiles = ko._block_errors(out[l] - pf, (128, 1)) / torch.tensor(
+            [min(128, M - 128 * i) for i in range(-(-M // 128))], device=DEV).sqrt()
+        worst = max(worst, (tiles.max() / yard).item())
+        assert (out[l] - pf).pow(2).mean().sqrt() <= ko.MLP_FRAC * yard
+        assert (tiles <= 0.5 * yard).all(), (l, (tiles.max() / yard).item())
+    print(f"\nRATIO mlp_forward M={M} L={L}: {worst:.2e}")
+
+
+@pytest.mark.parametrize("net,loss", [("fourier", "BCE"), ("fourier", "MSE"), ("fourier", "L1"),
+                                      ("relu", "MSE"), ("relu", "L1")])
+def test_train_kernel_specs_and_losses_match_oracle(net, loss):
+    """Every network / loss pair the dispatcher accepts: FourierNet (sin_relu / sigmoid) and FFReLUNet([2, h, 64, 64,
+    64, 1]) (relu / none), over an epoch end with a partial batch."""
+    pr = _fused_density(3, 300, M=451, h1=128, loss=loss, net=net)
+    for _ in range(3):
+        _check_train_step(pr, f"{net}/{loss}")
+
+
+def test_train_kernel_saturated_bce_rows():
+    """Rows whose output pre-activation z lies in [20, 40], where fp32 rounds the sigmoid to 1.  Intended behaviour of
+    the fused kernel: the gradient is that of the exact loss, dL/dz = p - y (so a y = 0 row still pulls z down), and the
+    reported loss is torch's fp32 definition, log clamped at -100.  The torch backend differs on these rows: its fp32
+    autograd returns a zero gradient there (tests/test_kernel_oracles.py::test_saturated_bce_rows_in_fp32_autograd)."""
+    pr = _fused_density(3, 300, M=451, h1=128)
+    o_b4 = ko.slots(pr.base_model.spec)[9][0]
+    pr.arena.theta[:, o_b4] = 30.0
+    for _ in range(2):
+        calls = pr.calls.copy()
+        loss = pr.fused.compute_grads().clone()
+        for l in range(3):
+            cache = {}
+            lf, gf, p = _oracle(pr, l, int(calls[l]), cache=cache)
+            ge = _oracle(pr, l, int(calls[l]), rounding=False)[1]
+            z = torch.logit(p)
+            assert ((z > 20) & (z < 40)).all()
+            _assert_grad_row(pr.arena.grad[l], gf, ge, pr.base_model.spec)
+            rows = ko.batch_rows(pr.shards.sizes, 300, pr.seed, l, int(calls[l]), pr.placement.lo).to(DEV)
+            y = pr.shards.y[rows]
+            p32 = torch.sigmoid(z.float())
+            assert (p32 == 1.0).all()
+            l32 = -(y * torch.log(p32).clamp_min(-100) + (1 - y) * torch.log(1 - p32).clamp_min(-100)).mean()
+            torch.testing.assert_close(loss[l], l32, rtol=1e-5, atol=0)
+            assert lf.item() < 0.5 * l32.item()          # the exact loss is far below the clamped one

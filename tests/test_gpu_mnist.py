@@ -6,6 +6,7 @@ import numpy as np
 import pytest
 import torch
 
+import kernel_oracles as ko
 from nn_distributed_training_b200.data.mnist import synthetic_mnist
 from nn_distributed_training_b200.data.sampler import BatchSchedule
 from nn_distributed_training_b200.models import MNISTConvNet
@@ -15,6 +16,13 @@ from nn_distributed_training_b200.problems.dist_mnist_problem import DistMNISTPr
 pytestmark = pytest.mark.gpu
 DEV = "cuda:0"
 METRICS = ["forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy", "current_epoch"]
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _fp32_references():
+    """The fp32 autograd comparisons in this module mean fp32, not TF32."""
+    with ko.fp32_references():
+        yield
 
 
 def _problem(N, B, backend, opt_conf, M=300, float_inputs=False, seed=0, graph=None, eval_every=1000):
@@ -418,3 +426,57 @@ def test_fp64_cluster_kernel_matches_generic_kernel_and_autograd(B, monkeypatch)
         torch.testing.assert_close(cl.arena.grad, ref.arena.grad, rtol=1e-9, atol=1e-11)
         torch.testing.assert_close(cl.arena.grad, gen.arena.grad, rtol=1e-9, atol=1e-11)
     assert (cl.calls == ref.calls).all()
+
+
+# ---- the cluster kernels at every instantiation the selector launches, against fp64 oracles ---------------------
+def _bench_layout_problem(L, B, dtype):
+    """bench.py's data layout at L nodes: one class per node, uint8 rows normalised in-kernel, a cycle, the paper's
+    net.  A node's shard holds B + B // 2 + 1 rows, so its second draw is a partial batch and its third opens epoch 1."""
+    M = B + B // 2 + 1
+    shards = [synthetic_mnist(M, seed=100 + g, classes=[g % 10]) for g in range(L)]
+    conf = {"problem_name": "t", "train_batch_size": B, "val_batch_size": 64, "metrics": METRICS,
+            "metrics_config": {"evaluate_frequency": 1000},
+            "optimizer_config": {"alg_name": "dsgd", "alpha0": 0.01, "mu": 0.001, "outer_iterations": 2, "profile": False}}
+    torch.manual_seed(0)
+    base = MNISTConvNet(3, 5, 64, dtype=dtype)
+    pr = DistMNISTProblem(nx.cycle_graph(L), base, torch.nn.NLLLoss(), shards, synthetic_mnist(64, seed=1), DEV, conf,
+                          backend="fused", seed=7)
+    for l in range(L):                      # a different network per node, so a node mix-up cannot go unnoticed
+        pr.arena.theta[l] *= 1.0 + 0.03 * l
+    return pr
+
+
+@pytest.mark.parametrize("nsplit,L", [(4, 3), (2, 10), (1, 12)])
+@pytest.mark.parametrize("B", [64, 37, 8])
+@pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
+def test_cluster_kernels_match_fp64_oracle_at_every_instantiation(dtype, B, nsplit, L):
+    """mnist_tc_train_kernel<MS> (fp32) and mnist_cl64_train_kernel<MS> (fp64) at MS = 16, 32, 64 samples per cluster:
+    the batch splits per node the selector picks on a 132-SM H100 for 3, 10 (bench.py) and 12 nodes.  The oracle is
+    float64 autograd on the rows the kernel drew.  fp64: agreement to 1e-9.  fp32 (3xTF32): the error is at most 0.1x
+    that of a 1xTF32 emulation of the three fc1-sized contractions, per tensor and per 16 x 8 block."""
+    if torch.cuda.get_device_properties(DEV).multi_processor_count != 132:
+        pytest.skip("node counts chosen for the 132 SMs of an H100 SXM")
+    pr = _bench_layout_problem(L, B, dtype)
+    fz, spec = pr.fused, pr.base_model.spec
+    assert (fz.cl64 if dtype == torch.float64 else fz.tc) and fz.S == nsplit
+    assert f"_train_kernel<{64 // nsplit}>" in fz.kernel_name
+    mean, std = pr.shards.norm
+    worst = {}
+    for step in range(3):                   # full batch, partial batch, first batch of the next epoch
+        calls = pr.calls.copy()
+        loss = fz.compute_grads().clone()
+        for l in range(L):
+            rows = ko.batch_rows(pr.shards.sizes, B, pr.seed, l, int(calls[l]), pr.placement.lo).to(DEV)
+            x, y, th = pr.shards.x[rows], pr.shards.y[rows], pr.arena.theta[l]
+            lr, gr = ko.convnet_fp64(th, spec, x, y, mean, std)
+            if dtype == torch.float64:
+                torch.testing.assert_close(loss[l], lr, rtol=1e-6, atol=1e-7)       # loss partials are stored as float
+                torch.testing.assert_close(pr.arena.grad[l], gr, rtol=1e-9, atol=1e-11)
+                continue
+            gt = ko.convnet_fp64(th, spec, x, y, mean, std, tf32_fc1=True)[1]
+            assert abs(loss[l].item() - lr.item()) <= 1e-5 * abs(lr.item()), (l, step, loss[l].item(), lr.item())
+            rat = ko.assert_close_to_oracle(pr.arena.grad[l].double(), gr, gt, ko.CONVNET_FRAC, spec=spec)
+            for k, v in rat.items():
+                worst[k] = max(worst.get(k, 0.0), *v)
+    if worst:
+        print(f"\nRATIO mnist_tc<{64 // nsplit}> B={B}: " + " ".join(f"{k}={v:.2e}" for k, v in worst.items()))
