@@ -99,6 +99,19 @@ NNDT_DEVINL void mbarrier_wait_parity(uint64_t* bar, uint32_t parity) {
   } while (!done);
 }
 
+// ---- thread-block clusters: barrier, rank, and fp64 distributed-shared-memory access -----------------------------
+NNDT_DEVINL void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+NNDT_DEVINL uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
+NNDT_DEVINL uint32_t map_to(const void* p, uint32_t rank) {
+  uint32_t r;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
+  return r;
+}
+NNDT_DEVINL double ld_dsmem(uint32_t a) { double v; asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory"); return v; }
+NNDT_DEVINL void st_dsmem(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+
 // cp.async helpers (LDGSTS)
 NNDT_DEVINL void cp_async16(void* smem, const void* gmem) {
   uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);

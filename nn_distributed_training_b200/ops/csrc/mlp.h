@@ -1,4 +1,4 @@
-// Launch interface of the tensor-core MLP kernels (mlp_tc.cu): networks of the form
+// Launch interface of the tensor-core MLP kernels (mlp_tc.cu: bf16, mlp_f64.cu: fp64): networks of the form
 //   d_in (<= 4) -> H1 (64|128|256) -> 64 -> 64 -> 64 -> 1
 // i.e. the reference's FourierNet [2,256,64,64,64,1] (models/fourier_nn.py:43-59) and ReLU MLPs
 // of the same shape family (models/relu_nn.py:4-41).
@@ -20,6 +20,7 @@ struct Args {
   int d_in, h1;
   int first_act, last_act, loss;
   float scale;
+  double scale64;       // the SIREN scale in full precision (fp64 kernels)
   // data: x [M, d_in] fp32 (or fp64 converted by the caller), y [M] fp32
   const float* x;
   const float* y;
@@ -37,6 +38,14 @@ struct Args {
 
 cudaError_t launch_forward(const Args& a, int ctas_per_node, cudaStream_t st);
 cudaError_t launch_train(const Args& a, int ctas, cudaStream_t st);
+
+// float64 kernels (mlp_f64.cu): DMMA tiles on 2-CTA clusters.  With them every pointer of Args except the index
+// arrays (shard_off, shard_len, calls, win_table) addresses doubles: theta, x, y, out, grad_part and loss_part.
+// Widths count clusters: `clusters_per_node` for the forward kernel, `clusters` for the training kernel, whose
+// CTA 2 c + r of cluster c owns slot 2 (c - first cluster of the node) + r, so S >= 2 (clusters per node + 1).
+cudaError_t launch_forward_f64(const Args& a, int clusters_per_node, cudaStream_t st);
+cudaError_t launch_train_f64(const Args& a, int clusters, cudaStream_t st);
+int f64_max_active_clusters(int h1);   // co-resident clusters of the training kernel (0: not launchable)
 
 }  // namespace mlp
 }  // namespace nndt

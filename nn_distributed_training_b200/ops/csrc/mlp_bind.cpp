@@ -1,4 +1,4 @@
-// Bindings of the tensor-core MLP kernels (mlp_tc.cu).
+// Bindings of the tensor-core MLP kernels (mlp_tc.cu, mlp_f64.cu).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <pybind11/pybind11.h>
@@ -22,9 +22,11 @@ void check(cudaError_t e, const char* what) {
   if (e != cudaSuccess) throw std::runtime_error(std::string(what) + ": " + cudaGetErrorString(e));
 }
 
+// With dtype64 the float64 kernels (mlp_f64.cu) run: every data pointer addresses doubles, and fwd_ctas / train_ctas
+// count 2-CTA clusters.
 struct MlpOp {
   mlp::Args a{};
-  int fwd_ctas = 1, train_ctas = 1;
+  int fwd_ctas = 1, train_ctas = 1, dtype64 = 0;
   explicit MlpOp(const py::dict& d) { update(d); }
   void update(const py::dict& d) {
     a.theta = ptr<const float>(d, "theta"); a.n_pad = geti(d, "n_pad"); a.L = geti(d, "L");
@@ -33,6 +35,8 @@ struct MlpOp {
     a.d_in = geti(d, "d_in"); a.h1 = geti(d, "h1");
     a.first_act = geti(d, "first_act"); a.last_act = geti(d, "last_act"); a.loss = geti(d, "loss");
     a.scale = (float)getf(d, "scale", 1.0);
+    a.scale64 = getf(d, "scale", 1.0);
+    dtype64 = geti(d, "dtype64");
     a.x = ptr<const float>(d, "x"); a.y = ptr<const float>(d, "y");
     a.n_rows = geti(d, "n_rows"); a.out = ptr<float>(d, "out");
     a.direct = geti(d, "direct"); a.batch = geti(d, "batch"); a.seed = geti(d, "seed"); a.node0 = geti(d, "node0");
@@ -41,8 +45,14 @@ struct MlpOp {
     a.grad_part = ptr<float>(d, "grad_part"); a.loss_part = ptr<float>(d, "loss_part"); a.S = geti(d, "S", 1);
     fwd_ctas = geti(d, "fwd_ctas", 1); train_ctas = geti(d, "train_ctas", 1);
   }
-  void forward() { check(mlp::launch_forward(a, fwd_ctas, at::cuda::getCurrentCUDAStream().stream()), "mlp_forward"); }
-  void train() { check(mlp::launch_train(a, train_ctas, at::cuda::getCurrentCUDAStream().stream()), "mlp_train"); }
+  void forward() {
+    cudaStream_t st = at::cuda::getCurrentCUDAStream().stream();
+    check(dtype64 ? mlp::launch_forward_f64(a, fwd_ctas, st) : mlp::launch_forward(a, fwd_ctas, st), "mlp_forward");
+  }
+  void train() {
+    cudaStream_t st = at::cuda::getCurrentCUDAStream().stream();
+    check(dtype64 ? mlp::launch_train_f64(a, train_ctas, st) : mlp::launch_train(a, train_ctas, st), "mlp_train");
+  }
 };
 }  // namespace
 
@@ -94,6 +104,7 @@ void bind_mlp(py::module& m) {
     check(lidar::launch_density(lidar_args(d), reinterpret_cast<const double*>(xy), n, reinterpret_cast<double*>(out),
                                 at::cuda::getCurrentCUDAStream().stream()), "lidar_density");
   });
+  m.def("mlp_f64_max_clusters", [](int h1) { return mlp::f64_max_active_clusters(h1); });
   py::class_<MlpOp>(m, "MlpOp")
       .def(py::init<const py::dict&>())
       .def("update", &MlpOp::update)

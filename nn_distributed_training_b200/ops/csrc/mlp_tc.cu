@@ -272,8 +272,6 @@ cudaError_t launch_forward(const Args& a, int ctas_per_node, cudaStream_t st) {
 // The weight gradients of a tile are added into this CTA's partial row of the node (the first tile stores); every
 // element is owned by one thread, so the read-modify-write needs no atomics.
 // =====================================================================================
-constexpr int kWinMax = 64;                           // max windows per period of the online stream
-constexpr int kWinTableLen = 2 + (kWinMax + 1) + 2 * kWinMax;
 constexpr int NTT = 512;       // training CTA: 16 warps = 8 row blocks of 16 x 2 column halves of 32
 
 template <int H1>
@@ -355,10 +353,8 @@ __global__ void __launch_bounds__(NTT, 1) mlp_train_kernel(const Args a) {
   bool have_acc = false; // this CTA's partial row of node `cur` holds the gradients of at least one tile
   float* gp = nullptr;   // that partial row
   int slot = 0;
-  uint32_t bs = 0, start = 0, key = 0, m = 0;
-  int shard_off = 0;
-  long long first_draw = 0;            // online sliding-window mode: index of the batch's first draw
-  const long long* wt = nullptr;       // [K, P, cum[0..KMAX], lb[KMAX], ub[KMAX]] of the current node
+  uint32_t bs = 0;
+  NodeStream ns{};                     // the current node's batch draws (unless direct)
   auto wk = [](const uint8_t* w) { return [w](int k, int n) { return ld_k(w, W_SLAB, n, k); }; };
   auto hk = [](const uint8_t* h) { return [h](int mm, int k) { return ld_k(h, ACT_SLAB, mm, k); }; };
 
@@ -397,15 +393,11 @@ __global__ void __launch_bounds__(NTT, 1) mlp_train_kernel(const Args a) {
       if (a.direct) {
         bs = (uint32_t)a.batch;
       } else {
-        m = (uint32_t)a.shard_len[l];
-        shard_off = a.shard_off[l];
-        const BatchLoc loc = locate_batch((uint32_t)a.calls[l], m, (uint32_t)a.batch);
-        bs = loc.size; start = loc.start;
-        key = mix_key((uint32_t)a.seed, (uint32_t)(a.node0 + l), loc.epoch);
-        if (a.win_table != nullptr) {
-          wt = reinterpret_cast<const long long*>(a.win_table) + (size_t)l * kWinTableLen;
-          first_draw = (long long)loc.epoch * m + loc.start;
-        }
+        const long long* wt = a.win_table != nullptr
+                                  ? reinterpret_cast<const long long*>(a.win_table) + (size_t)l * kWinTableLen : nullptr;
+        ns = node_stream((uint32_t)a.calls[l], (uint32_t)a.shard_len[l], (uint32_t)a.batch, (uint32_t)a.seed,
+                         (uint32_t)(a.node0 + l), a.shard_off[l], wt);
+        bs = ns.size;
       }
       __syncthreads();
     }
@@ -419,20 +411,7 @@ __global__ void __launch_bounds__(NTT, 1) mlp_train_kernel(const Args a) {
       int my_idx = -1;
       const uint32_t tt = t0 + tid;
       if (tt < bs) {
-        if (a.direct) {
-          my_idx = (int)(l * a.batch + tt);
-        } else if (wt != nullptr) {
-          // sliding window stream (floorplans/lidar/lidar.py:397-424 as index arithmetic)
-          const long long K = wt[0], P = wt[1];
-          const long long d = first_draw + tt, q = d / P, r = d - q * P;
-          int w = 0;
-          while (w + 1 < K && wt[2 + w + 1] <= r) ++w;
-          const long long lb = wt[2 + kWinMax + 1 + w], ub = wt[2 + kWinMax + 1 + kWinMax + w];
-          const uint32_t wkey = mix_key((uint32_t)a.seed, (uint32_t)(a.node0 + l), (uint32_t)(q * K + w));
-          my_idx = shard_off + (int)lb + (int)feistel_permute((uint32_t)(r - wt[2 + w]), (uint32_t)(ub - lb), wkey);
-        } else {
-          my_idx = shard_off + (int)feistel_permute(start + tt, m, key);
-        }
+        my_idx = a.direct ? (int)(l * a.batch + tt) : stream_row(ns, tt);
       }
       sm.ridx[tid] = my_idx;
       sm.ys[tid] = my_idx >= 0 ? a.y[my_idx] : 0.f;

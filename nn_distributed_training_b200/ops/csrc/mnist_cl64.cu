@@ -47,17 +47,6 @@ struct Smem {
 static_assert(sizeof(Smem) <= 227 * 1024, "shared memory budget");
 static_assert(6 * 80 <= 11 * 64, "conv shares fit h_loc");
 
-NNDT_DEVINL void cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-NNDT_DEVINL uint32_t cluster_rank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-NNDT_DEVINL uint32_t map_to(const void* p, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"((uint32_t)__cvta_generic_to_shared(p)), "r"(rank));
-  return r;
-}
-NNDT_DEVINL double ld_dsmem(uint32_t a) { double v; asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory"); return v; }
-NNDT_DEVINL void st_dsmem(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
 NNDT_DEVINL double wsum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

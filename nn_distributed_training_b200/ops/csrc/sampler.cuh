@@ -53,4 +53,44 @@ NNDT_DEVINL BatchLoc locate_batch(uint32_t call, uint32_t m, uint32_t B) {
   return o;
 }
 
+// ---- the draws of one node's batch, as the density training kernels (mlp_tc.cu, mlp_f64.cu) make them -----------
+// Online problems pass a per-node table of one period of the sliding-window stream
+// (data.sampler.OnlineWindowSchedule, built by ops/mlp_fused.py): [K, P, cum[0..kWinMax], lb[kWinMax], ub[kWinMax]].
+constexpr int kWinMax = 64;                           // max windows per period of the online stream
+constexpr int kWinTableLen = 2 + (kWinMax + 1) + 2 * kWinMax;
+
+struct NodeStream {
+  uint32_t size, start, m, key, seed, node;
+  int shard_off;
+  long long first_draw;     // window mode: index of the batch's first draw
+  const long long* wt;      // window table of the node, or nullptr: plain epoch sampling
+};
+
+NNDT_DEVINL NodeStream node_stream(uint32_t call, uint32_t m, uint32_t B, uint32_t seed, uint32_t node, int shard_off,
+                                   const long long* wt) {
+  const BatchLoc loc = locate_batch(call, m, B);
+  NodeStream s;
+  s.size = loc.size; s.start = loc.start; s.m = m; s.seed = seed; s.node = node; s.shard_off = shard_off;
+  s.key = mix_key(seed, node, loc.epoch);
+  s.first_draw = (long long)loc.epoch * m + loc.start;
+  s.wt = wt;
+  return s;
+}
+
+// row of the concatenated shards drawn at position tt (< s.size) of the batch
+NNDT_DEVINL int stream_row(const NodeStream& s, uint32_t tt) {
+  if (s.wt != nullptr) {
+    // sliding window stream (floorplans/lidar/lidar.py:397-424 as index arithmetic)
+    const long long* wt = s.wt;
+    const long long K = wt[0], P = wt[1];
+    const long long d = s.first_draw + tt, q = d / P, r = d - q * P;
+    int w = 0;
+    while (w + 1 < K && wt[2 + w + 1] <= r) ++w;
+    const long long lb = wt[2 + kWinMax + 1 + w], ub = wt[2 + kWinMax + 1 + kWinMax + w];
+    const uint32_t wkey = mix_key(s.seed, s.node, (uint32_t)(q * K + w));
+    return s.shard_off + (int)lb + (int)feistel_permute((uint32_t)(r - wt[2 + w]), (uint32_t)(ub - lb), wkey);
+  }
+  return s.shard_off + (int)feistel_permute(s.start + tt, s.m, s.key);
+}
+
 }  // namespace nndt

@@ -1,4 +1,5 @@
-"""Python side of the tensor-core MLP kernels (csrc/mlp_tc.cu)."""
+"""Python side of the tensor-core MLP kernels: csrc/mlp_tc.cu (float32 arm: bf16 operands, fp32 accumulation) and
+csrc/mlp_f64.cu (float64 arm: fp64 DMMA tiles on 2-CTA clusters)."""
 from __future__ import annotations
 
 import numpy as np
@@ -19,16 +20,30 @@ def shape_supported(spec: MLPSpec) -> bool:
             and spec.first in FIRST and spec.hidden == "relu" and spec.last in LAST)
 
 
-def supports(spec: MLPSpec, base_loss) -> bool:
-    return (TRAIN_KERNEL_READY and shape_supported(spec) and type(base_loss).__name__ in LOSS
-            and getattr(base_loss, "reduction", "mean") == "mean")
+def supports(spec: MLPSpec, base_loss, dtype=torch.float32) -> bool:
+    return (TRAIN_KERNEL_READY and dtype in (torch.float32, torch.float64) and shape_supported(spec)
+            and type(base_loss).__name__ in LOSS and getattr(base_loss, "reduction", "mean") == "mean")
+
+
+F64_TILE = 32      # rows of a cluster tile of the float64 kernels
+
+
+def f64_max_clusters(ext, h1: int) -> int:
+    """Co-resident 2-CTA clusters of the float64 training kernel; an error if it cannot launch at all."""
+    n = ext.mlp_f64_max_clusters(h1)
+    if n < 1:
+        raise RuntimeError(f"the float64 MLP kernel (h1={h1}) cannot be launched on this device")
+    return n
 
 
 def op_dict(arena, spec: MLPSpec, L: int):
     off = [s.offset for s in arena.layout.slots]
     assert len(off) == 10
+    if arena.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"no fused MLP kernel for {arena.dtype}")
     return dict(theta=arena.theta.data_ptr(), n_pad=arena.n_pad, L=L, off=off, d_in=spec.shape[0], h1=spec.shape[1],
-                first_act=FIRST[spec.first], last_act=LAST[spec.last], scale=float(spec.scale))
+                first_act=FIRST[spec.first], last_act=LAST[spec.last], scale=float(spec.scale),
+                dtype64=int(arena.dtype == torch.float64))
 
 
 class MlpForward:
@@ -37,15 +52,21 @@ class MlpForward:
     def __init__(self, arena, spec: MLPSpec, L: int, device):
         self.ext = load_ext(required=True)
         self.arena, self.spec, self.L, self.device = arena, spec, L, device
+        self.dtype = arena.dtype
         self.sms = torch.cuda.get_device_properties(device).multi_processor_count
+        if self.dtype == torch.float64:
+            self.max_clusters = f64_max_clusters(self.ext, spec.shape[1])
         self._cache = {}
 
     def __call__(self, x: torch.Tensor) -> torch.Tensor:
-        x = x.to(torch.float32).contiguous()
+        x = x.to(self.dtype).contiguous()
         M = x.shape[0]
-        out = torch.empty(self.L, M, dtype=torch.float32, device=self.device)
+        out = torch.empty(self.L, M, dtype=self.dtype, device=self.device)
         d = op_dict(self.arena, self.spec, self.L)
-        ctas = max(1, min(-(-M // 128), max(1, (2 * self.sms) // max(1, self.L))))
+        if self.dtype == torch.float64:      # 2-CTA clusters per node: one wave over all nodes
+            ctas = max(1, min(-(-M // F64_TILE), self.max_clusters // max(1, self.L)))
+        else:
+            ctas = max(1, min(-(-M // 128), max(1, (2 * self.sms) // max(1, self.L))))
         d.update(x=x.data_ptr(), n_rows=M, out=out.data_ptr(), fwd_ctas=ctas)
         op = self.ext.MlpOp(d)
         op.forward()
@@ -65,18 +86,25 @@ class FusedMLP:
         a, pl = problem.arena, problem.placement
         self.spec = problem.base_model.spec
         self.L, self.n_pad, self.B = pl.L, a.n_pad, problem.train_batch_size
+        self.dtype = a.dtype
         self.sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        tmax = -(-self.B // 128)
-        self.G = max(1, min(self.sms, self.L * tmax))
-        self.S = -(-self.G // self.L) + 1
+        if self.dtype == torch.float64:
+            # G 2-CTA clusters over the L x ceil(B / 32) tiles; each CTA of a cluster owns one partial row
+            tmax = -(-self.B // F64_TILE)
+            self.G = max(1, min(f64_max_clusters(self.ext, self.spec.shape[1]), self.L * tmax))
+            self.S = 2 * (-(-self.G // self.L) + 1)
+        else:
+            tmax = -(-self.B // 128)
+            self.G = max(1, min(self.sms, self.L * tmax))
+            self.S = -(-self.G // self.L) + 1
         sh = problem.shards
-        self.x = sh.x.to(torch.float32).contiguous()
-        self.y = sh.y.to(torch.float32).contiguous()
+        self.x = sh.x.to(self.dtype).contiguous()
+        self.y = sh.y.to(self.dtype).contiguous()
         self.shard_off = torch.tensor(sh.offsets[:-1], dtype=torch.int32, device=dev)
         self.shard_len = torch.tensor(sh.sizes, dtype=torch.int32, device=dev)
         self.calls = torch.zeros(self.L, dtype=torch.int32, device=dev)
-        self.grad_part = torch.zeros(self.L, self.S, self.n_pad, dtype=torch.float32, device=dev)
-        self.loss_part = torch.zeros(self.L, self.S, dtype=torch.float32, device=dev)
+        self.grad_part = torch.zeros(self.L, self.S, self.n_pad, dtype=self.dtype, device=dev)
+        self.loss_part = torch.zeros(self.L, self.S, dtype=self.dtype, device=dev)
         self.win_table = self._window_table()
         d = op_dict(a, self.spec, self.L)
         d.update(win_table=None if self.win_table is None else self.win_table.data_ptr())

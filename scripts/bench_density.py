@@ -1,6 +1,7 @@
 """Secondary benchmark: dist_online_dense_PAPER-shaped DiNNO (FourierNet [2,256,64,64,64,1],
 7 robots, batch 12 500, 5 primal steps/round) on a procedural floor plan.
-Prints one JSON line with rounds/s for the fused tensor-core path and the PyTorch-eager path."""
+Prints one JSON line with rounds/s for the fused tensor-core path and the PyTorch-eager path.
+DTYPE=float64 runs both paths in float64 (the reference's precision); the default is float32."""
 import glob, json, os, sys, tempfile, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -12,6 +13,7 @@ from nn_distributed_training_b200.optimizers import DiNNO
 from nn_distributed_training_b200.problems import DistOnlineDensityProblem
 
 N = int(os.environ.get("NODES", 7)); B = int(os.environ.get("BATCH", 12500)); PITS = 5
+DTYPE = {"float32": torch.float32, "float64": torch.float64}[os.environ.get("DTYPE", "float32")]
 K = int(sys.argv[1]) if len(sys.argv) > 1 else 50
 tmp = tempfile.mkdtemp()
 write_dataset(tmp, n_paths=N, seed=0)
@@ -30,8 +32,9 @@ for backend in ("fused", "torch"):
             "save_models": False, "metrics": ["validation_loss", "train_loss_moving_average"],
             "metrics_config": {"evaluate_frequency": 10 ** 9, "tloss_decay": 0.2, "mesh_only_at_end": True}, "optimizer_config": oc}
     torch.manual_seed(0)
-    pr = DistOnlineDensityProblem(FourierNet([2, 256, 64, 64, 64, 1], 0.05), torch.nn.BCELoss(), train, val, "cuda:0", conf,
+    pr = DistOnlineDensityProblem(FourierNet([2, 256, 64, 64, 64, 1], 0.05, dtype=DTYPE), torch.nn.BCELoss(), train, val, "cuda:0", conf,
                                   backend=backend, seed=0)
+    assert pr.backend == backend
     opt = DiNNO(pr, "cuda:0", dict(oc, consensus_backend="auto" if backend == "fused" else "torch"))
     k = K if backend == "fused" else max(3, K // 10)
     opt.run_rounds(5); opt.run_rounds(k)       # warm-up incl. graph capture of this chunk size
@@ -43,4 +46,4 @@ for backend in ("fused", "torch"):
     flop = N * PITS * B * 150e3
     out[backend] = {"ms_per_round": ms, "rounds_per_s": 1e3 / ms, "val_loss": pr.metrics["validation_loss"][-1].mean().item(),
                     "model_tflops": flop / (ms * 1e-3) / 1e12}
-print(json.dumps({"workload": "dist_online_dense DiNNO", "nodes": N, "batch": B, "primal_iterations": PITS, **out}))
+print(json.dumps({"workload": "dist_online_dense DiNNO", "dtype": str(DTYPE).replace("torch.", ""), "nodes": N, "batch": B, "primal_iterations": PITS, **out}))
