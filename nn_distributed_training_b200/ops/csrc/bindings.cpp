@@ -205,7 +205,8 @@ PYBIND11_MODULE(_C, m) {
     return py::bytes(reinterpret_cast<const char*>(buf), 128);
   });
   m.def("mnist_tc_max_clusters", []() { return mnist::tc_max_active_clusters(); });
-  m.def("mnist_cl64_max_clusters", []() { return mnist::cl64_max_active_clusters(); });
+  m.def("mnist_cl64_max_clusters", [](int nsplit) { return mnist::cl64_max_active_clusters(nsplit); }, py::arg("nsplit") = 1);
+  m.def("mnist_cl64_cluster_ctas", []() { return mnist::cl64_cluster_ctas(); });
   m.def("rank_barrier", [](uint64_t slots, uint64_t peer_slot, int world, int rank, int epoch, uint64_t gate, uint64_t err) {
     check(consensus::launch_rank_barrier(reinterpret_cast<int*>(slots), reinterpret_cast<const int64_t*>(peer_slot), world, rank,
                                          epoch, reinterpret_cast<const volatile int*>(gate), reinterpret_cast<int*>(err), cur_stream()),

@@ -112,6 +112,41 @@ NNDT_DEVINL uint32_t map_to(const void* p, uint32_t rank) {
 NNDT_DEVINL double ld_dsmem(uint32_t a) { double v; asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory"); return v; }
 NNDT_DEVINL void st_dsmem(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
 
+// ---- FP64 tensor-core tiles (DMMA) ------------------------------------------------------------------------------
+// m16n8k4 fragments (g = lane >> 2, t = lane & 3): A a0 (g, t), a1 (g + 8, t); B b0 (t, g);
+// C c0 (g, 2t), c1 (g, 2t + 1), c2 (g + 8, 2t), c3 (g + 8, 2t + 1).
+NNDT_DEVINL void dmma(double (&c)[4], double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a0), "d"(a1), "d"(b));
+}
+
+// c[j] += sum_k A(m0 + ., k) B(k, n0 + 8 j + .) over k < K (a multiple of 4)
+template <int NJ, class FA, class FB>
+NNDT_DEVINL void gemm(double (&c)[NJ][4], int m0, int n0, int K, int lane, FA A, FB B) {
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll 4
+  for (int k0 = 0; k0 < K; k0 += 4) {
+    const int k = k0 + t;
+    const double a0 = A(m0 + g, k), a1 = A(m0 + g + 8, k);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) dmma(c[j], a0, a1, B(k, n0 + 8 * j + g));
+  }
+}
+
+template <int NJ>
+NNDT_DEVINL void zero(double (&c)[NJ][4]) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) c[j][0] = c[j][1] = c[j][2] = c[j][3] = 0.0;
+}
+// row / column of accumulator element i of the 16 x 8 tile at (m0, n0)
+NNDT_DEVINL int frow(int m0, int lane, int i) { return m0 + (lane >> 2) + 8 * (i >> 1); }
+NNDT_DEVINL int fcol(int n0, int lane, int i) { return n0 + 2 * (lane & 3) + (i & 1); }
+
+// operand readers: at(s, ld)(i, j) = s[i][j], at_t(s, ld)(i, j) = s[j][i] of a row-major array with row stride ld
+NNDT_DEVINL auto at(const double* s, int ld) { return [s, ld](int i, int j) { return s[i * ld + j]; }; }
+NNDT_DEVINL auto at_t(const double* s, int ld) { return [s, ld](int i, int j) { return s[j * ld + i]; }; }
+
 // cp.async helpers (LDGSTS)
 NNDT_DEVINL void cp_async16(void* smem, const void* gmem) {
   uint32_t s = (uint32_t)__cvta_generic_to_shared(smem);

@@ -63,9 +63,11 @@ cudaError_t launch_generic_eval(const Args& a, const GenericShape& gs, int ctas_
 cudaError_t make_w1_tensor_map(const float* theta, int n_pad, int L, int off_w1, void* out_map128);
 cudaError_t launch_train_tc(const Args& a, const void* w1_map128, int nsplit, cudaStream_t st);
 int tc_max_active_clusters();
-// float64 twin of the K-split cluster kernel on the fp64 CUDA cores (mnist_cl64.cu); Args pointers address doubles
+// float64 K-split cluster kernel of the paper shape on the FP64 tensor cores (mnist_cl64.cu): nsplit clusters of
+// cl64_cluster_ctas() CTAs per node, one gradient row per cluster; Args pointers address doubles
 cudaError_t launch_train_cl64(const Args& a, const GenericShape& gs, int nsplit, cudaStream_t st);
-int cl64_max_active_clusters();
+int cl64_max_active_clusters(int nsplit);
+int cl64_cluster_ctas();
 cudaError_t launch_gather(const GatherArgs& a, cudaStream_t st);
 cudaError_t launch_train(const Args& a, int spb, int S, cudaStream_t st);
 cudaError_t launch_eval(const Args& a, int ctas_per_node, cudaStream_t st);

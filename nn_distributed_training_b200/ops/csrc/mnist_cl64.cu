@@ -1,18 +1,21 @@
-// float64 training kernel of the paper's MNISTConvNet(3, 5, 64) at batch <= 64: the K-split thread-block-cluster
-// decomposition of mnist_tc.cu with the contractions on the fp64 CUDA cores (fp64 operands would need the DMMA
-// tensor-core path and its fragment layouts for the same K-split; the vector DFMA units carry it here).  This is the kernel behind the framework's float64 arm — the
+// float64 training kernel of the paper's MNISTConvNet(3, 5, 64) at batch <= 64: a K-split thread-block-cluster
+// decomposition with the three fc1-sized contractions on the FP64 tensor cores (mma.sync m16n8k4, DMMA, fp64
+// accumulation) and the conv layer on the fp64 CUDA cores.  This is the kernel behind the framework's float64 arm — the
 // precision the reference runs end to end (experiments/dist_mnist_ex.py:19) — and replaces the batch-split generic
 // kernel (mnist_generic.cu) there, which streams the 221 KB fp64 W1 matrix three times per CTA.
 //
-// A node is `nsplit` clusters of 6 CTAs (MS = 64 / nsplit samples each); CTA c owns pooled rows {2c, 2c+1} of all three
-// channels = 72 of the 432 fc1 inputs for all MS samples: conv+ReLU+pool -> A_c [MS x 72]; H_c = A_c . W1_c^T reduced
-// over the cluster through distributed shared memory (reduce-scatter by samples, fc2 / loss / backward on the owners, dH
-// rows gathered back); da1_c = dH . W1_c and dW1_c = dH^T . A_c are local; dW1_c goes straight to its columns of the
-// gradient row; small gradients are reduced by rank 0 through DSMEM.  One gradient partial row per cluster.
-// GEMM tiling: a thread owns 2 rows x 4-5 strided columns; with rows padded to 73 / 65 doubles every operand read is
-// either a broadcast or conflict free, so the loops run at the DFMA rate.
-#include <type_traits>
-
+// A node is `nsplit` clusters of 4 CTAs (MS = 64 / nsplit samples each); CTA c owns pooled rows {3c, 3c+1, 3c+2} of all
+// three channels = 108 of the 432 fc1 inputs for all MS samples (image rows 6c .. 6c+9): conv+ReLU+pool -> A_c [MS x 108];
+// H_c = A_c . W1_c^T reduced over the cluster through distributed shared memory (reduce-scatter by samples, MS / 4 per
+// CTA; fc2 / loss / backward on the owners, dH rows gathered back); da1_c = dH . W1_c and dW1_c = dH^T . A_c are local;
+// dW1_c goes straight to its columns of the gradient row; small gradients are reduced through DSMEM.  One gradient
+// partial row per cluster.
+// Why 4 CTAs: a cluster must sit inside one GPC and a CTA fills its SM (shared memory and registers), so a GPC of n SMs
+// holds floor(n / CL) clusters.  On an H100 SXM (132 SMs) only 17 six-CTA clusters fit at once, and the 20 clusters of
+// 10 nodes x 2 batch splits ran in two waves; 4-CTA clusters keep every node count up to 12 in one wave.
+// Row strides are 4 mod 16 doubles (116, 68), so DMMA fragment reads, row-wise or transposed, are free of bank
+// conflicts.  Every sum runs in a fixed order and nothing is added atomically: two launches on the same inputs give
+// bitwise-equal gradients and losses.
 #include "mnist_device.cuh"
 
 namespace nndt {
@@ -20,38 +23,38 @@ namespace mnist {
 
 namespace cl64 {
 
-constexpr int NT = 512, CL = 6, CELLS = 24, KC = 72, WS = 73, HS = 65;
+constexpr int NT = 512, CL = 4, CELLS = 36, KC = 108, WS = 116, HS = 68;
+constexpr int PXR = 10 * HW;                  // image rows 6c .. 6c+9 of a sample: 280 pixels
+constexpr int KT = (KC + 7) / 8;              // 8-column tiles over a CTA's fc1 inputs; columns 108..111 fall in the row padding
 constexpr int PART_WC = 0, PART_BC = 75, PART_B1 = 78, PART_W2 = 142, PART_B2 = 782, PART_LOSS = 792, PART_N = 793;
 
+template <int MS>
 struct Smem {
-  double w[64 * WS];         // W1 slice [j][k], k = ch * 24 + cell; later da1 [s][72]
-  double a[64 * WS];         // A tile [s][k]; later (with dh) the scratch of the conv-grad reduction
-  double dh[64 * HS];        // dH [s][j]; before that, split-K partial sums of GEMM 1
-  double hpart[64 * HS];     // partial H [s][j] (read by the peers); later split-K partial sums of GEMM 2
-  alignas(16) unsigned char img[64 * 224 * 4];   // image rows 4c .. 4c+7: MS <= 32: normalised doubles [MS][224]; MS = 64: raw floats
-  double h_loc[11 * 64];     // later (rank 0) the six CTAs' conv-gradient shares [6][80]
-  double dh_loc[11 * 64];
+  static constexpr int NO = MS / CL;           // samples a CTA owns for fc2, the loss and their backward
+  static constexpr bool kDoublePix = MS <= 32; // pixels as normalised doubles; at MS = 64 they only fit as raw bytes
+  double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; later da1 [s][KC]
+  double a[MS * WS];         // A tile [s][k]; later the conv-grad warp sums
+  double h[MS * HS];         // partial H [s][j] (read by the peers); after barrier #2 dH [s][j]; later the conv-grad lists
+  alignas(16) unsigned char img[kDoublePix ? MS * PXR * 8 : MS * PXR];
+  double lut[kDoublePix ? 1 : 256];                         // MS = 64: normalised value of each u8 pixel
+  double h_loc[NO * HID > CL * 80 ? NO * HID : CL * 80];   // later (rank 0) the CTAs' conv-gradient shares [CL][80]
+  double dh_loc[NO * HID];
   double part[800];
   double w2[NCLS * HID];
   double b1[HID];
   double b2[16];
   double wc[80];
-  double z[11 * 16];
-  double dz[11 * 16];
-  double red[16];
-  int sidx[64];
-  int label[64];
-  float valid[64];
-  unsigned char arg[64 * KC];
+  double z[NO * 16];
+  double dz[NO * 16];
+  double red[NO];
+  int sidx[MS];
+  int label[MS];
+  float valid[MS];
+  unsigned char arg[MS * KC];
 };
-static_assert(sizeof(Smem) <= 227 * 1024, "shared memory budget");
-static_assert(6 * 80 <= 11 * 64, "conv shares fit h_loc");
+static_assert(sizeof(Smem<16>) <= 227 * 1024 && sizeof(Smem<32>) <= 227 * 1024 && sizeof(Smem<64>) <= 227 * 1024,
+              "shared memory budget");
 
-NNDT_DEVINL double wsum(double v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 NNDT_DEVINL double wmax(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -68,27 +71,30 @@ NNDT_DEVINL void stamp(long long* prof, int idx, int tid) {
 template <int MS>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(NT, 1)
 mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
+  using SM = Smem<MS>;
+  constexpr int NO = SM::NO;
+  constexpr bool kDoublePix = SM::kDoublePix;
+  static_assert(MS % 16 == 0 && NO <= NT / 32, "tile geometry");
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  Smem& sm = *reinterpret_cast<Smem*>(smem_raw);
+  SM& sm = *reinterpret_cast<SM*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int l = blockIdx.z, bsplit = blockIdx.y, nsplit = gridDim.y;
   const int c = (int)cluster_rank();
   const double* th = reinterpret_cast<const double*>(a.theta) + (size_t)l * a.n_pad;
-  auto own_lo = [](int r) { return (MS * r + CL - 1) / CL; };
   const double pmean = gs.mean, pis = gs.inv_std;
   const bool u8 = a.x_is_u8 != 0;
-  // pixels: with MS <= 32 samples the 8 x 28 slabs fit as normalised doubles, so conv and conv-grad read fp64 directly
-  constexpr bool kDoublePix = MS <= 32;
-  using PT = typename std::conditional<kDoublePix, double, float>::type;
-  PT* img = reinterpret_cast<PT*>(sm.img);
-  auto pix = [&](PT v) -> double {
-    if constexpr (kDoublePix) return v;
-    else return u8 ? ((double)v * (1.0 / 255.0) - pmean) * pis : (double)v;
+  double* imgd = reinterpret_cast<double*>(sm.img);
+  // pixel p (0 .. 279) of sample s's image rows 6c .. 6c+9.  fp32 inputs at MS = 64 have no room in shared memory and
+  // are read from L2 (the rows were just loaded); invalid samples are masked wherever their pixels would count.
+  auto pix = [&](int s, int p) -> double {
+    if constexpr (kDoublePix) return imgd[s * PXR + p];
+    else if (u8) return sm.lut[sm.img[s * PXR + p]];
+    else return (double)__ldg(reinterpret_cast<const float*>(a.x) + (size_t)sm.sidx[s] * 784 + 6 * HW * c + p);
   };
   long long* prof = a.prof != nullptr ? a.prof + ((l * nsplit + bsplit) * CL + c) * 64 : nullptr;
   stamp(prof, 0, tid);
 
-  // ---- data half: sampler + image rows 4c .. 4c+7 (224 contiguous pixels per sample), before the PDL wait ---------------
+  // ---- data half: sampler + image rows 6c .. 6c+9 (280 contiguous pixels per sample), before the PDL wait ----------------
   const int call = a.calls != nullptr ? a.calls[l] : 0;
   const BatchGeom bg = batch_geom<true>(a, l, call);
   if (tid < MS) {
@@ -101,29 +107,32 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     }
     sm.sidx[tid] = idx; sm.valid[tid] = ok; sm.label[tid] = lab;
   }
+  if constexpr (!kDoublePix)
+    if (tid < 256) sm.lut[tid] = ((double)tid * (1.0 / 255.0) - pmean) * pis;
   __syncthreads();
-  constexpr int NU8 = (MS * 14 + NT - 1) / NT, NF4 = (MS * 56 + NT - 1) / NT;
-  uint4 pu[NU8]; float4 pf[NF4];
+  // u8 rows: 35 8-byte chunks per sample (the window starts at byte 168 c, 8-byte aligned); fp32 rows: 70 float4
+  constexpr int NU8 = (MS * 35 + NT - 1) / NT, NF4 = kDoublePix ? (MS * 70 + NT - 1) / NT : 1;
+  uint2 pu[NU8]; float4 pf[NF4];
   if (u8) {
 #pragma unroll
     for (int i = 0; i < NU8; ++i) {
       const int o = tid + i * NT;
-      pu[i] = make_uint4(0, 0, 0, 0);
-      if (o < MS * 14) {
-        const int s = o / 14, q = o - s * 14;
+      pu[i] = make_uint2(0, 0);
+      if (o < MS * 35) {
+        const int s = o / 35, q = o - s * 35;
         if (sm.valid[s] != 0.f)
-          pu[i] = *reinterpret_cast<const uint4*>(reinterpret_cast<const unsigned char*>(a.x) + (size_t)sm.sidx[s] * 784 + 112 * c + 16 * q);
+          pu[i] = *reinterpret_cast<const uint2*>(reinterpret_cast<const unsigned char*>(a.x) + (size_t)sm.sidx[s] * 784 + 6 * HW * c + 8 * q);
       }
     }
-  } else {
+  } else if constexpr (kDoublePix) {
 #pragma unroll
     for (int i = 0; i < NF4; ++i) {
       const int o = tid + i * NT;
       pf[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (o < MS * 56) {
-        const int s = o / 56, q = o - s * 56;
+      if (o < MS * 70) {
+        const int s = o / 70, q = o - s * 70;
         if (sm.valid[s] != 0.f)
-          pf[i] = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.x) + (size_t)sm.sidx[s] * 784 + 112 * c + 4 * q);
+          pf[i] = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(a.x) + (size_t)sm.sidx[s] * 784 + 6 * HW * c + 4 * q);
       }
     }
   }
@@ -132,7 +141,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   pdl_launch_dependents();
   stamp(prof, 2, tid);
 
-  // ---- W1 slice [64 j][72 k] (three 24-column runs per row): loads in flight while the pixels are converted --------------
+  // ---- W1 slice [64 j][108 k] (three 36-column runs per row): loads in flight while the pixels are converted -------------
   constexpr int NW = (HID * KC + NT - 1) / NT;
   double wreg[NW];
 #pragma unroll
@@ -153,24 +162,25 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
 #pragma unroll
     for (int i = 0; i < NU8; ++i) {
       const int o = tid + i * NT;
-      if (o < MS * 14) {
-        const int s = o / 14, q = o - s * 14;
-        const uint32_t w[4] = {pu[i].x, pu[i].y, pu[i].z, pu[i].w};
-        PT* dst = img + s * 224 + 16 * q;
+      if (o < MS * 35) {
+        const int s = o / 35, q = o - s * 35;
+        if constexpr (kDoublePix) {
+          const uint32_t w[2] = {pu[i].x, pu[i].y};
+          double* dst = imgd + s * PXR + 8 * q;
 #pragma unroll
-        for (int j = 0; j < 16; ++j) {
-          const double v = (double)((w[j >> 2] >> (8 * (j & 3))) & 0xff);
-          if constexpr (kDoublePix) dst[j] = (v * (1.0 / 255.0) - pmean) * pis; else dst[j] = (float)v;
+          for (int j = 0; j < 8; ++j) dst[j] = ((double)((w[j >> 2] >> (8 * (j & 3))) & 0xff) * (1.0 / 255.0) - pmean) * pis;
+        } else {
+          *reinterpret_cast<uint2*>(sm.img + s * PXR + 8 * q) = pu[i];
         }
       }
     }
-  } else {
+  } else if constexpr (kDoublePix) {
 #pragma unroll
     for (int i = 0; i < NF4; ++i) {
       const int o = tid + i * NT;
-      if (o < MS * 56) {
-        PT* dst = img + (o / 56) * 224 + 4 * (o % 56);
-        dst[0] = (PT)pf[i].x; dst[1] = (PT)pf[i].y; dst[2] = (PT)pf[i].z; dst[3] = (PT)pf[i].w;
+      if (o < MS * 70) {
+        double* dst = imgd + (o / 70) * PXR + 4 * (o % 70);
+        dst[0] = pf[i].x; dst[1] = pf[i].y; dst[2] = pf[i].z; dst[3] = pf[i].w;
       }
     }
   }
@@ -186,11 +196,11 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   for (int it = tid; it < MS * CELLS; it += NT) {
     const int s = it / CELLS, cell = it - s * CELLS;
     const int pr = cell / PHW, px = cell - pr * PHW;
-    const PT* src = img + s * 224 + (2 * pr) * HW + 2 * px;
+    const int p0 = (2 * pr) * HW + 2 * px;
     double patch[6][6];
     if constexpr (kDoublePix) {
-      // a patch row is six consecutive doubles starting at the even column 2 px: three 16-byte loads, and consecutive lanes
-      // (consecutive px) read consecutive 16-byte chunks -> half the shared-memory wavefronts of 8-byte loads at stride 2
+      // a patch row is six consecutive doubles starting at an even column: three 16-byte loads
+      const double* src = imgd + s * PXR + p0;
 #pragma unroll
       for (int r = 0; r < 6; ++r)
 #pragma unroll
@@ -202,7 +212,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
 #pragma unroll
       for (int r = 0; r < 6; ++r)
 #pragma unroll
-        for (int q = 0; q < 6; ++q) patch[r][q] = pix(src[r * HW + q]);
+        for (int q = 0; q < 6; ++q) patch[r][q] = pix(s, p0 + r * HW + q);
     }
     const bool ok = sm.valid[s] != 0.f;
 #pragma unroll 1
@@ -229,68 +239,44 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   __syncthreads();
   stamp(prof, 4, tid);
 
-  // ---- GEMM 1: H_c[s][j] = sum_k A[s][k] W[j][k].  Register tile 4 rows x 4 columns (rows tr + RQ i, columns tc + 16 i):
-  //      per k a warp issues 4 + 4 shared-memory wavefronts for 16 DFMA instructions.  Split-K over NG = 512 / (4 MS) thread
-  //      groups; group g writes its partial tile to P_g (the contiguous dh + hpart arrays hold NG x MS = 128 rows) and the
-  //      partials are summed in fixed order (deterministic) into the rows the peers read.
-  constexpr int RQ = MS / 4, GT = MS * 4, NG = NT / GT, KG = KC / NG;
-  static_assert(KC % NG == 0 && NG * MS == 128, "split-K geometry");
-  const int grp = tid / GT, tg = tid - grp * GT, tr = tg >> 4, tc = tg & 15;
+  // ---- GEMM 1 (DMMA): partial H_c[s][j] = sum_k A[s][k] W[j][k] over this CTA's 108 inputs.  MS / 16 x 8 tiles of 16 x 8,
+  //      NJ1 adjacent column tiles per warp (all 16 warps busy at MS >= 32), the whole K range per tile: no split-K ----------
   {
-    double acc[4][4];
+    constexpr int NJ1 = MS == 64 ? 2 : 1, NGRP = 8 / NJ1;
+    if (warp < (MS / 16) * NGRP) {
+      const int m0 = 16 * (warp / NGRP), n0 = 8 * NJ1 * (warp % NGRP);
+      double acc[NJ1][4];
+      zero(acc);
+      gemm<NJ1>(acc, m0, n0, KC, lane, at(sm.a, WS), at_t(sm.w, WS));
 #pragma unroll
-    for (int r = 0; r < 4; ++r)
+      for (int j = 0; j < NJ1; ++j)
 #pragma unroll
-      for (int i = 0; i < 4; ++i) acc[r][i] = 0.0;
-#pragma unroll 2
-    for (int k = grp * KG; k < (grp + 1) * KG; ++k) {
-      double x[4], wv[4];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) x[r] = sm.a[(tr + RQ * r) * WS + k];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) wv[i] = sm.w[(tc + 16 * i) * WS + k];
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int i = 0; i < 4; ++i) acc[r][i] += x[r] * wv[i];
+        for (int i = 0; i < 4; ++i) sm.h[frow(m0, lane, i) * HS + fcol(n0 + 8 * j, lane, i)] = acc[j][i];
     }
-    double* P = sm.dh + (size_t)grp * MS * HS;
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int i = 0; i < 4; ++i) P[(tr + RQ * r) * HS + tc + 16 * i] = acc[r][i];
-  }
-  __syncthreads();
-  for (int o = tid; o < MS * HID; o += NT) {
-    const int s = o >> 6, j = o & 63;
-    double v = 0.0;
-#pragma unroll
-    for (int g = 0; g < NG; ++g) v += sm.dh[(size_t)g * MS * HS + s * HS + j];
-    sm.hpart[s * HS + j] = v;                         // hpart == P_{64 / MS}: every element is read before it is rewritten
   }
   stamp(prof, 5, tid);
-  cluster_sync();                                        // #1: all six partial H are in shared memory
+  cluster_sync();                                        // #1: all four partial H are in shared memory
   stamp(prof, 6, tid);
   if (c == 0 && tid == 0 && a.calls != nullptr) {
     if (a.arrive == nullptr || nsplit == 1) a.calls[l] = call + 1;
     else if (atomicAdd(a.arrive + l, 1u) == (unsigned)nsplit - 1) { a.arrive[l] = 0; a.calls[l] = call + 1; }
   }
 
-  // ---- reduce-scatter of H + fc2 / loss / their backward for this CTA's samples --------------------------------------------
-  const int s0 = own_lo(c), ns = own_lo(c + 1) - s0;
+  // ---- reduce-scatter of H + fc2 / loss / their backward for this CTA's samples s0 .. s0 + NO - 1 -------------------------
+  const int s0 = c * NO;
   const double inv_bs = 1.0 / (double)(bg.bs ? bg.bs : 1);
-  for (int o = tid; o < ns * HID; o += NT) {
+  for (int o = tid; o < NO * HID; o += NT) {
     const int sl = o >> 6, j = o & 63;
-    const double* src = sm.hpart + (s0 + sl) * HS + j;
+    const double* src = sm.h + (s0 + sl) * HS + j;
     double v = sm.b1[j];
 #pragma unroll
     for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(src, (uint32_t)r));
     sm.h_loc[o] = v > 0.0 ? v : 0.0;
   }
   __syncthreads();
-  {
-    const int o = tid >> 2, part = tid & 3;              // 4 lanes per logit
-    const bool live = o < ns * NCLS;
+  for (int base = 0; base < NO * NCLS; base += NT / 4) {  // 4 lanes per logit; the trip count is the same for every warp
+    const int o = base + (tid >> 2), part = tid & 3;
+    const bool live = o < NO * NCLS;
     const int sl = live ? o / NCLS : 0, cc = live ? o - sl * NCLS : 0;
     double v = 0.0;
     if (live) {
@@ -302,12 +288,12 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     if (live && part == 0) sm.z[sl * 16 + cc] = v + sm.b2[cc];
   }
   __syncthreads();
-  if (warp < ns) {                                       // log-softmax + NLL: one warp per sample, one lane per class
+  if (warp < NO) {                                       // log-softmax + NLL: one warp per sample, one lane per class
     const int sl = warp, s = s0 + sl;
     const bool cls = lane < NCLS;
     const double zc = cls ? sm.z[sl * 16 + lane] : -1.0e300;
     const double mx = wmax(zc);
-    const double se = wsum(cls ? exp(zc - mx) : 0.0);
+    const double se = warp_sum(cls ? exp(zc - mx) : 0.0);
     const double lse = mx + log(se);
     const int y = sm.label[s];
     const double ok = (double)sm.valid[s];
@@ -315,7 +301,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     if (lane == y) sm.red[sl] = ok * (lse - zc);
   }
   __syncthreads();
-  for (int o = tid; o < ns * HID; o += NT) {
+  for (int o = tid; o < NO * HID; o += NT) {
     const int sl = o >> 6, j = o & 63;
     double v = 0.0;
 #pragma unroll
@@ -326,27 +312,27 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   for (int o = tid; o < NCLS * HID; o += NT) {
     const int cc = o >> 6, j = o & 63;
     double v = 0.0;
-    for (int sl = 0; sl < ns; ++sl) v += sm.dz[sl * 16 + cc] * sm.h_loc[sl * HID + j];
+    for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + cc] * sm.h_loc[sl * HID + j];
     sm.part[PART_W2 + o] = v;
   }
   if (tid < HID) {
     double v = 0.0;
-    for (int sl = 0; sl < ns; ++sl) v += sm.dh_loc[sl * HID + tid];
+    for (int sl = 0; sl < NO; ++sl) v += sm.dh_loc[sl * HID + tid];
     sm.part[PART_B1 + tid] = v;
   } else if (tid >= 64 && tid < 64 + NCLS) {
     double v = 0.0;
-    for (int sl = 0; sl < ns; ++sl) v += sm.dz[sl * 16 + (tid - 64)];
+    for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + (tid - 64)];
     sm.part[PART_B2 + (tid - 64)] = v;
   } else if (tid == 96) {
     double v = 0.0;
-    for (int sl = 0; sl < ns; ++sl) v += sm.red[sl];
+    for (int sl = 0; sl < NO; ++sl) v += sm.red[sl];
     sm.part[PART_LOSS] = v * inv_bs;
   }
   stamp(prof, 7, tid);
   cluster_sync();                                        // #2: every owner's dH rows and fc2 / b1 / loss shares are final
   stamp(prof, 8, tid);
   double* gp = reinterpret_cast<double*>(a.grad_part) + ((size_t)l * nsplit + bsplit) * a.n_pad;
-  // CTA c reduces its sixth of the fc2 / b1 / loss shares over the cluster (the peers stay resident until the last barrier)
+  // CTA c reduces its quarter of the fc2 / b1 / loss shares over the cluster (the peers stay resident until the last barrier)
   {
     constexpr int NE = PART_N - PART_B1, PER = (NE + CL - 1) / CL;
     const int o = PART_B1 + c * PER + tid;
@@ -363,103 +349,60 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       }
     }
   }
-  // ---- gather all MS dH rows from their owners ------------------------------------------------------------------------------
+  // ---- gather all MS dH rows from their owners into the partial-H tile (every peer finished reading it before #2) -----------
   for (int o = tid; o < MS * HID; o += NT) {
-    const int s = o >> 6, j = o & 63;
-    int r = 0;
-#pragma unroll
-    for (int q = 1; q < CL; ++q) r += (s >= own_lo(q)) ? 1 : 0;
-    sm.dh[s * HS + j] = ld_dsmem(map_to(sm.dh_loc + (s - own_lo(r)) * HID + j, (uint32_t)r));
+    const int s = o >> 6, j = o & 63, r = s / NO;
+    sm.h[s * HS + j] = ld_dsmem(map_to(sm.dh_loc + (s - r * NO) * HID + j, (uint32_t)r));
   }
   __syncthreads();
   stamp(prof, 9, tid);
 
-  // ---- GEMM 2: da1_c[s][k] = sum_j dH[s][j] W[j][k]; tile 4 rows x 5 columns (k = tc + 16 i < 72).  With MS <= 32 the j range
-  //      is split over two thread groups: group 1 parks its partial tile in the (dead) hpart rows, group 0 adds it -----------
-  constexpr int NG2 = (MS <= 32) ? 2 : 1, JG = HID / NG2;
-  double d2[4][5];
+  // ---- GEMM 3 (DMMA): dW1_c[j][k] = sum_s dH[s][j] A[s][k], 4 x KT tiles straight to the gradient row; then GEMM 2 (DMMA):
+  //      da1_c[s][k] = sum_j dH[s][j] W[j][k], MS / 16 x KT tiles written over A ------------------------------------------------
+  {
+    constexpr int T3 = (HID / 16) * KT;
+#pragma unroll 1
+    for (int t = warp; t < T3; t += NT / 32) {
+      const int m0 = 16 * (t / KT), n0 = 8 * (t % KT);
+      double acc[1][4];
+      zero(acc);
+      gemm<1>(acc, m0, n0, MS, lane, at_t(sm.h, HS), at(sm.a, WS));
 #pragma unroll
-  for (int r = 0; r < 4; ++r)
-#pragma unroll
-    for (int i = 0; i < 5; ++i) d2[r][i] = 0.0;
-  if (grp < NG2) {
-#pragma unroll 2
-    for (int j = grp * JG; j < (grp + 1) * JG; ++j) {
-      double x[4], wv[5];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) x[r] = sm.dh[(tr + RQ * r) * HS + j];
-#pragma unroll
-      for (int i = 0; i < 5; ++i) wv[i] = (tc + 16 * i < KC) ? sm.w[j * WS + tc + 16 * i] : 0.0;
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int i = 0; i < 5; ++i) d2[r][i] += x[r] * wv[i];
-    }
-    if (NG2 == 2 && grp == 1) {
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int i = 0; i < 5; ++i)
-          if (tc + 16 * i < KC) sm.hpart[(tr + RQ * r) * KC + tc + 16 * i] = d2[r][i];
-    }
-  }
-  stamp(prof, 10, tid);
-  // ---- GEMM 3: dW1_c[j][k] = sum_s dH[s][j] A[s][k]; tile 4 features (tr3 + 16 r) x 5 columns; 256 threads -----------------
-  if (tid < 256) {
-    const int tr3 = tid >> 4, tc3 = tid & 15;
-    double d3[4][5];
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int i = 0; i < 5; ++i) d3[r][i] = 0.0;
-#pragma unroll 2
-    for (int s = 0; s < MS; ++s) {
-      double x[4], av[5];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) x[r] = sm.dh[s * HS + tr3 + 16 * r];
-#pragma unroll
-      for (int i = 0; i < 5; ++i) av[i] = (tc3 + 16 * i < KC) ? sm.a[s * WS + tc3 + 16 * i] : 0.0;
-#pragma unroll
-      for (int r = 0; r < 4; ++r)
-#pragma unroll
-        for (int i = 0; i < 5; ++i) d3[r][i] += x[r] * av[i];
-    }
-#pragma unroll
-    for (int i = 0; i < 5; ++i) {
-      const int k = tc3 + 16 * i;
-      if (k < KC) {
-        const int ch = k / CELLS, cell = k - ch * CELLS;
-        double* g = gp + a.off_w1 + ch * NPOOL + CELLS * c + cell;
-#pragma unroll
-        for (int r = 0; r < 4; ++r) g[(size_t)(tr3 + 16 * r) * FC1_IN] = d3[r][i];
-      }
-    }
-  }
-  __syncthreads();      // every read of W (GEMM 2) and of A / dH (GEMM 3) is done; group 1's partial tile is parked
-  stamp(prof, 11, tid);
-  double* da1 = sm.w;   // W's rows become da1 [s][72], masked by ReLU'(a1)
-  if (grp == 0) {
-#pragma unroll
-    for (int r = 0; r < 4; ++r)
-#pragma unroll
-      for (int i = 0; i < 5; ++i) {
-        const int s = tr + RQ * r, k = tc + 16 * i;
+      for (int i = 0; i < 4; ++i) {
+        const int j = frow(m0, lane, i), k = fcol(n0, lane, i);
         if (k < KC) {
-          const double v = d2[r][i] + (NG2 == 2 ? sm.hpart[s * KC + k] : 0.0);
-          da1[s * KC + k] = (sm.arg[s * KC + k] & 4) ? v : 0.0;
+          const int ch = k / CELLS, cell = k - ch * CELLS;
+          gp[a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell] = acc[0][i];
         }
       }
+    }
+  }
+  __syncthreads();      // every read of A (GEMM 3) is done
+  stamp(prof, 10, tid);
+  double* da1 = sm.a;   // A's rows become da1 [s][KC], masked by ReLU'(a1)
+#pragma unroll 1
+  for (int t = warp; t < (MS / 16) * KT; t += NT / 32) {
+    const int m0 = 16 * (t / KT), n0 = 8 * (t % KT);
+    double acc[1][4];
+    zero(acc);
+    gemm<1>(acc, m0, n0, HID, lane, at(sm.h, HS), at(sm.w, WS));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      const int s = frow(m0, lane, i), k = fcol(n0, lane, i);
+      if (k < KC) da1[s * KC + k] = (sm.arg[s * KC + k] & 4) ? acc[0][i] : 0.0;
+    }
   }
   __syncthreads();
+  stamp(prof, 11, tid);
   // ---- conv grads.  da1 is sparse (ReLU mask): (1) deterministic per-channel compaction of the non-zero (sample, cell)
   //      entries (ballot + prefix over 32-entry chunks, so the order — and the fp64 sums — never depend on timing);
   //      (2) five warps per channel walk that channel's dense list, each entry routes da1 to its argmax conv position;
-  //      (3) ONE fold over lane pairs + transposition through the dead A / dH tiles for all three channels --------------
+  //      (3) each warp folds its 26 sums over its lanes, and the five warp sums of a channel are added in warp order -------
   constexpr int NI = MS * CELLS, NCH = NI / 32, CGW = 5, CGT = CGW * 32;     // entries / chunks per channel; warps / threads per channel
-  static_assert(F * CGW <= NT / 32 && NI % 32 == 0 && NI <= 2048, "conv-grad work split");
-  unsigned short* list = reinterpret_cast<unsigned short*>(sm.hpart);      // [F][NI] (hpart is dead: group 1's partial was consumed)
+  static_assert(F * CGW <= NT / 32 && NI % 32 == 0 && NI <= 4096, "conv-grad work split");
+  unsigned short* list = reinterpret_cast<unsigned short*>(sm.h);           // [F][NI] entries it | argmax << 12 (dH is dead)
   int* ccount = reinterpret_cast<int*>(list + F * NI);                     // [F * NCH] chunk counts, then [F] totals
-  static_assert(sizeof(unsigned short) * F * NI + sizeof(int) * (F * NCH + F) <= sizeof(double) * 64 * HS, "lists fit hpart");
+  static_assert(sizeof(unsigned short) * F * NI + sizeof(int) * (F * NCH + F) <= sizeof(SM::h), "lists fit the dH tile");
   for (int q = warp; q < F * NCH; q += NT / 32) {
     const int ch = q / NCH, it = (q - ch * NCH) * 32 + lane;
     const int s = it / CELLS, cell = it - s * CELLS;
@@ -477,12 +420,11 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     const bool nz = da1[s * KC + ch * CELLS + cell] != 0.0;
     const unsigned b = __ballot_sync(0xffffffffu, nz);
     if (nz) list[ch * NI + pre + __popc(b & ((1u << lane) - 1u))] =
-        (unsigned short)(it | ((sm.arg[s * KC + ch * CELLS + cell] & 3) << 11));
+        (unsigned short)(it | ((sm.arg[s * KC + ch * CELLS + cell] & 3) << 12));
     if (qq == NCH - 1 && lane == 0) ccount[F * NCH + ch] = pre + __popc(b);
   }
   __syncthreads();
-  double* scratch = sm.a;                                                   // [F * 26][CGT / 2]
-  static_assert(sizeof(double) * F * 26 * (CGT / 2) <= sizeof(double) * (64 * WS + 64 * HS), "conv-grad scratch fits A + dH");
+  double* wsums = sm.w;                                                     // [F * CGW][26] (W is dead)
   {
     const int gch = warp / CGW, tl = tid - gch * CGT;
     if (gch < F) {
@@ -492,35 +434,35 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       const int n = ccount[F * NCH + gch];
       for (int j = tl; j < n; j += CGT) {
         const unsigned e = list[gch * NI + j];
-        const int it = e & 2047, ai = e >> 11;
+        const int it = e & 4095, ai = e >> 12;
         const int s = it / CELLS, cell = it - s * CELLS;
         const double g = da1[s * KC + gch * CELLS + cell];
         const int pr = cell / PHW, px = cell - pr * PHW;
-        const PT* src = img + s * 224 + (2 * pr + (ai >> 1)) * HW + 2 * px + (ai & 1);
+        const int p0 = (2 * pr + (ai >> 1)) * HW + 2 * px + (ai & 1);
 #pragma unroll
         for (int ky = 0; ky < KS; ++ky)
 #pragma unroll
-          for (int kx = 0; kx < KS; ++kx) cacc[ky * 5 + kx] += g * pix(src[ky * HW + kx]);
+          for (int kx = 0; kx < KS; ++kx) cacc[ky * 5 + kx] += g * pix(s, p0 + ky * HW + kx);
         cacc[25] += g;
       }
 #pragma unroll
       for (int i = 0; i < 26; ++i) {
-        const double v = cacc[i] + __shfl_xor_sync(0xffffffffu, cacc[i], 1);
-        if ((lane & 1) == 0) scratch[(gch * 26 + i) * (CGT / 2) + (tl >> 1)] = v;
+        const double v = warp_sum(cacc[i]);
+        if (lane == 0) wsums[warp * 26 + i] = v;
       }
     }
   }
   __syncthreads();
-  for (int o = warp; o < F * 26; o += NT / 32) {
+  if (tid < F * 26) {
+    const int ch = tid / 26, i = tid - ch * 26;
     double v = 0.0;
-    for (int q = lane; q < CGT / 2; q += 32) v += scratch[o * (CGT / 2) + q];
-    v = wsum(v);
-    const int ch = o / 26, i = o - ch * 26;
+#pragma unroll
+    for (int w = 0; w < CGW; ++w) v += wsums[(ch * CGW + w) * 26 + i];
     // this CTA's share goes straight into rank 0's collection buffer (its h_loc rows, dead since barrier #2)
-    if (lane == 0) st_dsmem(map_to(sm.h_loc + c * 80 + (i < 25 ? ch * 25 + i : 75 + ch), 0u), v);
+    st_dsmem(map_to(sm.h_loc + c * 80 + (i < 25 ? ch * 25 + i : 75 + ch), 0u), v);
   }
   stamp(prof, 12, tid);
-  cluster_sync();                                        // #3: all six conv-gradient shares are in rank 0's buffer
+  cluster_sync();                                        // #3: all four conv-gradient shares are in rank 0's buffer
   if (c == 0 && tid < 78) {
     double v = 0.0;
 #pragma unroll
@@ -531,18 +473,34 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
 }
 
 template <int MS>
+static cudaError_t prepare_ms() {
+  static cudaError_t prep = cudaFuncSetAttribute(mnist_cl64_train_kernel<MS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem<MS>));
+  return prep;
+}
+
+template <int MS>
 static cudaError_t launch_ms(const Args& a, const GenericShape& gs, cudaStream_t st) {
-  static cudaError_t prep = cudaFuncSetAttribute(mnist_cl64_train_kernel<MS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(Smem));
+  const cudaError_t prep = prepare_ms<MS>();
   if (prep != cudaSuccess) return prep;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(CL, 64 / MS, a.L); cfg.blockDim = dim3(NT);
-  cfg.dynamicSmemBytes = sizeof(Smem); cfg.stream = st;
+  cfg.dynamicSmemBytes = sizeof(Smem<MS>); cfg.stream = st;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   static const bool no_pdl = getenv("NNDT_NO_PDL") != nullptr;
   cfg.attrs = attr; cfg.numAttrs = no_pdl ? 0 : 1;
   return cudaLaunchKernelEx(&cfg, mnist_cl64_train_kernel<MS>, a, gs);
+}
+
+template <int MS>
+static int max_clusters_ms() {
+  if (prepare_ms<MS>() != cudaSuccess) { cudaGetLastError(); return 0; }
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(CL, 1, 1); cfg.blockDim = dim3(NT); cfg.dynamicSmemBytes = sizeof(Smem<MS>);
+  int n = 0;
+  if (cudaOccupancyMaxActiveClusters(&n, mnist_cl64_train_kernel<MS>, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
+  return n;
 }
 
 }  // namespace cl64
@@ -556,17 +514,16 @@ cudaError_t launch_train_cl64(const Args& a, const GenericShape& gs, int nsplit,
   return cudaErrorInvalidValue;
 }
 
-int cl64_max_active_clusters() {
-  if (cudaFuncSetAttribute(cl64::mnist_cl64_train_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(cl64::Smem)) != cudaSuccess) {
-    cudaGetLastError();
-    return 0;
+int cl64_max_active_clusters(int nsplit) {
+  switch (nsplit) {
+    case 1: return cl64::max_clusters_ms<64>();
+    case 2: return cl64::max_clusters_ms<32>();
+    case 4: return cl64::max_clusters_ms<16>();
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(cl64::CL, 1, 1); cfg.blockDim = dim3(cl64::NT); cfg.dynamicSmemBytes = sizeof(cl64::Smem);
-  int n = 0;
-  if (cudaOccupancyMaxActiveClusters(&n, cl64::mnist_cl64_train_kernel<64>, &cfg) != cudaSuccess) { cudaGetLastError(); return 0; }
-  return n;
+  return 0;
 }
+
+int cl64_cluster_ctas() { return cl64::CL; }
 
 }  // namespace mnist
 }  // namespace nndt

@@ -60,14 +60,19 @@ class FusedMnist:
             # 6 * nsplit * L CTAs in one wave — the conv / conv-grad phases are CUDA-core work that scales with SMs
             want = int(os.environ.get("NNDT_TC_SPLIT", "0"))
             self.S = want if want in (1, 2, 4) else max([n for n in (1, 2, 4) if 6 * n * self.L <= sms] or [1])
-        # float64, paper shape, batch <= 64: the same K-split cluster decomposition on the fp64 CUDA cores (csrc/mnist_cl64.cu);
-        # NNDT_MNIST_CL64=0 keeps the batch-split generic kernel (A/B)
+        # float64, paper shape, batch <= 64: a K-split cluster kernel with the fc1 contractions on the FP64 tensor cores
+        # (csrc/mnist_cl64.cu); NNDT_MNIST_CL64=0 keeps the batch-split generic kernel (A/B)
         self.cl64 = (self.generic and self.dtype == torch.float64 and mnist_kernel_is_paper_shape(spec) and self.B <= 64
-                     and os.environ.get("NNDT_MNIST_CL64", "1") != "0" and self.ext.mnist_cl64_max_clusters() >= 1)
+                     and os.environ.get("NNDT_MNIST_CL64", "1") != "0")
         if self.cl64:
             want = int(os.environ.get("NNDT_TC_SPLIT", "0"))
-            self.S = want if want in (1, 2, 4) else max([n for n in (1, 2, 4) if 6 * n * self.L <= sms] or [1])
-        self.kernel_name = (f"mnist_cl64_train_kernel<{64 // self.S}> (fp64 CUDA cores, {self.S} x 6-CTA cluster per node, DSMEM reduce)" if self.cl64 else
+            split = want if want in (1, 2, 4) else max([n for n in (1, 2, 4) if 6 * n * self.L <= sms] or [1])
+            self.cl64 = self.ext.mnist_cl64_max_clusters(split) >= 1
+            if self.cl64:
+                self.S = split
+        # CTAs per batch split: the cluster size of the cluster kernels, one CTA for the batch-split kernels
+        self.ctas_per_split = 6 if self.tc else self.ext.mnist_cl64_cluster_ctas() if self.cl64 else 1
+        self.kernel_name = (f"mnist_cl64_train_kernel<{64 // self.S}> (fp64 DMMA tiles, {self.S} x {self.ctas_per_split}-CTA cluster per node, DSMEM reduce)" if self.cl64 else
                             f"mnist_tc_train_kernel<{64 // self.S}> (3xTF32 mma.sync tiles, TMA tensor map, {self.S} x 6-CTA cluster per node)" if self.tc
                             else "convnet_generic_kernel (CUDA cores)" if self.generic else "mnist_kernel (mma.sync 3xTF32)")
         sh = problem.shards
@@ -103,7 +108,7 @@ class FusedMnist:
         if self.tc:
             self.base.update(tc=1, w1_map=self.ext.make_w1_tensor_map(a.theta.data_ptr(), a.n_pad, self.L, off[names[2]]))
         if os.environ.get("NNDT_STEP_PROF") == "1":     # scripts/profile_round_phases.py --per-step
-            self.step_prof = torch.zeros(self.L * self.S * (6 if (self.tc or self.cl64) else 1), 64, dtype=torch.int64, device=dev)
+            self.step_prof = torch.zeros(self.L * self.S * self.ctas_per_split, 64, dtype=torch.int64, device=dev)
             self.base["step_prof"] = self.step_prof.data_ptr()
         self.train_op = self.ext.MnistOp(self.base)
         self._setup_eval()
@@ -230,10 +235,10 @@ class FusedMnist:
         self.calls0 = torch.as_tensor(pr.calls[pl.lo: pl.lo + pl.L].astype(np.int32), device=dev)
         self.stage_round = torch.zeros(1, dtype=torch.int32, device=dev)
         self.stage_done = torch.zeros(1, dtype=torch.int32, device=dev)
-        # a training CTA fills an SM's register file (768 threads x 80 registers): a staging block that lands on
-        # an SM evicts a training CTA into a second wave, so the staging grid is sized to the SMs left over
+        # a training CTA fills an SM's register file: a staging block that lands on an SM evicts a training CTA into a
+        # second wave, so the staging grid is sized to the SMs left over by all L x S x ctas_per_split training CTAs
         sms = torch.cuda.get_device_properties(dev).multi_processor_count
-        ctas = self.L * self.S * (6 if (self.tc or self.cl64) else 1)
+        ctas = self.L * self.S * self.ctas_per_split
         free = sms - ctas if ctas <= sms else 0      # multi-wave grids leave no SM idle
         gather_blocks = int(os.environ.get("NNDT_GATHER_BLOCKS", "0")) or max(8, min(24, free - 2))
         self.direct_ops, self.gather_ops = [], []

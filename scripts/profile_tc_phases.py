@@ -23,8 +23,9 @@ PHASES = ["sampler + image loads issued", "PDL wait", "TMA issue, small tensors,
           "MMA 3 issue | da1 epilogue", "conv grads (under MMA 3) -> rank 0", "MMA 3 wait, dW1 epilogue -> global",
           "cluster sync 3, conv-grad sum (rank 0), exit"]
 PHASES64 = ["sampler + image loads issued", "PDL wait", "W1 slice + small tensors (L2), pixels", "conv + ReLU + pool -> A tile (fp64)",
-            "GEMM 1 (fc1 partial, DFMA)", "cluster sync 1", "reduce-scatter, fc2, loss, dz, dh, fc2 grads", "cluster sync 2",
-            "gather dH", "GEMM 2 (da1)", "GEMM 3 (dW1) -> global", "da1 -> smem, conv grads", "cluster sync 3, small-grad reduce (rank 0), sync 4"]
+            "GEMM 1 (fc1 partial, DMMA)", "cluster sync 1", "reduce-scatter, fc2, loss, dz, dh, fc2 grads", "cluster sync 2",
+            "fc2-grad reduce (1/4), gather dH", "GEMM 3 (dW1, DMMA) -> global", "GEMM 2 (da1, DMMA) -> smem", "conv grads -> rank 0",
+            "cluster sync 3, conv-grad sum (rank 0), exit"]
 
 
 def slot_errors(B):
