@@ -175,6 +175,7 @@ struct DinnoRoundOp {
 };
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp
+void bind_rl(py::module& m);      // rl_bind.cpp
 void bind_runtime(py::module& m); // runtime.cpp
 
 PYBIND11_MODULE(_C, m) {
@@ -220,5 +221,6 @@ PYBIND11_MODULE(_C, m) {
   bind_consensus<float>(m, "ConsensusOpF32");
   bind_consensus<double>(m, "ConsensusOpF64");
   bind_mlp(m);
+  bind_rl(m);
   bind_runtime(m);
 }

@@ -69,7 +69,7 @@ class _ConsensusPPO:
         from .eval_policy import rollout, save_rollout_gif
         os.makedirs(self.out_dir, exist_ok=True)
         actors = [self.pr.models[i].actor for i in range(self.pr.N)]
-        _, _, traj = rollout(actors, self.pr.env, record=True)
+        _, _, traj = rollout(actors, self.pr.env, record=True, backend=getattr(self.pr, "rollout_backend", "torch"))
         return save_rollout_gif(self.pr.env, traj, os.path.join(self.out_dir, f"{self.alg}_{self.conf.get('ID', 0)}_{k}.gif"))
 
     def save(self, k):

@@ -24,8 +24,10 @@ from .simple_tag import SimpleTagEnv, heuristic_prey_action
 
 class DistPPOProblem:
     # defaults of the reference's _init_hyperparameters (:391-436) — set explicitly, no exec()
+    # rollout_backend "cuda": each batch is one fused kernel launch (ops/tag_rollout.py) with its own Philox noise stream
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
-                    lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None)
+                    lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
+                    rollout_backend="torch")
 
     def __init__(self, base_actor, base_critic, graph, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
@@ -56,6 +58,12 @@ class DistPPOProblem:
         self.conf = {"metrics_config": {"evaluate_frequency": 10 ** 12}, "problem_name": "dist_ppo"}
         self.logger = {"delta_t": time.time_ns(), "t_so_far": 0, "i_so_far": 0, "batch_lens": [],
                        "batch_rews": [], "actor_losses": []}
+        if self.rollout_backend not in ("torch", "cuda"):
+            raise ValueError(f"rollout_backend must be 'torch' or 'cuda', not {self.rollout_backend!r}")
+        if self.rollout_backend == "cuda":
+            from ..ops import tag_rollout
+            tag_rollout.require(env, self.actors)
+        self._rollout_key, self._rollout_index = None, 0
 
     @property
     def actors(self):
@@ -87,6 +95,8 @@ class DistPPOProblem:
     # ---- data collection ---------------------------------------------------------------
     def split_rollout_marl(self):
         """Collect at least ``timesteps_per_batch`` predator steps (ALG STEP 3)."""
+        if self.rollout_backend == "cuda":
+            return self._split_rollout_cuda()
         env, N = self.env, self.N
         cycles = max(1, self.max_timesteps_per_episode // env.num_agents)
         obs_b = [[] for _ in range(N)]; act_b = [[] for _ in range(N)]
@@ -124,6 +134,27 @@ class DistPPOProblem:
         self.curr_log_probs = {i: torch.cat(lp_b[i]) for i in range(N)}
         self.curr_rtgs = {i: torch.cat([r.reshape(-1) for r in rtg_b[i]]) for i in range(N)}
         self.logger["batch_rews"] = ep_returns
+        self.logger["batch_lens"] = ep_lens
+        self.logger["t_so_far"] += int(np.sum(ep_lens))
+        self.logger["i_so_far"] += 1
+
+    def _split_rollout_cuda(self):
+        """The same batch as ``split_rollout_marl`` (episodes, cycles, layout, counts) from one kernel launch."""
+        from ..ops import tag_rollout
+        env, N = self.env, self.N
+        T = min(max(1, self.max_timesteps_per_episode // env.num_agents), env.max_cycles)
+        n_ep = max(1, -(-self.timesteps_per_batch // (N * env.E * T)))
+        if self._rollout_key is None:
+            self._rollout_key = tag_rollout.draw_key()
+        out = tag_rollout.rollout(env, self.actors, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
+                                  key=self._rollout_key, index=self._rollout_index)
+        self._rollout_index += 1
+        self.curr_obs = {i: out["obs"][i] for i in range(N)}
+        self.curr_acts = {i: out["acts"][i] for i in range(N)}
+        self.curr_log_probs = {i: out["log_probs"][i] for i in range(N)}
+        self.curr_rtgs = {i: out["rtgs"][i] for i in range(N)}
+        ep_lens = [T * env.num_agents] * (n_ep * env.E)
+        self.logger["batch_rews"] = out["ep_returns"].tolist()
         self.logger["batch_lens"] = ep_lens
         self.logger["t_so_far"] += int(np.sum(ep_lens))
         self.logger["i_so_far"] += 1

@@ -9,9 +9,18 @@ import torch
 from .simple_tag import SimpleTagEnv, heuristic_prey_action
 
 
-def rollout(actors, env: SimpleTagEnv, record=False):
+def rollout(actors, env: SimpleTagEnv, record=False, backend="torch"):
     """``actors``: one module (shared policy) or a list with one per predator.  Returns
-    (episode return per world, episode length, optional positions)."""
+    (episode return per world, episode length, optional positions).  ``backend="cuda"`` runs the deterministic
+    episode as one kernel launch (ops/tag_rollout.py)."""
+    if backend == "cuda":
+        from ..ops import tag_rollout
+        out = tag_rollout.rollout(env, actors, T=env.max_cycles, n_ep=1, gamma=1.0, cov_var=0.5, noise_scale=0.0,
+                                  debug=record)
+        traj = out["pos"][0, :, 0].cpu().numpy() if record else None
+        return out["ep_returns"].float().cpu().numpy(), env.max_cycles, traj
+    if backend != "torch":
+        raise ValueError(f"backend must be 'torch' or 'cuda', not {backend!r}")
     shared = not isinstance(actors, (list, tuple, dict))
     obs_adv, obs_good = env.reset()
     total = torch.zeros(env.E, device=env.device)
@@ -39,11 +48,11 @@ def save_rollout_gif(env: SimpleTagEnv, traj, out: str, size: int = 400, fps: in
     return out
 
 
-def eval_policy(actors, env: SimpleTagEnv, episodes=5, record=False, render_to=None):
+def eval_policy(actors, env: SimpleTagEnv, episodes=5, record=False, render_to=None, backend="torch"):
     """``render_to``: path of a GIF of the first episode (implies ``record``)."""
     rets = []
     for ep in range(episodes):
-        ret, length, traj = rollout(actors, env, record=(record or render_to is not None) and ep == 0)
+        ret, length, traj = rollout(actors, env, record=(record or render_to is not None) and ep == 0, backend=backend)
         if render_to is not None and ep == 0:
             save_rollout_gif(env, traj, render_to)
         rets.append(ret.mean())

@@ -17,7 +17,7 @@ from .simple_tag import SimpleTagEnv, heuristic_prey_action
 class PPO:
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
                     lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
-                    ID=0, out_dir="./trained")
+                    ID=0, out_dir="./trained", rollout_backend="torch")
 
     def __init__(self, policy_class, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
@@ -37,6 +37,12 @@ class PPO:
         self.logger = {"delta_t": time.time_ns(), "t_so_far": 0, "i_so_far": 0, "batch_lens": [], "batch_rews": [],
                        "actor_losses": []}
         self.avg_ep_rews, self.timesteps = [], []
+        if self.rollout_backend not in ("torch", "cuda"):
+            raise ValueError(f"rollout_backend must be 'torch' or 'cuda', not {self.rollout_backend!r}")
+        if self.rollout_backend == "cuda":
+            from ..ops import tag_rollout
+            tag_rollout.require(env, self.actor)
+        self._rollout_key, self._rollout_index = None, 0
 
     def _log_prob(self, mean, act):
         k = act.shape[-1]
@@ -52,6 +58,8 @@ class PPO:
         return self.critic(obs).squeeze(-1), self._log_prob(self.actor(obs), acts)
 
     def rollout(self):
+        if self.rollout_backend == "cuda":
+            return self._rollout_cuda()
         env = self.env
         cycles = max(1, self.max_timesteps_per_episode // env.num_agents)
         obs_b, act_b, lp_b, rtg_b, ep_ret, ep_len, t = [], [], [], [], [], [], 0
@@ -80,6 +88,23 @@ class PPO:
             ep_ret.extend(R.sum(0).sum(-1).tolist()); ep_len.extend([R.shape[0] * env.num_agents] * env.E)
         self.logger["batch_rews"], self.logger["batch_lens"] = ep_ret, ep_len
         return torch.cat(obs_b), torch.cat(act_b), torch.cat(lp_b), torch.cat(rtg_b), ep_len
+
+    def _rollout_cuda(self):
+        """``rollout()`` as one kernel launch with the shared actor; samples come back in the torch path's
+        [cycle, world, predator] order."""
+        from ..ops import tag_rollout
+        env = self.env
+        T = min(max(1, self.max_timesteps_per_episode // env.num_agents), env.max_cycles)
+        n_ep = max(1, -(-self.timesteps_per_batch // (env.n_adv * env.E * T)))
+        if self._rollout_key is None:
+            self._rollout_key = tag_rollout.draw_key()
+        out = tag_rollout.rollout(env, self.actor, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
+                                  key=self._rollout_key, index=self._rollout_index)
+        self._rollout_index += 1
+        flat = lambda x: x.transpose(0, 1).reshape(-1, *x.shape[2:])      # [N, R, ...] -> [R * N, ...]
+        ep_len = [T * env.num_agents] * (n_ep * env.E)
+        self.logger["batch_rews"], self.logger["batch_lens"] = out["ep_returns"].tolist(), ep_len
+        return flat(out["obs"]), flat(out["acts"]), flat(out["log_probs"]), flat(out["rtgs"]), ep_len
 
     def learn(self, total_timesteps):
         print(f"Learning... Running {self.max_timesteps_per_episode} timesteps per episode, "
@@ -114,7 +139,7 @@ class PPO:
         (the reference opens a pyglet window during rollouts, RL/ppo.py:197-199)."""
         from .eval_policy import rollout, save_rollout_gif
         os.makedirs(self.out_dir, exist_ok=True)
-        _, _, traj = rollout(self.actor, self.env, record=True)
+        _, _, traj = rollout(self.actor, self.env, record=True, backend=self.rollout_backend)
         return save_rollout_gif(self.env, traj, os.path.join(self.out_dir, f"render_{self.ID}_{i}.gif"))
 
     def save(self):

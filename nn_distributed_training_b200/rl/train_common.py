@@ -16,6 +16,8 @@ def parse_args(argv=None, default_id=0):
     ap.add_argument("--max_rl_timesteps", type=int, default=10_000_000)
     ap.add_argument("--num_envs", type=int, default=16, help="worlds stepped in lock-step by the batched environment")
     ap.add_argument("--device", default="cpu")
+    ap.add_argument("--rollout", choices=("torch", "cuda"), default="torch",
+                    help="cuda: each batch's rollout is one fused kernel launch (needs --device cuda)")
     ap.add_argument("--ID", type=int, default=default_id, help="suffix of the files written to --out_dir")
     ap.add_argument("--out_dir", default="./trained")
     ap.add_argument("--save_freq", type=int, default=10)
@@ -33,7 +35,8 @@ def make_problem(args):
                        max_cycles=STEPS_PER_EPISODE, device=args.device, seed=args.seed)
     hyper = {"timesteps_per_batch": 2000, "max_timesteps_per_episode": STEPS_PER_EPISODE, "gamma": 0.99,
              "n_updates_per_iteration": 5, "lr": 3e-4, "clip": 0.2, "render": bool(args.render),
-             "render_every_i": args.render_every_i, "save_freq": args.save_freq, "seed": args.seed}
+             "render_every_i": args.render_every_i, "save_freq": args.save_freq, "seed": args.seed,
+             "rollout_backend": args.rollout}
     obs_dim = env.observation_spaces["adversary_0"].shape[0]
     act_dim = env.action_spaces["adversary_0"].shape[0]
     base_actor = FFReLUNet([obs_dim, 64, 64, 64, act_dim])
