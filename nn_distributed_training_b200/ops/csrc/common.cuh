@@ -144,8 +144,58 @@ NNDT_DEVINL int frow(int m0, int lane, int i) { return m0 + (lane >> 2) + 8 * (i
 NNDT_DEVINL int fcol(int n0, int lane, int i) { return n0 + 2 * (lane & 3) + (i & 1); }
 
 // operand readers: at(s, ld)(i, j) = s[i][j], at_t(s, ld)(i, j) = s[j][i] of a row-major array with row stride ld
-NNDT_DEVINL auto at(const double* s, int ld) { return [s, ld](int i, int j) { return s[i * ld + j]; }; }
-NNDT_DEVINL auto at_t(const double* s, int ld) { return [s, ld](int i, int j) { return s[j * ld + i]; }; }
+template <class T> NNDT_DEVINL auto at(const T* s, int ld) { return [s, ld](int i, int j) { return s[i * ld + j]; }; }
+template <class T> NNDT_DEVINL auto at_t(const T* s, int ld) { return [s, ld](int i, int j) { return s[j * ld + i]; }; }
+
+// ---- FP32 on TF32 tensor cores with the 3xTF32 split ----------------------------------------------------------
+// mma.sync m16n8k8 TF32 with x = hi + lo (both TF32) and a.b ~ a_lo.b_hi + a_hi.b_lo + a_hi.b_hi, which keeps
+// fp32-level accuracy: the framework's contract is fp32 training, not TF32.
+// Fragment coordinates (g = lane >> 2, t = lane & 3):
+//   A (16x8, row major): a0 (g, t) a1 (g+8, t) a2 (g, t+4) a3 (g+8, t+4)
+//   B (8x8, col major) : b0 (k=t, n=g) b1 (k=t+4, n=g)
+//   C (16x8)           : c0 (g, 2t) c1 (g, 2t+1) c2 (g+8, 2t) c3 (g+8, 2t+1)   (as the DMMA tile)
+__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
+  const float r = x - __uint_as_float(hi);
+  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
+}
+__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
+}
+struct FragA { uint32_t hi[4], lo[4]; };
+struct FragB { uint32_t hi[2], lo[2]; };
+__device__ __forceinline__ FragA make_frag_a(float a0, float a1, float a2, float a3) {
+  FragA f;
+  split_tf32(a0, f.hi[0], f.lo[0]); split_tf32(a1, f.hi[1], f.lo[1]);
+  split_tf32(a2, f.hi[2], f.lo[2]); split_tf32(a3, f.hi[3], f.lo[3]);
+  return f;
+}
+__device__ __forceinline__ FragB make_frag_b(float b0, float b1) {
+  FragB f;
+  split_tf32(b0, f.hi[0], f.lo[0]); split_tf32(b1, f.hi[1], f.lo[1]);
+  return f;
+}
+__device__ __forceinline__ void mma3(float (&c)[4], const FragA& a, const FragB& b) {
+  mma_tf32(c, a.lo, b.hi);   // small terms first
+  mma_tf32(c, a.hi, b.lo);
+  mma_tf32(c, a.hi, b.hi);
+}
+
+// The fp32 counterpart of gemm(): c[j] += sum_k A(m0 + ., k) B(k, n0 + 8 j + .) over k < K (a multiple of 8), 3xTF32
+template <int NJ, class FA, class FB>
+NNDT_DEVINL void gemm(float (&c)[NJ][4], int m0, int n0, int K, int lane, FA A, FB B) {
+  const int g = lane >> 2, t = lane & 3;
+#pragma unroll 2
+  for (int k0 = 0; k0 < K; k0 += 8) {
+    const int k = k0 + t;
+    const FragA a = make_frag_a(A(m0 + g, k), A(m0 + g + 8, k), A(m0 + g, k + 4), A(m0 + g + 8, k + 4));
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) mma3(c[j], a, make_frag_b(B(k, n0 + 8 * j + g), B(k + 4, n0 + 8 * j + g)));
+  }
+}
 
 // cp.async helpers (LDGSTS)
 NNDT_DEVINL void cp_async16(void* smem, const void* gmem) {

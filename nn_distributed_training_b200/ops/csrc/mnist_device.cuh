@@ -139,43 +139,9 @@ __device__ __forceinline__ void conv_relu_pool(Smem<SPB, NT>& sm, int tid) {
 }
 
 // ---- tensor-core helpers for the three fc1-sized GEMMs (64 x 432 x <=8 samples) -----------------------------
-// mma.sync m16n8k8 TF32 with the 3xTF32 split (x = hi + lo, both TF32; a.b ~ a_lo.b_hi + a_hi.b_lo + a_hi.b_hi),
-// which keeps fp32-level accuracy: the framework's contract is fp32 training, not TF32.  A warpgroup-wide wgmma
-// tile does not fit here: the split needs hi and lo copies of the 110 KB weight tile in shared memory, and a 64 x 8
-// output tile would leave most of it idle — these GEMMs are latency-, not throughput-bound.
-// Fragment coordinates (g = lane >> 2, t = lane & 3):
-//   A (16x8, row major): a0 (g, t) a1 (g+8, t) a2 (g, t+4) a3 (g+8, t+4)
-//   B (8x8, col major) : b0 (k=t, n=g) b1 (k=t+4, n=g)
-//   C (16x8)           : c0 (g, 2t) c1 (g, 2t+1) c2 (g+8, 2t) c3 (g+8, 2t+1)
-__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(hi) : "f"(x));
-  const float r = x - __uint_as_float(hi);
-  asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(lo) : "f"(r));
-}
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], const uint32_t (&b)[2]) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b[0]), "r"(b[1]));
-}
-struct FragA { uint32_t hi[4], lo[4]; };
-struct FragB { uint32_t hi[2], lo[2]; };
-__device__ __forceinline__ FragA make_frag_a(float a0, float a1, float a2, float a3) {
-  FragA f;
-  split_tf32(a0, f.hi[0], f.lo[0]); split_tf32(a1, f.hi[1], f.lo[1]);
-  split_tf32(a2, f.hi[2], f.lo[2]); split_tf32(a3, f.hi[3], f.lo[3]);
-  return f;
-}
-__device__ __forceinline__ FragB make_frag_b(float b0, float b1) {
-  FragB f;
-  split_tf32(b0, f.hi[0], f.lo[0]); split_tf32(b1, f.hi[1], f.lo[1]);
-  return f;
-}
-__device__ __forceinline__ void mma3(float (&c)[4], const FragA& a, const FragB& b) {
-  mma_tf32(c, a.lo, b.hi);   // small terms first
-  mma_tf32(c, a.hi, b.lo);
-  mma_tf32(c, a.hi, b.hi);
-}
+// The 3xTF32 mma.sync helpers (common.cuh) keep fp32-level accuracy.  A warpgroup-wide wgmma tile does not fit here:
+// the split needs hi and lo copies of the 110 KB weight tile in shared memory, and a 64 x 8 output tile would leave
+// most of it idle — these GEMMs are latency-, not throughput-bound.
 
 // fc1 pre-activation partials: hpart[kg][s][j] = sum_{k in group kg} W1[j][k] a1[s][k]
 // warp w: rows j0 = 16 (w & 3), k-group kg = w >> 2 (9 k-steps of 8)

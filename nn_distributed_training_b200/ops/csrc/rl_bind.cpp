@@ -1,4 +1,4 @@
-// Binding of the fused predator-prey rollout (tag_rollout.cu).
+// Bindings of the fused predator-prey rollout (tag_rollout.cu) and of the PPO update kernels (ppo_update.cu).
 #include <torch/extension.h>
 #include <ATen/cuda/CUDAContext.h>
 #include <pybind11/pybind11.h>
@@ -7,6 +7,7 @@
 #include <stdexcept>
 #include <string>
 
+#include "ppo_update.h"
 #include "tag_rollout.h"
 
 namespace py = pybind11;
@@ -53,6 +54,50 @@ tag::Args tag_args(const py::dict& d) {
   a.eps = mptr(d, "eps"); a.pos_trace = mptr(d, "pos_trace");
   return a;
 }
+
+// W / b / gW / gb: [N][2][nl] pointers (gW / gb may be absent for the advantage pass).
+ppo::Args ppo_args(const py::dict& d) {
+  ppo::Args a{};
+  a.dtype64 = d["dtype64"].cast<int>();
+  a.N = d["N"].cast<int>();
+  a.R = d["R"].cast<int>();
+  auto dims = d["dims"].cast<std::vector<std::vector<int>>>();
+  if (a.N < 1 || a.N > ppo::kMaxNodes || dims.size() != 2) throw std::runtime_error("ppo_update: bad network description");
+  for (int n = 0; n < 2; ++n) {
+    a.nl[n] = dims[n].empty() ? 0 : (int)dims[n].size() - 1;   // no actor: the advantage pass
+    if (a.nl[n] > ppo::kMaxLayers || (a.nl[n] < 1 && (n == ppo::kCritic || !dims[n].empty())))
+      throw std::runtime_error("ppo_update: bad network description");
+    for (int l = 0; l < (int)dims[n].size(); ++l) a.dims[n][l] = dims[n][l];
+  }
+  using P3 = std::vector<std::vector<std::vector<uint64_t>>>;
+  auto table = [&](const char* k, bool required) {
+    P3 t;
+    if (d.contains(k) && !d[k].is_none()) t = d[k].cast<P3>();
+    else if (required) throw std::runtime_error(std::string("ppo_update: missing ") + k);
+    if (!t.empty() && (int)t.size() != a.N) throw std::runtime_error("ppo_update: bad network description");
+    for (auto& node : t) {
+      if (node.size() != 2) throw std::runtime_error("ppo_update: bad network description");
+      for (int n = 0; n < 2; ++n)
+        if ((int)node[n].size() != a.nl[n]) throw std::runtime_error("ppo_update: bad network description");
+    }
+    return t;
+  };
+  const P3 W = table("W", true), b = table("b", true), gW = table("gW", false), gb = table("gb", false);
+  for (int i = 0; i < a.N; ++i)
+    for (int n = 0; n < 2; ++n)
+      for (int l = 0; l < a.nl[n]; ++l) {
+        a.net[i][n].W[l] = reinterpret_cast<const void*>(W[i][n][l]);
+        a.net[i][n].b[l] = reinterpret_cast<const void*>(b[i][n][l]);
+        a.net[i][n].gW[l] = gW.empty() ? nullptr : reinterpret_cast<void*>(gW[i][n][l]);
+        a.net[i][n].gb[l] = gb.empty() ? nullptr : reinterpret_cast<void*>(gb[i][n][l]);
+      }
+  a.obs = cptr(d, "obs"); a.acts = cptr(d, "acts"); a.old_lp = cptr(d, "old_lp"); a.rtgs = cptr(d, "rtgs");
+  a.adv = mptr(d, "adv");
+  a.clip = d["clip"].cast<double>(); a.cov_var = d["cov_var"].cast<double>(); a.lp_const = d["lp_const"].cast<double>();
+  a.losses = mptr(d, "losses");
+  a.nonfinite = reinterpret_cast<int*>(mptr(d, "nonfinite"));
+  return a;
+}
 }  // namespace
 
 void bind_rl(py::module& m) {
@@ -61,5 +106,21 @@ void bind_rl(py::module& m) {
     if (const char* why = tag::check(a)) throw std::runtime_error(std::string("tag_rollout: ") + why);
     const cudaError_t e = tag::launch(a, at::cuda::getCurrentCUDAStream().stream());
     if (e != cudaSuccess) throw std::runtime_error(std::string("tag_rollout: ") + cudaGetErrorString(e));
+  });
+  m.def("ppo_grads", [](const py::dict& d) {
+    const ppo::Args a = ppo_args(d);
+    if (const char* why = ppo::check(a, true)) throw std::runtime_error(std::string("ppo_grads: ") + why);
+    const ppo::Plan p = ppo::plan(a, true);
+    if (p.err != cudaSuccess) throw std::runtime_error(std::string("ppo_grads: ") + cudaGetErrorString(p.err));
+    // partial slots from the caching allocator, on the current device and stream
+    at::Tensor work = at::empty({(int64_t)p.work_bytes}, at::TensorOptions().dtype(at::kByte).device(at::kCUDA));
+    const cudaError_t e = ppo::grads(a, p, work.data_ptr(), at::cuda::getCurrentCUDAStream().stream());
+    if (e != cudaSuccess) throw std::runtime_error(std::string("ppo_grads: ") + cudaGetErrorString(e));
+  });
+  m.def("ppo_advantages", [](const py::dict& d) {
+    const ppo::Args a = ppo_args(d);
+    if (const char* why = ppo::check(a, false)) throw std::runtime_error(std::string("ppo_advantages: ") + why);
+    const cudaError_t e = ppo::advantages(a, at::cuda::getCurrentCUDAStream().stream());
+    if (e != cudaSuccess) throw std::runtime_error(std::string("ppo_advantages: ") + cudaGetErrorString(e));
   });
 }

@@ -38,6 +38,26 @@ def _linears(actor) -> Optional[List[nn.Linear]]:
     return [m for m in actor.seq if isinstance(m, nn.Linear)]
 
 
+def relu_mlp_shape(nets: Sequence[nn.Module], what: str, dtype: torch.dtype):
+    """``(shape, None)`` if every net is a ReLU MLP (``FFReLUNet``) with biases, parameters of ``dtype``, one common
+    shape ``[d0, h1..hk, out]`` with k <= 4 hidden layers and widths <= 64 — what the sm_90a RL kernels run — and
+    ``(None, reason)`` otherwise.  ``what`` names the nets in the reason ("actor", "critic")."""
+    shape = None
+    for a in nets:
+        lin = _linears(a)
+        if lin is None:
+            return None, f"{what} {type(a).__name__} is not a ReLU MLP (FFReLUNet)"
+        s = [lin[0].in_features] + [m.out_features for m in lin]
+        if shape is not None and s != shape:
+            return None, f"predators' {what}s differ in shape"
+        shape = s
+        if any(m.bias is None for m in lin) or any(p.dtype != dtype for p in a.parameters()):
+            return None, f"{what} parameters must have biases and the dtype {dtype}"
+    if not 1 <= len(shape) - 1 <= MAX_LAYERS or any(not 1 <= w <= MAX_WIDTH for w in shape):
+        return None, f"{what} {shape}: needs <= {MAX_LAYERS - 1} hidden layers of width <= {MAX_WIDTH}"
+    return shape, None
+
+
 def unsupported_reason(env, actors) -> Optional[str]:
     """Why the kernel cannot run this environment / these actors (``None`` if it can).  The device is not checked."""
     acts = _actor_list(env, actors)
@@ -50,19 +70,9 @@ def unsupported_reason(env, actors) -> Optional[str]:
     if env.dtype not in (torch.float32, torch.float64):
         return f"environment dtype {env.dtype} (needs float32 or float64)"
     obs_dim = env.observation_spaces["adversary_0"].shape[0]
-    shape = None
-    for a in acts:
-        lin = _linears(a)
-        if lin is None:
-            return f"actor {type(a).__name__} is not a ReLU MLP (FFReLUNet)"
-        s = [lin[0].in_features] + [m.out_features for m in lin]
-        if shape is not None and s != shape:
-            return "predators' actors differ in shape"
-        shape = s
-        if any(m.bias is None for m in lin) or any(p.dtype != env.dtype for p in a.parameters()):
-            return f"actor parameters must have biases and the environment's dtype {env.dtype}"
-    if not 1 <= len(shape) - 1 <= MAX_LAYERS or any(not 1 <= w <= MAX_WIDTH for w in shape):
-        return f"actor {shape}: needs <= {MAX_LAYERS - 1} hidden layers of width <= {MAX_WIDTH}"
+    shape, why = relu_mlp_shape(acts, "actor", env.dtype)
+    if why is not None:
+        return why
     if shape[0] != obs_dim or shape[-1] != ACT_DIM:
         return f"actor {shape}: needs input {obs_dim} and output {ACT_DIM}"
     return None

@@ -25,7 +25,8 @@ class ReferenceProblemAdapter:
     (``N, graph, models, local_batch_loss(i), evaluate_metrics, update_graph``)
     so the arena-based optimizers can drive it: all nodes are local, the models'
     parameters are re-pointed into arena rows and gradients come from autograd.
-    Used for user-defined problems and the PPO problem (rl/dist_ppo.py)."""
+    Used for user-defined problems and the PPO problem (rl/dist_ppo.py).  A problem with a non-None
+    ``batched_grads(grad_rows)`` computes every node's gradient in one call instead."""
 
     fused = None
     backend = "torch"
@@ -65,6 +66,12 @@ class ReferenceProblemAdapter:
         return t
 
     def compute_grads(self):
+        hook = getattr(self.inner, "batched_grads", None)
+        if hook is not None:   # one call fills every node's arena.grad row (e.g. DistPPOProblem's update kernels)
+            if getattr(self, "_grad_views", None) is None:
+                self._grad_views = [self.layout.views(self.arena.grad[i]) for i in range(self.N)]
+            torch.sum(hook(self._grad_views), dim=1, out=self.last_losses)
+            return self.last_losses
         for i in range(self.N):
             loss = self.inner.local_batch_loss(i)
             grads = torch.autograd.grad(loss, list(self.models[i].parameters()))

@@ -11,6 +11,7 @@ def get_args(argv=None):
     p.add_argument("--total_timesteps", type=int, default=10_000_000)
     p.add_argument("--device", type=str, default="cpu")
     p.add_argument("--rollout", choices=("torch", "cuda"), default="torch")  # cuda: fused rollout kernel (--device cuda)
+    p.add_argument("--update", choices=("torch", "cuda"), default="torch")   # cuda: fused PPO update kernels (--device cuda)
     p.add_argument("--render", type=str, default="")          # test mode: write a GIF of the first episode here
     p.add_argument("--out_dir", type=str, default="./trained")  # train mode: weights + reward curves
     p.add_argument("--ID", type=int, default=0)

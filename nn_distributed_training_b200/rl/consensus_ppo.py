@@ -50,6 +50,7 @@ class _ConsensusPPO:
             self.pr.split_rollout_marl()
             self.pr.update_advantage()
             self._consensus(k)
+            self.pr.check_update()
             self.avg_ep_rews.append(self.pr.avg_episode_reward())
             self.timesteps.append(self.pr.logger["t_so_far"])
             self.agreements.append(agreement(self.pr))

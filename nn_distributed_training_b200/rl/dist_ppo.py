@@ -25,9 +25,12 @@ from .simple_tag import SimpleTagEnv, heuristic_prey_action
 class DistPPOProblem:
     # defaults of the reference's _init_hyperparameters (:391-436) — set explicitly, no exec()
     # rollout_backend "cuda": each batch is one fused kernel launch (ops/tag_rollout.py) with its own Philox noise stream
+    # update_backend "cuda": advantages and every node's gradients per primal step are fused kernels (ops/ppo_update.py);
+    # a non-finite actor mean then raises from check_update(), which the trainers call at the end of every iteration,
+    # and at the latest from the next update_advantage() -- not inside the primal step as on the torch path
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
                     lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
-                    rollout_backend="torch")
+                    rollout_backend="torch", update_backend="torch")
 
     def __init__(self, base_actor, base_critic, graph, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
@@ -64,6 +67,16 @@ class DistPPOProblem:
             from ..ops import tag_rollout
             tag_rollout.require(env, self.actors)
         self._rollout_key, self._rollout_index = None, 0
+        if self.update_backend not in ("torch", "cuda"):
+            raise ValueError(f"update_backend must be 'torch' or 'cuda', not {self.update_backend!r}")
+        # batched gradient hook of ReferenceProblemAdapter.compute_grads (None: per-node autograd)
+        self.batched_grads = None
+        if self.update_backend == "cuda":
+            from ..ops import ppo_update
+            ppo_update.require(self.actors, self.critics)
+            self.batched_grads = self._cuda_grads
+            self._nonfinite = torch.zeros(1, device=self.device, dtype=torch.int32)
+            self._checked = True   # the flag holds nothing unchecked
 
     @property
     def actors(self):
@@ -133,6 +146,11 @@ class DistPPOProblem:
         self.curr_acts = {i: torch.cat(act_b[i]) for i in range(N)}
         self.curr_log_probs = {i: torch.cat(lp_b[i]) for i in range(N)}
         self.curr_rtgs = {i: torch.cat([r.reshape(-1) for r in rtg_b[i]]) for i in range(N)}
+        if self.update_backend == "cuda":
+            self._stack_batch(dict(obs=torch.stack([self.curr_obs[i] for i in range(N)]),
+                                   acts=torch.stack([self.curr_acts[i] for i in range(N)]),
+                                   log_probs=torch.stack([self.curr_log_probs[i] for i in range(N)]),
+                                   rtgs=torch.stack([self.curr_rtgs[i] for i in range(N)])))
         self.logger["batch_rews"] = ep_returns
         self.logger["batch_lens"] = ep_lens
         self.logger["t_so_far"] += int(np.sum(ep_lens))
@@ -149,15 +167,20 @@ class DistPPOProblem:
         out = tag_rollout.rollout(env, self.actors, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
                                   key=self._rollout_key, index=self._rollout_index)
         self._rollout_index += 1
-        self.curr_obs = {i: out["obs"][i] for i in range(N)}
-        self.curr_acts = {i: out["acts"][i] for i in range(N)}
-        self.curr_log_probs = {i: out["log_probs"][i] for i in range(N)}
-        self.curr_rtgs = {i: out["rtgs"][i] for i in range(N)}
+        self._stack_batch(out)
         ep_lens = [T * env.num_agents] * (n_ep * env.E)
         self.logger["batch_rews"] = out["ep_returns"].tolist()
         self.logger["batch_lens"] = ep_lens
         self.logger["t_so_far"] += int(np.sum(ep_lens))
         self.logger["i_so_far"] += 1
+
+    def _stack_batch(self, out):
+        """Keep the batch as ``[N, R, ...]`` tensors (the update kernels' layout); ``curr_*[i]`` are views of row i."""
+        self._batch = {k: out[k] for k in ("obs", "acts", "log_probs", "rtgs")}
+        self.curr_obs = {i: out["obs"][i] for i in range(self.N)}
+        self.curr_acts = {i: out["acts"][i] for i in range(self.N)}
+        self.curr_log_probs = {i: out["log_probs"][i] for i in range(self.N)}
+        self.curr_rtgs = {i: out["rtgs"][i] for i in range(self.N)}
 
     def compute_rtgs(self, batch_rews):
         out = []
@@ -169,6 +192,12 @@ class DistPPOProblem:
         return torch.tensor(out, dtype=torch.float)
 
     def update_advantage(self):
+        if self.update_backend == "cuda":
+            from ..ops import ppo_update
+            self.check_update()   # the previous iteration's steps, if the driver did not check them
+            self._adv = ppo_update.advantages(self.critics, self._batch["obs"], self._batch["rtgs"])
+            self.A_k = {i: self._adv[i] for i in range(self.N)}
+            return
         self.A_k = {}
         with torch.no_grad():
             for i in range(self.N):
@@ -192,6 +221,29 @@ class DistPPOProblem:
         so the sum's gradient is the pair of separate gradients the reference uses."""
         a, c = self.ev_ppo_loss(i)
         return a + c
+
+    def _cuda_grads(self, grad_out):
+        """Every node's gradient of ``local_batch_loss`` at once (update_backend "cuda"): fills ``grad_out[i]`` (one
+        tensor per parameter of models[i]) and returns the per-node losses ``[N, 2]`` without a host synchronisation."""
+        from ..ops import ppo_update
+        b = self._batch
+        losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], b["rtgs"], self._adv,
+                                  self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite)
+        self.logger["actor_losses"].extend(losses[i, 0] for i in range(self.N))
+        self._checked = False
+        return losses
+
+    def check_update(self):
+        """End of an iteration: under update_backend "cuda", raise if any actor mean of the primal steps since the last
+        check was not finite (the torch path raises inside the step).  One host synchronisation, none if no step ran
+        since the last check."""
+        if self.update_backend != "cuda" or self._checked:
+            return
+        bad = int(self._nonfinite.item())
+        self._nonfinite.zero_()
+        self._checked = True
+        if bad:
+            raise NameError("actor returning something weird")
 
     def update_graph(self):
         return

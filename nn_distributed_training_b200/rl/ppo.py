@@ -17,7 +17,7 @@ from .simple_tag import SimpleTagEnv, heuristic_prey_action
 class PPO:
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
                     lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
-                    ID=0, out_dir="./trained", rollout_backend="torch")
+                    ID=0, out_dir="./trained", rollout_backend="torch", update_backend="torch")
 
     def __init__(self, policy_class, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
@@ -43,6 +43,11 @@ class PPO:
             from ..ops import tag_rollout
             tag_rollout.require(env, self.actor)
         self._rollout_key, self._rollout_index = None, 0
+        if self.update_backend not in ("torch", "cuda"):
+            raise ValueError(f"update_backend must be 'torch' or 'cuda', not {self.update_backend!r}")
+        if self.update_backend == "cuda":
+            from ..ops import ppo_update
+            ppo_update.require(self.actor, self.critic)
 
     def _log_prob(self, mean, act):
         k = act.shape[-1]
@@ -114,18 +119,10 @@ class PPO:
             obs, acts, lps, rtgs, lens = self.rollout()
             t_so_far += int(np.sum(lens)); i_so_far += 1
             self.logger["t_so_far"], self.logger["i_so_far"] = t_so_far, i_so_far
-            with torch.no_grad():
-                V, _ = self.evaluate(obs, acts)
-            A = rtgs - V
-            A = (A - A.mean()) / (A.std() + 1e-10)
-            for _ in range(self.n_updates_per_iteration):
-                V, cur = self.evaluate(obs, acts)
-                ratios = torch.exp(cur - lps)
-                actor_loss = (-torch.min(ratios * A, torch.clamp(ratios, 1 - self.clip, 1 + self.clip) * A)).mean()
-                critic_loss = nn.functional.mse_loss(V, rtgs)
-                self.actor_optim.zero_grad(); actor_loss.backward(); self.actor_optim.step()
-                self.critic_optim.zero_grad(); critic_loss.backward(); self.critic_optim.step()
-                self.logger["actor_losses"].append(actor_loss.detach())
+            if self.update_backend == "cuda":
+                self._update_cuda(obs, acts, lps, rtgs)
+            else:
+                self._update_torch(obs, acts, lps, rtgs)
             self.avg_ep_rews.append(float(np.mean(self.logger["batch_rews"])))
             self.timesteps.append(t_so_far)
             self._log_summary()
@@ -133,6 +130,37 @@ class PPO:
                 self.save()
             if self.render and i_so_far % self.render_every_i == 0:
                 self.render_episode(i_so_far)
+
+    def _update_torch(self, obs, acts, lps, rtgs):
+        with torch.no_grad():
+            V, _ = self.evaluate(obs, acts)
+        A = rtgs - V
+        A = (A - A.mean()) / (A.std() + 1e-10)
+        for _ in range(self.n_updates_per_iteration):
+            V, cur = self.evaluate(obs, acts)
+            ratios = torch.exp(cur - lps)
+            actor_loss = (-torch.min(ratios * A, torch.clamp(ratios, 1 - self.clip, 1 + self.clip) * A)).mean()
+            critic_loss = nn.functional.mse_loss(V, rtgs)
+            self.actor_optim.zero_grad(); actor_loss.backward(); self.actor_optim.step()
+            self.critic_optim.zero_grad(); critic_loss.backward(); self.critic_optim.step()
+            self.logger["actor_losses"].append(actor_loss.detach())
+
+    def _update_cuda(self, obs, acts, lps, rtgs):
+        """The same update with the fused kernels (ops/ppo_update.py): the batch is one node of the kernels' [N, R, ...]
+        layout; each step's gradients land in p.grad and the two Adam steps run as on the torch path."""
+        from ..ops import ppo_update
+        obs, acts, lps, rtgs = obs.unsqueeze(0), acts.unsqueeze(0), lps.unsqueeze(0), rtgs.unsqueeze(0)
+        A = ppo_update.advantages(self.critic, obs, rtgs)
+        params = list(self.actor.parameters()) + list(self.critic.parameters())
+        for _ in range(self.n_updates_per_iteration):
+            for p in params:
+                if p.grad is None:
+                    p.grad = torch.zeros_like(p)
+            losses = ppo_update.grads(self.actor, self.critic, obs, acts, lps, rtgs, A, self.clip, self.cov_var,
+                                      [[p.grad for p in params]])
+            self.actor_optim.step()
+            self.critic_optim.step()
+            self.logger["actor_losses"].append(losses[0, 0])
 
     def render_episode(self, i):
         """``render=True``: an animated GIF of one episode of the current policy every ``render_every_i`` iterations

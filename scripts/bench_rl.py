@@ -1,12 +1,19 @@
-"""Time multi-agent PPO rollouts and whole DiNNO-PPO iterations for the three rollout paths.
+"""Time multi-agent PPO rollouts and whole DiNNO-PPO iterations for the three rollout paths and the two update paths.
 
-    python scripts/bench_rl.py [--envs 16 256 4096] [--paths cpu cuda kernel] [--repeats 2]
+    python scripts/bench_rl.py [--envs 16 256 4096] [--paths cpu cuda kernel] [--updates torch cuda] [--repeats 2]
+    python scripts/bench_rl.py --profile OUT_DIR [--envs 16 4096]
 
 Paths: ``cpu`` = torch rollout on the CPU, ``cuda`` = torch rollout on the GPU, ``kernel`` = the fused rollout kernel
-(ops/csrc/tag_rollout.cu).  The problem is ``train_cadmm_multi``'s (3 predators, 1 prey, 8 obstacles, [12,64,64,64,5]
-actors, 2000 steps per batch, 50 cycles per episode); an iteration is the trainer's loop body: rollout, advantages and
-one DiNNO round of 5 primal steps.  Every timing ends in a device synchronise, follows a warm-up, and is repeated
-``--repeats`` times so the spread shows.  The card's name and power limit are printed by the same run.
+(ops/csrc/tag_rollout.cu).  Updates: ``torch`` = per-node autograd, ``cuda`` = the fused update kernels
+(ops/csrc/ppo_update.cu; GPU paths only).  The problem is ``train_cadmm_multi``'s (3 predators, 1 prey, 8 obstacles,
+[12,64,64,64,5] actors, 2000 steps per batch, 50 cycles per episode); an iteration is the trainer's loop body: rollout,
+advantages and one DiNNO round of 5 primal steps.  Every timing ends in a device synchronise and follows a warm-up; the
+update paths of one (num_envs, path) are timed alternately, ``--repeats`` times, so the spread shows.  The card's name
+and power limit are printed by the same run.
+
+``--profile`` is a separate run (tracing slows the host): one ``torch.profiler`` trace per (num_envs, update) of the
+kernel rollout path under OUT_DIR, and a split of an iteration's wall time into the rollout kernel, the update kernels,
+the other device work (consensus ops) and host gaps, plus the grad kernel's achieved FLOP/s from ``grad_flops``.
 """
 from __future__ import annotations
 
@@ -41,10 +48,19 @@ def _timed(fn, dev, n):
     return (time.perf_counter() - t0) / n
 
 
-def bench(path, E, repeats, budget_s):
+def grad_flops(actor_shape, critic_shape):
+    """FLOP per sample of one primal step of the update: forward, dW and dH of every layer (no dH into the input)."""
+    f = 0
+    for shape in (actor_shape, critic_shape):
+        mac = [a * b for a, b in zip(shape[:-1], shape[1:])]
+        f += 2 * sum(mac) + 2 * sum(mac) + 2 * sum(mac[1:])
+    return f
+
+
+def setup(path, E, update):
     dev = "cpu" if path == "cpu" else "cuda"
     args = parse_args(["--num_envs", str(E), "--device", dev, "--rollout", "cuda" if path == "kernel" else "torch",
-                       "--seed", "0", "--no_writeout"])
+                       "--update", update, "--seed", "0", "--no_writeout"])
     pr, hyper = make_problem(args)
     conf = dict(common_conf(args), rho_init=1.0, rho_scaling=1.0, primal_lr_start=hyper["lr"], primal_lr_finish=0.001,
                 lr_decay_type="constant", persistant_primal_opt=False, primal_iterations=hyper["n_updates_per_iteration"],
@@ -56,48 +72,109 @@ def bench(path, E, repeats, budget_s):
         pr.split_rollout_marl()
         pr.update_advantage()
         tr._consensus(k[0])
+        pr.check_update()
         k[0] += 1
 
     iteration()                                           # warm-up: module loads, allocator, fused-kernel set-up
     pr.split_rollout_marl()
-    t_roll = _timed(pr.split_rollout_marl, dev, 1)
-    n_roll = max(1, min(200, int(budget_s / max(t_roll, 1e-6))))
-    t_it = _timed(iteration, dev, 1)
-    n_it = max(1, min(50, int(budget_s / max(t_it, 1e-6))))
+    return pr, iteration, dev
+
+
+def bench(path, E, updates, repeats, budget_s):
+    runs = {u: setup(path, E, u) for u in updates}
+    n = {}
+    for u, (pr, iteration, dev) in runs.items():
+        t_roll = _timed(pr.split_rollout_marl, dev, 1)
+        t_it = _timed(iteration, dev, 1)
+        n[u] = (max(1, min(200, int(budget_s / max(t_roll, 1e-6)))), max(1, min(50, int(budget_s / max(t_it, 1e-6)))))
     rows = []
     for r in range(repeats):
-        rows.append(dict(path=path, num_envs=E, repeat=r, rollout_ms=1e3 * _timed(pr.split_rollout_marl, dev, n_roll),
-                         iteration_ms=1e3 * _timed(iteration, dev, n_it), n_rollout=n_roll, n_iteration=n_it,
-                         samples_per_rollout=int(pr.curr_obs[0].shape[0]) * pr.N))
-        print(json.dumps(rows[-1]), flush=True)
+        for u, (pr, iteration, dev) in runs.items():       # update paths alternate within each repeat
+            n_roll, n_it = n[u]
+            rows.append(dict(path=path, update=u, num_envs=E, repeat=r,
+                             rollout_ms=1e3 * _timed(pr.split_rollout_marl, dev, n_roll),
+                             iteration_ms=1e3 * _timed(iteration, dev, n_it), n_rollout=n_roll, n_iteration=n_it,
+                             samples_per_rollout=int(pr.curr_obs[0].shape[0]) * pr.N))
+            print(json.dumps(rows[-1]), flush=True)
     return rows
+
+
+def profile(E, update, out_dir, n=5):
+    from torch.profiler import ProfilerActivity, profile as tprofile
+    pr, iteration, _ = setup("kernel", E, update)
+    torch.cuda.synchronize()
+    with tprofile(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+        t0 = time.perf_counter()
+        for _ in range(n):
+            iteration()
+        torch.cuda.synchronize()
+        wall = (time.perf_counter() - t0) / n
+    prof.export_chrome_trace(os.path.join(out_dir, f"trace_E{E}_{update}.json"))
+    split = dict(rollout_kernel=0.0, update_kernels=0.0, other_device=0.0)
+    grad_us, grad_calls = 0.0, 0
+    for ev in prof.key_averages():
+        dt = getattr(ev, "device_time_total", None)
+        if dt is None:
+            dt = ev.cuda_time_total
+        if ev.device_type.name != "CUDA" or dt <= 0:
+            continue
+        name = ev.key
+        if "tag_rollout" in name:
+            split["rollout_kernel"] += dt
+        elif "ppo_" in name or "adv_norm" in name:
+            split["update_kernels"] += dt
+            if "ppo_grad_kernel" in name and "true>" in name:
+                grad_us += dt
+                grad_calls += ev.count
+        else:
+            split["other_device"] += dt
+    row = {k: v / 1e3 / n for k, v in split.items()}           # ms per iteration
+    row.update(num_envs=E, update=update, iteration_ms_traced=1e3 * wall,
+               host_gaps_ms=1e3 * wall - sum(v / 1e3 / n for v in split.values()))
+    if grad_calls:
+        samples = int(pr.curr_obs[0].shape[0]) * pr.N
+        fl = grad_flops(pr.models[0].actor.shape, pr.models[0].critic.shape) * samples
+        row.update(grad_kernel_us=grad_us / grad_calls, grad_flop_per_call=fl,
+                   grad_tflops=fl / (grad_us / grad_calls * 1e-6) / 1e12)
+    print(json.dumps(row), flush=True)
+    return row
 
 
 def main(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument("--envs", type=int, nargs="+", default=[16, 256, 4096])
     ap.add_argument("--paths", nargs="+", default=["cpu", "cuda", "kernel"], choices=["cpu", "cuda", "kernel"])
+    ap.add_argument("--updates", nargs="+", default=["torch"], choices=["torch", "cuda"])
     ap.add_argument("--repeats", type=int, default=2)
+    ap.add_argument("--profile", default=None, help="profile the kernel rollout path with each update into this directory")
     ap.add_argument("--budget", type=float, default=2.0, help="seconds per timed window (at least one call)")
     ap.add_argument("--out", default=None, help="also write the rows as JSON here")
     a = ap.parse_args(argv)
-    if any(p != "cpu" for p in a.paths):
+    if any(p != "cpu" for p in a.paths) or a.profile:
         if not torch.cuda.is_available():
             raise SystemExit("the cuda and kernel paths need a CUDA device")
         q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv"], capture_output=True, text=True)
         print(q.stdout.strip(), flush=True)
     torch.set_num_threads(max(1, torch.get_num_threads()))
     print(f"cpu threads: {torch.get_num_threads()}", flush=True)
+    if a.profile:
+        os.makedirs(a.profile, exist_ok=True)
+        rows = [profile(E, u, a.profile) for E in a.envs for u in a.updates]
+        with open(os.path.join(a.profile, "split.json"), "w") as f:
+            json.dump(rows, f, indent=1)
+        return
     rows = []
     for E in a.envs:
         for p in a.paths:
-            rows += bench(p, E, a.repeats, a.budget)
-    print("\n| num_envs | path | rollout ms | iteration ms |\n|---|---|---|---|")
+            rows += bench(p, E, [u for u in a.updates if p != "cpu" or u == "torch"], a.repeats, a.budget)
+    print("\n| num_envs | path | update | rollout ms | iteration ms |\n|---|---|---|---|---|")
     for E in a.envs:
         for p in a.paths:
-            rs = [r for r in rows if r["num_envs"] == E and r["path"] == p]
-            print(f"| {E} | {p} | {', '.join(f'{r['rollout_ms']:.3g}' for r in rs)} | "
-                  f"{', '.join(f'{r['iteration_ms']:.3g}' for r in rs)} |")
+            for u in a.updates:
+                rs = [r for r in rows if r["num_envs"] == E and r["path"] == p and r["update"] == u]
+                if rs:
+                    print(f"| {E} | {p} | {u} | {', '.join(f'{r['rollout_ms']:.3g}' for r in rs)} | "
+                          f"{', '.join(f'{r['iteration_ms']:.3g}' for r in rs)} |")
     if a.out:
         with open(a.out, "w") as f:
             json.dump(rows, f, indent=1)
