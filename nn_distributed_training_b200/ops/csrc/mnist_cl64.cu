@@ -32,10 +32,13 @@ template <int MS>
 struct Smem {
   static constexpr int NO = MS / CL;           // samples a CTA owns for fc2, the loss and their backward
   static constexpr bool kDoublePix = MS <= 32; // pixels as normalised doubles; at MS = 64 they only fit as raw bytes
-  double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; later da1 [s][KC]
-  double a[MS * WS];         // A tile [s][k]; later the conv-grad warp sums
-  double h[MS * HS];         // partial H [s][j] (read by the peers); after barrier #2 dH [s][j]; later the conv-grad lists
-  alignas(16) unsigned char img[kDoublePix ? MS * PXR * 8 : MS * PXR];
+  // sample stride of the pixel rows; as doubles 282 (141 16-byte units, odd), so the same patch row of eight consecutive
+  // samples starts in eight different 16-byte bank groups
+  static constexpr int PXS = kDoublePix ? PXR + 2 : PXR;
+  double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; later the conv-grad warp sums
+  double a[MS * WS];         // A tile [s][k]; later da1 [k][s]
+  double h[MS * HS];         // partial H [s][j] (read by the peers); after barrier #2 dH [s][j]
+  alignas(16) unsigned char img[kDoublePix ? MS * PXS * 8 : MS * PXS];
   double lut[kDoublePix ? 1 : 256];                         // MS = 64: normalised value of each u8 pixel
   double h_loc[NO * HID > CL * 80 ? NO * HID : CL * 80];   // later (rank 0) the CTAs' conv-gradient shares [CL][80]
   double dh_loc[NO * HID];
@@ -60,6 +63,22 @@ NNDT_DEVINL double wmax(double v) {
   for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
+// one exchange step of warp_reduce_scatter16: the lanes with bit 2H set keep the upper half of their H values
+template <int H>
+NNDT_DEVINL void fold_half(double (&v)[16], int lane) {
+  const bool up = (lane & (2 * H)) != 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    const double send = up ? v[i] : v[i + H], keep = up ? v[i + H] : v[i];
+    v[i] = keep + __shfl_xor_sync(0xffffffffu, send, 2 * H);
+  }
+}
+// Sums v[0 .. 15] over the warp in a fixed order with 16 shuffles instead of 80: every exchange step halves the values a
+// lane keeps.  Afterwards lanes 2i and 2i + 1 hold the warp total of v[i] in v[0].
+NNDT_DEVINL void warp_reduce_scatter16(double (&v)[16], int lane) {
+  fold_half<8>(v, lane); fold_half<4>(v, lane); fold_half<2>(v, lane); fold_half<1>(v, lane);
+  v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
+}
 NNDT_DEVINL void stamp(long long* prof, int idx, int tid) {
   if (prof != nullptr && tid == 0) {
     long long t;
@@ -72,7 +91,7 @@ template <int MS>
 __global__ void __cluster_dims__(CL, 1, 1) __launch_bounds__(NT, 1)
 mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   using SM = Smem<MS>;
-  constexpr int NO = SM::NO;
+  constexpr int NO = SM::NO, PXS = SM::PXS;
   constexpr bool kDoublePix = SM::kDoublePix;
   static_assert(MS % 16 == 0 && NO <= NT / 32, "tile geometry");
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -87,7 +106,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   // pixel p (0 .. 279) of sample s's image rows 6c .. 6c+9.  fp32 inputs at MS = 64 have no room in shared memory and
   // are read from L2 (the rows were just loaded); invalid samples are masked wherever their pixels would count.
   auto pix = [&](int s, int p) -> double {
-    if constexpr (kDoublePix) return imgd[s * PXR + p];
+    if constexpr (kDoublePix) return imgd[s * PXS + p];
     else if (u8) return sm.lut[sm.img[s * PXR + p]];
     else return (double)__ldg(reinterpret_cast<const float*>(a.x) + (size_t)sm.sidx[s] * 784 + 6 * HW * c + p);
   };
@@ -166,7 +185,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
         const int s = o / 35, q = o - s * 35;
         if constexpr (kDoublePix) {
           const uint32_t w[2] = {pu[i].x, pu[i].y};
-          double* dst = imgd + s * PXR + 8 * q;
+          double* dst = imgd + s * PXS + 8 * q;
 #pragma unroll
           for (int j = 0; j < 8; ++j) dst[j] = ((double)((w[j >> 2] >> (8 * (j & 3))) & 0xff) * (1.0 / 255.0) - pmean) * pis;
         } else {
@@ -179,7 +198,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     for (int i = 0; i < NF4; ++i) {
       const int o = tid + i * NT;
       if (o < MS * 70) {
-        double* dst = imgd + (o / 70) * PXR + 4 * (o % 70);
+        double* dst = imgd + (o / 70) * PXS + 4 * (o % 70);
         dst[0] = pf[i].x; dst[1] = pf[i].y; dst[2] = pf[i].z; dst[3] = pf[i].w;
       }
     }
@@ -200,7 +219,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     double patch[6][6];
     if constexpr (kDoublePix) {
       // a patch row is six consecutive doubles starting at an even column: three 16-byte loads
-      const double* src = imgd + s * PXR + p0;
+      const double* src = imgd + s * PXS + p0;
 #pragma unroll
       for (int r = 0; r < 6; ++r)
 #pragma unroll
@@ -379,7 +398,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   }
   __syncthreads();      // every read of A (GEMM 3) is done
   stamp(prof, 10, tid);
-  double* da1 = sm.a;   // A's rows become da1 [s][KC], masked by ReLU'(a1)
+  double* da1 = sm.a;   // A's rows become da1 [k][s] (sample-minor for the conv-grad pass), masked by ReLU'(a1)
 #pragma unroll 1
   for (int t = warp; t < (MS / 16) * KT; t += NT / 32) {
     const int m0 = 16 * (t / KT), n0 = 8 * (t % KT);
@@ -389,77 +408,87 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       const int s = frow(m0, lane, i), k = fcol(n0, lane, i);
-      if (k < KC) da1[s * KC + k] = (sm.arg[s * KC + k] & 4) ? acc[0][i] : 0.0;
+      if (k < KC) da1[k * MS + s] = (sm.arg[s * KC + k] & 4) ? acc[0][i] : 0.0;
     }
   }
   __syncthreads();
   stamp(prof, 11, tid);
-  // ---- conv grads.  da1 is sparse (ReLU mask): (1) deterministic per-channel compaction of the non-zero (sample, cell)
-  //      entries (ballot + prefix over 32-entry chunks, so the order — and the fp64 sums — never depend on timing);
-  //      (2) five warps per channel walk that channel's dense list, each entry routes da1 to its argmax conv position;
-  //      (3) each warp folds its 26 sums over its lanes, and the five warp sums of a channel are added in warp order -------
-  constexpr int NI = MS * CELLS, NCH = NI / 32, CGW = 5, CGT = CGW * 32;     // entries / chunks per channel; warps / threads per channel
-  static_assert(F * CGW <= NT / 32 && NI % 32 == 0 && NI <= 4096, "conv-grad work split");
-  unsigned short* list = reinterpret_cast<unsigned short*>(sm.h);           // [F][NI] entries it | argmax << 12 (dH is dead)
-  int* ccount = reinterpret_cast<int*>(list + F * NI);                     // [F * NCH] chunk counts, then [F] totals
-  static_assert(sizeof(unsigned short) * F * NI + sizeof(int) * (F * NCH + F) <= sizeof(SM::h), "lists fit the dH tile");
-  for (int q = warp; q < F * NCH; q += NT / 32) {
-    const int ch = q / NCH, it = (q - ch * NCH) * 32 + lane;
-    const int s = it / CELLS, cell = it - s * CELLS;
-    const unsigned b = __ballot_sync(0xffffffffu, da1[s * KC + ch * CELLS + cell] != 0.0);
-    if (lane == 0) ccount[q] = __popc(b);
-  }
-  __syncthreads();
-  for (int q = warp; q < F * NCH; q += NT / 32) {
-    const int ch = q / NCH, qq = q - ch * NCH, it = qq * 32 + lane;
-    const int s = it / CELLS, cell = it - s * CELLS;
-    int pre = 0;
-    for (int j = lane; j < qq; j += 32) pre += ccount[ch * NCH + j];
+  // ---- conv grads without gathers: warps 3ky .. 3ky+2 own tap row ky of all three channels.  A thread walks whole pooled
+  //      rows (sample s, pooled row pr, px = 0 .. 11) with columns 2px .. 2px+5 of patch rows 2pr+ky and 2pr+ky+1 in
+  //      registers, two new columns per cell.  Each cell's gradient goes to all four pool positions, zero except at its
+  //      argmax, so every lane runs the same 20 DFMA per channel and no address depends on the argmax.  Warp 15 sums the
+  //      bias gradients.  Every warp folds its sums over its lanes and a tap row's three warp sums are added in warp order ---
+  constexpr int KW = 3, NRUN = MS * 3;   // warps per tap row; (sample, pooled row) runs
+  static_assert(KS * KW < NT / 32 && F * KS <= 16, "conv-grad work split");
+  double* wsums = sm.w;                  // [NT / 32][16] (W is dead)
+  // columns p, p + 1 (p even) of sample s's rows: one 16-byte load from the double rows
+  auto pix2 = [&](int s, int p) -> double2 {
+    if constexpr (kDoublePix) return *reinterpret_cast<const double2*>(imgd + s * PXS + p);
+    else return make_double2(pix(s, p), pix(s, p + 1));
+  };
+  if (warp < KS * KW) {
+    const int ky = warp / KW;
+    double acc[16];                      // [ch][kx]; slot 15 stays zero
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) pre += __shfl_xor_sync(0xffffffffu, pre, o);
-    const bool nz = da1[s * KC + ch * CELLS + cell] != 0.0;
-    const unsigned b = __ballot_sync(0xffffffffu, nz);
-    if (nz) list[ch * NI + pre + __popc(b & ((1u << lane) - 1u))] =
-        (unsigned short)(it | ((sm.arg[s * KC + ch * CELLS + cell] & 3) << 12));
-    if (qq == NCH - 1 && lane == 0) ccount[F * NCH + ch] = pre + __popc(b);
-  }
-  __syncthreads();
-  double* wsums = sm.w;                                                     // [F * CGW][26] (W is dead)
-  {
-    const int gch = warp / CGW, tl = tid - gch * CGT;
-    if (gch < F) {
-      double cacc[26];
+    for (int i = 0; i < 16; ++i) acc[i] = 0.0;
+#pragma unroll 1
+    for (int r = tid - ky * KW * 32; r < NRUN; r += KW * 32) {
+      const int s = r % MS, pr = r / MS;                   // consecutive lanes take consecutive samples
+      const int rb = (2 * pr + ky) * HW;
+      double x0[6], x1[6];
 #pragma unroll
-      for (int i = 0; i < 26; ++i) cacc[i] = 0.0;
-      const int n = ccount[F * NCH + gch];
-      for (int j = tl; j < n; j += CGT) {
-        const unsigned e = list[gch * NI + j];
-        const int it = e & 4095, ai = e >> 12;
-        const int s = it / CELLS, cell = it - s * CELLS;
-        const double g = da1[s * KC + gch * CELLS + cell];
-        const int pr = cell / PHW, px = cell - pr * PHW;
-        const int p0 = (2 * pr + (ai >> 1)) * HW + 2 * px + (ai & 1);
+      for (int px = 0; px < PHW; ++px) {
+        const int p = rb + 2 * px;
+        if (px == 0) {
 #pragma unroll
-        for (int ky = 0; ky < KS; ++ky)
+          for (int q = 0; q < 6; q += 2) {
+            const double2 u = pix2(s, p + q), v = pix2(s, p + HW + q);
+            x0[q] = u.x; x0[q + 1] = u.y; x1[q] = v.x; x1[q + 1] = v.y;
+          }
+        } else {
 #pragma unroll
-          for (int kx = 0; kx < KS; ++kx) cacc[ky * 5 + kx] += g * pix(s, p0 + ky * HW + kx);
-        cacc[25] += g;
+          for (int q = 0; q < 4; ++q) { x0[q] = x0[q + 2]; x1[q] = x1[q + 2]; }
+          const double2 u = pix2(s, p + 4), v = pix2(s, p + HW + 4);
+          x0[4] = u.x; x0[5] = u.y; x1[4] = v.x; x1[5] = v.y;
+        }
+#pragma unroll
+        for (int ch = 0; ch < F; ++ch) {
+          const int k = ch * CELLS + pr * PHW + px;
+          const double g = da1[k * MS + s];
+          const int ai = sm.arg[s * KC + k] & 3;
+          const double g00 = ai == 0 ? g : 0.0, g01 = ai == 1 ? g : 0.0, g10 = ai == 2 ? g : 0.0, g11 = ai == 3 ? g : 0.0;
+#pragma unroll
+          for (int kx = 0; kx < KS; ++kx) {
+            double& t = acc[ch * KS + kx];
+            t = fma(g00, x0[kx], t); t = fma(g01, x0[kx + 1], t);
+            t = fma(g10, x1[kx], t); t = fma(g11, x1[kx + 1], t);
+          }
+        }
       }
-#pragma unroll
-      for (int i = 0; i < 26; ++i) {
-        const double v = warp_sum(cacc[i]);
-        if (lane == 0) wsums[warp * 26 + i] = v;
-      }
+    }
+    warp_reduce_scatter16(acc, lane);
+    if ((lane & 1) == 0 && (lane >> 1) < F * KS) wsums[warp * 16 + (lane >> 1)] = acc[0];
+  } else if (warp == KS * KW) {
+#pragma unroll 1
+    for (int ch = 0; ch < F; ++ch) {
+      double v = 0.0;
+      for (int o = lane; o < CELLS * MS; o += 32) v += da1[ch * CELLS * MS + o];
+      v = warp_sum(v);
+      if (lane == 0) wsums[warp * 16 + ch] = v;
     }
   }
   __syncthreads();
-  if (tid < F * 26) {
-    const int ch = tid / 26, i = tid - ch * 26;
+  if (tid < 78) {
     double v = 0.0;
+    if (tid < 75) {
+      const int ch = tid / 25, t = tid - ch * 25, ky = t / KS, kx = t - ky * KS;
 #pragma unroll
-    for (int w = 0; w < CGW; ++w) v += wsums[(ch * CGW + w) * 26 + i];
+      for (int w = 0; w < KW; ++w) v += wsums[(ky * KW + w) * 16 + ch * KS + kx];
+    } else {
+      v = wsums[KS * KW * 16 + (tid - 75)];
+    }
     // this CTA's share goes straight into rank 0's collection buffer (its h_loc rows, dead since barrier #2)
-    st_dsmem(map_to(sm.h_loc + c * 80 + (i < 25 ? ch * 25 + i : 75 + ch), 0u), v);
+    st_dsmem(map_to(sm.h_loc + c * 80 + tid, 0u), v);
   }
   stamp(prof, 12, tid);
   cluster_sync();                                        // #3: all four conv-gradient shares are in rank 0's buffer

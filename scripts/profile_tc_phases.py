@@ -24,7 +24,7 @@ PHASES = ["sampler + image loads issued", "PDL wait", "TMA issue, small tensors,
           "cluster sync 3, conv-grad sum (rank 0), exit"]
 PHASES64 = ["sampler + image loads issued", "PDL wait", "W1 slice + small tensors (L2), pixels", "conv + ReLU + pool -> A tile (fp64)",
             "GEMM 1 (fc1 partial, DMMA)", "cluster sync 1", "reduce-scatter, fc2, loss, dz, dh, fc2 grads", "cluster sync 2",
-            "fc2-grad reduce (1/4), gather dH", "GEMM 3 (dW1, DMMA) -> global", "GEMM 2 (da1, DMMA) -> smem", "conv grads -> rank 0",
+            "fc2-grad reduce (1/4), gather dH", "GEMM 3 (dW1, DMMA) -> global", "GEMM 2 (da1, DMMA) -> smem", "conv grads (tap-row blocks) -> rank 0",
             "cluster sync 3, conv-grad sum (rank 0), exit"]
 
 
