@@ -26,6 +26,11 @@ namespace cl64 {
 constexpr int NT = 512, CL = 4, CELLS = 36, KC = 108, WS = 116, HS = 68;
 constexpr int PXR = 10 * HW;                  // image rows 6c .. 6c+9 of a sample: 280 pixels
 constexpr int KT = (KC + 7) / 8;              // 8-column tiles over a CTA's fc1 inputs; columns 108..111 fall in the row padding
+// rows of w2 and of the owners' h hold the 64 hidden units as four 16-unit runs 17 apart: the fc2 logits are summed by
+// 4 lanes per class over one run each, and with runs 17 apart (class rows 68 = 4 mod 16) the 32 lanes of a warp read
+// every 8-byte bank twice instead of all hitting one
+constexpr int HR = 68;
+NNDT_DEVINL int hr(int j) { return (j >> 4) * 17 + (j & 15); }
 constexpr int PART_WC = 0, PART_BC = 75, PART_B1 = 78, PART_W2 = 142, PART_B2 = 782, PART_LOSS = 792, PART_N = 793;
 
 template <int MS>
@@ -35,19 +40,18 @@ struct Smem {
   // sample stride of the pixel rows; as doubles 282 (141 16-byte units, odd), so the same patch row of eight consecutive
   // samples starts in eight different 16-byte bank groups
   static constexpr int PXS = kDoublePix ? PXR + 2 : PXR;
-  double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; later the conv-grad warp sums
-  double a[MS * WS];         // A tile [s][k]; later da1 [k][s]
+  double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; after GEMM 2 da1 [k][s], then the conv-grad warp sums
+  double a[MS * WS];         // A tile [s][k]
   double h[MS * HS];         // partial H [s][j] (read by the peers); after barrier #2 dH [s][j]
   alignas(16) unsigned char img[kDoublePix ? MS * PXS * 8 : MS * PXS];
   double lut[kDoublePix ? 1 : 256];                         // MS = 64: normalised value of each u8 pixel
-  double h_loc[NO * HID > CL * 80 ? NO * HID : CL * 80];   // later (rank 0) the CTAs' conv-gradient shares [CL][80]
+  double h_loc[NO * HR > CL * 80 ? NO * HR : CL * 80];     // [sl][hr(j)]; later (rank 0) the conv-gradient shares [CL][80]
   double dh_loc[NO * HID];
   double part[800];
-  double w2[NCLS * HID];
-  double b1[HID];
-  double b2[16];
+  double w2[NCLS * HR];                                     // [cc][hr(j)]
+  alignas(16) double b1[HID];                               // b1, b2 arrive by 16-byte cp.async with the W1 slice
+  alignas(16) double b2[16];
   double wc[80];
-  double z[NO * 16];
   double dz[NO * 16];
   double red[NO];
   int sidx[MS];
@@ -94,6 +98,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   constexpr int NO = SM::NO, PXS = SM::PXS;
   constexpr bool kDoublePix = SM::kDoublePix;
   static_assert(MS % 16 == 0 && NO <= NT / 32, "tile geometry");
+  static_assert(CELLS % 2 == 0 && NCLS % 2 == 0 && 32 + NCLS / 2 <= NT, "16-byte parameter copies");
   extern __shared__ __align__(16) unsigned char smem_raw[];
   SM& sm = *reinterpret_cast<SM*>(smem_raw);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -155,28 +160,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       }
     }
   }
-  stamp(prof, 1, tid);
-  pdl_wait();                 // the parameters of this step are final
-  pdl_launch_dependents();
-  stamp(prof, 2, tid);
-
-  // ---- W1 slice [64 j][108 k] (three 36-column runs per row): loads in flight while the pixels are converted -------------
-  constexpr int NW = (HID * KC + NT - 1) / NT;
-  double wreg[NW];
-#pragma unroll
-  for (int i = 0; i < NW; ++i) {
-    const int o = tid + i * NT;
-    wreg[i] = 0.0;
-    if (o < HID * KC) {
-      const int j = o / KC, r = o - j * KC, ch = r / CELLS, cell = r - ch * CELLS;
-      wreg[i] = __ldcg(th + a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell);
-    }
-  }
-  for (int o = tid; o < NCLS * HID; o += NT) sm.w2[o] = __ldcg(th + a.off_w2 + o);
-  if (tid < 75) sm.wc[tid] = __ldcg(th + a.off_wc + tid);
-  else if (tid < 78) sm.wc[tid] = __ldcg(th + a.off_bc + (tid - 75));
-  else if (tid >= 96 && tid < 96 + HID) sm.b1[tid - 96] = __ldcg(th + a.off_b1 + (tid - 96));
-  else if (tid >= 160 && tid < 160 + NCLS) sm.b2[tid - 160] = __ldcg(th + a.off_b2 + (tid - 160));
+  // the rows are data, not parameters: they are normalised into shared memory before the PDL wait
   if (u8) {
 #pragma unroll
     for (int i = 0; i < NU8; ++i) {
@@ -203,10 +187,35 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       }
     }
   }
+  stamp(prof, 1, tid);
+  pdl_wait();                 // the parameters of this step are final
+  pdl_launch_dependents();
+  stamp(prof, 2, tid);
+
+  // ---- W1 slice [64 j][108 k] (three 36-double runs per row, 16-byte chunks), b1, b2: asynchronous copies that land
+  //      while the conv runs.  The 78 conv weights and biases and w2 (re-laid out, so not a plain copy) are loaded
+  //      through registers, their L2 round trip under the copy issue; only these are waited for before the conv ------------
+  constexpr int NW2 = (NCLS * HID + NT - 1) / NT;
+  double wcv = 0.0, w2v[NW2];
+  if (tid < 75) wcv = __ldcg(th + a.off_wc + tid);
+  else if (tid < 78) wcv = __ldcg(th + a.off_bc + (tid - 75));
 #pragma unroll
-  for (int i = 0; i < NW; ++i) {
+  for (int i = 0; i < NW2; ++i) {
     const int o = tid + i * NT;
-    if (o < HID * KC) sm.w[(o / KC) * WS + (o % KC)] = wreg[i];
+    w2v[i] = o < NCLS * HID ? __ldcg(th + a.off_w2 + o) : 0.0;
+  }
+  for (int o = tid; o < HID * KC / 2; o += NT) {
+    const int j = o / (KC / 2), r = o - j * (KC / 2), ch = r / (CELLS / 2), q = 2 * (r - ch * (CELLS / 2));
+    cp_async16(sm.w + j * WS + ch * CELLS + q, th + a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + q);
+  }
+  if (tid < HID / 2) cp_async16(sm.b1 + 2 * tid, th + a.off_b1 + 2 * tid);
+  else if (tid >= 32 && tid < 32 + NCLS / 2) cp_async16(sm.b2 + 2 * (tid - 32), th + a.off_b2 + 2 * (tid - 32));
+  cp_async_commit();
+  if (tid < 78) sm.wc[tid] = wcv;
+#pragma unroll
+  for (int i = 0; i < NW2; ++i) {
+    const int o = tid + i * NT;
+    if (o < NCLS * HID) sm.w2[(o / HID) * HR + hr(o % HID)] = w2v[i];
   }
   __syncthreads();
   stamp(prof, 3, tid);
@@ -255,6 +264,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       sm.arg[s * KC + ch * CELLS + cell] = (unsigned char)(ai | (m > 0.0 ? 4 : 0));
     }
   }
+  cp_async_wait<0>();   // this thread's W1 / w2 / b1 / b2 chunks have landed; the barrier publishes everyone's
   __syncthreads();
   stamp(prof, 4, tid);
 
@@ -281,57 +291,68 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     else if (atomicAdd(a.arrive + l, 1u) == (unsigned)nsplit - 1) { a.arrive[l] = 0; a.calls[l] = call + 1; }
   }
 
-  // ---- reduce-scatter of H + fc2 / loss / their backward for this CTA's samples s0 .. s0 + NO - 1 -------------------------
+  // ---- reduce-scatter of H + fc2 / loss / their backward for this CTA's samples s0 .. s0 + NO - 1: one warp per sample,
+  //      lanes own hidden units j = lane and lane + 32; from the DSMEM sum to dh the warp needs no block barrier --------
   const int s0 = c * NO;
   const double inv_bs = 1.0 / (double)(bg.bs ? bg.bs : 1);
-  for (int o = tid; o < NO * HID; o += NT) {
-    const int sl = o >> 6, j = o & 63;
-    const double* src = sm.h + (s0 + sl) * HS + j;
-    double v = sm.b1[j];
-#pragma unroll
-    for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(src, (uint32_t)r));
-    sm.h_loc[o] = v > 0.0 ? v : 0.0;
-  }
-  __syncthreads();
-  for (int base = 0; base < NO * NCLS; base += NT / 4) {  // 4 lanes per logit; the trip count is the same for every warp
-    const int o = base + (tid >> 2), part = tid & 3;
-    const bool live = o < NO * NCLS;
-    const int sl = live ? o / NCLS : 0, cc = live ? o - sl * NCLS : 0;
-    double v = 0.0;
-    if (live) {
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj) { const int j = part * 16 + jj; v += sm.h_loc[sl * HID + j] * sm.w2[cc * HID + j]; }
-    }
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    if (live && part == 0) sm.z[sl * 16 + cc] = v + sm.b2[cc];
-  }
-  __syncthreads();
-  if (warp < NO) {                                       // log-softmax + NLL: one warp per sample, one lane per class
+  if (warp < NO) {
     const int sl = warp, s = s0 + sl;
+    double hv[2];
+#pragma unroll
+    for (int q = 0; q < 2; ++q) {
+      const int j = lane + 32 * q;
+      const double* src = sm.h + s * HS + j;
+      double v = sm.b1[j];
+#pragma unroll
+      for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(src, (uint32_t)r));
+      hv[q] = v > 0.0 ? v : 0.0;
+      sm.h_loc[sl * HR + hr(j)] = hv[q];
+    }
+    __syncwarp();
+    // logits: 4 lanes per class, each summing 16 consecutive hidden units, folded over lane bits 0 and 1; 40 partial sums,
+    // so lanes 0 .. 7 take a second one (classes 8 and 9)
+    double zp[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int o = lane + 32 * r, cc = o >> 2, part = o & 3;
+      double v = 0.0;
+      if (o < 4 * NCLS) {
+#pragma unroll
+        for (int jj = 0; jj < 16; ++jj) v += sm.h_loc[sl * HR + part * 17 + jj] * sm.w2[cc * HR + part * 17 + jj];
+      }
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      zp[r] = v;
+    }
+    static_assert(NCLS > 8 && NCLS <= 16, "two rounds of four lanes per class");
+    const double z0 = __shfl_sync(0xffffffffu, zp[0], (4 * lane) & 31), z1 = __shfl_sync(0xffffffffu, zp[1], (4 * lane) & 31);
+    // log-softmax + NLL, one lane per class
     const bool cls = lane < NCLS;
-    const double zc = cls ? sm.z[sl * 16 + lane] : -1.0e300;
+    const double zc = cls ? (lane < 8 ? z0 : z1) + sm.b2[lane] : -1.0e300;
     const double mx = wmax(zc);
     const double se = warp_sum(cls ? exp(zc - mx) : 0.0);
     const double lse = mx + log(se);
     const int y = sm.label[s];
     const double ok = (double)sm.valid[s];
-    if (cls) sm.dz[sl * 16 + lane] = ok * inv_bs * (exp(zc - lse) - (lane == y ? 1.0 : 0.0));
+    const double dzc = cls ? ok * inv_bs * (exp(zc - lse) - (lane == y ? 1.0 : 0.0)) : 0.0;
+    if (cls) sm.dz[sl * 16 + lane] = dzc;
     if (lane == y) sm.red[sl] = ok * (lse - zc);
-  }
-  __syncthreads();
-  for (int o = tid; o < NO * HID; o += NT) {
-    const int sl = o >> 6, j = o & 63;
-    double v = 0.0;
+    // dh = dz . W2, masked by ReLU'(h)
+    double dh[2] = {0.0, 0.0};
 #pragma unroll
-    for (int cc = 0; cc < NCLS; ++cc) v += sm.dz[sl * 16 + cc] * sm.w2[cc * HID + j];
-    sm.dh_loc[o] = sm.h_loc[o] > 0.0 ? v : 0.0;
+    for (int cc = 0; cc < NCLS; ++cc) {
+      const double d = __shfl_sync(0xffffffffu, dzc, cc);
+      dh[0] += d * sm.w2[cc * HR + hr(lane)];
+      dh[1] += d * sm.w2[cc * HR + hr(lane + 32)];
+    }
+#pragma unroll
+    for (int q = 0; q < 2; ++q) sm.dh_loc[sl * HID + lane + 32 * q] = hv[q] > 0.0 ? dh[q] : 0.0;
   }
   __syncthreads();
   for (int o = tid; o < NCLS * HID; o += NT) {
     const int cc = o >> 6, j = o & 63;
     double v = 0.0;
-    for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + cc] * sm.h_loc[sl * HID + j];
+    for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + cc] * sm.h_loc[sl * HR + hr(j)];
     sm.part[PART_W2 + o] = v;
   }
   if (tid < HID) {
@@ -376,43 +397,61 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   __syncthreads();
   stamp(prof, 9, tid);
 
-  // ---- GEMM 3 (DMMA): dW1_c[j][k] = sum_s dH[s][j] A[s][k], 4 x KT tiles straight to the gradient row; then GEMM 2 (DMMA):
-  //      da1_c[s][k] = sum_j dH[s][j] W[j][k], MS / 16 x KT tiles written over A ------------------------------------------------
-  {
-    constexpr int T3 = (HID / 16) * KT;
-#pragma unroll 1
-    for (int t = warp; t < T3; t += NT / 32) {
-      const int m0 = 16 * (t / KT), n0 = 8 * (t % KT);
-      double acc[1][4];
-      zero(acc);
-      gemm<1>(acc, m0, n0, MS, lane, at_t(sm.h, HS), at(sm.a, WS));
+  // ---- GEMM 2 (DMMA): da1_c[s][k] = sum_j dH[s][j] W[j][k], MS / 16 x KT / 2 pairs of adjacent 16 x 8 tiles, accumulators
+  //      held in registers until every warp is done reading W; then da1 [k][s] (sample-minor for the conv-grad pass, masked
+  //      by ReLU'(a1)) is written over the dead W slice.  A stays intact for GEMM 3 --------------------------------------------
+  constexpr int NP2 = (MS / 16) * (KT / 2), NR2 = (NP2 + NT / 32 - 1) / (NT / 32);
+  static_assert(KT % 2 == 0 && KC * MS + (NT / 32) * 16 <= HID * WS, "da1 and the conv-grad warp sums fit in the W slice");
+  double acc2[NR2][2][4];
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int j = frow(m0, lane, i), k = fcol(n0, lane, i);
-        if (k < KC) {
-          const int ch = k / CELLS, cell = k - ch * CELLS;
-          gp[a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell] = acc[0][i];
-        }
-      }
-    }
+  for (int r = 0; r < NR2; ++r) {
+    zero(acc2[r]);
+    const int p = warp + r * (NT / 32);
+    if (p < NP2) gemm<2>(acc2[r], 16 * (p / (KT / 2)), 16 * (p % (KT / 2)), HID, lane, at(sm.h, HS), at(sm.w, WS));
   }
-  __syncthreads();      // every read of A (GEMM 3) is done
+  __syncthreads();      // every read of W is done
   stamp(prof, 10, tid);
-  double* da1 = sm.a;   // A's rows become da1 [k][s] (sample-minor for the conv-grad pass), masked by ReLU'(a1)
-#pragma unroll 1
-  for (int t = warp; t < (MS / 16) * KT; t += NT / 32) {
-    const int m0 = 16 * (t / KT), n0 = 8 * (t % KT);
-    double acc[1][4];
-    zero(acc);
-    gemm<1>(acc, m0, n0, HID, lane, at(sm.h, HS), at(sm.w, WS));
+  double* da1 = sm.w;
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const int s = frow(m0, lane, i), k = fcol(n0, lane, i);
-      if (k < KC) da1[k * MS + s] = (sm.arg[s * KC + k] & 4) ? acc[0][i] : 0.0;
+  for (int r = 0; r < NR2; ++r) {
+    const int p = warp + r * (NT / 32);
+    if (p < NP2) {
+      const int m0 = 16 * (p / (KT / 2)), n0 = 16 * (p % (KT / 2));
+#pragma unroll
+      for (int jt = 0; jt < 2; ++jt)
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int s = frow(m0, lane, i), k = fcol(n0 + 8 * jt, lane, i);
+          if (k < KC) da1[k * MS + s] = (sm.arg[s * KC + k] & 4) ? acc2[r][jt][i] : 0.0;
+        }
     }
   }
   __syncthreads();
   stamp(prof, 11, tid);
+  // ---- GEMM 3 (DMMA): dW1_c[j][k] = sum_s dH[s][j] A[s][k], 4 x KT / 2 pairs of 16 x 8 tiles straight to the gradient row
+  //      (column pairs as 16-byte stores).  No barrier follows: a warp goes on to its conv-grad rows while others still run
+  //      their DMMA and stores --------------------------------------------------------------------------------------------
+  {
+    constexpr int NP3 = (HID / 16) * (KT / 2);
+#pragma unroll 1
+    for (int p = warp; p < NP3; p += NT / 32) {
+      const int m0 = 16 * (p / (KT / 2)), n0 = 16 * (p % (KT / 2));
+      double acc[2][4];
+      zero(acc);
+      gemm<2>(acc, m0, n0, MS, lane, at_t(sm.h, HS), at(sm.a, WS));
+#pragma unroll
+      for (int jt = 0; jt < 2; ++jt)
+#pragma unroll
+        for (int i = 0; i < 4; i += 2) {
+          const int j = frow(m0, lane, i), k = fcol(n0 + 8 * jt, lane, i);   // k even: k and k + 1 share a channel run
+          if (k < KC) {
+            const int ch = k / CELLS, cell = k - ch * CELLS;
+            *reinterpret_cast<double2*>(gp + a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell) =
+                make_double2(acc[jt][i], acc[jt][i + 1]);
+          }
+        }
+    }
+  }
   // ---- conv grads without gathers: warps 3ky .. 3ky+2 own tap row ky of all three channels.  A thread walks whole pooled
   //      rows (sample s, pooled row pr, px = 0 .. 11) with columns 2px .. 2px+5 of patch rows 2pr+ky and 2pr+ky+1 in
   //      registers, two new columns per cell.  Each cell's gradient goes to all four pool positions, zero except at its
@@ -420,7 +459,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   //      bias gradients.  Every warp folds its sums over its lanes and a tap row's three warp sums are added in warp order ---
   constexpr int KW = 3, NRUN = MS * 3;   // warps per tap row; (sample, pooled row) runs
   static_assert(KS * KW < NT / 32 && F * KS <= 16, "conv-grad work split");
-  double* wsums = sm.w;                  // [NT / 32][16] (W is dead)
+  double* wsums = sm.w + KC * MS;        // [NT / 32][16], behind da1
   // columns p, p + 1 (p even) of sample s's rows: one 16-byte load from the double rows
   auto pix2 = [&](int s, int p) -> double2 {
     if constexpr (kDoublePix) return *reinterpret_cast<const double2*>(imgd + s * PXS + p);
