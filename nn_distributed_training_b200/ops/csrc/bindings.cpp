@@ -10,7 +10,6 @@
 
 #include "consensus.h"
 #include "mnist.h"
-#include "dinno_round.h"
 
 namespace py = pybind11;
 using namespace nndt;
@@ -104,8 +103,6 @@ static consensus::Common<T> common_from(const py::dict& d) {
   c.flags = ptr<int>(d, "flags"); c.peer_flag = ptr<const int64_t>(d, "peer_flag");
   c.world = geti(d, "world", 1); c.rank = geti(d, "rank", 0);
   c.done_ctr = ptr<unsigned int>(d, "done_ctr"); c.err = ptr<int>(d, "err");
-  c.flags_in_kernel = geti(d, "flags_in_kernel", 1);
-  c.flag_pull = geti(d, "flag_pull", 0); c.peer_pub = ptr<const int64_t>(d, "peer_pub");
   c.notify_mask = d.contains("notify_mask") ? d["notify_mask"].cast<unsigned long long>() : ~0ull;
   c.node_order = ptr<const int>(d, "node_order");
   c.timeline = ptr<long long>(d, "timeline");
@@ -133,7 +130,6 @@ struct ConsensusOp {
     check(consensus::launch_dinno_update<T>(dn, cur_stream()), "dinno_update");
   }
   void local_sum() { check(consensus::launch_local_sum<T>(c, cur_stream()), "local_sum"); }
-  void publish() { check(consensus::launch_publish_round<T>(c, cur_stream()), "publish_round"); }
   void dsgd_mix() { check(consensus::launch_dsgd_mix<T>(c, cur_stream()), "dsgd_mix"); }
   void dsgd_step() { check(consensus::launch_dsgd_step<T>(c, cur_stream()), "dsgd_step"); }
   void dsgt_init() { check(consensus::launch_dsgt_init<T>(gt, cur_stream()), "dsgt_init"); }
@@ -147,32 +143,12 @@ static void bind_consensus(py::module& m, const char* name) {
       .def(py::init<const py::dict&>())
       .def("dinno_update", &ConsensusOp<T>::dinno_update)
       .def("local_sum", &ConsensusOp<T>::local_sum)
-      .def("publish", &ConsensusOp<T>::publish)
       .def("dsgd_mix", &ConsensusOp<T>::dsgd_mix)
       .def("dsgd_step", &ConsensusOp<T>::dsgd_step)
       .def("dsgt_init", &ConsensusOp<T>::dsgt_init)
       .def("dsgt_mix", &ConsensusOp<T>::dsgt_mix)
       .def("dsgt_track", &ConsensusOp<T>::dsgt_track);
 }
-
-// One launch per DiNNO round (dinno_round.cu): mnist dict + consensus dict + per-step batch sources
-struct DinnoRoundOp {
-  round::RoundArgs a{};
-  int S = 1;
-  DinnoRoundOp(const py::dict& md, const py::dict& cd, const py::list& steps) {
-    MnistOp mo(md);
-    ConsensusOp<float> co(cd);
-    a.m = mo.a; a.d = co.dn; S = mo.S;
-    a.prof = ptr<long long>(md, "prof");
-    if ((int)steps.size() != a.d.pits || a.d.pits > round::kMaxSteps) throw std::runtime_error("DinnoRoundOp: bad step list");
-    for (int p = 0; p < a.d.pits; ++p) {
-      const py::dict sd = steps[p].cast<py::dict>();
-      a.x_step[p] = ptr<const void>(sd, "x"); a.y_step[p] = ptr<const int64_t>(sd, "y");
-      a.bs_step[p] = ptr<const int>(sd, "direct_bs");
-    }
-  }
-  void launch() { check(round::launch_dinno_round(a, S, cur_stream()), "dinno_round"); }
-};
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp
 void bind_rl(py::module& m);      // rl_bind.cpp
@@ -214,10 +190,6 @@ PYBIND11_MODULE(_C, m) {
           "rank_barrier");
   });
   m.def("spin", [](long long cycles) { check(consensus::launch_spin(cycles, cur_stream()), "spin"); });
-  py::class_<DinnoRoundOp>(m, "DinnoRoundOp")
-      .def(py::init<const py::dict&, const py::dict&, const py::list&>())
-      .def("launch", &DinnoRoundOp::launch);
-  m.def("dinno_round_max_clusters", [](int S) { return round::max_active_clusters(S); });
   bind_consensus<float>(m, "ConsensusOpF32");
   bind_consensus<double>(m, "ConsensusOpF64");
   bind_mlp(m);

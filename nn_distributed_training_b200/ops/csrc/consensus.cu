@@ -63,16 +63,6 @@ __global__ void __launch_bounds__(THREADS) local_sum_kernel(const Common<T> c) {
 }
 
 
-// Announce "every round below *round_ctr is published" to the peers.  Runs after the round's last kernel (kernel
-// boundary = happens-before for all of its stores), so one thread's system fence + release stores are cumulative over
-// the whole round; launched on a forked graph branch, nothing local waits for it.  Reading the *current* counter is
-// always truthful: it only advances once the corresponding rows are written.
-template <typename T>
-__global__ void publish_round_kernel(const Common<T> c) {
-  const int k = *reinterpret_cast<volatile int*>(c.round_ctr);
-  announce_round(c, k);
-}
-
 // ------------------------------------------------------------------ DiNNO ----
 template <typename T, int U>
 __global__ void __launch_bounds__(THREADS) dinno_update_kernel(const DinnoArgs<T> a) {
@@ -461,10 +451,6 @@ template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStrea
   const int per_block = THREADS * Vec<T>::N;
   return launch_pdl(local_sum_kernel<T>, dim3((c.n_pad + per_block - 1) / per_block), dim3(THREADS), 0, st, c);
 }
-template <typename T> cudaError_t launch_publish_round(const Common<T>& c, cudaStream_t st) {
-  publish_round_kernel<T><<<1, 32, 0, st>>>(c);
-  return cudaGetLastError();
-}
 // kernels that sum gradient partials: the 4-deep variant when the producer writes <= 4 partial rows per node
 #define NNDT_BY_S(S, KERNEL, ARG, C)                                                              \
   ((S) <= 4 ? launch_pdl(KERNEL<T, 4>, grid_for(C, KERNEL<T, 4>), dim3(THREADS), 0, st, ARG)     \
@@ -491,7 +477,6 @@ template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaSt
 
 #define NNDT_INST(T)                                                                  \
   template cudaError_t launch_local_sum<T>(const Common<T>&, cudaStream_t);           \
-  template cudaError_t launch_publish_round<T>(const Common<T>&, cudaStream_t);       \
   template cudaError_t launch_consensus_metric<T>(const int64_t*, int, int, int, int, double*, double*, double*, cudaStream_t); \
   template cudaError_t launch_dinno_update<T>(const DinnoArgs<T>&, cudaStream_t);     \
   template cudaError_t launch_dsgd_mix<T>(const Common<T>&, cudaStream_t);            \

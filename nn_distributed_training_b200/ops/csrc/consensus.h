@@ -45,11 +45,6 @@ struct Common {
   int* flags;                 // [world] local slots written by peers (round published)
   const int64_t* peer_flag;   // [world] address of *their* slot for this rank
   int world, rank;
-  // flag transport: push (default) = the producer stores k+1 into the reader's local slot over NVLink and readers spin on
-  // local memory; pull = the producer only releases its own counter (slot `rank` of its own array, no remote store on its
-  // critical path) and readers poll that slot over NVLink through `peer_pub`.
-  int flag_pull;
-  const int64_t* peer_pub;    // [world] address of rank r's own counter (pull mode)
   unsigned long long notify_mask;  // ranks that ever own a neighbor of a local node: the only ones told about a new round
   const int* node_order;      // [L] launch order of the local nodes (nodes with remote neighbors first), nullptr = identity
   long long* timeline;        // debug (NNDT_TIMELINE=1): [4096][16] %globaltimer stamps of the update kernels, nullptr = off
@@ -59,8 +54,6 @@ struct Common {
   // neighbor read verifies it (nullptr = off)
   int* pub_seq;               // [2 parity, pub_L] local tags, written with the published rows
   const int64_t* nbr_seq;     // [G, L, dmax, 2] device addresses of the neighbors' tags per parity
-  int flags_in_kernel;        // who tells the peers that a round is published: 2 = the first consensus kernel of the round that
-                              // reads it (default), 1 = the last kernel of the round that wrote it, 0 = publish_round_kernel
   // complete-graph ("sum") mode: Metropolis weights are uniform 1/N, so every aggregate is a function of
   // S = sum over ALL nodes.  Each rank reduces its local rows into `sum_local` and the consumers fetch the
   // network-wide sum either with one NVLS in-switch reduction (multimem.ld_reduce over `sum_mc`) or, on a
@@ -93,7 +86,6 @@ template <typename T> cudaError_t launch_dsgt_init(const DsgtArgs<T>& a, cudaStr
 template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStream_t st);
-template <typename T> cudaError_t launch_publish_round(const Common<T>& c, cudaStream_t st);
 
 // All-rank barrier on the device (bench start alignment, metric quiescence): every rank stores `epoch` into its slot of
 // every peer's array and spins until all of its own slots reached it; with `gate` != nullptr the kernel first spins on that

@@ -1,4 +1,4 @@
-// Device-side helpers of the consensus kernels (shared by consensus.cu and dinno_round.cu).
+// Device-side helpers of the consensus kernels (consensus.cu).
 #pragma once
 #include "common.cuh"
 #include "consensus.h"
@@ -57,10 +57,10 @@ NNDT_DEVINL void tl_stamp(const Common<T>& c, int k, int step, int which) {
   c.timeline[(size_t)((k * 4 + step) & 4095) * 16 + (first ? 0 : 8) + which] = t;
 }
 
-// spin until rank r has published round k (push: peers store into our local slot; pull: poll r's own counter over NVLink)
+// spin until rank r has published round k (the peer stores into our local slot)
 template <typename T>
 NNDT_DEVINL void wait_rank(const Common<T>& c, int r, int k) {
-  const int* f = c.flag_pull ? reinterpret_cast<const int*>(c.peer_pub[r]) : c.flags + r;
+  const int* f = c.flags + r;
   if (ld_acquire_sys(f) >= k) return;
   if (*reinterpret_cast<volatile int*>(c.err) != 0) return;      // a peer already timed out: do not stack 10 s spins
   const long long t0 = clock64();
@@ -109,42 +109,31 @@ NNDT_DEVINL void tag_published(const Common<T>& c, int l, int k) {
 }
 
 // tell the peers that every round below `kn` is published (called by threads 0..world-1 of ONE block after the rows are
-// ordered before this point at gpu scope).  push: one remote store per rank that ever owns a neighbor; pull: a single
-// release of this rank's own counter — nothing crosses NVLink on the producer's critical path.
+// ordered before this point at gpu scope): one remote store per rank that ever owns a neighbor
 template <typename T>
 NNDT_DEVINL void announce_round(const Common<T>& c, int kn) {
-  if (c.flag_pull) {
-    if (threadIdx.x == 0) { __threadfence_system(); st_release_sys(c.flags + c.rank, kn); }
-  } else {
-    __threadfence_system();
-    if ((int)threadIdx.x < c.world && (int)threadIdx.x != c.rank && ((c.notify_mask >> threadIdx.x) & 1ull))
-      st_release_sys(reinterpret_cast<int*>(c.peer_flag[threadIdx.x]), kn);
-  }
+  __threadfence_system();
+  if ((int)threadIdx.x < c.world && (int)threadIdx.x != c.rank && ((c.notify_mask >> threadIdx.x) & 1ull))
+    st_release_sys(reinterpret_cast<int*>(c.peer_flag[threadIdx.x]), kn);
 }
 
-// First consensus kernel of round k (the one that reads neighbor rows).  flags_in_kernel == 2: block (0, 0) announces
-// "round k published" HERE instead of the last block of round k - 1's final kernel: that kernel wrote the rows, it is
-// complete and flushed by the time any block of this one runs (every kernel passes griddepcontrol.wait before it lets its
-// dependents launch), and the system fence + NVLink flag stores (3-4 us when they sit at the end of a kernel the next
-// forward/backward waits for) now overlap the forward/backward kernel this launch runs under.
+// First consensus kernel of round k (the one that reads neighbor rows).  Block (0, 0) announces "round k published"
+// here rather than at the end of round k - 1's final kernel: that kernel wrote the rows, it is complete and flushed by
+// the time any block of this one runs (every kernel passes griddepcontrol.wait before it lets its dependents launch),
+// and the system fence + NVLink flag stores (3-4 us when they sit at the end of a kernel the next forward/backward
+// waits for) overlap the forward/backward kernel this launch runs under.
 template <typename T>
 NNDT_DEVINL void begin_round(const Common<T>& c, int gid, int l, int k) {
-  if (c.world > 1 && c.flags_in_kernel == 2 && blockIdx.x == 0 && blockIdx.y == 0) announce_round(c, k);
+  if (c.world > 1 && blockIdx.x == 0 && blockIdx.y == 0) announce_round(c, k);
   if (c.sum_mode) wait_all_sums(c, k); else wait_neighbors(c, gid, l, k);
 }
 
-// last block of the launch: advance the round counter and announce the new round to peers
+// last block of the launch: advance the round counter (the next round's first kernel announces it to the peers)
 template <typename T>
 NNDT_DEVINL void finish_round(const Common<T>& c, int k) {
-  // flags_in_kernel == 0: a separate publish_round_kernel on a forked graph branch announces the round to the
-  // peers (system fence + remote flag stores off the local critical path); this kernel only advances the counter.
-  const bool announce = c.world > 1 && c.flags_in_kernel == 1;
   __shared__ bool is_last;
   __syncthreads();
   if (threadIdx.x == 0) {
-    // release this block's published rows before arriving (the CTA barrier makes the fence cumulative over every
-    // thread's stores).  Otherwise the kernel boundary is the only consumer-side ordering needed.
-    if (announce) __threadfence();
     const unsigned total = gridDim.x * gridDim.y;
     is_last = (atomicAdd(c.done_ctr, 1u) == total - 1);
   }
@@ -154,7 +143,6 @@ NNDT_DEVINL void finish_round(const Common<T>& c, int k) {
       *c.done_ctr = 0;
       *c.round_ctr = k + 1;
     }
-    if (announce) announce_round(c, k + 1);
   }
 }
 

@@ -38,7 +38,7 @@ __global__ void __launch_bounds__(NT, 1) mnist_kernel(const Args a) {
     if (!early) {
       pdl_wait();
       pdl_launch_dependents();
-      stage_params<SPB, NT>(sm, a, th, tid, true);    // TMA + small loads fly while the sampler chain runs
+      stage_params<SPB, NT>(sm, a, th, tid);    // TMA + small loads fly while the sampler chain runs
     }
     const int call = a.calls != nullptr ? a.calls[l] : 0;
     const BatchGeom bg = batch_geom<true>(a, l, call);
@@ -54,20 +54,20 @@ __global__ void __launch_bounds__(NT, 1) mnist_kernel(const Args a) {
       pdl_wait();               // parameters of this step are now final
       pdl_launch_dependents();
       phase_stamp(prof, 22, tid);
-      stage_params<SPB, NT>(sm, a, th, tid, true);
+      stage_params<SPB, NT>(sm, a, th, tid);
     }
     commit_images<SPB, NT>(sm, a, tid, img);
     if (tid < SPB) sm.label[tid] = lab;
-    compute_chunk<SPB, NT, true>(sm, a, l, blockIdx.x, gridDim.x, bg, 0, tid, prof);
+    compute_chunk<SPB, NT, true>(sm, a, l, blockIdx.x, gridDim.x, bg, tid, prof);
     phase_stamp(prof, 23, tid);
   } else {
     pdl_wait();
     pdl_launch_dependents();
-    stage_params<SPB, NT>(sm, a, th, tid, true);
+    stage_params<SPB, NT>(sm, a, th, tid);
     const BatchGeom bg = batch_geom<false>(a, l, 0);
     const int n_chunks = (a.n_val + SPB - 1) / SPB;
     for (int chunk = blockIdx.x; chunk < n_chunks; chunk += gridDim.x)
-      process_chunk<SPB, NT, false>(sm, a, l, blockIdx.x, gridDim.x, chunk, bg, 0, tid);
+      process_chunk<SPB, NT, false>(sm, a, l, blockIdx.x, gridDim.x, chunk, bg, tid);
   }
 }
 

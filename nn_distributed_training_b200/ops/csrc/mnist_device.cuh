@@ -1,5 +1,4 @@
-// Device-side building blocks of the MNIST conv-net forward/backward (shared by mnist.cu's per-step kernel
-// and dinno_round.cu's one-launch-per-round cluster kernel).
+// Device-side building blocks of the MNIST conv-net forward/backward (the batch-split kernel of mnist.cu).
 #pragma once
 #include "common.cuh"
 #include "sampler.cuh"
@@ -170,14 +169,14 @@ __device__ __forceinline__ void fc1_forward(Smem<SPB, NT>& sm, int tid) {
 // stage fc1 weights with the TMA engine (one bulk copy per 1728-byte row into the padded smem rows,
 // completion tracked by an mbarrier transaction count) and the small tensors with L2 loads
 template <int SPB, int NT>
-__device__ __forceinline__ void stage_params(Smem<SPB, NT>& sm, const Args& a, const float* th, int tid, bool init_bar) {
+__device__ __forceinline__ void stage_params(Smem<SPB, NT>& sm, const Args& a, const float* th, int tid) {
   // warp 1 drives the TMA engine (each lane queues two row copies) and warps 2+ fetch the small tensors, so
   // warp 0 is free to run the sampler chain (draw counter -> permutation -> label) that gates the image loads
   const float* w1g = th + a.off_w1;
   if ((tid >> 5) == 1) {
     const int lane = tid & 31;
     if (lane == 0) {
-      if (init_bar) mbarrier_init(&sm.w1_bar, 1);
+      mbarrier_init(&sm.w1_bar, 1);
       mbarrier_expect_tx(&sm.w1_bar, HID * FC1_IN * 4);
     }
     __syncwarp();
@@ -213,7 +212,7 @@ __device__ __forceinline__ BatchGeom batch_geom(const Args& a, int l, int call) 
   return g;
 }
 
-// optional %globaltimer stamps of the phase boundaries (profiling builds of the round kernel only)
+// optional %globaltimer stamps of the phase boundaries (a.prof, scripts/profile_round_phases.py)
 __device__ __forceinline__ void phase_stamp(long long* prof, int idx, int tid) {
   if (prof != nullptr && tid == 0) {
     long long t;
@@ -250,9 +249,8 @@ __device__ __forceinline__ int select_samples(Smem<SPB, NT>& sm, const Args& a, 
 }
 template <int SPB, int NT, bool TRAIN>
 __device__ __forceinline__ void load_chunk(Smem<SPB, NT>& sm, const Args& a, int l, int slice, int chunk,
-                                           const BatchGeom& bg, int tid, long long* prof = nullptr) {
+                                           const BatchGeom& bg, int tid) {
   const int lab = select_samples<SPB, NT, TRAIN>(sm, a, l, slice, chunk, bg, tid);
-  phase_stamp(prof, 0, tid);
   ImgRegs<SPB, NT> r;
   issue_image_loads<SPB, NT>(sm, a, tid, r);
   commit_images<SPB, NT>(sm, a, tid, r);
@@ -263,8 +261,7 @@ __device__ __forceinline__ void load_chunk(Smem<SPB, NT>& sm, const Args& a, int
 // Training writes the slice's partial gradient row and loss.
 template <int SPB, int NT, bool TRAIN>
 __device__ __forceinline__ void compute_chunk(Smem<SPB, NT>& sm, const Args& a, int l, int slice, int S,
-                                              const BatchGeom& bg, uint32_t w1_parity, int tid,
-                                              long long* prof = nullptr) {
+                                              const BatchGeom& bg, int tid, long long* prof = nullptr) {
   const float inv_bs = bg.inv_bs;
     if (SPB < 8) {   // sample padding of the MMA operands (never written afterwards)
       for (int o = tid; o < (8 - SPB) * A1_STRIDE; o += NT) sm.a1[SPB * A1_STRIDE + o] = 0.f;
@@ -273,7 +270,7 @@ __device__ __forceinline__ void compute_chunk(Smem<SPB, NT>& sm, const Args& a, 
     __syncthreads();   // images + staged small tensors visible
     phase_stamp(prof, 1, tid);
     conv_relu_pool<SPB, NT>(sm, tid);
-    mbarrier_wait_parity(&sm.w1_bar, w1_parity);   // fc1 weights have landed (no-op after the first chunk)
+    mbarrier_wait_parity(&sm.w1_bar, 0);   // fc1 weights have landed (no-op after the first chunk)
     __syncthreads();
     phase_stamp(prof, 2, tid);
 
@@ -484,10 +481,9 @@ namespace nndt {
 namespace mnist {
 template <int SPB, int NT, bool TRAIN>
 __device__ __forceinline__ void process_chunk(Smem<SPB, NT>& sm, const Args& a, int l, int slice, int S, int chunk,
-                                              const BatchGeom& bg, uint32_t w1_parity, int tid,
-                                              long long* prof = nullptr) {
-  load_chunk<SPB, NT, TRAIN>(sm, a, l, slice, chunk, bg, tid, prof);
-  compute_chunk<SPB, NT, TRAIN>(sm, a, l, slice, S, bg, w1_parity, tid, prof);
+                                              const BatchGeom& bg, int tid) {
+  load_chunk<SPB, NT, TRAIN>(sm, a, l, slice, chunk, bg, tid);
+  compute_chunk<SPB, NT, TRAIN>(sm, a, l, slice, S, bg, tid);
 }
 }  // namespace mnist
 }  // namespace nndt

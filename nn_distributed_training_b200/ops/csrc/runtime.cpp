@@ -199,58 +199,7 @@ class HostFedRunner {
   int64_t round_ = 0;
 };
 
-// Two-stream round driver for device-initiated staging: copy graph (GPU pulls the next round's rows from pinned
-// host memory) on a side stream, round graph (kernels + D2H loss read) on the compute stream, double buffered.
-class PullRunner {
- public:
-  PullRunner(std::vector<uint64_t> copy_execs, std::vector<uint64_t> round_execs, uint64_t compute_stream)
-      : copy_execs_(std::move(copy_execs)), round_execs_(std::move(round_execs)),
-        compute_(reinterpret_cast<cudaStream_t>(compute_stream)) {
-    cuda_check(cudaStreamCreateWithFlags(&copy_, cudaStreamNonBlocking), "cudaStreamCreate");
-    for (int b = 0; b < 2; ++b) {
-      cuda_check(cudaEventCreateWithFlags(&copied_[b], cudaEventDisableTiming), "cudaEventCreate");
-      cuda_check(cudaEventCreateWithFlags(&consumed_[b], cudaEventDisableTiming), "cudaEventCreate");
-    }
-  }
-  ~PullRunner() {
-    cudaStreamSynchronize(copy_);
-    for (int b = 0; b < 2; ++b) { cudaEventDestroy(copied_[b]); cudaEventDestroy(consumed_[b]); }
-    cudaStreamDestroy(copy_);
-  }
-  // stage round `round_` (and keep one round of look-ahead), then run it
-  void run(int rounds) {
-    py::gil_scoped_release rel;
-    for (int i = 0; i < rounds; ++i, ++round_) {
-      if (staged_ == round_) stage();          // first call: nothing staged yet
-      stage();                                 // look-ahead: round_ + 1 copies while round_ computes
-      const int b = (int)(round_ & 1);
-      cuda_check(cudaStreamWaitEvent(compute_, copied_[b], 0), "wait copied");
-      cuda_check(cudaGraphLaunch(reinterpret_cast<cudaGraphExec_t>(round_execs_[b]), compute_), "round graph");
-      cuda_check(cudaEventRecord(consumed_[b], compute_), "record consumed");
-    }
-  }
-  int64_t rounds_done() const { return round_; }
-
- private:
-  void stage() {
-    if (staged_ > round_ + 1) return;
-    const int b = (int)(staged_ & 1);
-    if (staged_ >= 2) cuda_check(cudaStreamWaitEvent(copy_, consumed_[b], 0), "wait consumed");
-    cuda_check(cudaGraphLaunch(reinterpret_cast<cudaGraphExec_t>(copy_execs_[b]), copy_), "copy graph");
-    cuda_check(cudaEventRecord(copied_[b], copy_), "record copied");
-    ++staged_;
-  }
-  std::vector<uint64_t> copy_execs_, round_execs_;
-  cudaStream_t compute_, copy_ = nullptr;
-  cudaEvent_t copied_[2], consumed_[2];
-  int64_t round_ = 0, staged_ = 0;
-};
-
 void bind_runtime(py::module& m) {
-  py::class_<PullRunner>(m, "PullRunner")
-      .def(py::init<std::vector<uint64_t>, std::vector<uint64_t>, uint64_t>())
-      .def("run", &PullRunner::run)
-      .def("rounds_done", &PullRunner::rounds_done);
   py::class_<HostBatchLoader>(m, "HostBatchLoader")
       .def(py::init<uint64_t, uint64_t, int, std::vector<int>, std::vector<int>, std::vector<int64_t>, int, int, int,
                     int, std::vector<uint64_t>, std::vector<uint64_t>, std::vector<uint64_t>, int>())

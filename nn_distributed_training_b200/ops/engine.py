@@ -20,7 +20,7 @@ OPT_CODE = {"sgd": 0, "adam": 1, "adamw": 2}
 
 
 class ConsensusEngine:
-    def __init__(self, opt, graphs_per_round: List, forked_graphs: bool = False):
+    def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
         pr = self.pr = opt.pr
         self.ext = load_ext(required=True)
@@ -121,14 +121,8 @@ class ConsensusEngine:
         for r in range(ctx.world_size):
             peer_flag[r] = self.flag_buf.peer_ptrs[r] + 4 * ctx.rank
         self.t_peer_flag = torch.as_tensor(peer_flag, device=dev)
-        # pull transport: rank r's own counter is slot r of its own array; readers poll it over NVLink
-        peer_pub = np.zeros(max(ctx.world_size, 1), dtype=np.int64)
-        for r in range(ctx.world_size):
-            peer_pub[r] = self.flag_buf.peer_ptrs[r] + 4 * r
-        self.t_peer_pub = torch.as_tensor(peer_pub, device=dev)
-        self.flag_mode = os.environ.get("NNDT_FLAG_MODE", str(opt.conf.get("flag_transport", pr.conf.get("flag_transport", "push"))))
-        if self.flag_mode not in ("push", "pull"):
-            raise ValueError(f"flag_transport must be push or pull, got {self.flag_mode!r}")
+        # a producer stores "round k published" into each reader's local flag slot; readers spin on local memory
+        self.flag_mode = "push"
         # ranks that own a neighbor of a local node in ANY round's graph: the only ones that need this rank's flags
         notify = 0
         remote_node = np.zeros(L, dtype=bool)
@@ -184,7 +178,6 @@ class ConsensusEngine:
                  graph_id=self.t_gid.data_ptr(), calls=None if calls is None else calls.data_ptr(),
                  flags=self.flag_buf.local.data_ptr(), peer_flag=self.t_peer_flag.data_ptr(),
                  world=ctx.world_size, rank=ctx.rank, done_ctr=self.done_ctr.data_ptr(), err=self.err.data_ptr(),
-                 flag_pull=int(self.flag_mode == "pull"), peer_pub=self.t_peer_pub.data_ptr(),
                  notify_mask=int(self.notify_mask) if ctx.world_size > 1 else 0,
                  node_order=self.t_node_order.data_ptr() if ctx.world_size > 1 else None)
         self.timeline = None
@@ -195,27 +188,6 @@ class ConsensusEngine:
         # published buffer is allocated with the max count, so pass that as the row count of pub
         d["L"] = L
         d["pub_L"] = self.Lpub
-        # multi-GPU: the "round published" flags can be written by publish_round_kernel on a forked graph branch
-        # (round_program.py) instead of the round's last kernel.
-        # Off by default.  The one-CTA publish kernel becomes ready together with the next round's forward/backward
-        # kernel, whose PDL-launched update kernel fills every remaining register file with CTAs that spin on the
-        # peers' flags: with the fp64 cluster kernel nothing is left for the publish CTA until the forward/backward
-        # CTAs exit, i.e. every rank announces its round ~34 us late (scripts/timeline_rounds.py, 2 GPUs: flag wait
-        # 33.9 us vs 2.5 us with the announcement inside the round's last kernel).  (In round 1 the fork gained
-        # 1.9 us / round on the host-fed fp32 graphs and cost 2.9 us on the resident ones.)
-        sp = opt.conf.get("separate_publish", pr.conf.get("separate_publish", False))
-        if os.environ.get("NNDT_SEPARATE_PUBLISH") in ("0", "1"):       # A/B switch
-            sp = os.environ["NNDT_SEPARATE_PUBLISH"] == "1"
-        if sp == "auto":
-            sp = forked_graphs
-        self.separate_publish = bool(ctx.world_size > 1 and sp)
-        # in-kernel announcement: "start" = by the first consensus kernel of the round that READS the rows (its block 0,
-        # under the forward/backward kernel), "end" = by the last kernel of the round that wrote them (3-4 us of system
-        # fence + NVLink stores on the critical path of every round)
-        self.announce = os.environ.get("NNDT_ANNOUNCE", str(opt.conf.get("announce", pr.conf.get("announce", "start"))))
-        if self.announce not in ("start", "end"):
-            raise ValueError(f"announce must be 'start' or 'end', got {self.announce!r}")
-        d["flags_in_kernel"] = 0 if self.separate_publish else (2 if self.announce == "start" else 1)
         if pr.fused is not None and getattr(pr, "track_tloss", False) and self.dtype == torch.float32:
             # the kernel that consumes a gradient also folds that step's loss into the EMA tracker
             d.update(loss_part=pr.fused.loss_part.data_ptr(), tloss=pr.tloss_local.data_ptr(),

@@ -107,7 +107,7 @@ class FusedMnist:
             linear_width=spec.linear_width, dtype64=int(self.dtype == torch.float64), cl64=int(self.cl64))
         if self.tc:
             self.base.update(tc=1, w1_map=self.ext.make_w1_tensor_map(a.theta.data_ptr(), a.n_pad, self.L, off[names[2]]))
-        if os.environ.get("NNDT_STEP_PROF") == "1":     # scripts/profile_round_phases.py --per-step
+        if os.environ.get("NNDT_STEP_PROF") == "1":     # scripts/profile_round_phases.py
             self.step_prof = torch.zeros(self.L * self.S * self.ctas_per_split, 64, dtype=torch.int64, device=dev)
             self.base["step_prof"] = self.step_prof.data_ptr()
         self.train_op = self.ext.MnistOp(self.base)
@@ -119,32 +119,6 @@ class FusedMnist:
         """Enqueue fwd+bwd of the next batch of every local node (graph-capturable).
         The draw counter is advanced by the consensus kernel that consumes the partials."""
         self.train_op.train()
-
-    # ---- one launch per DiNNO round (csrc/dinno_round.cu) -----------------------
-    MAX_ROUND_STEPS = 8
-
-    def supports_round_kernel(self, opt) -> bool:
-        """The cluster kernel needs the node's S batch slices in one cluster (S <= 8 CTAs) and fp32 state."""
-        return (not self.generic and not self.tc and opt.alg_name == "dinno" and self.spb == SPB and self.S <= 8 and 1 <= opt.pits <= self.MAX_ROUND_STEPS
-                and self.pr.arena.dtype == torch.float32 and self.ext.dinno_round_max_clusters(self.S) >= 1)
-
-    def round_op(self, cons_dict, stage_set=None):
-        """``DinnoRoundOp`` running all primal iterations of a round; ``stage_set`` selects the host-fed
-        staging buffers (one batch source per step) instead of the resident shards."""
-        P = int(cons_dict["pits"])
-        md = dict(self.base)
-        if getattr(self, "round_prof", None) is not None:
-            md["prof"] = self.round_prof.data_ptr()     # scripts/profile_round_phases.py
-        if stage_set is None:
-            steps = [dict(x=self.x.data_ptr(), y=self.y.data_ptr(), direct_bs=None) for _ in range(P)]
-        else:
-            md.update(direct=1)
-            if getattr(self, "loss_mode", "memcpy") == "mirror":
-                md.update(loss_mirror=self.loss_host.data_ptr())
-            b = stage_set
-            steps = [dict(x=self.x_stage[b, p].data_ptr(), y=self.y_stage[b, p].data_ptr(),
-                          direct_bs=self.bs_stage[b, p].data_ptr()) for p in range(P)]
-        return self.ext.DinnoRoundOp(md, cons_dict, steps)
 
     def compute_grads(self) -> torch.Tensor:
         """Eager API: fills ``arena.grad`` and advances the counters itself."""
@@ -264,21 +238,6 @@ class FusedMnist:
                               h2d_bytes=P * L * B * (784 * xb + 8) if source == "host" else 0,
                               d2h_bytes=L * self.S * 4 if source == "host" else 0)
         return self.host_feed
-
-    def make_pull_runner(self, round_graphs):
-        """Capture the two staging graphs and build the native two-stream driver."""
-        copy_graphs = []
-        side = torch.cuda.Stream(device=self.pr.device)
-        for b in range(2):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, stream=side):
-                self.gather_ops[b].launch()
-            copy_graphs.append(g)
-        self._graphs = (copy_graphs, round_graphs)
-        stream = torch.cuda.current_stream(self.pr.device).cuda_stream
-        self.runner = self.ext.PullRunner([g.raw_cuda_graph_exec() for g in copy_graphs],
-                                          [g.raw_cuda_graph_exec() for g in round_graphs], stream)
-        return self.runner
 
     def make_runner(self, graphs, nslots):
         """Native per-round driver (csrc/runtime.cpp: HostFedRunner) over the two captured round graphs."""

@@ -2,8 +2,6 @@
 
 A round is a short, fixed kernel sequence
     DiNNO:  [fwd/bwd, dinno_update(p)] x primal_iterations
-            (MNIST: ONE cluster kernel per round, csrc/dinno_round.cu — fwd/bwd and the update of
-             every primal iteration separated by cluster barriers instead of kernel boundaries)
     DSGD :  dsgd_mix, fwd/bwd, dsgd_step
     DSGT :  dsgt_mix, fwd/bwd, dsgt_track
 whose per-round scalars come from device schedules indexed by a device round
@@ -32,20 +30,16 @@ def _nvtx(name):
     return torch.cuda.nvtx.range(name)
 
 
-def _round_ops(opt, eng, grads, round_op=None, publish=None):
+def _round_ops(opt, eng, grads):
     with _nvtx(f"consensus_round/{opt.alg_name}"):
-        _round_ops_impl(opt, eng, grads, round_op)
-        if eng.separate_publish:
-            (publish or eng.op.publish)()      # announce the round to the peers (forked branch under capture)
+        _round_ops_impl(opt, eng, grads)
 
 
-def _round_ops_impl(opt, eng, grads, round_op=None):
+def _round_ops_impl(opt, eng, grads):
     alg = opt.alg_name
     if eng.sum_mode:
         eng.op.local_sum()   # complete graph: per-rank partial sums feeding the NVLS reduction
-    if round_op is not None:
-        round_op.launch()    # whole DiNNO round (all primal iterations) in one cluster launch
-    elif alg == "dinno":
+    if alg == "dinno":
         for p in range(opt.pits):
             grads(p)
             eng.op.dinno_update(p)
@@ -76,8 +70,7 @@ class RoundProgram:
         graphs = pr.plan_graphs(opt.oits, opt.k, self.dpr, init_draws,
                                 refresh=getattr(opt, "refresh_graph", True))
         self.capturable = pr.fused is not None and os.environ.get("NNDT_NO_GRAPH", "0") != "1"
-        # ---- input pipeline of the fused MNIST problem (decided first: the engine's peer-announcement mode depends on
-        #      whether the rounds run in forked multi-round graphs) -----------------------------------------------------
+        # ---- input pipeline of the fused MNIST problem ------------------------------------------------------------
         pipeline = "resident"
         if pr.fused is not None:
             pipeline = pr.conf.get("input_pipeline", "auto")
@@ -88,18 +81,13 @@ class RoundProgram:
                 pipeline = "staged" if can_stage else "resident"
             if not hasattr(pr.fused, "enable_host_feed"):
                 pipeline = "resident"
-        forked = (pipeline == "staged" or (pipeline == "host" and pr.conf.get("host_gather", "gpu_pull") == "gpu_pull")) \
-            and os.environ.get("NNDT_PULL_DRIVER", pr.conf.get("host_pull_driver", "graph")) == "graph"
-        self.eng = ConsensusEngine(opt, graphs, forked_graphs=forked)
+        self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows
         pr._metric_engine = (self.eng, lambda: opt.k)
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
-        self._round_ops = None
         self.pipeline = "resident"
-        self._pub_side = None
-        self._pub_pending = False
         if pr.fused is not None:
             pr.fused.sync_calls_from_host()
             self._deferred_pipeline = None
@@ -110,13 +98,6 @@ class RoundProgram:
                     self._deferred_pipeline = pipeline
                 else:
                     self._enable_pipeline(pipeline)
-            # opt-in: slower than the PDL-overlapped per-step kernels when it was measured, kept as the
-            # in-kernel phase profiler (scripts/profile_round_phases.py) and for launch-bound environments
-            want = pr.conf.get("fused_round", opt.conf.get("fused_round", False)) or os.environ.get("NNDT_FUSED_ROUND") == "1"
-            if (want and os.environ.get("NNDT_NO_FUSED_ROUND", "0") != "1"
-                    and getattr(pr.fused, "supports_round_kernel", lambda o: False)(opt)):
-                sets = [0, 1] if self.host_mode else [None]
-                self._round_ops = {b: pr.fused.round_op(self.eng._keep, b) for b in sets}
 
     def _enable_pipeline(self, pipeline: str):
         pr = self.pr
@@ -132,38 +113,12 @@ class RoundProgram:
         self._pull_primed = False
         self._side = None
 
-    # ---- peer announcement off the critical path ---------------------------------------------------------------
-    def _publish_forked(self):
-        """Under capture: run publish_round_kernel on a side stream that forks after the round's last kernel, so the
-        system fence + remote flag stores overlap the next round's forward/backward; joined at the end of the graph."""
-        if self._pub_side is None:
-            self._pub_side = torch.cuda.Stream(device=self.pr.device)
-        main = torch.cuda.current_stream(self.pr.device)
-        self._pub_side.wait_stream(main)
-        with torch.cuda.stream(self._pub_side):
-            self.eng.op.publish()
-        self._pub_pending = True
-
-    def _join_publish(self):
-        if self._pub_pending:
-            torch.cuda.current_stream(self.pr.device).wait_stream(self._pub_side)
-            self._pub_pending = False
-
-    def round_op(self):
-        if self._round_ops is None:
-            return None
-        return self._round_ops[self._stage_set if self.host_mode else None]
-
     def launches_per_round(self) -> int:
-        """Kernel launches of one communication round (the staging kernel of the host-fed / staged pipelines and the
-        forked peer announcement included)."""
+        """Kernel launches of one communication round (the staging kernel of the host-fed / staged pipelines
+        included)."""
         n = 1 if self.eng.sum_mode else 0
         if self.host_mode and self.pr.fused.host_feed["mode"] == "gpu_pull":
             n += 1
-        if self.eng.separate_publish:
-            n += 1
-        if self._round_ops is not None:
-            return n + 1
         return n + (2 * self.opt.pits if self.opt.alg_name == "dinno" else 3)
 
     def grads(self, p: int = 0):
@@ -208,10 +163,9 @@ class RoundProgram:
                 with torch.cuda.stream(side):
                     fz.gather_ops[b ^ 1].launch()
                 self._stage_set = b
-                _round_ops(self.opt, self.eng, self.grads, self.round_op(), self._publish_forked)
+                _round_ops(self.opt, self.eng, self.grads)
                 fz.loss_readback()
                 main.wait_stream(side)     # round i+1 consumes what was just staged (also joins the fork)
-            self._join_publish()
         return g
 
     def _pull_graph(self, r: int, parity: int):
@@ -239,12 +193,11 @@ class RoundProgram:
 
     def _run_host_fed(self, rounds: int):
         """Host-fed rounds.  ``gpu_pull`` (default): multi-round graphs with the staging kernel forked inside
-        (``_capture_pull_graph``); ``host_pull_driver: runner`` keeps the native two-stream driver
-        (csrc/runtime.cpp: PullRunner) that launches one staging graph + one round graph per round.
-        ``cpu_loader``: the native runner issues, per round, the H2D copy of that round's inputs, the captured
-        round graph (kernels + D2H loss read) and the slot hand-back to the loader threads."""
+        (``_capture_pull_graph``).  ``cpu_loader``: the native runner issues, per round, the H2D copy of that
+        round's inputs, the captured round graph (kernels + D2H loss read) and the slot hand-back to the loader
+        threads."""
         fz = self.pr.fused
-        if fz.host_feed["mode"] == "gpu_pull" and os.environ.get("NNDT_PULL_DRIVER", self.pr.conf.get("host_pull_driver", "graph")) == "graph":
+        if fz.host_feed["mode"] == "gpu_pull":
             return self._run_pull_graphs(rounds)
         if self._runner is None:
             graphs = []
@@ -252,13 +205,10 @@ class RoundProgram:
                 self._stage_set = b
                 g = torch.cuda.CUDAGraph()
                 with torch.cuda.graph(g):
-                    _round_ops(self.opt, self.eng, self.grads, self.round_op())
+                    _round_ops(self.opt, self.eng, self.grads)
                     fz.loss_readback()
                 graphs.append(g)
-            if fz.host_feed["mode"] == "gpu_pull":
-                self._runner = fz.make_pull_runner(graphs)
-            else:
-                self._runner = fz.make_runner(graphs, fz.host_feed["nslots"])
+            self._runner = fz.make_runner(graphs, fz.host_feed["nslots"])
         # graphs were captured on torch's capture stream but are launched on the current stream
         self._runner.run(rounds)
         self._count(rounds)
@@ -269,8 +219,7 @@ class RoundProgram:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads, self.round_op(), self._publish_forked)
-                self._join_publish()
+                    _round_ops(self.opt, self.eng, self.grads)
             self._graphs[r] = g
         return g
 
@@ -280,8 +229,7 @@ class RoundProgram:
         if not self.capturable:
             return
         if self.host_mode:
-            fz = self.pr.fused
-            if fz.host_feed["mode"] == "gpu_pull" and os.environ.get("NNDT_PULL_DRIVER", self.pr.conf.get("host_pull_driver", "graph")) == "graph":
+            if self.pr.fused.host_feed["mode"] == "gpu_pull":
                 self._run_pull_graphs(rounds, capture_only=True)
             return
         left = rounds
@@ -301,7 +249,7 @@ class RoundProgram:
                 self._resident_graph(r).replay()
             else:
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads, self.round_op())
+                    _round_ops(self.opt, self.eng, self.grads)
             self._count(r)
             left -= r
 

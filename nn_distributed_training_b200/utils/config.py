@@ -80,7 +80,6 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
 PROBLEM_CHOICES = {
     "input_pipeline": ("auto", "resident", "staged", "host"),
     "host_gather": ("gpu_pull", "cpu_loader"),
-    "host_pull_driver": ("graph", "runner"),
     "host_loss": ("mirror", "memcpy"),
 }
 

@@ -3,6 +3,9 @@
 One graph node per GPU on a cycle; times the fused `dsgd_mix` kernel, which pulls both neighbors'
 parameter rows over NVLink (P2P loads through the pointer table) and mixes them in registers, and —
 as the baseline — an NCCL all_gather of the same rows followed by a torch matmul-free mix.
+As in training, every `dsgd_mix` launch starts by announcing its round to the peers (a system fence and one
+NVLink flag store per peer), so the fused time includes that announcement.  The round counter stays at 0,
+so no rank ever waits for a peer.
 Launch: torchrun --nproc-per-node G scripts/bench_exchange.py
 Prints one JSON line per n on rank 0: device time (max over ranks), inbound GB/s per GPU."""
 import json, os, sys

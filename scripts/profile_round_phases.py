@@ -1,5 +1,6 @@
-"""In-kernel phase timing of the one-launch DiNNO round (csrc/dinno_round.cu): every CTA stamps
-%globaltimer at its phase boundaries; prints the mean/max duration of each phase over CTAs for the last round.
+"""In-kernel phase timing of the batch-split MNIST training kernel (mnist_kernel<spb, 768, train> in
+csrc/mnist.cu): with NNDT_STEP_PROF=1 every CTA stamps %globaltimer at its phase boundaries; prints the mean/max
+duration of each phase over the CTAs of the last launch.
 
     python scripts/profile_round_phases.py [--nodes 10] [--rounds 200]
 """
@@ -17,8 +18,11 @@ INNER = ["(images committed)", "conv+relu+pool (+W1 TMA wait)", "fc1 (mma)", "h 
          "fc2 grads, dh", "b1, da1 (mma), dW1 (mma) -> global", "conv-grad acc -> smem"]
 
 
-def per_step(args):
-    """Phase stamps of the last launch of mnist_kernel<spb, 768, train> (the production per-step path)."""
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--nodes", type=int, default=10)
+    ap.add_argument("--rounds", type=int, default=200)
+    args = ap.parse_args()
     from nn_distributed_training_b200.optimizers import DiNNO
     from nn_distributed_training_b200.parallel.context import DistContext
     os.environ["NNDT_STEP_PROF"] = "1"
@@ -43,59 +47,6 @@ def per_step(args):
     print(f"{'CTA lifetime':44s} {((t[:, 23] - t[:, 20]) / 1e3).mean().item():9.2f}")
     print(f"{'after the wait':44s} {((t[:, 23] - t[:, 22]) / 1e3).mean().item():9.2f}")
     print(f"{'first CTA start -> last CTA end':44s} {(t[:, 23].max() - t[:, 20].min()).item() / 1e3:9.2f}")
-
-
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--nodes", type=int, default=10)
-    ap.add_argument("--rounds", type=int, default=200)
-    ap.add_argument("--per-step", action="store_true", help="profile the default per-step kernel (any samples-per-CTA)")
-    args = ap.parse_args()
-    if args.per_step:
-        return per_step(args)
-    from nn_distributed_training_b200.optimizers import DiNNO
-    from nn_distributed_training_b200.parallel.context import DistContext
-    os.environ["NNDT_NO_GRAPH"] = "0"
-    os.environ["NNDT_SPB"] = "8"
-    os.environ["NNDT_FUSED_ROUND"] = "1"
-    ctx = DistContext.single(torch.device("cuda:0"))
-    pr = bench.build_problem(ctx, args.nodes, bench.opt_conf(4000), eval_every=10 ** 9, samples_per_node=4000)
-    S = pr.fused.S
-    pr.fused.round_prof = torch.zeros(args.nodes * S, 64, dtype=torch.int64, device="cuda:0")
-    opt = DiNNO(pr, ctx.device, pr.conf["optimizer_config"])
-    opt.run_rounds(args.rounds)
-    torch.cuda.synchronize()
-    t = pr.fused.round_prof.cpu().double()
-    P = opt.pits
-    names = ["launch->pdl_wait"]
-    idx = [(0, 1)]
-    prev = 1
-    for p in range(P):
-        names += [f"step{p} fwd/bwd", f"step{p} cluster barrier", f"step{p} update"]
-        idx += [(prev, 2 + 4 * p), (2 + 4 * p, 3 + 4 * p), (3 + 4 * p, 4 + 4 * p)]
-        prev = 4 + 4 * p
-        if p < P - 1:
-            names.append(f"step{p} fence + barrier")
-            idx.append((4 + 4 * p, 5 + 4 * p))
-            prev = 5 + 4 * p
-    names.append("finish_round")
-    idx.append((prev, 63))
-    print(f"{'phase':28s} {'mean us':>9s} {'max us':>9s}")
-    for n, (a, b) in zip(names, idx):
-        d = (t[:, b] - t[:, a]) / 1e3
-        print(f"{n:28s} {d.mean().item():9.2f} {d.max().item():9.2f}")
-    inner = ["sample idx", "load images", "conv+relu+pool (+W1 TMA wait)", "fc1 (mma)", "h reduce", "fc2", "softmax/loss",
-             "fc2 grads, dh", "b1, da1 (mma), dW1 (mma) -> global", "conv-grad acc -> smem"]
-    for p in range(min(P, 3)):
-        base = 16 + 16 * p
-        prev = 1 if p == 0 else 5 + 4 * (p - 1)
-        for j, n in enumerate(inner):
-            d = (t[:, base + j] - t[:, prev if j == 0 else base + j - 1]) / 1e3
-            print(f"  step{p} {n:30s} {d.mean().item():7.2f} {d.max().item():7.2f}")
-        d = (t[:, 2 + 4 * p] - t[:, base + len(inner) - 1]) / 1e3
-        print(f"  step{p} {'conv-grad reduce + store':30s} {d.mean().item():7.2f} {d.max().item():7.2f}")
-    print(f"{'kernel span (all CTAs)':28s} {(t[:, 63].max() - t[:, 0].min()).item() / 1e3:9.2f}")
-    print(f"{'first start -> last start':28s} {(t[:, 0].max() - t[:, 0].min()).item() / 1e3:9.2f}")
 
 
 if __name__ == "__main__":

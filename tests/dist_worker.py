@@ -29,13 +29,12 @@ CONFS = {
 METRICS = ["forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy", "current_epoch"]
 
 
-def build(ctx, N, graph, conf, backend, M=200, pipeline="resident", separate_publish=False):
+def build(ctx, N, graph, conf, backend, M=200, pipeline="resident"):
     data = synthetic_mnist(M * N, seed=3)
     val = synthetic_mnist(128, seed=4)
     shards = [data.select(torch.arange(i * M, (i + 1) * M)) for i in range(N)]
     pconf = {"problem_name": "t", "train_batch_size": 32, "val_batch_size": 64, "metrics": METRICS,
-             "metrics_config": {"evaluate_frequency": 3}, "optimizer_config": conf, "input_pipeline": pipeline,
-             "separate_publish": separate_publish}
+             "metrics_config": {"evaluate_frequency": 3}, "optimizer_config": conf, "input_pipeline": pipeline}
     torch.manual_seed(5)
     base = MNISTConvNet(3, 5, 64)
     return DistMNISTProblem(graph, base, torch.nn.NLLLoss(), shards, val, ctx.device, pconf, ctx=ctx,
@@ -103,8 +102,7 @@ def main():
     ap.add_argument("--cuda", type=int, default=0)
     ap.add_argument("--nodes", type=int, default=6)
     ap.add_argument("--graph", default="cycle")
-    ap.add_argument("--pipeline", default="resident")   # host: device-initiated staging + forked peer announcement
-    ap.add_argument("--separate-publish", type=int, default=0)   # 1: peers announced by publish_round_kernel on a forked branch
+    ap.add_argument("--pipeline", default="resident")   # host: device-initiated staging inside multi-round graphs
     ap.add_argument("--delayed", type=int, default=0)   # 1: time-varying graphs (link drops) + a deliberately slow rank
     args = ap.parse_args()
     ctx = DistContext.from_env(use_cuda=bool(args.cuda))
@@ -115,7 +113,7 @@ def main():
         return delayed(ctx, N, G, backend)
     ok = True
     for alg, conf in CONFS.items():
-        pr = build(ctx, N, G, conf, backend, pipeline=args.pipeline, separate_publish=bool(args.separate_publish))
+        pr = build(ctx, N, G, conf, backend, pipeline=args.pipeline)
         opt = build_optimizer(pr, ctx.device, copy.deepcopy(conf))
         opt.train()
         theta = pr.gather_rows(pr.arena.theta).cpu()
@@ -131,8 +129,7 @@ def main():
             vd = (vl - pr1.metrics["validation_loss"][-1]).abs().max().item()
             good = bad < 5e-3 and rel < 1e-2 and vd < 1e-3
             eng = getattr(getattr(opt, "_program", None), "eng", None)
-            how = "" if eng is None else (f" sum_mode={eng.sum_mode} mc={bool(eng.sum_buf and eng.sum_buf.multicast_ptr)}"
-                                          f" separate_publish={eng.separate_publish}")
+            how = "" if eng is None else f" sum_mode={eng.sum_mode} mc={bool(eng.sum_buf and eng.sum_buf.multicast_ptr)}"
             print(f"[dist] {alg} world={ctx.world_size} graph={args.graph}{how} bad={bad:.2e} rel={rel:.2e} "
                   f"val_diff={vd:.2e} {'OK' if good else 'MISMATCH'}", flush=True)
             ok = ok and good

@@ -29,16 +29,13 @@ def test_gloo_two_ranks_match_single_process(graph):
 @pytest.mark.parametrize("graph,pipeline", [("cycle", "auto"), ("complete", "resident"), ("cycle", "host")])
 def test_nccl_peer_mapped_ranks_match_single_process(graph, pipeline):
     """``host``: rows pulled from pinned host memory by the staging kernel inside multi-round graphs, peers
-    announced by publish_round_kernel on a forked branch; the single-process oracle uses resident shards."""
+    announced by the first consensus kernel of each round; the single-process oracle uses resident shards."""
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
     nproc = min(8, n)         # every GPU of the box: 2 on the development boxes, 8 on the scaling box
-    forked = pipeline == "host"           # also cover the optional forked announcement (default: inside the round's last kernel)
-    r = _launch(nproc, ["--cuda", "1", "--nodes", str(3 * nproc), "--graph", graph, "--pipeline", pipeline,
-                        "--separate-publish", str(int(forked))], 29612)
+    r = _launch(nproc, ["--cuda", "1", "--nodes", str(3 * nproc), "--graph", graph, "--pipeline", pipeline], 29612)
     assert "DIST_RESULT PASS" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
-    assert f"separate_publish={forked}" in r.stdout
 
 
 @pytest.mark.gpu

@@ -141,31 +141,6 @@ def test_fused_training_matches_torch_ops(cls, conf, graph):
         _assert_mostly_close(oa.y, ob.y)
 
 
-@pytest.mark.parametrize("graph", ["cycle", "complete"])
-@pytest.mark.parametrize("conf", [DINNO, dict(DINNO, primal_optimizer="sgd", primal_iterations=3),
-                                  dict(DINNO, primal_optimizer="adamw", persistant_primal_opt=True)])
-def test_dinno_round_cluster_kernel_matches_per_step_kernels(conf, graph, monkeypatch):
-    monkeypatch.setenv("NNDT_MNIST_TC", "0")        # the one-launch round kernel builds on the batch-split kernel
-    """csrc/dinno_round.cu (opt-in: one cluster launch per round) vs the per-step kernels it replaces: same
-    arithmetic, same partial-sum order -> the trained parameters agree to rounding."""
-    monkeypatch.setenv("NNDT_SPB", "8")      # one cluster of 8 CTAs per node
-    N = 6
-    G = {"cycle": nx.cycle_graph(N), "complete": nx.complete_graph(N)}[graph]
-    a = _problem(N, 64, "fused", conf, graph=G, eval_every=4)
-    b = _problem(N, 64, "fused", conf, graph=G, eval_every=4)
-    b.arena.theta.copy_(a.arena.theta)
-    oa = DiNNO(a, DEV, dict(copy.deepcopy(conf), fused_round=True))
-    ob = DiNNO(b, DEV, dict(copy.deepcopy(conf), fused_round=False))
-    oa.train()
-    ob.train()
-    assert oa._program.round_op() is not None and ob._program.round_op() is None
-    assert oa._program.launches_per_round() < ob._program.launches_per_round()
-    assert a.forward_cnt == b.forward_cnt
-    assert torch.equal(a.fused.calls, b.fused.calls)
-    assert (a.arena.theta - b.arena.theta).abs().max().item() <= 1e-6 * b.arena.theta.abs().max().item()
-    assert torch.allclose(oa.duals, ob.duals, rtol=1e-5, atol=1e-7)
-
-
 def test_consensus_kernels_fp64_with_autograd_model():
     """fp64 arena on the GPU: autograd forward/backward + fused fp64 consensus kernels (eager)."""
     torch.manual_seed(0)
