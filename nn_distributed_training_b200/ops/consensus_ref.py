@@ -28,12 +28,15 @@ def dinno_exchange_(theta_k: torch.Tensor, theta_all: torch.Tensor, adj_rows: to
     (optimizers/dinno.py:123).  ``delta`` is the only neighbor-dependent term the
     primal gradient needs (closed form of ``rho sum_j |theta-(theta_i^k+theta_j^k)/2|^2``,
     optimizers/dinno.py:85-89,124), so no ``[d_i, n]`` stack is ever built.
-    Differences are accumulated (not sums) so the terms vanish exactly at
-    consensus and keep their precision in fp32 near it.
+    Differences are accumulated per neighbor (not ``sum_j theta_j - d_i theta_i``),
+    as the fused kernel and the reference do, so the terms vanish exactly at
+    consensus and keep their precision near it.  ``deg`` is implied by
+    ``adj_rows`` and kept for the call signature.
     """
     a = adj_rows.to(theta_all.dtype)
-    d = deg.to(theta_k.dtype).unsqueeze(1)
-    delta.copy_(a @ theta_all - d * theta_k)
+    delta.zero_()
+    for j in torch.nonzero(a.any(0)).flatten().tolist():
+        delta.add_(torch.where(a[:, j: j + 1] != 0, theta_all[j] - theta_k, 0.0))
     dual.add_(delta, alpha=-rho)
 
 

@@ -42,8 +42,10 @@ def _density(L, B, M, h1=256, loss="BCE", net="fourier", backend="fused", seed=0
     pr = DistDensityProblem(nx.cycle_graph(L), base, lossf, shards, val, DEV, conf, backend=backend, seed=3)
     assert pr.dtype == torch.float64
     if perturb:
+        # not affine in l: on a cycle an affine perturbation makes delta of the interior nodes exactly 0, and a result
+        # that then hangs on the sign of a round-off residue (tests/test_consensus_oracle.py)
         for l in range(L):
-            pr.arena.theta[l] *= 1.0 + 0.03 * l
+            pr.arena.theta[l] *= 1.0 + 0.03 * l * l
     return pr
 
 
@@ -186,17 +188,20 @@ DSGD_C = {"alg_name": "dsgd", "alpha0": 0.05, "mu": 0.01, "outer_iterations": 7,
 DSGT_C = {"alg_name": "dsgt", "alpha": 0.02, "init_grads": True, "outer_iterations": 7, "profile": False}
 
 
-@pytest.mark.parametrize("cls,conf,consensus", [(DiNNO, DINNO, "torch"), (DSGD, DSGD_C, "auto"), (DSGT, DSGT_C, "auto")])
-def test_f64_fused_density_training_matches_torch_fp64(cls, conf, consensus):
-    """Fused fp64 forward/backward against autograd in float64, the reference run on the PyTorch consensus ops:
-    agreement to fp64 round-off over the whole run.  DSGD and DSGT run their fp64 consensus kernels under CUDA graphs.
-    DiNNO drives the fused forward/backward from the PyTorch consensus ops: on this problem its fused Adam consensus
-    kernel ends 8.5e-5 (relative) away from the PyTorch ops with either forward/backward (H100), while the fused
-    forward/backward alone stays within 1e-14 of autograd."""
+@pytest.mark.parametrize("cls,conf", [(DiNNO, DINNO), (DSGD, DSGD_C), (DSGT, DSGT_C)])
+def test_f64_fused_density_training_matches_torch_fp64(cls, conf):
+    """Fused fp64 forward/backward and fp64 consensus kernels under CUDA graphs against autograd and the PyTorch
+    consensus ops in float64: agreement to fp64 round-off over the whole run.  The nodes start from a perturbation that
+    is not affine in l; an affine one makes delta of the interior nodes of the cycle exactly 0 in exact arithmetic,
+    so on coordinates without a loss gradient Adam steps by +-lr on the sign of a round-off residue, and the run
+    depended on how delta was rounded rather than on the kernels (it ended 8.5e-5 apart while the exchange of the
+    PyTorch ops took sums instead of per-neighbor differences)."""
     a = _density(4, 500, M=700, opt_conf=copy.deepcopy(conf))
     b = _density(4, 500, M=700, backend="torch", opt_conf=copy.deepcopy(conf))
     b.arena.theta.copy_(a.arena.theta)
-    cls(a, DEV, dict(copy.deepcopy(conf), consensus_backend=consensus)).train()
+    opt = cls(a, DEV, dict(copy.deepcopy(conf), consensus_backend="auto"))
+    assert opt._use_engine()
+    opt.train()
     cls(b, DEV, dict(copy.deepcopy(conf), consensus_backend="torch")).train()
     rel = ((a.arena.theta - b.arena.theta).norm() / b.arena.theta.norm()).item()
     assert rel < 1e-8, rel
