@@ -124,6 +124,7 @@ struct ConsensusOp {
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
+    gt.alpha_row = ptr<const T>(d, "alpha_row"); gt.own_tracker = geti(d, "own_tracker", 0);
   }
   void dinno_update(int step) {
     dn.step = step;

@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_init_kernel(const DsgtArgs<T> a)
   step_bookkeeping(c, l);
 }
 
-template <typename T>
+template <typename T, bool OWN>
 __global__ void __launch_bounds__(THREADS) dsgt_mix_kernel(const DsgtArgs<T> a) {
   pdl_wait();
   pdl_launch_dependents();
@@ -246,18 +246,53 @@ __global__ void __launch_bounds__(THREADS) dsgt_mix_kernel(const DsgtArgs<T> a) 
   const size_t row = (size_t)l * c.n_pad;
   const T* ys = pub_row(c, ri.par, 1, l);
   for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
-    if (c.sum_mode) {
-      const DPack<N> st = network_sum(c, ri.par, 0, i), sy = network_sum(c, ri.par, 1, i);
-      Pack<T> th;
+    Pack<T> al;                         // the step of each coordinate: the row, or alpha_k everywhere
+    if (a.alpha_row != nullptr) {
+      al = ldv(a.alpha_row + i);
+    } else {
 #pragma unroll
-      for (int u = 0; u < N; ++u) th.v[u] = (T)((st.v[u] - (double)alpha * sy.v[u]) / (double)c.n_total);
+      for (int u = 0; u < N; ++u) al.v[u] = alpha;
+    }
+    if (c.sum_mode) {
+      const DPack<N> st = network_sum(c, ri.par, 0, i);
+      Pack<T> th;
+      if (OWN) {                        // theta_i = S_theta / N - alpha (.) y_i
+        const Pack<T> y = ldv(ys + i);
+#pragma unroll
+        for (int u = 0; u < N; ++u) th.v[u] = (T)(st.v[u] / (double)c.n_total) - al.v[u] * y.v[u];
+      } else {                          // theta_i = (S_theta - alpha (.) S_y) / N
+        const DPack<N> sy = network_sum(c, ri.par, 1, i);
+#pragma unroll
+        for (int u = 0; u < N; ++u) th.v[u] = (T)((st.v[u] - (double)al.v[u] * sy.v[u]) / (double)c.n_total);
+      }
       stv(c.theta + row + i, th);
       continue;
     }
     Pack<T> th = ldv(c.theta + row + i);
     const Pack<T> y = ldv(ys + i);
+    if (OWN) {
 #pragma unroll
-    for (int u = 0; u < N; ++u) th.v[u] = ws * (th.v[u] - alpha * y.v[u]);
+      for (int u = 0; u < N; ++u) th.v[u] *= ws;
+      for (int e0 = 0; e0 < deg; e0 += 2) {
+        Pack<T> q[2];
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          if (e0 + j < deg) q[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
+#pragma unroll
+        for (int j = 0; j < 2; ++j)
+          if (e0 + j < deg) {
+            const T we = w[e0 + j];
+#pragma unroll
+            for (int u = 0; u < N; ++u) th.v[u] += we * q[j].v[u];
+          }
+      }
+#pragma unroll
+      for (int u = 0; u < N; ++u) th.v[u] -= al.v[u] * y.v[u];
+      stv(c.theta + row + i, th);
+      continue;
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] = ws * (th.v[u] - al.v[u] * y.v[u]);
     for (int e0 = 0; e0 < deg; e0 += 2) {
       Pack<T> qt[2], qy[2];
 #pragma unroll
@@ -271,7 +306,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_mix_kernel(const DsgtArgs<T> a) 
         if (e0 + j < deg) {
           const T we = w[e0 + j];
 #pragma unroll
-          for (int u = 0; u < N; ++u) th.v[u] += we * (qt[j].v[u] - alpha * qy[j].v[u]);
+          for (int u = 0; u < N; ++u) th.v[u] += we * (qt[j].v[u] - al.v[u] * qy[j].v[u]);
         }
     }
     stv(c.theta + row + i, th);
@@ -468,7 +503,10 @@ template <typename T> cudaError_t launch_dsgt_init(const DsgtArgs<T>& a, cudaStr
   return NNDT_BY_S(a.c.S, dsgt_init_kernel, a, a.c);
 }
 template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStream_t st) {
-  return launch_pdl(dsgt_mix_kernel<T>, grid_for(a.c, dsgt_mix_kernel<T>), dim3(THREADS), 0, st, a);
+  // the own-tracker step is a template parameter: as a runtime branch it raised the register count past the
+  // 64 per thread that keep 4 CTAs resident per SM
+  return a.own_tracker ? launch_pdl(dsgt_mix_kernel<T, true>, grid_for(a.c, dsgt_mix_kernel<T, true>), dim3(THREADS), 0, st, a)
+                       : launch_pdl(dsgt_mix_kernel<T, false>, grid_for(a.c, dsgt_mix_kernel<T, false>), dim3(THREADS), 0, st, a);
 }
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st) {
   return NNDT_BY_S(a.c.S, dsgt_track_kernel, a, a.c);

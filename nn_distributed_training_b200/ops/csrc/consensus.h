@@ -77,6 +77,12 @@ template <typename T>
 struct DsgtArgs {
   Common<T> c;
   T* g_old;                        // [L, n_pad]
+  // dsgt_mix variants (the distributed-PPO form): a per-coordinate step row instead of the alpha[k] schedule (constant
+  // over rounds, 0 on the padding; nullptr = schedule), and the own-tracker step
+  //   theta_i <- sum_j W_ij theta_j - alpha (.) y_i        (own_tracker = 1; y_i un-mixed)
+  // instead of theta_i <- sum_j W_ij (theta_j - alpha y_j)
+  const T* alpha_row;              // [n_pad] or nullptr
+  int own_tracker;
 };
 
 template <typename T> cudaError_t launch_dinno_update(const DinnoArgs<T>& a, cudaStream_t st);

@@ -19,6 +19,31 @@ from ..utils.graph_generation import Topology
 OPT_CODE = {"sgd": 0, "adam": 1, "adamw": 2}
 
 
+def schedule_horizon(opt) -> int:
+    """Rounds the device schedules cover: ``opt.horizon`` (``None``: ``outer_iterations``), at most ``outer_iterations``."""
+    H = getattr(opt, "horizon", None)
+    H = opt.oits if H is None else int(H)
+    if not 1 <= H <= opt.oits:
+        raise ValueError(f"schedule horizon {H} outside 1..outer_iterations ({opt.oits})")
+    return H
+
+
+def schedule_tables(opt, H: int):
+    """Host (float64) ``rho`` / ``lr`` / ``alpha`` tables of rounds ``[0, H)``: entry k is ``rho_at(k)``, ``lr_at(k)`` and
+    ``alpha_table()[k]`` with the configured ``outer_iterations`` (linear and log lr decay depend on it), so a table
+    built for a horizon is a prefix of the full one.  A DSGT per-coordinate step leaves ``alpha`` zero (the kernel reads
+    the row instead)."""
+    rho = np.zeros(H); lr = np.zeros(H); alpha = np.zeros(H)
+    if opt.alg_name == "dinno":
+        rho[:] = [opt.rho_at(k) for k in range(H)]
+        lr[:] = [opt.lr_at(k) for k in range(H)]
+    elif opt.alg_name == "dsgd":
+        alpha[:] = opt.alpha_table(H)
+    elif not torch.is_tensor(opt.alpha):
+        alpha[:] = opt.alpha
+    return rho, lr, alpha
+
+
 class ConsensusEngine:
     def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
@@ -42,28 +67,32 @@ class ConsensusEngine:
             self.pub[k0 & 1, 1, :L].copy_(opt.y)
 
         # ---- schedules ----------------------------------------------------------
-        rho = np.zeros(oits); lr = np.zeros(oits); alpha = np.zeros(oits)
-        if opt.alg_name == "dinno":
-            rho[:] = [opt.rho_at(k) for k in range(oits)]
-            lr[:] = [opt.lr_at(k) for k in range(oits)]
-        elif opt.alg_name == "dsgd":
-            alpha[:] = opt.alpha_table()
-        else:
-            alpha[:] = opt.alpha
+        H = self.horizon = schedule_horizon(opt)
+        rho, lr, alpha = schedule_tables(opt, H)
         self.rho = torch.as_tensor(rho.astype(npdt), device=dev)
         self.lr = torch.as_tensor(lr.astype(npdt), device=dev)
         self.alpha = torch.as_tensor(alpha.astype(npdt), device=dev)
+        # DSGT with a per-coordinate step: the [n_pad] row replaces the alpha_k schedule in dsgt_mix
+        self.alpha_row = None
+        if opt.alg_name == "dsgt" and torch.is_tensor(opt.alpha):
+            self.alpha_row = opt.alpha.detach().to(device=dev, dtype=self.dtype).reshape(-1).contiguous()
+            if self.alpha_row.numel() != n_pad:
+                raise ValueError(f"per-coordinate alpha has {self.alpha_row.numel()} entries for rows of {n_pad}")
 
         # ---- topology tables ------------------------------------------------------
         topos: List[Topology] = []
         key_to_id: Dict[bytes, int] = {}
-        gid = np.zeros(oits, dtype=np.int32)
+        gid = np.zeros(H, dtype=np.int32)
+        by_object: Dict[int, int] = {}     # a static plan repeats one graph object: build its topology once
         for k, g in enumerate(graphs_per_round):
-            t = pr._topo_cache.get(g) if hasattr(pr, "_topo_cache") else Topology(g)
-            if t.key not in key_to_id:
-                key_to_id[t.key] = len(topos)
-                topos.append(t)
-            gid[k] = key_to_id[t.key]
+            gi = by_object.get(id(g))
+            if gi is None:
+                t = pr._topo_cache.get(g) if hasattr(pr, "_topo_cache") else Topology(g)
+                if t.key not in key_to_id:
+                    key_to_id[t.key] = len(topos)
+                    topos.append(t)
+                gi = by_object[id(g)] = key_to_id[t.key]
+            gid[k] = gi
         self.topos = topos
         G = len(topos)
         dmax = max(1, max(t.max_degree for t in topos))
@@ -204,7 +233,8 @@ class ConsensusEngine:
                      v=None if opt.v is None else opt.v.data_ptr(),
                      pits=opt.pits, opt=OPT_CODE[opt.opt_kind], persistent=int(opt.persistent))
         if opt.alg_name == "dsgt":
-            d.update(g_old=opt.g.data_ptr())
+            d.update(g_old=opt.g.data_ptr(), own_tracker=int(bool(getattr(opt, "own_tracker_step", False))),
+                     alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d

@@ -105,9 +105,10 @@ def _batch(name, t, shape, dtype, dev):
     return t.contiguous()
 
 
-def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor) -> torch.Tensor:
+def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``[N, R]`` normalised advantages ``(A - mean) / (std + 1e-10)`` of ``A = rtgs - critic_i(obs[i])``, with node
-    ``i``'s mean and unbiased std (so NaN for R = 1, as torch's ``std``).  ``critics``: one per node."""
+    ``i``'s mean and unbiased std (so NaN for R = 1, as torch's ``std``).  ``critics``: one per node.  ``out``: a
+    contiguous ``[N, R]`` tensor of the batch dtype to write them into (returned)."""
     crits = _as_list(critics)
     require(None, crits)
     ext = load_ext(required=True)
@@ -118,10 +119,19 @@ def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor) -> torch.Tensor:
     d = _desc(None, crits, dt, N, R)
     obs = _batch("obs", obs, (N, R, d["dims"][1][0]), dt, dev)
     rtgs = rtgs.contiguous()
-    adv = torch.empty(N, R, device=dev, dtype=dt)
+    adv = torch.empty(N, R, device=dev, dtype=dt) if out is None else _out("out", out, (N, R), dt, dev)
     d.update(obs=obs.data_ptr(), rtgs=rtgs.data_ptr(), adv=adv.data_ptr())
     ext.ppo_advantages(d)
     return adv
+
+
+def _out(name, t, shape, dtype, dev):
+    """An output tensor the kernel writes in place: exactly ``shape``, ``dtype``, ``dev`` and contiguous."""
+    if not torch.is_tensor(t) or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != dev \
+            or not t.is_contiguous():
+        got = (tuple(t.shape), t.dtype, t.device) if torch.is_tensor(t) else type(t).__name__
+        raise ValueError(f"{name}: expected a contiguous {tuple(shape)} {dtype} tensor on {dev}, got {got}")
+    return t
 
 
 # Network and gradient descriptions already validated, keyed by every parameter's and gradient tensor's address and
@@ -159,11 +169,13 @@ def _grads_desc(acts_l, crits, grad_out, N, R, dt, dev):
 
 def grads(actors, critics, obs: torch.Tensor, acts: torch.Tensor, old_lp: torch.Tensor, rtgs: torch.Tensor,
           adv: torch.Tensor, clip: float, cov_var: float, grad_out: Sequence[Sequence[torch.Tensor]],
-          nonfinite: Optional[torch.Tensor] = None) -> torch.Tensor:
+          nonfinite: Optional[torch.Tensor] = None, losses_out: Optional[torch.Tensor] = None) -> torch.Tensor:
     """One primal step of every node: writes the gradients of node ``i``'s PPO-clip actor loss and critic MSE into
     ``grad_out[i]`` — one tensor per parameter, in ``parameters()`` order of the actor then the critic (arena-row views
-    or ``p.grad``) — and returns ``losses [N, 2]`` (actor, critic).  ``nonfinite``, an int32 CUDA tensor, is set to 1
-    if an actor mean is not finite; it is never cleared here.  Nothing is synchronised."""
+    or ``p.grad``) — and returns ``losses [N, 2]`` (actor, critic), written into ``losses_out`` when given (a
+    contiguous ``[N, 2]`` tensor of the batch dtype, for example a row of a buffer a CUDA graph replays into).
+    ``nonfinite``, an int32 CUDA tensor, is set to 1 if an actor mean is not finite; it is never cleared here.  Nothing
+    is synchronised."""
     acts_l, crits = _as_list(actors), _as_list(critics)
     ext = load_ext(required=True)
     if rtgs.dim() != 2:
@@ -178,7 +190,7 @@ def grads(actors, critics, obs: torch.Tensor, acts: torch.Tensor, old_lp: torch.
     old_lp = _batch("old_lp", old_lp, (N, R), dt, dev)
     adv = _batch("adv", adv, (N, R), dt, dev)
     rtgs = rtgs.contiguous()
-    losses = torch.empty(N, 2, device=dev, dtype=dt)
+    losses = torch.empty(N, 2, device=dev, dtype=dt) if losses_out is None else _out("losses_out", losses_out, (N, 2), dt, dev)
     if nonfinite is None:
         nonfinite = torch.zeros(1, device=dev, dtype=torch.int32)
     elif nonfinite.dtype != torch.int32 or nonfinite.device != dev:

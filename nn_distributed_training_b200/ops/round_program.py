@@ -13,12 +13,13 @@ eagerly around an autograd step.
 """
 from __future__ import annotations
 
+import gc
 import os
 from typing import Dict
 
 import torch
 
-from .engine import ConsensusEngine
+from .engine import ConsensusEngine, schedule_horizon
 
 MAX_ROUNDS_PER_GRAPH = 64
 PULL_ROUNDS_PER_GRAPH = 64     # host-fed / staged rounds captured per graph (staging kernel forked inside the graph); a
@@ -55,6 +56,13 @@ def _round_ops_impl(opt, eng, grads):
         raise NameError("Unknown distributed opt algorithm.")
 
 
+def _collect_before_capture():
+    """Collect cyclic garbage before a capture: an unreachable program of an earlier run (optimizer, program and problem
+    reference each other) may still own CUDA graphs, and the collector destroying one of them in the middle of a capture
+    invalidates that capture."""
+    gc.collect()
+
+
 def draws_per_round(opt) -> int:
     return opt.pits if opt.alg_name == "dinno" else 1
 
@@ -67,9 +75,12 @@ class RoundProgram:
         pr = self.pr = opt.pr
         self.dpr = draws_per_round(opt)
         init_draws = 1 if (opt.alg_name == "dsgt" and opt.init_grads and not opt._initialised) else 0
-        graphs = pr.plan_graphs(opt.oits, opt.k, self.dpr, init_draws,
+        graphs = pr.plan_graphs(schedule_horizon(opt), opt.k, self.dpr, init_draws,
                                 refresh=getattr(opt, "refresh_graph", True))
-        self.capturable = pr.fused is not None and os.environ.get("NNDT_NO_GRAPH", "0") != "1"
+        # a problem without a fused forward/backward kernel is captured when its gradient step is (a batched hook over
+        # fixed buffers, ReferenceProblemAdapter.capturable_grads); per-node autograd runs eagerly between the kernels
+        self.capturable = ((pr.fused is not None or getattr(pr, "capturable_grads", False))
+                           and os.environ.get("NNDT_NO_GRAPH", "0") != "1")
         # ---- input pipeline of the fused MNIST problem ------------------------------------------------------------
         pipeline = "resident"
         if pr.fused is not None:
@@ -153,6 +164,7 @@ class RoundProgram:
         if self._side is None:
             self._side = torch.cuda.Stream(device=self.pr.device)
         side = self._side
+        _collect_before_capture()
         g = torch.cuda.CUDAGraph()
         with torch.cuda.graph(g):
             main = torch.cuda.current_stream(self.pr.device)
@@ -216,12 +228,17 @@ class RoundProgram:
     def _resident_graph(self, r: int):
         g = self._graphs.get(r)
         if g is None:
+            _collect_before_capture()
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 for _ in range(r):
                     _round_ops(self.opt, self.eng, self.grads)
             self._graphs[r] = g
         return g
+
+    def drop_graphs(self):
+        """Forget the captured resident-round graphs (their kernels read buffers that have been reallocated)."""
+        self._graphs.clear()
 
     def prepare(self, rounds: int):
         """Capture (without executing) every CUDA graph that ``run(rounds)`` will replay from the current state, so a
@@ -240,6 +257,9 @@ class RoundProgram:
 
     def run(self, rounds: int):
         """Execute ``rounds`` consecutive rounds starting at the device round counter."""
+        if self.opt.k + rounds > self.eng.horizon:
+            raise RuntimeError(f"rounds {self.opt.k}..{self.opt.k + rounds - 1} run past the schedule horizon of "
+                               f"{self.eng.horizon} rounds")
         if self.host_mode:
             return self._run_host_fed(rounds)
         left = rounds
@@ -263,7 +283,7 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name == "dsgd" and opt.k > 0:
-            opt.alph = opt.alpha_table()[opt.k - 1]
+            opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
 
 
 def run_fused_training(opt, profiler=None):

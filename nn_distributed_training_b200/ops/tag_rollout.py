@@ -108,11 +108,13 @@ def reset_positions(env, n_ep: int) -> torch.Tensor:
 
 
 def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_scale: float = 1.0, key: int = 0,
-            index: int = 0, pos0: Optional[torch.Tensor] = None, debug: bool = False) -> Dict[str, torch.Tensor]:
+            index: int = 0, pos0: Optional[torch.Tensor] = None, debug: bool = False,
+            out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
     """Run ``n_ep`` episodes of ``T`` cycles in ``env.E`` worlds each.  ``actors``: one module shared by every predator,
     or one per predator.  ``pos0`` defaults to ``reset_positions(env, n_ep)``.  ``debug`` adds the standard-normal
-    draws ``eps [N, R, 5]`` and the positions after every cycle ``pos [n_ep, T, E, A, 2]``.  Afterwards ``env`` holds
-    the last episode's final state, as after the torch loop."""
+    draws ``eps [N, R, 5]`` and the positions after every cycle ``pos [n_ep, T, E, A, 2]``.  ``out``: contiguous
+    ``obs`` / ``acts`` / ``log_probs`` / ``rtgs`` tensors of the batch's shapes to write into (persistent buffers);
+    the returned dict holds them.  Afterwards ``env`` holds the last episode's final state, as after the torch loop."""
     require(env, actors)
     ext = load_ext(required=True)
     dev, dt = env.device, env.dtype
@@ -149,8 +151,14 @@ def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_
     dims = [lins[0][0].in_features] + [m.out_features for m in lins[0]]
     R = n_ep * T * E
     kw = dict(device=dev, dtype=dt)
-    out = dict(obs=torch.empty(N, R, dims[0], **kw), acts=torch.empty(N, R, ACT_DIM, **kw),
-               log_probs=torch.empty(N, R, **kw), rtgs=torch.empty(N, R, **kw), ep_returns=torch.empty(n_ep * E, **kw))
+    shapes = dict(obs=(N, R, dims[0]), acts=(N, R, ACT_DIM), log_probs=(N, R), rtgs=(N, R))
+    given = out or {}
+    for k, t in given.items():
+        if k not in shapes or not torch.is_tensor(t) or tuple(t.shape) != shapes[k] or t.dtype != dt \
+                or t.device.type != torch.device(dev).type or not t.is_contiguous():
+            raise ValueError(f"out[{k!r}]: expected a contiguous {shapes.get(k)} {dt} tensor on {dev}")
+    out = {k: given[k] if k in given else torch.empty(*shp, **kw) for k, shp in shapes.items()}
+    out["ep_returns"] = torch.empty(n_ep * E, **kw)
     final_pos = torch.empty(n_ep, E, A, 2, **kw)
     final_vel = torch.empty(n_ep, E, A, 2, **kw)
     if debug:

@@ -50,6 +50,17 @@ class ReferenceProblemAdapter:
         self.last_losses = torch.zeros(self.N, device=self.device, dtype=self.dtype)
 
     @property
+    def capturable_grads(self) -> bool:
+        """True when ``compute_grads`` may be captured in a CUDA graph and replayed: the inner problem's
+        ``batched_grads`` hook reads only tensors at fixed addresses and has no per-call host side effects, which the
+        problem states with its own ``capturable_grads``.  Otherwise the consensus kernels run eagerly around it."""
+        return getattr(self.inner, "batched_grads", None) is not None and bool(getattr(self.inner, "capturable_grads", False))
+
+    def plan_graphs(self, oits: int, k0: int, draws_per_round: int, init_draws: int = 0, refresh: bool = True):
+        """Communication graph of rounds ``0..oits-1``: the inner problem's graph, which is static."""
+        return [self.inner.graph] * oits
+
+    @property
     def graph(self):
         return self.inner.graph
 
@@ -94,6 +105,9 @@ class ConsensusOptimizer:
         self.conf = conf
         self.device = torch.device(device)
         self.oits = int(conf["outer_iterations"])
+        # rounds [0, horizon) whose schedules the fused engine builds (None: all oits); a driver that knows it stops early
+        # (the PPO trainers stop at max_rl_timesteps) sets it so no table of outer_iterations entries is built
+        self.horizon = None
         self.k = 0  # next round to execute (resume point)
         self.mixing_order = conf.get("mixing_order", "jacobi")
         if self.mixing_order not in ("jacobi", "reference"):
@@ -183,17 +197,32 @@ class ConsensusOptimizer:
         prog.prepare(n)
 
     def _use_engine(self) -> bool:
-        """Fused sm_90a consensus kernels: any arena problem on a CUDA device with the
-        synchronous (Jacobi) update order; the PyTorch ops remain for CPU/gloo, for
-        foreign problem objects and for the reference-order oracle mode."""
-        if self.mixing_order != "jacobi" or not isinstance(self.pr, ConsensusProblem):
+        """Fused sm_90a consensus kernels.  ``consensus_backend``: ``torch`` never; ``auto`` (default) for any arena
+        problem on a CUDA device with the synchronous (Jacobi) update order, while foreign problem objects, CPU/gloo and
+        the reference-order oracle mode keep the PyTorch ops; ``fused`` also for a foreign problem (through
+        ``ReferenceProblemAdapter``), and a configuration the kernels cannot run raises ``ValueError`` naming why."""
+        backend = self.conf.get("consensus_backend", "auto")
+        if backend == "torch":
             return False
-        if self.device.type != "cuda" or self.conf.get("consensus_backend", "auto") == "torch":
+        if backend != "fused" and not isinstance(self.pr, ConsensusProblem):
             return False
+        why = self._engine_unsupported()
+        if why is not None and backend == "fused":
+            raise ValueError(f"consensus backend 'fused' cannot run this {self.alg_name.upper()} run: {why}")
+        return why is None
+
+    def _engine_unsupported(self) -> Optional[str]:
+        """Why the fused consensus kernels cannot run this optimizer (``None`` if they can)."""
+        if self.mixing_order != "jacobi":
+            return f"mixing_order {self.mixing_order!r} runs on the PyTorch ops only"
+        if self.device.type != "cuda":
+            return f"it needs a CUDA device (the device is {self.device})"
         if self.arena.dtype not in (torch.float32, torch.float64):
-            return False
+            return f"parameter dtype {self.arena.dtype} (needs float32 or float64)"
         from ..ops import fused_available
-        return fused_available()
+        if not fused_available():
+            return "no CUDA device or no sm_90a extension is available"
+        return None
 
     def _round(self, k: int):
         raise NotImplementedError

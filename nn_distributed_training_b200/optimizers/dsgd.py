@@ -31,9 +31,10 @@ class DSGD(ConsensusOptimizer):
         # Q6: the reference never refreshes a dynamic graph for DSGD
         self.refresh_graph = bool(conf.get("update_graph", True))
 
-    def alpha_table(self):
+    def alpha_table(self, n=None):
+        """alpha of rounds 0..n-1 (default: all ``outer_iterations``)."""
         out, a = [], self.alph0
-        for _ in range(self.oits):
+        for _ in range(self.oits if n is None else int(n)):
             a = ref.dsgd_alpha(a, self.mu)
             out.append(a)
         return out

@@ -8,6 +8,10 @@
 
 The reference's per-tensor ``norm().item()`` host syncs (:100,105, SURVEY Q16)
 are dropped.  ``mixing_order: reference`` reproduces its sequential sweeps.
+
+The distributed-PPO variants (rl/consensus_ppo.py) also run on the fused kernels:
+a per-coordinate step ``alpha`` (a tensor [n_pad]) and ``own_tracker_step``
+    theta_i^{k+1} = sum_j W_ij theta_j^k - alpha y_i^k
 """
 from __future__ import annotations
 
@@ -75,14 +79,6 @@ class DSGT(ConsensusOptimizer):
         loss = inner.local_batch_loss(i)
         grads = torch.autograd.grad(loss, list(pr.models[i].parameters()))
         pr.arena.set_row_from_grads(i, grads)
-
-    def _use_engine(self) -> bool:
-        # the fused dsgt_mix kernel implements theta_i <- sum_j W_ij (theta_j - alpha y_j) with a scalar alpha: the RL
-        # variant (own tracker, un-mixed) and per-coordinate step sizes stay on the PyTorch ops instead of being
-        # silently ignored
-        if self.own_tracker_step or torch.is_tensor(self.alpha):
-            return False
-        return super()._use_engine()
 
     def state_dict(self) -> Dict:
         sd = super().state_dict()

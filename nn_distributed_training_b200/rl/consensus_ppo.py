@@ -29,20 +29,80 @@ def agreement(problem) -> np.ndarray:
         return torch.cdist(th, th.mean(0, keepdim=True)).reshape(-1).cpu().numpy()
 
 
+def schedule_horizon(conf, problem, oits: int, rounds_per_iteration: int) -> int:
+    """Rounds a trainer can run: every batch collects at least ``timesteps_per_batch`` steps (on both rollout paths),
+    so ``train()`` stops after ``ceil(max_rl_timesteps / timesteps_per_batch)`` iterations at the latest, or at
+    ``outer_iterations``.  At most ``oits``, the inner optimizer's round count."""
+    its = min(int(conf.get("outer_iterations", 10 ** 12)),
+              -(-int(conf["max_rl_timesteps"]) // int(problem.timesteps_per_batch)))
+    return max(1, min(int(oits), its * int(rounds_per_iteration)))
+
+
 class _ConsensusPPO:
+    """``consensus_backend`` (conf): ``torch`` (default) runs each round as PyTorch ops from Python; ``fused`` runs an
+    iteration's rounds on the sm_90a consensus kernels (ops/csrc/consensus.cu), replayed from one CUDA graph when the
+    gradient step is the update kernels (update_backend "cuda") and eagerly around per-node autograd otherwise."""
     alg = "base"
 
     def __init__(self, ddl_problem, device, conf):
         self.pr, self.conf, self.device = ddl_problem, conf, torch.device(device)
         self.out_dir = conf.get("out_dir", "./trained")
+        backend = conf.get("consensus_backend", "torch")
+        if backend not in ("torch", "fused"):
+            raise ValueError(f"consensus_backend must be 'torch' or 'fused', not {backend!r}")
         self.inner = self._make_inner()
+        self.fused = backend == "fused"
+        if self.fused:
+            self.inner._use_engine()          # raises ValueError naming what the fused kernels cannot run
+            self.inner.horizon = schedule_horizon(self.conf, self.pr, self.inner.oits, self.rounds_per_iteration())
+            if self.pr.batched_grads is not None:
+                self.pr.use_fixed_batch(self.steps_per_iteration())
+            self._batch_version = None
         self.avg_ep_rews, self.timesteps, self.agreements = [], [], []
 
     def _make_inner(self):
         raise NotImplementedError
 
+    def rounds_per_iteration(self) -> int:
+        """Consensus rounds of one iteration."""
+        return self.pr.n_updates_per_iteration
+
+    def steps_per_iteration(self) -> int:
+        """Gradient steps (``compute_grads`` calls) of one iteration."""
+        return self.pr.n_updates_per_iteration
+
     def _consensus(self, k):
-        self.inner._round(k)
+        if self.fused:
+            return self._fused_rounds()
+        for _ in range(self.rounds_per_iteration()):
+            self.inner._round(k)
+
+    def _fused_rounds(self):
+        """The iteration's rounds on the fused kernels: ``inner.run_rounds``, the same rounds and schedule values as
+        ``_round(k)`` on the torch path."""
+        pr, inner = self.pr, self.inner
+        if inner.alg_name == "dsgt":
+            # the torch trainer never runs _before_training, so init_grads is not honoured there and y = g = 0 at the
+            # first round; marking the tracker initialised keeps the engine from starting a dsgt_init of its own (after
+            # a caller's _before_training the engine takes the optimizer's y and g, as it always does)
+            inner._initialised = True
+        prog = getattr(inner, "_program", None)
+        if prog is not None and pr.batch_version != self._batch_version:
+            prog.drop_graphs()               # the batch buffers moved (R changed): recapture against the new ones
+        self._batch_version = pr.batch_version
+        if pr.capturable_grads:
+            pr.begin_steps()
+        inner.run_rounds(self.rounds_per_iteration())
+        if pr.capturable_grads:
+            pr.end_steps()
+
+    def agreement(self) -> np.ndarray:
+        """``agreement(problem)`` of the current parameters; on the fused path the consensus-metric kernel's distance to
+        the mean on the published rows (fp64 accumulation; the arena padding is zero), in the parameters' dtype."""
+        if not self.fused:
+            return agreement(self.pr)
+        _, mean = self.inner._program.eng.consensus_metric(self.inner.k)
+        return mean.reshape(-1).to(self.inner.arena.dtype).numpy()
 
     def train(self, profiler=None):
         k = 0
@@ -53,7 +113,7 @@ class _ConsensusPPO:
             self.pr.check_update()
             self.avg_ep_rews.append(self.pr.avg_episode_reward())
             self.timesteps.append(self.pr.logger["t_so_far"])
-            self.agreements.append(agreement(self.pr))
+            self.agreements.append(self.agreement())
             self.pr._log_summary()
             if profiler is not None:
                 profiler.step()
@@ -99,6 +159,12 @@ class DiNNOPPO(_ConsensusPPO):
         c.setdefault("consensus_backend", "torch")
         return DiNNO(self.pr, self.device, c)
 
+    def rounds_per_iteration(self) -> int:
+        return 1
+
+    def steps_per_iteration(self) -> int:
+        return self.inner.pits
+
 
 class DSGDPPO(_ConsensusPPO):
     """conf: alpha0, mu, max_rl_timesteps, ID; ``n_updates_per_iteration`` mix+step passes per rollout."""
@@ -110,10 +176,6 @@ class DSGDPPO(_ConsensusPPO):
         c.setdefault("outer_iterations", 10 ** 12)
         c.setdefault("consensus_backend", "torch")
         return DSGD(self.pr, self.device, c)
-
-    def _consensus(self, k):
-        for _ in range(self.pr.n_updates_per_iteration):
-            self.inner._round(k)
 
 
 class DSGTPPO(_ConsensusPPO):
@@ -137,7 +199,3 @@ class DSGTPPO(_ConsensusPPO):
                 alpha[s.offset: s.offset + s.numel] = c["alpha_actor"] if s.name.startswith("actor") else c["alpha_critic"]
             inner.alpha = alpha
         return inner
-
-    def _consensus(self, k):
-        for _ in range(self.pr.n_updates_per_iteration):
-            self.inner._round(k)

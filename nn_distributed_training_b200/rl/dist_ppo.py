@@ -22,6 +22,9 @@ from .model import ActorCritic
 from .simple_tag import SimpleTagEnv, heuristic_prey_action
 
 
+BATCH_KEYS = ("obs", "acts", "log_probs", "rtgs")
+
+
 class DistPPOProblem:
     # defaults of the reference's _init_hyperparameters (:391-436) — set explicitly, no exec()
     # rollout_backend "cuda": each batch is one fused kernel launch (ops/tag_rollout.py) with its own Philox noise stream
@@ -71,12 +74,61 @@ class DistPPOProblem:
             raise ValueError(f"update_backend must be 'torch' or 'cuda', not {self.update_backend!r}")
         # batched gradient hook of ReferenceProblemAdapter.compute_grads (None: per-node autograd)
         self.batched_grads = None
+        # fused consensus (use_fixed_batch): the batch lives in persistent buffers, so the gradient step can be replayed
+        self.fixed_batch = False
+        self.batch_version = 0
         if self.update_backend == "cuda":
             from ..ops import ppo_update
             ppo_update.require(self.actors, self.critics)
             self.batched_grads = self._cuda_grads
             self._nonfinite = torch.zeros(1, device=self.device, dtype=torch.int32)
             self._checked = True   # the flag holds nothing unchecked
+
+    @property
+    def capturable_grads(self) -> bool:
+        """True when ``batched_grads`` reads only tensors at fixed addresses and has no per-call host side effects, so
+        the consensus rounds around it can be captured in a CUDA graph and replayed (``ReferenceProblemAdapter``)."""
+        return self.fixed_batch and self.batched_grads is not None
+
+    def use_fixed_batch(self, steps_per_iteration: int):
+        """Fused-consensus mode of the trainers: from the next batch on, ``obs`` / ``acts`` / ``log_probs`` / ``rtgs``
+        and the advantages live in persistent ``[N, R, ...]`` buffers (reallocated, with ``batch_version`` bumped, only
+        when R changes) and each primal step's ``[N, 2]`` losses go to row ``s`` of ``step_losses [steps_per_iteration,
+        N, 2]``, s counted from ``begin_steps()``; ``end_steps()`` then logs them.  ``curr_*[i]`` / ``A_k[i]`` stay views of
+        row i."""
+        self.fixed_batch = True
+        self._bufs = None
+        self._loss_step = 0
+        self._in_steps = False
+        if self.update_backend == "cuda":
+            p = next(self.models[0].parameters())
+            self.step_losses = torch.zeros(int(steps_per_iteration), self.N, 2, device=p.device, dtype=p.dtype)
+
+    def _into_buffers(self, out):
+        b = self._bufs
+        if b is None or any(b[k].shape != out[k].shape or b[k].dtype != out[k].dtype for k in BATCH_KEYS):
+            b = self._bufs = {k: torch.empty(out[k].shape, dtype=out[k].dtype, device=out[k].device) for k in BATCH_KEYS}
+            b["adv"] = torch.empty(out["rtgs"].shape, dtype=out["rtgs"].dtype, device=out["rtgs"].device)
+            self.batch_version += 1
+        for k in BATCH_KEYS:
+            if out[k] is not b[k]:
+                b[k].copy_(out[k])
+        return b
+
+    def begin_steps(self):
+        """Fused consensus: the next primal step writes its losses into row 0 of ``step_losses``."""
+        self._loss_step = 0
+        self._in_steps = True
+
+    def end_steps(self):
+        """Fused consensus, after the steps of an iteration ran (replayed or eager): log their actor losses as the
+        update path does and mark the non-finite flag unchecked for ``check_update()``."""
+        self._in_steps = False
+        if self.update_backend != "cuda":
+            return
+        vals = self.step_losses.clone()
+        self.logger["actor_losses"].extend(vals[s, i, 0] for s in range(vals.shape[0]) for i in range(self.N))
+        self._checked = False
 
     @property
     def actors(self):
@@ -164,8 +216,10 @@ class DistPPOProblem:
         n_ep = max(1, -(-self.timesteps_per_batch // (N * env.E * T)))
         if self._rollout_key is None:
             self._rollout_key = tag_rollout.draw_key()
+        b, R = getattr(self, "_bufs", None), n_ep * T * env.E
+        into = {k: b[k] for k in BATCH_KEYS} if self.fixed_batch and b is not None and b["rtgs"].shape == (N, R) else None
         out = tag_rollout.rollout(env, self.actors, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
-                                  key=self._rollout_key, index=self._rollout_index)
+                                  key=self._rollout_key, index=self._rollout_index, out=into)
         self._rollout_index += 1
         self._stack_batch(out)
         ep_lens = [T * env.num_agents] * (n_ep * env.E)
@@ -176,7 +230,9 @@ class DistPPOProblem:
 
     def _stack_batch(self, out):
         """Keep the batch as ``[N, R, ...]`` tensors (the update kernels' layout); ``curr_*[i]`` are views of row i."""
-        self._batch = {k: out[k] for k in ("obs", "acts", "log_probs", "rtgs")}
+        if self.fixed_batch:
+            out = self._into_buffers(out)
+        self._batch = {k: out[k] for k in BATCH_KEYS}
         self.curr_obs = {i: out["obs"][i] for i in range(self.N)}
         self.curr_acts = {i: out["acts"][i] for i in range(self.N)}
         self.curr_log_probs = {i: out["log_probs"][i] for i in range(self.N)}
@@ -195,7 +251,8 @@ class DistPPOProblem:
         if self.update_backend == "cuda":
             from ..ops import ppo_update
             self.check_update()   # the previous iteration's steps, if the driver did not check them
-            self._adv = ppo_update.advantages(self.critics, self._batch["obs"], self._batch["rtgs"])
+            self._adv = ppo_update.advantages(self.critics, self._batch["obs"], self._batch["rtgs"],
+                                              out=self._bufs["adv"] if self.fixed_batch else None)
             self.A_k = {i: self._adv[i] for i in range(self.N)}
             return
         self.A_k = {}
@@ -227,6 +284,16 @@ class DistPPOProblem:
         tensor per parameter of models[i]) and returns the per-node losses ``[N, 2]`` without a host synchronisation."""
         from ..ops import ppo_update
         b = self._batch
+        if self.fixed_batch:     # fused consensus: replayable, the trainer logs step_losses after the iteration
+            slot = self._loss_step % self.step_losses.shape[0]
+            self._loss_step += 1
+            losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], b["rtgs"],
+                                      self._adv, self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite,
+                                      losses_out=self.step_losses[slot])
+            self._checked = False
+            if not self._in_steps:   # a step outside the trainer's iteration (DSGT's init_grads): logged as it runs
+                self.logger["actor_losses"].extend(losses.clone()[:, 0])
+            return losses
         losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], b["rtgs"], self._adv,
                                   self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite)
         self.logger["actor_losses"].extend(losses[i, 0] for i in range(self.N))

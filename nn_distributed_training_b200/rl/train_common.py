@@ -21,6 +21,9 @@ def parse_args(argv=None, default_id=0):
     ap.add_argument("--update", choices=("torch", "cuda"), default="torch",
                     help="cuda: advantages and each primal step's gradients of every predator are fused kernels "
                          "(needs --device cuda)")
+    ap.add_argument("--consensus", choices=("torch", "cuda"), default="torch",
+                    help="cuda: each iteration's consensus rounds run on the fused consensus kernels, replayed from one "
+                         "CUDA graph with --update cuda (needs --device cuda)")
     ap.add_argument("--ID", type=int, default=default_id, help="suffix of the files written to --out_dir")
     ap.add_argument("--out_dir", default="./trained")
     ap.add_argument("--save_freq", type=int, default=10)
@@ -49,4 +52,4 @@ def make_problem(args):
 
 def common_conf(args):
     return {"max_rl_timesteps": args.max_rl_timesteps, "ID": args.ID, "out_dir": args.out_dir,
-            "writeout": not args.no_writeout}
+            "writeout": not args.no_writeout, "consensus_backend": "fused" if args.consensus == "cuda" else "torch"}
