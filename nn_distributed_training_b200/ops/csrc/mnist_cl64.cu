@@ -83,6 +83,40 @@ NNDT_DEVINL void warp_reduce_scatter16(double (&v)[16], int lane) {
   fold_half<8>(v, lane); fold_half<4>(v, lane); fold_half<2>(v, lane); fold_half<1>(v, lane);
   v[0] += __shfl_xor_sync(0xffffffffu, v[0], 1);
 }
+// The DMMA k-loop of this kernel: c[j] += sum_k A(m0 + ., k) B(k, n0 + 8 j + .) over k < K, step by step in the k order of
+// gemm() in common.cuh, so every accumulator sees the same products in the same sequence.  K is a compile-time constant
+// and the loop is unrolled; the fragments of step k + 4 are read before the DMMA of step k, and the mma is not volatile,
+// so the compiler may schedule the shared-memory reads of the next step under the current DMMA chain.
+NNDT_DEVINL void dmma_nv(double (&c)[4], double a0, double a1, double b) {
+  asm("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+      : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+      : "d"(a0), "d"(a1), "d"(b));
+}
+template <int NJ, int K, class FA, class FB>
+NNDT_DEVINL void gemm_k(double (&c)[NJ][4], int m0, int n0, int lane, FA A, FB B) {
+  static_assert(K % 4 == 0, "k steps of 4");
+  const int g = lane >> 2, t = lane & 3;
+  double a0 = A(m0 + g, t), a1 = A(m0 + g + 8, t), b[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) b[j] = B(t, n0 + 8 * j + g);
+#pragma unroll
+  for (int k0 = 0; k0 < K; k0 += 4) {
+    double na0 = 0.0, na1 = 0.0, nb[NJ];
+    if (k0 + 4 < K) {
+      const int k = k0 + 4 + t;
+      na0 = A(m0 + g, k); na1 = A(m0 + g + 8, k);
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) nb[j] = B(k, n0 + 8 * j + g);
+    }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) dmma_nv(c[j], a0, a1, b[j]);
+    if (k0 + 4 < K) {
+      a0 = na0; a1 = na1;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) b[j] = nb[j];
+    }
+  }
+}
 NNDT_DEVINL void stamp(long long* prof, int idx, int tid) {
   if (prof != nullptr && tid == 0) {
     long long t;
@@ -276,7 +310,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       const int m0 = 16 * (warp / NGRP), n0 = 8 * NJ1 * (warp % NGRP);
       double acc[NJ1][4];
       zero(acc);
-      gemm<NJ1>(acc, m0, n0, KC, lane, at(sm.a, WS), at_t(sm.w, WS));
+      gemm_k<NJ1, KC>(acc, m0, n0, lane, at(sm.a, WS), at_t(sm.w, WS));
 #pragma unroll
       for (int j = 0; j < NJ1; ++j)
 #pragma unroll
@@ -407,7 +441,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   for (int r = 0; r < NR2; ++r) {
     zero(acc2[r]);
     const int p = warp + r * (NT / 32);
-    if (p < NP2) gemm<2>(acc2[r], 16 * (p / (KT / 2)), 16 * (p % (KT / 2)), HID, lane, at(sm.h, HS), at(sm.w, WS));
+    if (p < NP2) gemm_k<2, HID>(acc2[r], 16 * (p / (KT / 2)), 16 * (p % (KT / 2)), lane, at(sm.h, HS), at(sm.w, WS));
   }
   __syncthreads();      // every read of W is done
   stamp(prof, 10, tid);
@@ -428,29 +462,34 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   }
   __syncthreads();
   stamp(prof, 11, tid);
-  // ---- GEMM 3 (DMMA): dW1_c[j][k] = sum_s dH[s][j] A[s][k], 4 x KT / 2 pairs of 16 x 8 tiles straight to the gradient row
-  //      (column pairs as 16-byte stores).  No barrier follows: a warp goes on to its conv-grad rows while others still run
-  //      their DMMA and stores --------------------------------------------------------------------------------------------
-  {
-    constexpr int NP3 = (HID / 16) * (KT / 2);
+  // ---- GEMM 3 (DMMA) on warps 12 .. 15, one per SM sub-partition: dW1_c[j][k] = sum_s dH[s][j] A[s][k].  Warp 12 + q owns
+  //      hidden rows 16q .. 16q+15 and all KT column tiles, KT / 2 at a time: that many independent DMMA chains share the dH
+  //      fragments.  Tiles go straight to the gradient row (column pairs as 16-byte stores).  Meanwhile warps 0 .. 11 run
+  //      their conv-grad rows, so the FP64 pipe of every sub-partition is busy while its tensor cores run GEMM 3; warps
+  //      12 .. 15 follow with their own conv-grad rows (warp 15: the bias sums).  No barrier on either side ----------------
+  constexpr int W3 = NT / 32 - HID / 16, NJ3 = KT / 2;   // first GEMM 3 warp; column tiles per pass
+  if (warp >= W3) {
+    const int m0 = 16 * (warp - W3);
 #pragma unroll 1
-    for (int p = warp; p < NP3; p += NT / 32) {
-      const int m0 = 16 * (p / (KT / 2)), n0 = 16 * (p % (KT / 2));
-      double acc[2][4];
+    for (int n0 = 0; n0 < 8 * KT; n0 += 8 * NJ3) {
+      double acc[NJ3][4];
       zero(acc);
-      gemm<2>(acc, m0, n0, MS, lane, at_t(sm.h, HS), at(sm.a, WS));
+      gemm_k<NJ3, MS>(acc, m0, n0, lane, at_t(sm.h, HS), at(sm.a, WS));
 #pragma unroll
-      for (int jt = 0; jt < 2; ++jt)
+      for (int jt = 0; jt < NJ3; ++jt)
 #pragma unroll
         for (int i = 0; i < 4; i += 2) {
           const int j = frow(m0, lane, i), k = fcol(n0 + 8 * jt, lane, i);   // k even: k and k + 1 share a channel run
           if (k < KC) {
+            // __stcg keeps the pair one 16-byte store: a plain double2 assignment was split into two 8-byte stores,
+            // which doubled the partial-sector writes of the 55 KB dW1 slice
             const int ch = k / CELLS, cell = k - ch * CELLS;
-            *reinterpret_cast<double2*>(gp + a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell) =
-                make_double2(acc[jt][i], acc[jt][i + 1]);
+            __stcg(reinterpret_cast<double2*>(gp + a.off_w1 + (size_t)j * FC1_IN + ch * NPOOL + CELLS * c + cell),
+                   make_double2(acc[jt][i], acc[jt][i + 1]));
           }
         }
     }
+    stamp(prof, 12, tid - W3 * 32);      // lane 0 of warp 12: its GEMM 3 stores are issued
   }
   // ---- conv grads without gathers: warps 3ky .. 3ky+2 own tap row ky of all three channels.  A thread walks whole pooled
   //      rows (sample s, pooled row pr, px = 0 .. 11) with columns 2px .. 2px+5 of patch rows 2pr+ky and 2pr+ky+1 in
@@ -529,7 +568,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     // this CTA's share goes straight into rank 0's collection buffer (its h_loc rows, dead since barrier #2)
     st_dsmem(map_to(sm.h_loc + c * 80 + tid, 0u), v);
   }
-  stamp(prof, 12, tid);
+  stamp(prof, 13, tid);
   cluster_sync();                                        // #3: all four conv-gradient shares are in rank 0's buffer
   if (c == 0 && tid < 78) {
     double v = 0.0;
@@ -537,7 +576,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     for (int r = 0; r < CL; ++r) v += sm.h_loc[r * 80 + tid];
     gp[tid < 75 ? a.off_wc + tid : a.off_bc + (tid - 75)] = v;
   }
-  stamp(prof, 13, tid);
+  stamp(prof, 14, tid);
 }
 
 template <int MS>
