@@ -134,60 +134,17 @@ class FusedMnist:
         self.calls.copy_(torch.as_tensor(self.pr.calls[pl.lo: pl.lo + pl.L].astype(np.int32)))
 
     # ---- host-fed batches (end-to-end input pipeline) -----------------------
-    def enable_host_feed(self, steps_per_round: int, nslots: int = 4, threads: int = 4, mode: str = "gpu_pull"):
-        """Switch to the host-fed input pipeline: the dataset stays in (pinned) host memory and
-        every round's minibatches cross PCIe; each round also reads its losses back (D2H).
-        This is the path ``bench.py`` times end to end; the default keeps shards in HBM.
+    def enable_host_feed(self, steps_per_round: int, source: str):
+        """Switch to a staged input pipeline: a staging kernel on a side stream gathers the *next* round's rows into
+        one of two compact device staging sets (in-kernel sampler) while the current round computes, and the training
+        kernel reads the staged batch by direct indexing.
 
-        ``mode="gpu_pull"``: a staging kernel on a side stream pulls the *next* round's rows
-        straight out of the pinned host dataset (device-initiated H2D, in-kernel sampler) while
-        the current round computes — no CPU work per round.
-        ``mode="cpu_loader"``: native loader threads (csrc/runtime.cpp) assemble rounds into a
-        ring of pinned slots and the runner issues one ``cudaMemcpyAsync`` per round."""
-        if mode in ("gpu_pull", "staged"):
-            return self._enable_gpu_pull(steps_per_round, source="device" if mode == "staged" else "host")
-        pr, dev = self.pr, self.pr.device
-        P, L, B = int(steps_per_round), self.L, self.B
-        xb = 1 if self.x_is_u8 else 4
-        self.host_x = self.x.cpu().contiguous()
-        self.host_y = self.y.cpu().contiguous()
-        kw = dict(pin_memory=True)
-        self.x_pin = torch.empty(nslots, P, L, B, 784, dtype=self.x.dtype, **kw)
-        self.y_pin = torch.empty(nslots, P, L, B, dtype=torch.int64, **kw)
-        self.bs_pin = torch.empty(nslots, P, L, dtype=torch.int32, **kw)
-        # two device staging sets: the H2D copy of round r+1 overlaps the kernels of round r
-        self.x_stage = torch.zeros(2, P, L, B, 784, dtype=self.x.dtype, device=dev)
-        self.y_stage = torch.zeros(2, P, L, B, dtype=torch.int64, device=dev)
-        self.bs_stage = torch.zeros(2, P, L, dtype=torch.int32, device=dev)
-        self.loss_host = torch.zeros(L, self.S, dtype=torch.float32, **kw)
-        self.direct_ops = []
-        for b in range(2):
-            ops = []
-            for p in range(P):
-                d = dict(self.base)
-                d.update(direct=1, x=self.x_stage[b, p].data_ptr(), y=self.y_stage[b, p].data_ptr(),
-                         direct_bs=self.bs_stage[b, p].data_ptr())
-                ops.append(self.ext.MnistOp(d))
-            self.direct_ops.append(ops)
-        pl = pr.placement
-        calls0 = [int(c) for c in pr.calls[pl.lo: pl.lo + pl.L]]
-        self.loader = self.ext.HostBatchLoader(
-            self.host_x.data_ptr(), self.host_y.data_ptr(), 784 * xb,
-            [int(o) for o in pr.shards.offsets[:-1]], [int(m) for m in pr.shards.sizes], calls0,
-            B, P, pr.seed, pl.lo,
-            [self.x_pin[s].data_ptr() for s in range(nslots)],
-            [self.y_pin[s].data_ptr() for s in range(nslots)],
-            [self.bs_pin[s].data_ptr() for s in range(nslots)], threads)
-        self.host_feed = dict(P=P, nslots=nslots, mode="cpu_loader",
-                              h2d_bytes=P * L * B * (784 * xb + 8) + P * L * 4,
-                              d2h_bytes=L * self.S * 4)
-        return self.host_feed
-
-    def _enable_gpu_pull(self, steps_per_round: int, source: str = "host"):
-        """``source="host"``: rows come out of the pinned host copy of the dataset (PCIe).  ``source="device"``
-        (``input_pipeline: staged``): the same staging kernel gathers the next round's rows from the HBM-resident
-        shards into the compact staging set, so the training kernel never runs the sampler chain or a random HBM
-        gather on its critical path."""
+        ``source="host"`` (``input_pipeline: host``, what ``bench.py`` times end to end): the dataset stays in pinned
+        host memory and the staging kernel pulls the rows over PCIe (device-initiated H2D, no CPU work per round); the
+        training kernel stores each step's losses straight into the pinned ``loss_host`` buffer.  ``source="device"``
+        (``input_pipeline: staged``): the rows come from the HBM-resident shards, so the training kernel never runs the
+        sampler chain or a random HBM gather on its critical path."""
+        assert source in ("host", "device"), source
         pr, dev = self.pr, self.pr.device
         P, L, B = int(steps_per_round), self.L, self.B
         xb = 1 if self.x_is_u8 else 4
@@ -200,11 +157,9 @@ class FusedMnist:
         self.y_stage = torch.zeros(2, P, L, B, dtype=torch.int64, device=dev)
         self.bs_stage = torch.zeros(2, P, L, dtype=torch.int32, device=dev)
         self.loss_host = torch.zeros(L, self.S, dtype=torch.float32, pin_memory=True)
-        # result read-back: "mirror" = the training kernel stores each step's losses straight into this pinned host
-        # buffer over PCIe (no copy node on the round's critical path); "memcpy" = a D2H copy node per round
-        self.loss_mode = str(pr.conf.get("host_loss", os.environ.get("NNDT_HOST_LOSS", "mirror")))
-        if source == "device":
-            self.loss_mode = "none"          # nothing crosses PCIe in the staged-resident pipeline
+        # the training kernel stores each step's losses straight into this pinned host buffer over PCIe (no copy node on
+        # the round's critical path); nothing crosses PCIe in the staged-resident pipeline
+        self.loss_mode = "mirror" if source == "host" else "none"
         pl = pr.placement
         self.calls0 = torch.as_tensor(pr.calls[pl.lo: pl.lo + pl.L].astype(np.int32), device=dev)
         self.stage_round = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -233,30 +188,12 @@ class FusedMnist:
                 shard_off=self.shard_off.data_ptr(), shard_len=self.shard_len.data_ptr(),
                 calls0=self.calls0.data_ptr(), stage_round=self.stage_round.data_ptr(),
                 done_ctr=self.stage_done.data_ptr(), max_blocks=gather_blocks)))
+        # bench.py reads loader, loss_mode, loss_host and host_feed's mode / h2d_bytes / d2h_bytes for its e2e record
         self.loader = None
-        self.host_feed = dict(P=P, nslots=2, mode="gpu_pull", source=source,
+        self.host_feed = dict(P=P, mode="gpu_pull", source=source,
                               h2d_bytes=P * L * B * (784 * xb + 8) if source == "host" else 0,
                               d2h_bytes=L * self.S * 4 if source == "host" else 0)
         return self.host_feed
-
-    def make_runner(self, graphs, nslots):
-        """Native per-round driver (csrc/runtime.cpp: HostFedRunner) over the two captured round graphs."""
-        self._graphs = graphs
-        stream = torch.cuda.current_stream(self.pr.device).cuda_stream
-        self.runner = self.ext.HostFedRunner(
-            self.loader, [g.raw_cuda_graph_exec() for g in graphs], stream,
-            [self.x_pin[s].data_ptr() for s in range(nslots)], [self.y_pin[s].data_ptr() for s in range(nslots)],
-            [self.bs_pin[s].data_ptr() for s in range(nslots)],
-            [self.x_stage[b].data_ptr() for b in range(2)], [self.y_stage[b].data_ptr() for b in range(2)],
-            [self.bs_stage[b].data_ptr() for b in range(2)],
-            self.x_pin[0].numel() * self.x_pin.element_size(), self.y_pin[0].numel() * 8, self.bs_pin[0].numel() * 4)
-        return self.runner
-
-    def loss_readback(self):
-        """Enqueue the D2H read of the round's per-node losses (nothing to enqueue when the kernel mirrors them
-        into the pinned host buffer itself)."""
-        if getattr(self, "loss_mode", "memcpy") == "memcpy":
-            self.loss_host.copy_(self.loss_part, non_blocking=True)
 
     # ---- validation ---------------------------------------------------------
     def _setup_eval(self):

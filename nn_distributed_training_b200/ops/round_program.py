@@ -111,13 +111,9 @@ class RoundProgram:
                     self._enable_pipeline(pipeline)
 
     def _enable_pipeline(self, pipeline: str):
-        pr = self.pr
-        pr.fused.enable_host_feed(self.dpr, nslots=int(pr.conf.get("host_slots", 4)),
-                                  threads=int(pr.conf.get("host_threads", 4)),
-                                  mode="staged" if pipeline == "staged" else pr.conf.get("host_gather", "gpu_pull"))
+        self.pr.fused.enable_host_feed(self.dpr, source="device" if pipeline == "staged" else "host")
         self.host_mode = True
         self.pipeline = pipeline
-        self._runner = None
         self._stage_set = 0
         self._pull_graphs: Dict = {}
         self._pull_parity = 0
@@ -128,7 +124,7 @@ class RoundProgram:
         """Kernel launches of one communication round (the staging kernel of the host-fed / staged pipelines
         included)."""
         n = 1 if self.eng.sum_mode else 0
-        if self.host_mode and self.pr.fused.host_feed["mode"] == "gpu_pull":
+        if self.host_mode:
             n += 1
         return n + (2 * self.opt.pits if self.opt.alg_name == "dinno" else 3)
 
@@ -159,7 +155,8 @@ class RoundProgram:
     def _capture_pull_graph(self, R: int, parity: int):
         """``R`` host-fed rounds as ONE graph with two branches: while round i computes on the capture stream,
         the staging kernel pulls round i+1's rows out of pinned host memory on a forked stream (device-initiated
-        H2D over PCIe); every round ends with the D2H read of its losses.  No CPU work per round at all."""
+        H2D over PCIe); the training kernel stores every step's losses into pinned host memory itself.  No CPU work
+        per round at all."""
         fz = self.pr.fused
         if self._side is None:
             self._side = torch.cuda.Stream(device=self.pr.device)
@@ -176,7 +173,6 @@ class RoundProgram:
                     fz.gather_ops[b ^ 1].launch()
                 self._stage_set = b
                 _round_ops(self.opt, self.eng, self.grads)
-                fz.loss_readback()
                 main.wait_stream(side)     # round i+1 consumes what was just staged (also joins the fork)
         return g
 
@@ -203,28 +199,6 @@ class RoundProgram:
                 self._pull_parity = parity
                 self._count(r)
 
-    def _run_host_fed(self, rounds: int):
-        """Host-fed rounds.  ``gpu_pull`` (default): multi-round graphs with the staging kernel forked inside
-        (``_capture_pull_graph``).  ``cpu_loader``: the native runner issues, per round, the H2D copy of that
-        round's inputs, the captured round graph (kernels + D2H loss read) and the slot hand-back to the loader
-        threads."""
-        fz = self.pr.fused
-        if fz.host_feed["mode"] == "gpu_pull":
-            return self._run_pull_graphs(rounds)
-        if self._runner is None:
-            graphs = []
-            for b in range(2):
-                self._stage_set = b
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    _round_ops(self.opt, self.eng, self.grads)
-                    fz.loss_readback()
-                graphs.append(g)
-            self._runner = fz.make_runner(graphs, fz.host_feed["nslots"])
-        # graphs were captured on torch's capture stream but are launched on the current stream
-        self._runner.run(rounds)
-        self._count(rounds)
-
     def _resident_graph(self, r: int):
         g = self._graphs.get(r)
         if g is None:
@@ -246,8 +220,7 @@ class RoundProgram:
         if not self.capturable:
             return
         if self.host_mode:
-            if self.pr.fused.host_feed["mode"] == "gpu_pull":
-                self._run_pull_graphs(rounds, capture_only=True)
+            self._run_pull_graphs(rounds, capture_only=True)
             return
         left = rounds
         while left > 0:
@@ -261,7 +234,7 @@ class RoundProgram:
             raise RuntimeError(f"rounds {self.opt.k}..{self.opt.k + rounds - 1} run past the schedule horizon of "
                                f"{self.eng.horizon} rounds")
         if self.host_mode:
-            return self._run_host_fed(rounds)
+            return self._run_pull_graphs(rounds)
         left = rounds
         while left > 0:
             r = min(left, MAX_ROUNDS_PER_GRAPH)

@@ -79,8 +79,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
 # extension keys of a problem config (absent from the reference's schema) and their legal values
 PROBLEM_CHOICES = {
     "input_pipeline": ("auto", "resident", "staged", "host"),
-    "host_gather": ("gpu_pull", "cpu_loader"),
-    "host_loss": ("mirror", "memcpy"),
+    "host_gather": ("gpu_pull",),
+    "host_loss": ("mirror",),
 }
 
 

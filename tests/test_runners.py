@@ -51,10 +51,15 @@ def test_config_errors_are_explicit():
             "metrics_config": {"evaluate_frequency": 1},
             "optimizer_config": {"alg_name": "dsgd", "alpha0": 0.1, "mu": 0.0, "outer_iterations": 2}}
     assert validate_problem(dict(base, input_pipeline="staged", samples_per_cta=5), "p", "mnist")["input_pipeline"] == "staged"
+    validate_problem(dict(base, input_pipeline="host", host_gather="gpu_pull", host_loss="mirror"), "p", "mnist")
     with pytest.raises(ConfigError, match="input_pipeline"):
         validate_problem(dict(base, input_pipeline="disk"), "p", "mnist")
     with pytest.raises(ConfigError, match="samples_per_cta"):
         validate_problem(dict(base, samples_per_cta=12), "p", "mnist")
+    with pytest.raises(ConfigError, match="host_gather"):
+        validate_problem(dict(base, host_gather="cpu_loader"), "p", "mnist")
+    with pytest.raises(ConfigError, match="host_loss"):
+        validate_problem(dict(base, host_loss="memcpy"), "p", "mnist")
     with pytest.raises(ConfigError, match="fault_injection"):
         validate_problem(dict(base, fault_injection={"link_drop_prob": 1.5}), "p", "mnist")
 
