@@ -2,13 +2,15 @@
 (reference: centralized/*.ipynb — the 0.985 MNIST accuracy and the 2.34 online-density validation
 loss drawn as reference lines in its figures, BASELINE.md).
 
-    python -m nn_distributed_training_b200.experiments.centralized mnist <config.yaml>
-    python -m nn_distributed_training_b200.experiments.centralized density <config.yaml>
+    python -m nn_distributed_training_b200.experiments.centralized mnist <config.yaml> [--backend torch|fused]
+    python -m nn_distributed_training_b200.experiments.centralized density <config.yaml> [--backend torch|fused]
+
+``--backend fused`` trains on the sm_90a kernels (ops/local_train.py); its batches come from the in-kernel sampler
+instead of ``torch.randperm``.
 """
 from __future__ import annotations
 
-import os
-import sys
+import argparse
 
 import numpy as np
 import torch
@@ -18,11 +20,19 @@ from . import density_common as dc
 from ..data.mnist import load_mnist
 from ..data.shards import Shard
 from ..models import FourierNet, MNISTConvNet
+from ..ops import local_train
 from ..utils.config import load_experiment
 
 
 def train_centralized(model, loss, train: Shard, val: Shard, device, epochs=6, lr=0.005, batch=100, val_batch=128,
-                      squeeze=False, verbose=True):
+                      squeeze=False, verbose=True, backend="torch", seed=0):
+    """Adam on the union shard, evaluated after every epoch; ``backend``: torch (autograd) | fused (sm_90a kernels,
+    ``ValueError`` when they cannot run this model / device)."""
+    if backend not in local_train.BACKENDS:
+        raise ValueError(f"backend must be one of {'|'.join(local_train.BACKENDS)} (got {backend!r})")
+    if backend == "fused":
+        return local_train.centralized(model, loss, train, val, device, epochs, lr, batch, val_batch, squeeze,
+                                       verbose=verbose, seed=seed)
     model = model.to(device)
     dtype = next(model.parameters()).dtype
     opt = torch.optim.Adam(model.parameters(), lr=lr)
@@ -52,7 +62,7 @@ def train_centralized(model, loss, train: Shard, val: Shard, device, epochs=6, l
     return hist
 
 
-def centralized_mnist(yaml_pth):
+def centralized_mnist(yaml_pth, backend="torch"):
     conf = load_experiment(yaml_pth, "mnist")["experiment"]
     ctx = common.make_context(conf)
     train, _ = load_mnist(conf["data_dir"], True)
@@ -61,10 +71,10 @@ def centralized_mnist(yaml_pth):
     solo = conf["individual_training"]
     return train_centralized(MNISTConvNet(m["num_filters"], m["kernel_size"], m["linear_width"]), common.make_loss(conf["loss"]),
                              train, val, ctx.device, epochs=solo["epochs"], lr=solo["lr"], batch=solo["train_batch_size"],
-                             val_batch=solo["val_batch_size"])
+                             val_batch=solo["val_batch_size"], backend=backend, seed=int(conf.get("seed", 0)))
 
 
-def centralized_density(yaml_pth, online=True):
+def centralized_density(yaml_pth, online=True, backend="torch"):
     from ..floorplans.lidar import RandomPoseLidarDataset, TrajectoryLidarDataset
     conf = load_experiment(yaml_pth, "online_density" if online else "density")["experiment"]
     ctx = common.make_context(conf)
@@ -78,12 +88,20 @@ def centralized_density(yaml_pth, online=True):
     solo = conf["individual_training"]
     model = FourierNet(conf["model"]["shape"], scale=conf["model"]["scale"])
     return train_centralized(model, common.make_loss(conf["loss"]), train, val, ctx.device, epochs=solo["epochs"], lr=solo["lr"],
-                             batch=solo["train_batch_size"], val_batch=solo["val_batch_size"], squeeze=True)
+                             batch=solo["train_batch_size"], val_batch=solo["val_batch_size"], squeeze=True,
+                             backend=backend, seed=int(conf.get("seed", 0)))
+
+
+def main(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.splitlines()[0])
+    ap.add_argument("kind", choices=("mnist", "density", "offline_density"))
+    ap.add_argument("config")
+    ap.add_argument("--backend", choices=local_train.BACKENDS, default="torch")
+    args = ap.parse_args(argv)
+    if args.kind == "mnist":
+        return centralized_mnist(args.config, backend=args.backend)
+    return centralized_density(args.config, online=(args.kind != "offline_density"), backend=args.backend)
 
 
 if __name__ == "__main__":
-    kind, path = sys.argv[1], sys.argv[2]
-    if kind == "mnist":
-        centralized_mnist(path)
-    else:
-        centralized_density(path, online=(kind != "offline_density"))
+    main()

@@ -1,6 +1,7 @@
 """Shared helpers of the lidar density runners."""
 from __future__ import annotations
 
+import copy
 import glob
 import os
 
@@ -61,6 +62,14 @@ def mesh_inputs(val_set, device, dtype):
     X, Y = np.meshgrid(val_set.lidar.xs, val_set.lidar.ys)
     mesh = np.hstack((X[::8, ::8].reshape(-1, 1), Y[::8, ::8].reshape(-1, 1)))
     return torch.as_tensor(mesh, dtype=dtype, device=device)
+
+
+def solo_results(base_model, loss, train_sets, val_set, device, conf, seed=0):
+    """``{node: train_solo result}`` of every node, on the backend ``conf['backend']`` names (torch | fused)."""
+    if conf["backend"] == "fused":
+        from ..ops import local_train
+        return local_train.solo_density(base_model, loss, train_sets, val_set, device, conf, seed=seed)
+    return {i: train_solo(copy.deepcopy(base_model), loss, s, val_set, device, conf) for i, s in enumerate(train_sets)}
 
 
 def train_solo(model, loss, train_set, val_set, device, conf):

@@ -1,7 +1,6 @@
 """Offline lidar density mapping runner (reference: experiments/dist_dense_ex.py)."""
 from __future__ import annotations
 
-import copy
 import os
 import sys
 
@@ -61,9 +60,9 @@ def experiment(yaml_pth):
     solo_confs = exp_conf["individual_training"]
     if solo_confs["train_solo"] and ctx.is_main:
         print("Performing individual training ...")
-        solo = {}
+        solo = dc.solo_results(base_model, base_loss, train_subsets[:N], val_set, ctx.device, solo_confs,
+                               seed=int(exp_conf.get("seed", 0)))
         for i in range(N):
-            solo[i] = dc.train_solo(copy.deepcopy(base_model), base_loss, train_subsets[i], val_set, ctx.device, solo_confs)
             if solo_confs["verbose"]:
                 print("Node {} - Validation loss = {:.4f}".format(i, solo[i]["validation_loss"]))
         if exp_conf["writeout"]:

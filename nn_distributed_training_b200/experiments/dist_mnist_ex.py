@@ -14,6 +14,7 @@ import torch
 from . import common
 from ..data.mnist import load_mnist
 from ..models import MNISTConvNet
+from ..ops import local_train
 from ..problems import DistMNISTProblem
 from ..utils import graph_generation
 from ..utils.config import load_experiment
@@ -97,8 +98,13 @@ def experiment(yaml_pth):
     if solo_confs["train_solo"] and ctx.is_main:
         print("Performing individual training ...")
         solo_results = {}
+        if solo_confs["backend"] == "fused":
+            solo_results = local_train.solo_mnist(base_model, base_loss, train_subsets, val, ctx.device, solo_confs,
+                                                  seed=int(exp_conf.get("seed", 0)))
         for i in range(N):
-            solo_results[i] = train_solo(copy.deepcopy(base_model), base_loss, train_subsets[i], val, ctx.device, solo_confs)
+            if solo_confs["backend"] == "torch":
+                solo_results[i] = train_solo(copy.deepcopy(base_model), base_loss, train_subsets[i], val, ctx.device,
+                                             solo_confs)
             if solo_confs["verbose"]:
                 print("Node {} - Validation Acc = {:.4f}".format(i, solo_results[i]["validation_accuracy"]))
         if exp_conf["writeout"]:

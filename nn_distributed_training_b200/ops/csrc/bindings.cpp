@@ -138,6 +138,23 @@ struct ConsensusOp {
   void dsgt_track() { check(consensus::launch_dsgt_track<T>(gt, cur_stream()), "dsgt_track"); }
 };
 
+// local optimizer step of non-communicating nodes (solo / centralized baselines)
+template <typename T>
+struct LocalStepOp {
+  consensus::LocalArgs<T> a{};
+  explicit LocalStepOp(const py::dict& d) {
+    a.c = common_from<T>(d);
+    if (a.c.calls == nullptr) throw std::runtime_error("local_step needs the per-node step counter `calls`");
+    a.m = ptr<T>(d, "m"); a.v = ptr<T>(d, "v");
+    a.budget = ptr<const int>(d, "budget"); a.arrive = ptr<unsigned int>(d, "arrive");
+    a.lr = (T)getf(d, "local_lr"); a.opt = geti(d, "opt", 1);
+    if (a.budget == nullptr || a.arrive == nullptr) throw std::runtime_error("local_step needs `budget` and `arrive`");
+    if (a.opt != consensus::kSGD && (a.m == nullptr || a.v == nullptr))
+      throw std::runtime_error("local_step with Adam / AdamW needs the moment rows `m` and `v`");
+  }
+  void step() { check(consensus::launch_local_step<T>(a, cur_stream()), "local_step"); }
+};
+
 template <typename T>
 static void bind_consensus(py::module& m, const char* name) {
   py::class_<ConsensusOp<T>>(m, name)
@@ -193,6 +210,8 @@ PYBIND11_MODULE(_C, m) {
   m.def("spin", [](long long cycles) { check(consensus::launch_spin(cycles, cur_stream()), "spin"); });
   bind_consensus<float>(m, "ConsensusOpF32");
   bind_consensus<double>(m, "ConsensusOpF64");
+  py::class_<LocalStepOp<float>>(m, "LocalStepOpF32").def(py::init<const py::dict&>()).def("step", &LocalStepOp<float>::step);
+  py::class_<LocalStepOp<double>>(m, "LocalStepOpF64").def(py::init<const py::dict&>()).def("step", &LocalStepOp<double>::step);
   bind_mlp(m);
   bind_rl(m);
   bind_runtime(m);

@@ -148,6 +148,50 @@ __global__ void __launch_bounds__(THREADS) dinno_update_kernel(const DinnoArgs<T
   if (last) { tag_published(c, l, ri.k); finish_round(c, ri.k); }
 }
 
+// ------------------------------------------------------------- local step ----
+// One optimizer step per node that has not used up its budget; a node at its budget is left bitwise untouched (theta,
+// moments, calls).  The forward/backward kernel before it has already run for every node, so a finished node's
+// gradient is computed and dropped here.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) local_step_kernel(const LocalArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = blockIdx.y;
+  // calls / budget / theta / moments were last written two launches back: readable before the dependency wait
+  const int call = c.calls[l];
+  if (call >= a.budget[l]) {
+    pdl_wait();
+    pdl_launch_dependents();
+    return;
+  }
+  const OptCoef<T> q = opt_coef(a.opt, a.lr, call + 1);
+  const size_t row = (size_t)l * c.n_pad;
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    Pack<T> m, v;
+    if (a.opt != kSGD) {
+      m = ldv(a.m + row + i);
+      v = ldv(a.v + row + i);
+    }
+    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    opt_apply(q, th, m, v, g);
+    if (a.opt != kSGD) {
+      stv(a.m + row + i, m);
+      stv(a.v + row + i, v);
+    }
+    stv(c.theta + row + i, th);
+  }
+  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
+  // the last CTA of node l to arrive advances its counter: every CTA has read `call` by then
+  __syncthreads();
+  if (threadIdx.x == 0 && atomicAdd(a.arrive + l, 1u) == gridDim.x - 1) {
+    a.arrive[l] = 0;
+    c.calls[l] = call + 1;
+  }
+}
+
 // ------------------------------------------------------------------- DSGD ----
 template <typename T>
 __global__ void __launch_bounds__(THREADS) dsgd_mix_kernel(const Common<T> c) {
@@ -493,6 +537,9 @@ template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStrea
 template <typename T> cudaError_t launch_dinno_update(const DinnoArgs<T>& a, cudaStream_t st) {
   return NNDT_BY_S(a.c.S, dinno_update_kernel, a, a.c);
 }
+template <typename T> cudaError_t launch_local_step(const LocalArgs<T>& a, cudaStream_t st) {
+  return NNDT_BY_S(a.c.S, local_step_kernel, a, a.c);
+}
 template <typename T> cudaError_t launch_dsgd_mix(const Common<T>& c, cudaStream_t st) {
   return launch_pdl(dsgd_mix_kernel<T>, grid_for(c, dsgd_mix_kernel<T>), dim3(THREADS), 0, st, c);
 }
@@ -517,6 +564,7 @@ template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaSt
   template cudaError_t launch_local_sum<T>(const Common<T>&, cudaStream_t);           \
   template cudaError_t launch_consensus_metric<T>(const int64_t*, int, int, int, int, double*, double*, double*, cudaStream_t); \
   template cudaError_t launch_dinno_update<T>(const DinnoArgs<T>&, cudaStream_t);     \
+  template cudaError_t launch_local_step<T>(const LocalArgs<T>&, cudaStream_t);       \
   template cudaError_t launch_dsgd_mix<T>(const Common<T>&, cudaStream_t);            \
   template cudaError_t launch_dsgd_step<T>(const Common<T>&, cudaStream_t);           \
   template cudaError_t launch_dsgt_init<T>(const DsgtArgs<T>&, cudaStream_t);         \

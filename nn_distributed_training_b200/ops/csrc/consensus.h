@@ -85,6 +85,20 @@ struct DsgtArgs {
   int own_tracker;
 };
 
+// Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient
+// partials are summed and one torch.optim SGD / Adam / AdamW step is applied, while c.calls[l] < budget[l].
+// Uses c.L, c.n_pad, c.S, c.theta, c.grad_part and c.calls (the node's step counter, required).
+template <typename T>
+struct LocalArgs {
+  Common<T> c;
+  T* m; T* v;                      // [L, n_pad] moments (nullptr with SGD)
+  const int* budget;               // [L] steps each node takes in all
+  unsigned int* arrive;            // [L] CTA arrival counters: calls[l] advances once every CTA of node l has read it
+  T lr;
+  int opt;
+};
+
+template <typename T> cudaError_t launch_local_step(const LocalArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dinno_update(const DinnoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dsgd_mix(const Common<T>& c, cudaStream_t st);
 template <typename T> cudaError_t launch_dsgd_step(const Common<T>& c, cudaStream_t st);

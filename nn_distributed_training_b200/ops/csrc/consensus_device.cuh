@@ -231,32 +231,27 @@ NNDT_DEVINL void step_bookkeeping(const Common<T>& c, int l) {
   }
 }
 
-// ---- DiNNO arithmetic on one vector (optimizers/dinno.py:74-91): augmented-Lagrangian gradient + optimizer step ----
+// ---- torch.optim step on one vector: SGD, Adam (betas 0.9 / 0.999, eps 1e-8), AdamW (+ weight decay 0.01) ----
 template <typename T>
-struct DinnoCoef {
-  T rho, lr, step_size, bc2s;
-  int deg, opt;
+struct OptCoef {
+  T lr, step_size, bc2s;
+  int opt;
 };
+// coefficients of optimizer step t (1-based, the torch.optim `step` count)
 template <typename T>
-NNDT_DEVINL DinnoCoef<T> dinno_coef(const DinnoArgs<T>& a, int k, int step, int deg) {
-  DinnoCoef<T> q;
-  q.rho = a.c.rho[k]; q.lr = a.c.lr[k];
-  const int t = a.persistent ? k * a.pits + step + 1 : step + 1;
+NNDT_DEVINL OptCoef<T> opt_coef(int opt, T lr, int t) {
+  OptCoef<T> q;
+  q.lr = lr;
   const T bc1 = (T)1 - pow((T)0.9, (T)t);
   q.bc2s = sqrt((T)1 - pow((T)0.999, (T)t));
   q.step_size = q.lr / bc1;
-  q.deg = deg; q.opt = a.opt;
+  q.opt = opt;
   return q;
 }
 template <typename T>
-NNDT_DEVINL void dinno_apply(const DinnoCoef<T>& q, Pack<T>& th, const Pack<T>& thk, const Pack<T>& dl, const Pack<T>& du,
-                             Pack<T>& m, Pack<T>& v, const Pack<T>& gl) {
+NNDT_DEVINL void opt_apply(const OptCoef<T>& q, Pack<T>& th, Pack<T>& m, Pack<T>& v, const Pack<T>& g) {
   constexpr int N = Vec<T>::N;
   const T b1 = (T)0.9, b2 = (T)0.999, eps = (T)1e-8, wd = (T)1e-2;
-  Pack<T> g;
-#pragma unroll
-  for (int u = 0; u < N; ++u)
-    g.v[u] = gl.v[u] + du.v[u] + (T)2 * q.rho * (T)q.deg * (th.v[u] - thk.v[u]) - q.rho * dl.v[u];
   if (q.opt == kSGD) {
 #pragma unroll
     for (int u = 0; u < N; ++u) th.v[u] -= q.lr * g.v[u];
@@ -269,6 +264,33 @@ NNDT_DEVINL void dinno_apply(const DinnoCoef<T>& q, Pack<T>& th, const Pack<T>& 
       th.v[u] -= q.step_size * m.v[u] / (sqrt(v.v[u]) / q.bc2s + eps);
     }
   }
+}
+
+// ---- DiNNO arithmetic on one vector (optimizers/dinno.py:74-91): augmented-Lagrangian gradient + optimizer step ----
+template <typename T>
+struct DinnoCoef {
+  OptCoef<T> o;
+  T rho;
+  int deg;
+};
+template <typename T>
+NNDT_DEVINL DinnoCoef<T> dinno_coef(const DinnoArgs<T>& a, int k, int step, int deg) {
+  DinnoCoef<T> q;
+  q.rho = a.c.rho[k];
+  const int t = a.persistent ? k * a.pits + step + 1 : step + 1;
+  q.o = opt_coef(a.opt, a.c.lr[k], t);
+  q.deg = deg;
+  return q;
+}
+template <typename T>
+NNDT_DEVINL void dinno_apply(const DinnoCoef<T>& q, Pack<T>& th, const Pack<T>& thk, const Pack<T>& dl, const Pack<T>& du,
+                             Pack<T>& m, Pack<T>& v, const Pack<T>& gl) {
+  constexpr int N = Vec<T>::N;
+  Pack<T> g;
+#pragma unroll
+  for (int u = 0; u < N; ++u)
+    g.v[u] = gl.v[u] + du.v[u] + (T)2 * q.rho * (T)q.deg * (th.v[u] - thk.v[u]) - q.rho * dl.v[u];
+  opt_apply(q.o, th, m, v, g);
 }
 
 }  // namespace consensus

@@ -118,7 +118,9 @@ def validate_problem(conf: Dict[str, Any], path: str, kind: str) -> Dict[str, An
 
 
 SOLO_DEFAULT = {"train_solo": False, "optimizer": "adam", "lr": 0.005, "epochs": 1,
-                "train_batch_size": 100, "val_batch_size": 100, "verbose": True}
+                "train_batch_size": 100, "val_batch_size": 100, "verbose": True, "backend": "torch"}
+# torch: per-node autograd; fused: every node at once on the sm_90a kernels (ops/local_train.py)
+SOLO_BACKENDS = ("torch", "fused")
 
 
 def validate_experiment(conf: Dict[str, Any], kind: str) -> Dict[str, Any]:
@@ -133,6 +135,9 @@ def validate_experiment(conf: Dict[str, Any], kind: str) -> Dict[str, Any]:
     if kind in ("mnist", "density", "online_density"):
         exp["individual_training"] = _fill(exp.get("individual_training", {}), SOLO_DEFAULT,
                                            "experiment.individual_training")
+        if exp["individual_training"]["backend"] not in SOLO_BACKENDS:
+            raise ConfigError(f"experiment.individual_training.backend must be one of {'|'.join(SOLO_BACKENDS)} "
+                              f"(got {exp['individual_training']['backend']!r})")
     if kind == "mnist":
         exp = _fill(exp, {"data_dir": "../data/", "data_split_type": "random"}, "experiment")
         if exp["data_split_type"] not in ("random", "hetero"):
