@@ -13,6 +13,7 @@ from __future__ import annotations
 import math
 from typing import Optional, Tuple
 
+import numpy as np
 import torch
 
 ADAM_BETA1, ADAM_BETA2, ADAM_EPS = 0.9, 0.999, 1e-8
@@ -91,6 +92,19 @@ def dsgt_mix(theta_all: torch.Tensor, y_all: torch.Tensor, w_rows: torch.Tensor,
 def dsgt_track(y_all: torch.Tensor, w_rows: torch.Tensor, g_new: torch.Tensor, g_old: torch.Tensor) -> torch.Tensor:
     """``y_i <- sum_j W_ij y_j + g_i^{new} - g_i^{old}``."""
     return w_rows.to(y_all.dtype) @ y_all + g_new - g_old
+
+
+# ------------------------------------------------------ Exact Diffusion ----
+def ed_weights(W):
+    """``A = (I + W) / 2`` of a float64 Metropolis matrix: the combine weights of Exact Diffusion."""
+    return 0.5 * (np.eye(W.shape[0]) + W)
+
+
+def ed_step_(theta: torch.Tensor, psi: torch.Tensor, grad: torch.Tensor, alpha: float):
+    """``psi' = theta - alpha g``; ``theta <- psi' + (theta - psi)``; ``psi <- psi'``, on the mixed rows ``theta``."""
+    corr = theta - psi
+    psi.copy_(theta).add_(grad, alpha=-alpha)
+    theta.copy_(psi).add_(corr)
 
 
 # ------------------------------------------------------------- metrics ----

@@ -118,9 +118,11 @@ struct ConsensusOp {
   consensus::Common<T> c{};
   consensus::DinnoArgs<T> dn{};
   consensus::DsgtArgs<T> gt{};
+  consensus::EdArgs<T> ed{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c;
+    dn.c = c; gt.c = c; ed.c = c;
+    ed.psi = ptr<T>(d, "psi");
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
@@ -136,6 +138,11 @@ struct ConsensusOp {
   void dsgt_init() { check(consensus::launch_dsgt_init<T>(gt, cur_stream()), "dsgt_init"); }
   void dsgt_mix() { check(consensus::launch_dsgt_mix<T>(gt, cur_stream()), "dsgt_mix"); }
   void dsgt_track() { check(consensus::launch_dsgt_track<T>(gt, cur_stream()), "dsgt_track"); }
+  void ed_mix() { check(consensus::launch_ed_mix<T>(ed, cur_stream()), "ed_mix"); }
+  void ed_step() {
+    if (ed.psi == nullptr) throw std::runtime_error("ed_step needs the Exact Diffusion row `psi`");
+    check(consensus::launch_ed_step<T>(ed, cur_stream()), "ed_step");
+  }
 };
 
 // local optimizer step of non-communicating nodes (solo / centralized baselines)
@@ -165,7 +172,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dsgd_step", &ConsensusOp<T>::dsgd_step)
       .def("dsgt_init", &ConsensusOp<T>::dsgt_init)
       .def("dsgt_mix", &ConsensusOp<T>::dsgt_mix)
-      .def("dsgt_track", &ConsensusOp<T>::dsgt_track);
+      .def("dsgt_track", &ConsensusOp<T>::dsgt_track)
+      .def("ed_mix", &ConsensusOp<T>::ed_mix)
+      .def("ed_step", &ConsensusOp<T>::ed_step);
 }
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp

@@ -1,9 +1,10 @@
-// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT.
+// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
 //   optimizers/dsgd.py:37-46 / :55-58      -> dsgd_mix / dsgd_step
 //   optimizers/dsgt.py:58-75 / :87-103     -> dsgt_mix / dsgt_track
+// Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
 //
 // Every kernel is a single pass over the node's 16-byte vectorised parameter row: neighbor
 // rows are pulled straight from the (local or NVLink-peer) published buffers named by the
@@ -407,6 +408,70 @@ __global__ void __launch_bounds__(THREADS) dsgt_track_kernel(const DsgtArgs<T> a
   finish_round(c, ri.k);
 }
 
+// -------------------------------------------------------- Exact Diffusion ----
+// The pointer-table mix is dsgd_mix_kernel fed with the weights of A = (I + W) / 2.  On the complete graph A's rows
+// are (1/2) e_i + 1 / (2N), so the combine is (theta_i + S / N) / 2 with S the fp64 network sum.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) ed_sum_mix_kernel(const Common<T> c) {
+  pdl_wait();
+  pdl_launch_dependents();
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  begin_round(c, ri.gid, l, ri.k);
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    const DPack<N> sall = network_sum(c, ri.par, 0, i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] = (T)(0.5 * ((double)th.v[u] + sall.v[u] / (double)c.n_total));
+    stv(c.theta + row + i, th);
+  }
+}
+
+// adapt psi' = theta - alpha_k g, correct theta <- psi' + (theta - psi), psi <- psi'; theta is published.  Round 0
+// starts from psi = theta (the mixed row), so its step is plain DSGD.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) ed_step_kernel(const EdArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const bool init = ri.k == 0;
+  const size_t row = (size_t)l * c.n_pad;
+  // theta (written by the mix two launches back) and psi (the previous round's step) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> th = ldv(c.theta + row + i);
+    Pack<T> dc;
+    if (init) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) dc.v[u] = (T)0;
+    } else {
+      const Pack<T> ps = ldv(a.psi + row + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) dc.v[u] = th.v[u] - ps.v[u];
+    }
+    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> pn, tn;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      pn.v[u] = th.v[u] - alpha * g.v[u];
+      tn.v[u] = pn.v[u] + dc.v[u];
+    }
+    stv(a.psi + row + i, pn);
+    stv(c.theta + row + i, tn);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, tn);
+  }
+  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
+  step_bookkeeping(c, l);
+  tag_published(c, l, ri.k);
+  finish_round(c, ri.k);
+}
+
 // ------------------------------------------------------------ consensus metric ----
 NNDT_DEVINL double block_sum(double v) {
   __shared__ double red[THREADS / 32];
@@ -558,6 +623,13 @@ template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st) {
   return NNDT_BY_S(a.c.S, dsgt_track_kernel, a, a.c);
 }
+template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t st) {
+  return a.c.sum_mode ? launch_pdl(ed_sum_mix_kernel<T>, grid_for(a.c, ed_sum_mix_kernel<T>), dim3(THREADS), 0, st, a.c)
+                      : launch_pdl(dsgd_mix_kernel<T>, grid_for(a.c, dsgd_mix_kernel<T>), dim3(THREADS), 0, st, a.c);
+}
+template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st) {
+  return NNDT_BY_S(a.c.S, ed_step_kernel, a, a.c);
+}
 #undef NNDT_BY_S
 
 #define NNDT_INST(T)                                                                  \
@@ -569,7 +641,9 @@ template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaSt
   template cudaError_t launch_dsgd_step<T>(const Common<T>&, cudaStream_t);           \
   template cudaError_t launch_dsgt_init<T>(const DsgtArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_dsgt_mix<T>(const DsgtArgs<T>&, cudaStream_t);          \
-  template cudaError_t launch_dsgt_track<T>(const DsgtArgs<T>&, cudaStream_t);
+  template cudaError_t launch_dsgt_track<T>(const DsgtArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_ed_mix<T>(const EdArgs<T>&, cudaStream_t);              \
+  template cudaError_t launch_ed_step<T>(const EdArgs<T>&, cudaStream_t);
 NNDT_INST(float)
 NNDT_INST(double)
 

@@ -85,6 +85,14 @@ struct DsgtArgs {
   int own_tracker;
 };
 
+// Exact Diffusion (Yuan, Ying, Zhao, Sayed 2019): DSGD's single published channel plus one local row psi.  The mix is
+// DSGD's with the weights of A = (I + W) / 2 in the topology tables (complete-graph sum mode: (theta_i + S / N) / 2).
+template <typename T>
+struct EdArgs {
+  Common<T> c;
+  T* psi;                          // [L, n_pad] the adapt step of the previous round; set from theta in round 0
+};
+
 // Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient
 // partials are summed and one torch.optim SGD / Adam / AdamW step is applied, while c.calls[l] < budget[l].
 // Uses c.L, c.n_pad, c.S, c.theta, c.grad_part and c.calls (the node's step counter, required).
@@ -105,6 +113,8 @@ template <typename T> cudaError_t launch_dsgd_step(const Common<T>& c, cudaStrea
 template <typename T> cudaError_t launch_dsgt_init(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStream_t st);
 
 // All-rank barrier on the device (bench start alignment, metric quiescence): every rank stores `epoch` into its slot of

@@ -13,6 +13,7 @@ import numpy as np
 import torch
 
 from . import load_ext
+from .consensus_ref import ed_weights
 from ..parallel.symm import SymmetricBuffer
 from ..utils.graph_generation import Topology
 
@@ -37,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name == "dsgd":
+    elif opt.alg_name in ("dsgd", "exact_diffusion"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):
         alpha[:] = opt.alpha
@@ -103,13 +104,15 @@ class ConsensusEngine:
         deg = np.zeros((G, L), dtype=np.int32)
         nbr_rank = -np.ones((G, L, dmax), dtype=np.int32)
         for gi, t in enumerate(topos):
+            # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel
+            Wt = ed_weights(t.W) if opt.alg_name == "exact_diffusion" else t.W
             for l, g in enumerate(pl.local_nodes):
                 nb = t.neighbors_noself[g]
                 deg[gi, l] = len(nb)
-                self_w[gi, l] = t.W[g, g]
+                self_w[gi, l] = Wt[g, g]
                 for e, j in enumerate(nb):
                     r, lj = int(pl.node_rank[j]), int(pl.node_local[j])
-                    nbr_w[gi, l, e] = t.W[g, j]
+                    nbr_w[gi, l, e] = Wt[g, j]
                     if r != ctx.rank:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
@@ -235,6 +238,8 @@ class ConsensusEngine:
         if opt.alg_name == "dsgt":
             d.update(g_old=opt.g.data_ptr(), own_tracker=int(bool(getattr(opt, "own_tracker_step", False))),
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
+        if opt.alg_name == "exact_diffusion":
+            d.update(psi=opt.psi.data_ptr())
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d

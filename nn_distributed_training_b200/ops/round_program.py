@@ -4,6 +4,7 @@ A round is a short, fixed kernel sequence
     DiNNO:  [fwd/bwd, dinno_update(p)] x primal_iterations
     DSGD :  dsgd_mix, fwd/bwd, dsgd_step
     DSGT :  dsgt_mix, fwd/bwd, dsgt_track
+    Exact Diffusion:  ed_mix, fwd/bwd, ed_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -52,6 +53,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.dsgt_mix()
         grads(0)
         eng.op.dsgt_track()
+    elif alg == "exact_diffusion":
+        eng.op.ed_mix()
+        grads(0)
+        eng.op.ed_step()
     else:  # pragma: no cover
         raise NameError("Unknown distributed opt algorithm.")
 
@@ -255,7 +260,7 @@ class RoundProgram:
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name == "dsgd" and opt.k > 0:
+        if opt.alg_name in ("dsgd", "exact_diffusion") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
 
 

@@ -1,8 +1,9 @@
 from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgt import DSGT
+from .exact_diffusion import ExactDiffusion
 
-ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT}
+ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -15,7 +15,7 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgt")
+ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
 DENSITY_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "mesh_grid_density",
@@ -28,6 +28,7 @@ OPT_SCHEMA = {
               "profile": False},
     "dsgd": {"alpha0": REQUIRED, "mu": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
     "dsgt": {"alpha": REQUIRED, "init_grads": True, "outer_iterations": REQUIRED, "profile": False},
+    "exact_diffusion": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -71,6 +72,9 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
+    if alg == "exact_diffusion" and c.get("mixing_order", "jacobi") != "jacobi":
+        raise ConfigError(f"{path}.mixing_order: exact_diffusion runs the synchronous 'jacobi' order only "
+                          f"(got {c['mixing_order']!r})")
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c
