@@ -107,6 +107,128 @@ def ed_step_(theta: torch.Tensor, psi: torch.Tensor, grad: torch.Tensor, alpha: 
     theta.copy_(psi).add_(corr)
 
 
+# ------------------------------------------------------------ CHOCO-SGD ----
+# Code rows (the byte layout of csrc/consensus.h, the only other place it is written).  A row of n_pad elements is cut
+# into nb = n_pad / 32 blocks of 32; scales are in the arena dtype T:
+#   none: [n_pad] T                        v itself
+#   int8: [n_pad] int8, [nb] T scales      scale = max|v| / 127, code = clamp(rint(v / scale), -127, 127), dec = code scale
+#   sign: [nb] uint32 words, [nb] T        bit e % 32 of word e // 32 set when v_e >= 0; scale = sum|v| / n_live over the
+#                                          live elements, dec = +-scale on live elements and 0 on padding and holes
+# The arithmetic is the kernel's: divisions and the decode product are single IEEE operations, round half to even, and
+# the sign scale's sum runs in the kernel's order (elements of a lane in turn, then halving over the 32 / VEC lanes
+# of the block), so both paths produce the same bytes from the same v.
+CHOCO_COMPRESSORS = ("none", "int8", "sign")
+CHOCO_CODE = {"none": 0, "int8": 1, "sign": 2}
+CHOCO_BLOCK = 32
+CHOCO_VEC = {torch.float32: 4, torch.float64: 2}      # elements per thread in the kernels (16-byte vectors)
+
+
+def choco_code_bytes(compressor: str, n_pad: int, dtype: torch.dtype) -> int:
+    """Bytes of one code row."""
+    s = torch.empty((), dtype=dtype).element_size()
+    nb = n_pad // CHOCO_BLOCK
+    return {"none": n_pad * s, "int8": n_pad + nb * s, "sign": 4 * nb + nb * s}[compressor]
+
+
+def choco_live(layout) -> torch.Tensor:
+    """``[n_pad]`` bool: True on parameter elements, False on row padding and slot-alignment holes."""
+    live = torch.zeros(layout.n_pad, dtype=torch.bool)
+    for s in layout.slots:
+        live[s.offset: s.offset + s.numel] = True
+    return live
+
+
+def choco_live_words(live: torch.Tensor) -> torch.Tensor:
+    """The ``[n_pad / 32]`` bit mask the kernels read (bit e % 32 of word e // 32), as int32."""
+    bits = np.packbits(live.cpu().numpy().astype(np.uint8), bitorder="little")
+    return torch.from_numpy(bits.view(np.int32).copy())
+
+
+def _blocks(x: torch.Tensor) -> torch.Tensor:
+    return x.reshape(x.shape[:-1] + (x.shape[-1] // CHOCO_BLOCK, CHOCO_BLOCK))
+
+
+def choco_encode(v: torch.Tensor, compressor: str, live: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Code rows ``[L, code_bytes]`` (uint8) of ``v [L, n_pad]`` and their decoded values ``[L, n_pad]``."""
+    L, n_pad = v.shape
+    dt = v.dtype
+    if compressor == "none":
+        return v.contiguous().view(torch.uint8).clone(), v.clone()
+    vb = _blocks(v)
+    lb = _blocks(live.to(v.device))
+    if compressor == "int8":
+        m = vb.abs().amax(-1, keepdim=True)
+        sc = m / torch.full_like(m, 127.0)           # a tensor divisor: true division, not a reciprocal product
+        pos = sc > 0
+        q = torch.where(pos, torch.round(vb / torch.where(pos, sc, torch.ones_like(sc))), torch.zeros_like(vb))
+        q = q.clamp_(-127.0, 127.0)
+        dec = (q * sc).reshape(L, n_pad)
+        codes = torch.cat([q.to(torch.int8).reshape(L, n_pad).view(torch.uint8),
+                           sc.reshape(L, -1).contiguous().view(torch.uint8)], dim=1)
+        return codes, dec
+    if compressor != "sign":
+        raise ValueError(f"unknown compressor {compressor!r}")
+    vec = CHOCO_VEC[dt]
+    a = torch.where(lb, vb.abs(), torch.zeros_like(vb)).reshape(L, -1, CHOCO_BLOCK // vec, vec)
+    p = a[..., 0]
+    for u in range(1, vec):
+        p = p + a[..., u]
+    while p.shape[-1] > 1:
+        h = p.shape[-1] // 2
+        p = p[..., :h] + p[..., h:]
+    p = p[..., 0]
+    nl = lb.sum(-1).to(dt).expand_as(p)
+    sc = torch.where(nl > 0, p / torch.where(nl > 0, nl, torch.ones_like(nl)), torch.zeros_like(p))
+    bits = vb >= 0
+    shifts = torch.arange(CHOCO_BLOCK, device=v.device, dtype=torch.int64)
+    words = (bits.to(torch.int64) << shifts).sum(-1)
+    wbytes = torch.stack([(words >> (8 * k)) & 255 for k in range(4)], dim=-1).to(torch.uint8).reshape(L, -1)
+    scb = sc.unsqueeze(-1)
+    dec = torch.where(lb, torch.where(bits, scb, -scb), torch.zeros_like(vb)).reshape(L, n_pad)
+    codes = torch.cat([wbytes, sc.contiguous().view(torch.uint8)], dim=1)
+    return codes, dec
+
+
+def choco_decode(codes: torch.Tensor, compressor: str, n_pad: int, dtype: torch.dtype,
+                 live: torch.Tensor) -> torch.Tensor:
+    """``dec(q)`` of code rows ``[R, code_bytes]`` (uint8) -> ``[R, n_pad]`` in ``dtype``."""
+    codes = codes.contiguous()
+    R = codes.shape[0]
+    if compressor == "none":
+        return codes.view(dtype).clone()
+    nb = n_pad // CHOCO_BLOCK
+    if compressor == "int8":
+        q = codes[:, :n_pad].contiguous().view(torch.int8).to(dtype).reshape(R, nb, CHOCO_BLOCK)
+        sc = codes[:, n_pad:].contiguous().view(dtype)
+        return (q * sc.unsqueeze(-1)).reshape(R, n_pad)
+    if compressor != "sign":
+        raise ValueError(f"unknown compressor {compressor!r}")
+    wb = codes[:, :4 * nb].to(torch.int64).reshape(R, nb, 4)
+    words = wb[..., 0] | (wb[..., 1] << 8) | (wb[..., 2] << 16) | (wb[..., 3] << 24)
+    shifts = torch.arange(CHOCO_BLOCK, device=codes.device, dtype=torch.int64)
+    bits = ((words.unsqueeze(-1) >> shifts) & 1).bool()
+    sc = codes[:, 4 * nb:].contiguous().view(dtype).unsqueeze(-1)
+    lb = _blocks(live.to(codes.device))
+    zero = torch.zeros((), dtype=dtype, device=codes.device)
+    return torch.where(lb, torch.where(bits, sc, -sc), zero).reshape(R, n_pad)
+
+
+def choco_mix_(theta: torch.Tensor, x_hat: torch.Tensor, s: torch.Tensor, dec_all: torch.Tensor,
+               w_rows: torch.Tensor, gamma: float):
+    """``s_i += sum_j W_ij dec(q_j)`` (own term included); ``theta_i += gamma (s_i - x_hat_i)``."""
+    s.add_(w_rows.to(dec_all.dtype) @ dec_all)
+    theta.add_(s - x_hat, alpha=gamma)
+
+
+def choco_step_(theta: torch.Tensor, x_hat: torch.Tensor, grad: torch.Tensor, alpha: float, compressor: str,
+                live: torch.Tensor) -> torch.Tensor:
+    """``theta -= alpha g``; ``q = Q(theta - x_hat)``; ``x_hat += dec(q)``; returns the code rows ``q`` to publish."""
+    theta.add_(grad, alpha=-alpha)
+    codes, dec = choco_encode(theta - x_hat, compressor, live)
+    x_hat.add_(dec)
+    return codes
+
+
 # ------------------------------------------------------------- metrics ----
 def consensus_error(theta_all: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Pairwise and to-mean distances of L2-normalised parameter rows

@@ -119,10 +119,14 @@ struct ConsensusOp {
   consensus::DinnoArgs<T> dn{};
   consensus::DsgtArgs<T> gt{};
   consensus::EdArgs<T> ed{};
+  consensus::ChocoArgs<T> ch{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c;
+    dn.c = c; gt.c = c; ed.c = c; ch.c = c;
     ed.psi = ptr<T>(d, "psi");
+    ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
+    ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
+    ch.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
@@ -142,6 +146,18 @@ struct ConsensusOp {
   void ed_step() {
     if (ed.psi == nullptr) throw std::runtime_error("ed_step needs the Exact Diffusion row `psi`");
     check(consensus::launch_ed_step<T>(ed, cur_stream()), "ed_step");
+  }
+  void choco_check(const char* what) const {
+    if (ch.x_hat == nullptr || ch.s == nullptr || ch.live == nullptr || ch.code_stride <= 0)
+      throw std::runtime_error(std::string(what) + " needs the CHOCO rows `x_hat`, `s`, the `live` mask and `code_stride`");
+  }
+  void choco_mix() {
+    choco_check("choco_mix");
+    check(consensus::launch_choco_mix<T>(ch, cur_stream()), "choco_mix");
+  }
+  void choco_step() {
+    choco_check("choco_step");
+    check(consensus::launch_choco_step<T>(ch, cur_stream()), "choco_step");
   }
 };
 
@@ -174,7 +190,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dsgt_mix", &ConsensusOp<T>::dsgt_mix)
       .def("dsgt_track", &ConsensusOp<T>::dsgt_track)
       .def("ed_mix", &ConsensusOp<T>::ed_mix)
-      .def("ed_step", &ConsensusOp<T>::ed_step);
+      .def("ed_step", &ConsensusOp<T>::ed_step)
+      .def("choco_mix", &ConsensusOp<T>::choco_mix)
+      .def("choco_step", &ConsensusOp<T>::choco_step);
 }
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp

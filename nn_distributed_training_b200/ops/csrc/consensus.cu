@@ -1,10 +1,12 @@
-// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion.
+// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion /
+// CHOCO-SGD.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
 //   optimizers/dsgd.py:37-46 / :55-58      -> dsgd_mix / dsgd_step
 //   optimizers/dsgt.py:58-75 / :87-103     -> dsgt_mix / dsgt_track
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
+// CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
 //
 // Every kernel is a single pass over the node's 16-byte vectorised parameter row: neighbor
 // rows are pulled straight from the (local or NVLink-peer) published buffers named by the
@@ -472,6 +474,157 @@ __global__ void __launch_bounds__(THREADS) ed_step_kernel(const EdArgs<T> a) {
   finish_round(c, ri.k);
 }
 
+// ---------------------------------------------------------------- CHOCO-SGD ----
+// The published rows are code rows (consensus.h).  Round k: choco_mix reads the codes q^{k-1} of the node and its
+// neighbors (all zero in round 0), s_i += W_ii dec(q_i) + sum_j W_ij dec(q_j), theta_i += gamma (s_i - x_hat_i);
+// choco_step takes theta_i -= alpha_k g_i, q_i = Q(theta_i - x_hat_i), x_hat_i += dec(q_i) and publishes q_i.
+template <typename T, int Q>
+__global__ void __launch_bounds__(THREADS) choco_mix_kernel(const ChocoArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const char* own = code_row(a, ri.par, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const unsigned lw = Q == kCodeSign ? a.live[i >> 5] : 0u;
+    Pack<T> t = choco_decode<T, Q>(own, c.n_pad, i, lw);
+#pragma unroll
+    for (int u = 0; u < N; ++u) t.v[u] *= ws;
+    // four neighbor code rows in flight per thread, decoded in registers
+    for (int e0 = 0; e0 < deg; e0 += 4) {
+      Pack<T> q[4];
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (e0 + j < deg) q[j] = choco_decode<T, Q>(nbr_code_row(a, ri.gid, l, e0 + j, ri.par), c.n_pad, i, lw);
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (e0 + j < deg) {
+          const T we = w[e0 + j];
+#pragma unroll
+          for (int u = 0; u < N; ++u) t.v[u] += we * q[j].v[u];
+        }
+    }
+    Pack<T> s = ldv(a.s + row + i);
+    const Pack<T> xh = ldv(a.x_hat + row + i);
+    Pack<T> th = ldv(c.theta + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      s.v[u] += t.v[u];
+      th.v[u] += a.gamma * (s.v[u] - xh.v[u]);
+    }
+    stv(a.s + row + i, s);
+    stv(c.theta + row + i, th);
+  }
+}
+
+// The G = 32 / N lanes holding one 32-element block reduce its scale with xor shuffles; the loop runs per warp, so
+// every lane takes part, also the lanes past the end of a row shorter than a warp's span.
+template <typename T, int U, int Q>
+__global__ void __launch_bounds__(THREADS) choco_step_kernel(const ChocoArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  constexpr int G = 32 / N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  char* out = code_row(a, ri.par ^ 1, l);
+  const int lane = threadIdx.x & 31;
+  // theta (written by the mix two launches back) and x_hat (the previous round's step) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int w0 = (blockIdx.x * THREADS + (threadIdx.x & ~31)) * N; w0 < c.n_pad; w0 += gridDim.x * THREADS * N) {
+    const int i = w0 + lane * N;
+    const bool in = i < c.n_pad;
+    Pack<T> th, xh;
+#pragma unroll
+    for (int u = 0; u < N; ++u) { th.v[u] = (T)0; xh.v[u] = (T)0; }
+    if (in) {
+      th = ldv(c.theta + row + i);
+      xh = ldv(a.x_hat + row + i);
+    }
+    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    Pack<T> v;
+    if (in) {
+      const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) th.v[u] -= alpha * g.v[u];
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) v.v[u] = th.v[u] - xh.v[u];
+    Pack<T> d;
+    const bool head = (lane & (G - 1)) == 0;      // the lane that stores the block's scale / sign word
+    if (Q == kCodeNone) {
+      d = v;
+      if (in) stv(reinterpret_cast<T*>(out) + i, v);
+    } else if (Q == kCodeInt8) {
+      T m = (T)0;
+#pragma unroll
+      for (int u = 0; u < N; ++u) m = fmax(m, fabs(v.v[u]));
+#pragma unroll
+      for (int o = G / 2; o >= 1; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+      const T sc = div_rn(m, (T)127);
+      signed char q[N];
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const T r = sc > (T)0 ? rint(div_rn(v.v[u], sc)) : (T)0;
+        q[u] = (signed char)fmin(fmax(r, (T)-127), (T)127);
+        d.v[u] = mul_rn((T)q[u], sc);
+      }
+      if (in) {
+        if (N == 4) *reinterpret_cast<int*>(out + i) = *reinterpret_cast<const int*>(q);
+        else *reinterpret_cast<short*>(out + i) = *reinterpret_cast<const short*>(q);
+        if (head) reinterpret_cast<T*>(out + c.n_pad)[i >> 5] = sc;
+      }
+    } else {
+      const unsigned lw = in ? a.live[i >> 5] : 0u;
+      // sum |v| over the live elements: in element order within the lane, then halving across the block's lanes
+      T p = (T)0;
+      unsigned bits = 0u;
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const int b = (i & 31) + u;
+        const T av = ((lw >> b) & 1u) ? fabs(v.v[u]) : (T)0;
+        p = u == 0 ? av : p + av;
+        if (v.v[u] >= (T)0) bits |= 1u << b;
+      }
+#pragma unroll
+      for (int o = G / 2; o >= 1; o >>= 1) {
+        p += __shfl_xor_sync(0xffffffffu, p, o);
+        bits |= __shfl_xor_sync(0xffffffffu, bits, o);
+      }
+      const int nl = __popc(lw);
+      const T sc = nl > 0 ? div_rn(p, (T)nl) : (T)0;
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const int b = (i & 31) + u;
+        d.v[u] = ((lw >> b) & 1u) ? (((bits >> b) & 1u) ? sc : -sc) : (T)0;
+      }
+      if (in && head) {
+        reinterpret_cast<unsigned*>(out)[i >> 5] = bits;
+        reinterpret_cast<T*>(out + (c.n_pad >> 3))[i >> 5] = sc;
+      }
+    }
+    if (in) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) xh.v[u] += d.v[u];
+      stv(c.theta + row + i, th);
+      stv(a.x_hat + row + i, xh);
+    }
+  }
+  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
+  step_bookkeeping(c, l);
+  tag_published(c, l, ri.k);
+  finish_round(c, ri.k);
+}
+
 // ------------------------------------------------------------ consensus metric ----
 NNDT_DEVINL double block_sum(double v) {
   __shared__ double red[THREADS / 32];
@@ -630,6 +783,32 @@ template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st) {
   return NNDT_BY_S(a.c.S, ed_step_kernel, a, a.c);
 }
+// the compressor is a template parameter, not a runtime branch (see dsgt_mix above)
+template <typename T, int Q> static cudaError_t choco_mix_q(const ChocoArgs<T>& a, cudaStream_t st) {
+  return launch_pdl(choco_mix_kernel<T, Q>, grid_for(a.c, choco_mix_kernel<T, Q>), dim3(THREADS), 0, st, a);
+}
+// more than 4 gradient partials: 8 loads in flight (the summation order is the same for any depth); 16, as the other
+// step kernels use, took 164 registers (fp64) or spilled (fp32) next to the encoder
+template <typename T, int Q> static cudaError_t choco_step_q(const ChocoArgs<T>& a, cudaStream_t st) {
+  return a.c.S <= 4 ? launch_pdl(choco_step_kernel<T, 4, Q>, grid_for(a.c, choco_step_kernel<T, 4, Q>), dim3(THREADS), 0, st, a)
+                    : launch_pdl(choco_step_kernel<T, 8, Q>, grid_for(a.c, choco_step_kernel<T, 8, Q>), dim3(THREADS), 0, st, a);
+}
+template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st) {
+  switch (a.code) {
+    case kCodeNone: return choco_mix_q<T, kCodeNone>(a, st);
+    case kCodeInt8: return choco_mix_q<T, kCodeInt8>(a, st);
+    case kCodeSign: return choco_mix_q<T, kCodeSign>(a, st);
+  }
+  return cudaErrorInvalidValue;
+}
+template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st) {
+  switch (a.code) {
+    case kCodeNone: return choco_step_q<T, kCodeNone>(a, st);
+    case kCodeInt8: return choco_step_q<T, kCodeInt8>(a, st);
+    case kCodeSign: return choco_step_q<T, kCodeSign>(a, st);
+  }
+  return cudaErrorInvalidValue;
+}
 #undef NNDT_BY_S
 
 #define NNDT_INST(T)                                                                  \
@@ -643,7 +822,9 @@ template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_
   template cudaError_t launch_dsgt_mix<T>(const DsgtArgs<T>&, cudaStream_t);          \
   template cudaError_t launch_dsgt_track<T>(const DsgtArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_ed_mix<T>(const EdArgs<T>&, cudaStream_t);              \
-  template cudaError_t launch_ed_step<T>(const EdArgs<T>&, cudaStream_t);
+  template cudaError_t launch_ed_step<T>(const EdArgs<T>&, cudaStream_t);             \
+  template cudaError_t launch_choco_mix<T>(const ChocoArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);
 NNDT_INST(float)
 NNDT_INST(double)
 

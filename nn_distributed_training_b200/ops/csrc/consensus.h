@@ -93,6 +93,27 @@ struct EdArgs {
   T* psi;                          // [L, n_pad] the adapt step of the previous round; set from theta in round 0
 };
 
+// CHOCO-SGD (Koloskova, Stich, Jaggi 2019), memory-efficient form: nodes publish a compressed code of
+// v = theta - x_hat instead of theta.  The published buffer holds code rows of `code_stride` bytes (nbr_ptr points at
+// them); per block of 32 elements (b = i / 32, nb = n_pad / 32 blocks):
+//   kCodeNone: [n_pad] T                          v itself
+//   kCodeInt8: [n_pad] int8 codes, [nb] T scales  dec = code * scale, scale = max|v| / 127
+//   kCodeSign: [nb] uint32 sign words, [nb] T     bit (i % 32) of word b set when v >= 0; dec = +-scale on live
+//                                                 elements (bit set in `live`), 0 elsewhere; scale = sum|v| / n_live
+// The same layout is written by ops/consensus_ref.py: choco_encode / choco_decode.
+enum Code : int { kCodeNone = 0, kCodeInt8 = 1, kCodeSign = 2 };
+
+template <typename T>
+struct ChocoArgs {
+  Common<T> c;
+  T* x_hat;                        // [L, n_pad] public estimate: the sum of the node's decoded codes
+  T* s;                            // [L, n_pad] sum_j W_ij x_hat_j (own term included)
+  const unsigned* live;            // [n_pad / 32] bit mask of the parameter elements (row padding and slot holes clear)
+  T gamma;                         // consensus step
+  int code;                        // Code
+  long long code_stride;           // bytes per code row of the published buffer
+};
+
 // Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient
 // partials are summed and one torch.optim SGD / Adam / AdamW step is applied, while c.calls[l] < budget[l].
 // Uses c.L, c.n_pad, c.S, c.theta, c.grad_part and c.calls (the node's step counter, required).
@@ -115,6 +136,8 @@ template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStream_t st);
 
 // All-rank barrier on the device (bench start alignment, metric quiescence): every rank stores `epoch` into its slot of

@@ -293,5 +293,48 @@ NNDT_DEVINL void dinno_apply(const DinnoCoef<T>& q, Pack<T>& th, const Pack<T>& 
   opt_apply(q.o, th, m, v, g);
 }
 
+// ---- CHOCO code rows (layout in consensus.h) ----
+// the products and quotients that make or decode a code are rounded on their own (never contracted into an FMA, and
+// IEEE division under --use_fast_math), so ops/consensus_ref.py produces the same bytes
+NNDT_DEVINL float mul_rn(float x, float y) { return __fmul_rn(x, y); }
+NNDT_DEVINL double mul_rn(double x, double y) { return __dmul_rn(x, y); }
+NNDT_DEVINL float div_rn(float x, float y) { return __fdiv_rn(x, y); }
+NNDT_DEVINL double div_rn(double x, double y) { return __ddiv_rn(x, y); }
+
+template <typename T>
+NNDT_DEVINL char* code_row(const ChocoArgs<T>& a, int par, int l) {
+  return reinterpret_cast<char*>(a.c.pub) + ((size_t)par * a.c.C * a.c.pub_L + l) * (size_t)a.code_stride;
+}
+template <typename T>
+NNDT_DEVINL const char* nbr_code_row(const ChocoArgs<T>& a, int gid, int l, int e, int par) {
+  return reinterpret_cast<const char*>(nbr_row(a.c, gid, l, e, par, 0));
+}
+
+// dec(q) of the Vec<T>::N elements at i (i a multiple of N) of a code row; `lw` = live word of the block (sign only)
+template <typename T, int Q>
+NNDT_DEVINL Pack<T> choco_decode(const char* row, int n_pad, int i, unsigned lw) {
+  constexpr int N = Vec<T>::N;
+  Pack<T> d;
+  if (Q == kCodeNone) {
+    d = ldv(reinterpret_cast<const T*>(row) + i);
+  } else if (Q == kCodeInt8) {
+    const T sc = reinterpret_cast<const T*>(row + n_pad)[i >> 5];
+    signed char q[N];
+    if (N == 4) *reinterpret_cast<int*>(q) = *reinterpret_cast<const int*>(row + i);
+    else *reinterpret_cast<short*>(q) = *reinterpret_cast<const short*>(row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) d.v[u] = mul_rn((T)q[u], sc);
+  } else {
+    const unsigned w = reinterpret_cast<const unsigned*>(row)[i >> 5];
+    const T sc = reinterpret_cast<const T*>(row + (n_pad >> 3))[i >> 5];
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      const int b = (i & 31) + u;
+      d.v[u] = ((lw >> b) & 1u) ? (((w >> b) & 1u) ? sc : -sc) : (T)0;
+    }
+  }
+  return d;
+}
+
 }  // namespace consensus
 }  // namespace nndt

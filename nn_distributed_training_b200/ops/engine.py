@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import load_ext
-from .consensus_ref import ed_weights
+from .consensus_ref import CHOCO_CODE, choco_live_words, ed_weights
 from ..parallel.symm import SymmetricBuffer
 from ..utils.graph_generation import Topology
 
@@ -38,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "exact_diffusion"):
+    elif opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):
         alpha[:] = opt.alpha
@@ -55,15 +55,22 @@ class ConsensusEngine:
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
         self.C = 2 if opt.alg_name == "dsgt" else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
+        itemsize = a.theta.element_size()
+        self.choco = opt.alg_name == "choco_sgd"
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
+        # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows
+        self.row_bytes = opt.code_bytes if self.choco else n_pad * itemsize
         Lmax = max(pl.counts)
-        self.pub_buf = SymmetricBuffer((2, self.C, Lmax, n_pad), self.dtype, ctx)
+        self.pub_buf = SymmetricBuffer((2, self.C, Lmax, self.row_bytes // itemsize), self.dtype, ctx)
         self.pub = self.pub_buf.local
         self.Lpub = Lmax
         k0 = opt.k
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
-        self.pub[k0 & 1, 0, :L].copy_(a.theta)
+        if self.choco:
+            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
+        else:
+            self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if opt.alg_name == "dsgt" and getattr(opt, "_initialised", False):
             self.pub[k0 & 1, 1, :L].copy_(opt.y)
 
@@ -96,8 +103,10 @@ class ConsensusEngine:
             gid[k] = gi
         self.topos = topos
         G = len(topos)
+        if self.choco and G > 1:
+            raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
+                             f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
         dmax = max(1, max(t.max_degree for t in topos))
-        itemsize = a.theta.element_size()
         nbr_ptr = np.zeros((G, L, dmax, 2, self.C), dtype=np.int64)
         nbr_w = np.zeros((G, L, dmax), dtype=npdt)
         self_w = np.zeros((G, L), dtype=npdt)
@@ -117,8 +126,8 @@ class ConsensusEngine:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
                         for ch in range(self.C):
-                            row = ((par * self.C + ch) * self.Lpub + lj) * n_pad
-                            nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * itemsize
+                            row = (par * self.C + ch) * self.Lpub + lj
+                            nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
         self.dmax = dmax
         self.t_nbr_ptr = torch.as_tensor(nbr_ptr, device=dev)
         self.t_nbr_w = torch.as_tensor(nbr_w, device=dev)
@@ -172,7 +181,8 @@ class ConsensusEngine:
             ctx.barrier()
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
+        # (CHOCO-SGD always pulls through the pointer table: its published rows are codes; complete_graph_mode is ignored)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco
                          and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -240,9 +250,21 @@ class ConsensusEngine:
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
         if opt.alg_name == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
+        self.t_live = None
+        if self.choco:
+            self.t_live = choco_live_words(opt.live).to(dev)
+            d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
+                     code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d
+
+    def bytes_per_round(self) -> Dict[str, int]:
+        """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
+        neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
+        counted)."""
+        deg = int(self.t_deg[0].sum().item())
+        return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg}
 
     def consensus_metric(self, k: int):
         """Fused consensus-error metric (csrc/consensus.cu: consensus_metric_kernel) on the rows published

@@ -1,9 +1,11 @@
+from .choco import ChocoSGD
 from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
 
-ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion}
+ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
+              "choco_sgd": ChocoSGD}
 
 
 def build_optimizer(problem, device, opt_conf):

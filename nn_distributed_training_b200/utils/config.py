@@ -15,7 +15,8 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion")
+ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd")
+CHOCO_COMPRESSORS = ("none", "int8", "sign")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
 DENSITY_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "mesh_grid_density",
@@ -29,6 +30,8 @@ OPT_SCHEMA = {
     "dsgd": {"alpha0": REQUIRED, "mu": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
     "dsgt": {"alpha": REQUIRED, "init_grads": True, "outer_iterations": REQUIRED, "profile": False},
     "exact_diffusion": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False},
+    "choco_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED,
+                  "outer_iterations": REQUIRED, "profile": False},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -72,9 +75,18 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg == "exact_diffusion" and c.get("mixing_order", "jacobi") != "jacobi":
-        raise ConfigError(f"{path}.mixing_order: exact_diffusion runs the synchronous 'jacobi' order only "
+    if alg in ("exact_diffusion", "choco_sgd") and c.get("mixing_order", "jacobi") != "jacobi":
+        raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
+    if alg == "choco_sgd":
+        if not 0.0 < float(c["gamma"]) <= 1.0:
+            raise ConfigError(f"{path}.gamma must be in (0, 1] (got {c['gamma']!r})")
+        if c["compressor"] not in CHOCO_COMPRESSORS:
+            raise ConfigError(f"{path}.compressor must be one of {'|'.join(CHOCO_COMPRESSORS)} (got {c['compressor']!r})")
+        # s = sum_j W_ij x_hat_j is only valid for a fixed W: the graph is never refreshed
+        if c.setdefault("update_graph", False):
+            raise ConfigError(f"{path}.update_graph: choco_sgd needs a fixed graph (its sum of the neighbors' estimates "
+                              f"is only valid for a fixed mixing matrix)")
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c
