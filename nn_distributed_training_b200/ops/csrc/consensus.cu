@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(THREADS) dinno_update_kernel(const DinnoArgs<T
 #pragma unroll
         for (int u = 0; u < N; ++u) dl.v[u] = (T)(sall.v[u] - (double)c.n_total * (double)thk.v[u]);
       } else {
-        // up to four neighbor rows in flight per thread: over NVLink a load is ~2 us, issued one by one they add up
+        // for_neighbors<4> written out: through the helper's lambdas this kernel compiles to a different stream
         for (int e0 = 0; e0 < deg; e0 += 4) {
           Pack<T> q[4];
 #pragma unroll
@@ -135,7 +135,7 @@ __global__ void __launch_bounds__(THREADS) dinno_update_kernel(const DinnoArgs<T
         v = ldv(a.v + row + i);
       }
     }
-    if (!waited) { tl_stamp(c, ri.k, a.step, 2); pdl_wait(); pdl_launch_dependents(); waited = true; tl_stamp(c, ri.k, a.step, 3); }
+    if (!waited) { tl_stamp(c, ri.k, a.step, 2); release_dependents_once(waited); tl_stamp(c, ri.k, a.step, 3); }
     const Pack<T> gl = sum_partials<U>(c, l, i);
     dinno_apply(cf, th, thk, dl, du, m, v, gl);
     if (a.opt != kSGD) {
@@ -145,10 +145,9 @@ __global__ void __launch_bounds__(THREADS) dinno_update_kernel(const DinnoArgs<T
     stv(c.theta + row + i, th);
     if (last) stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
   }
-  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
+  release_dependents_once(waited);
   tl_stamp(c, ri.k, a.step, 4);
-  step_bookkeeping(c, l);
-  if (last) { tag_published(c, l, ri.k); finish_round(c, ri.k); }
+  end_step(c, l, ri.k, last);
 }
 
 // ------------------------------------------------------------- local step ----
@@ -177,7 +176,7 @@ __global__ void __launch_bounds__(THREADS) local_step_kernel(const LocalArgs<T> 
       m = ldv(a.m + row + i);
       v = ldv(a.v + row + i);
     }
-    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    release_dependents_once(waited);
     const Pack<T> g = sum_partials<U>(c, l, i);
     opt_apply(q, th, m, v, g);
     if (a.opt != kSGD) {
@@ -186,7 +185,7 @@ __global__ void __launch_bounds__(THREADS) local_step_kernel(const LocalArgs<T> 
     }
     stv(c.theta + row + i, th);
   }
-  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
+  release_dependents_once(waited);
   // the last CTA of node l to arrive advances its counter: every CTA has read `call` by then
   __syncthreads();
   if (threadIdx.x == 0 && atomicAdd(a.arrive + l, 1u) == gridDim.x - 1) {
@@ -220,19 +219,11 @@ __global__ void __launch_bounds__(THREADS) dsgd_mix_kernel(const Common<T> c) {
     Pack<T> th = ldv(c.theta + row + i);
 #pragma unroll
     for (int u = 0; u < N; ++u) th.v[u] *= ws;
-    for (int e0 = 0; e0 < deg; e0 += 4) {
-      Pack<T> q[4];
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (e0 + j < deg) q[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (e0 + j < deg) {
-          const T we = w[e0 + j];
-#pragma unroll
-          for (int u = 0; u < N; ++u) th.v[u] += we * q[j].v[u];
-        }
-    }
+                       for (int u = 0; u < N; ++u) th.v[u] += w[e] * q.v[u];
+                     });
     stv(c.theta + row + i, th);
   }
 }
@@ -254,9 +245,7 @@ __global__ void __launch_bounds__(THREADS) dsgd_step_kernel(const Common<T> c) {
     stv(c.theta + row + i, th);
     stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
   }
-  step_bookkeeping(c, l);
-  tag_published(c, l, ri.k);
-  finish_round(c, ri.k);
+  end_step(c, l, ri.k, true);
 }
 
 // ------------------------------------------------------------------- DSGT ----
@@ -320,6 +309,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_mix_kernel(const DsgtArgs<T> a) 
     if (OWN) {
 #pragma unroll
       for (int u = 0; u < N; ++u) th.v[u] *= ws;
+      // for_neighbors<2> written out, as below
       for (int e0 = 0; e0 < deg; e0 += 2) {
         Pack<T> q[2];
 #pragma unroll
@@ -340,6 +330,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_mix_kernel(const DsgtArgs<T> a) 
     }
 #pragma unroll
     for (int u = 0; u < N; ++u) th.v[u] = ws * (th.v[u] - al.v[u] * y.v[u]);
+    // for_neighbors<2> written out: through the helper's lambdas this loop compiles to a different stream
     for (int e0 = 0; e0 < deg; e0 += 2) {
       Pack<T> qt[2], qy[2];
 #pragma unroll
@@ -383,6 +374,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_track_kernel(const DsgtArgs<T> a
       y = ldv(ys + i);
 #pragma unroll
       for (int u = 0; u < N; ++u) y.v[u] *= ws;
+      // for_neighbors<4> written out: through the helper's lambdas this kernel compiles to a different stream
       for (int e0 = 0; e0 < deg; e0 += 4) {
         Pack<T> q[4];
 #pragma unroll
@@ -405,9 +397,7 @@ __global__ void __launch_bounds__(THREADS) dsgt_track_kernel(const DsgtArgs<T> a
     stv(pub_row(c, ri.par ^ 1, 1, l) + i, y);
     stv(pub_row(c, ri.par ^ 1, 0, l) + i, ldv(c.theta + row + i));
   }
-  step_bookkeeping(c, l);
-  tag_published(c, l, ri.k);
-  finish_round(c, ri.k);
+  end_step(c, l, ri.k, true);
 }
 
 // -------------------------------------------------------- Exact Diffusion ----
@@ -456,7 +446,7 @@ __global__ void __launch_bounds__(THREADS) ed_step_kernel(const EdArgs<T> a) {
 #pragma unroll
       for (int u = 0; u < N; ++u) dc.v[u] = th.v[u] - ps.v[u];
     }
-    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    release_dependents_once(waited);
     const Pack<T> g = sum_partials<U>(c, l, i);
     Pack<T> pn, tn;
 #pragma unroll
@@ -468,10 +458,8 @@ __global__ void __launch_bounds__(THREADS) ed_step_kernel(const EdArgs<T> a) {
     stv(c.theta + row + i, tn);
     stv(pub_row(c, ri.par ^ 1, 0, l) + i, tn);
   }
-  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
-  step_bookkeeping(c, l);
-  tag_published(c, l, ri.k);
-  finish_round(c, ri.k);
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
 }
 
 // ---------------------------------------------------------------- CHOCO-SGD ----
@@ -497,20 +485,12 @@ __global__ void __launch_bounds__(THREADS) choco_mix_kernel(const ChocoArgs<T> a
     Pack<T> t = choco_decode<T, Q>(own, c.n_pad, i, lw);
 #pragma unroll
     for (int u = 0; u < N; ++u) t.v[u] *= ws;
-    // four neighbor code rows in flight per thread, decoded in registers
-    for (int e0 = 0; e0 < deg; e0 += 4) {
-      Pack<T> q[4];
+    // the neighbor code rows are decoded in registers
+    for_neighbors<4>(deg, [&](int e) { return choco_decode<T, Q>(nbr_code_row(a, ri.gid, l, e, ri.par), c.n_pad, i, lw); },
+                     [&](int e, const Pack<T>& q) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (e0 + j < deg) q[j] = choco_decode<T, Q>(nbr_code_row(a, ri.gid, l, e0 + j, ri.par), c.n_pad, i, lw);
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (e0 + j < deg) {
-          const T we = w[e0 + j];
-#pragma unroll
-          for (int u = 0; u < N; ++u) t.v[u] += we * q[j].v[u];
-        }
-    }
+                       for (int u = 0; u < N; ++u) t.v[u] += w[e] * q.v[u];
+                     });
     Pack<T> s = ldv(a.s + row + i);
     const Pack<T> xh = ldv(a.x_hat + row + i);
     Pack<T> th = ldv(c.theta + row + i);
@@ -550,7 +530,7 @@ __global__ void __launch_bounds__(THREADS) choco_step_kernel(const ChocoArgs<T> 
       th = ldv(c.theta + row + i);
       xh = ldv(a.x_hat + row + i);
     }
-    if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+    release_dependents_once(waited);
     Pack<T> v;
     if (in) {
       const Pack<T> g = sum_partials<U>(c, l, i);
@@ -619,10 +599,8 @@ __global__ void __launch_bounds__(THREADS) choco_step_kernel(const ChocoArgs<T> 
       stv(a.x_hat + row + i, xh);
     }
   }
-  if (!waited) { pdl_wait(); pdl_launch_dependents(); }
-  step_bookkeeping(c, l);
-  tag_published(c, l, ri.k);
-  finish_round(c, ri.k);
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
 }
 
 // ------------------------------------------------------------ consensus metric ----
@@ -748,68 +726,62 @@ template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStrea
   const int per_block = THREADS * Vec<T>::N;
   return launch_pdl(local_sum_kernel<T>, dim3((c.n_pad + per_block - 1) / per_block), dim3(THREADS), 0, st, c);
 }
-// kernels that sum gradient partials: the 4-deep variant when the producer writes <= 4 partial rows per node
-#define NNDT_BY_S(S, KERNEL, ARG, C)                                                              \
-  ((S) <= 4 ? launch_pdl(KERNEL<T, 4>, grid_for(C, KERNEL<T, 4>), dim3(THREADS), 0, st, ARG)     \
-            : launch_pdl(KERNEL<T, 16>, grid_for(C, KERNEL<T, 16>), dim3(THREADS), 0, st, ARG))
+template <typename T, typename K, typename A>
+static cudaError_t launch_one_wave(K kernel, const Common<T>& c, const A& a, cudaStream_t st) {
+  return launch_pdl(kernel, grid_for(c, kernel), dim3(THREADS), 0, st, a);
+}
+// kernels that sum gradient partials: the shallow variant (4 loads in flight) when the producer writes <= 4 partial
+// rows per node, the deep one otherwise
+template <typename T, typename K, typename A>
+static cudaError_t launch_by_s(K shallow, K deep, const Common<T>& c, const A& a, cudaStream_t st) {
+  return launch_one_wave(c.S <= 4 ? shallow : deep, c, a, st);
+}
 template <typename T> cudaError_t launch_dinno_update(const DinnoArgs<T>& a, cudaStream_t st) {
-  return NNDT_BY_S(a.c.S, dinno_update_kernel, a, a.c);
+  return launch_by_s(dinno_update_kernel<T, 4>, dinno_update_kernel<T, 16>, a.c, a, st);
 }
 template <typename T> cudaError_t launch_local_step(const LocalArgs<T>& a, cudaStream_t st) {
-  return NNDT_BY_S(a.c.S, local_step_kernel, a, a.c);
+  return launch_by_s(local_step_kernel<T, 4>, local_step_kernel<T, 16>, a.c, a, st);
 }
 template <typename T> cudaError_t launch_dsgd_mix(const Common<T>& c, cudaStream_t st) {
-  return launch_pdl(dsgd_mix_kernel<T>, grid_for(c, dsgd_mix_kernel<T>), dim3(THREADS), 0, st, c);
+  return launch_one_wave(dsgd_mix_kernel<T>, c, c, st);
 }
 template <typename T> cudaError_t launch_dsgd_step(const Common<T>& c, cudaStream_t st) {
-  return NNDT_BY_S(c.S, dsgd_step_kernel, c, c);
+  return launch_by_s(dsgd_step_kernel<T, 4>, dsgd_step_kernel<T, 16>, c, c, st);
 }
 template <typename T> cudaError_t launch_dsgt_init(const DsgtArgs<T>& a, cudaStream_t st) {
-  return NNDT_BY_S(a.c.S, dsgt_init_kernel, a, a.c);
+  return launch_by_s(dsgt_init_kernel<T, 4>, dsgt_init_kernel<T, 16>, a.c, a, st);
 }
 template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStream_t st) {
   // the own-tracker step is a template parameter: as a runtime branch it raised the register count past the
   // 64 per thread that keep 4 CTAs resident per SM
-  return a.own_tracker ? launch_pdl(dsgt_mix_kernel<T, true>, grid_for(a.c, dsgt_mix_kernel<T, true>), dim3(THREADS), 0, st, a)
-                       : launch_pdl(dsgt_mix_kernel<T, false>, grid_for(a.c, dsgt_mix_kernel<T, false>), dim3(THREADS), 0, st, a);
+  return launch_one_wave(a.own_tracker ? dsgt_mix_kernel<T, true> : dsgt_mix_kernel<T, false>, a.c, a, st);
 }
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st) {
-  return NNDT_BY_S(a.c.S, dsgt_track_kernel, a, a.c);
+  return launch_by_s(dsgt_track_kernel<T, 4>, dsgt_track_kernel<T, 16>, a.c, a, st);
 }
 template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t st) {
-  return a.c.sum_mode ? launch_pdl(ed_sum_mix_kernel<T>, grid_for(a.c, ed_sum_mix_kernel<T>), dim3(THREADS), 0, st, a.c)
-                      : launch_pdl(dsgd_mix_kernel<T>, grid_for(a.c, dsgd_mix_kernel<T>), dim3(THREADS), 0, st, a.c);
+  return launch_one_wave(a.c.sum_mode ? ed_sum_mix_kernel<T> : dsgd_mix_kernel<T>, a.c, a.c, st);
 }
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st) {
-  return NNDT_BY_S(a.c.S, ed_step_kernel, a, a.c);
+  return launch_by_s(ed_step_kernel<T, 4>, ed_step_kernel<T, 16>, a.c, a, st);
 }
-// the compressor is a template parameter, not a runtime branch (see dsgt_mix above)
-template <typename T, int Q> static cudaError_t choco_mix_q(const ChocoArgs<T>& a, cudaStream_t st) {
-  return launch_pdl(choco_mix_kernel<T, Q>, grid_for(a.c, choco_mix_kernel<T, Q>), dim3(THREADS), 0, st, a);
+// the compressor is a template parameter, not a runtime branch (see dsgt_mix above).  With more than 4 gradient
+// partials the step keeps 8 loads in flight (the summation order is the same for any depth); 16, as the other step
+// kernels use, took 164 registers (fp64) or spilled (fp32) next to the encoder
+template <typename T, int Q> static cudaError_t launch_choco_q(const ChocoArgs<T>& a, bool step, cudaStream_t st) {
+  return step ? launch_by_s(choco_step_kernel<T, 4, Q>, choco_step_kernel<T, 8, Q>, a.c, a, st)
+              : launch_one_wave(choco_mix_kernel<T, Q>, a.c, a, st);
 }
-// more than 4 gradient partials: 8 loads in flight (the summation order is the same for any depth); 16, as the other
-// step kernels use, took 164 registers (fp64) or spilled (fp32) next to the encoder
-template <typename T, int Q> static cudaError_t choco_step_q(const ChocoArgs<T>& a, cudaStream_t st) {
-  return a.c.S <= 4 ? launch_pdl(choco_step_kernel<T, 4, Q>, grid_for(a.c, choco_step_kernel<T, 4, Q>), dim3(THREADS), 0, st, a)
-                    : launch_pdl(choco_step_kernel<T, 8, Q>, grid_for(a.c, choco_step_kernel<T, 8, Q>), dim3(THREADS), 0, st, a);
-}
-template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st) {
+template <typename T> static cudaError_t launch_choco(const ChocoArgs<T>& a, bool step, cudaStream_t st) {
   switch (a.code) {
-    case kCodeNone: return choco_mix_q<T, kCodeNone>(a, st);
-    case kCodeInt8: return choco_mix_q<T, kCodeInt8>(a, st);
-    case kCodeSign: return choco_mix_q<T, kCodeSign>(a, st);
+    case kCodeNone: return launch_choco_q<T, kCodeNone>(a, step, st);
+    case kCodeInt8: return launch_choco_q<T, kCodeInt8>(a, step, st);
+    case kCodeSign: return launch_choco_q<T, kCodeSign>(a, step, st);
   }
   return cudaErrorInvalidValue;
 }
-template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st) {
-  switch (a.code) {
-    case kCodeNone: return choco_step_q<T, kCodeNone>(a, st);
-    case kCodeInt8: return choco_step_q<T, kCodeInt8>(a, st);
-    case kCodeSign: return choco_step_q<T, kCodeSign>(a, st);
-  }
-  return cudaErrorInvalidValue;
-}
-#undef NNDT_BY_S
+template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, false, st); }
+template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, true, st); }
 
 #define NNDT_INST(T)                                                                  \
   template cudaError_t launch_local_sum<T>(const Common<T>&, cudaStream_t);           \

@@ -46,6 +46,13 @@ NNDT_DEVINL int node_of_block(const Common<T>& c) {
   return c.node_order != nullptr ? c.node_order[blockIdx.y] : (int)blockIdx.y;
 }
 
+// A kernel that prefetches what the preceding kernel does not write calls this after its first loads and once more
+// after its loop: the first call waits for that kernel (griddepcontrol.wait) and lets the next one launch, the others
+// do nothing.  The second call covers a thread that got no loop iteration.
+NNDT_DEVINL void release_dependents_once(bool& waited) {
+  if (!waited) { pdl_wait(); pdl_launch_dependents(); waited = true; }
+}
+
 // debug timeline: stamp `which` (0..7) of update launch (round k, primal step) by the first and the last block of the grid
 template <typename T>
 NNDT_DEVINL void tl_stamp(const Common<T>& c, int k, int step, int which) {
@@ -150,6 +157,22 @@ template <typename T>
 NNDT_DEVINL const T* nbr_row(const Common<T>& c, int gid, int l, int e, int par, int chan) {
   return reinterpret_cast<const T*>(c.nbr_ptr[(((size_t)(gid * c.L + l) * c.dmax + e) * 2 + par) * c.C + chan]);
 }
+
+// Pull the neighbors' values at this thread's element: up to D neighbor rows in flight per thread, load(e) for each
+// before acc(e, value) combines any, in neighbor order.  Over NVLink a load is ~2 us; issued one by one they add up.
+template <int D, class FL, class FA>
+NNDT_DEVINL void for_neighbors(int deg, FL load, FA acc) {
+  for (int e0 = 0; e0 < deg; e0 += D) {
+    decltype(load(0)) q[D];
+#pragma unroll
+    for (int j = 0; j < D; ++j)
+      if (e0 + j < deg) q[j] = load(e0 + j);
+#pragma unroll
+    for (int j = 0; j < D; ++j)
+      if (e0 + j < deg) acc(e0 + j, q[j]);
+  }
+}
+
 template <typename T>
 NNDT_DEVINL T* pub_row(const Common<T>& c, int par, int chan, int l) {
   return c.pub + ((size_t)(par * c.C + chan) * c.pub_L + l) * c.n_pad;
@@ -229,6 +252,15 @@ NNDT_DEVINL void step_bookkeeping(const Common<T>& c, int l) {
       c.tloss[l] = t != 0.f ? (1.f - c.tdecay) * t + c.tdecay * loss : loss;
     }
   }
+}
+
+// End of a launch that consumes a gradient.  On the round's last step (`last`) it also tags the rows it published and
+// then advances the round.  The order is part of the publication protocol: each block tags before it arrives at the
+// launch's counter, so when the last arrival advances the round every node's rows of round k + 1 carry their tag.
+template <typename T>
+NNDT_DEVINL void end_step(const Common<T>& c, int l, int k, bool last) {
+  step_bookkeeping(c, l);
+  if (last) { tag_published(c, l, k); finish_round(c, k); }
 }
 
 // ---- torch.optim step on one vector: SGD, Adam (betas 0.9 / 0.999, eps 1e-8), AdamW (+ weight decay 0.01) ----
