@@ -229,6 +229,30 @@ def choco_step_(theta: torch.Tensor, x_hat: torch.Tensor, grad: torch.Tensor, al
     return codes
 
 
+# ------------------------------------------------------------------ SGP ----
+# Push-sum (Stochastic Gradient Push): numerator rows x [L, n_pad] and float64 weights w [L].  The combine weights are
+# the column-stochastic A of Topology.push_weights, rounded to the arena dtype; w is mixed with those same rounded
+# weights (in float64), so x and w see one matrix.
+def sgp_debias(x: torch.Tensor, w: torch.Tensor) -> torch.Tensor:
+    """``theta = x / w``: w rounded to x's dtype, then one IEEE division in that dtype (csrc: sgp_debias)."""
+    return x / w.to(x.dtype).unsqueeze(1)
+
+
+def sgp_mix_(x: torch.Tensor, w: torch.Tensor, theta: torch.Tensor, x_all: torch.Tensor, w_all: torch.Tensor,
+             a_rows: torch.Tensor):
+    """``x_i <- sum_j A_ij x_j``, ``w_i <- sum_j A_ij w_j`` (own term included), ``theta_i <- x_i / w_i``."""
+    a = a_rows.to(x_all.dtype)
+    x.copy_(a @ x_all)
+    w.copy_(a.to(torch.float64) @ w_all.to(torch.float64))
+    theta.copy_(sgp_debias(x, w))
+
+
+def sgp_step_(x: torch.Tensor, w: torch.Tensor, theta: torch.Tensor, grad: torch.Tensor, alpha: float):
+    """``x <- x - alpha g`` (g taken at theta = x / w); ``theta <- x / w``."""
+    x.add_(grad, alpha=-alpha)
+    theta.copy_(sgp_debias(x, w))
+
+
 # ------------------------------------------------------------- metrics ----
 def consensus_error(theta_all: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Pairwise and to-mean distances of L2-normalised parameter rows

@@ -120,9 +120,13 @@ struct ConsensusOp {
   consensus::DsgtArgs<T> gt{};
   consensus::EdArgs<T> ed{};
   consensus::ChocoArgs<T> ch{};
+  consensus::SgpArgs<T> sg{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; ch.c = c;
+    dn.c = c; gt.c = c; ed.c = c; ch.c = c; sg.c = c;
+    sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
+    sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
+    sg.rdr_deg = ptr<const int>(d, "rdr_deg"); sg.rdr_rank = ptr<const int>(d, "rdr_rank"); sg.rmax = geti(d, "rmax", 1);
     ed.psi = ptr<T>(d, "psi");
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
@@ -159,6 +163,18 @@ struct ConsensusOp {
     choco_check("choco_step");
     check(consensus::launch_choco_step<T>(ch, cur_stream()), "choco_step");
   }
+  void sgp_check(const char* what) const {
+    if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0 || sg.rdr_deg == nullptr || sg.rdr_rank == nullptr)
+      throw std::runtime_error(std::string(what) + " needs the SGP rows `x`, `w`, `row_stride` and the reader tables");
+  }
+  void sgp_mix() {
+    sgp_check("sgp_mix");
+    check(consensus::launch_sgp_mix<T>(sg, cur_stream()), "sgp_mix");
+  }
+  void sgp_step() {
+    sgp_check("sgp_step");
+    check(consensus::launch_sgp_step<T>(sg, cur_stream()), "sgp_step");
+  }
 };
 
 // local optimizer step of non-communicating nodes (solo / centralized baselines)
@@ -192,7 +208,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("ed_mix", &ConsensusOp<T>::ed_mix)
       .def("ed_step", &ConsensusOp<T>::ed_step)
       .def("choco_mix", &ConsensusOp<T>::choco_mix)
-      .def("choco_step", &ConsensusOp<T>::choco_step);
+      .def("choco_step", &ConsensusOp<T>::choco_step)
+      .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
+      .def("sgp_step", &ConsensusOp<T>::sgp_step);
 }
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp

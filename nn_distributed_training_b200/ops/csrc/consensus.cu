@@ -1,5 +1,5 @@
 // Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion /
-// CHOCO-SGD.
+// CHOCO-SGD / SGP.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
@@ -7,6 +7,7 @@
 //   optimizers/dsgt.py:58-75 / :87-103     -> dsgt_mix / dsgt_track
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
+// SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 //
 // Every kernel is a single pass over the node's 16-byte vectorised parameter row: neighbor
 // rows are pulled straight from the (local or NVLink-peer) published buffers named by the
@@ -603,6 +604,77 @@ __global__ void __launch_bounds__(THREADS) choco_step_kernel(const ChocoArgs<T> 
   end_step(c, l, ri.k, true);
 }
 
+// -------------------------------------------------------------------- SGP ----
+// Round k: sgp_mix pulls the in-neighbors' rows (x, w) of round k, x_i <- sum_j A_ij x_j, w_i <- sum_j A_ij w_j,
+// theta_i <- x_i / w_i; sgp_step takes x_i -= alpha_k g_i(theta_i), theta_i <- x_i / w_i and publishes (x_i, w_i).
+template <typename T>
+__global__ void __launch_bounds__(THREADS) sgp_mix_kernel(const SgpArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_sgp_round(a, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  // the new push-sum weight, from the node's own published row (a.w[l] is stored below): every CTA of the node sums
+  // in the same order, so all of them divide by the same bits
+  double wn = (double)ws * row_weight(sgp_row(a, ri.par, l), c.n_pad);
+  for_neighbors<4>(deg, [&](int e) { return row_weight(nbr_row(c, ri.gid, l, e, ri.par, 0), c.n_pad); },
+                   [&](int e, double q) { wn += (double)w[e] * q; });
+  if (blockIdx.x == 0 && threadIdx.x == 0) a.w[l] = wn;
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> x = ldv(a.x + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) x.v[u] *= ws;
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
+#pragma unroll
+                       for (int u = 0; u < N; ++u) x.v[u] += w[e] * q.v[u];
+                     });
+    Pack<T> th;
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] = sgp_debias(x.v[u], wn);
+    stv(a.x + row + i, x);
+    stv(c.theta + row + i, th);
+  }
+}
+
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) sgp_step_kernel(const SgpArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  T* out = sgp_row(a, ri.par ^ 1, l);
+  // w and x (written by the mix two launches back) are read before the programmatic-dependency wait; only the
+  // gradient partials of the forward/backward kernel after it
+  const double wn = a.w[l];
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> x = ldv(a.x + row + i);
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> th;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      x.v[u] -= alpha * g.v[u];
+      th.v[u] = sgp_debias(x.v[u], wn);
+    }
+    stv(a.x + row + i, x);
+    stv(c.theta + row + i, th);
+    stv(out + i, x);
+  }
+  release_dependents_once(waited);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *reinterpret_cast<double*>(out + c.n_pad) = wn;
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------------------ consensus metric ----
 NNDT_DEVINL double block_sum(double v) {
   __shared__ double red[THREADS / 32];
@@ -783,6 +855,14 @@ template <typename T> static cudaError_t launch_choco(const ChocoArgs<T>& a, boo
 template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, false, st); }
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, true, st); }
 
+template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(sgp_mix_kernel<T>, a.c, a, st);
+}
+// beyond 4 gradient partials the step keeps 8 loads in flight: 16 spilled in fp32 (the summation order is the same)
+template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(sgp_step_kernel<T, 4>, sgp_step_kernel<T, 8>, a.c, a, st);
+}
+
 #define NNDT_INST(T)                                                                  \
   template cudaError_t launch_local_sum<T>(const Common<T>&, cudaStream_t);           \
   template cudaError_t launch_consensus_metric<T>(const int64_t*, int, int, int, int, double*, double*, double*, cudaStream_t); \
@@ -796,7 +876,9 @@ template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaS
   template cudaError_t launch_ed_mix<T>(const EdArgs<T>&, cudaStream_t);              \
   template cudaError_t launch_ed_step<T>(const EdArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_choco_mix<T>(const ChocoArgs<T>&, cudaStream_t);        \
-  template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);
+  template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);
 NNDT_INST(float)
 NNDT_INST(double)
 

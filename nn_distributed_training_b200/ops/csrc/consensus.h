@@ -114,6 +114,23 @@ struct ChocoArgs {
   long long code_stride;           // bytes per code row of the published buffer
 };
 
+// SGP, Stochastic Gradient Push (Assran et al. 2019): push-sum gossip over a column-stochastic A, on directed graphs.
+// The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
+// A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
+// `row_stride` = n_pad * sizeof(T) + 16 bytes.  theta = x / w is the de-biased row the forward/backward kernel reads.
+// Node i overwrites its row of parity (k+1)&1 at the end of round k; its round-(k-1) readers are its out-neighbors,
+// which on a directed graph are not the ranks it pulls from, so the SGP kernels also wait for them (rdr_rank).
+template <typename T>
+struct SgpArgs {
+  Common<T> c;
+  T* x;                            // [L, n_pad] numerators
+  double* w;                       // [L] push-sum weights
+  long long row_stride;            // bytes per published row
+  const int* rdr_deg;              // [G, L] readers (out-neighbors) of each local node
+  const int* rdr_rank;             // [G, L, rmax] owning rank of each reader, -1 when local
+  int rmax;
+};
+
 // Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient
 // partials are summed and one torch.optim SGD / Adam / AdamW step is applied, while c.calls[l] < budget[l].
 // Uses c.L, c.n_pad, c.S, c.theta, c.grad_part and c.calls (the node's step counter, required).
@@ -138,6 +155,8 @@ template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStream_t st);
 
 // All-rank barrier on the device (bench start alignment, metric quiescence): every rank stores `epoch` into its slot of

@@ -368,5 +368,59 @@ NNDT_DEVINL Pack<T> choco_decode(const char* row, int n_pad, int i, unsigned lw)
   return d;
 }
 
+// ---- SGP (layout in consensus.h) ----
+template <typename T>
+NNDT_DEVINL T* sgp_row(const SgpArgs<T>& a, int par, int l) {
+  return reinterpret_cast<T*>(reinterpret_cast<char*>(a.c.pub) + ((size_t)par * a.c.pub_L + l) * (size_t)a.row_stride);
+}
+// the float64 push-sum weight in the tail of a published row
+template <typename T>
+NNDT_DEVINL double row_weight(const T* row, int n_pad) {
+  return *reinterpret_cast<const double*>(row + n_pad);
+}
+// theta = x / w: w rounded to T, then one IEEE division (ops/consensus_ref.py: sgp_debias)
+template <typename T>
+NNDT_DEVINL T sgp_debias(T x, double w) {
+  return div_rn(x, (T)w);
+}
+
+// wait_neighbors for a directed graph.  Node l overwrites its row of parity (k+1)&1 at the end of round k; the nodes
+// that read that buffer in round k-1 are l's round-(k-1) out-neighbors (readers), which on a directed graph are not the
+// in-neighbors l pulls from.  A rank publishes round k only after its round-(k-1) reads, so waiting for "round k
+// published" from the ranks of in_k(l) and out_{k-1}(l) closes the write-after-read window (tests/
+// test_protocol_model_directed.py).  On an undirected graph the set is wait_neighbors' N_k and N_{k-1}.
+template <typename T>
+NNDT_DEVINL void wait_in_and_readers(const SgpArgs<T>& a, int gid, int l, int k) {
+  const Common<T>& c = a.c;
+  const bool check = c.nbr_seq != nullptr;
+  if (c.world > 1 || check) {
+    const int d = c.deg[gid * c.L + l];
+    if ((int)threadIdx.x < d) {
+      const int r = c.world > 1 ? c.nbr_rank[(gid * c.L + l) * c.dmax + threadIdx.x] : -1;
+      if (r >= 0) wait_rank(c, r, k);
+      if (check) {
+        const int* tag = reinterpret_cast<const int*>(c.nbr_seq[((size_t)(gid * c.L + l) * c.dmax + threadIdx.x) * 2 + (k & 1)]);
+        if (ld_acquire_sys(tag) != k) *c.err = 2;
+      }
+    }
+    if (c.world > 1 && k > 0) {
+      const int gp = c.graph_id[k - 1];
+      const int t = (int)threadIdx.x - 32;                    // a different warp than the in-neighbor waiters
+      if (t >= 0 && t < a.rdr_deg[gp * c.L + l]) {
+        const int r = a.rdr_rank[(gp * c.L + l) * a.rmax + t];
+        if (r >= 0) wait_rank(c, r, k);
+      }
+    }
+    __syncthreads();
+  }
+}
+
+// begin_round of the SGP mix: announce round k, then wait for in_k(l) and out_{k-1}(l)
+template <typename T>
+NNDT_DEVINL void begin_sgp_round(const SgpArgs<T>& a, int gid, int l, int k) {
+  if (a.c.world > 1 && blockIdx.x == 0 && blockIdx.y == 0) announce_round(a.c, k);
+  wait_in_and_readers(a, gid, l, k);
+}
+
 }  // namespace consensus
 }  // namespace nndt

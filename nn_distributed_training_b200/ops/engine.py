@@ -38,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd"):
+    elif opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):
         alpha[:] = opt.alpha
@@ -57,10 +57,17 @@ class ConsensusEngine:
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
+        self.sgp = opt.alg_name == "sgp"
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
-        # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows
-        self.row_bytes = opt.code_bytes if self.choco else n_pad * itemsize
+        # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
+        # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w
+        if self.choco:
+            self.row_bytes = opt.code_bytes
+        elif self.sgp:
+            self.row_bytes = n_pad * itemsize + 16
+        else:
+            self.row_bytes = n_pad * itemsize
         Lmax = max(pl.counts)
         self.pub_buf = SymmetricBuffer((2, self.C, Lmax, self.row_bytes // itemsize), self.dtype, ctx)
         self.pub = self.pub_buf.local
@@ -69,6 +76,9 @@ class ConsensusEngine:
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
         if self.choco:
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
+        elif self.sgp:
+            self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.x)
+            self.pub_weights(k0 & 1).copy_(opt.w)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if opt.alg_name == "dsgt" and getattr(opt, "_initialised", False):
@@ -113,8 +123,12 @@ class ConsensusEngine:
         deg = np.zeros((G, L), dtype=np.int32)
         nbr_rank = -np.ones((G, L, dmax), dtype=np.int32)
         for gi, t in enumerate(topos):
-            # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel
-            Wt = ed_weights(t.W) if opt.alg_name == "exact_diffusion" else t.W
+            # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
+            # push-sum weights, over the in-neighbors
+            if self.sgp:
+                Wt = t.push_weights
+            else:
+                Wt = ed_weights(t.W) if opt.alg_name == "exact_diffusion" else t.W
             for l, g in enumerate(pl.local_nodes):
                 nb = t.neighbors_noself[g]
                 deg[gi, l] = len(nb)
@@ -135,6 +149,21 @@ class ConsensusEngine:
         self.t_deg = torch.as_tensor(deg, device=dev)
         self.t_nbr_rank = torch.as_tensor(nbr_rank, device=dev)
         self.t_gid = torch.as_tensor(gid, device=dev)
+        # SGP: the ranks that read each local node's row (its out-neighbors), which the mix also waits for
+        self.t_rdr_deg = self.t_rdr_rank = None
+        rdr_rank = -np.ones((G, L, 1), dtype=np.int32)
+        if self.sgp:
+            rmax = max(1, max(t.max_readers for t in topos))
+            rdr_deg = np.zeros((G, L), dtype=np.int32)
+            rdr_rank = -np.ones((G, L, rmax), dtype=np.int32)
+            for gi, t in enumerate(topos):
+                for l, g in enumerate(pl.local_nodes):
+                    rdr_deg[gi, l] = len(t.readers[g])
+                    for e, j in enumerate(t.readers[g]):
+                        if int(pl.node_rank[j]) != ctx.rank:
+                            rdr_rank[gi, l, e] = int(pl.node_rank[j])
+            self.t_rdr_deg = torch.as_tensor(rdr_deg, device=dev)
+            self.t_rdr_rank = torch.as_tensor(rdr_rank, device=dev)
 
         # ---- optional protocol self-check (SURVEY 5.2): published rows carry their round, neighbor reads verify it ----
         self.seq_buf = None
@@ -167,7 +196,8 @@ class ConsensusEngine:
         # ranks that own a neighbor of a local node in ANY round's graph: the only ones that need this rank's flags
         notify = 0
         remote_node = np.zeros(L, dtype=bool)
-        for r in np.unique(nbr_rank[nbr_rank >= 0]):
+        # (SGP: also the ranks of the in-neighbors, which wait for this rank as one of their readers)
+        for r in np.unique(np.concatenate([nbr_rank[nbr_rank >= 0], rdr_rank[rdr_rank >= 0]])):
             notify |= 1 << int(r)
         for l in range(L):
             remote_node[l] = bool((nbr_rank[:, l, :] >= 0).any())
@@ -181,8 +211,9 @@ class ConsensusEngine:
             ctx.barrier()
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
-        # (CHOCO-SGD always pulls through the pointer table: its published rows are codes; complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco
+        # (CHOCO-SGD and SGP always pull through the pointer table: their published rows are codes / numerators with a
+        # weight; complete_graph_mode is ignored)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco and not self.sgp
                          and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -255,14 +286,24 @@ class ConsensusEngine:
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
                      code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
+        if self.sgp:
+            d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes),
+                     rdr_deg=self.t_rdr_deg.data_ptr(), rdr_rank=self.t_rdr_rank.data_ptr(),
+                     rmax=int(self.t_rdr_rank.shape[2]))
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d
 
+    def pub_weights(self, par: int) -> torch.Tensor:
+        """SGP: the float64 push-sum weights in the tails of this rank's published rows of parity ``par`` (a view)."""
+        tail = self.pr.arena.n_pad * self.pub.element_size()
+        rows = self.pub[par, 0, :self.pr.placement.L].view(torch.uint8)
+        return rows[:, tail: tail + 8].view(torch.float64)[:, 0]
+
     def bytes_per_round(self) -> Dict[str, int]:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
         neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
-        counted)."""
+        counted).  An SGP row includes its 16-byte weight tail."""
         deg = int(self.t_deg[0].sum().item())
         return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg}
 

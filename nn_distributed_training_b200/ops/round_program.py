@@ -6,6 +6,7 @@ A round is a short, fixed kernel sequence
     DSGT :  dsgt_mix, fwd/bwd, dsgt_track
     Exact Diffusion:  ed_mix, fwd/bwd, ed_step
     CHOCO-SGD:  choco_mix, fwd/bwd, choco_step
+    SGP:  sgp_mix, fwd/bwd, sgp_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -62,6 +63,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.choco_mix()
         grads(0)
         eng.op.choco_step()
+    elif alg == "sgp":
+        eng.op.sgp_mix()
+        grads(0)
+        eng.op.sgp_step()
     else:  # pragma: no cover
         raise NameError("Unknown distributed opt algorithm.")
 
@@ -105,8 +110,8 @@ class RoundProgram:
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD publishes
-        # codes, so its metric reads the parameter rows (all_theta) at the evaluation points instead
-        pr._metric_engine = None if self.eng.choco else (self.eng, lambda: opt.k)
+        # codes and SGP numerators, so their metric reads the parameter rows (all_theta) at the evaluation points instead
+        pr._metric_engine = None if (self.eng.choco or self.eng.sgp) else (self.eng, lambda: opt.k)
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
         self.pipeline = "resident"
@@ -266,7 +271,7 @@ class RoundProgram:
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd") and opt.k > 0:
+        if opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "choco_sgd":
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))

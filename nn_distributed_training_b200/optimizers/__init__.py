@@ -3,9 +3,10 @@ from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
+from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
-              "choco_sgd": ChocoSGD}
+              "choco_sgd": ChocoSGD, "sgp": SGP}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -15,7 +15,9 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd")
+ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd", "sgp")
+# graph types that generate an nx.DiGraph (utils/graph_generation.py); only push-sum SGP runs on them
+DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 CHOCO_COMPRESSORS = ("none", "int8", "sign")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
@@ -32,6 +34,7 @@ OPT_SCHEMA = {
     "exact_diffusion": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False},
     "choco_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED,
                   "outer_iterations": REQUIRED, "profile": False},
+    "sgp": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -75,7 +78,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg in ("exact_diffusion", "choco_sgd") and c.get("mixing_order", "jacobi") != "jacobi":
+    if alg in ("exact_diffusion", "choco_sgd", "sgp") and c.get("mixing_order", "jacobi") != "jacobi":
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
     if alg == "choco_sgd":
@@ -180,7 +183,26 @@ def validate_experiment(conf: Dict[str, Any], kind: str) -> Dict[str, Any]:
             raise ConfigError("missing top-level key `problem_configs`")
         out["problem_configs"] = {k: validate_problem(v, f"problem_configs.{k}", pk)
                                   for k, v in out["problem_configs"].items()}
+    _check_directed_graph(out)
     return out
+
+
+def _check_directed_graph(conf: Dict[str, Any]) -> None:
+    """A directed ``experiment.graph`` has no Metropolis matrix: only SGP runs on it, and link-drop fault injection
+    (which drops undirected edges) does not apply to it."""
+    g = conf["experiment"].get("graph")
+    if not isinstance(g, dict) or g.get("type") not in DIRECTED_GRAPH_TYPES:
+        return
+    probs = conf.get("problem_configs") or ({"problem": conf["problem"]} if "problem" in conf else {})
+    for k, p in probs.items():
+        path = f"problem_configs.{k}" if "problem_configs" in conf else k
+        alg = p["optimizer_config"]["alg_name"]
+        if alg != "sgp":
+            raise ConfigError(f"experiment.graph.type: the directed graph {g['type']!r} runs with alg_name sgp only "
+                              f"({path}.optimizer_config.alg_name is {alg!r})")
+        if p.get("fault_injection"):
+            raise ConfigError(f"{path}.fault_injection: link-drop fault injection drops undirected edges and does not "
+                              f"apply to the directed graph {g['type']!r}")
 
 
 def load_experiment(yaml_pth: str, kind: str) -> Dict[str, Any]:

@@ -28,15 +28,34 @@ import torch
 # --------------------------------------------------------------------------
 def adjacency(graph: nx.Graph) -> np.ndarray:
     """Boolean adjacency [N, N] with nodes taken in ``range(N)`` order and the
-    diagonal cleared (self loops never carry a mixing weight)."""
+    diagonal cleared (self loops never carry a mixing weight).  An undirected
+    graph gives a symmetric matrix; a ``DiGraph`` keeps its direction
+    (``adj[u, v]`` for the edge ``u -> v``)."""
     n = graph.number_of_nodes()
     adj = np.zeros((n, n), dtype=bool)
     if graph.number_of_edges():
         e = np.asarray(list(graph.edges()), dtype=np.int64)
         adj[e[:, 0], e[:, 1]] = True
-        adj[e[:, 1], e[:, 0]] = True
+        if not graph.is_directed():
+            adj[e[:, 1], e[:, 0]] = True
     np.fill_diagonal(adj, False)
     return adj
+
+
+def push_weights_from_adjacency(adj: np.ndarray) -> np.ndarray:
+    """Column-stochastic push-sum matrix (float64): ``A_ij = 1 / (d_out(j) + 1)``
+    for every edge ``j -> i`` and for ``i = j``.  Each node sets its column from
+    its own out-degree, so no node needs to know anything about the others."""
+    adj = np.asarray(adj, dtype=bool)
+    inv = 1.0 / (adj.sum(1).astype(np.float64) + 1.0)      # per sender j: 1 / (d_out(j) + 1)
+    a = np.where(adj.T, inv[None, :], 0.0)
+    a[np.diag_indices_from(a)] = inv
+    return a
+
+
+def is_strongly_connected_adj(adj: np.ndarray) -> bool:
+    """Every node reaches every other along the edges' direction."""
+    return is_connected_adj(adj) and is_connected_adj(np.asarray(adj).T)
 
 
 def metropolis_from_adjacency(adj: np.ndarray, degs: np.ndarray | None = None) -> np.ndarray:
@@ -160,13 +179,43 @@ def disk_with_fied(N, targ, num_restarts=50, tol=0.01, rng: random.Random | None
     raise NameError("Never found a viable graph!")
 
 
+DIRECTED_TYPES = ("directed_cycle", "exponential", "random_directed")
+
+
 def generate_from_conf(graph_conf) -> Tuple[int, nx.Graph]:
     """Build a graph from a YAML ``graph:`` block (reference :69-104).
     Types: wheel | cycle | complete | random (+ ``p``, ``gen_attempts``), and —
-    new here — ``path``, ``star``, ``disk`` (``target_fied``)."""
+    new here — ``path``, ``star``, ``disk`` (``target_fied``) and the directed
+    ``directed_cycle`` (``i -> i+1``), ``exponential`` (``i -> i + 2^m mod N``
+    for every ``2^m < N``) and ``random_directed`` (``p``, ``seed``,
+    ``gen_attempts``: strongly connected).  Directed graphs (``DIRECTED_TYPES``)
+    are an ``nx.DiGraph``; an edge ``u -> v`` means v reads u's row."""
     N = int(graph_conf["num_nodes"])
     kind = graph_conf["type"]
-    if kind == "wheel":
+    if kind == "directed_cycle":
+        graph = nx.DiGraph()
+        graph.add_nodes_from(range(N))
+        graph.add_edges_from((i, (i + 1) % N) for i in range(N) if N > 1)
+    elif kind == "exponential":
+        graph = nx.DiGraph()
+        graph.add_nodes_from(range(N))
+        m = 1
+        while m < N:
+            graph.add_edges_from((i, (i + m) % N) for i in range(N))
+            m *= 2
+    elif kind == "random_directed":
+        seed = graph_conf.get("seed", None)
+        graph = nx.gnp_random_graph(N, graph_conf["p"], seed=seed, directed=True)
+        for k in range(int(graph_conf["gen_attempts"])):
+            if nx.is_strongly_connected(graph):
+                break
+            graph = nx.gnp_random_graph(N, graph_conf["p"], seed=None if seed is None else seed + k + 1, directed=True)
+        if not nx.is_strongly_connected(graph):
+            raise NameError(
+                "A strongly connected random directed graph could not be generated,"
+                " increase p or gen_attempts."
+            )
+    elif kind == "wheel":
         graph = nx.wheel_graph(N)
     elif kind == "cycle":
         graph = nx.cycle_graph(N)
@@ -220,6 +269,12 @@ def gen_delaunay(N):
 # --------------------------------------------------------------------------
 # Topology: cached per-graph tables used by the optimizers / kernels
 # --------------------------------------------------------------------------
+def topology_key(graph: nx.Graph, adj: np.ndarray | None = None) -> bytes:
+    """Identifies the edge set; a directed graph never shares a key with an undirected one."""
+    adj = adjacency(graph) if adj is None else adj
+    return (b"D" if graph.is_directed() else b"") + adj.tobytes()
+
+
 class Topology:
     """Immutable view of one communication graph.
 
@@ -228,28 +283,49 @@ class Topology:
     ``W`` is the float64 Metropolis matrix; ``key`` identifies the edge set so
     callers can cache device tables across rounds (the reference rebuilds W
     every round, SURVEY Q2).
+
+    Every topology also has ``push_weights``, the column-stochastic float64
+    matrix ``A_ij = 1 / (d_out(j) + 1)`` of push-sum (SGP), and ``readers[i]``,
+    the nodes that read node i's row.  For an undirected graph ``readers`` are
+    the neighbors.  For an ``nx.DiGraph`` (``directed``) ``neighbors`` and
+    ``neighbors_noself`` are the in-neighbors (the nodes i pulls from),
+    ``readers`` the out-neighbors, ``deg`` the in-degrees, and ``W`` is
+    ``None``: Metropolis weights are undefined on a directed graph.
     """
 
     def __init__(self, graph: nx.Graph):
         self.graph = graph
         self.N = graph.number_of_nodes()
+        self.directed = graph.is_directed()
         self.adj = adjacency(graph)
+        pull = graph.predecessors if self.directed else graph.neighbors
         self.neighbors: List[List[int]] = [
-            [int(j) for j in graph.neighbors(i)] for i in range(self.N)
+            [int(j) for j in pull(i)] for i in range(self.N)
         ]
         # consensus kernels never treat a node as its own neighbor; the
         # reference would (cycle_graph(1)), which is a no-op for every update.
         self.neighbors_noself = [[j for j in nb if j != i] for i, nb in enumerate(self.neighbors)]
         self.deg = np.asarray([len(nb) for nb in self.neighbors_noself], dtype=np.int64)
-        self.W = metropolis_from_adjacency(self.adj, laplacian_degrees(graph))
-        self.key = self.adj.tobytes()
+        if self.directed:
+            self.readers = [[int(j) for j in graph.successors(i) if j != i] for i in range(self.N)]
+            self.W = None
+        else:
+            self.readers = self.neighbors_noself
+            self.W = metropolis_from_adjacency(self.adj, laplacian_degrees(graph))
+        self.push_weights = push_weights_from_adjacency(self.adj)
+        self.key = topology_key(graph, self.adj)
 
     @property
     def max_degree(self) -> int:
         return int(self.deg.max()) if self.N else 0
 
+    @property
+    def max_readers(self) -> int:
+        return max((len(r) for r in self.readers), default=0)
+
     def is_connected(self) -> bool:
-        return is_connected_adj(self.adj)
+        """Connected; strongly connected for a directed graph."""
+        return is_strongly_connected_adj(self.adj) if self.directed else is_connected_adj(self.adj)
 
     def is_complete(self) -> bool:
         return self.N > 1 and bool((self.deg == self.N - 1).all())
@@ -271,7 +347,7 @@ class TopologyCache:
         self._by_key: Dict[bytes, Topology] = {}
 
     def get(self, graph: nx.Graph) -> Topology:
-        key = adjacency(graph).tobytes()
+        key = topology_key(graph)
         topo = self._by_key.get(key)
         if topo is None:
             topo = Topology(graph)
