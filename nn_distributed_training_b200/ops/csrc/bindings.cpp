@@ -94,6 +94,7 @@ static consensus::Common<T> common_from(const py::dict& d) {
   c.nbr_ptr = ptr<const int64_t>(d, "nbr_ptr"); c.nbr_w = ptr<const T>(d, "nbr_w");
   c.self_w = ptr<const T>(d, "self_w"); c.deg = ptr<const int>(d, "deg");
   c.nbr_rank = ptr<const int>(d, "nbr_rank"); c.dmax = geti(d, "dmax");
+  c.rdr_deg = ptr<const int>(d, "rdr_deg"); c.rdr_rank = ptr<const int>(d, "rdr_rank"); c.rmax = geti(d, "rmax", 1);
   c.round_ctr = ptr<int>(d, "round_ctr");
   c.rho = ptr<const T>(d, "rho"); c.lr = ptr<const T>(d, "lr"); c.alpha = ptr<const T>(d, "alpha");
   c.graph_id = ptr<const int>(d, "graph_id");
@@ -126,7 +127,6 @@ struct ConsensusOp {
     dn.c = c; gt.c = c; ed.c = c; ch.c = c; sg.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
-    sg.rdr_deg = ptr<const int>(d, "rdr_deg"); sg.rdr_rank = ptr<const int>(d, "rdr_rank"); sg.rmax = geti(d, "rmax", 1);
     ed.psi = ptr<T>(d, "psi");
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
@@ -164,8 +164,8 @@ struct ConsensusOp {
     check(consensus::launch_choco_step<T>(ch, cur_stream()), "choco_step");
   }
   void sgp_check(const char* what) const {
-    if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0 || sg.rdr_deg == nullptr || sg.rdr_rank == nullptr)
-      throw std::runtime_error(std::string(what) + " needs the SGP rows `x`, `w`, `row_stride` and the reader tables");
+    if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0)
+      throw std::runtime_error(std::string(what) + " needs the SGP rows `x`, `w` and `row_stride`");
   }
   void sgp_mix() {
     sgp_check("sgp_mix");

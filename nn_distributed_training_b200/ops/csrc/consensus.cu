@@ -616,7 +616,7 @@ __global__ void __launch_bounds__(THREADS) sgp_mix_kernel(const SgpArgs<T> a) {
   const int l = node_of_block(c);
   const RoundInfo<T> ri = round_info(c);
   const int deg = c.deg[ri.gid * c.L + l];
-  begin_sgp_round(a, ri.gid, l, ri.k);
+  begin_round(c, ri.gid, l, ri.k);
   const T ws = c.self_w[ri.gid * c.L + l];
   const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
   // the new push-sum weight, from the node's own published row (a.w[l] is stored below): every CTA of the node sums

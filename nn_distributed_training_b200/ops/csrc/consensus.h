@@ -31,6 +31,11 @@ struct Common {
   const int* deg;             // [G, L]
   const int* nbr_rank;        // [G, L, dmax] owning rank of each neighbor, -1 when local
   int dmax;
+  // readers of each local node: the nodes that pull its row (its out-neighbors), which wait_neighbors also waits for.
+  // rdr_deg == nullptr: every planned graph is undirected, the readers are the neighbors (deg, nbr_rank, dmax)
+  const int* rdr_deg;         // [G, L] or nullptr
+  const int* rdr_rank;        // [G, L, rmax] owning rank of each reader, -1 when local
+  int rmax;
   // device-side schedules
   int* round_ctr;             // [1]
   const T* rho; const T* lr; const T* alpha;   // [oits]
@@ -118,17 +123,13 @@ struct ChocoArgs {
 // The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
 // A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
 // `row_stride` = n_pad * sizeof(T) + 16 bytes.  theta = x / w is the de-biased row the forward/backward kernel reads.
-// Node i overwrites its row of parity (k+1)&1 at the end of round k; its round-(k-1) readers are its out-neighbors,
-// which on a directed graph are not the ranks it pulls from, so the SGP kernels also wait for them (rdr_rank).
+// A plan with a directed graph carries reader tables (Common::rdr_deg): the round-start wait covers the out-neighbors.
 template <typename T>
 struct SgpArgs {
   Common<T> c;
   T* x;                            // [L, n_pad] numerators
   double* w;                       // [L] push-sum weights
   long long row_stride;            // bytes per published row
-  const int* rdr_deg;              // [G, L] readers (out-neighbors) of each local node
-  const int* rdr_rank;             // [G, L, rmax] owning rank of each reader, -1 when local
-  int rmax;
 };
 
 // Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient

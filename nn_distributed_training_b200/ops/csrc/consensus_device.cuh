@@ -76,12 +76,18 @@ NNDT_DEVINL void wait_rank(const Common<T>& c, int r, int k) {
   }
 }
 
-// Wait until every rank owning a neighbor of local node l has published round k; with the sequence check enabled,
-// also verify that the row about to be read is tagged with round k.
-// Buffer reuse on time-varying graphs: this node overwrites pub[(k+1)&1] at the end of round k, the buffer its
-// round-(k-1) neighbors read during round k-1.  A rank publishes round k only after its round-(k-1) reads, so also
-// waiting for "round k published" from the ranks of the round-(k-1) neighbors (a no-op on static graphs: same set)
-// closes the write-after-read window without a separate "consumed" counter.
+// Round-start wait of local node l, for directed and undirected graphs alike.
+//  1. threads 0..deg-1: every rank owning an in-neighbor of l in graph `gid` has published round k; with the sequence
+//     check enabled, also verify that the row about to be read is tagged with round k.
+//  2. threads 32.. (k > 0): every rank owning a round-(k-1) reader of l has published round k.  Node l overwrites
+//     pub[(k+1)&1] at the end of round k, the buffer its round-(k-1) readers read during round k-1.  A rank publishes
+//     round k only after its round-(k-1) reads, so this wait closes the write-after-read window without a separate
+//     "consumed" counter (tests/test_protocol_model.py, tests/test_protocol_model_directed.py).
+// The readers of l are its out-neighbors.  With a directed graph in the plan they are not the nodes l pulls from and
+// come from the reader tables (rdr_deg, rdr_rank).  Without reader tables every graph is undirected, the readers are
+// the neighbors of graph_id[k-1], and step 2 is skipped when that graph is `gid`: step 1 waited for the same ranks.
+// (Step 2 picks the rank in two branches and waits once: with the table pointers selected first,
+// dinno_update_kernel<double, 16> compiled to 246 registers instead of 168.)
 template <typename T>
 NNDT_DEVINL void wait_neighbors(const Common<T>& c, int gid, int l, int k) {
   const bool check = c.nbr_seq != nullptr;
@@ -96,14 +102,14 @@ NNDT_DEVINL void wait_neighbors(const Common<T>& c, int gid, int l, int k) {
       }
     }
     if (c.world > 1 && k > 0) {
-      const int gp = c.graph_id[k - 1];
-      if (gp != gid) {
-        const int t = (int)threadIdx.x - 32;                  // a different warp than the current-graph waiters
-        if (t >= 0 && t < c.deg[gp * c.L + l]) {
-          const int r = c.nbr_rank[(gp * c.L + l) * c.dmax + t];
-          if (r >= 0) wait_rank(c, r, k);
-        }
+      const int gp = c.graph_id[k - 1], t = (int)threadIdx.x - 32;   // a different warp than the in-neighbor waiters
+      int r = -1;
+      if (c.rdr_deg != nullptr) {
+        if (t >= 0 && t < c.rdr_deg[gp * c.L + l]) r = c.rdr_rank[(gp * c.L + l) * c.rmax + t];
+      } else if (gp != gid) {
+        if (t >= 0 && t < c.deg[gp * c.L + l]) r = c.nbr_rank[(gp * c.L + l) * c.dmax + t];
       }
+      if (r >= 0) wait_rank(c, r, k);
     }
     __syncthreads();
   }
@@ -382,44 +388,6 @@ NNDT_DEVINL double row_weight(const T* row, int n_pad) {
 template <typename T>
 NNDT_DEVINL T sgp_debias(T x, double w) {
   return div_rn(x, (T)w);
-}
-
-// wait_neighbors for a directed graph.  Node l overwrites its row of parity (k+1)&1 at the end of round k; the nodes
-// that read that buffer in round k-1 are l's round-(k-1) out-neighbors (readers), which on a directed graph are not the
-// in-neighbors l pulls from.  A rank publishes round k only after its round-(k-1) reads, so waiting for "round k
-// published" from the ranks of in_k(l) and out_{k-1}(l) closes the write-after-read window (tests/
-// test_protocol_model_directed.py).  On an undirected graph the set is wait_neighbors' N_k and N_{k-1}.
-template <typename T>
-NNDT_DEVINL void wait_in_and_readers(const SgpArgs<T>& a, int gid, int l, int k) {
-  const Common<T>& c = a.c;
-  const bool check = c.nbr_seq != nullptr;
-  if (c.world > 1 || check) {
-    const int d = c.deg[gid * c.L + l];
-    if ((int)threadIdx.x < d) {
-      const int r = c.world > 1 ? c.nbr_rank[(gid * c.L + l) * c.dmax + threadIdx.x] : -1;
-      if (r >= 0) wait_rank(c, r, k);
-      if (check) {
-        const int* tag = reinterpret_cast<const int*>(c.nbr_seq[((size_t)(gid * c.L + l) * c.dmax + threadIdx.x) * 2 + (k & 1)]);
-        if (ld_acquire_sys(tag) != k) *c.err = 2;
-      }
-    }
-    if (c.world > 1 && k > 0) {
-      const int gp = c.graph_id[k - 1];
-      const int t = (int)threadIdx.x - 32;                    // a different warp than the in-neighbor waiters
-      if (t >= 0 && t < a.rdr_deg[gp * c.L + l]) {
-        const int r = a.rdr_rank[(gp * c.L + l) * a.rmax + t];
-        if (r >= 0) wait_rank(c, r, k);
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// begin_round of the SGP mix: announce round k, then wait for in_k(l) and out_{k-1}(l)
-template <typename T>
-NNDT_DEVINL void begin_sgp_round(const SgpArgs<T>& a, int gid, int l, int k) {
-  if (a.c.world > 1 && blockIdx.x == 0 && blockIdx.y == 0) announce_round(a.c, k);
-  wait_in_and_readers(a, gid, l, k);
 }
 
 }  // namespace consensus

@@ -45,6 +45,17 @@ def schedule_tables(opt, H: int):
     return rho, lr, alpha
 
 
+WAIT_THREADS = 256     # consensus_device.cuh: THREADS
+
+
+def check_wait_capacity(dmax: int, rmax: int) -> None:
+    """The round-start wait has one thread per in-neighbor (threads ``0..dmax-1`` of a node's CTA) and one per reader
+    of the previous round (``32..32+rmax-1``); a node with more would go on without waiting for the last of them."""
+    if dmax > WAIT_THREADS or rmax > WAIT_THREADS - 32:
+        raise ValueError(f"a node with {dmax} in-neighbors / {rmax} readers exceeds what the consensus kernels wait "
+                         f"for ({WAIT_THREADS} in-neighbors, {WAIT_THREADS - 32} readers)")
+
+
 class ConsensusEngine:
     def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
@@ -117,11 +128,18 @@ class ConsensusEngine:
             raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
                              f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
         dmax = max(1, max(t.max_degree for t in topos))
+        # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
+        # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
+        directed = any(t.directed for t in topos)
+        rmax = max(1, max(t.max_readers for t in topos))
+        check_wait_capacity(dmax, rmax if directed or G > 1 else 0)    # a static undirected graph has no second wait
         nbr_ptr = np.zeros((G, L, dmax, 2, self.C), dtype=np.int64)
         nbr_w = np.zeros((G, L, dmax), dtype=npdt)
         self_w = np.zeros((G, L), dtype=npdt)
         deg = np.zeros((G, L), dtype=np.int32)
         nbr_rank = -np.ones((G, L, dmax), dtype=np.int32)
+        rdr_deg = np.zeros((G, L), dtype=np.int32) if directed else None
+        rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
             # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
             # push-sum weights, over the in-neighbors
@@ -142,6 +160,11 @@ class ConsensusEngine:
                         for ch in range(self.C):
                             row = (par * self.C + ch) * self.Lpub + lj
                             nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
+                if directed:
+                    rdr_deg[gi, l] = len(t.readers[g])
+                    for e, j in enumerate(t.readers[g]):
+                        if int(pl.node_rank[j]) != ctx.rank:
+                            rdr_rank[gi, l, e] = int(pl.node_rank[j])
         self.dmax = dmax
         self.t_nbr_ptr = torch.as_tensor(nbr_ptr, device=dev)
         self.t_nbr_w = torch.as_tensor(nbr_w, device=dev)
@@ -149,21 +172,8 @@ class ConsensusEngine:
         self.t_deg = torch.as_tensor(deg, device=dev)
         self.t_nbr_rank = torch.as_tensor(nbr_rank, device=dev)
         self.t_gid = torch.as_tensor(gid, device=dev)
-        # SGP: the ranks that read each local node's row (its out-neighbors), which the mix also waits for
-        self.t_rdr_deg = self.t_rdr_rank = None
-        rdr_rank = -np.ones((G, L, 1), dtype=np.int32)
-        if self.sgp:
-            rmax = max(1, max(t.max_readers for t in topos))
-            rdr_deg = np.zeros((G, L), dtype=np.int32)
-            rdr_rank = -np.ones((G, L, rmax), dtype=np.int32)
-            for gi, t in enumerate(topos):
-                for l, g in enumerate(pl.local_nodes):
-                    rdr_deg[gi, l] = len(t.readers[g])
-                    for e, j in enumerate(t.readers[g]):
-                        if int(pl.node_rank[j]) != ctx.rank:
-                            rdr_rank[gi, l, e] = int(pl.node_rank[j])
-            self.t_rdr_deg = torch.as_tensor(rdr_deg, device=dev)
-            self.t_rdr_rank = torch.as_tensor(rdr_rank, device=dev)
+        self.t_rdr_deg = torch.as_tensor(rdr_deg, device=dev) if directed else None
+        self.t_rdr_rank = torch.as_tensor(rdr_rank, device=dev) if directed else None
 
         # ---- optional protocol self-check (SURVEY 5.2): published rows carry their round, neighbor reads verify it ----
         self.seq_buf = None
@@ -196,8 +206,9 @@ class ConsensusEngine:
         # ranks that own a neighbor of a local node in ANY round's graph: the only ones that need this rank's flags
         notify = 0
         remote_node = np.zeros(L, dtype=bool)
-        # (SGP: also the ranks of the in-neighbors, which wait for this rank as one of their readers)
-        for r in np.unique(np.concatenate([nbr_rank[nbr_rank >= 0], rdr_rank[rdr_rank >= 0]])):
+        # (directed graphs: the in-neighbors wait for this rank as one of their readers, the readers as an in-neighbor)
+        peers = np.concatenate([nbr_rank.ravel(), rdr_rank.ravel()]) if directed else nbr_rank
+        for r in np.unique(peers[peers >= 0]):
             notify |= 1 << int(r)
         for l in range(L):
             remote_node[l] = bool((nbr_rank[:, l, :] >= 0).any())
@@ -259,13 +270,14 @@ class ConsensusEngine:
             d["timeline"] = self.timeline.data_ptr()
         # the C++ side indexes pub rows with stride L; when ranks host different node counts the
         # published buffer is allocated with the max count, so pass that as the row count of pub
-        d["L"] = L
         d["pub_L"] = self.Lpub
         if pr.fused is not None and getattr(pr, "track_tloss", False) and self.dtype == torch.float32:
             # the kernel that consumes a gradient also folds that step's loss into the EMA tracker
             d.update(loss_part=pr.fused.loss_part.data_ptr(), tloss=pr.tloss_local.data_ptr(),
                      tdecay=float(pr.tloss_decay), loss_S=int(pr.fused.loss_part.shape[1]))
             pr.fused.ema_in_kernel = True
+        if directed:
+            d.update(rdr_deg=self.t_rdr_deg.data_ptr(), rdr_rank=self.t_rdr_rank.data_ptr(), rmax=rmax)
         if self.seq_buf is not None:
             d.update(pub_seq=self.seq_buf.local.data_ptr(), nbr_seq=self.t_nbr_seq.data_ptr())
         if self.sum_mode:
@@ -287,9 +299,7 @@ class ConsensusEngine:
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
                      code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
         if self.sgp:
-            d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes),
-                     rdr_deg=self.t_rdr_deg.data_ptr(), rdr_rank=self.t_rdr_rank.data_ptr(),
-                     rmax=int(self.t_rdr_rank.shape[2]))
+            d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d

@@ -1,6 +1,6 @@
-"""Model check of the publication protocol on directed graphs (ops/csrc/consensus_device.cuh: begin_sgp_round /
-wait_in_and_readers), in the style of tests/test_protocol_model.py — CPU only, no kernels: every rank is a small state
-machine and all interleavings of a few rounds are explored.
+"""Model check of the publication protocol on directed graphs (ops/csrc/consensus_device.cuh: begin_round /
+wait_neighbors with reader tables), with the explorer of tests/test_protocol_model.py — CPU only, no kernels: every
+rank is a small state machine and all interleavings of a few rounds are explored.
 
 Protocol of rank r in round k (published rows double buffered by round parity), on a directed graph where r pulls from
 its in-neighbors in_k(r) and its row is read by its out-neighbors out_k(r):
@@ -12,77 +12,13 @@ Safety: every read returns the row of round k; liveness: no deadlock."""
 import itertools
 import random
 
-import test_protocol_model as undirected
-
-
-def explore_sets(reads, waits, n_ranks, announce_at_start=True, max_states=400_000):
-    """DFS over all interleavings of the protocol with explicit sets: rank r reads ``reads[k][r]`` in round k after
-    waiting for "round k published" from ``waits[k][r]``.  The state machine and search order are those of
-    ``test_protocol_model.explore``, which computes its wait set inside (N_k, plus N_{k-1} with ``wait_prev``);
-    ``test_the_state_machine_is_the_undirected_models`` holds the two to the same results.  Returns
-    (violation, deadlock, n_states)."""
-    K = len(reads)
-
-    def program(r):
-        steps = []
-        for k in range(K):
-            if announce_at_start:
-                steps.append(("announce", k))
-            steps.append(("wait", k, tuple(sorted(waits[k][r]))))
-            for j in sorted(reads[k][r]):
-                steps.append(("read", k, j))
-            steps.append(("write", k))
-            if not announce_at_start:
-                steps.append(("announce", k + 1))
-        return steps
-
-    progs = [program(r) for r in range(n_ranks)]
-    init = (tuple(0 for _ in range(n_ranks)), tuple(0 for _ in range(n_ranks)),
-            tuple((0, -1) for _ in range(n_ranks)))
-    seen = {init}
-    stack = [init]
-    while stack and len(seen) < max_states:
-        pcs, flags, pubs = stack.pop()
-        progressed = False
-        done = True
-        for r in range(n_ranks):
-            if pcs[r] >= len(progs[r]):
-                continue
-            done = False
-            st = progs[r][pcs[r]]
-            nflags, npubs = flags, pubs
-            if st[0] == "announce":
-                nflags = flags[:r] + (max(flags[r], st[1]),) + flags[r + 1:]
-            elif st[0] == "wait":
-                if any(flags[j] < st[1] for j in st[2]):
-                    continue
-            elif st[0] == "read":
-                k, j = st[1], st[2]
-                if pubs[j][k & 1] != k:
-                    return (r, k, j, pubs[j][k & 1]), None, len(seen)
-            elif st[0] == "write":
-                k = st[1]
-                p = list(pubs[r])
-                p[(k + 1) & 1] = k + 1
-                npubs = pubs[:r] + (tuple(p),) + pubs[r + 1:]
-            progressed = True
-            nxt = (pcs[:r] + (pcs[r] + 1,) + pcs[r + 1:], nflags, npubs)
-            if nxt not in seen:
-                seen.add(nxt)
-                stack.append(nxt)
-        if not done and not progressed:
-            return None, (pcs, flags), len(seen)
-    return None, None, len(seen)
+from test_protocol_model import directed_waits, explore_sets
 
 
 def explore(ins, n_ranks, wait_readers, announce_at_start=True, max_states=400_000):
     """The directed protocol: ins[k][r] = in-neighbor ranks of r in round k; r waits for in_k(r), and with
-    ``wait_readers`` also for out_{k-1}(r) (wait_in_and_readers)."""
-    K = len(ins)
-    outs = [[{j for j in range(n_ranks) if r in ins[k][j]} for r in range(n_ranks)] for k in range(K)]
-    waits = [[set(ins[k][r]) | (outs[k - 1][r] if (wait_readers and k > 0) else set()) for r in range(n_ranks)]
-             for k in range(K)]
-    return explore_sets(ins, waits, n_ranks, announce_at_start, max_states)
+    ``wait_readers`` also for out_{k-1}(r)."""
+    return explore_sets(ins, directed_waits(ins, n_ranks, wait_readers), n_ranks, announce_at_start, max_states)
 
 
 def _ring(n):
@@ -123,22 +59,6 @@ def test_on_undirected_graphs_the_set_is_the_union_wait():
 
 
 MAX_RANDOM = 200_000
-
-
-def test_the_state_machine_is_the_undirected_models():
-    """With the undirected wait set (N_k, plus N_{k-1}), ``explore_sets`` gives exactly what
-    ``test_protocol_model.explore`` gives on that model's cases: the same hazard, the same verdicts, the same number
-    of states searched."""
-    ring = [undirected._sym(4, [(0, 1), (1, 2), (2, 3), (3, 0)])] * 3
-    for graphs, n in ((undirected.DYNAMIC, 3), (ring, 4)):
-        for wait_prev in (False, True):
-            for at_start in (True, False):
-                K = len(graphs)
-                waits = [[set(graphs[k][r]) | (set(graphs[k - 1][r]) if (wait_prev and k > 0) else set())
-                          for r in range(n)] for k in range(K)]
-                got = explore_sets(graphs, waits, n, announce_at_start=at_start, max_states=300_000)
-                want = undirected.explore(graphs, n, wait_prev, announce_at_start=at_start, max_states=300_000)
-                assert got == want, (n, wait_prev, at_start, got, want)
 
 
 def test_random_time_varying_digraphs_random_schedules():
