@@ -253,6 +253,27 @@ def sgp_step_(x: torch.Tensor, w: torch.Tensor, theta: torch.Tensor, grad: torch
     theta.copy_(sgp_debias(x, w))
 
 
+# ---------------------------------------------------------- Push-DIGing ----
+# Gradient tracking on push-sum gossip: numerators u [L, n_pad], float64 weights w [L], trackers y [L, n_pad].  SGP's
+# rounding rules: the weights of A rounded to the arena dtype, w mixed in float64 with those rounded weights, and
+# theta = u / w by sgp_debias.
+def pdg_mix_(u: torch.Tensor, w: torch.Tensor, theta: torch.Tensor, ysum: torch.Tensor, u_all: torch.Tensor,
+             y_all: torch.Tensor, w_all: torch.Tensor, a_rows: torch.Tensor, alpha: float):
+    """``u_i <- sum_j A_ij (u_j - alpha y_j)``, ``ysum_i <- sum_j A_ij y_j``, ``w_i <- sum_j A_ij w_j`` (own terms
+    included), ``theta_i <- u_i / w_i``."""
+    a = a_rows.to(u_all.dtype)
+    u.copy_(a @ (u_all - alpha * y_all))
+    ysum.copy_(a @ y_all)
+    w.copy_(a.to(torch.float64) @ w_all.to(torch.float64))
+    theta.copy_(sgp_debias(u, w))
+
+
+def pdg_track_(y: torch.Tensor, g_old: torch.Tensor, ysum: torch.Tensor, grad: torch.Tensor):
+    """``y <- ysum + (g - g_old)``, ``g_old <- g`` (g taken at theta = u / w)."""
+    y.copy_(ysum + (grad - g_old))
+    g_old.copy_(grad)
+
+
 # ------------------------------------------------------------- metrics ----
 def consensus_error(theta_all: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Pairwise and to-mean distances of L2-normalised parameter rows

@@ -122,11 +122,14 @@ struct ConsensusOp {
   consensus::EdArgs<T> ed{};
   consensus::ChocoArgs<T> ch{};
   consensus::SgpArgs<T> sg{};
+  consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; ch.c = c; sg.c = c;
+    dn.c = c; gt.c = c; ed.c = c; ch.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
+    pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
+    pd.row_stride = sg.row_stride;
     ed.psi = ptr<T>(d, "psi");
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
@@ -175,6 +178,19 @@ struct ConsensusOp {
     sgp_check("sgp_step");
     check(consensus::launch_sgp_step<T>(sg, cur_stream()), "sgp_step");
   }
+  void pdg_check(const char* what) const {
+    if (pd.u == nullptr || pd.w == nullptr || pd.ysum == nullptr || pd.g_old == nullptr || pd.row_stride <= 0 || c.C != 2)
+      throw std::runtime_error(std::string(what) + " needs the Push-DIGing rows `u`, `w`, `ysum`, `g_old`, `row_stride` "
+                               "and two published channels");
+  }
+  void pdg_mix() {
+    pdg_check("pdg_mix");
+    check(consensus::launch_pdg_mix<T>(pd, cur_stream()), "pdg_mix");
+  }
+  void pdg_track() {
+    pdg_check("pdg_track");
+    check(consensus::launch_pdg_track<T>(pd, cur_stream()), "pdg_track");
+  }
 };
 
 // local optimizer step of non-communicating nodes (solo / centralized baselines)
@@ -210,7 +226,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("choco_mix", &ConsensusOp<T>::choco_mix)
       .def("choco_step", &ConsensusOp<T>::choco_step)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
-      .def("sgp_step", &ConsensusOp<T>::sgp_step);
+      .def("sgp_step", &ConsensusOp<T>::sgp_step)
+      .def("pdg_mix", &ConsensusOp<T>::pdg_mix)
+      .def("pdg_track", &ConsensusOp<T>::pdg_track);
 }
 
 void bind_mlp(py::module& m);     // mlp_bind.cpp

@@ -1,5 +1,5 @@
 // Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion /
-// CHOCO-SGD / SGP.
+// CHOCO-SGD / SGP / Push-DIGing.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
@@ -8,6 +8,7 @@
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
+// Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
 // Every kernel is a single pass over the node's 16-byte vectorised parameter row: neighbor
 // rows are pulled straight from the (local or NVLink-peer) published buffers named by the
@@ -675,6 +676,94 @@ __global__ void __launch_bounds__(THREADS) sgp_step_kernel(const SgpArgs<T> a) {
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------- Push-DIGing ----
+// Round k: pdg_mix pulls each in-neighbor's u row, y row and w tail of round k once,
+//   u_i <- sum_j A_ij (u_j - alpha y_j),  ysum_i <- sum_j A_ij y_j,  w_i <- sum_j A_ij w_j,  theta_i <- u_i / w_i;
+// pdg_track forms y_i <- ysum_i + (g_i - g_old_i) from the local rows and publishes (u_i, w_i) and y_i.  Every neighbor
+// read of the round happens in the mix, after begin_round, as in SGP.
+template <typename T>
+struct UYPack { Pack<T> u, y; };
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS) pdg_mix_kernel(const PushDigArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T alpha = c.alpha[ri.k];
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const T* ys = pdg_row(a, ri.par, 1, l);
+  // the new push-sum weight, summed in one order by every CTA of the node (as in sgp_mix): all divide by the same bits
+  double wn = (double)ws * row_weight(pdg_row(a, ri.par, 0, l), c.n_pad);
+  for_neighbors<4>(deg, [&](int e) { return row_weight(nbr_row(c, ri.gid, l, e, ri.par, 0), c.n_pad); },
+                   [&](int e, double q) { wn += (double)w[e] * q; });
+  if (blockIdx.x == 0 && threadIdx.x == 0) a.w[l] = wn;
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> y = ldv(ys + i);
+    Pack<T> u = ldv(a.u + row + i), s;
+#pragma unroll
+    for (int v = 0; v < N; ++v) {
+      u.v[v] = ws * (u.v[v] - alpha * y.v[v]);
+      s.v[v] = ws * y.v[v];
+    }
+    for_neighbors<2>(deg,
+                     [&](int e) {
+                       return UYPack<T>{ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i),
+                                        ldv(nbr_row(c, ri.gid, l, e, ri.par, 1) + i)};
+                     },
+                     [&](int e, const UYPack<T>& q) {
+                       const T we = w[e];
+#pragma unroll
+                       for (int v = 0; v < N; ++v) {
+                         u.v[v] += we * (q.u.v[v] - alpha * q.y.v[v]);
+                         s.v[v] += we * q.y.v[v];
+                       }
+                     });
+    Pack<T> th;
+#pragma unroll
+    for (int v = 0; v < N; ++v) th.v[v] = sgp_debias(u.v[v], wn);
+    stv(a.u + row + i, u);
+    stv(c.theta + row + i, th);
+    stv(a.ysum + row + i, s);
+  }
+}
+
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) pdg_track_kernel(const PushDigArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const size_t row = (size_t)l * c.n_pad;
+  T* ou = pdg_row(a, ri.par ^ 1, 0, l);
+  T* oy = pdg_row(a, ri.par ^ 1, 1, l);
+  // u, ysum and w (written by the mix two launches back) and g_old (the previous round) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  const double wn = a.w[l];
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> u = ldv(a.u + row + i);
+    Pack<T> y = ldv(a.ysum + row + i);
+    const Pack<T> go = ldv(a.g_old + row + i);
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+    for (int v = 0; v < N; ++v) y.v[v] += g.v[v] - go.v[v];
+    stv(a.g_old + row + i, g);
+    stv(oy + i, y);
+    stv(ou + i, u);
+  }
+  release_dependents_once(waited);
+  if (blockIdx.x == 0 && threadIdx.x == 0) *reinterpret_cast<double*>(ou + c.n_pad) = wn;
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------------------ consensus metric ----
 NNDT_DEVINL double block_sum(double v) {
   __shared__ double red[THREADS / 32];
@@ -863,6 +952,14 @@ template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStrea
   return launch_by_s(sgp_step_kernel<T, 4>, sgp_step_kernel<T, 8>, a.c, a, st);
 }
 
+template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(pdg_mix_kernel<T>, a.c, a, st);
+}
+// beyond 4 gradient partials the track keeps 8 loads in flight, as sgp_step: 16 spilled in fp32
+template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(pdg_track_kernel<T, 4>, pdg_track_kernel<T, 8>, a.c, a, st);
+}
+
 #define NNDT_INST(T)                                                                  \
   template cudaError_t launch_local_sum<T>(const Common<T>&, cudaStream_t);           \
   template cudaError_t launch_consensus_metric<T>(const int64_t*, int, int, int, int, double*, double*, double*, cudaStream_t); \
@@ -878,7 +975,9 @@ template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStrea
   template cudaError_t launch_choco_mix<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
-  template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);
+  template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_pdg_mix<T>(const PushDigArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_pdg_track<T>(const PushDigArgs<T>&, cudaStream_t);
 NNDT_INST(float)
 NNDT_INST(double)
 

@@ -132,6 +132,20 @@ struct SgpArgs {
   long long row_stride;            // bytes per published row
 };
 
+// Push-DIGing (Nedić, Olshevsky, Shi 2017): DSGT's gradient tracking on push-sum gossip, for directed and time-varying
+// graphs.  The topology tables are SGP's (in-neighbors, A = push weights).  Two published channels, each row of
+// `row_stride` = n_pad * sizeof(T) + 16 bytes: channel 0 holds the numerators u with the float64 push-sum weight w in
+// its tail, channel 1 the tracker y (its tail is never read).  theta = u / w is the row the forward/backward kernel reads.
+template <typename T>
+struct PushDigArgs {
+  Common<T> c;
+  T* u;                            // [L, n_pad] numerators
+  double* w;                       // [L] push-sum weights
+  T* ysum;                         // [L, n_pad] sum_j A_ij y_j^pub of the round (own term included)
+  T* g_old;                        // [L, n_pad] the gradient of the previous round
+  long long row_stride;            // bytes per published row
+};
+
 // Local optimizer step of nodes that do not communicate (solo and centralized baselines): per node, the gradient
 // partials are summed and one torch.optim SGD / Adam / AdamW step is applied, while c.calls[l] < budget[l].
 // Uses c.L, c.n_pad, c.S, c.theta, c.grad_part and c.calls (the node's step counter, required).
@@ -158,6 +172,8 @@ template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaSt
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_local_sum(const Common<T>& c, cudaStream_t st);
 
 // All-rank barrier on the device (bench start alignment, metric quiescence): every rank stores `epoch` into its slot of

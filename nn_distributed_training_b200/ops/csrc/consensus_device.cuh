@@ -390,5 +390,12 @@ NNDT_DEVINL T sgp_debias(T x, double w) {
   return div_rn(x, (T)w);
 }
 
+// ---- Push-DIGing (layout in consensus.h): row of channel `chan` (0: u with the w tail, 1: y) ----
+template <typename T>
+NNDT_DEVINL T* pdg_row(const PushDigArgs<T>& a, int par, int chan, int l) {
+  const Common<T>& c = a.c;
+  return reinterpret_cast<T*>(reinterpret_cast<char*>(c.pub) + ((size_t)(par * c.C + chan) * c.pub_L + l) * (size_t)a.row_stride);
+}
+
 }  // namespace consensus
 }  // namespace nndt

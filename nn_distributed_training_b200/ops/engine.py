@@ -40,7 +40,7 @@ def schedule_tables(opt, H: int):
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):
+    elif not torch.is_tensor(opt.alpha):     # DSGT and Push-DIGing: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -64,18 +64,21 @@ class ConsensusEngine:
         dev, a, pl, ctx = pr.device, pr.arena, pr.placement, pr.ctx
         self.dtype = a.dtype
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
-        self.C = 2 if opt.alg_name == "dsgt" else 1
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging") else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
         self.sgp = opt.alg_name == "sgp"
+        self.pdg = opt.alg_name == "push_diging"
+        push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
         # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
-        # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w
+        # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w (Push-DIGing: both
+        # channels, u with w in the tail and y, have that stride)
         if self.choco:
             self.row_bytes = opt.code_bytes
-        elif self.sgp:
+        elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
         else:
             self.row_bytes = n_pad * itemsize
@@ -90,6 +93,10 @@ class ConsensusEngine:
         elif self.sgp:
             self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.x)
             self.pub_weights(k0 & 1).copy_(opt.w)
+        elif self.pdg:
+            self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.u)
+            self.pub_weights(k0 & 1).copy_(opt.w)
+            self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if opt.alg_name == "dsgt" and getattr(opt, "_initialised", False):
@@ -142,8 +149,8 @@ class ConsensusEngine:
         rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
             # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
-            # push-sum weights, over the in-neighbors
-            if self.sgp:
+            # push-sum weights, over the in-neighbors (as Push-DIGing)
+            if push_sum:
                 Wt = t.push_weights
             else:
                 Wt = ed_weights(t.W) if opt.alg_name == "exact_diffusion" else t.W
@@ -222,9 +229,9 @@ class ConsensusEngine:
             ctx.barrier()
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
-        # (CHOCO-SGD and SGP always pull through the pointer table: their published rows are codes / numerators with a
-        # weight; complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco and not self.sgp
+        # (CHOCO-SGD, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
+        # numerators with a weight; complete_graph_mode is ignored)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco and not push_sum
                          and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -300,12 +307,16 @@ class ConsensusEngine:
                      code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
         if self.sgp:
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
+        if self.pdg:
+            d.update(u=opt.u.data_ptr(), w=opt.w.data_ptr(), ysum=opt.ysum.data_ptr(), g_old=opt.g.data_ptr(),
+                     row_stride=int(self.row_bytes))
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
         self.op = cls(d)
         self._keep = d
 
     def pub_weights(self, par: int) -> torch.Tensor:
-        """SGP: the float64 push-sum weights in the tails of this rank's published rows of parity ``par`` (a view)."""
+        """SGP, Push-DIGing: the float64 push-sum weights in the tails of this rank's published rows of parity ``par``
+        (channel 0; a view)."""
         tail = self.pr.arena.n_pad * self.pub.element_size()
         rows = self.pub[par, 0, :self.pr.placement.L].view(torch.uint8)
         return rows[:, tail: tail + 8].view(torch.float64)[:, 0]
@@ -313,7 +324,7 @@ class ConsensusEngine:
     def bytes_per_round(self) -> Dict[str, int]:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
         neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
-        counted).  An SGP row includes its 16-byte weight tail."""
+        counted).  An SGP or Push-DIGing row includes its 16-byte tail."""
         deg = int(self.t_deg[0].sum().item())
         return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg}
 

@@ -7,6 +7,7 @@ A round is a short, fixed kernel sequence
     Exact Diffusion:  ed_mix, fwd/bwd, ed_step
     CHOCO-SGD:  choco_mix, fwd/bwd, choco_step
     SGP:  sgp_mix, fwd/bwd, sgp_step
+    Push-DIGing:  pdg_mix, fwd/bwd, pdg_track
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -67,6 +68,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.sgp_mix()
         grads(0)
         eng.op.sgp_step()
+    elif alg == "push_diging":
+        eng.op.pdg_mix()
+        grads(0)
+        eng.op.pdg_track()
     else:  # pragma: no cover
         raise NameError("Unknown distributed opt algorithm.")
 
@@ -110,8 +115,9 @@ class RoundProgram:
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD publishes
-        # codes and SGP numerators, so their metric reads the parameter rows (all_theta) at the evaluation points instead
-        pr._metric_engine = None if (self.eng.choco or self.eng.sgp) else (self.eng, lambda: opt.k)
+        # codes, SGP and Push-DIGing numerators, so their metric reads the parameter rows (all_theta) at the evaluation
+        # points instead
+        pr._metric_engine = None if (self.eng.choco or self.eng.sgp or self.eng.pdg) else (self.eng, lambda: opt.k)
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
         self.pipeline = "resident"
@@ -269,6 +275,8 @@ class RoundProgram:
         if opt.alg_name == "dsgt":
             par = opt.k & 1
             opt.y.copy_(eng.pub[par, 1, :L])
+        if opt.alg_name == "push_diging":       # y is the first n_pad elements of channel 1 (u and w are shared)
+            opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp") and opt.k > 0:

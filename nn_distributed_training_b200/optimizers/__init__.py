@@ -3,10 +3,11 @@ from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
+from .push_diging import PushDIGing
 from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
-              "choco_sgd": ChocoSGD, "sgp": SGP}
+              "choco_sgd": ChocoSGD, "sgp": SGP, "push_diging": PushDIGing}
 
 
 def build_optimizer(problem, device, opt_conf):

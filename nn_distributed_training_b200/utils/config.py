@@ -15,9 +15,10 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd", "sgp")
-# graph types that generate an nx.DiGraph (utils/graph_generation.py); only push-sum SGP runs on them
+ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd", "sgp", "push_diging")
+# graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
+DIRECTED_ALGS = ("sgp", "push_diging")
 CHOCO_COMPRESSORS = ("none", "int8", "sign")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
@@ -35,6 +36,7 @@ OPT_SCHEMA = {
     "choco_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED,
                   "outer_iterations": REQUIRED, "profile": False},
     "sgp": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
+    "push_diging": {"alpha": REQUIRED, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -78,7 +80,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg in ("exact_diffusion", "choco_sgd", "sgp") and c.get("mixing_order", "jacobi") != "jacobi":
+    if alg in ("exact_diffusion", "choco_sgd", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
     if alg == "choco_sgd":
@@ -188,8 +190,8 @@ def validate_experiment(conf: Dict[str, Any], kind: str) -> Dict[str, Any]:
 
 
 def _check_directed_graph(conf: Dict[str, Any]) -> None:
-    """A directed ``experiment.graph`` has no Metropolis matrix: only SGP runs on it, and link-drop fault injection
-    (which drops undirected edges) does not apply to it."""
+    """A directed ``experiment.graph`` has no Metropolis matrix: only the push-sum algorithms (SGP, Push-DIGing) run on
+    it, and link-drop fault injection (which drops undirected edges) does not apply to it."""
     g = conf["experiment"].get("graph")
     if not isinstance(g, dict) or g.get("type") not in DIRECTED_GRAPH_TYPES:
         return
@@ -197,9 +199,9 @@ def _check_directed_graph(conf: Dict[str, Any]) -> None:
     for k, p in probs.items():
         path = f"problem_configs.{k}" if "problem_configs" in conf else k
         alg = p["optimizer_config"]["alg_name"]
-        if alg != "sgp":
-            raise ConfigError(f"experiment.graph.type: the directed graph {g['type']!r} runs with alg_name sgp only "
-                              f"({path}.optimizer_config.alg_name is {alg!r})")
+        if alg not in DIRECTED_ALGS:
+            raise ConfigError(f"experiment.graph.type: the directed graph {g['type']!r} runs with alg_name "
+                              f"{' or '.join(DIRECTED_ALGS)} only ({path}.optimizer_config.alg_name is {alg!r})")
         if p.get("fault_injection"):
             raise ConfigError(f"{path}.fault_injection: link-drop fault injection drops undirected edges and does not "
                               f"apply to the directed graph {g['type']!r}")
