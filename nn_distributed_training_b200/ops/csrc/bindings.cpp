@@ -257,6 +257,9 @@ PYBIND11_MODULE(_C, m) {
   m.def("convnet_generic_smem_bytes", [](int F, int KS, int LW, int dtype64, int spb) {
     return (size_t)mnist::generic_smem_bytes(mnist::GenericShape{F, KS, LW, dtype64, 0.0, 1.0}, dtype64, spb);
   });
+  m.def("convnet_generic_eval_spb", [](int F, int KS, int LW, int dtype64) {
+    return mnist::generic_eval_spb(mnist::GenericShape{F, KS, LW, dtype64, 0.0, 1.0});
+  });
   m.def("make_w1_tensor_map", [](uint64_t theta, int n_pad, int L, int off_w1) {
     unsigned char buf[128];
     check(mnist::make_w1_tensor_map(reinterpret_cast<const float*>(theta), n_pad, L, off_w1, buf), "make_w1_tensor_map");

@@ -56,6 +56,7 @@ struct GatherArgs {
 // fp64.  With dtype64 the Args pointers theta / grad_part / val_loss address doubles (loss_part stays float).
 struct GenericShape { int F, KS, LW, dtype64; double mean, inv_std; };   // mean / inv_std in full precision for the fp64 arm
 size_t generic_smem_bytes(const GenericShape& gs, int dtype64, int spb);
+int generic_eval_spb(const GenericShape& gs);   // samples per CTA of launch_generic_eval: 8, or 4 past 160 KB of smem
 cudaError_t launch_generic_train(const Args& a, const GenericShape& gs, int spb, int S, cudaStream_t st);
 cudaError_t launch_generic_eval(const Args& a, const GenericShape& gs, int ctas_per_node, cudaStream_t st);
 // Tensor-core training kernel of the paper shape (mnist_tc.cu): K-split over a 6-CTA cluster per node, batch <= 64,

@@ -390,9 +390,13 @@ cudaError_t launch_generic_train(const Args& a, const GenericShape& gs, int spb,
   return gs.dtype64 ? dispatch<double, true>(a, gs, spb, grid, st) : dispatch<float, true>(a, gs, spb, grid, st);
 }
 
+int generic_eval_spb(const GenericShape& gs) {
+  return generic_smem_bytes(gs, gs.dtype64, 8) <= 160 * 1024 ? 8 : 4;
+}
+
 cudaError_t launch_generic_eval(const Args& a, const GenericShape& gs, int ctas_per_node, cudaStream_t st) {
   const dim3 grid(ctas_per_node, a.L);
-  const int spb = generic_smem_bytes(gs, gs.dtype64, 8) <= 160 * 1024 ? 8 : 4;
+  const int spb = generic_eval_spb(gs);
   return gs.dtype64 ? dispatch<double, false>(a, gs, spb, grid, st) : dispatch<float, false>(a, gs, spb, grid, st);
 }
 

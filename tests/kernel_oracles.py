@@ -4,7 +4,8 @@
   on exactly the rows the kernel used without a second problem object drawing them.
 * ``convnet_fp64`` is ``MNISTConvNet`` in float64 autograd (``csrc/mnist_tc.cu`` and ``csrc/mnist_cl64.cu``); with
   ``tf32_fc1=True`` the operands of its three fc1-sized contractions are rounded to TF32 first, which is the error a
-  1xTF32 kernel would make: the yardstick of the 3xTF32 kernel.
+  1xTF32 kernel would make: the yardstick of the 3xTF32 kernel.  ``convnet_fp64_eval`` is the same forward per sample
+  (NLL and logits), the oracle of the evaluation kernels.
 * ``mlp_bf16_faithful`` is the density MLP of ``csrc/mlp_tc.cu`` written out by hand, rounding to bf16 exactly where
   the kernel rounds and nowhere else; ``rounding=False`` gives the exact math of the same network.
 * ``assert_close_to_oracle`` accepts a kernel when its error is a small fraction of a yardstick's error, per tensor and
@@ -112,19 +113,68 @@ class _Tf32Linear(torch.autograd.Function):
         return gt @ round_tf32(w), gt.T @ round_tf32(a)
 
 
-def convnet_fp64(theta_row, spec, x, y, mean=0.0, std=1.0, tf32_fc1=False, dtype=torch.float64):
-    """Mean NLL loss and flat gradient (arena layout, length of ``theta_row``) of ``MNISTConvNet`` on rows ``x``
-    (uint8 pixels normalised as ``(x / 255 - mean) / std``, or float inputs), computed in ``dtype`` autograd."""
-    params = [p.requires_grad_(True) for p in unflatten(theta_row, spec, dtype)]
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    return t.to(torch.float32).to(torch.float64)
+
+
+def _pool_argmax_f32(x, wc, mean, std):
+    """Argmax ``[n, F, 12, 12]`` of every 2 x 2 max-pool window as an fp32 kernel finds it: the inputs normalised in
+    fp32, each conv output an ``fmaf`` chain over the taps in (ky, kx) order, the bias added after the max, and the
+    first maximum winning.  (The fp64 product of two fp32 values is exact; the sum is rounded twice, which can move
+    the rare ulp.)"""
+    n, ks = x.shape[0], wc.shape[-1]
+    if x.dtype == torch.uint8:
+        xin = _f32(_f32(x.to(torch.float64) * _f32(torch.tensor(1 / 255.0)).item() - _f32(torch.tensor(mean)).item())
+                   * _f32(torch.tensor(1.0 / std)).item())
+    else:
+        xin = _f32(x.to(torch.float64))
+    xin = xin.reshape(n, 1, 28, 28)
+    w = _f32(wc.detach().to(torch.float64))
+    co = 28 - ks + 1
+    acc = torch.zeros(n, w.shape[0], co, co, dtype=torch.float64, device=x.device)
+    for ky in range(ks):
+        for kx in range(ks):
+            acc = _f32(w[:, 0, ky, kx].reshape(1, -1, 1, 1) * xin[:, :, ky: ky + co, kx: kx + co] + acc)
+    win = acc[..., : co // 2 * 2, : co // 2 * 2].unfold(2, 2, 2).unfold(3, 2, 2).flatten(-2)
+    return win.argmax(-1)                                  # the first of equal maxima, like the kernels
+
+
+def _convnet_forward(params, spec, x, y, mean, std, tf32_fc1, dtype, pool_f32=False):
+    """Logits ``[n, 10]`` and per-sample NLL ``[n]`` of ``MNISTConvNet`` with parameter tensors ``params`` on rows
+    ``x`` (uint8 pixels normalised as ``(x / 255 - mean) / std``, or float inputs), in ``dtype``.  ``pool_f32=True``
+    takes each max-pool window's argmax from ``_pool_argmax_f32`` instead: where two conv outputs of a window are
+    closer than fp32 can resolve, an fp32 kernel routes that cell to another position than fp64 does."""
     wc, bc, w1, b1, w2, b2 = params
     x = x.reshape(x.shape[0], 1, spec.in_hw, spec.in_hw)
     xin = (x.to(dtype) / 255.0 - mean) / std if x.dtype == torch.uint8 else x.to(dtype)
-    a = F.max_pool2d(F.relu(F.conv2d(xin, wc, bc)), 2).flatten(1)
+    c = F.relu(F.conv2d(xin, wc, bc))
+    if pool_f32:
+        po = c.shape[-1] // 2
+        win = c[..., : 2 * po, : 2 * po].unfold(2, 2, 2).unfold(3, 2, 2).flatten(-2)
+        a = win.gather(-1, _pool_argmax_f32(x, wc, mean, std).unsqueeze(-1)).flatten(1)
+    else:
+        a = F.max_pool2d(c, 2).flatten(1)
     h = (_Tf32Linear.apply(a, w1) if tf32_fc1 else a @ w1.T) + b1
-    out = F.log_softmax(F.relu(h) @ w2.T + b2, dim=1)
-    loss = F.nll_loss(out, y.to(out.device).long())
+    z = F.relu(h) @ w2.T + b2
+    return z, F.nll_loss(F.log_softmax(z, dim=1), y.to(z.device).long(), reduction="none")
+
+
+def convnet_fp64(theta_row, spec, x, y, mean=0.0, std=1.0, tf32_fc1=False, dtype=torch.float64, pool_f32=False):
+    """Mean NLL loss and flat gradient (arena layout, length of ``theta_row``) of ``MNISTConvNet`` on rows ``x``
+    (uint8 pixels normalised as ``(x / 255 - mean) / std``, or float inputs), computed in ``dtype`` autograd;
+    ``pool_f32``: see ``_convnet_forward``."""
+    params = [p.requires_grad_(True) for p in unflatten(theta_row, spec, dtype)]
+    loss = _convnet_forward(params, spec, x, y, mean, std, tf32_fc1, dtype, pool_f32)[1].mean()
     grads = torch.autograd.grad(loss, params)
     return loss.detach(), flatten([g.detach() for g in grads], spec, theta_row.shape[-1])
+
+
+def convnet_fp64_eval(theta_row, spec, x, y, mean=0.0, std=1.0, tf32_fc1=False, dtype=torch.float64):
+    """Per-sample NLL ``[n]`` and logits ``[n, 10]`` of ``MNISTConvNet`` on rows ``x``, the forward of
+    ``convnet_fp64``: what the evaluation kernels store per validation sample."""
+    with torch.no_grad():
+        z, nll = _convnet_forward(unflatten(theta_row, spec, dtype), spec, x, y, mean, std, tf32_fc1, dtype)
+    return nll, z
 
 
 # ---- density MLP (FourierNet / FFReLUNet [2, h1, 64, 64, 64, 1]) -----------------------------------------------------
