@@ -107,6 +107,31 @@ def ed_step_(theta: torch.Tensor, psi: torch.Tensor, grad: torch.Tensor, alpha: 
     theta.copy_(psi).add_(corr)
 
 
+# --------------------------------------------------- DSGD with momentum ----
+def dsgdm_step_(theta: torch.Tensor, m: torch.Tensor, x_prev: Optional[torch.Tensor], grad: torch.Tensor, alpha: float,
+                alpha_prev: float, beta: float, quasi_global: bool, nesterov: bool, first: bool):
+    """The momentum step on the mixed rows ``x = theta`` (``first``: round 0, where ``m`` and ``x_prev`` are not read).
+
+    local:         ``m <- beta m + g``
+    quasi-global:  ``m <- beta m + (1 - beta) (x_prev - x) / alpha_prev`` after round 0 (``m`` holds mhat, 0 in round
+                   0); the step's momentum is ``beta mhat + g``; ``x_prev <- x``
+    both:          ``theta <- x - alpha (nesterov ? g + beta mom : mom)``"""
+    if quasi_global:
+        if first:
+            m.zero_()
+        else:
+            m.mul_(beta).add_((x_prev - theta) / alpha_prev, alpha=1.0 - beta)
+        x_prev.copy_(theta)
+        mom = grad.add(m, alpha=beta)
+    else:
+        if first:
+            m.copy_(grad)
+        else:
+            m.mul_(beta).add_(grad)
+        mom = m
+    theta.add_(grad.add(mom, alpha=beta) if nesterov else mom, alpha=-alpha)
+
+
 # ------------------------------------------------------------ CHOCO-SGD ----
 # Code rows (the byte layout of csrc/consensus.h, the only other place it is written).  A row of n_pad elements is cut
 # into nb = n_pad / 32 blocks of 32; scales are in the arena dtype T:

@@ -120,17 +120,22 @@ struct ConsensusOp {
   consensus::DinnoArgs<T> dn{};
   consensus::DsgtArgs<T> gt{};
   consensus::EdArgs<T> ed{};
+  consensus::MomentumArgs<T> mo{};
+  bool mo_qg = false;
   consensus::ChocoArgs<T> ch{};
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; ch.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
     pd.row_stride = sg.row_stride;
     ed.psi = ptr<T>(d, "psi");
+    mo_qg = geti(d, "quasi_global", 0) != 0;
+    mo.m = ptr<T>(d, "m"); mo.x_prev = mo_qg ? ptr<T>(d, "x_prev") : nullptr;
+    mo.beta = (T)getf(d, "beta", 0.0); mo.nesterov = geti(d, "nesterov", 0);
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
     ch.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
@@ -153,6 +158,11 @@ struct ConsensusOp {
   void ed_step() {
     if (ed.psi == nullptr) throw std::runtime_error("ed_step needs the Exact Diffusion row `psi`");
     check(consensus::launch_ed_step<T>(ed, cur_stream()), "ed_step");
+  }
+  void dsgdm_step() {
+    if (mo.m == nullptr || (mo_qg && mo.x_prev == nullptr))
+      throw std::runtime_error("dsgdm_step needs the momentum row `m` (and `x_prev` with quasi-global momentum)");
+    check(consensus::launch_dsgdm_step<T>(mo, cur_stream()), "dsgdm_step");
   }
   void choco_check(const char* what) const {
     if (ch.x_hat == nullptr || ch.s == nullptr || ch.live == nullptr || ch.code_stride <= 0)
@@ -223,6 +233,7 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dsgt_track", &ConsensusOp<T>::dsgt_track)
       .def("ed_mix", &ConsensusOp<T>::ed_mix)
       .def("ed_step", &ConsensusOp<T>::ed_step)
+      .def("dsgdm_step", &ConsensusOp<T>::dsgdm_step)
       .def("choco_mix", &ConsensusOp<T>::choco_mix)
       .def("choco_step", &ConsensusOp<T>::choco_step)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)

@@ -1,11 +1,12 @@
-// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGT / Exact Diffusion /
-// CHOCO-SGD / SGP / Push-DIGing.
+// Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGD with momentum / DSGT /
+// Exact Diffusion / CHOCO-SGD / SGP / Push-DIGing.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
 //   optimizers/dsgd.py:37-46 / :55-58      -> dsgd_mix / dsgd_step
 //   optimizers/dsgt.py:58-75 / :87-103     -> dsgt_mix / dsgt_track
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
+// DSGD with momentum (no reference counterpart, optimizers/dsgdm.py)       -> dsgd_mix / dsgdm_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
@@ -459,6 +460,64 @@ __global__ void __launch_bounds__(THREADS) ed_step_kernel(const EdArgs<T> a) {
     stv(a.psi + row + i, pn);
     stv(c.theta + row + i, tn);
     stv(pub_row(c, ri.par ^ 1, 0, l) + i, tn);
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
+// ---------------------------------------------------------- DSGD with momentum ----
+// The mix is dsgd_mix_kernel.  The step, on the mixed row x (theta after the mix) with alpha_k from the schedule:
+//   local (QG = false):   m <- beta m + g
+//   quasi-global (QG):    mhat <- beta mhat + (1 - beta) (x_prev - x) / alpha_{k-1};  m = beta mhat + g;  x_prev <- x
+//   theta <- x - alpha_k (NEST ? g + beta m : m);  theta is published.
+// Round 0 reads neither the momentum row nor x_prev and takes them as zero (m = g, mhat = 0): its step is DSGD's.
+// The 4-deep variant is held to 64 registers (4 CTAs per SM) without spilling; the quasi-global step's IEEE division
+// otherwise takes it to 76 in fp64.  The deep variant keeps the compiler's choice (a minimum of 0 CTAs sets no limit).
+template <typename T, int U, bool QG, bool NEST>
+__global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 0) dsgdm_step_kernel(const MomentumArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const bool init = ri.k == 0;
+  const T alpha_prev = QG && !init ? c.alpha[ri.k - 1] : (T)1;
+  const T beta = a.beta, beta_c = (T)1 - a.beta;
+  const size_t row = (size_t)l * c.n_pad;
+  // theta (written by the mix two launches back), the momentum row and x_prev (the previous round's step) are read,
+  // and mhat is advanced, before the programmatic-dependency wait; only the gradient partials of the forward/backward
+  // kernel after it
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> x = ldv(c.theta + row + i);
+    Pack<T> mb;                         // local: m of the previous round; quasi-global: mhat of this round
+    if (init) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) mb.v[u] = (T)0;
+    } else {
+      mb = ldv(a.m + row + i);
+      if (QG) {
+        const Pack<T> xp = ldv(a.x_prev + row + i);
+#pragma unroll
+        for (int u = 0; u < N; ++u) mb.v[u] = beta * mb.v[u] + beta_c * div_rn(xp.v[u] - x.v[u], alpha_prev);
+      }
+    }
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> m, th;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      m.v[u] = beta * mb.v[u] + g.v[u];
+      th.v[u] = x.v[u] - alpha * (NEST ? g.v[u] + beta * m.v[u] : m.v[u]);
+    }
+    if (QG) {
+      stv(a.m + row + i, mb);
+      stv(a.x_prev + row + i, x);
+    } else {
+      stv(a.m + row + i, m);
+    }
+    stv(c.theta + row + i, th);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
   }
   release_dependents_once(waited);
   end_step(c, l, ri.k, true);
@@ -926,6 +985,15 @@ template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st) {
   return launch_by_s(ed_step_kernel<T, 4>, ed_step_kernel<T, 16>, a.c, a, st);
 }
+// the momentum mode and Nesterov are template parameters, not runtime branches (see dsgt_mix above).  Beyond 4 gradient
+// partials the step keeps 8 loads in flight, as sgp_step: 16 spilled in fp32
+template <typename T, bool QG, bool NEST> static cudaError_t launch_dsgdm(const MomentumArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(dsgdm_step_kernel<T, 4, QG, NEST>, dsgdm_step_kernel<T, 8, QG, NEST>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_dsgdm_step(const MomentumArgs<T>& a, cudaStream_t st) {
+  if (a.x_prev != nullptr) return a.nesterov ? launch_dsgdm<T, true, true>(a, st) : launch_dsgdm<T, true, false>(a, st);
+  return a.nesterov ? launch_dsgdm<T, false, true>(a, st) : launch_dsgdm<T, false, false>(a, st);
+}
 // the compressor is a template parameter, not a runtime branch (see dsgt_mix above).  With more than 4 gradient
 // partials the step keeps 8 loads in flight (the summation order is the same for any depth); 16, as the other step
 // kernels use, took 164 registers (fp64) or spilled (fp32) next to the encoder
@@ -972,6 +1040,7 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_dsgt_track<T>(const DsgtArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_ed_mix<T>(const EdArgs<T>&, cudaStream_t);              \
   template cudaError_t launch_ed_step<T>(const EdArgs<T>&, cudaStream_t);             \
+  template cudaError_t launch_dsgdm_step<T>(const MomentumArgs<T>&, cudaStream_t);    \
   template cudaError_t launch_choco_mix<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \

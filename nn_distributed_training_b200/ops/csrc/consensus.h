@@ -98,6 +98,19 @@ struct EdArgs {
   T* psi;                          // [L, n_pad] the adapt step of the previous round; set from theta in round 0
 };
 
+// DSGD with momentum: DSGD's single published channel and its mix (dsgd_mix_kernel), and a step that keeps a momentum
+// row.  Local momentum: m is the heavy-ball row.  Quasi-global momentum (Lin, Karimireddy, Stich, Jaggi 2021; selected
+// by x_prev != nullptr): m is mhat, the average of the rows' displacement (x_prev - x) / alpha_{k-1} over rounds, and
+// x_prev the mixed row of the previous round.
+template <typename T>
+struct MomentumArgs {
+  Common<T> c;
+  T* m;                            // [L, n_pad] momentum (local) or mhat (quasi-global); read from round 1 on
+  T* x_prev;                       // [L, n_pad] quasi-global: the previous round's mixed row; nullptr = local momentum
+  T beta;                          // momentum coefficient, also mhat's averaging coefficient
+  int nesterov;                    // step along g + beta m instead of m
+};
+
 // CHOCO-SGD (Koloskova, Stich, Jaggi 2019), memory-efficient form: nodes publish a compressed code of
 // v = theta - x_hat instead of theta.  The published buffer holds code rows of `code_stride` bytes (nbr_ptr points at
 // them); per block of 32 elements (b = i / 32, nb = n_pad / 32 blocks):
@@ -168,6 +181,7 @@ template <typename T> cudaError_t launch_dsgt_mix(const DsgtArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_dsgt_track(const DsgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_ed_mix(const EdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_dsgdm_step(const MomentumArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);

@@ -38,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp"):
+    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT and Push-DIGing: a constant step
         alpha[:] = opt.alpha
@@ -300,6 +300,9 @@ class ConsensusEngine:
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
         if opt.alg_name == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
+        if opt.alg_name == "dsgdm":
+            d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
+                     quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
         self.t_live = None
         if self.choco:
             self.t_live = choco_live_words(opt.live).to(dev)

@@ -3,6 +3,7 @@
 A round is a short, fixed kernel sequence
     DiNNO:  [fwd/bwd, dinno_update(p)] x primal_iterations
     DSGD :  dsgd_mix, fwd/bwd, dsgd_step
+    DSGD with momentum:  dsgd_mix, fwd/bwd, dsgdm_step
     DSGT :  dsgt_mix, fwd/bwd, dsgt_track
     Exact Diffusion:  ed_mix, fwd/bwd, ed_step
     CHOCO-SGD:  choco_mix, fwd/bwd, choco_step
@@ -52,6 +53,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.dsgd_mix()
         grads(0)
         eng.op.dsgd_step()
+    elif alg == "dsgdm":
+        eng.op.dsgd_mix()
+        grads(0)
+        eng.op.dsgdm_step()
     elif alg == "dsgt":
         eng.op.dsgt_mix()
         grads(0)
@@ -279,7 +284,7 @@ class RoundProgram:
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name in ("dsgd", "exact_diffusion", "choco_sgd", "sgp") and opt.k > 0:
+        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "choco_sgd":
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))

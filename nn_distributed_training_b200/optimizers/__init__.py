@@ -1,12 +1,13 @@
 from .choco import ChocoSGD
 from .dinno import DiNNO
 from .dsgd import DSGD
+from .dsgdm import DSGDm
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
 from .push_diging import PushDIGing
 from .sgp import SGP
 
-ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
+ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "sgp": SGP, "push_diging": PushDIGing}
 
 

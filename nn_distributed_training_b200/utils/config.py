@@ -15,11 +15,12 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgt", "exact_diffusion", "choco_sgd", "sgp", "push_diging")
+ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "sgp", "push_diging")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
 CHOCO_COMPRESSORS = ("none", "int8", "sign")
+MOMENTUM_MODES = ("local", "quasi_global")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
 DENSITY_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "mesh_grid_density",
@@ -31,6 +32,8 @@ OPT_SCHEMA = {
               "primal_lr_start": REQUIRED, "primal_lr_finish": None, "lr_decay_type": "constant",
               "profile": False},
     "dsgd": {"alpha0": REQUIRED, "mu": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
+    "dsgdm": {"alpha0": REQUIRED, "mu": 0.0, "beta": REQUIRED, "momentum": REQUIRED, "nesterov": False,
+              "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
     "dsgt": {"alpha": REQUIRED, "init_grads": True, "outer_iterations": REQUIRED, "profile": False},
     "exact_diffusion": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False},
     "choco_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED,
@@ -80,9 +83,14 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg in ("exact_diffusion", "choco_sgd", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
+    if alg in ("dsgdm", "exact_diffusion", "choco_sgd", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
+    if alg == "dsgdm":
+        if not 0.0 <= float(c["beta"]) < 1.0:
+            raise ConfigError(f"{path}.beta must be in [0, 1) (got {c['beta']!r})")
+        if c["momentum"] not in MOMENTUM_MODES:
+            raise ConfigError(f"{path}.momentum must be one of {'|'.join(MOMENTUM_MODES)} (got {c['momentum']!r})")
     if alg == "choco_sgd":
         if not 0.0 < float(c["gamma"]) <= 1.0:
             raise ConfigError(f"{path}.gamma must be in (0, 1] (got {c['gamma']!r})")
