@@ -23,7 +23,9 @@ namespace mnist {
 
 namespace cl64 {
 
-constexpr int NT = 512, CL = 4, CELLS = 36, KC = 108, WS = 116, HS = 68;
+// 20 warps of 96 registers a thread (61,440 of the SM's 65,536): the forward conv takes fewer rounds than at 16 warps,
+// and GEMM 3 gets four warps of its own beside the 15 conv-gradient warps and the bias warp
+constexpr int NT = 640, CL = 4, CELLS = 36, KC = 108, WS = 116, HS = 68;
 constexpr int PXR = 10 * HW;                  // image rows 6c .. 6c+9 of a sample: 280 pixels
 constexpr int KT = (KC + 7) / 8;              // 8-column tiles over a CTA's fc1 inputs; columns 108..111 fall in the row padding
 // rows of w2 and of the owners' h hold the 64 hidden units as four 16-unit runs 17 apart: the fc2 logits are summed by
@@ -254,40 +256,51 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   __syncthreads();
   stamp(prof, 3, tid);
 
-  // ---- conv + ReLU + maxpool: one (sample, pooled cell) per item, the 6x6 patch in fp64 registers ---------------------------
+  // ---- conv + ReLU + maxpool: one (sample, pooled cell) per item.  Two rows of the 6x6 patch are in fp64 registers at a
+  //      time, one new row per tap row, and the four pool positions of all three channels accumulate together; each
+  //      accumulator takes its products in (ky, kx) order ------------------------------------------------------------------
   for (int it = tid; it < MS * CELLS; it += NT) {
     const int s = it / CELLS, cell = it - s * CELLS;
     const int pr = cell / PHW, px = cell - pr * PHW;
     const int p0 = (2 * pr) * HW + 2 * px;
-    double patch[6][6];
-    if constexpr (kDoublePix) {
-      // a patch row is six consecutive doubles starting at an even column: three 16-byte loads
-      const double* src = imgd + s * PXS + p0;
-#pragma unroll
-      for (int r = 0; r < 6; ++r)
+    auto patch_row = [&](double (&x)[6], int r) {
+      if constexpr (kDoublePix) {
+        // a patch row is six consecutive doubles starting at an even column: three 16-byte loads
+        const double* src = imgd + s * PXS + p0 + r * HW;
 #pragma unroll
         for (int q = 0; q < 6; q += 2) {
-          const double2 v = *reinterpret_cast<const double2*>(src + r * HW + q);
-          patch[r][q] = v.x; patch[r][q + 1] = v.y;
+          const double2 v = *reinterpret_cast<const double2*>(src + q);
+          x[q] = v.x; x[q + 1] = v.y;
         }
-    } else {
+      } else {
 #pragma unroll
-      for (int r = 0; r < 6; ++r)
+        for (int q = 0; q < 6; ++q) x[q] = pix(s, p0 + r * HW + q);
+      }
+    };
+    double acc[F][4], x0[6], x1[6];
 #pragma unroll
-        for (int q = 0; q < 6; ++q) patch[r][q] = pix(s, p0 + r * HW + q);
+    for (int ch = 0; ch < F; ++ch)
+#pragma unroll
+      for (int i = 0; i < 4; ++i) acc[ch][i] = 0;
+    patch_row(x0, 0);
+#pragma unroll
+    for (int ky = 0; ky < KS; ++ky) {
+      patch_row(x1, ky + 1);
+#pragma unroll
+      for (int kx = 0; kx < KS; ++kx)
+#pragma unroll
+        for (int ch = 0; ch < F; ++ch) {
+          const double w = sm.wc[ch * 25 + ky * 5 + kx];
+          acc[ch][0] += w * x0[kx]; acc[ch][1] += w * x0[kx + 1];
+          acc[ch][2] += w * x1[kx]; acc[ch][3] += w * x1[kx + 1];
+        }
+#pragma unroll
+      for (int q = 0; q < 6; ++q) x0[q] = x1[q];
     }
     const bool ok = sm.valid[s] != 0.f;
-#pragma unroll 1
+#pragma unroll
     for (int ch = 0; ch < F; ++ch) {
-      double a00 = 0, a01 = 0, a10 = 0, a11 = 0;
-#pragma unroll
-      for (int ky = 0; ky < KS; ++ky)
-#pragma unroll
-        for (int kx = 0; kx < KS; ++kx) {
-          const double w = sm.wc[ch * 25 + ky * 5 + kx];
-          a00 += w * patch[ky][kx]; a01 += w * patch[ky][kx + 1];
-          a10 += w * patch[ky + 1][kx]; a11 += w * patch[ky + 1][kx + 1];
-        }
+      const double a00 = acc[ch][0], a01 = acc[ch][1], a10 = acc[ch][2], a11 = acc[ch][3];
       double m = a00; int ai = 0;                      // first maximum wins, like ATen's max_pool2d
       if (a01 > m) { m = a01; ai = 1; }
       if (a10 > m) { m = a10; ai = 2; }
@@ -303,7 +316,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   stamp(prof, 4, tid);
 
   // ---- GEMM 1 (DMMA): partial H_c[s][j] = sum_k A[s][k] W[j][k] over this CTA's 108 inputs.  MS / 16 x 8 tiles of 16 x 8,
-  //      NJ1 adjacent column tiles per warp (all 16 warps busy at MS >= 32), the whole K range per tile: no split-K ----------
+  //      NJ1 adjacent column tiles per warp (16 of the 20 warps busy at MS >= 32), the whole K range per tile: no split-K ----------
   {
     constexpr int NJ1 = MS == 64 ? 2 : 1, NGRP = 8 / NJ1;
     if (warp < (MS / 16) * NGRP) {
@@ -405,12 +418,15 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   stamp(prof, 7, tid);
   cluster_sync();                                        // #2: every owner's dH rows and fc2 / b1 / loss shares are final
   stamp(prof, 8, tid);
-  double* gp = reinterpret_cast<double*>(a.grad_part) + ((size_t)l * nsplit + bsplit) * a.n_pad;
+  // this split's gradient row, formed where it is written: a pointer held from here to the end would cost two registers
+  // through GEMM 2 and the conv grads, and the kernel has 96 per thread
+  auto grad_row = [&]() { return reinterpret_cast<double*>(a.grad_part) + ((size_t)l * nsplit + bsplit) * a.n_pad; };
   // CTA c reduces its quarter of the fc2 / b1 / loss shares over the cluster (the peers stay resident until the last barrier)
   {
     constexpr int NE = PART_N - PART_B1, PER = (NE + CL - 1) / CL;
     const int o = PART_B1 + c * PER + tid;
     if (tid < PER && o < PART_N) {
+      double* gp = grad_row();
       double v = 0.0;
 #pragma unroll
       for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(sm.part + o, (uint32_t)r));
@@ -462,13 +478,16 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   }
   __syncthreads();
   stamp(prof, 11, tid);
-  // ---- GEMM 3 (DMMA) on warps 12 .. 15, one per SM sub-partition: dW1_c[j][k] = sum_s dH[s][j] A[s][k].  Warp 12 + q owns
-  //      hidden rows 16q .. 16q+15 and all KT column tiles, KT / 2 at a time: that many independent DMMA chains share the dH
-  //      fragments.  Tiles go straight to the gradient row (column pairs as 16-byte stores).  Meanwhile warps 0 .. 11 run
-  //      their conv-grad rows, so the FP64 pipe of every sub-partition is busy while its tensor cores run GEMM 3; warps
-  //      12 .. 15 follow with their own conv-grad rows (warp 15: the bias sums).  No barrier on either side ----------------
-  constexpr int W3 = NT / 32 - HID / 16, NJ3 = KT / 2;   // first GEMM 3 warp; column tiles per pass
+  // ---- GEMM 3 (DMMA) on warps 16 .. 19, one per SM sub-partition: dW1_c[j][k] = sum_s dH[s][j] A[s][k].  Warp 16 + q owns
+  //      hidden rows 16q .. 16q+15 and all KT column tiles, two at a time: two independent DMMA chains share the dH
+  //      fragments (seven, with their next fragments in flight, do not fit in 96 registers).  Tiles go straight to the
+  //      gradient row (column pairs as 16-byte stores).  Meanwhile warps 0 .. 14 run their conv-grad rows and warp 15 the
+  //      bias sums, so the FP64 pipe of every sub-partition is busy while its tensor cores run GEMM 3.  No barrier on
+  //      either side -----------------------------------------------------------------------------------------------------
+  constexpr int W3 = NT / 32 - HID / 16, NJ3 = 2;   // first GEMM 3 warp; column tiles per pass
+  static_assert(KT % NJ3 == 0, "GEMM 3 passes cover the column tiles");
   if (warp >= W3) {
+    double* gp = grad_row();
     const int m0 = 16 * (warp - W3);
 #pragma unroll 1
     for (int n0 = 0; n0 < 8 * KT; n0 += 8 * NJ3) {
@@ -489,7 +508,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
           }
         }
     }
-    stamp(prof, 12, tid - W3 * 32);      // lane 0 of warp 12: its GEMM 3 stores are issued
+    stamp(prof, 12, tid - W3 * 32);      // lane 0 of warp W3: its GEMM 3 stores are issued
   }
   // ---- conv grads without gathers: warps 3ky .. 3ky+2 own tap row ky of all three channels.  A thread walks whole pooled
   //      rows (sample s, pooled row pr, px = 0 .. 11) with columns 2px .. 2px+5 of patch rows 2pr+ky and 2pr+ky+1 in
@@ -571,6 +590,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   stamp(prof, 13, tid);
   cluster_sync();                                        // #3: all four conv-gradient shares are in rank 0's buffer
   if (c == 0 && tid < 78) {
+    double* gp = grad_row();
     double v = 0.0;
 #pragma unroll
     for (int r = 0; r < CL; ++r) v += sm.h_loc[r * 80 + tid];

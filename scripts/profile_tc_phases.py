@@ -25,8 +25,8 @@ PHASES = ["sampler + image loads issued", "PDL wait", "TMA issue, small tensors,
 PHASES64 = ["sampler, image rows -> smem (fp64)", "PDL wait", "W1 copies issued, conv weights + w2 (L2)",
             "conv + ReLU + pool -> A tile (fp64), W1 copy wait", "GEMM 1 (fc1 partial, DMMA)", "cluster sync 1",
             "head: warp per sample (H sum, fc2, loss, dz, dh), fc2 grads", "cluster sync 2", "fc2-grad reduce (1/4), gather dH",
-            "GEMM 2 (da1, DMMA) -> registers", "da1 -> smem (over W)", "GEMM 3 (dW1, warps 12-15) -> global | conv grads",
-            "conv grads after GEMM 3 -> rank 0", "cluster sync 3, conv-grad sum (rank 0), exit"]
+            "GEMM 2 (da1, DMMA) -> registers", "da1 -> smem (over W)", "GEMM 3 (dW1, warps 16-19) -> global | conv grads",
+            "bias warp, conv grads still running after GEMM 3 -> rank 0", "cluster sync 3, conv-grad sum (rank 0), exit"]
 
 
 def slot_errors(B):
