@@ -254,6 +254,33 @@ def choco_step_(theta: torch.Tensor, x_hat: torch.Tensor, grad: torch.Tensor, al
     return codes
 
 
+# ----------------------------------------------------------------- BEER ----
+# Gradient tracking with both channels gossiped as CHOCO codes: channel 0 codes theta - h, channel 1 codes v - g, with
+# CHOCO's encoder, decoder and byte layout.
+def beer_mix_(theta: torch.Tensor, h: torch.Tensor, s_h: torch.Tensor, v: torch.Tensor, s_g: torch.Tensor,
+              dec_h_all: torch.Tensor, dec_g_all: torch.Tensor, w_rows: torch.Tensor, gamma: float, alpha: float):
+    """``s_h_i += sum_j W_ij dec(qh_j)``, ``s_g_i += sum_j W_ij dec(qg_j)`` (own terms included);
+    ``theta_i += gamma (s_h_i - h_i) - alpha v_i``."""
+    w = w_rows.to(dec_h_all.dtype)
+    s_h.add_(w @ dec_h_all)
+    s_g.add_(w @ dec_g_all)
+    theta.add_(gamma * (s_h - h) - alpha * v)
+
+
+def beer_step_(theta: torch.Tensor, h: torch.Tensor, v: torch.Tensor, g: torch.Tensor, s_g: torch.Tensor,
+               m_old: torch.Tensor, grad: torch.Tensor, gamma: float, compressor: str,
+               live: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``v += gamma (s_g - g) + grad - m_old``; ``m_old <- grad``; ``qh = Q(theta - h)``, ``h += dec(qh)``;
+    ``qg = Q(v - g)``, ``g += dec(qg)``; returns the code rows ``(qh, qg)`` to publish."""
+    v.add_(gamma * (s_g - g) + grad - m_old)
+    m_old.copy_(grad)
+    codes_h, dec_h = choco_encode(theta - h, compressor, live)
+    h.add_(dec_h)
+    codes_g, dec_g = choco_encode(v - g, compressor, live)
+    g.add_(dec_g)
+    return codes_h, codes_g
+
+
 # ------------------------------------------------------------------ SGP ----
 # Push-sum (Stochastic Gradient Push): numerator rows x [L, n_pad] and float64 weights w [L].  The combine weights are
 # the column-stochastic A of Topology.push_weights, rounded to the arena dtype; w is mixed with those same rounded

@@ -123,11 +123,12 @@ struct ConsensusOp {
   consensus::MomentumArgs<T> mo{};
   bool mo_qg = false;
   consensus::ChocoArgs<T> ch{};
+  consensus::BeerArgs<T> be{};
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -139,6 +140,9 @@ struct ConsensusOp {
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
     ch.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
+    be.h = ptr<T>(d, "h"); be.s_h = ptr<T>(d, "s_h"); be.v = ptr<T>(d, "v"); be.g = ptr<T>(d, "g");
+    be.s_g = ptr<T>(d, "s_g"); be.m_old = ptr<T>(d, "m_old");
+    be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride;
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
@@ -175,6 +179,20 @@ struct ConsensusOp {
   void choco_step() {
     choco_check("choco_step");
     check(consensus::launch_choco_step<T>(ch, cur_stream()), "choco_step");
+  }
+  void beer_check(const char* what) const {
+    if (be.h == nullptr || be.s_h == nullptr || be.v == nullptr || be.g == nullptr || be.s_g == nullptr ||
+        be.m_old == nullptr || be.live == nullptr || be.code_stride <= 0 || c.C != 2)
+      throw std::runtime_error(std::string(what) + " needs the BEER rows `h`, `s_h`, `v`, `g`, `s_g`, `m_old`, the `live` "
+                               "mask, `code_stride` and two published channels");
+  }
+  void beer_mix() {
+    beer_check("beer_mix");
+    check(consensus::launch_beer_mix<T>(be, cur_stream()), "beer_mix");
+  }
+  void beer_step() {
+    beer_check("beer_step");
+    check(consensus::launch_beer_step<T>(be, cur_stream()), "beer_step");
   }
   void sgp_check(const char* what) const {
     if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0)
@@ -236,6 +254,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dsgdm_step", &ConsensusOp<T>::dsgdm_step)
       .def("choco_mix", &ConsensusOp<T>::choco_mix)
       .def("choco_step", &ConsensusOp<T>::choco_step)
+      .def("beer_mix", &ConsensusOp<T>::beer_mix)
+      .def("beer_step", &ConsensusOp<T>::beer_step)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
       .def("sgp_step", &ConsensusOp<T>::sgp_step)
       .def("pdg_mix", &ConsensusOp<T>::pdg_mix)

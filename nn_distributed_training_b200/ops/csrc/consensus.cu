@@ -1,5 +1,5 @@
 // Fused neighbor-exchange + mixing + optimizer-update kernels for DiNNO / DSGD / DSGD with momentum / DSGT /
-// Exact Diffusion / CHOCO-SGD / SGP / Push-DIGing.
+// Exact Diffusion / CHOCO-SGD / BEER / SGP / Push-DIGing.
 //
 // Reference call sites replaced (all Python loops over nodes x parameter tensors):
 //   optimizers/dinno.py:103-125 + :74-91  -> dinno_update   (exchange, dual ascent, prox-grad, Adam/SGD/AdamW)
@@ -8,6 +8,7 @@
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
 // DSGD with momentum (no reference counterpart, optimizers/dsgdm.py)       -> dsgd_mix / dsgdm_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
+// BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
@@ -664,6 +665,128 @@ __global__ void __launch_bounds__(THREADS) choco_step_kernel(const ChocoArgs<T> 
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------------- BEER ----
+// Two channels of CHOCO code rows (consensus.h): channel 0 codes theta - h, channel 1 codes v - g.  Round k: beer_mix
+// reads both codes of round k-1 of the node and its neighbors (all zero in round 0),
+//   s_h_i += W_ii dec(qh_i) + sum_j W_ij dec(qh_j),  s_g_i += W_ii dec(qg_i) + sum_j W_ij dec(qg_j),
+//   theta_i += gamma (s_h_i - h_i) - alpha v_i;
+// beer_step takes v_i += gamma (s_g_i - g_i) + grad_i - m_old_i, m_old_i <- grad_i, qh_i = Q(theta_i - h_i),
+// h_i += dec(qh_i), qg_i = Q(v_i - g_i), g_i += dec(qg_i) and publishes (qh_i, qg_i).  The tracker update sits in the
+// step, beside the gradient it needs: folded into the mix it would move as many row loads as it saves and add a store.
+template <typename T>
+struct HGPack { Pack<T> h, g; };
+
+template <typename T, int Q>
+__global__ void __launch_bounds__(THREADS) beer_mix_kernel(const BeerArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T alpha = c.alpha[ri.k];
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const char* own_h = beer_code_row(a, ri.par, 0, l);
+  const char* own_g = beer_code_row(a, ri.par, 1, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const unsigned lw = Q == kCodeSign ? a.live[i >> 5] : 0u;
+    Pack<T> th = choco_decode<T, Q>(own_h, c.n_pad, i, lw), tg = choco_decode<T, Q>(own_g, c.n_pad, i, lw);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      th.v[u] *= ws;
+      tg.v[u] *= ws;
+    }
+    // two neighbors' two code rows in flight, decoded in registers
+    for_neighbors<2>(deg,
+                     [&](int e) {
+                       return HGPack<T>{
+                           choco_decode<T, Q>(reinterpret_cast<const char*>(nbr_row(c, ri.gid, l, e, ri.par, 0)), c.n_pad, i, lw),
+                           choco_decode<T, Q>(reinterpret_cast<const char*>(nbr_row(c, ri.gid, l, e, ri.par, 1)), c.n_pad, i, lw)};
+                     },
+                     [&](int e, const HGPack<T>& q) {
+                       const T we = w[e];
+#pragma unroll
+                       for (int u = 0; u < N; ++u) {
+                         th.v[u] += we * q.h.v[u];
+                         tg.v[u] += we * q.g.v[u];
+                       }
+                     });
+    Pack<T> sh = ldv(a.s_h + row + i), sg = ldv(a.s_g + row + i);
+    const Pack<T> h = ldv(a.h + row + i), v = ldv(a.v + row + i);
+    Pack<T> x = ldv(c.theta + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      sh.v[u] += th.v[u];
+      sg.v[u] += tg.v[u];
+      x.v[u] += a.gamma * (sh.v[u] - h.v[u]) - alpha * v.v[u];
+    }
+    stv(a.s_h + row + i, sh);
+    stv(a.s_g + row + i, sg);
+    stv(c.theta + row + i, x);
+  }
+}
+
+// Per-warp loop as in choco_step: both encoders reduce their blocks' scales with warp shuffles.
+template <typename T, int U, int Q>
+__global__ void __launch_bounds__(THREADS) beer_step_kernel(const BeerArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const size_t row = (size_t)l * c.n_pad;
+  char* out_h = beer_code_row(a, ri.par ^ 1, 0, l);
+  char* out_g = beer_code_row(a, ri.par ^ 1, 1, l);
+  const int lane = threadIdx.x & 31;
+  // theta and s_g (written by the mix two launches back), h, v, g and m_old (the previous round's step) are read
+  // before the programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int w0 = (blockIdx.x * THREADS + (threadIdx.x & ~31)) * N; w0 < c.n_pad; w0 += gridDim.x * THREADS * N) {
+    const int i = w0 + lane * N;
+    const bool in = i < c.n_pad;
+    Pack<T> x, h, v, g, sg, mo, gr;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      x.v[u] = (T)0; h.v[u] = (T)0; v.v[u] = (T)0; g.v[u] = (T)0; sg.v[u] = (T)0; mo.v[u] = (T)0; gr.v[u] = (T)0;
+    }
+    if (in) {
+      x = ldv(c.theta + row + i);
+      h = ldv(a.h + row + i);
+      v = ldv(a.v + row + i);
+      g = ldv(a.g + row + i);
+      sg = ldv(a.s_g + row + i);
+      mo = ldv(a.m_old + row + i);
+    }
+    release_dependents_once(waited);
+    if (in) gr = sum_partials<U>(c, l, i);
+    Pack<T> dx, dv;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      v.v[u] += a.gamma * (sg.v[u] - g.v[u]) + gr.v[u] - mo.v[u];
+      dx.v[u] = x.v[u] - h.v[u];
+      dv.v[u] = v.v[u] - g.v[u];
+    }
+    const Pack<T> qh = choco_encode<T, Q>(dx, out_h, c.n_pad, i, in, lane, a.live);
+    const Pack<T> qg = choco_encode<T, Q>(dv, out_g, c.n_pad, i, in, lane, a.live);
+    if (in) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        h.v[u] += qh.v[u];
+        g.v[u] += qg.v[u];
+      }
+      stv(a.h + row + i, h);
+      stv(a.v + row + i, v);
+      stv(a.g + row + i, g);
+      stv(a.m_old + row + i, gr);
+    }
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
 // -------------------------------------------------------------------- SGP ----
 // Round k: sgp_mix pulls the in-neighbors' rows (x, w) of round k, x_i <- sum_j A_ij x_j, w_i <- sum_j A_ij w_j,
 // theta_i <- x_i / w_i; sgp_step takes x_i -= alpha_k g_i(theta_i), theta_i <- x_i / w_i and publishes (x_i, w_i).
@@ -1011,6 +1134,21 @@ template <typename T> static cudaError_t launch_choco(const ChocoArgs<T>& a, boo
 }
 template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, false, st); }
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st) { return launch_choco(a, true, st); }
+// as CHOCO: the compressor is a template parameter, and beyond 4 gradient partials the step keeps 8 loads in flight
+template <typename T, int Q> static cudaError_t launch_beer_q(const BeerArgs<T>& a, bool step, cudaStream_t st) {
+  return step ? launch_by_s(beer_step_kernel<T, 4, Q>, beer_step_kernel<T, 8, Q>, a.c, a, st)
+              : launch_one_wave(beer_mix_kernel<T, Q>, a.c, a, st);
+}
+template <typename T> static cudaError_t launch_beer(const BeerArgs<T>& a, bool step, cudaStream_t st) {
+  switch (a.code) {
+    case kCodeNone: return launch_beer_q<T, kCodeNone>(a, step, st);
+    case kCodeInt8: return launch_beer_q<T, kCodeInt8>(a, step, st);
+    case kCodeSign: return launch_beer_q<T, kCodeSign>(a, step, st);
+  }
+  return cudaErrorInvalidValue;
+}
+template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStream_t st) { return launch_beer(a, false, st); }
+template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st) { return launch_beer(a, true, st); }
 
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(sgp_mix_kernel<T>, a.c, a, st);
@@ -1043,6 +1181,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_dsgdm_step<T>(const MomentumArgs<T>&, cudaStream_t);    \
   template cudaError_t launch_choco_mix<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_beer_mix<T>(const BeerArgs<T>&, cudaStream_t);          \
+  template cudaError_t launch_beer_step<T>(const BeerArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_pdg_mix<T>(const PushDigArgs<T>&, cudaStream_t);        \

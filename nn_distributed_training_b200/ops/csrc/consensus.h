@@ -132,6 +132,24 @@ struct ChocoArgs {
   long long code_stride;           // bytes per code row of the published buffer
 };
 
+// BEER (Zhao, Li, Li, Richtárik, Chi 2022): DSGT's gradient tracking with both the parameters and the tracker gossiped
+// through CHOCO's compressed differences.  Two published channels of CHOCO code rows (`code_stride` bytes, layout
+// above): channel 0 the code of theta - h, channel 1 the code of v - g.
+template <typename T>
+struct BeerArgs {
+  Common<T> c;
+  T* h;                            // [L, n_pad] public estimate of theta: the sum of the node's decoded channel-0 codes
+  T* s_h;                          // [L, n_pad] sum_j W_ij h_j (own term included)
+  T* v;                            // [L, n_pad] gradient tracker
+  T* g;                            // [L, n_pad] public estimate of v: the sum of the node's decoded channel-1 codes
+  T* s_g;                          // [L, n_pad] sum_j W_ij g_j (own term included)
+  T* m_old;                        // [L, n_pad] the gradient of the previous round
+  const unsigned* live;            // [n_pad / 32] bit mask of the parameter elements
+  T gamma;                         // consensus step
+  int code;                        // Code
+  long long code_stride;           // bytes per code row of the published buffer
+};
+
 // SGP, Stochastic Gradient Push (Assran et al. 2019): push-sum gossip over a column-stochastic A, on directed graphs.
 // The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
 // A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
@@ -184,6 +202,8 @@ template <typename T> cudaError_t launch_ed_step(const EdArgs<T>& a, cudaStream_
 template <typename T> cudaError_t launch_dsgdm_step(const MomentumArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st);

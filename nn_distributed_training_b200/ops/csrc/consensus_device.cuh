@@ -374,6 +374,78 @@ NNDT_DEVINL Pack<T> choco_decode(const char* row, int n_pad, int i, unsigned lw)
   return d;
 }
 
+// Q(v) of the Vec<T>::N elements at i, stored into the code row `out`; returns dec(Q(v)).  Every lane of the warp calls
+// it: the G = 32 / N lanes holding one 32-element block reduce its scale with xor shuffles, and a lane past the end of
+// the row (`in` false, v = 0) takes part in them and stores nothing.  The same arithmetic as the encoder written out in
+// choco_step_kernel, which keeps its own copy: called through this function, its int8 variants compiled to a different
+// instruction schedule (same instruction count).
+template <typename T, int Q>
+NNDT_DEVINL Pack<T> choco_encode(const Pack<T>& v, char* out, int n_pad, int i, bool in, int lane, const unsigned* live) {
+  constexpr int N = Vec<T>::N;
+  constexpr int G = 32 / N;
+  Pack<T> d;
+  const bool head = (lane & (G - 1)) == 0;      // the lane that stores the block's scale / sign word
+  if (Q == kCodeNone) {
+    d = v;
+    if (in) stv(reinterpret_cast<T*>(out) + i, v);
+  } else if (Q == kCodeInt8) {
+    T m = (T)0;
+#pragma unroll
+    for (int u = 0; u < N; ++u) m = fmax(m, fabs(v.v[u]));
+#pragma unroll
+    for (int o = G / 2; o >= 1; o >>= 1) m = fmax(m, __shfl_xor_sync(0xffffffffu, m, o));
+    const T sc = div_rn(m, (T)127);
+    signed char q[N];
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      const T r = sc > (T)0 ? rint(div_rn(v.v[u], sc)) : (T)0;
+      q[u] = (signed char)fmin(fmax(r, (T)-127), (T)127);
+      d.v[u] = mul_rn((T)q[u], sc);
+    }
+    if (in) {
+      if (N == 4) *reinterpret_cast<int*>(out + i) = *reinterpret_cast<const int*>(q);
+      else *reinterpret_cast<short*>(out + i) = *reinterpret_cast<const short*>(q);
+      if (head) reinterpret_cast<T*>(out + n_pad)[i >> 5] = sc;
+    }
+  } else {
+    const unsigned lw = in ? live[i >> 5] : 0u;
+    // sum |v| over the live elements: in element order within the lane, then halving across the block's lanes
+    T p = (T)0;
+    unsigned bits = 0u;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      const int b = (i & 31) + u;
+      const T av = ((lw >> b) & 1u) ? fabs(v.v[u]) : (T)0;
+      p = u == 0 ? av : p + av;
+      if (v.v[u] >= (T)0) bits |= 1u << b;
+    }
+#pragma unroll
+    for (int o = G / 2; o >= 1; o >>= 1) {
+      p += __shfl_xor_sync(0xffffffffu, p, o);
+      bits |= __shfl_xor_sync(0xffffffffu, bits, o);
+    }
+    const int nl = __popc(lw);
+    const T sc = nl > 0 ? div_rn(p, (T)nl) : (T)0;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      const int b = (i & 31) + u;
+      d.v[u] = ((lw >> b) & 1u) ? (((bits >> b) & 1u) ? sc : -sc) : (T)0;
+    }
+    if (in && head) {
+      reinterpret_cast<unsigned*>(out)[i >> 5] = bits;
+      reinterpret_cast<T*>(out + (n_pad >> 3))[i >> 5] = sc;
+    }
+  }
+  return d;
+}
+
+// ---- BEER (layout in consensus.h): code row of channel `chan` (0: theta - h, 1: v - g) ----
+template <typename T>
+NNDT_DEVINL char* beer_code_row(const BeerArgs<T>& a, int par, int chan, int l) {
+  const Common<T>& c = a.c;
+  return reinterpret_cast<char*>(c.pub) + ((size_t)(par * c.C + chan) * c.pub_L + l) * (size_t)a.code_stride;
+}
+
 // ---- SGP (layout in consensus.h) ----
 template <typename T>
 NNDT_DEVINL T* sgp_row(const SgpArgs<T>& a, int par, int l) {

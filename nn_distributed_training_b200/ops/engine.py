@@ -40,7 +40,7 @@ def schedule_tables(opt, H: int):
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):     # DSGT and Push-DIGing: a constant step
+    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER and Push-DIGing: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -64,10 +64,11 @@ class ConsensusEngine:
         dev, a, pl, ctx = pr.device, pr.arena, pr.placement, pr.ctx
         self.dtype = a.dtype
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging") else 1
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
+        self.beer = opt.alg_name == "beer"
         self.sgp = opt.alg_name == "sgp"
         self.pdg = opt.alg_name == "push_diging"
         push_sum = self.sgp or self.pdg
@@ -75,8 +76,8 @@ class ConsensusEngine:
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
         # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
         # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w (Push-DIGing: both
-        # channels, u with w in the tail and y, have that stride)
-        if self.choco:
+        # channels, u with w in the tail and y, have that stride).  BEER publishes two channels of CHOCO code rows.
+        if self.choco or self.beer:
             self.row_bytes = opt.code_bytes
         elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
@@ -90,6 +91,9 @@ class ConsensusEngine:
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
         if self.choco:
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
+        elif self.beer:
+            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code_h)
+            self.pub[k0 & 1, 1, :L].view(torch.uint8).copy_(opt.code_g)
         elif self.sgp:
             self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.x)
             self.pub_weights(k0 & 1).copy_(opt.w)
@@ -134,6 +138,10 @@ class ConsensusEngine:
         if self.choco and G > 1:
             raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
                              f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
+        if self.beer and G > 1:
+            raise ValueError("beer needs a fixed graph: the planned graph sequence of this problem has "
+                             f"{G} topologies (s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a "
+                             "fixed W)")
         dmax = max(1, max(t.max_degree for t in topos))
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
@@ -229,9 +237,9 @@ class ConsensusEngine:
             ctx.barrier()
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
-        # (CHOCO-SGD, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
+        # (CHOCO-SGD, BEER, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
         # numerators with a weight; complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not self.choco and not push_sum
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not (self.choco or self.beer) and not push_sum
                          and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -308,6 +316,11 @@ class ConsensusEngine:
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
                      code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
+        if self.beer:
+            self.t_live = choco_live_words(opt.live).to(dev)
+            d.update(h=opt.h.data_ptr(), s_h=opt.s_h.data_ptr(), v=opt.v.data_ptr(), g=opt.g.data_ptr(),
+                     s_g=opt.s_g.data_ptr(), m_old=opt.m_old.data_ptr(), live=self.t_live.data_ptr(),
+                     gamma=float(opt.gamma), code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
         if self.sgp:
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
         if self.pdg:

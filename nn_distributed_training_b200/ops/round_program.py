@@ -7,6 +7,7 @@ A round is a short, fixed kernel sequence
     DSGT :  dsgt_mix, fwd/bwd, dsgt_track
     Exact Diffusion:  ed_mix, fwd/bwd, ed_step
     CHOCO-SGD:  choco_mix, fwd/bwd, choco_step
+    BEER:  beer_mix, fwd/bwd, beer_step
     SGP:  sgp_mix, fwd/bwd, sgp_step
     Push-DIGing:  pdg_mix, fwd/bwd, pdg_track
 whose per-round scalars come from device schedules indexed by a device round
@@ -69,6 +70,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.choco_mix()
         grads(0)
         eng.op.choco_step()
+    elif alg == "beer":
+        eng.op.beer_mix()
+        grads(0)
+        eng.op.beer_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -119,10 +124,11 @@ class RoundProgram:
                 pipeline = "resident"
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
-        # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD publishes
-        # codes, SGP and Push-DIGing numerators, so their metric reads the parameter rows (all_theta) at the evaluation
-        # points instead
-        pr._metric_engine = None if (self.eng.choco or self.eng.sgp or self.eng.pdg) else (self.eng, lambda: opt.k)
+        # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
+        # publish codes, SGP and Push-DIGing numerators, so their metric reads the parameter rows (all_theta) at the
+        # evaluation points instead
+        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg)
+                             else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
         self.pipeline = "resident"
@@ -288,6 +294,9 @@ class RoundProgram:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "choco_sgd":
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
+        if opt.alg_name == "beer":              # h, s_h, v, g, s_g and m_old are the optimizer's own rows
+            opt.code_h.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
+            opt.code_g.copy_(eng.pub[opt.k & 1, 1, :L].view(torch.uint8))
 
 
 def run_fused_training(opt, profiler=None):

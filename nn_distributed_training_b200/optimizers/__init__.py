@@ -1,3 +1,4 @@
+from .beer import BEER
 from .choco import ChocoSGD
 from .dinno import DiNNO
 from .dsgd import DSGD
@@ -8,7 +9,8 @@ from .push_diging import PushDIGing
 from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
-              "choco_sgd": ChocoSGD, "sgp": SGP, "push_diging": PushDIGing}
+              "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
+              "push_diging": PushDIGing}
 
 
 def build_optimizer(problem, device, opt_conf):

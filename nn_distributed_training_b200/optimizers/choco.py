@@ -104,8 +104,9 @@ class ChocoSGD(ConsensusOptimizer):
         self.code.copy_(sd["code"].to(self.device))
 
 
-def check_static_plan(graphs):
-    """Raise ``ValueError`` when a planned graph sequence holds more than one topology."""
+def check_static_plan(graphs, alg="choco_sgd", why="s = sum_j W_ij x_hat_j is only valid for a fixed W"):
+    """Raise ``ValueError`` when a planned graph sequence holds more than one topology (``alg`` and ``why`` name the
+    optimizer and its reason in the message)."""
     from ..utils.graph_generation import Topology
     keys = set()
     seen = set()
@@ -115,5 +116,5 @@ def check_static_plan(graphs):
         seen.add(id(g))
         keys.add(Topology(g).key)
         if len(keys) > 1:
-            raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem changes "
-                             "during the run (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
+            raise ValueError(f"{alg} needs a fixed graph: the planned graph sequence of this problem changes "
+                             f"during the run ({why})")

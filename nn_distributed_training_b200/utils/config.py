@@ -15,7 +15,7 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "sgp", "push_diging")
+ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -38,6 +38,7 @@ OPT_SCHEMA = {
     "exact_diffusion": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False},
     "choco_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED,
                   "outer_iterations": REQUIRED, "profile": False},
+    "beer": {"alpha": REQUIRED, "gamma": REQUIRED, "compressor": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
     "sgp": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
     "push_diging": {"alpha": REQUIRED, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
 }
@@ -83,7 +84,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg in ("dsgdm", "exact_diffusion", "choco_sgd", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
+    if alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
     if alg == "dsgdm":
@@ -100,6 +101,15 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         if c.setdefault("update_graph", False):
             raise ConfigError(f"{path}.update_graph: choco_sgd needs a fixed graph (its sum of the neighbors' estimates "
                               f"is only valid for a fixed mixing matrix)")
+    if alg == "beer":
+        if not 0.0 < float(c["gamma"]) <= 1.0:
+            raise ConfigError(f"{path}.gamma must be in (0, 1] (got {c['gamma']!r})")
+        if c["compressor"] not in CHOCO_COMPRESSORS:
+            raise ConfigError(f"{path}.compressor must be one of {'|'.join(CHOCO_COMPRESSORS)} (got {c['compressor']!r})")
+        # s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a fixed W: the graph is never refreshed
+        if c.setdefault("update_graph", False):
+            raise ConfigError(f"{path}.update_graph: beer needs a fixed graph (its sums of the neighbors' estimates "
+                              f"are only valid for a fixed mixing matrix)")
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c
