@@ -281,6 +281,33 @@ def beer_step_(theta: torch.Tensor, h: torch.Tensor, v: torch.Tensor, g: torch.T
     return codes_h, codes_g
 
 
+# ----------------------------------------------------------------- K-GT ----
+def kgt_mix_(theta: torch.Tensor, c: Optional[torch.Tensor], theta_all: torch.Tensor, y_all: Optional[torch.Tensor],
+             y: Optional[torch.Tensor], w_rows: torch.Tensor):
+    """``theta_i <- sum_j W_ij theta_j``; with a correction row ``c`` also ``c_i += sum_j W_ij y_j - y_i`` (own terms
+    included).  Without it this is DSGD's mix."""
+    theta.copy_(dsgd_mix(theta_all, w_rows))
+    if c is not None:
+        c.add_(dsgd_mix(y_all, w_rows) - y)
+
+
+def kgt_step_(theta: torch.Tensor, c: Optional[torch.Tensor], d: Optional[torch.Tensor], grad: torch.Tensor,
+              alpha: float, p: int, K: int) -> Optional[torch.Tensor]:
+    """Local step ``p`` of ``K``: ``u = g + c`` (``g`` without ``c``), ``theta -= alpha u``, ``d = u`` (p = 0) or
+    ``d += u``.  Returns ``y = d / K`` on the last step with a correction row, else ``None``.  Without ``c`` this is
+    DSGD's step."""
+    if c is None:
+        dsgd_step_(theta, grad, alpha)
+        return None
+    u = grad + c
+    theta.sub_(alpha * u)
+    if p == 0:
+        d.copy_(u)
+    else:
+        d.add_(u)
+    return d / K if p == K - 1 else None
+
+
 # ------------------------------------------------------------------ SGP ----
 # Push-sum (Stochastic Gradient Push): numerator rows x [L, n_pad] and float64 weights w [L].  The combine weights are
 # the column-stochastic A of Topology.push_weights, rounded to the arena dtype; w is mixed with those same rounded

@@ -124,11 +124,12 @@ struct ConsensusOp {
   bool mo_qg = false;
   consensus::ChocoArgs<T> ch{};
   consensus::BeerArgs<T> be{};
+  consensus::KgtArgs<T> kg{};
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -143,6 +144,8 @@ struct ConsensusOp {
     be.h = ptr<T>(d, "h"); be.s_h = ptr<T>(d, "s_h"); be.v = ptr<T>(d, "v"); be.g = ptr<T>(d, "g");
     be.s_g = ptr<T>(d, "s_g"); be.m_old = ptr<T>(d, "m_old");
     be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride;
+    kg.corr = ptr<T>(d, "corr"); kg.dacc = ptr<T>(d, "dacc");
+    kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
@@ -193,6 +196,20 @@ struct ConsensusOp {
   void beer_step() {
     beer_check("beer_step");
     check(consensus::launch_beer_step<T>(be, cur_stream()), "beer_step");
+  }
+  void kgt_mix() {
+    if (!kg.correction || kg.corr == nullptr || c.C != 2)
+      throw std::runtime_error("kgt_mix needs correction mode, the K-GT row `corr` and two published channels "
+                               "(local DSGD mixes with dsgd_mix)");
+    check(consensus::launch_kgt_mix<T>(kg, cur_stream()), "kgt_mix");
+  }
+  void kgt_step(int step) {
+    if (kg.K < 1 || step < 0 || step >= kg.K)
+      throw std::runtime_error("kgt_step: step " + std::to_string(step) + " outside 0.." + std::to_string(kg.K - 1));
+    if (kg.correction && (kg.corr == nullptr || kg.dacc == nullptr || c.C != 2))
+      throw std::runtime_error("kgt_step with correction needs the K-GT rows `corr`, `dacc` and two published channels");
+    kg.step = step;
+    check(consensus::launch_kgt_step<T>(kg, cur_stream()), "kgt_step");
   }
   void sgp_check(const char* what) const {
     if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0)
@@ -256,6 +273,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("choco_step", &ConsensusOp<T>::choco_step)
       .def("beer_mix", &ConsensusOp<T>::beer_mix)
       .def("beer_step", &ConsensusOp<T>::beer_step)
+      .def("kgt_mix", &ConsensusOp<T>::kgt_mix)
+      .def("kgt_step", &ConsensusOp<T>::kgt_step)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
       .def("sgp_step", &ConsensusOp<T>::sgp_step)
       .def("pdg_mix", &ConsensusOp<T>::pdg_mix)

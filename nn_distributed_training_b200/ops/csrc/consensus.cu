@@ -9,6 +9,7 @@
 // DSGD with momentum (no reference counterpart, optimizers/dsgdm.py)       -> dsgd_mix / dsgdm_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
 // BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
+// K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
@@ -787,6 +788,128 @@ __global__ void __launch_bounds__(THREADS) beer_step_kernel(const BeerArgs<T> a)
   end_step(c, l, ri.k, true);
 }
 
+// -------------------------------------------------------------------- K-GT ----
+// Channel 0 of the published buffer is theta, channel 1 the tracker y (correction mode).  Round k: kgt_mix pulls the
+// rows published at the end of round k-1, theta_i <- sum_j W_ij theta_j and c_i += sum_j W_ij y_j - y_i (own terms
+// included); then K x [fwd/bwd, kgt_step(p)].  Local DSGD mixes with dsgd_mix_kernel and publishes theta only.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) kgt_mix_kernel(const KgtArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const T* ys = pub_row(c, ri.par, 1, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> y = ldv(ys + i);
+    Pack<T> cr = ldv(a.corr + row + i);
+    if (c.sum_mode) {     // W = 11^T / N: theta_i = S_theta / N, c_i += S_y / N - y_i
+      const DPack<N> st = network_sum(c, ri.par, 0, i);
+      const DPack<N> sy = network_sum(c, ri.par, 1, i);
+      Pack<T> th;
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        th.v[u] = (T)(st.v[u] / (double)c.n_total);
+        cr.v[u] += (T)(sy.v[u] / (double)c.n_total - (double)y.v[u]);
+      }
+      stv(c.theta + row + i, th);
+      stv(a.corr + row + i, cr);
+      continue;
+    }
+    Pack<T> th = ldv(c.theta + row + i), yw;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      th.v[u] *= ws;
+      yw.v[u] = ws * y.v[u];
+    }
+    // for_neighbors<2> written out, as in dsgt_mix: two channels of two neighbors in flight
+    for (int e0 = 0; e0 < deg; e0 += 2) {
+      Pack<T> qt[2], qy[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          qt[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
+          qy[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 1) + i);
+        }
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          const T we = w[e0 + j];
+#pragma unroll
+          for (int u = 0; u < N; ++u) {
+            th.v[u] += we * qt[j].v[u];
+            yw.v[u] += we * qy[j].v[u];
+          }
+        }
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) cr.v[u] += yw.v[u] - y.v[u];
+    stv(c.theta + row + i, th);
+    stv(a.corr + row + i, cr);
+  }
+}
+
+// Local step p of K: u = g + c (CORR; g without it), theta -= alpha_k u, d = u (p = 0) or d + u.  The last step
+// publishes theta and y = d / K (one IEEE division, exact for K = 1) into the next parity and ends the round; the
+// others keep theta and d local and only advance the draw counters.  Local DSGD writes DSGD's step, th -= alpha * g.
+// The 4-deep variant is held to 64 registers (4 CTAs per SM) and the 8-deep one to 128, with no spills: left to the
+// compiler, the fp32 IEEE division took the 4-deep correction step to 125 and the fp64 8-deep local step spilled at 80.
+template <typename T, int U, bool CORR>
+__global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 2) kgt_step_kernel(const KgtArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const bool first = a.step == 0, last = a.step == a.K - 1;
+  const T kf = (T)a.K;
+  const size_t row = (size_t)l * c.n_pad;
+  // theta, c and d (written by the mix or the previous step, two launches back) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    Pack<T> cr, dd;
+    if (CORR) {
+      cr = ldv(a.corr + row + i);
+      if (!first) dd = ldv(a.dacc + row + i);
+    }
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    if (CORR) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const T uu = g.v[u] + cr.v[u];
+        th.v[u] -= alpha * uu;
+        dd.v[u] = first ? uu : dd.v[u] + uu;
+      }
+    } else {
+#pragma unroll
+      for (int u = 0; u < N; ++u) th.v[u] -= alpha * g.v[u];
+    }
+    stv(c.theta + row + i, th);
+    if (last) {
+      stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+      if (CORR) {
+        Pack<T> y;
+#pragma unroll
+        for (int u = 0; u < N; ++u) y.v[u] = div_rn(dd.v[u], kf);
+        stv(pub_row(c, ri.par ^ 1, 1, l) + i, y);
+      }
+    } else if (CORR) {
+      stv(a.dacc + row + i, dd);
+    }
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, last);
+}
+
 // -------------------------------------------------------------------- SGP ----
 // Round k: sgp_mix pulls the in-neighbors' rows (x, w) of round k, x_i <- sum_j A_ij x_j, w_i <- sum_j A_ij w_j,
 // theta_i <- x_i / w_i; sgp_step takes x_i -= alpha_k g_i(theta_i), theta_i <- x_i / w_i and publishes (x_i, w_i).
@@ -1150,6 +1273,18 @@ template <typename T> static cudaError_t launch_beer(const BeerArgs<T>& a, bool 
 template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStream_t st) { return launch_beer(a, false, st); }
 template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st) { return launch_beer(a, true, st); }
 
+template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(kgt_mix_kernel<T>, a.c, a, st);
+}
+// the correction is a template parameter (see dsgt_mix above); beyond 4 gradient partials the step keeps 8 loads in
+// flight, as sgp_step
+template <typename T, bool CORR> static cudaError_t launch_kgt(const KgtArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(kgt_step_kernel<T, 4, CORR>, kgt_step_kernel<T, 8, CORR>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st) {
+  return a.correction ? launch_kgt<T, true>(a, st) : launch_kgt<T, false>(a, st);
+}
+
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(sgp_mix_kernel<T>, a.c, a, st);
 }
@@ -1183,6 +1318,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_choco_step<T>(const ChocoArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_beer_mix<T>(const BeerArgs<T>&, cudaStream_t);          \
   template cudaError_t launch_beer_step<T>(const BeerArgs<T>&, cudaStream_t);         \
+  template cudaError_t launch_kgt_mix<T>(const KgtArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_pdg_mix<T>(const PushDigArgs<T>&, cudaStream_t);        \

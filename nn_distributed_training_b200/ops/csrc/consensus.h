@@ -150,6 +150,18 @@ struct BeerArgs {
   long long code_stride;           // bytes per code row of the published buffer
 };
 
+// K-GT (Liu, Lin, Koloskova, Stich 2023): gradient tracking with `K` local steps per communication round, and local
+// DSGD (Koloskova et al. 2020) when `correction` is 0.  Correction mode publishes two channels, theta and y (the mean
+// direction of the round's steps); local DSGD publishes theta only and mixes with dsgd_mix_kernel.  `step` is the
+// index of the launch within the round, 0 .. K-1; the last one publishes.
+template <typename T>
+struct KgtArgs {
+  Common<T> c;
+  T* corr;                         // [L, n_pad] correction c_i, zero at the start (correction mode)
+  T* dacc;                         // [L, n_pad] sum of the round's directions g + c; not read before step 0 writes it
+  int step, K, correction;
+};
+
 // SGP, Stochastic Gradient Push (Assran et al. 2019): push-sum gossip over a column-stochastic A, on directed graphs.
 // The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
 // A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
@@ -204,6 +216,8 @@ template <typename T> cudaError_t launch_choco_mix(const ChocoArgs<T>& a, cudaSt
 template <typename T> cudaError_t launch_choco_step(const ChocoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st);

@@ -40,7 +40,7 @@ def schedule_tables(opt, H: int):
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER and Push-DIGing: a constant step
+    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing and K-GT: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -64,7 +64,9 @@ class ConsensusEngine:
         dev, a, pl, ctx = pr.device, pr.arena, pr.placement, pr.ctx
         self.dtype = a.dtype
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") else 1
+        # K-GT publishes its tracker y in channel 1; local DSGD (kgt without correction) publishes theta only
+        kgt_corr = opt.alg_name == "kgt" and opt.correction
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") or kgt_corr else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
@@ -103,7 +105,7 @@ class ConsensusEngine:
             self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
-        if opt.alg_name == "dsgt" and getattr(opt, "_initialised", False):
+        if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
             self.pub[k0 & 1, 1, :L].copy_(opt.y)
 
         # ---- schedules ----------------------------------------------------------
@@ -308,6 +310,9 @@ class ConsensusEngine:
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
         if opt.alg_name == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
+        if opt.alg_name == "kgt":
+            d.update(local_steps=opt.local_steps, correction=int(opt.correction),
+                     corr=opt.c.data_ptr() if kgt_corr else None, dacc=opt.d.data_ptr() if kgt_corr else None)
         if opt.alg_name == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
@@ -340,7 +345,8 @@ class ConsensusEngine:
     def bytes_per_round(self) -> Dict[str, int]:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
         neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
-        counted).  An SGP or Push-DIGing row includes its 16-byte tail."""
+        counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
+        steps."""
         deg = int(self.t_deg[0].sum().item())
         return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg}
 

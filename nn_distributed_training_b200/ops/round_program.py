@@ -10,6 +10,7 @@ A round is a short, fixed kernel sequence
     BEER:  beer_mix, fwd/bwd, beer_step
     SGP:  sgp_mix, fwd/bwd, sgp_step
     Push-DIGing:  pdg_mix, fwd/bwd, pdg_track
+    K-GT:  kgt_mix, [fwd/bwd, kgt_step(p)] x local_steps       (local DSGD: dsgd_mix in place of kgt_mix)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -74,6 +75,14 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.beer_mix()
         grads(0)
         eng.op.beer_step()
+    elif alg == "kgt":
+        if opt.correction:
+            eng.op.kgt_mix()
+        else:
+            eng.op.dsgd_mix()
+        for p in range(opt.local_steps):
+            grads(p)
+            eng.op.kgt_step(p)
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -94,7 +103,9 @@ def _collect_before_capture():
 
 
 def draws_per_round(opt) -> int:
-    return opt.pits if opt.alg_name == "dinno" else 1
+    if opt.alg_name == "dinno":
+        return opt.pits
+    return opt.local_steps if opt.alg_name == "kgt" else 1
 
 
 class RoundProgram:
@@ -159,7 +170,9 @@ class RoundProgram:
         n = 1 if self.eng.sum_mode else 0
         if self.host_mode:
             n += 1
-        return n + (2 * self.opt.pits if self.opt.alg_name == "dinno" else 3)
+        if self.opt.alg_name == "dinno":
+            return n + 2 * self.opt.pits
+        return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
         pr = self.pr
@@ -286,6 +299,8 @@ class RoundProgram:
         if opt.alg_name == "dsgt":
             par = opt.k & 1
             opt.y.copy_(eng.pub[par, 1, :L])
+        if opt.alg_name == "kgt" and opt.correction:      # c is the optimizer's own row; d is dead between rounds
+            opt.y.copy_(eng.pub[opt.k & 1, 1, :L])
         if opt.alg_name == "push_diging":       # y is the first n_pad elements of channel 1 (u and w are shared)
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:

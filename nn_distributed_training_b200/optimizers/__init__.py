@@ -5,12 +5,13 @@ from .dsgd import DSGD
 from .dsgdm import DSGDm
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
+from .kgt import KGT
 from .push_diging import PushDIGing
 from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
-              "push_diging": PushDIGing}
+              "push_diging": PushDIGing, "kgt": KGT}
 
 
 def build_optimizer(problem, device, opt_conf):

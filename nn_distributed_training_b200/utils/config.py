@@ -15,7 +15,7 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging")
+ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -41,6 +41,8 @@ OPT_SCHEMA = {
     "beer": {"alpha": REQUIRED, "gamma": REQUIRED, "compressor": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
     "sgp": {"alpha0": REQUIRED, "mu": 0.0, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
     "push_diging": {"alpha": REQUIRED, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
+    "kgt": {"alpha": REQUIRED, "local_steps": REQUIRED, "correction": True, "outer_iterations": REQUIRED,
+            "profile": False, "update_graph": True},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -84,7 +86,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging") and c.get("mixing_order", "jacobi") != "jacobi":
+    if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt")
+            and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
     if alg == "dsgdm":
@@ -110,6 +113,14 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         if c.setdefault("update_graph", False):
             raise ConfigError(f"{path}.update_graph: beer needs a fixed graph (its sums of the neighbors' estimates "
                               f"are only valid for a fixed mixing matrix)")
+    if alg == "kgt":
+        ls = c["local_steps"]
+        if isinstance(ls, bool) or not isinstance(ls, int) or ls < 1:
+            raise ConfigError(f"{path}.local_steps must be an integer >= 1 (got {ls!r})")
+        if not float(c["alpha"]) > 0.0:
+            raise ConfigError(f"{path}.alpha must be > 0 (got {c['alpha']!r})")
+        if not isinstance(c["correction"], bool):
+            raise ConfigError(f"{path}.correction must be true or false (got {c['correction']!r})")
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c
