@@ -308,6 +308,76 @@ def kgt_step_(theta: torch.Tensor, c: Optional[torch.Tensor], d: Optional[torch.
     return d / K if p == K - 1 else None
 
 
+# ---------------------------------------------------------- ClippedGossip ----
+ATTACK_CODE = {"sign_flip": 1, "alie": 2}      # consensus.h: Attack (0 = honest)
+CLIP_SLACK = 1e-6      # consensus.h: kClipSlack, a prefix of (rounded) weights fits in delta up to this
+
+
+def cg_distances(theta_i: torch.Tensor, nbr_rows: torch.Tensor) -> np.ndarray:
+    """``d_ij = |theta_j^pub - theta_i|_2`` of every neighbor row (``nbr_rows`` [deg, n_pad]), accumulated in fp64."""
+    if nbr_rows.shape[0] == 0:
+        return np.zeros(0)
+    diff = nbr_rows.double() - theta_i.double()
+    return (diff * diff).sum(1).sqrt().cpu().numpy()
+
+
+def cg_factors(d: np.ndarray, w: np.ndarray, delta: float) -> Tuple[np.ndarray, float]:
+    """Radius and clipping factors of one node: the neighbors in order of decreasing distance (ties: the smaller index
+    first) are clipped while their Metropolis weights ``w`` sum to at most ``delta`` (up to ``CLIP_SLACK``); ``tau`` is the distance of the
+    first one that does not fit (0 when all fit) and the factor of edge j is ``min(1, tau / d_ij)`` (1 at d_ij = 0)."""
+    order = sorted(range(len(d)), key=lambda e: (-d[e], e))
+    cum, tau = 0.0, 0.0
+    for e in order:
+        if cum + float(w[e]) > delta + CLIP_SLACK:
+            tau = float(d[e])
+            break
+        cum += float(w[e])
+    f = np.array([tau / d[e] if d[e] > tau else 1.0 for e in range(len(d))])
+    return f, tau
+
+
+def cg_mix_(theta: torch.Tensor, pub_all: torch.Tensor, w_rows: np.ndarray, nbrs, lo: int, delta: float):
+    """Self-centred clipped mix of the local rows ``theta`` [L, n_pad]:
+    ``theta_i <- theta_i + sum_j W_ij min(1, tau_i / d_ij) (theta_j^pub - theta_i)``, in neighbor order, the
+    coefficient ``W_ij * factor`` rounded to the row dtype once (as cg_mix_kernel).  ``pub_all`` [N, n_pad] holds every
+    node's published row, ``w_rows`` the Metropolis matrix (host, rounded to the row dtype), ``nbrs[g]`` the neighbors
+    of node g in table order.  Returns the factors of every local node."""
+    out = []
+    for l in range(theta.shape[0]):
+        nb = list(nbrs[lo + l])
+        th0 = theta[l].clone()
+        rows = pub_all[nb] if nb else pub_all[:0]
+        w = np.array([float(w_rows[lo + l, j]) for j in nb])
+        f, _ = cg_factors(cg_distances(th0, rows), w, delta)
+        acc = th0.clone()
+        for e in range(len(nb)):
+            coef = torch.tensor(w[e] * f[e], dtype=theta.dtype)
+            acc += coef * (rows[e] - th0)
+        theta[l].copy_(acc)
+        out.append(f)
+    return out
+
+
+def cg_publish_(pub: torch.Tensor, theta: torch.Tensor, pub_all: torch.Tensor, attack, nbrs, byz, lo: int,
+                scale: float, z: float):
+    """Write into ``pub`` [L, n_pad] the rows the local nodes publish after their step.  ``attack[l]``: 0 honest (theta), 1 sign flip
+    (``-scale theta``), 2 ALIE (``mu - z sigma``, the fp64 element-wise mean and population standard deviation of the
+    node's honest neighbors' rows in ``pub_all``, the rows read this round; theta without an honest neighbor)."""
+    out = theta.clone()          # pub_all may alias pub (one process holds every row)
+    s = torch.tensor(scale, dtype=theta.dtype)
+    for l, code in enumerate(attack):
+        if code == 1:
+            out[l] = -(s * theta[l])
+        elif code == 2:
+            hon = [j for j in nbrs[lo + l] if j not in byz]
+            if hon:
+                x = pub_all[hon].double()
+                mu = x.mean(0)
+                sigma = ((x - mu) ** 2).mean(0).sqrt()
+                out[l] = (mu - z * sigma).to(theta.dtype)
+    pub.copy_(out)
+
+
 # ------------------------------------------------------------------ SGP ----
 # Push-sum (Stochastic Gradient Push): numerator rows x [L, n_pad] and float64 weights w [L].  The combine weights are
 # the column-stochastic A of Topology.push_weights, rounded to the arena dtype; w is mixed with those same rounded

@@ -125,11 +125,13 @@ struct ConsensusOp {
   consensus::ChocoArgs<T> ch{};
   consensus::BeerArgs<T> be{};
   consensus::KgtArgs<T> kg{};
+  consensus::ClipArgs<T> cg{};
+  int cg_adaptive = 0;
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; cg.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -146,6 +148,10 @@ struct ConsensusOp {
     be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride;
     kg.corr = ptr<T>(d, "corr"); kg.dacc = ptr<T>(d, "dacc");
     kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
+    cg.dist_part = ptr<double>(d, "dist_part"); cg.pstride = geti(d, "pstride", 0);
+    cg.attack = ptr<const int>(d, "attack"); cg.nbr_byz = ptr<const int>(d, "nbr_byz");
+    cg.delta = getf(d, "clip_delta", 0.0); cg.scale = getf(d, "attack_scale", 1.0); cg.z = getf(d, "attack_z", 1.0);
+    cg_adaptive = geti(d, "clip_adaptive", 0);
     dn.dual = ptr<T>(d, "dual"); dn.delta = ptr<T>(d, "delta"); dn.m = ptr<T>(d, "m"); dn.v = ptr<T>(d, "v");
     dn.pits = geti(d, "pits", 1); dn.opt = geti(d, "opt", 1); dn.persistent = geti(d, "persistent", 0);
     gt.g_old = ptr<T>(d, "g_old");
@@ -211,6 +217,27 @@ struct ConsensusOp {
     kg.step = step;
     check(consensus::launch_kgt_step<T>(kg, cur_stream()), "kgt_step");
   }
+  void cg_check(const char* what, bool clip) const {
+    if (c.C != 1 || c.sum_mode)
+      throw std::runtime_error(std::string(what) + " needs one published channel and the pointer-table neighbors");
+    if (clip && (!cg_adaptive || cg.dist_part == nullptr || cg.pstride <= 0 || c.dmax > consensus::kClipMaxDeg))
+      throw std::runtime_error(std::string(what) + " needs clip: adaptive, the distance partials `dist_part` with "
+                               "`pstride` and at most " + std::to_string(consensus::kClipMaxDeg) + " neighbors per node");
+    if (cg.attack != nullptr && cg.nbr_byz == nullptr)
+      throw std::runtime_error(std::string(what) + " with attackers needs the Byzantine-neighbor table `nbr_byz`");
+  }
+  void cg_dist() {
+    cg_check("cg_dist", true);
+    check(consensus::launch_cg_dist<T>(cg, cur_stream()), "cg_dist");
+  }
+  void cg_mix() {
+    cg_check("cg_mix", true);
+    check(consensus::launch_cg_mix<T>(cg, cur_stream()), "cg_mix");
+  }
+  void cg_step() {
+    cg_check("cg_step", false);
+    check(consensus::launch_cg_step<T>(cg, cur_stream()), "cg_step");
+  }
   void sgp_check(const char* what) const {
     if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0)
       throw std::runtime_error(std::string(what) + " needs the SGP rows `x`, `w` and `row_stride`");
@@ -275,6 +302,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("beer_step", &ConsensusOp<T>::beer_step)
       .def("kgt_mix", &ConsensusOp<T>::kgt_mix)
       .def("kgt_step", &ConsensusOp<T>::kgt_step)
+      .def("cg_dist", &ConsensusOp<T>::cg_dist)
+      .def("cg_mix", &ConsensusOp<T>::cg_mix)
+      .def("cg_step", &ConsensusOp<T>::cg_step)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
       .def("sgp_step", &ConsensusOp<T>::sgp_step)
       .def("pdg_mix", &ConsensusOp<T>::pdg_mix)

@@ -10,6 +10,7 @@
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
 // BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
+// ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
@@ -910,6 +911,194 @@ __global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 2) kgt_step_kernel(const
   end_step(c, l, ri.k, last);
 }
 
+// ----------------------------------------------------------- ClippedGossip ----
+// Round k (layout and rules in consensus.h): cg_dist, cg_mix, fwd/bwd, cg_step; with `clip: none` dsgd_mix replaces
+// the first two.  A clipped edge needs its distance over the whole row before any element is mixed, and the row is
+// spread over the CTAs of the node, so the distances take a launch of their own: cg_dist writes one fp64 partial sum
+// per fixed chunk of the row, and cg_mix, after the programmatic-dependency wait, adds them in chunk order.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) cg_dist_kernel(const ClipArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const size_t row = (size_t)l * c.n_pad;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nchunk = cg_chunks(c);
+  __shared__ double red[THREADS / 32][4];
+  // four neighbors per pass, one partial per chunk of THREADS * N elements with a fixed-order block reduction: the
+  // partials, and so the distances, do not depend on the grid (the number of local nodes, the GPU's SM count)
+  for (int e0 = 0; e0 < deg; e0 += 4) {
+    for (int ch = blockIdx.x; ch < nchunk; ch += gridDim.x) {
+      const int i = (ch * THREADS + threadIdx.x) * N;
+      double s[4] = {0.0, 0.0, 0.0, 0.0};
+      if (i < c.n_pad) {
+        const Pack<T> th = ldv(c.theta + row + i);
+        Pack<T> q[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (e0 + j < deg) q[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (e0 + j < deg) {
+#pragma unroll
+            for (int u = 0; u < N; ++u) {
+              const double d = (double)q[j].v[u] - (double)th.v[u];
+              s[j] += d * d;
+            }
+          }
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+#pragma unroll
+        for (int o = 16; o >= 1; o >>= 1) s[j] += __shfl_xor_sync(0xffffffffu, s[j], o);
+        if (lane == 0) red[warp][j] = s[j];
+      }
+      __syncthreads();
+      if ((int)threadIdx.x < 4 && e0 + (int)threadIdx.x < deg) {
+        double t = red[0][threadIdx.x];
+#pragma unroll
+        for (int w = 1; w < THREADS / 32; ++w) t += red[w][threadIdx.x];
+        a.dist_part[((size_t)l * c.dmax + e0 + threadIdx.x) * a.pstride + ch] = t;
+      }
+      __syncthreads();
+    }
+  }
+}
+
+// Every CTA of node l sums the distance partials in chunk order (so all of them agree on the distances), thread 0 picks
+// the radius: it walks the neighbors from the farthest (ties: the smaller index first) while their Metropolis weights
+// sum to at most delta (up to kClipSlack), and tau is the distance of the first neighbor that does not fit (0 when all
+// fit).  Then the self-centred mix theta_i + sum_j W_ij min(1, tau / d_ij) (theta_j - theta_i) of the CTA's slice.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) cg_mix_kernel(const ClipArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  __shared__ double dist[kClipMaxDeg];
+  __shared__ T coef[kClipMaxDeg];
+  __shared__ bool clipped[kClipMaxDeg];
+  for (int e = threadIdx.x; e < deg; e += THREADS) {
+    const double* p = a.dist_part + ((size_t)l * c.dmax + e) * a.pstride;
+    double s = 0.0;
+    const int nchunk = cg_chunks(c);
+    for (int b = 0; b < nchunk; ++b) s += p[b];
+    dist[e] = sqrt(s);
+    clipped[e] = false;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double cum = 0.0, tau = 0.0;
+    for (int t = 0; t < deg; ++t) {
+      int b = -1;
+      for (int e = 0; e < deg; ++e)
+        if (!clipped[e] && (b < 0 || dist[e] > dist[b])) b = e;
+      if (cum + (double)w[b] > a.delta + kClipSlack) { tau = dist[b]; break; }
+      cum += (double)w[b];
+      clipped[b] = true;
+    }
+    for (int e = 0; e < deg; ++e) coef[e] = dist[e] > tau ? (T)((double)w[e] * (tau / dist[e])) : w[e];
+  }
+  __syncthreads();
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> th0 = ldv(c.theta + row + i);
+    Pack<T> th = th0;
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
+                       const T ce = coef[e];
+#pragma unroll
+                       for (int u = 0; u < N; ++u) th.v[u] += ce * (q.v[u] - th0.v[u]);
+                     });
+    stv(c.theta + row + i, th);
+  }
+}
+
+// ALIE row of a Byzantine node at element i: mu - z sigma, the element-wise mean and population standard deviation
+// (fp64) of its honest neighbors' rows of round k; its own theta when it has no honest neighbor.  These are the rows
+// cg_mix read this round: the round-start wait that covered those reads still holds, because no neighbor overwrites
+// them before this node has published round k + 1 (DESIGN §2.8).
+template <typename T>
+NNDT_DEVINL Pack<T> alie_row(const ClipArgs<T>& a, const RoundInfo<T>& ri, int l, int i, const Pack<T>& th) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int deg = c.deg[ri.gid * c.L + l];
+  const int* byz = a.nbr_byz + (size_t)(ri.gid * c.L + l) * c.dmax;
+  double mu[N], var[N];
+#pragma unroll
+  for (int u = 0; u < N; ++u) mu[u] = var[u] = 0.0;
+  int h = 0;
+  for (int e = 0; e < deg; ++e)
+    if (!byz[e]) {
+      const Pack<T> q = ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) mu[u] += (double)q.v[u];
+      ++h;
+    }
+  if (h == 0) return th;
+#pragma unroll
+  for (int u = 0; u < N; ++u) mu[u] /= (double)h;
+  for (int e = 0; e < deg; ++e)
+    if (!byz[e]) {
+      const Pack<T> q = ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const double d = (double)q.v[u] - mu[u];
+        var[u] += d * d;
+      }
+    }
+  Pack<T> r;
+#pragma unroll
+  for (int u = 0; u < N; ++u) r.v[u] = (T)(mu[u] - a.z * sqrt(var[u] / (double)h));
+  return r;
+}
+
+// dsgd_step's arithmetic, written out identically; with ATK a node's attack code picks the row it publishes: theta
+// (honest), -scale theta (sign flip) or the ALIE row.  ATK is false on a rank that hosts no attacker.
+template <typename T, int U, bool ATK>
+__global__ void __launch_bounds__(THREADS) cg_step_kernel(const ClipArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  const int atk = ATK ? a.attack[l] : (int)kHonest;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] -= alpha * g.v[u];
+    stv(c.theta + row + i, th);
+    if (atk == kHonest) {
+      stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+    } else if (atk == kSignFlip) {
+      const T s = (T)a.scale;
+      Pack<T> p;
+#pragma unroll
+      for (int u = 0; u < N; ++u) p.v[u] = -(s * th.v[u]);
+      stv(pub_row(c, ri.par ^ 1, 0, l) + i, p);
+    }
+  }
+  // the ALIE rows in a loop of their own, over the thread's own stores of theta: inside the step loop the fp64
+  // square root's slow-path call spilled the gradient loads
+  if (atk == kAlie)
+    for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N)
+      stv(pub_row(c, ri.par ^ 1, 0, l) + i, alie_row(a, ri, l, i, ldv(c.theta + row + i)));
+  end_step(c, l, ri.k, true);
+}
+
 // -------------------------------------------------------------------- SGP ----
 // Round k: sgp_mix pulls the in-neighbors' rows (x, w) of round k, x_i <- sum_j A_ij x_j, w_i <- sum_j A_ij w_j,
 // theta_i <- x_i / w_i; sgp_step takes x_i -= alpha_k g_i(theta_i), theta_i <- x_i / w_i and publishes (x_i, w_i).
@@ -1285,6 +1474,22 @@ template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStrea
   return a.correction ? launch_kgt<T, true>(a, st) : launch_kgt<T, false>(a, st);
 }
 
+template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st) {
+  if (cg_chunks(a.c) > a.pstride) return cudaErrorInvalidValue;
+  return launch_one_wave(cg_dist_kernel<T>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st) {
+  if (cg_chunks(a.c) > a.pstride) return cudaErrorInvalidValue;
+  return launch_one_wave(cg_mix_kernel<T>, a.c, a, st);
+}
+// beyond 4 gradient partials the step keeps 8 loads in flight, as sgp_step: 16 spilled in fp32, as dsgd_step's does
+// (the summation order is the same for any depth).  A rank with an attacker keeps 4 in flight at any count: the fp32
+// 8-deep attack variant spilled around the fp64 square root's slow-path call.
+template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st) {
+  if (a.attack == nullptr) return launch_by_s(cg_step_kernel<T, 4, false>, cg_step_kernel<T, 8, false>, a.c, a, st);
+  return launch_one_wave(cg_step_kernel<T, 4, true>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(sgp_mix_kernel<T>, a.c, a, st);
 }
@@ -1320,6 +1525,9 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_beer_step<T>(const BeerArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_kgt_mix<T>(const KgtArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_cg_dist<T>(const ClipArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_cg_mix<T>(const ClipArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_cg_step<T>(const ClipArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_pdg_mix<T>(const PushDigArgs<T>&, cudaStream_t);        \

@@ -162,6 +162,31 @@ struct KgtArgs {
   int step, K, correction;
 };
 
+// ClippedGossip (He, Karimireddy, Jaggi 2022): DSGD's single published channel with a self-centred clipped mix, and
+// Byzantine nodes that publish an attack row instead of theta.  Round k: cg_dist reduces the squared
+// distances |theta_j^pub - theta_i|^2 of every neighbor, one partial per fixed chunk of the row, into dist_part; cg_mix
+// sums the partials in chunk order (every CTA of a node gets the same distances), picks the radius tau_i and mixes
+//   theta_i <- theta_i + sum_j W_ij min(1, tau_i / d_ij) (theta_j^pub - theta_i);
+// cg_step is dsgd_step, and a Byzantine node publishes -scale theta_i (sign flip) or mu - z sigma of its honest
+// neighbors' rows of round k (ALIE) in place of theta_i.
+enum Attack : int { kHonest = 0, kSignFlip = 1, kAlie = 2 };
+constexpr int kClipMaxDeg = 128;   // neighbors per node cg_mix sorts in shared memory
+// a prefix of weights fits in delta up to this slack: the weights of an fp32 table are rounded (1/10 becomes
+// 0.100000001), and two of them must still fit in delta = 0.2
+constexpr double kClipSlack = 1e-6;
+
+template <typename T>
+struct ClipArgs {
+  Common<T> c;
+  double* dist_part;               // [L, dmax, pstride] partial sums of the squared distances, one per chunk of
+                                   // THREADS * (16 / sizeof(T)) elements of the row
+  int pstride;                     // >= the chunk count of a row
+  const int* attack;               // [L] Attack code of each local node, nullptr = no attacker on this rank
+  const int* nbr_byz;              // [G, L, dmax] 1 when the neighbor is Byzantine (ALIE averages the others)
+  double delta;                    // Metropolis weight of the neighbors that may be clipped
+  double scale, z;                 // sign-flip scale, ALIE's z
+};
+
 // SGP, Stochastic Gradient Push (Assran et al. 2019): push-sum gossip over a column-stochastic A, on directed graphs.
 // The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
 // A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
@@ -218,6 +243,9 @@ template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st);

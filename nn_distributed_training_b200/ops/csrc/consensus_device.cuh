@@ -446,6 +446,12 @@ NNDT_DEVINL char* beer_code_row(const BeerArgs<T>& a, int par, int chan, int l) 
   return reinterpret_cast<char*>(c.pub) + ((size_t)(par * c.C + chan) * c.pub_L + l) * (size_t)a.code_stride;
 }
 
+// ---- ClippedGossip: chunks of THREADS * N elements, one distance partial each ----
+template <typename T>
+__host__ __device__ __forceinline__ int cg_chunks(const Common<T>& c) {
+  return (c.n_pad + THREADS * Vec<T>::N - 1) / (THREADS * Vec<T>::N);
+}
+
 // ---- SGP (layout in consensus.h) ----
 template <typename T>
 NNDT_DEVINL T* sgp_row(const SgpArgs<T>& a, int par, int l) {

@@ -38,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp"):
+    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing and K-GT: a constant step
         alpha[:] = opt.alpha
@@ -54,6 +54,17 @@ def check_wait_capacity(dmax: int, rmax: int) -> None:
     if dmax > WAIT_THREADS or rmax > WAIT_THREADS - 32:
         raise ValueError(f"a node with {dmax} in-neighbors / {rmax} readers exceeds what the consensus kernels wait "
                          f"for ({WAIT_THREADS} in-neighbors, {WAIT_THREADS - 32} readers)")
+
+
+CLIP_MAX_DEG = 128     # consensus.h: kClipMaxDeg
+
+
+def check_clip_capacity(dmax: int) -> None:
+    """ClippedGossip's ``clip: adaptive`` mix picks the radius from every neighbor's distance in shared memory, for at
+    most ``CLIP_MAX_DEG`` neighbors per node."""
+    if dmax > CLIP_MAX_DEG:
+        raise ValueError(f"clipped_gossip with clip: adaptive handles at most {CLIP_MAX_DEG} neighbors per node on the "
+                         f"fused kernels; the planned graphs have a node with {dmax}")
 
 
 class ConsensusEngine:
@@ -73,6 +84,7 @@ class ConsensusEngine:
         self.beer = opt.alg_name == "beer"
         self.sgp = opt.alg_name == "sgp"
         self.pdg = opt.alg_name == "push_diging"
+        self.cg = opt.alg_name == "clipped_gossip"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -103,6 +115,8 @@ class ConsensusEngine:
             self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.u)
             self.pub_weights(k0 & 1).copy_(opt.w)
             self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
+        elif self.cg:                               # an attacker's published row is not its theta
+            self.pub[k0 & 1, 0, :L].copy_(opt.pub)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
@@ -240,9 +254,9 @@ class ConsensusEngine:
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
         # (CHOCO-SGD, BEER, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
-        # numerators with a weight; complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not (self.choco or self.beer) and not push_sum
-                         and opt.conf.get("complete_graph_mode", "sum") == "sum")
+        # numerators with a weight; so does ClippedGossip, which clips per edge; complete_graph_mode is ignored)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not (self.choco or self.beer or self.cg)
+                         and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
         if self.sum_mode:
@@ -313,6 +327,26 @@ class ConsensusEngine:
         if opt.alg_name == "kgt":
             d.update(local_steps=opt.local_steps, correction=int(opt.correction),
                      corr=opt.c.data_ptr() if kgt_corr else None, dacc=opt.d.data_ptr() if kgt_corr else None)
+        self.dist_part = self.t_attack = self.t_nbr_byz = None
+        if self.cg:
+            if opt.clip == "adaptive":
+                check_clip_capacity(dmax)
+            # fp64 partials of the squared neighbor distances: one per chunk of THREADS * (16 / itemsize) elements
+            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+            self.dist_part = torch.zeros(L * dmax * pstride, dtype=torch.float64, device=dev)
+            byz = set(opt.byzantine)
+            nbr_byz = np.zeros((G, L, dmax), dtype=np.int32)
+            for gi, t in enumerate(topos):
+                for l, g in enumerate(pl.local_nodes):
+                    for e, j in enumerate(t.neighbors_noself[g]):
+                        nbr_byz[gi, l, e] = int(j in byz)
+            self.t_nbr_byz = torch.as_tensor(nbr_byz, device=dev)
+            if any(opt.attack):
+                self.t_attack = torch.as_tensor(np.asarray(opt.attack, dtype=np.int32), device=dev)
+            d.update(dist_part=self.dist_part.data_ptr(), pstride=pstride, clip_adaptive=int(opt.clip == "adaptive"),
+                     clip_delta=float(opt.delta), attack_scale=float(opt.scale), attack_z=float(opt.z),
+                     attack=None if self.t_attack is None else self.t_attack.data_ptr(),
+                     nbr_byz=self.t_nbr_byz.data_ptr())
         if opt.alg_name == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
@@ -346,9 +380,12 @@ class ConsensusEngine:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
         neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
         counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
-        steps."""
+        steps.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
+        for the mix (``clip: none`` once, as DSGD; an ALIE attacker also reads its honest neighbors' rows, not
+        counted)."""
         deg = int(self.t_deg[0].sum().item())
-        return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg}
+        reads = 2 if self.cg and self.opt.clip == "adaptive" else 1
+        return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg * reads}
 
     def consensus_metric(self, k: int):
         """Fused consensus-error metric (csrc/consensus.cu: consensus_metric_kernel) on the rows published

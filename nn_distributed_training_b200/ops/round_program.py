@@ -11,6 +11,7 @@ A round is a short, fixed kernel sequence
     SGP:  sgp_mix, fwd/bwd, sgp_step
     Push-DIGing:  pdg_mix, fwd/bwd, pdg_track
     K-GT:  kgt_mix, [fwd/bwd, kgt_step(p)] x local_steps       (local DSGD: dsgd_mix in place of kgt_mix)
+    ClippedGossip:  cg_dist, cg_mix, fwd/bwd, cg_step           (clip: none: dsgd_mix, fwd/bwd, cg_step)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -83,6 +84,14 @@ def _round_ops_impl(opt, eng, grads):
         for p in range(opt.local_steps):
             grads(p)
             eng.op.kgt_step(p)
+    elif alg == "clipped_gossip":
+        if opt.clip == "adaptive":
+            eng.op.cg_dist()
+            eng.op.cg_mix()
+        else:
+            eng.op.dsgd_mix()
+        grads(0)
+        eng.op.cg_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -136,9 +145,10 @@ class RoundProgram:
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
-        # publish codes, SGP and Push-DIGing numerators, so their metric reads the parameter rows (all_theta) at the
-        # evaluation points instead
-        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg)
+        # publish codes, SGP and Push-DIGing numerators and ClippedGossip's attackers attack rows, so their metric reads
+        # the parameter rows (all_theta) at the evaluation points instead
+        attacked = self.eng.cg and bool(opt.byzantine)
+        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -172,6 +182,8 @@ class RoundProgram:
             n += 1
         if self.opt.alg_name == "dinno":
             return n + 2 * self.opt.pits
+        if self.opt.alg_name == "clipped_gossip" and self.opt.clip == "adaptive":
+            return n + 4
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
@@ -305,8 +317,10 @@ class RoundProgram:
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp") and opt.k > 0:
+        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
+        if opt.alg_name == "clipped_gossip":
+            opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
         if opt.alg_name == "choco_sgd":
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
         if opt.alg_name == "beer":              # h, s_h, v, g, s_g and m_old are the optimizer's own rows

@@ -1,4 +1,5 @@
 from .beer import BEER
+from .clipped_gossip import ClippedGossip
 from .choco import ChocoSGD
 from .dinno import DiNNO
 from .dsgd import DSGD
@@ -11,7 +12,7 @@ from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
-              "push_diging": PushDIGing, "kgt": KGT}
+              "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -255,6 +255,9 @@ class ConsensusProblem:
         out = dict(self.metrics)
         if getattr(self, "data_source", None) is not None:
             out["data_source"] = self.data_source     # extra key next to the reference's metric lists
+        byz = self.conf.get("optimizer_config", {}).get("byzantine")
+        if byz:
+            out["byzantine_nodes"] = sorted(int(v) for v in byz["nodes"])   # summaries average the other nodes
         torch.save(out, path)
 
     def state_dicts(self) -> Dict[int, dict]:

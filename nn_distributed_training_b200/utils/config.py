@@ -15,7 +15,8 @@ import yaml
 
 REQUIRED = object()
 
-ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt")
+ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
+        "clipped_gossip")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -43,6 +44,8 @@ OPT_SCHEMA = {
     "push_diging": {"alpha": REQUIRED, "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
     "kgt": {"alpha": REQUIRED, "local_steps": REQUIRED, "correction": True, "outer_iterations": REQUIRED,
             "profile": False, "update_graph": True},
+    "clipped_gossip": {"alpha0": REQUIRED, "mu": 0.0, "clip": REQUIRED, "outer_iterations": REQUIRED, "profile": False,
+                       "update_graph": True},
 }
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
@@ -86,7 +89,10 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt")
+    if "byzantine" in c and alg != "clipped_gossip":
+        raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only "
+                          f"(alg_name is {alg!r})")
+    if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -121,6 +127,21 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.alpha must be > 0 (got {c['alpha']!r})")
         if not isinstance(c["correction"], bool):
             raise ConfigError(f"{path}.correction must be true or false (got {c['correction']!r})")
+    if alg == "clipped_gossip":
+        if c["clip"] not in ("none", "adaptive"):
+            raise ConfigError(f"{path}.clip must be one of none|adaptive (got {c['clip']!r})")
+        if c["clip"] == "adaptive":
+            if "delta" not in c:
+                raise ConfigError(f"missing required key {path}.delta (clip: adaptive)")
+            dl = c["delta"]
+            if isinstance(dl, bool) or not isinstance(dl, (int, float)) or not 0.0 <= float(dl) < 1.0:
+                raise ConfigError(f"{path}.delta must be in [0, 1) (got {dl!r})")
+        if c.get("byzantine") is not None:
+            from ..optimizers.clipped_gossip import check_byzantine
+            try:
+                check_byzantine(c["byzantine"], None)
+            except ValueError as e:
+                raise ConfigError(f"{path}.{e}") from None
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c
@@ -215,7 +236,25 @@ def validate_experiment(conf: Dict[str, Any], kind: str) -> Dict[str, Any]:
         out["problem_configs"] = {k: validate_problem(v, f"problem_configs.{k}", pk)
                                   for k, v in out["problem_configs"].items()}
     _check_directed_graph(out)
+    _check_byzantine_nodes(out)
     return out
+
+
+def _check_byzantine_nodes(conf: Dict[str, Any]) -> None:
+    """Byzantine node ids against the node count of ``experiment.graph``: in range, and not every node."""
+    g = conf["experiment"].get("graph")
+    if not isinstance(g, dict) or "num_nodes" not in g:
+        return
+    from ..optimizers.clipped_gossip import check_byzantine
+    probs = conf.get("problem_configs") or ({"problem": conf["problem"]} if "problem" in conf else {})
+    for k, p in probs.items():
+        byz = p["optimizer_config"].get("byzantine")
+        if byz is not None:
+            path = f"problem_configs.{k}" if "problem_configs" in conf else k
+            try:
+                check_byzantine(byz, int(g["num_nodes"]))
+            except ValueError as e:
+                raise ConfigError(f"{path}.optimizer_config.{e}") from None
 
 
 def _check_directed_graph(conf: Dict[str, Any]) -> None:

@@ -42,12 +42,16 @@ def summarize_run(run_dir: str, eval_every: Optional[int] = None) -> Dict[str, d
     summary = {}
     for name, m in res.items():
         s = {}
+        # a run with Byzantine nodes is summarised over its honest nodes
+        byz = set(m.get("byzantine_nodes", ()))
         acc = _stack(m.get("top1_accuracy"))
         if acc is not None:
-            s["final_top1_mean"] = float(acc[-1].mean()); s["final_top1_min"] = float(acc[-1].min())
+            a = acc[-1][[i for i in range(acc.shape[1]) if i not in byz]]
+            s["final_top1_mean"] = float(a.mean()); s["final_top1_min"] = float(a.min())
         vl = _stack(m.get("validation_loss"))
         if vl is not None:
-            s["final_val_loss_mean"] = float(vl[-1].mean()); s["first_val_loss_mean"] = float(vl[0].mean())
+            honest = [i for i in range(vl.shape[1]) if i not in byz]
+            s["final_val_loss_mean"] = float(vl[-1][honest].mean()); s["first_val_loss_mean"] = float(vl[0][honest].mean())
         ce = m.get("consensus_error")
         if ce:
             last = ce[-1]
