@@ -112,6 +112,34 @@ NNDT_DEVINL uint32_t map_to(const void* p, uint32_t rank) {
 NNDT_DEVINL double ld_dsmem(uint32_t a) { double v; asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory"); return v; }
 NNDT_DEVINL void st_dsmem(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
 
+// ---- cluster pushes: a producer stores into a peer's shared memory and the bytes complete a transaction count on the
+//      peer's mbarrier (release at cluster scope); the consumer waits on its own mbarrier for just those bytes.  Both
+//      addresses come from map_to() for the consumer's rank ------------------------------------------------------------
+NNDT_DEVINL void st_async(uint32_t a, double v, uint32_t bar) {
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.f64 [%0], %1, [%2];" ::"r"(a), "d"(v), "r"(bar) : "memory");
+}
+NNDT_DEVINL void st_async(uint32_t a, double v0, double v1, uint32_t bar) {   // 16-byte aligned pair
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.v2.f64 [%0], {%1, %2}, [%3];" ::"r"(a), "d"(v0), "d"(v1), "r"(bar)
+               : "memory");
+}
+// the relaxed half of a split cluster barrier: the arrive after this CTA's mbarrier inits, the wait before its first push
+NNDT_DEVINL void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
+NNDT_DEVINL void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
+// mbarrier_wait_parity with acquire at cluster scope: the bytes were written by peers' st_async
+NNDT_DEVINL void mbarrier_wait_parity_cluster(uint64_t* bar, uint32_t parity) {
+  const uint32_t addr = smem_addr_u32(bar);
+  uint32_t done;
+  do {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+        "selp.u32 %0, 1, 0, p;\n\t}\n"
+        : "=r"(done)
+        : "r"(addr), "r"(parity)
+        : "memory");
+  } while (!done);
+}
+
 // ---- FP64 tensor-core tiles (DMMA) ------------------------------------------------------------------------------
 // m16n8k4 fragments (g = lane >> 2, t = lane & 3): A a0 (g, t), a1 (g + 8, t); B b0 (t, g);
 // C c0 (g, 2t), c1 (g, 2t + 1), c2 (g + 8, 2t), c3 (g + 8, 2t + 1).

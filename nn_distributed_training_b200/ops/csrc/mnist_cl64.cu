@@ -8,8 +8,9 @@
 // three channels = 108 of the 432 fc1 inputs for all MS samples (image rows 6c .. 6c+9): conv+ReLU+pool -> A_c [MS x 108];
 // H_c = A_c . W1_c^T reduced over the cluster through distributed shared memory (reduce-scatter by samples, MS / 4 per
 // CTA; fc2 / loss / backward on the owners, dH rows gathered back); da1_c = dH . W1_c and dW1_c = dH^T . A_c are local;
-// dW1_c goes straight to its columns of the gradient row; small gradients are reduced through DSMEM.  One gradient
-// partial row per cluster.
+// dW1_c goes straight to its columns of the gradient row; small gradients are reduced through DSMEM.  At MS <= 32 the
+// partial H, dH and the small-gradient shares are pushed (st.async) on transaction barriers instead of read between
+// cluster barriers.  One gradient partial row per cluster.
 // Why 4 CTAs: a cluster must sit inside one GPC and a CTA fills its SM (shared memory and registers), so a GPC of n SMs
 // holds floor(n / CL) clusters.  On an H100 SXM (132 SMs) only 17 six-CTA clusters fit at once, and the 20 clusters of
 // 10 nodes x 2 batch splits ran in two waves; 4-CTA clusters keep every node count up to 12 in one wave.
@@ -38,13 +39,19 @@ constexpr int PART_WC = 0, PART_BC = 75, PART_B1 = 78, PART_W2 = 142, PART_B2 = 
 template <int MS>
 struct Smem {
   static constexpr int NO = MS / CL;           // samples a CTA owns for fc2, the loss and their backward
+  // MS <= 32: partial H, dH and the fc2 / b1 / b2 / loss shares cross CTAs as pushes (st.async) into receive buffers,
+  // each counted on the receiver's transaction barrier.  MS = 64 has no room for the buffers and keeps the
+  // cluster-barrier path: its owners' partial H and dH rows are read by the peers (ld.shared::cluster)
+  static constexpr bool kPush = MS <= 32;
+  static constexpr int PER = (PART_N - PART_B1 + CL - 1) / CL;   // fc2 / b1 / b2 / loss entries each CTA reduces
   static constexpr bool kDoublePix = MS <= 32; // pixels as normalised doubles; at MS = 64 they only fit as raw bytes
   // sample stride of the pixel rows; as doubles 282 (141 16-byte units, odd), so the same patch row of eight consecutive
   // samples starts in eight different 16-byte bank groups
   static constexpr int PXS = kDoublePix ? PXR + 2 : PXR;
   double w[HID * WS];        // W1 slice [j][k], k = ch * 36 + cell; after GEMM 2 da1 [k][s], then the conv-grad warp sums
   double a[MS * WS];         // A tile [s][k]
-  double h[MS * HS];         // partial H [s][j] (read by the peers); after barrier #2 dH [s][j]
+  // kPush: dH [s][j], pushed by the owners.  Otherwise partial H [s][j] (read by the peers), after barrier #2 dH [s][j]
+  alignas(16) double h[MS * HS];
   alignas(16) unsigned char img[kDoublePix ? MS * PXS * 8 : MS * PXS];
   double lut[kDoublePix ? 1 : 256];                         // MS = 64: normalised value of each u8 pixel
   double h_loc[NO * HR > CL * 80 ? NO * HR : CL * 80];     // [sl][hr(j)]; later (rank 0) the conv-gradient shares [CL][80]
@@ -60,6 +67,11 @@ struct Smem {
   int label[MS];
   float valid[MS];
   unsigned char arg[MS * KC];
+  // kPush receive buffers: [src rank][sl][j] the four partial H of this CTA's samples (later, on rank 0, the conv-gradient
+  // shares [CL][80]), and [src rank][PER] the shares of this CTA's quarter of the fc2 / b1 / b2 / loss gradients
+  alignas(16) double hin[kPush ? CL * NO * HID : 2];
+  double shr[kPush ? CL * PER : 1];
+  uint64_t bar[3];           // kPush: H in, dH in, shares in; each completes once per launch (parity 0)
 };
 static_assert(sizeof(Smem<16>) <= 227 * 1024 && sizeof(Smem<32>) <= 227 * 1024 && sizeof(Smem<64>) <= 227 * 1024,
               "shared memory budget");
@@ -153,6 +165,18 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   };
   long long* prof = a.prof != nullptr ? a.prof + ((l * nsplit + bsplit) * CL + c) * 64 : nullptr;
   stamp(prof, 0, tid);
+  constexpr bool kPush = SM::kPush;
+  constexpr int PER = SM::PER;
+  if constexpr (kPush) {
+    static_assert(CL * NO * HID >= CL * 80, "rank 0's partial-H buffer holds the conv-gradient shares");
+    if (tid == 0) {
+      for (int i = 0; i < 3; ++i) mbarrier_init(&sm.bar[i], 1);
+      mbarrier_expect_tx(&sm.bar[0], CL * NO * HID * 8);
+      mbarrier_expect_tx(&sm.bar[1], MS * HID * 8);
+      mbarrier_expect_tx(&sm.bar[2], CL * min(PER, PART_N - PART_B1 - c * PER) * 8);
+    }
+    cluster_arrive_relaxed();   // waited for before the first push, after GEMM 1: no peer pushes into an uninitialised barrier
+  }
 
   // ---- data half: sampler + image rows 6c .. 6c+9 (280 contiguous pixels per sample), before the PDL wait ----------------
   const int call = a.calls != nullptr ? a.calls[l] : 0;
@@ -316,14 +340,29 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   stamp(prof, 4, tid);
 
   // ---- GEMM 1 (DMMA): partial H_c[s][j] = sum_k A[s][k] W[j][k] over this CTA's 108 inputs.  MS / 16 x 8 tiles of 16 x 8,
-  //      NJ1 adjacent column tiles per warp (16 of the 20 warps busy at MS >= 32), the whole K range per tile: no split-K ----------
+  //      NJ1 adjacent column tiles per warp (16 of the 20 warps busy at MS >= 32), the whole K range per tile: no split-K.
+  //      kPush: accumulator pairs go straight to the owner of each sample (s / NO), invalid samples' zero rows included,
+  //      so every byte count is static -----------------------------------------------------------------------------------
   {
     constexpr int NJ1 = MS == 64 ? 2 : 1, NGRP = 8 / NJ1;
-    if (warp < (MS / 16) * NGRP) {
-      const int m0 = 16 * (warp / NGRP), n0 = 8 * NJ1 * (warp % NGRP);
-      double acc[NJ1][4];
-      zero(acc);
-      gemm_k<NJ1, KC>(acc, m0, n0, lane, at(sm.a, WS), at_t(sm.w, WS));
+    const bool busy = warp < (MS / 16) * NGRP;
+    const int m0 = 16 * (warp / NGRP), n0 = 8 * NJ1 * (warp % NGRP);
+    double acc[NJ1][4];
+    zero(acc);
+    if (busy) gemm_k<NJ1, KC>(acc, m0, n0, lane, at(sm.a, WS), at_t(sm.w, WS));
+    if constexpr (kPush) {
+      cluster_wait();
+      if (busy) {
+#pragma unroll
+        for (int j = 0; j < NJ1; ++j)
+#pragma unroll
+          for (int i = 0; i < 4; i += 2) {
+            const int s = frow(m0, lane, i), r = s / NO;
+            st_async(map_to(sm.hin + (c * NO + s - r * NO) * HID + fcol(n0 + 8 * j, lane, i), (uint32_t)r), acc[j][i],
+                     acc[j][i + 1], map_to(&sm.bar[0], (uint32_t)r));
+          }
+      }
+    } else if (busy) {
 #pragma unroll
       for (int j = 0; j < NJ1; ++j)
 #pragma unroll
@@ -331,8 +370,14 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     }
   }
   stamp(prof, 5, tid);
-  cluster_sync();                                        // #1: all four partial H are in shared memory
+  if constexpr (kPush) {
+    if (warp < NO) mbarrier_wait_parity_cluster(&sm.bar[0], 0);   // the four partial H of this CTA's samples
+  } else {
+    cluster_sync();                                      // #1: all four partial H are in shared memory
+  }
   stamp(prof, 6, tid);
+  // every CTA of the cluster has read `call`: it had before its partial H, which thread 0 has received (kPush) or which
+  // barrier #1 published
   if (c == 0 && tid == 0 && a.calls != nullptr) {
     if (a.arrive == nullptr || nsplit == 1) a.calls[l] = call + 1;
     else if (atomicAdd(a.arrive + l, 1u) == (unsigned)nsplit - 1) { a.arrive[l] = 0; a.calls[l] = call + 1; }
@@ -351,7 +396,10 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       const double* src = sm.h + s * HS + j;
       double v = sm.b1[j];
 #pragma unroll
-      for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(src, (uint32_t)r));
+      for (int r = 0; r < CL; ++r) {
+        if constexpr (kPush) v += sm.hin[(r * NO + sl) * HID + j];
+        else v += ld_dsmem(map_to(src, (uint32_t)r));
+      }
       hv[q] = v > 0.0 ? v : 0.0;
       sm.h_loc[sl * HR + hr(j)] = hv[q];
     }
@@ -393,58 +441,86 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
       dh[1] += d * sm.w2[cc * HR + hr(lane + 32)];
     }
 #pragma unroll
-    for (int q = 0; q < 2; ++q) sm.dh_loc[sl * HID + lane + 32 * q] = hv[q] > 0.0 ? dh[q] : 0.0;
+    for (int q = 0; q < 2; ++q) {
+      dh[q] = hv[q] > 0.0 ? dh[q] : 0.0;
+      sm.dh_loc[sl * HID + lane + 32 * q] = dh[q];
+    }
+    if constexpr (kPush) {
+      // lane i pushes hidden units 2i, 2i + 1 of sample s into the dH tile of every CTA, this one included
+      const int e = (2 * lane) & 31;
+      const double e0 = __shfl_sync(0xffffffffu, dh[0], e), e1 = __shfl_sync(0xffffffffu, dh[1], e);
+      const double o0 = __shfl_sync(0xffffffffu, dh[0], e + 1), o1 = __shfl_sync(0xffffffffu, dh[1], e + 1);
+#pragma unroll
+      for (int r = 0; r < CL; ++r)
+        st_async(map_to(sm.h + s * HS + 2 * lane, (uint32_t)r), lane < 16 ? e0 : e1, lane < 16 ? o0 : o1,
+                 map_to(&sm.bar[1], (uint32_t)r));
+    }
   }
   __syncthreads();
+  // the fc2 / b1 / b2 / loss shares: kPush sends entry o straight to the CTA that reduces it; otherwise the peers read it
+  auto share = [&](int o, double v) {
+    if constexpr (kPush) {
+      const int e = o - PART_B1, q = e / PER;
+      st_async(map_to(sm.shr + c * PER + (e - q * PER), (uint32_t)q), v, map_to(&sm.bar[2], (uint32_t)q));
+    } else {
+      sm.part[o] = v;
+    }
+  };
   for (int o = tid; o < NCLS * HID; o += NT) {
     const int cc = o >> 6, j = o & 63;
     double v = 0.0;
     for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + cc] * sm.h_loc[sl * HR + hr(j)];
-    sm.part[PART_W2 + o] = v;
+    share(PART_W2 + o, v);
   }
   if (tid < HID) {
     double v = 0.0;
     for (int sl = 0; sl < NO; ++sl) v += sm.dh_loc[sl * HID + tid];
-    sm.part[PART_B1 + tid] = v;
+    share(PART_B1 + tid, v);
   } else if (tid >= 64 && tid < 64 + NCLS) {
     double v = 0.0;
     for (int sl = 0; sl < NO; ++sl) v += sm.dz[sl * 16 + (tid - 64)];
-    sm.part[PART_B2 + (tid - 64)] = v;
+    share(PART_B2 + (tid - 64), v);
   } else if (tid == 96) {
     double v = 0.0;
     for (int sl = 0; sl < NO; ++sl) v += sm.red[sl];
-    sm.part[PART_LOSS] = v * inv_bs;
+    share(PART_LOSS, v * inv_bs);
   }
   stamp(prof, 7, tid);
-  cluster_sync();                                        // #2: every owner's dH rows and fc2 / b1 / loss shares are final
+  if constexpr (kPush) mbarrier_wait_parity_cluster(&sm.bar[1], 0);   // all MS dH rows
+  else cluster_sync();                                   // #2: every owner's dH rows and fc2 / b1 / loss shares are final
   stamp(prof, 8, tid);
   // this split's gradient row, formed where it is written: a pointer held from here to the end would cost two registers
   // through GEMM 2 and the conv grads, and the kernel has 96 per thread
   auto grad_row = [&]() { return reinterpret_cast<double*>(a.grad_part) + ((size_t)l * nsplit + bsplit) * a.n_pad; };
-  // CTA c reduces its quarter of the fc2 / b1 / loss shares over the cluster (the peers stay resident until the last barrier)
-  {
-    constexpr int NE = PART_N - PART_B1, PER = (NE + CL - 1) / CL;
-    const int o = PART_B1 + c * PER + tid;
-    if (tid < PER && o < PART_N) {
-      double* gp = grad_row();
-      double v = 0.0;
+  // CTA c reduces entries PART_B1 + c PER + i of the fc2 / b1 / b2 / loss shares over the cluster, ranks in order
+  auto reduce_share = [&](int i) {
+    const int o = PART_B1 + c * PER + i;
+    if (o >= PART_N) return;
+    double* gp = grad_row();
+    double v = 0.0;
 #pragma unroll
-      for (int r = 0; r < CL; ++r) v += ld_dsmem(map_to(sm.part + o, (uint32_t)r));
-      if (o < PART_W2) gp[a.off_b1 + (o - PART_B1)] = v;
-      else if (o < PART_B2) gp[a.off_w2 + (o - PART_W2)] = v;
-      else if (o < PART_LOSS) gp[a.off_b2 + (o - PART_B2)] = v;
-      else {
-        a.loss_part[l * nsplit + bsplit] = (float)v;
-        if (a.loss_mirror != nullptr) a.loss_mirror[l * nsplit + bsplit] = (float)v;
-      }
+    for (int r = 0; r < CL; ++r) {
+      if constexpr (kPush) v += sm.shr[r * PER + i];
+      else v += ld_dsmem(map_to(sm.part + o, (uint32_t)r));
     }
+    if (o < PART_W2) gp[a.off_b1 + (o - PART_B1)] = v;
+    else if (o < PART_B2) gp[a.off_w2 + (o - PART_W2)] = v;
+    else if (o < PART_LOSS) gp[a.off_b2 + (o - PART_B2)] = v;
+    else {
+      a.loss_part[l * nsplit + bsplit] = (float)v;
+      if (a.loss_mirror != nullptr) a.loss_mirror[l * nsplit + bsplit] = (float)v;
+    }
+  };
+  if constexpr (!kPush) {
+    // (the peers stay resident until the last barrier)
+    if (tid < PER) reduce_share(tid);
+    // ---- gather all MS dH rows from their owners into the partial-H tile (every peer finished reading it before #2) ---------
+    for (int o = tid; o < MS * HID; o += NT) {
+      const int s = o >> 6, j = o & 63, r = s / NO;
+      sm.h[s * HS + j] = ld_dsmem(map_to(sm.dh_loc + (s - r * NO) * HID + j, (uint32_t)r));
+    }
+    __syncthreads();
   }
-  // ---- gather all MS dH rows from their owners into the partial-H tile (every peer finished reading it before #2) -----------
-  for (int o = tid; o < MS * HID; o += NT) {
-    const int s = o >> 6, j = o & 63, r = s / NO;
-    sm.h[s * HS + j] = ld_dsmem(map_to(sm.dh_loc + (s - r * NO) * HID + j, (uint32_t)r));
-  }
-  __syncthreads();
   stamp(prof, 9, tid);
 
   // ---- GEMM 2 (DMMA): da1_c[s][k] = sum_j dH[s][j] W[j][k], MS / 16 x KT / 2 pairs of adjacent 16 x 8 tiles, accumulators
@@ -487,6 +563,12 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
   constexpr int W3 = NT / 32 - HID / 16, NJ3 = 2;   // first GEMM 3 warp; column tiles per pass
   static_assert(KT % NJ3 == 0, "GEMM 3 passes cover the column tiles");
   if (warp >= W3) {
+    // kPush: the shares of this CTA's quarter arrived while GEMM 2 ran; these warps reduce them first, as they end about
+    // 3 us before the conv-gradient warps
+    if constexpr (kPush) {
+      mbarrier_wait_parity_cluster(&sm.bar[2], 0);
+      for (int i = tid - W3 * 32; i < PER; i += NT - W3 * 32) reduce_share(i);
+    }
     double* gp = grad_row();
     const int m0 = 16 * (warp - W3);
 #pragma unroll 1
@@ -575,6 +657,10 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     }
   }
   __syncthreads();
+  // this CTA's share goes straight into rank 0's collection buffer.  kPush: rank 0's partial-H buffer, last read by its head
+  // warps before they pushed dH, which every peer has received before it gets here.  Otherwise its h_loc rows, dead since
+  // barrier #2
+  double* cin = kPush ? sm.hin : sm.h_loc;
   if (tid < 78) {
     double v = 0.0;
     if (tid < 75) {
@@ -584,8 +670,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     } else {
       v = wsums[KS * KW * 16 + (tid - 75)];
     }
-    // this CTA's share goes straight into rank 0's collection buffer (its h_loc rows, dead since barrier #2)
-    st_dsmem(map_to(sm.h_loc + c * 80 + tid, 0u), v);
+    st_dsmem(map_to(cin + c * 80 + tid, 0u), v);
   }
   stamp(prof, 13, tid);
   cluster_sync();                                        // #3: all four conv-gradient shares are in rank 0's buffer
@@ -593,7 +678,7 @@ mnist_cl64_train_kernel(const Args a, const GenericShape gs) {
     double* gp = grad_row();
     double v = 0.0;
 #pragma unroll
-    for (int r = 0; r < CL; ++r) v += sm.h_loc[r * 80 + tid];
+    for (int r = 0; r < CL; ++r) v += cin[r * 80 + tid];
     gp[tid < 75 ? a.off_wc + tid : a.off_bc + (tid - 75)] = v;
   }
   stamp(prof, 14, tid);

@@ -22,9 +22,12 @@ PHASES = ["sampler + image loads issued", "PDL wait", "TMA issue, small tensors,
           "cluster sync 2", "fc2-grad reduce (1/6), gather dH, re-swizzle W", "MMA 2 (da1) | re-swizzle A; re-swizzle dH",
           "MMA 3 issue | da1 epilogue", "conv grads (under MMA 3) -> rank 0", "MMA 3 wait, dW1 epilogue -> global",
           "cluster sync 3, conv-grad sum (rank 0), exit"]
+# MS <= 32 pushes H, dH and the fc2 shares (st.async): the sync rows are mbarrier waits, the reduce and gather row is empty and
+# the fc2-grad reduce runs on the GEMM 3 warps before GEMM 3
 PHASES64 = ["sampler, image rows -> smem (fp64)", "PDL wait", "W1 copies issued, conv weights + w2 (L2)",
-            "conv + ReLU + pool -> A tile (fp64), W1 copy wait", "GEMM 1 (fc1 partial, DMMA)", "cluster sync 1",
-            "head: warp per sample (H sum, fc2, loss, dz, dh), fc2 grads", "cluster sync 2", "fc2-grad reduce (1/4), gather dH",
+            "conv + ReLU + pool -> A tile (fp64), W1 copy wait", "GEMM 1 (fc1 partial, DMMA), H pushes",
+            "cluster sync 1 | H pushes wait", "head: warp per sample (H sum, fc2, loss, dz, dh), fc2 grads",
+            "cluster sync 2 | dH pushes wait", "fc2-grad reduce (1/4), gather dH (MS = 64)",
             "GEMM 2 (da1, DMMA) -> registers", "da1 -> smem (over W)", "GEMM 3 (dW1, warps 16-19) -> global | conv grads",
             "bias warp, conv grads still running after GEMM 3 -> rank 0", "cluster sync 3, conv-grad sum (rank 0), exit"]
 
