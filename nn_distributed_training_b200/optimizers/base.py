@@ -232,9 +232,26 @@ class ConsensusOptimizer:
         run_fused_training(self, profiler)
 
     # -- checkpoint / resume (SURVEY §5.4: the reference has none) ---------
+    # What a checkpoint carries beyond ``k`` and ``theta`` to resume bit-exactly: ``STATE`` names the optimizer's rows
+    # of the rank's nodes, ``SCALARS`` its host scalars.  A row that exists only in some configurations is listed only
+    # there (an instance sets its own tuple); a listed row that is ``None`` is saved as ``None`` and not restored.
+    STATE = ()
+    SCALARS = ()
+
     def state_dict(self) -> Dict:
-        return {"k": self.k, "theta": self.arena.theta.detach().cpu().clone()}
+        sd = {"k": self.k, "theta": self.arena.theta.detach().cpu().clone()}
+        sd.update({name: getattr(self, name) for name in self.SCALARS})
+        for name in self.STATE:
+            row = getattr(self, name)
+            sd[name] = None if row is None else row.cpu().clone()
+        return sd
 
     def load_state_dict(self, sd: Dict):
         self.k = int(sd["k"])
         self.arena.theta.copy_(sd["theta"].to(self.device))
+        for name in self.SCALARS:       # with the type the attribute has in a freshly built optimizer (float, int)
+            setattr(self, name, type(getattr(self, name))(sd[name]))
+        for name in self.STATE:
+            row = getattr(self, name)
+            if row is not None and sd[name] is not None:
+                row.copy_(sd[name].to(self.device))

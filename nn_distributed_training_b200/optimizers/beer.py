@@ -27,8 +27,6 @@ synchronous (Jacobi) order on undirected graphs exists.
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -40,6 +38,7 @@ FIXED_W = "s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a fi
 
 class BEER(ConsensusOptimizer):
     alg_name = "beer"
+    STATE = ("h", "s_h", "v", "g", "s_g", "m_old", "code_h", "code_g")
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -94,15 +93,3 @@ class BEER(ConsensusOptimizer):
                                     self.compressor, self.live)
             self.code_h.copy_(qh)
             self.code_g.copy_(qg)
-
-    STATE = ("h", "s_h", "v", "g", "s_g", "m_old", "code_h", "code_g")
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update({k: getattr(self, k).cpu().clone() for k in self.STATE})
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        for k in self.STATE:
-            getattr(self, k).copy_(sd[k].to(self.device))

@@ -26,8 +26,6 @@ a moving online-density plan) is refused.  Only the synchronous (Jacobi) order e
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -36,6 +34,8 @@ from ..ops import consensus_ref as ref
 
 class ChocoSGD(ConsensusOptimizer):
     alg_name = "choco_sgd"
+    STATE = ("x_hat", "s", "code")
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -90,18 +90,6 @@ class ChocoSGD(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             self.code.copy_(ref.choco_step_(a.theta, self.x_hat, a.grad, self.alph, self.compressor, self.live))
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(alph=self.alph, x_hat=self.x_hat.cpu().clone(), s=self.s.cpu().clone(), code=self.code.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])
-        self.x_hat.copy_(sd["x_hat"].to(self.device))
-        self.s.copy_(sd["s"].to(self.device))
-        self.code.copy_(sd["code"].to(self.device))
 
 
 def check_static_plan(graphs, alg="choco_sgd", why="s = sum_j W_ij x_hat_j is only valid for a fixed W"):

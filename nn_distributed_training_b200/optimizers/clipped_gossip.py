@@ -23,7 +23,7 @@ from __future__ import annotations
 
 import math
 import numbers
-from typing import Dict, List
+from typing import List
 
 import numpy as np
 import torch
@@ -63,6 +63,8 @@ def check_byzantine(byz, N: int) -> List[int]:
 
 class ClippedGossip(ConsensusOptimizer):
     alg_name = "clipped_gossip"
+    STATE = ("pub",)
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -127,14 +129,3 @@ class ClippedGossip(ConsensusOptimizer):
             ref.dsgd_step_(a.theta, a.grad, self.alph)
             ref.cg_publish_(self.pub, a.theta, pub_all, self.attack, topo.neighbors_noself, set(self.byzantine), lo,
                             self.scale, self.z)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(alph=self.alph, pub=self.pub.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])
-        self.pub.copy_(sd["pub"].to(self.device))
-

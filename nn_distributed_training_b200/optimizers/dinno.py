@@ -13,7 +13,6 @@ one elementwise kernel over the arena row (ops/csrc/consensus.cu: dinno_update).
 from __future__ import annotations
 
 import math
-from typing import Dict
 
 import numpy as np
 import torch
@@ -40,6 +39,8 @@ def primal_lr_table(conf) -> np.ndarray:
 
 class DiNNO(ConsensusOptimizer):
     alg_name = "dinno"
+    STATE = ("duals", "m", "v")
+    SCALARS = ("rho", "t")
 
     def __init__(self, ddl_problem, device, conf):
         super().__init__(ddl_problem, device, conf)
@@ -104,18 +105,3 @@ class DiNNO(ConsensusOptimizer):
             self.t += 1
             with torch.no_grad():
                 ref.optimizer_step_(a.theta, g, self.opt_kind, lr, self.m, self.v, self.t)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(rho=self.rho, duals=self.duals.cpu().clone(), t=self.t,
-                  m=None if self.m is None else self.m.cpu().clone(),
-                  v=None if self.v is None else self.v.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.rho, self.t = float(sd["rho"]), int(sd["t"])
-        self.duals.copy_(sd["duals"].to(self.device))
-        if self.m is not None and sd.get("m") is not None:
-            self.m.copy_(sd["m"].to(self.device))
-            self.v.copy_(sd["v"].to(self.device))

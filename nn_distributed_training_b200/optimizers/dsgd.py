@@ -12,8 +12,6 @@ matrix is cached per edge set instead of being rebuilt every round (Q2).
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -22,6 +20,7 @@ from ..ops import consensus_ref as ref
 
 class DSGD(ConsensusOptimizer):
     alg_name = "dsgd"
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         super().__init__(ddl_problem, device, conf)
@@ -55,12 +54,3 @@ class DSGD(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             ref.dsgd_step_(a.theta, a.grad, self.alph)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd["alph"] = self.alph
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])

@@ -23,8 +23,6 @@ exists.
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -35,6 +33,8 @@ MOMENTUM_MODES = ("local", "quasi_global")
 
 class DSGDm(ConsensusOptimizer):
     alg_name = "dsgdm"
+    STATE = ("m",)
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -59,6 +59,8 @@ class DSGDm(ConsensusOptimizer):
                                      f"alpha = {a!r} (alpha0 = {self.alph0}, mu = {self.mu})")
         self.m = self.arena.zeros()
         self.x_prev = self.arena.zeros() if self.quasi_global else None
+        if self.quasi_global:
+            self.STATE = ("m", "x_prev")
 
     def alpha_table(self, n=None):
         """alpha of rounds 0..n-1 (default: all ``outer_iterations``): DSGD's schedule."""
@@ -82,17 +84,3 @@ class DSGDm(ConsensusOptimizer):
         with torch.no_grad():
             ref.dsgdm_step_(a.theta, self.m, self.x_prev, a.grad, self.alph, alpha_prev, self.beta, self.quasi_global,
                             self.nesterov, k == 0)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(alph=self.alph, m=self.m.cpu().clone())
-        if self.quasi_global:
-            sd["x_prev"] = self.x_prev.cpu().clone()
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])
-        self.m.copy_(sd["m"].to(self.device))
-        if self.quasi_global:
-            self.x_prev.copy_(sd["x_prev"].to(self.device))

@@ -25,6 +25,7 @@ from ..ops import consensus_ref as ref
 
 class DSGT(ConsensusOptimizer):
     alg_name = "dsgt"
+    STATE = ("y", "g")
 
     def __init__(self, ddl_problem, device, conf):
         super().__init__(ddl_problem, device, conf)
@@ -80,16 +81,15 @@ class DSGT(ConsensusOptimizer):
         grads = torch.autograd.grad(loss, list(pr.models[i].parameters()))
         pr.arena.set_row_from_grads(i, grads)
 
+    # ``initialised`` is saved under another name than its attribute, and ``alpha`` may be a per-coordinate row
     def state_dict(self) -> Dict:
         sd = super().state_dict()
-        sd.update(y=self.y.cpu().clone(), g=self.g.cpu().clone(), initialised=self._initialised,
+        sd.update(initialised=self._initialised,
                   alpha=self.alpha.detach().cpu().clone() if torch.is_tensor(self.alpha) else float(self.alpha))
         return sd
 
     def load_state_dict(self, sd: Dict):
         super().load_state_dict(sd)
-        self.y.copy_(sd["y"].to(self.device))
-        self.g.copy_(sd["g"].to(self.device))
         self._initialised = bool(sd["initialised"])
         if "alpha" in sd:
             self.alpha = sd["alpha"].to(self.device) if torch.is_tensor(sd["alpha"]) else float(sd["alpha"])

@@ -15,8 +15,6 @@ theta holds the value before the mix, as it does for DSGD.  Only the synchronous
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -25,6 +23,8 @@ from ..ops import consensus_ref as ref
 
 class ExactDiffusion(ConsensusOptimizer):
     alg_name = "exact_diffusion"
+    STATE = ("psi",)
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -58,13 +58,3 @@ class ExactDiffusion(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             ref.ed_step_(a.theta, self.psi, a.grad, self.alph)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(alph=self.alph, psi=self.psi.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])
-        self.psi.copy_(sd["psi"].to(self.device))

@@ -27,7 +27,6 @@ undirected graphs exists; changing graphs and link drops are allowed, as for DSG
 from __future__ import annotations
 
 import numbers
-from typing import Dict
 
 import torch
 
@@ -62,6 +61,7 @@ class KGT(ConsensusOptimizer):
         self.c = a.zeros() if self.correction else None
         self.y = a.zeros() if self.correction else None      # the published tracker of the last round
         self.d = a.zeros() if self.correction else None      # the round's direction sum (dead between rounds)
+        self.STATE = ("c", "y") if self.correction else ()
 
     def _round(self, k: int):
         pr, a = self.pr, self.arena
@@ -78,15 +78,3 @@ class KGT(ConsensusOptimizer):
                 y = ref.kgt_step_(a.theta, self.c, self.d, a.grad, self.alpha, p, self.local_steps)
         if self.correction:
             self.y.copy_(y)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        if self.correction:
-            sd.update(c=self.c.cpu().clone(), y=self.y.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        if self.correction:
-            self.c.copy_(sd["c"].to(self.device))
-            self.y.copy_(sd["y"].to(self.device))

@@ -20,8 +20,6 @@ undirected cycle the push weights are the Metropolis weights, ``w`` stays 1 and 
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -30,6 +28,7 @@ from ..ops import consensus_ref as ref
 
 class PushDIGing(ConsensusOptimizer):
     alg_name = "push_diging"
+    STATE = ("u", "w", "y", "g")
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -63,15 +62,3 @@ class PushDIGing(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             ref.pdg_track_(self.y, self.g, self.ysum, a.grad)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(u=self.u.cpu().clone(), w=self.w.cpu().clone(), y=self.y.cpu().clone(), g=self.g.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.u.copy_(sd["u"].to(self.device))
-        self.w.copy_(sd["w"].to(self.device))
-        self.y.copy_(sd["y"].to(self.device))
-        self.g.copy_(sd["g"].to(self.device))

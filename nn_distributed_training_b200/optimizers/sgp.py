@@ -16,8 +16,6 @@ to rounding and SGP is DSGD.  Only the synchronous (Jacobi) order exists.
 """
 from __future__ import annotations
 
-from typing import Dict
-
 import torch
 
 from .base import ConsensusOptimizer
@@ -26,6 +24,8 @@ from ..ops import consensus_ref as ref
 
 class SGP(ConsensusOptimizer):
     alg_name = "sgp"
+    STATE = ("x", "w")
+    SCALARS = ("alph",)
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
@@ -64,14 +64,3 @@ class SGP(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             ref.sgp_step_(self.x, self.w, a.theta, a.grad, self.alph)
-
-    def state_dict(self) -> Dict:
-        sd = super().state_dict()
-        sd.update(alph=self.alph, x=self.x.cpu().clone(), w=self.w.cpu().clone())
-        return sd
-
-    def load_state_dict(self, sd: Dict):
-        super().load_state_dict(sd)
-        self.alph = float(sd["alph"])
-        self.x.copy_(sd["x"].to(self.device))
-        self.w.copy_(sd["w"].to(self.device))

@@ -1,5 +1,6 @@
-"""One rank per GPU (or per CPU process): the distributed run must reproduce the
-single-process run — gloo/world_size 2 here on CPU, NCCL + peer-mapped kernels on GPUs."""
+"""One rank per GPU (or per CPU process): the distributed run of every consensus optimizer must reproduce the
+single-process run — gloo/world_size 2 here on CPU, NCCL + peer-mapped kernels on GPUs.  The cases are those of
+``dist_worker.py``'s table."""
 import os
 import subprocess
 import sys
@@ -18,36 +19,88 @@ def _launch(nproc, extra, port):
     return subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=env)
 
 
-@pytest.mark.parametrize("graph", ["cycle", "wheel"])
-def test_gloo_two_ranks_match_single_process(graph):
-    r = _launch(2, ["--cuda", "0", "--nodes", "4", "--graph", graph], 29611)
+def _cases(rows, port0):
+    """``(case, graph, options)`` rows -> parameters ``(worker arguments, master port)`` with readable ids; every launch
+    gets its own port."""
+    out = []
+    for i, (case, graph, opts) in enumerate(rows):
+        args = ["--case", case, "--graph", graph] + [a for k, v in opts.items() for a in ("--" + k, str(v))]
+        tags = [f"correction{v}" if k == "correction" else str(v) for k, v in opts.items() if k != "delayed"]
+        name = "-".join([case, *tags, graph] + (["delayed"] if opts.get("delayed") else []))
+        out.append(pytest.param(args, port0 + i, id=name))
+    return out
+
+
+TRIO = "dinno_dsgd_dsgt"
+
+# The PyTorch path with two CPU ranks.  The directed cases gather in-neighbor rows (numerators, trackers) and the float64
+# weights across ranks, each rank with its slice of the push-sum matrix; ``switching`` changes the directed graph every
+# round.
+GLOO_CASES = _cases([
+    (TRIO, "cycle", {}), (TRIO, "wheel", {}),
+    ("exact_diffusion", "wheel", {}),
+    ("choco_sgd", "wheel", {}),
+    ("sgp", "random_directed", {}), ("sgp", "switching", {}),
+    ("push_diging", "random_directed", {}), ("push_diging", "switching", {}),
+    ("dsgdm", "wheel", {"momentum": "local"}), ("dsgdm", "wheel", {"momentum": "quasi_global"}),
+    ("beer", "wheel", {}),
+    ("kgt", "wheel", {"correction": 1}), ("kgt", "wheel", {"correction": 0}),
+    ("clipped_gossip", "cycle", {"clip": "none", "attack": "sign_flip"}),
+    ("clipped_gossip", "wheel", {"clip": "adaptive", "attack": "sign_flip"}),
+    ("clipped_gossip", "wheel", {"clip": "none", "attack": "alie"}),
+    ("clipped_gossip", "cycle", {"clip": "adaptive", "attack": "alie"}),
+], 29700)
+GLOO_NODES = {"sgp": 6, "push_diging": 6}       # directed graphs of 6 nodes; 4 otherwise
+
+# NCCL + peer-mapped consensus kernels, one rank per GPU.  ``pipeline`` (the trio): ``host`` pulls the rows from pinned
+# host memory by the staging kernel inside multi-round graphs, peers announced by the first consensus kernel of each
+# round; the single-process run uses resident shards.  ``delayed``: one rank is held back by spin kernels and every
+# neighbor read is checked against its round tag; cases that allow a changing graph also drop links every round, which
+# opens the write-after-read window of the double-buffered published rows.  On the directed cycle a rank reads only its
+# predecessor, so without the wait for its readers it could run ahead of them and overwrite a buffer still being read;
+# ``switching`` takes the readers from the previous round's graph.
+NCCL_CASES = _cases([
+    (TRIO, "cycle", {"pipeline": "auto"}), (TRIO, "complete", {"pipeline": "resident"}),
+    (TRIO, "cycle", {"pipeline": "host"}), (TRIO, "wheel", {"delayed": 1}),
+    ("exact_diffusion", "cycle", {"delayed": 0}), ("exact_diffusion", "complete", {"delayed": 0}),
+    ("exact_diffusion", "wheel", {"delayed": 1}),
+    ("choco_sgd", "cycle", {"delayed": 0}), ("choco_sgd", "complete", {"delayed": 0}),
+    ("choco_sgd", "wheel", {"delayed": 1}),
+    ("sgp", "directed_cycle", {"delayed": 0}), ("sgp", "exponential", {"delayed": 0}),
+    ("sgp", "random_directed", {"delayed": 0}), ("sgp", "directed_cycle", {"delayed": 1}),
+    ("sgp", "switching", {"delayed": 1}),
+    ("push_diging", "directed_cycle", {"delayed": 0}), ("push_diging", "exponential", {"delayed": 0}),
+    ("push_diging", "random_directed", {"delayed": 0}), ("push_diging", "directed_cycle", {"delayed": 1}),
+    ("push_diging", "switching", {"delayed": 1}),
+    ("dsgdm", "cycle", {"delayed": 0, "momentum": "local"}),
+    ("dsgdm", "complete", {"delayed": 0, "momentum": "quasi_global"}),
+    ("dsgdm", "wheel", {"delayed": 1, "momentum": "quasi_global"}),
+    ("beer", "cycle", {"delayed": 0}), ("beer", "complete", {"delayed": 0}), ("beer", "wheel", {"delayed": 1}),
+    ("kgt", "cycle", {"delayed": 0, "correction": 0}), ("kgt", "complete", {"delayed": 0, "correction": 1}),
+    ("kgt", "wheel", {"delayed": 1, "correction": 1}),
+    ("clipped_gossip", "cycle", {"delayed": 0, "clip": "none", "attack": "sign_flip"}),
+    ("clipped_gossip", "complete", {"delayed": 0, "clip": "adaptive", "attack": "alie"}),
+    ("clipped_gossip", "wheel", {"delayed": 1, "clip": "adaptive", "attack": "alie"}),
+    ("clipped_gossip", "cycle", {"delayed": 1, "clip": "adaptive", "attack": "sign_flip"}),
+], 29750)
+
+
+@pytest.mark.parametrize("args,port", GLOO_CASES)
+def test_gloo_two_ranks_match_single_process(args, port):
+    nodes = GLOO_NODES.get(args[1], 4)
+    r = _launch(2, ["--cuda", "0", "--nodes", str(nodes)] + args, port)
     assert "DIST_RESULT PASS" in r.stdout, r.stdout[-2000:] + r.stderr[-2000:]
 
 
 @pytest.mark.gpu
 @pytest.mark.multigpu
-@pytest.mark.parametrize("graph,pipeline", [("cycle", "auto"), ("complete", "resident"), ("cycle", "host")])
-def test_nccl_peer_mapped_ranks_match_single_process(graph, pipeline):
-    """``host``: rows pulled from pinned host memory by the staging kernel inside multi-round graphs, peers
-    announced by the first consensus kernel of each round; the single-process oracle uses resident shards."""
+@pytest.mark.parametrize("args,port", NCCL_CASES)
+def test_nccl_peer_mapped_ranks_match_single_process(args, port):
     n = torch.cuda.device_count()
     if n < 2:
         pytest.skip("needs >= 2 GPUs")
     nproc = min(8, n)         # every GPU of the box: 2 on the development boxes, 8 on the scaling box
-    r = _launch(nproc, ["--cuda", "1", "--nodes", str(3 * nproc), "--graph", graph, "--pipeline", pipeline], 29612)
-    assert "DIST_RESULT PASS" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
-
-
-@pytest.mark.gpu
-@pytest.mark.multigpu
-def test_time_varying_graph_with_delayed_rank_matches_single_process():
-    """Write-after-read window of the double-buffered published rows on time-varying graphs: link drops change the graph
-    every round, one rank is delayed by spin kernels, the sequence check verifies every neighbor read."""
-    n = torch.cuda.device_count()
-    if n < 2:
-        pytest.skip("needs >= 2 GPUs")
-    nproc = min(8, n)
-    r = _launch(nproc, ["--cuda", "1", "--nodes", str(3 * nproc), "--graph", "wheel", "--delayed", "1"], 29615)
+    r = _launch(nproc, ["--cuda", "1", "--nodes", str(3 * nproc)] + args, port)
     assert "DIST_RESULT PASS" in r.stdout, r.stdout[-3000:] + r.stderr[-3000:]
 
 
