@@ -139,20 +139,60 @@ def dsgdm_step_(theta: torch.Tensor, m: torch.Tensor, x_prev: Optional[torch.Ten
 #   int8: [n_pad] int8, [nb] T scales      scale = max|v| / 127, code = clamp(rint(v / scale), -127, 127), dec = code scale
 #   sign: [nb] uint32 words, [nb] T        bit e % 32 of word e // 32 set when v_e >= 0; scale = sum|v| / n_live over the
 #                                          live elements, dec = +-scale on live elements and 0 on padding and holes
+#   topk: [k] T values, [k] uint32 indices the k live elements of largest |v| (choco_topk_select), indices ascending,
+#         zero padding to a multiple of 16 B  values exact (not rescaled); dec = v at the indices, 0 elsewhere
 # The arithmetic is the kernel's: divisions and the decode product are single IEEE operations, round half to even, and
 # the sign scale's sum runs in the kernel's order (elements of a lane in turn, then halving over the 32 / VEC lanes
 # of the block), so both paths produce the same bytes from the same v.
-CHOCO_COMPRESSORS = ("none", "int8", "sign")
-CHOCO_CODE = {"none": 0, "int8": 1, "sign": 2}
+CHOCO_COMPRESSORS = ("none", "int8", "sign", "topk")
+CHOCO_CODE = {"none": 0, "int8": 1, "sign": 2, "topk": 3}
 CHOCO_BLOCK = 32
 CHOCO_VEC = {torch.float32: 4, torch.float64: 2}      # elements per thread in the kernels (16-byte vectors)
+TOPK_RATIO_DEFAULT = 0.01
 
 
-def choco_code_bytes(compressor: str, n_pad: int, dtype: torch.dtype) -> int:
-    """Bytes of one code row."""
+def choco_topk_k(ratio: float, n_live: int) -> int:
+    """Entries a top-k code row keeps: ``max(1, ceil(ratio * n_live))`` of the ``n_live`` parameter elements."""
+    if not 0.0 < float(ratio) <= 1.0:
+        raise ValueError(f"topk_ratio must be in (0, 1] (got {ratio!r})")
+    return max(1, math.ceil(float(ratio) * int(n_live)))
+
+
+def choco_k(conf, compressor: str, live: torch.Tensor, alg: str) -> Optional[int]:
+    """The k of a ``topk`` compressor from an optimizer config (``topk_ratio``, default ``TOPK_RATIO_DEFAULT``), None
+    for the other compressors; ``topk_ratio`` with another compressor is refused."""
+    ratio = conf.get("topk_ratio")
+    if compressor != "topk":
+        if ratio is not None:
+            raise ValueError(f"{alg} topk_ratio applies to compressor topk only (compressor is {compressor!r})")
+        return None
+    return choco_topk_k(TOPK_RATIO_DEFAULT if ratio is None else ratio, int(live.sum()))
+
+
+def choco_code_bytes(compressor: str, n_pad: int, dtype: torch.dtype, k: Optional[int] = None) -> int:
+    """Bytes of one code row (``k``: entries of a top-k row)."""
     s = torch.empty((), dtype=dtype).element_size()
     nb = n_pad // CHOCO_BLOCK
+    if compressor == "topk":
+        return -(-k * (s + 4) // 16) * 16
     return {"none": n_pad * s, "int8": n_pad + nb * s, "sign": 4 * nb + nb * s}[compressor]
+
+
+def choco_topk_keys(v: torch.Tensor, live: torch.Tensor) -> torch.Tensor:
+    """Selection keys of ``v [L, n_pad]``: the IEEE bit pattern with the sign bit cleared (so ``+0`` and ``-0`` tie and
+    the order is exact in both dtypes) as int64, ``-1`` on padding and holes (never selected)."""
+    if v.dtype == torch.float64:
+        key = v.contiguous().view(torch.int64) & 0x7FFFFFFFFFFFFFFF
+    else:
+        key = (v.contiguous().view(torch.int32) & 0x7FFFFFFF).to(torch.int64)
+    return torch.where(live.to(v.device), key, torch.full_like(key, -1))
+
+
+def choco_topk_select(v: torch.Tensor, live: torch.Tensor, k: int) -> torch.Tensor:
+    """``[L, k]`` indices (int64, ascending) of the k live elements of each row with the largest ``|v|``; ties go to the
+    smaller index."""
+    order = torch.sort(choco_topk_keys(v, live), dim=1, descending=True, stable=True).indices
+    return order[:, :k].sort(dim=1).values
 
 
 def choco_live(layout) -> torch.Tensor:
@@ -173,12 +213,21 @@ def _blocks(x: torch.Tensor) -> torch.Tensor:
     return x.reshape(x.shape[:-1] + (x.shape[-1] // CHOCO_BLOCK, CHOCO_BLOCK))
 
 
-def choco_encode(v: torch.Tensor, compressor: str, live: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+def choco_encode(v: torch.Tensor, compressor: str, live: torch.Tensor,
+                 k: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Code rows ``[L, code_bytes]`` (uint8) of ``v [L, n_pad]`` and their decoded values ``[L, n_pad]``."""
     L, n_pad = v.shape
     dt = v.dtype
     if compressor == "none":
         return v.contiguous().view(torch.uint8).clone(), v.clone()
+    if compressor == "topk":
+        idx = choco_topk_select(v, live, k)
+        vals = v.gather(1, idx)
+        codes = torch.zeros(L, choco_code_bytes("topk", n_pad, dt, k), dtype=torch.uint8, device=v.device)
+        s = v.element_size()
+        codes[:, : k * s] = vals.contiguous().view(torch.uint8)
+        codes[:, k * s: k * (s + 4)] = idx.to(torch.int32).contiguous().view(torch.uint8)
+        return codes, torch.zeros_like(v).scatter_(1, idx, vals)
     vb = _blocks(v)
     lb = _blocks(live.to(v.device))
     if compressor == "int8":
@@ -215,12 +264,17 @@ def choco_encode(v: torch.Tensor, compressor: str, live: torch.Tensor) -> Tuple[
 
 
 def choco_decode(codes: torch.Tensor, compressor: str, n_pad: int, dtype: torch.dtype,
-                 live: torch.Tensor) -> torch.Tensor:
+                 live: torch.Tensor, k: Optional[int] = None) -> torch.Tensor:
     """``dec(q)`` of code rows ``[R, code_bytes]`` (uint8) -> ``[R, n_pad]`` in ``dtype``."""
     codes = codes.contiguous()
     R = codes.shape[0]
     if compressor == "none":
         return codes.view(dtype).clone()
+    if compressor == "topk":
+        s = torch.empty((), dtype=dtype).element_size()
+        vals = codes[:, : k * s].contiguous().view(dtype)
+        idx = codes[:, k * s: k * (s + 4)].contiguous().view(torch.int32).to(torch.int64)
+        return torch.zeros(R, n_pad, dtype=dtype, device=codes.device).scatter_(1, idx, vals)
     nb = n_pad // CHOCO_BLOCK
     if compressor == "int8":
         q = codes[:, :n_pad].contiguous().view(torch.int8).to(dtype).reshape(R, nb, CHOCO_BLOCK)
@@ -246,10 +300,10 @@ def choco_mix_(theta: torch.Tensor, x_hat: torch.Tensor, s: torch.Tensor, dec_al
 
 
 def choco_step_(theta: torch.Tensor, x_hat: torch.Tensor, grad: torch.Tensor, alpha: float, compressor: str,
-                live: torch.Tensor) -> torch.Tensor:
+                live: torch.Tensor, k: Optional[int] = None) -> torch.Tensor:
     """``theta -= alpha g``; ``q = Q(theta - x_hat)``; ``x_hat += dec(q)``; returns the code rows ``q`` to publish."""
     theta.add_(grad, alpha=-alpha)
-    codes, dec = choco_encode(theta - x_hat, compressor, live)
+    codes, dec = choco_encode(theta - x_hat, compressor, live, k)
     x_hat.add_(dec)
     return codes
 
@@ -269,14 +323,14 @@ def beer_mix_(theta: torch.Tensor, h: torch.Tensor, s_h: torch.Tensor, v: torch.
 
 def beer_step_(theta: torch.Tensor, h: torch.Tensor, v: torch.Tensor, g: torch.Tensor, s_g: torch.Tensor,
                m_old: torch.Tensor, grad: torch.Tensor, gamma: float, compressor: str,
-               live: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+               live: torch.Tensor, k: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """``v += gamma (s_g - g) + grad - m_old``; ``m_old <- grad``; ``qh = Q(theta - h)``, ``h += dec(qh)``;
     ``qg = Q(v - g)``, ``g += dec(qg)``; returns the code rows ``(qh, qg)`` to publish."""
     v.add_(gamma * (s_g - g) + grad - m_old)
     m_old.copy_(grad)
-    codes_h, dec_h = choco_encode(theta - h, compressor, live)
+    codes_h, dec_h = choco_encode(theta - h, compressor, live, k)
     h.add_(dec_h)
-    codes_g, dec_g = choco_encode(v - g, compressor, live)
+    codes_g, dec_g = choco_encode(v - g, compressor, live, k)
     g.add_(dec_g)
     return codes_h, codes_g
 

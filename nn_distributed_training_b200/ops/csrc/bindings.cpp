@@ -143,9 +143,10 @@ struct ConsensusOp {
     ch.x_hat = ptr<T>(d, "x_hat"); ch.s = ptr<T>(d, "s"); ch.live = ptr<const unsigned>(d, "live");
     ch.gamma = (T)getf(d, "gamma", 1.0); ch.code = geti(d, "code", 0);
     ch.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
+    ch.topk_k = geti(d, "topk_k", 0);
     be.h = ptr<T>(d, "h"); be.s_h = ptr<T>(d, "s_h"); be.v = ptr<T>(d, "v"); be.g = ptr<T>(d, "g");
     be.s_g = ptr<T>(d, "s_g"); be.m_old = ptr<T>(d, "m_old");
-    be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride;
+    be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride; be.topk_k = ch.topk_k;
     kg.corr = ptr<T>(d, "corr"); kg.dacc = ptr<T>(d, "dacc");
     kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
     cg.dist_part = ptr<double>(d, "dist_part"); cg.pstride = geti(d, "pstride", 0);

@@ -68,6 +68,22 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   cfg.attrs = attr; cfg.numAttrs = no_pdl ? 0 : 1;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
 }
+// launch_pdl for a kernel run as thread-block clusters of `cluster_x` CTAs along x: the PDL and cluster-dimension
+// attributes go through cudaLaunchKernelEx together
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, int cluster_x,
+                                      cudaStream_t st, Args&&... args) {
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+  static const bool no_pdl = getenv("NNDT_NO_PDL") != nullptr;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster_x; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr; cfg.numAttrs = no_pdl ? 1 : 2;
+  return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
 
 // ---- TMA bulk copy (cp.async.bulk, SASS: UBLKCP) + mbarrier transaction tracking ---------------------
 NNDT_DEVINL uint32_t smem_addr_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -111,6 +127,12 @@ NNDT_DEVINL uint32_t map_to(const void* p, uint32_t rank) {
 }
 NNDT_DEVINL double ld_dsmem(uint32_t a) { double v; asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory"); return v; }
 NNDT_DEVINL void st_dsmem(uint32_t a, double v) { asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+NNDT_DEVINL uint32_t ld_dsmem_u32(uint32_t a) { uint32_t v; asm volatile("ld.shared::cluster.u32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
+NNDT_DEVINL unsigned long long ld_dsmem_u64(uint32_t a) {
+  unsigned long long v;
+  asm volatile("ld.shared::cluster.u64 %0, [%1];" : "=l"(v) : "r"(a) : "memory");
+  return v;
+}
 
 // ---- cluster pushes: a producer stores into a peer's shared memory and the bytes complete a transaction count on the
 //      peer's mbarrier (release at cluster scope); the consumer waits on its own mbarrier for just those bytes.  Both

@@ -8,7 +8,9 @@
 // Exact Diffusion (no reference counterpart, optimizers/exact_diffusion.py) -> dsgd_mix or ed_sum_mix / ed_step
 // DSGD with momentum (no reference counterpart, optimizers/dsgdm.py)       -> dsgd_mix / dsgdm_step
 // CHOCO-SGD (no reference counterpart, optimizers/choco.py)                -> choco_mix / choco_step
+//                                                          (top-k codes)   -> choco_topk_mix / choco_topk_step
 // BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
+//                                                          (top-k codes)   -> beer_topk_mix / beer_topk_step
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
@@ -789,6 +791,266 @@ __global__ void __launch_bounds__(THREADS) beer_step_kernel(const BeerArgs<T> a)
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------ top-k (CHOCO-SGD, BEER) ----
+// kCodeTopk rows (consensus.h).  A code row holds only k entries, so neither kernel can work by position.
+//
+// The step runs one thread-block cluster of kTopkCluster CTAs per node, grid (CS, L): CTA r owns the contiguous slice
+// [r sl, (r + 1) sl) of the row (topk_slice), so index order is (cluster rank, position in the slice).  It computes
+// the dense step's arithmetic, keeps v in shared memory, selects with topk_threshold and writes the entries with
+// topk_emit, and adds dec(q) = v to x_hat (BEER: h, g) at the selected indices only (x_hat is never -0, so x_hat + 0
+// at the others would not change a bit).  A final cluster barrier keeps every CTA resident until its peers have read
+// its shared memory.  The cluster has 8 CTAs, the portable size, which holds the PAPER MNIST row (n_pad 28 544) at
+// 3 584 elements per CTA; 16 CTAs would need the non-portable attribute and double the DSMEM loads of every histogram
+// reduction, and were not measured.  The digit is 8 bits: one bin per thread of the 256-thread CTA, so a histogram
+// reduction is one DSMEM load per thread and peer, and a pass is one warp's scan of 256 bins.  On an H100 80GB HBM3
+// (700 W) the step takes 25 us in fp64 against int8's 4.5 us (README.md).
+//
+// The mix gathers, per chunk of THREADS * N elements, each row's entries in the chunk into a zeroed shared tile (a warp
+// per row: binary search on the ascending indices, then a scatter), 8 rows at a time (BEER: 4 rows of both channels),
+// and then runs the dense mix's arithmetic on the tiles in the same order: with topk_ratio 1 it is bitwise the
+// compressor none.
+// The grid is only kTopkCluster CTAs per node, so the step kernels take the registers they need (126-158, no spills)
+// rather than a cap that keeps several CTAs resident per SM: with the default cap the fp64 8-deep CHOCO step spilled.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS, 1) choco_topk_step_kernel(const ChocoArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char topk_smem[];
+  __shared__ TopkShared sh;
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  const int sl = topk_slice(c.n_pad), base = blockIdx.x * sl, len = max(0, min(sl, c.n_pad - base));
+  T* sv = reinterpret_cast<T*>(topk_smem);
+  unsigned* slive = reinterpret_cast<unsigned*>(sv + sl);
+  // theta and x_hat are read before the programmatic-dependency wait, as in choco_step
+  bool waited = false;
+  for (int j = threadIdx.x * N; j < len; j += THREADS * N) {
+    const int i = base + j;
+    Pack<T> th = ldv(c.theta + row + i);
+    const Pack<T> xh = ldv(a.x_hat + row + i);
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> v;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      th.v[u] -= alpha * g.v[u];
+      v.v[u] = th.v[u] - xh.v[u];
+    }
+    stv(c.theta + row + i, th);
+    stv(sv + j, v);
+  }
+  release_dependents_once(waited);
+  topk_live_words(slive, a.live, base, len);
+  __syncthreads();
+  int pc = 0;
+  const TopkThr<T> thr = topk_threshold(sv, len, slive, a.topk_k, sh, pc);
+  char* out = code_row(a, ri.par ^ 1, l);
+  T* vals = reinterpret_cast<T*>(out);
+  unsigned* idx = reinterpret_cast<unsigned*>(out + (size_t)a.topk_k * sizeof(T));
+  topk_emit(sv, len, slive, thr, sh, 0, [&](int j, unsigned pos) {
+    const T v = sv[j];
+    vals[pos] = v;
+    idx[pos] = (unsigned)(base + j);
+    a.x_hat[row + base + j] += v;
+  });
+  topk_pad(out, a.topk_k, (int)sizeof(T), a.code_stride);
+  cluster_sync();
+  end_step(c, l, ri.k, true);
+}
+
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS, 1) beer_topk_step_kernel(const BeerArgs<T> a) {
+  extern __shared__ __align__(16) unsigned char topk_smem[];
+  __shared__ TopkShared sh;
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const size_t row = (size_t)l * c.n_pad;
+  const int sl = topk_slice(c.n_pad), base = blockIdx.x * sl, len = max(0, min(sl, c.n_pad - base));
+  T* sdx = reinterpret_cast<T*>(topk_smem);       // channel 0: theta - h
+  T* sdv = sdx + sl;                               // channel 1: v - g
+  unsigned* slive = reinterpret_cast<unsigned*>(sdv + sl);
+  // theta, s_g, h, v, g and m_old are read before the programmatic-dependency wait, as in beer_step
+  bool waited = false;
+  for (int j = threadIdx.x * N; j < len; j += THREADS * N) {
+    const int i = base + j;
+    const Pack<T> x = ldv(c.theta + row + i), h = ldv(a.h + row + i), g = ldv(a.g + row + i);
+    const Pack<T> sg = ldv(a.s_g + row + i), mo = ldv(a.m_old + row + i);
+    Pack<T> v = ldv(a.v + row + i);
+    release_dependents_once(waited);
+    const Pack<T> gr = sum_partials<U>(c, l, i);
+    Pack<T> dx, dv;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      v.v[u] += a.gamma * (sg.v[u] - g.v[u]) + gr.v[u] - mo.v[u];
+      dx.v[u] = x.v[u] - h.v[u];
+      dv.v[u] = v.v[u] - g.v[u];
+    }
+    stv(a.v + row + i, v);
+    stv(a.m_old + row + i, gr);
+    stv(sdx + j, dx);
+    stv(sdv + j, dv);
+  }
+  release_dependents_once(waited);
+  topk_live_words(slive, a.live, base, len);
+  __syncthreads();
+  int pc = 0;
+#pragma unroll 1
+  for (int ch = 0; ch < 2; ++ch) {
+    const T* sv = ch == 0 ? sdx : sdv;
+    T* est = ch == 0 ? a.h : a.g;
+    const TopkThr<T> thr = topk_threshold(sv, len, slive, a.topk_k, sh, pc);
+    char* out = beer_code_row(a, ri.par ^ 1, ch, l);
+    T* vals = reinterpret_cast<T*>(out);
+    unsigned* idx = reinterpret_cast<unsigned*>(out + (size_t)a.topk_k * sizeof(T));
+    topk_emit(sv, len, slive, thr, sh, ch, [&](int j, unsigned pos) {
+      const T v = sv[j];
+      vals[pos] = v;
+      idx[pos] = (unsigned)(base + j);
+      est[row + base + j] += v;
+    });
+    topk_pad(out, a.topk_k, (int)sizeof(T), a.code_stride);
+  }
+  cluster_sync();
+  end_step(c, l, ri.k, true);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS) choco_topk_mix_kernel(const ChocoArgs<T> a) {
+  constexpr int N = Vec<T>::N, CH = THREADS * N, R = THREADS / 32;
+  __shared__ __align__(16) T tile[R][CH];
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const char* own = code_row(a, ri.par, l);
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, o = threadIdx.x * N;
+  Pack<T> zero;
+#pragma unroll
+  for (int u = 0; u < N; ++u) zero.v[u] = (T)0;
+  for (int c0 = blockIdx.x * CH; c0 < c.n_pad; c0 += gridDim.x * CH) {
+    Pack<T> t;
+    // rows r = 0 (own) .. deg (neighbor r - 1), R at a time: warp q gathers row r0 + q
+    for (int r0 = 0; r0 <= deg; r0 += R) {
+#pragma unroll
+      for (int q = 0; q < R; ++q) stv(&tile[q][o], zero);
+      __syncthreads();
+      if (r0 + wid <= deg)
+        topk_gather(r0 + wid == 0 ? own : nbr_code_row(a, ri.gid, l, r0 + wid - 1, ri.par), a.topk_k, c0, CH, tile[wid], lane);
+      __syncthreads();
+      for (int q = 0; q < R && r0 + q <= deg; ++q) {
+        const Pack<T> d = ldv(&tile[q][o]);
+        if (r0 + q == 0) {
+          t = d;
+#pragma unroll
+          for (int u = 0; u < N; ++u) t.v[u] *= ws;
+        } else {
+          const int e = r0 + q - 1;
+#pragma unroll
+          for (int u = 0; u < N; ++u) t.v[u] += w[e] * d.v[u];
+        }
+      }
+    }
+    const int i = c0 + o;
+    if (i < c.n_pad) {
+      Pack<T> s = ldv(a.s + row + i);
+      const Pack<T> xh = ldv(a.x_hat + row + i);
+      Pack<T> th = ldv(c.theta + row + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        s.v[u] += t.v[u];
+        th.v[u] += a.gamma * (s.v[u] - xh.v[u]);
+      }
+      stv(a.s + row + i, s);
+      stv(c.theta + row + i, th);
+    }
+    __syncthreads();      // the tiles are read before the next chunk zeroes them
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS) beer_topk_mix_kernel(const BeerArgs<T> a) {
+  constexpr int N = Vec<T>::N, CH = THREADS * N, R = THREADS / 64;
+  __shared__ __align__(16) T tile[2][R][CH];
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T alpha = c.alpha[ri.k];
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  // warp wid gathers channel wid / R of row r0 + wid % R
+  const int lane = threadIdx.x & 31, ch = (threadIdx.x >> 5) / R, wq = (threadIdx.x >> 5) % R, o = threadIdx.x * N;
+  const char* own = beer_code_row(a, ri.par, ch, l);
+  Pack<T> zero;
+#pragma unroll
+  for (int u = 0; u < N; ++u) zero.v[u] = (T)0;
+  for (int c0 = blockIdx.x * CH; c0 < c.n_pad; c0 += gridDim.x * CH) {
+    Pack<T> th, tg;
+    for (int r0 = 0; r0 <= deg; r0 += R) {
+#pragma unroll
+      for (int q = 0; q < R; ++q) {
+        stv(&tile[0][q][o], zero);
+        stv(&tile[1][q][o], zero);
+      }
+      __syncthreads();
+      const int r = r0 + wq;
+      if (r <= deg)
+        topk_gather(r == 0 ? own : reinterpret_cast<const char*>(nbr_row(c, ri.gid, l, r - 1, ri.par, ch)), a.topk_k,
+                    c0, CH, tile[ch][wq], lane);
+      __syncthreads();
+      for (int q = 0; q < R && r0 + q <= deg; ++q) {
+        const Pack<T> dh = ldv(&tile[0][q][o]), dg = ldv(&tile[1][q][o]);
+        if (r0 + q == 0) {
+          th = dh;
+          tg = dg;
+#pragma unroll
+          for (int u = 0; u < N; ++u) {
+            th.v[u] *= ws;
+            tg.v[u] *= ws;
+          }
+        } else {
+          const T we = w[r0 + q - 1];
+#pragma unroll
+          for (int u = 0; u < N; ++u) {
+            th.v[u] += we * dh.v[u];
+            tg.v[u] += we * dg.v[u];
+          }
+        }
+      }
+    }
+    const int i = c0 + o;
+    if (i < c.n_pad) {
+      Pack<T> sh = ldv(a.s_h + row + i), sg = ldv(a.s_g + row + i);
+      const Pack<T> h = ldv(a.h + row + i), v = ldv(a.v + row + i);
+      Pack<T> x = ldv(c.theta + row + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        sh.v[u] += th.v[u];
+        sg.v[u] += tg.v[u];
+        x.v[u] += a.gamma * (sh.v[u] - h.v[u]) - alpha * v.v[u];
+      }
+      stv(a.s_h + row + i, sh);
+      stv(a.s_g + row + i, sg);
+      stv(c.theta + row + i, x);
+    }
+    __syncthreads();
+  }
+}
+
 // -------------------------------------------------------------------- K-GT ----
 // Channel 0 of the published buffer is theta, channel 1 the tracker y (correction mode).  Round k: kgt_mix pulls the
 // rows published at the end of round k-1, theta_i <- sum_j W_ij theta_j and c_i += sum_j W_ij y_j - y_i (own terms
@@ -1436,11 +1698,26 @@ template <typename T, int Q> static cudaError_t launch_choco_q(const ChocoArgs<T
   return step ? launch_by_s(choco_step_kernel<T, 4, Q>, choco_step_kernel<T, 8, Q>, a.c, a, st)
               : launch_one_wave(choco_mix_kernel<T, Q>, a.c, a, st);
 }
+// top-k step: one cluster of kTopkCluster CTAs per node, grid (CS, L), with `chans` slices of v in dynamic shared memory
+template <typename T, typename K, typename A>
+static cudaError_t launch_topk_step(K kernel, const Common<T>& c, int chans, int k, long long stride, const A& a,
+                                    cudaStream_t st) {
+  const int sl = topk_slice(c.n_pad);
+  const size_t smem = (size_t)chans * sl * sizeof(T) + sl / 8;      // the slices of v, then the slice's live words
+  if (smem > (size_t)kTopkRowSmem || k < 1 || stride < (long long)k * (long long)(sizeof(T) + 4)) return cudaErrorInvalidValue;
+  const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTopkRowSmem);
+  if (e != cudaSuccess) return e;
+  return launch_pdl_cluster(kernel, dim3(kTopkCluster, c.L), dim3(THREADS), smem, kTopkCluster, st, a);
+}
 template <typename T> static cudaError_t launch_choco(const ChocoArgs<T>& a, bool step, cudaStream_t st) {
   switch (a.code) {
     case kCodeNone: return launch_choco_q<T, kCodeNone>(a, step, st);
     case kCodeInt8: return launch_choco_q<T, kCodeInt8>(a, step, st);
     case kCodeSign: return launch_choco_q<T, kCodeSign>(a, step, st);
+    case kCodeTopk:
+      if (!step) return launch_one_wave(choco_topk_mix_kernel<T>, a.c, a, st);
+      return launch_topk_step(a.c.S <= 4 ? choco_topk_step_kernel<T, 4> : choco_topk_step_kernel<T, 8>, a.c, 1, a.topk_k,
+                              a.code_stride, a, st);
   }
   return cudaErrorInvalidValue;
 }
@@ -1456,6 +1733,10 @@ template <typename T> static cudaError_t launch_beer(const BeerArgs<T>& a, bool 
     case kCodeNone: return launch_beer_q<T, kCodeNone>(a, step, st);
     case kCodeInt8: return launch_beer_q<T, kCodeInt8>(a, step, st);
     case kCodeSign: return launch_beer_q<T, kCodeSign>(a, step, st);
+    case kCodeTopk:
+      if (!step) return launch_one_wave(beer_topk_mix_kernel<T>, a.c, a, st);
+      return launch_topk_step(a.c.S <= 4 ? beer_topk_step_kernel<T, 4> : beer_topk_step_kernel<T, 8>, a.c, 2, a.topk_k,
+                              a.code_stride, a, st);
   }
   return cudaErrorInvalidValue;
 }

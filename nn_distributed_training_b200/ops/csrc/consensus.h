@@ -118,8 +118,18 @@ struct MomentumArgs {
 //   kCodeInt8: [n_pad] int8 codes, [nb] T scales  dec = code * scale, scale = max|v| / 127
 //   kCodeSign: [nb] uint32 sign words, [nb] T     bit (i % 32) of word b set when v >= 0; dec = +-scale on live
 //                                                 elements (bit set in `live`), 0 elsewhere; scale = sum|v| / n_live
+//   kCodeTopk: [k] T values, [k] uint32 indices   the k = topk_k live elements of largest |v|, indices ascending, then
+//                                                 zero padding to a multiple of 16 bytes (values first: fp64 values stay
+//                                                 8-byte aligned for any k); dec = v at the indices (exact), 0 elsewhere.
+//              Selection: keys are the IEEE bits of v with the sign bit cleared (+0 and -0 tie; the integer order is
+//              the order of |v| in both dtypes), ordered by key descending, ties by the smaller index; the first k.
 // The same layout is written by ops/consensus_ref.py: choco_encode / choco_decode.
-enum Code : int { kCodeNone = 0, kCodeInt8 = 1, kCodeSign = 2 };
+enum Code : int { kCodeNone = 0, kCodeInt8 = 1, kCodeSign = 2, kCodeTopk = 3 };
+// The top-k step selects with one thread-block cluster of kTopkCluster CTAs per node, each holding the v of its slice
+// of the row (both channels for BEER) in shared memory: rows whose slices need more than kTopkRowSmem bytes are
+// refused (ops/engine.py: check_topk_capacity)
+constexpr int kTopkCluster = 8;
+constexpr int kTopkRowSmem = 220 * 1024;
 
 template <typename T>
 struct ChocoArgs {
@@ -130,6 +140,7 @@ struct ChocoArgs {
   T gamma;                         // consensus step
   int code;                        // Code
   long long code_stride;           // bytes per code row of the published buffer
+  int topk_k;                      // entries of a kCodeTopk row
 };
 
 // BEER (Zhao, Li, Li, Richtárik, Chi 2022): DSGT's gradient tracking with both the parameters and the tracker gossiped
@@ -148,6 +159,7 @@ struct BeerArgs {
   T gamma;                         // consensus step
   int code;                        // Code
   long long code_stride;           // bytes per code row of the published buffer
+  int topk_k;                      // entries of a kCodeTopk row
 };
 
 // K-GT (Liu, Lin, Koloskova, Stich 2023): gradient tracking with `K` local steps per communication round, and local

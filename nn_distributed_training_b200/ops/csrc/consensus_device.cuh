@@ -446,6 +446,203 @@ NNDT_DEVINL char* beer_code_row(const BeerArgs<T>& a, int par, int chan, int l) 
   return reinterpret_cast<char*>(c.pub) + ((size_t)(par * c.C + chan) * c.pub_L + l) * (size_t)a.code_stride;
 }
 
+// ---- top-k code rows (layout in consensus.h) ----
+// the slice of the row one CTA of the step's cluster owns: a multiple of 32 elements, so every slice starts 16-byte
+// aligned and holds whole live words
+__host__ __device__ __forceinline__ int topk_slice(int n_pad) {
+  return ((n_pad + kTopkCluster - 1) / kTopkCluster + 31) / 32 * 32;
+}
+
+// selection keys: the IEEE bits with the sign bit cleared, as an unsigned integer ordered as |v|
+template <typename T> struct TopkKey;
+template <> struct TopkKey<float> {
+  using K = unsigned;
+  static constexpr int kPasses = 4;                 // 31 key bits, 8-bit digits from bit 24 down
+  static NNDT_DEVINL K key(float v) { return __float_as_uint(v) & 0x7fffffffu; }
+};
+template <> struct TopkKey<double> {
+  using K = unsigned long long;
+  static constexpr int kPasses = 8;                 // 63 key bits, 8-bit digits from bit 56 down
+  static NNDT_DEVINL K key(double v) { return (unsigned long long)__double_as_longlong(v) & 0x7fffffffffffffffull; }
+};
+
+constexpr int kTopkBins = 256;                      // one 8-bit digit; THREADS == kTopkBins: a thread per bin
+struct TopkShared {
+  unsigned hist[2][kTopkBins];                      // this CTA's digit histograms, double buffered (peers read them)
+  unsigned tot[kTopkBins];                          // the cluster's sums of the current pass
+  unsigned long long cta_cnt[2];                    // per channel: (above << 32) | equal keys of this CTA (peers read)
+  unsigned long long warp_cnt[THREADS / 32];
+  int bin, kr, cnt;                                 // the digit a pass picked, the entries still to take, its bin count
+};
+
+// the k-th largest key so far: keys k with (k & mask) > prefix are selected, and of those equal to prefix the first kr
+template <typename T>
+struct TopkThr {
+  typename TopkKey<T>::K prefix, mask;
+  int kr;
+};
+
+// live bit of slice element j: `live` is the slice's copy of the mask in shared memory (slices start on a word)
+NNDT_DEVINL bool live_at(const unsigned* live, int j) { return (live[j >> 5] >> (j & 31)) & 1u; }
+
+// copy the live words of the slice [base, base + len) into shared memory
+NNDT_DEVINL void topk_live_words(unsigned* dst, const unsigned* live, int base, int len) {
+  for (int w = threadIdx.x; w < (len >> 5); w += THREADS) dst[w] = live[(base >> 5) + w];
+}
+
+// MSD radix select over the cluster: sv [len] is this CTA's slice and `live` its live words in shared memory; every CTA
+// of the cluster calls it and gets the same result.  Each pass counts this CTA's live keys that match the prefix so far per 8-bit digit (warp
+// aggregated shared atomics), sums the cluster's histograms through DSMEM and picks the digit where the count from the
+// top reaches kr.  It stops early when that digit's bin holds exactly kr keys: all of them are selected and no tie is
+// left.  `pc` counts passes over the channels of a launch: the histograms are double buffered, so the one cluster
+// barrier of a pass also guarantees that the peers have read the buffer it zeroes (they read it two passes back).
+template <typename T>
+NNDT_DEVINL TopkThr<T> topk_threshold(const T* sv, int len, const unsigned* live, int k, TopkShared& sh, int& pc) {
+  using KT = TopkKey<T>;
+  using K = typename KT::K;
+  TopkThr<T> r;
+  r.prefix = 0; r.mask = 0; r.kr = k;
+  for (int p = 0; p < KT::kPasses; ++p) {
+    const int shift = 8 * (KT::kPasses - 1 - p);
+    unsigned* h = sh.hist[pc & 1];
+    ++pc;
+    h[threadIdx.x] = 0u;
+    __syncthreads();
+    for (int j = threadIdx.x; j < len; j += THREADS) {     // len is a multiple of 32: whole warps iterate
+      int bin = -1;
+      if (live_at(live, j)) {
+        const K key = KT::key(sv[j]);
+        if ((key & r.mask) == r.prefix) bin = (int)(key >> shift) & (kTopkBins - 1);
+      }
+      const unsigned same = __match_any_sync(0xffffffffu, bin);
+      if (bin >= 0 && (int)(threadIdx.x & 31) == __ffs(same) - 1) atomicAdd(&h[bin], (unsigned)__popc(same));
+    }
+    cluster_sync();
+    unsigned part[kTopkCluster], t = 0u;          // all loads in flight before the first add
+#pragma unroll
+    for (int q = 0; q < kTopkCluster; ++q) part[q] = ld_dsmem_u32(map_to(h + threadIdx.x, q));
+#pragma unroll
+    for (int q = 0; q < kTopkCluster; ++q) t += part[q];
+    sh.tot[threadIdx.x] = t;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+      // lane holds bins 8 lane .. 8 lane + 7; `above` counts the keys in the bins of the higher lanes
+      const int lane = threadIdx.x;
+      unsigned cnt[8], s = 0u;
+#pragma unroll
+      for (int u = 0; u < 8; ++u) { cnt[u] = sh.tot[8 * lane + u]; s += cnt[u]; }
+      unsigned suf = s;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const unsigned x = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += x;
+      }
+      unsigned cum = suf - s;
+      if (cum < (unsigned)r.kr && (unsigned)r.kr <= suf) {
+        for (int u = 7; u >= 0; --u) {
+          if (cum + cnt[u] >= (unsigned)r.kr) {
+            sh.bin = 8 * lane + u; sh.kr = r.kr - (int)cum; sh.cnt = (int)cnt[u];
+            break;
+          }
+          cum += cnt[u];
+        }
+      }
+    }
+    __syncthreads();
+    r.prefix |= (K)sh.bin << shift;
+    r.mask |= (K)(kTopkBins - 1) << shift;
+    r.kr = sh.kr;
+    if (sh.cnt == r.kr) break;
+  }
+  return r;
+}
+
+// Position of every selected entry of the slice in the code row, index order: thread t walks the contiguous segment
+// t of the slice; a block scan and a cluster exclusive scan of the packed (above, equal) counts give the entries
+// before it.  emit(j, pos) is called once per selected slice element j.
+template <typename T, class F>
+NNDT_DEVINL void topk_emit(const T* sv, int len, const unsigned* live, const TopkThr<T>& thr, TopkShared& sh, int ch,
+                           F emit) {
+  using KT = TopkKey<T>;
+  using K = typename KT::K;
+  const int seg = (len + THREADS - 1) / THREADS;
+  const int j0 = min(len, (int)threadIdx.x * seg), j1 = min(len, j0 + seg);
+  unsigned gt = 0u, eq = 0u;
+  for (int j = j0; j < j1; ++j) {
+    if (!live_at(live, j)) continue;
+    const K mk = KT::key(sv[j]) & thr.mask;
+    gt += mk > thr.prefix;
+    eq += mk == thr.prefix;
+  }
+  const unsigned long long mine = ((unsigned long long)gt << 32) | eq;
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  unsigned long long incl = mine;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned long long x = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += x;
+  }
+  if (lane == 31) sh.warp_cnt[wid] = incl;
+  __syncthreads();
+  unsigned long long before = incl - mine, cta = 0ull;
+  for (int w = 0; w < THREADS / 32; ++w) {
+    const unsigned long long x = sh.warp_cnt[w];
+    if (w < wid) before += x;
+    cta += x;
+  }
+  if (threadIdx.x == 0) sh.cta_cnt[ch] = cta;
+  cluster_sync();
+  const unsigned rank = cluster_rank();
+  for (unsigned q = 0; q < rank; ++q) before += ld_dsmem_u64(map_to(&sh.cta_cnt[ch], q));
+  unsigned gtb = (unsigned)(before >> 32), eqb = (unsigned)before;
+  const unsigned kr = (unsigned)thr.kr;
+  for (int j = j0; j < j1; ++j) {
+    if (!live_at(live, j)) continue;
+    const K mk = KT::key(sv[j]) & thr.mask;
+    if (mk > thr.prefix) {
+      emit(j, gtb + min(eqb, kr));
+      ++gtb;
+    } else if (mk == thr.prefix) {
+      if (eqb < kr) emit(j, gtb + eqb);
+      ++eqb;
+    }
+  }
+}
+
+// zero the bytes of a code row past its k entries (cluster rank 0 of the node)
+NNDT_DEVINL void topk_pad(char* out, int k, int value_bytes, long long stride) {
+  if (blockIdx.x != 0) return;
+  for (long long b = (long long)k * (value_bytes + 4) + threadIdx.x; b < stride; b += THREADS) out[b] = 0;
+}
+
+// first j in [0, k) with idx[j] >= key (k when there is none), by the 32 lanes of a warp: each round probes 32 evenly
+// spaced entries, so a row of k entries takes about log32(k) dependent loads
+NNDT_DEVINL int warp_lower_bound(const unsigned* idx, int k, unsigned key, int lane) {
+  int lo = 0, hi = k;                               // the answer lies in [lo, hi]
+  while (lo < hi) {
+    const int step = (hi - lo + 31) >> 5;
+    const int p = lo + lane * step;
+    const unsigned m = __ballot_sync(0xffffffffu, p >= hi || idx[p] >= key);
+    if (m == 0u) { lo += 31 * step + 1; continue; }
+    const int f = __ffs(m) - 1;
+    if (f == 0) break;
+    hi = min(hi, lo + f * step);
+    lo += (f - 1) * step + 1;
+  }
+  return lo;
+}
+
+// scatter the entries of a top-k code row that fall in the elements [c0, c0 + len) into tile [len] (zeroed by the
+// caller), by one warp
+template <typename T>
+NNDT_DEVINL void topk_gather(const char* code, int k, int c0, int len, T* tile, int lane) {
+  const T* vals = reinterpret_cast<const T*>(code);
+  const unsigned* idx = reinterpret_cast<const unsigned*>(code + (size_t)k * sizeof(T));
+  const int lo = warp_lower_bound(idx, k, (unsigned)c0, lane);
+  const int hi = lo + warp_lower_bound(idx + lo, min(k - lo, len), (unsigned)(c0 + len), lane);
+  for (int j = lo + lane; j < hi; j += 32) tile[idx[j] - c0] = vals[j];
+}
+
 // ---- ClippedGossip: chunks of THREADS * N elements, one distance partial each ----
 template <typename T>
 __host__ __device__ __forceinline__ int cg_chunks(const Common<T>& c) {

@@ -67,6 +67,32 @@ def check_clip_capacity(dmax: int) -> None:
                          f"fused kernels; the planned graphs have a node with {dmax}")
 
 
+TOPK_CLUSTER = 8              # consensus.h: kTopkCluster
+TOPK_ROW_SMEM = 220 * 1024    # consensus.h: kTopkRowSmem
+
+
+def topk_slice(n_pad: int) -> int:
+    """Elements of the row one CTA of the top-k step's cluster holds (consensus_device.cuh: topk_slice)."""
+    return -(-(-(-n_pad // TOPK_CLUSTER)) // 32) * 32
+
+
+def topk_max_row(itemsize: int, chans: int) -> int:
+    """The longest row the top-k step selects from: its slices of v and live bits fit ``TOPK_ROW_SMEM``."""
+    return 8 * TOPK_ROW_SMEM // (8 * chans * itemsize + 1) // 32 * 32 * TOPK_CLUSTER
+
+
+def check_topk_capacity(alg: str, n_pad: int, itemsize: int, chans: int) -> None:
+    """The top-k step keeps ``v`` of its slice of the row (``chans`` channels) and the slice's live bits in the shared
+    memory of each CTA of a ``TOPK_CLUSTER``-CTA cluster, at most ``TOPK_ROW_SMEM`` bytes."""
+    sl = topk_slice(n_pad)
+    need = chans * sl * itemsize + sl // 8          # the slices of v, then the slice's live words
+    if need > TOPK_ROW_SMEM:
+        raise ValueError(f"{alg} with compressor topk selects in the shared memory of one {TOPK_CLUSTER}-CTA cluster "
+                         f"per node: rows of at most {topk_max_row(itemsize, chans)} elements at this dtype (the row "
+                         f"has n_pad = {n_pad}, "
+                         f"{need} bytes per CTA against a limit of {TOPK_ROW_SMEM})")
+
+
 class ConsensusEngine:
     def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
@@ -151,6 +177,8 @@ class ConsensusEngine:
             gid[k] = gi
         self.topos = topos
         G = len(topos)
+        if (self.choco or self.beer) and opt.compressor == "topk":
+            check_topk_capacity(opt.alg_name, n_pad, itemsize, self.C)
         if self.choco and G > 1:
             raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
                              f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
@@ -354,12 +382,13 @@ class ConsensusEngine:
         if self.choco:
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
-                     code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
+                     code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes), topk_k=int(opt.topk_k or 0))
         if self.beer:
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(h=opt.h.data_ptr(), s_h=opt.s_h.data_ptr(), v=opt.v.data_ptr(), g=opt.g.data_ptr(),
                      s_g=opt.s_g.data_ptr(), m_old=opt.m_old.data_ptr(), live=self.t_live.data_ptr(),
-                     gamma=float(opt.gamma), code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes))
+                     gamma=float(opt.gamma), code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes),
+                     topk_k=int(opt.topk_k or 0))
         if self.sgp:
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
         if self.pdg:

@@ -4,7 +4,8 @@ reference.
 CHOCO-SGD compresses gossip but keeps DSGD's bias on heterogeneous data; DSGT removes the bias but pulls two full rows
 per edge.  BEER is DSGT's gradient tracking with both the parameters and the tracker gossiped through CHOCO's
 compressed differences (error feedback through public estimates).  Each node publishes two code rows per round, in
-CHOCO's formats and byte layouts (``compressor``: ``none``, ``int8`` or ``sign``, ``ops/consensus_ref.py``).  Node i
+CHOCO's formats and byte layouts (``compressor``: ``none``, ``int8``, ``sign`` or ``topk`` with ``topk_ratio``,
+``ops/consensus_ref.py``).  Node i
 keeps ``theta`` (x), ``h`` (public estimate of x: the sum of its decoded x-codes), ``s_h = sum_j W_ij h_j``, the tracker
 ``v``, ``g`` (public estimate of v), ``s_g = sum_j W_ij g_j`` (own terms included) and ``m_old``, the previous round's
 gradient.  With a constant step ``alpha`` (the paper's eta) and the consensus step ``gamma`` in (0, 1], round k is
@@ -64,7 +65,8 @@ class BEER(ConsensusOptimizer):
         if a.n_pad % 128 != 0:
             raise ValueError(f"beer needs rows padded to a multiple of 128 elements (n_pad = {a.n_pad})")
         self.live = ref.choco_live(a.layout).to(self.device)
-        self.code_bytes = ref.choco_code_bytes(self.compressor, a.n_pad, a.dtype)
+        self.topk_k = ref.choco_k(conf, self.compressor, self.live, "beer")     # entries of a top-k code row (else None)
+        self.code_bytes = ref.choco_code_bytes(self.compressor, a.n_pad, a.dtype, self.topk_k)
         self.h, self.s_h = a.zeros(), a.zeros()
         self.v, self.g, self.s_g = a.zeros(), a.zeros(), a.zeros()
         self.m_old = a.zeros()
@@ -79,7 +81,7 @@ class BEER(ConsensusOptimizer):
 
     def _decode_all(self, code):
         a = self.arena
-        return ref.choco_decode(self.pr.gather_rows(code), self.compressor, a.n_pad, a.dtype, self.live)
+        return ref.choco_decode(self.pr.gather_rows(code), self.compressor, a.n_pad, a.dtype, self.live, self.topk_k)
 
     def _round(self, k: int):
         pr, a = self.pr, self.arena
@@ -90,6 +92,6 @@ class BEER(ConsensusOptimizer):
         pr.compute_grads()
         with torch.no_grad():
             qh, qg = ref.beer_step_(a.theta, self.h, self.v, self.g, self.s_g, self.m_old, a.grad, self.gamma,
-                                    self.compressor, self.live)
+                                    self.compressor, self.live, self.topk_k)
             self.code_h.copy_(qh)
             self.code_g.copy_(qg)

@@ -2,8 +2,9 @@
 form of the paper's appendix.  No counterpart in the reference.
 
 Nodes publish a *code* of the difference between their parameters and their public estimate ``x_hat`` instead of the
-parameters themselves (``compressor``: ``none``, ``int8`` with one scale per 32 elements, or ``sign``, one bit per
-element and one scale per 32; byte layouts in ``ops/consensus_ref.py``).  ``x_hat_i`` is the sum of node i's decoded
+parameters themselves (``compressor``: ``none``, ``int8`` with one scale per 32 elements, ``sign``, one bit per
+element and one scale per 32, or ``topk``, the ``k = max(1, ceil(topk_ratio n_live))`` entries of largest magnitude
+with their indices, ``topk_ratio`` default 0.01; byte layouts in ``ops/consensus_ref.py``).  ``x_hat_i`` is the sum of node i's decoded
 codes, known to every neighbor; ``s_i = sum_j W_ij x_hat_j`` (own term included) is kept by node i, so nobody stores
 copies of its neighbors' estimates.  With DSGD's step schedule ``alpha_k = alpha_{k-1} (1 - mu alpha_{k-1})`` and the
 consensus step ``gamma`` in (0, 1], round k of node i is
@@ -61,7 +62,8 @@ class ChocoSGD(ConsensusOptimizer):
         if a.n_pad % 128 != 0:
             raise ValueError(f"choco_sgd needs rows padded to a multiple of 128 elements (n_pad = {a.n_pad})")
         self.live = ref.choco_live(a.layout).to(self.device)
-        self.code_bytes = ref.choco_code_bytes(self.compressor, a.n_pad, a.dtype)
+        self.topk_k = ref.choco_k(conf, self.compressor, self.live, "choco_sgd")     # entries of a top-k code row (else None)
+        self.code_bytes = ref.choco_code_bytes(self.compressor, a.n_pad, a.dtype, self.topk_k)
         self.x_hat = a.zeros()
         self.s = a.zeros()
         # the code row published at the end of the last round (all zero before round 0: it decodes to 0)
@@ -85,11 +87,13 @@ class ChocoSGD(ConsensusOptimizer):
         topo = pr.topology()
         self.alph = ref.dsgd_alpha(self.alph, self.mu)
         with torch.no_grad():
-            dec_all = ref.choco_decode(pr.gather_rows(self.code), self.compressor, a.n_pad, a.dtype, self.live)
+            dec_all = ref.choco_decode(pr.gather_rows(self.code), self.compressor, a.n_pad, a.dtype, self.live,
+                                       self.topk_k)
             ref.choco_mix_(a.theta, self.x_hat, self.s, dec_all, self._rows(topo, topo.W), self.gamma)
         pr.compute_grads()
         with torch.no_grad():
-            self.code.copy_(ref.choco_step_(a.theta, self.x_hat, a.grad, self.alph, self.compressor, self.live))
+            self.code.copy_(ref.choco_step_(a.theta, self.x_hat, a.grad, self.alph, self.compressor, self.live,
+                                            self.topk_k))
 
 
 def check_static_plan(graphs, alg="choco_sgd", why="s = sum_j W_ij x_hat_j is only valid for a fixed W"):

@@ -13,6 +13,8 @@ from typing import Any, Dict, Iterable, Optional
 
 import yaml
 
+from ..ops.consensus_ref import CHOCO_COMPRESSORS, TOPK_RATIO_DEFAULT
+
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
@@ -20,7 +22,6 @@ ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer"
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
-CHOCO_COMPRESSORS = ("none", "int8", "sign")
 MOMENTUM_MODES = ("local", "quasi_global")
 MNIST_METRICS = ("forward_pass_count", "validation_loss", "consensus_error", "top1_accuracy",
                  "current_epoch", "validation_as_vector")
@@ -54,6 +55,19 @@ OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_fo
 
 class ConfigError(ValueError):
     pass
+
+
+def _check_compressor(c: Dict[str, Any], path: str) -> None:
+    """CHOCO-SGD / BEER: the compressor, and ``topk_ratio`` (default ``TOPK_RATIO_DEFAULT``) with ``topk`` only."""
+    if c["compressor"] not in CHOCO_COMPRESSORS:
+        raise ConfigError(f"{path}.compressor must be one of {'|'.join(CHOCO_COMPRESSORS)} (got {c['compressor']!r})")
+    if c["compressor"] != "topk":
+        if "topk_ratio" in c:
+            raise ConfigError(f"{path}.topk_ratio applies to compressor topk only (compressor is {c['compressor']!r})")
+        return
+    r = c.setdefault("topk_ratio", TOPK_RATIO_DEFAULT)
+    if isinstance(r, bool) or not isinstance(r, (int, float)) or not 0.0 < float(r) <= 1.0:
+        raise ConfigError(f"{path}.topk_ratio must be in (0, 1] (got {r!r})")
 
 
 def _fill(d: Dict[str, Any], schema: Dict[str, Any], path: str, extra: Iterable[str] = ()) -> Dict[str, Any]:
@@ -104,8 +118,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
     if alg == "choco_sgd":
         if not 0.0 < float(c["gamma"]) <= 1.0:
             raise ConfigError(f"{path}.gamma must be in (0, 1] (got {c['gamma']!r})")
-        if c["compressor"] not in CHOCO_COMPRESSORS:
-            raise ConfigError(f"{path}.compressor must be one of {'|'.join(CHOCO_COMPRESSORS)} (got {c['compressor']!r})")
+        _check_compressor(c, path)
         # s = sum_j W_ij x_hat_j is only valid for a fixed W: the graph is never refreshed
         if c.setdefault("update_graph", False):
             raise ConfigError(f"{path}.update_graph: choco_sgd needs a fixed graph (its sum of the neighbors' estimates "
@@ -113,8 +126,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
     if alg == "beer":
         if not 0.0 < float(c["gamma"]) <= 1.0:
             raise ConfigError(f"{path}.gamma must be in (0, 1] (got {c['gamma']!r})")
-        if c["compressor"] not in CHOCO_COMPRESSORS:
-            raise ConfigError(f"{path}.compressor must be one of {'|'.join(CHOCO_COMPRESSORS)} (got {c['compressor']!r})")
+        _check_compressor(c, path)
         # s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a fixed W: the graph is never refreshed
         if c.setdefault("update_graph", False):
             raise ConfigError(f"{path}.update_graph: beer needs a fixed graph (its sums of the neighbors' estimates "

@@ -5,6 +5,7 @@ round, bytes published per row and pulled per round, and final accuracy.
                                  [--accuracy-rounds 2000] [--accuracy-dtypes fp32]
                                  [--sweep 0.1,0.3,0.5,0.8,1.0] [--sweep-rounds 500] [--gamma-from-sweep]
                                  [--data-source auto|mnist|synthetic|synthetic_hard] [--out FILE.json]
+                                 [--topk 0.01,0.05] [--step-launches 2000]
 
 The problems are those of ``experiments/dist_mnist_beer.yaml`` (a 10-node cycle, the heterogeneous class split,
 MNISTConvNet(3, 5, 64), batch 64, on the fused sm_90a kernels), with ``choco_sign`` added at CHOCO int8's gamma and
@@ -18,7 +19,12 @@ and is not tuned.
   * ``--sweep``: the compressed CHOCO and BEER runs of ``--sweep-rounds`` rounds at each gamma (fp32), mean top-1 at the
     end; with ``--gamma-from-sweep`` the accuracy runs take each of them at its best swept gamma (the first of a tie);
   * accuracy: one run of ``--accuracy-rounds`` rounds per configuration and dtype; the mean over nodes of the top-1
-    accuracy at the last evaluation.
+    accuracy at the last evaluation;
+  * ``--topk``: ``choco_topk<ratio>`` and ``beer_topk<ratio>`` configurations per ratio (the int8 problems with
+    compressor topk), measured, swept and run with the others; ``--step-launches``: the step kernels alone, int8
+    against each top-k ratio, timed with CUDA events over that many back-to-back launches replayed from one CUDA graph
+    (ms per launch, per dtype).
+Without ``--topk`` the output is that of the six configurations above.
 The card's name and power limit are printed in the same run.  Prints one JSON line (and writes it to ``--out``).
 """
 from __future__ import annotations
@@ -37,6 +43,7 @@ sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "scripts"))
 
 from bench_algorithms import card  # noqa: E402
+from bench_compression import step_kernel_times  # noqa: E402
 from nn_distributed_training_b200.data.mnist import load_mnist  # noqa: E402
 from nn_distributed_training_b200.experiments.dist_mnist_ex import split_hetero  # noqa: E402
 from nn_distributed_training_b200.models import MNISTConvNet  # noqa: E402
@@ -63,6 +70,8 @@ def main(argv=None):
     ap.add_argument("--data-dir", default=os.path.join(ROOT, "..", "data"))
     ap.add_argument("--data-source", default="auto", choices=["auto", "mnist", "synthetic", "synthetic_hard"])
     ap.add_argument("--out", default=None)
+    ap.add_argument("--topk", default="")
+    ap.add_argument("--step-launches", type=int, default=0)
     args = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("bench_beer.py measures the fused kernels and needs a CUDA device")
@@ -88,6 +97,13 @@ def main(argv=None):
     problems["beer_none"]["optimizer_config"]["gamma"] = 1.0
     names = ["dsgt", "choco_int8", "choco_sign", "beer_none", "beer_int8", "beer_sign"]
     swept = ["choco_int8", "choco_sign", "beer_int8", "beer_sign"]
+    for r in [float(x) for x in args.topk.split(",") if x]:
+        for alg in ("choco", "beer"):
+            name = f"{alg}_topk{r:g}"
+            problems[name] = copy.deepcopy(problems[f"{alg}_int8"])
+            problems[name]["optimizer_config"].update(compressor="topk", topk_ratio=r)
+            names.append(name)
+            swept.append(name)
     gammas = {}
 
     def build(name, dtype, rounds, eval_every, gamma=None):
@@ -132,6 +148,16 @@ def main(argv=None):
         print(f"{dname}: ms/round " + "  ".join(f"{a} {med[a]:.4f}" for a in names) + f"   (all {times})", flush=True)
         print(f"{dname}: bytes (row / pulled per round) "
               + "  ".join(f"{a} {b['row']}/{b['pulled']}" for a, b in record["bytes"][dname].items()), flush=True)
+
+    if args.step_launches > 0:
+        dts = [d for d in args.dtypes.split(",") if d]
+        kernels = {}
+        for alg, step_of in (("choco", lambda op: op.choco_step), ("beer", lambda op: op.beer_step)):
+            for d, v in step_kernel_times(build, [n for n in names if n.startswith(alg + "_")
+                                                  and n.split("_")[1] not in ("none", "sign")],
+                                          dts, args.step_launches, step_of).items():
+                kernels.setdefault(d, {}).update(v)
+        record["step_kernel_ms"] = kernels
 
     for g in [float(x) for x in args.sweep.split(",") if x]:
         for name in swept:

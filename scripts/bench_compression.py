@@ -5,6 +5,7 @@ per row and pulled per round, and final accuracy.
                                         [--accuracy-rounds 2000] [--accuracy-dtypes fp32]
                                         [--sweep 0.1,0.3,0.5,0.8,1.0] [--sweep-rounds 500]
                                         [--data-source auto|mnist|synthetic|synthetic_hard] [--out FILE.json]
+                                        [--topk 0.01,0.05] [--step-launches 2000]
 
 The problems are those of ``experiments/dist_mnist_choco.yaml`` (a 10-node cycle, the heterogeneous class split,
 MNISTConvNet(3, 5, 64), batch 64, on the fused sm_90a kernels), with ``choco_none`` added at the int8 problem's gamma.
@@ -14,7 +15,11 @@ MNISTConvNet(3, 5, 64), batch 64, on the fused sm_90a kernels), with ``choco_non
   * bytes: one published row per node and everything this process's nodes pull per round, from the engine;
   * accuracy: one run of ``--accuracy-rounds`` rounds per configuration and dtype; the mean over nodes of the top-1
     accuracy at the last evaluation;
-  * ``--sweep``: the int8 and sign runs of ``--sweep-rounds`` rounds at each gamma (fp32), mean top-1 at the end.
+  * ``--sweep``: the int8 and sign runs of ``--sweep-rounds`` rounds at each gamma (fp32), mean top-1 at the end;
+  * ``--topk``: a ``choco_topk<ratio>`` configuration per ratio (the int8 problem with compressor topk), measured with
+    the others; ``--step-launches``: the step kernel alone, int8 against each top-k ratio, timed with CUDA events over
+    that many back-to-back launches replayed from one CUDA graph (ms per launch, per dtype).
+Without ``--topk`` the output is that of the four configurations above.
 The card's name and power limit are printed in the same run.  Prints one JSON line (and writes it to ``--out``).
 """
 from __future__ import annotations
@@ -58,6 +63,8 @@ def main(argv=None):
     ap.add_argument("--data-dir", default=os.path.join(ROOT, "..", "data"))
     ap.add_argument("--data-source", default="auto", choices=["auto", "mnist", "synthetic", "synthetic_hard"])
     ap.add_argument("--out", default=None)
+    ap.add_argument("--topk", default="")
+    ap.add_argument("--step-launches", type=int, default=0)
     args = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("bench_compression.py measures the fused kernels and needs a CUDA device")
@@ -79,6 +86,10 @@ def main(argv=None):
     problems["choco_none"] = copy.deepcopy(problems["choco_int8"])
     problems["choco_none"]["optimizer_config"]["compressor"] = "none"
     names = ["dsgd", "choco_none", "choco_int8", "choco_sign"]
+    for r in [float(x) for x in args.topk.split(",") if x]:
+        problems[f"choco_topk{r:g}"] = copy.deepcopy(problems["choco_int8"])
+        problems[f"choco_topk{r:g}"]["optimizer_config"].update(compressor="topk", topk_ratio=r)
+        names.append(f"choco_topk{r:g}")
 
     def build(name, dtype, rounds, eval_every, gamma=None):
         pc = copy.deepcopy(problems[name])
@@ -123,6 +134,12 @@ def main(argv=None):
         print(f"{dname}: bytes (row / pulled per round) "
               + "  ".join(f"{a} {b['row']}/{b['pulled']}" for a, b in record["bytes"][dname].items()), flush=True)
 
+    if args.step_launches > 0:
+        record["step_kernel_ms"] = step_kernel_times(build, [n for n in names if n.startswith("choco_")
+                                                            and n.split("_")[1] not in ("none", "sign")],
+                                                     [d for d in args.dtypes.split(",") if d], args.step_launches,
+                                                     lambda op: op.choco_step)
+
     for g in [float(x) for x in args.sweep.split(",") if x]:
         for name in ("choco_int8", "choco_sign"):
             pr, opt = build(name, torch.float32, args.sweep_rounds, args.sweep_rounds, gamma=g)
@@ -148,6 +165,40 @@ def main(argv=None):
     if args.out:
         with open(args.out, "w") as f:
             f.write(line + "\n")
+
+
+def step_kernel_times(build, names, dtypes, launches, step_of):
+    """The step kernel alone: ``launches`` back-to-back launches of it captured in one CUDA graph (each launch advances
+    the round counter, so the problem's schedule covers two replays), the second replay timed with CUDA events; ms per
+    launch per dtype and name."""
+    out = {}
+    for dname in dtypes:
+        for name in names:
+            pr, opt = build(name, DTYPES[dname], 2 * launches + 2, 10 ** 9)
+            opt.run_rounds(1)
+            torch.cuda.synchronize()
+            step = step_of(opt._program.eng.op)
+            graph, stream = torch.cuda.CUDAGraph(), torch.cuda.Stream()
+            with torch.cuda.stream(stream):
+                step()                                   # once outside the capture: first-launch set-up
+                torch.cuda.synchronize()
+                with torch.cuda.graph(graph, stream=stream):
+                    for _ in range(launches):
+                        step()
+            graph.replay()
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            torch.cuda.synchronize()
+            t0.record()
+            graph.replay()
+            t1.record()
+            torch.cuda.synchronize()
+            opt._program.eng.check()
+            ms = round(t0.elapsed_time(t1) / launches, 5)
+            out.setdefault(dname, {})[name] = ms
+            print(f"{dname} {name}: step kernel {ms * 1000:.2f} us per launch ({launches} launches in one graph)",
+                  flush=True)
+            del graph, pr, opt
+    return out
 
 
 if __name__ == "__main__":
