@@ -362,6 +362,46 @@ def kgt_step_(theta: torch.Tensor, c: Optional[torch.Tensor], d: Optional[torch.
     return d / K if p == K - 1 else None
 
 
+# ------------------------------------------------- decentralized adaptive ----
+DADAPTIVE_VARIANTS = ("amsgrad", "adagrad")
+
+
+def dadaptive_mix_(theta: torch.Tensor, ut: Optional[torch.Tensor], theta_all: torch.Tensor,
+                   ut_all: Optional[torch.Tensor], w_rows: torch.Tensor):
+    """``x_i = sum_j W_ij theta_j`` into ``theta``; with tracking also ``z_i = sum_j W_ij u~_j`` into ``ut`` (the row
+    holds z until the step turns it into the new tracker).  Without tracking this is DSGD's mix."""
+    theta.copy_(dsgd_mix(theta_all, w_rows))
+    if ut is not None:
+        ut.copy_(dsgd_mix(ut_all, w_rows))
+
+
+def dadaptive_step_(theta: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tensor], vhat: torch.Tensor,
+                    ut: Optional[torch.Tensor], grad: torch.Tensor, alpha: float, beta1: float, beta2: float,
+                    eps: float, k: int, adagrad: bool):
+    """The adaptive step of round ``k`` on the mixed rows ``x = theta`` (``ut`` holds z of the mix, or is ``None``
+    without tracking):
+
+        m <- beta1 m + (1 - beta1) g
+        amsgrad:  v <- beta2 v + (1 - beta2) g^2;  vhat' = max(vhat, v)
+        adagrad:  vhat' = vhat + (g^2 - vhat) / (k + 1)
+        tracking: u~ <- z + (vhat' - vhat);  u = max(u~, eps)      own: u = max(vhat', eps)
+        vhat <- vhat';  theta <- x - alpha m / sqrt(u)"""
+    m.mul_(beta1).add_(grad, alpha=1.0 - beta1)
+    g2 = grad * grad
+    if adagrad:
+        vn = vhat + (g2 - vhat) / float(k + 1)
+    else:
+        v.mul_(beta2).add_(g2, alpha=1.0 - beta2)
+        vn = torch.maximum(vhat, v)
+    if ut is not None:
+        ut.add_(vn - vhat)
+        u = ut.clamp_min(eps)
+    else:
+        u = vn.clamp_min(eps)
+    vhat.copy_(vn)
+    theta.sub_(alpha * (m / u.sqrt()))
+
+
 # ---------------------------------------------------------- ClippedGossip ----
 ATTACK_CODE = {"sign_flip": 1, "alie": 2}      # consensus.h: Attack (0 = honest)
 CLIP_SLACK = 1e-6      # consensus.h: kClipSlack, a prefix of (rounded) weights fits in delta up to this

@@ -125,13 +125,14 @@ struct ConsensusOp {
   consensus::ChocoArgs<T> ch{};
   consensus::BeerArgs<T> be{};
   consensus::KgtArgs<T> kg{};
+  consensus::DAdaptiveArgs<T> ad{};
   consensus::ClipArgs<T> cg{};
   int cg_adaptive = 0;
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; cg.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; cg.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -149,6 +150,9 @@ struct ConsensusOp {
     be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride; be.topk_k = ch.topk_k;
     kg.corr = ptr<T>(d, "corr"); kg.dacc = ptr<T>(d, "dacc");
     kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
+    ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
+    ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
+    ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
     cg.dist_part = ptr<double>(d, "dist_part"); cg.pstride = geti(d, "pstride", 0);
     cg.attack = ptr<const int>(d, "attack"); cg.nbr_byz = ptr<const int>(d, "nbr_byz");
     cg.delta = getf(d, "clip_delta", 0.0); cg.scale = getf(d, "attack_scale", 1.0); cg.z = getf(d, "attack_z", 1.0);
@@ -217,6 +221,19 @@ struct ConsensusOp {
       throw std::runtime_error("kgt_step with correction needs the K-GT rows `corr`, `dacc` and two published channels");
     kg.step = step;
     check(consensus::launch_kgt_step<T>(kg, cur_stream()), "kgt_step");
+  }
+  void dadaptive_mix() {
+    if (!ad.tracking || ad.ut == nullptr || c.C != 2)
+      throw std::runtime_error("dadaptive_mix needs tracking, the tracker row `ut` and two published channels (the "
+                               "own-second-moment variant mixes with dsgd_mix)");
+    check(consensus::launch_dadaptive_mix<T>(ad, cur_stream()), "dadaptive_mix");
+  }
+  void dadaptive_step() {
+    if (ad.m == nullptr || ad.vhat == nullptr || (!ad.adagrad && ad.v == nullptr) ||
+        (ad.tracking && (ad.ut == nullptr || c.C != 2)) || (!ad.tracking && c.C != 1))
+      throw std::runtime_error("dadaptive_step needs the rows `ad_m`, `vhat`, `ad_v` (amsgrad) and, with tracking, `ut` "
+                               "and two published channels (one without)");
+    check(consensus::launch_dadaptive_step<T>(ad, cur_stream()), "dadaptive_step");
   }
   void cg_check(const char* what, bool clip) const {
     if (c.C != 1 || c.sum_mode)
@@ -303,6 +320,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("beer_step", &ConsensusOp<T>::beer_step)
       .def("kgt_mix", &ConsensusOp<T>::kgt_mix)
       .def("kgt_step", &ConsensusOp<T>::kgt_step)
+      .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
+      .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("cg_dist", &ConsensusOp<T>::cg_dist)
       .def("cg_mix", &ConsensusOp<T>::cg_mix)
       .def("cg_step", &ConsensusOp<T>::cg_step)

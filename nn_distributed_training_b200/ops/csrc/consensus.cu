@@ -12,6 +12,8 @@
 // BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
 //                                                          (top-k codes)   -> beer_topk_mix / beer_topk_step
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
+// decentralized AMSGrad / AdaGrad (no reference counterpart,
+//                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
@@ -1173,6 +1175,135 @@ __global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 2) kgt_step_kernel(const
   end_step(c, l, ri.k, last);
 }
 
+// ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
+// Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
+// dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
+// z_i = sum_j W_ij u~_j into ut (own terms included: the own u~ is the node's published row, since ut holds z); then
+// fwd/bwd and dadaptive_step.  Without tracking the mix is dsgd_mix_kernel.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) dadaptive_mix_kernel(const DAdaptiveArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const T* us = pub_row(c, ri.par, 1, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th, z;
+    if (c.sum_mode) {     // W = 11^T / N: x_i = S_theta / N, z_i = S_u~ / N
+      const DPack<N> st = network_sum(c, ri.par, 0, i);
+      const DPack<N> su = network_sum(c, ri.par, 1, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        th.v[u] = (T)(st.v[u] / (double)c.n_total);
+        z.v[u] = (T)(su.v[u] / (double)c.n_total);
+      }
+      stv(c.theta + row + i, th);
+      stv(a.ut + row + i, z);
+      continue;
+    }
+    th = ldv(c.theta + row + i);
+    z = ldv(us + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      th.v[u] *= ws;
+      z.v[u] *= ws;
+    }
+    // for_neighbors<2> written out, as in dsgt_mix: two channels of two neighbors in flight
+    for (int e0 = 0; e0 < deg; e0 += 2) {
+      Pack<T> qt[2], qu[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          qt[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
+          qu[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 1) + i);
+        }
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          const T we = w[e0 + j];
+#pragma unroll
+          for (int u = 0; u < N; ++u) {
+            th.v[u] += we * qt[j].v[u];
+            z.v[u] += we * qu[j].v[u];
+          }
+        }
+    }
+    stv(c.theta + row + i, th);
+    stv(a.ut + row + i, z);
+  }
+}
+
+// The step on the mixed row x (theta after the mix), with alpha_k from the schedule:
+//   m <- beta1 m + (1 - beta1) g
+//   amsgrad (!ADAGRAD):  v <- beta2 v + (1 - beta2) g^2;  vhat' = max(vhat, v)
+//   adagrad:             vhat' = vhat + (g^2 - vhat) / (k + 1)        (k from the round counter: right after a resume)
+//   TRACK:  u~ = z + (vhat' - vhat), u = max(u~, eps);   otherwise u = max(vhat', eps)
+//   theta <- x - alpha_k m / sqrt(u);  m, v and vhat' are stored, theta (and u~) published into the next parity.
+// u~ is not stored: the next mix reads the node's own published row.  The square root and the quotients are correctly
+// rounded (sqrt_rn / div_rn), so the fp32 step carries a few units of round-off, not the approximations of
+// --use_fast_math.  The 4-deep variant is held to 80 registers (3 CTAs per SM) and the 8-deep one to 128, with no
+// spills: at kgt_step's 64 the fp64 steps and the fp32 tracked AMSGrad step spilled around the IEEE slow paths.
+template <typename T, int U, bool ADAGRAD, bool TRACK>
+__global__ void __launch_bounds__(THREADS, U <= 4 ? 3 : 2) dadaptive_step_kernel(const DAdaptiveArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const T b1 = a.beta1, b1c = (T)1 - a.beta1, b2 = a.beta2, b2c = (T)1 - a.beta2, eps = a.eps;
+  const T cnt = (T)(ri.k + 1);
+  const size_t row = (size_t)l * c.n_pad;
+  // theta and z (written by the mix two launches back) and m, v, vhat (the previous round's step) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    Pack<T> m = ldv(a.m + row + i);
+    Pack<T> vh = ldv(a.vhat + row + i);
+    Pack<T> v, z;
+    if (!ADAGRAD) v = ldv(a.v + row + i);
+    if (TRACK) z = ldv(a.ut + row + i);
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      m.v[u] = b1 * m.v[u] + b1c * g.v[u];
+      const T g2 = g.v[u] * g.v[u];
+      T vn;
+      if (ADAGRAD) {
+        vn = vh.v[u] + div_rn(g2 - vh.v[u], cnt);
+      } else {
+        v.v[u] = b2 * v.v[u] + b2c * g2;
+        vn = v.v[u] > vh.v[u] ? v.v[u] : vh.v[u];
+      }
+      T uu;
+      if (TRACK) {
+        z.v[u] += vn - vh.v[u];             // u~
+        uu = z.v[u] > eps ? z.v[u] : eps;
+      } else {
+        uu = vn > eps ? vn : eps;
+      }
+      vh.v[u] = vn;
+      th.v[u] -= alpha * div_rn(m.v[u], sqrt_rn(uu));
+    }
+    stv(a.m + row + i, m);
+    if (!ADAGRAD) stv(a.v + row + i, v);
+    stv(a.vhat + row + i, vh);
+    stv(c.theta + row + i, th);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+    if (TRACK) stv(pub_row(c, ri.par ^ 1, 1, l) + i, z);
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
 // ----------------------------------------------------------- ClippedGossip ----
 // Round k (layout and rules in consensus.h): cg_dist, cg_mix, fwd/bwd, cg_step; with `clip: none` dsgd_mix replaces
 // the first two.  A clipped edge needs its distance over the whole row before any element is mixed, and the row is
@@ -1755,6 +1886,20 @@ template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStrea
   return a.correction ? launch_kgt<T, true>(a, st) : launch_kgt<T, false>(a, st);
 }
 
+template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
+}
+// the variant and the tracking are template parameters (see dsgt_mix above); beyond 4 gradient partials the step keeps
+// 8 loads in flight, as kgt_step
+template <typename T, bool ADAGRAD, bool TRACK>
+static cudaError_t launch_dadaptive(const DAdaptiveArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(dadaptive_step_kernel<T, 4, ADAGRAD, TRACK>, dadaptive_step_kernel<T, 8, ADAGRAD, TRACK>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st) {
+  if (a.adagrad) return a.tracking ? launch_dadaptive<T, true, true>(a, st) : launch_dadaptive<T, true, false>(a, st);
+  return a.tracking ? launch_dadaptive<T, false, true>(a, st) : launch_dadaptive<T, false, false>(a, st);
+}
+
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st) {
   if (cg_chunks(a.c) > a.pstride) return cudaErrorInvalidValue;
   return launch_one_wave(cg_dist_kernel<T>, a.c, a, st);
@@ -1806,6 +1951,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_beer_step<T>(const BeerArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_kgt_mix<T>(const KgtArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
+  template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_cg_dist<T>(const ClipArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_cg_mix<T>(const ClipArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_cg_step<T>(const ClipArgs<T>&, cudaStream_t);           \

@@ -174,6 +174,21 @@ struct KgtArgs {
   int step, K, correction;
 };
 
+// Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
+// channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
+// z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
+// tracking one channel and dsgd_mix_kernel; the step divides by the node's own vhat.
+template <typename T>
+struct DAdaptiveArgs {
+  Common<T> c;
+  T* m;                            // [L, n_pad] first moment, zero at the start
+  T* v;                            // [L, n_pad] amsgrad: second moment, zero at the start; nullptr with adagrad
+  T* vhat;                         // [L, n_pad] amsgrad: max of v; adagrad: running mean of g^2.  eps at the start
+  T* ut;                           // [L, n_pad] tracking: z of the round's mix (read by the step); nullptr = own vhat
+  T beta1, beta2, eps;
+  int adagrad, tracking;
+};
+
 // ClippedGossip (He, Karimireddy, Jaggi 2022): DSGD's single published channel with a self-centred clipped mix, and
 // Byzantine nodes that publish an attack row instead of theta.  Round k: cg_dist reduces the squared
 // distances |theta_j^pub - theta_i|^2 of every neighbor, one partial per fixed chunk of the row, into dist_part; cg_mix
@@ -255,6 +270,8 @@ template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st);

@@ -338,6 +338,9 @@ NNDT_DEVINL float mul_rn(float x, float y) { return __fmul_rn(x, y); }
 NNDT_DEVINL double mul_rn(double x, double y) { return __dmul_rn(x, y); }
 NNDT_DEVINL float div_rn(float x, float y) { return __fdiv_rn(x, y); }
 NNDT_DEVINL double div_rn(double x, double y) { return __ddiv_rn(x, y); }
+// correctly rounded square root (a plain sqrtf is an approximation under --use_fast_math)
+NNDT_DEVINL float sqrt_rn(float x) { return __fsqrt_rn(x); }
+NNDT_DEVINL double sqrt_rn(double x) { return __dsqrt_rn(x); }
 
 template <typename T>
 NNDT_DEVINL char* code_row(const ChocoArgs<T>& a, int par, int l) {

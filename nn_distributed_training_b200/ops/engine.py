@@ -40,7 +40,7 @@ def schedule_tables(opt, H: int):
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing and K-GT: a constant step
+    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT and dadaptive: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -101,9 +101,11 @@ class ConsensusEngine:
         dev, a, pl, ctx = pr.device, pr.arena, pr.placement, pr.ctx
         self.dtype = a.dtype
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
-        # K-GT publishes its tracker y in channel 1; local DSGD (kgt without correction) publishes theta only
+        # K-GT publishes its tracker y in channel 1; local DSGD (kgt without correction) publishes theta only.  So does
+        # dadaptive with its second-moment tracker u~ (tracking) or without it
         kgt_corr = opt.alg_name == "kgt" and opt.correction
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") or kgt_corr else 1
+        ad_track = opt.alg_name == "dadaptive" and opt.tracking
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") or kgt_corr or ad_track else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
@@ -147,6 +149,8 @@ class ConsensusEngine:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
             self.pub[k0 & 1, 1, :L].copy_(opt.y)
+        if ad_track:
+            self.pub[k0 & 1, 1, :L].copy_(opt.ut)
 
         # ---- schedules ----------------------------------------------------------
         H = self.horizon = schedule_horizon(opt)
@@ -355,6 +359,10 @@ class ConsensusEngine:
         if opt.alg_name == "kgt":
             d.update(local_steps=opt.local_steps, correction=int(opt.correction),
                      corr=opt.c.data_ptr() if kgt_corr else None, dacc=opt.d.data_ptr() if kgt_corr else None)
+        if opt.alg_name == "dadaptive":
+            d.update(ad_m=opt.m.data_ptr(), ad_v=None if opt.v is None else opt.v.data_ptr(),
+                     vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if ad_track else None, beta1=opt.beta1,
+                     beta2=opt.beta2, ad_eps=opt.eps, adagrad=int(opt.adagrad), tracking=int(ad_track))
         self.dist_part = self.t_attack = self.t_nbr_byz = None
         if self.cg:
             if opt.clip == "adaptive":
@@ -409,7 +417,7 @@ class ConsensusEngine:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
         neighbors per round (``pulled``: one published row per neighbor edge of the first graph; the own row is not
         counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
-        steps.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
+        steps.  dadaptive with tracking publishes two rows (theta and u~), without it one.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
         for the mix (``clip: none`` once, as DSGD; an ALIE attacker also reads its honest neighbors' rows, not
         counted)."""
         deg = int(self.t_deg[0].sum().item())

@@ -12,6 +12,7 @@ A round is a short, fixed kernel sequence
     Push-DIGing:  pdg_mix, fwd/bwd, pdg_track
     K-GT:  kgt_mix, [fwd/bwd, kgt_step(p)] x local_steps       (local DSGD: dsgd_mix in place of kgt_mix)
     ClippedGossip:  cg_dist, cg_mix, fwd/bwd, cg_step           (clip: none: dsgd_mix, fwd/bwd, cg_step)
+    decentralized AMSGrad / AdaGrad:  dadaptive_mix, fwd/bwd, dadaptive_step     (own second moment: dsgd_mix first)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -92,6 +93,13 @@ def _round_ops_impl(opt, eng, grads):
             eng.op.dsgd_mix()
         grads(0)
         eng.op.cg_step()
+    elif alg == "dadaptive":
+        if opt.tracking:
+            eng.op.dadaptive_mix()
+        else:
+            eng.op.dsgd_mix()
+        grads(0)
+        eng.op.dadaptive_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -313,6 +321,8 @@ class RoundProgram:
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name == "kgt" and opt.correction:      # c is the optimizer's own row; d is dead between rounds
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L])
+        if opt.alg_name == "dadaptive" and opt.tracking:  # the fused ut row holds the mix's z; u~ is the published row
+            opt.ut.copy_(eng.pub[opt.k & 1, 1, :L])
         if opt.alg_name == "push_diging":       # y is the first n_pad elements of channel 1 (u and w are shared)
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:

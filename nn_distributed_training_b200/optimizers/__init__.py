@@ -1,6 +1,7 @@
 from .beer import BEER
 from .clipped_gossip import ClippedGossip
 from .choco import ChocoSGD
+from .dadaptive import DAdaptive
 from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgdm import DSGDm
@@ -12,7 +13,7 @@ from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
-              "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip}
+              "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -13,12 +13,14 @@ from typing import Any, Dict, Iterable, Optional
 
 import yaml
 
-from ..ops.consensus_ref import CHOCO_COMPRESSORS, TOPK_RATIO_DEFAULT
+import math
+
+from ..ops.consensus_ref import CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, TOPK_RATIO_DEFAULT
 
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip")
+        "clipped_gossip", "dadaptive")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -47,7 +49,11 @@ OPT_SCHEMA = {
             "profile": False, "update_graph": True},
     "clipped_gossip": {"alpha0": REQUIRED, "mu": 0.0, "clip": REQUIRED, "outer_iterations": REQUIRED, "profile": False,
                        "update_graph": True},
+    # beta2 (default DADAPTIVE_BETA2) is filled in for variant amsgrad only
+    "dadaptive": {"alpha": REQUIRED, "variant": REQUIRED, "tracking": True, "beta1": 0.9, "eps": 1e-8,
+                  "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
 }
+DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
 OPT_EXTRA = ("mixing_order", "update_graph", "consensus_backend", "persistent_follows_schedule",
              "checkpoint_every", "checkpoint_dir", "resume")
@@ -68,6 +74,31 @@ def _check_compressor(c: Dict[str, Any], path: str) -> None:
     r = c.setdefault("topk_ratio", TOPK_RATIO_DEFAULT)
     if isinstance(r, bool) or not isinstance(r, (int, float)) or not 0.0 < float(r) <= 1.0:
         raise ConfigError(f"{path}.topk_ratio must be in (0, 1] (got {r!r})")
+
+
+def _real(x) -> bool:
+    return not isinstance(x, bool) and isinstance(x, (int, float))
+
+
+def _check_dadaptive(c: Dict[str, Any], path: str) -> None:
+    """Decentralized AMSGrad / AdaGrad: the variant, the tracking switch, the moment coefficients (``beta2`` with
+    amsgrad only, default ``DADAPTIVE_BETA2``), ``eps`` and the step."""
+    if c["variant"] not in DADAPTIVE_VARIANTS:
+        raise ConfigError(f"{path}.variant must be one of {'|'.join(DADAPTIVE_VARIANTS)} (got {c['variant']!r})")
+    if not isinstance(c["tracking"], bool):
+        raise ConfigError(f"{path}.tracking must be true or false (got {c['tracking']!r})")
+    if c["variant"] == "adagrad":
+        if "beta2" in c:
+            raise ConfigError(f"{path}.beta2 applies to variant amsgrad only (variant is 'adagrad')")
+    else:
+        c.setdefault("beta2", DADAPTIVE_BETA2)
+    for key in ("beta1", "beta2"):
+        if key in c and (not _real(c[key]) or not 0.0 <= float(c[key]) < 1.0):
+            raise ConfigError(f"{path}.{key} must be in [0, 1) (got {c[key]!r})")
+    if not _real(c["eps"]) or not (math.isfinite(float(c["eps"])) and float(c["eps"]) > 0.0):
+        raise ConfigError(f"{path}.eps must be finite and > 0 (got {c['eps']!r})")
+    if not _real(c["alpha"]) or not float(c["alpha"]) > 0.0:
+        raise ConfigError(f"{path}.alpha must be > 0 (got {c['alpha']!r})")
 
 
 def _fill(d: Dict[str, Any], schema: Dict[str, Any], path: str, extra: Iterable[str] = ()) -> Dict[str, Any]:
@@ -106,7 +137,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
     if "byzantine" in c and alg != "clipped_gossip":
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only "
                           f"(alg_name is {alg!r})")
-    if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip")
+    if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
+                "dadaptive")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -139,6 +171,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.alpha must be > 0 (got {c['alpha']!r})")
         if not isinstance(c["correction"], bool):
             raise ConfigError(f"{path}.correction must be true or false (got {c['correction']!r})")
+    if alg == "dadaptive":
+        _check_dadaptive(c, path)
     if alg == "clipped_gossip":
         if c["clip"] not in ("none", "adaptive"):
             raise ConfigError(f"{path}.clip must be one of none|adaptive (got {c['clip']!r})")
