@@ -11,7 +11,7 @@ optimizers/dsgd.py:34-58, optimizers/dsgt.py:33-103.
 from __future__ import annotations
 
 import math
-from typing import Optional, Tuple
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -400,6 +400,35 @@ def dadaptive_step_(theta: torch.Tensor, m: torch.Tensor, v: Optional[torch.Tens
         u = vn.clamp_min(eps)
     vhat.copy_(vn)
     theta.sub_(alpha * (m / u.sqrt()))
+
+
+# --------------------------------------------------------------- RelaySum ----
+def relaysum_mix_(theta: torch.Tensor, msg_all: List[torch.Tensor], src_node: torch.Tensor, src_slot: torch.Tensor,
+                  live: torch.Tensor, reach_m1: torch.Tensor, n: int) -> torch.Tensor:
+    """The mix of round k for the local rows ``theta`` (holding h): ``r_e = m_{j_e -> i}``, gathered from
+    ``msg_all[s]`` (every node's published message slot s, ``[N, n_pad]``) at ``[src_slot, src_node]`` (``[L, dmax]``,
+    the neighbor j_e and its reverse slot; ``live`` marks e < deg_i), then ``x = h + (sum_e r_e - (R_i^k - 1) h) / n``
+    with e ascending (``reach_m1``: ``[L]``).  Returns ``r`` (``[L, dmax, n_pad]``, zero past deg_i) for the step."""
+    r = torch.stack(msg_all)[src_slot, src_node]
+    r = torch.where(live[:, :, None], r, torch.zeros((), dtype=r.dtype))
+    s = torch.zeros_like(theta)
+    for e in range(r.shape[1]):
+        s = s + r[:, e]
+    theta.copy_(theta + (s - reach_m1[:, None] * theta) / n)
+    return r
+
+
+def relaysum_step_(theta: torch.Tensor, msg: torch.Tensor, r: torch.Tensor, live: torch.Tensor, grad: torch.Tensor,
+                   alpha: float):
+    """``h = x - alpha g`` into ``theta``, and the messages ``m_{i -> j_e} = h + sum_{e' != e} r_e'`` (e' ascending)
+    into ``msg[:, e]`` (``[L, dmax, n_pad]``; zero past deg_i)."""
+    theta.add_(grad, alpha=-alpha)
+    for e in range(msg.shape[1]):
+        m = theta.clone()
+        for f in range(r.shape[1]):
+            if f != e:
+                m = m + r[:, f]
+        msg[:, e] = torch.where(live[:, e, None], m, torch.zeros((), dtype=m.dtype))
 
 
 # ---------------------------------------------------------- ClippedGossip ----

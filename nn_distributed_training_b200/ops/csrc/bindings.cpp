@@ -126,13 +126,14 @@ struct ConsensusOp {
   consensus::BeerArgs<T> be{};
   consensus::KgtArgs<T> kg{};
   consensus::DAdaptiveArgs<T> ad{};
+  consensus::RelayArgs<T> rs{};
   consensus::ClipArgs<T> cg{};
   int cg_adaptive = 0;
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; cg.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; sg.c = c; pd.c = c;
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -153,6 +154,8 @@ struct ConsensusOp {
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
+    rs.reach = ptr<const T>(d, "reach"); rs.rin = ptr<T>(d, "rin"); rs.diam = geti(d, "diam", 0);
+    rs.n = (T)geti(d, "relay_n", 0);
     cg.dist_part = ptr<double>(d, "dist_part"); cg.pstride = geti(d, "pstride", 0);
     cg.attack = ptr<const int>(d, "attack"); cg.nbr_byz = ptr<const int>(d, "nbr_byz");
     cg.delta = getf(d, "clip_delta", 0.0); cg.scale = getf(d, "attack_scale", 1.0); cg.z = getf(d, "attack_z", 1.0);
@@ -234,6 +237,20 @@ struct ConsensusOp {
       throw std::runtime_error("dadaptive_step needs the rows `ad_m`, `vhat`, `ad_v` (amsgrad) and, with tracking, `ut` "
                                "and two published channels (one without)");
     check(consensus::launch_dadaptive_step<T>(ad, cur_stream()), "dadaptive_step");
+  }
+  void relay_check(const char* what) const {
+    if (rs.reach == nullptr || rs.rin == nullptr || rs.n < (T)1 || rs.diam < 0 || c.sum_mode || c.C != c.dmax)
+      throw std::runtime_error(std::string(what) + " needs the reach table `reach`, the received rows `rin`, the node "
+                               "count `relay_n`, the pointer-table neighbors and one published channel per neighbor "
+                               "slot (C = dmax)");
+  }
+  void relay_mix() {
+    relay_check("relay_mix");
+    check(consensus::launch_relay_mix<T>(rs, cur_stream()), "relay_mix");
+  }
+  void relay_step() {
+    relay_check("relay_step");
+    check(consensus::launch_relay_step<T>(rs, cur_stream()), "relay_step");
   }
   void cg_check(const char* what, bool clip) const {
     if (c.C != 1 || c.sum_mode)
@@ -322,6 +339,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("kgt_step", &ConsensusOp<T>::kgt_step)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
+      .def("relay_mix", &ConsensusOp<T>::relay_mix)
+      .def("relay_step", &ConsensusOp<T>::relay_step)
       .def("cg_dist", &ConsensusOp<T>::cg_dist)
       .def("cg_mix", &ConsensusOp<T>::cg_mix)
       .def("cg_step", &ConsensusOp<T>::cg_step)

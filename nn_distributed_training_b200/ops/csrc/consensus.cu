@@ -14,6 +14,7 @@
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
+// RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
 // ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
@@ -1304,6 +1305,94 @@ __global__ void __launch_bounds__(THREADS, U <= 4 ? 3 : 2) dadaptive_step_kernel
   end_step(c, l, ri.k, true);
 }
 
+// ---------------------------------------------------------------- RelaySum ----
+// Layout in consensus.h.  Round k: relay_mix pulls the deg messages published for this node at the end of round k-1
+// (r_e = m_{j_e -> l}, e ascending), keeps them in rin and writes x = h + (sum_e r_e - (R_l^k - 1) h) / n into theta;
+// then fwd/bwd and relay_step.  The product and the quotient are rounded on their own (mul_rn / div_rn), as the PyTorch
+// ops round them.  Every neighbor read of the round is in this kernel.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) relay_mix_kernel(const RelayArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T rm1 = a.reach[l * (a.diam + 1) + min(ri.k, a.diam)];
+  const size_t row = (size_t)l * c.n_pad;
+  T* rin = a.rin + (size_t)l * c.dmax * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> x = ldv(c.theta + row + i), s;
+#pragma unroll
+    for (int u = 0; u < N; ++u) s.v[u] = (T)0;
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
+                       stv(rin + (size_t)e * c.n_pad + i, q);
+#pragma unroll
+                       for (int u = 0; u < N; ++u) s.v[u] += q.v[u];
+                     });
+#pragma unroll
+    for (int u = 0; u < N; ++u) x.v[u] += div_rn(s.v[u] - mul_rn(rm1, x.v[u]), a.n);
+    stv(c.theta + row + i, x);
+  }
+}
+
+// h = x - alpha_k g into theta, and for each neighbor e the message h + sum_{e' != e} r_e' (e' ascending) into channel e
+// of parity k+1.  theta and the D received rows (written by the mix two launches back) are read before the
+// programmatic-dependency wait, the gradient partials after it.  A star hub of degree deg adds deg (deg - 1) rows per
+// element.  -Xptxas -v, no spills: <T, 4, 4> is held to 80 registers (3 CTAs per SM), <T, 8, 4> and <T, 4, 16> to
+// 128 (2 CTAs).  <T, 8, 16> spilled at 128, so a node of degree above 4 sums its partials 4 deep.
+template <typename T, int U, int D>
+__global__ void __launch_bounds__(THREADS, U <= 4 && D <= 4 ? 3 : 2) relay_step_kernel(const RelayArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  const T* rin = a.rin + (size_t)l * c.dmax * c.n_pad;
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> h = ldv(c.theta + row + i);
+    Pack<T> r[D];
+    // the D received rows are prefetched with theta while the partials fit beside them (U = 4 with D = 4); otherwise
+    // they are loaded after the partials are summed, whose registers are then free
+    constexpr bool kPrefetch = U <= 4 && D <= 4;
+    if (kPrefetch) {
+#pragma unroll
+      for (int e = 0; e < D; ++e)
+        if (e < deg) r[e] = ldv(rin + (size_t)e * c.n_pad + i);
+    }
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    if (!kPrefetch) {
+#pragma unroll
+      for (int e = 0; e < D; ++e)
+        if (e < deg) r[e] = ldv(rin + (size_t)e * c.n_pad + i);
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) h.v[u] -= alpha * g.v[u];
+    stv(c.theta + row + i, h);
+#pragma unroll
+    for (int e = 0; e < D; ++e)
+      if (e < deg) {
+        Pack<T> m = h;
+#pragma unroll
+        for (int f = 0; f < D; ++f)
+          if (f < deg && f != e) {
+#pragma unroll
+            for (int u = 0; u < N; ++u) m.v[u] += r[f].v[u];
+          }
+        stv(pub_row(c, ri.par ^ 1, e, l) + i, m);
+      }
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
 // ----------------------------------------------------------- ClippedGossip ----
 // Round k (layout and rules in consensus.h): cg_dist, cg_mix, fwd/bwd, cg_step; with `clip: none` dsgd_mix replaces
 // the first two.  A clipped edge needs its distance over the whole row before any element is mixed, and the row is
@@ -1900,6 +1989,18 @@ template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& 
   return a.tracking ? launch_dadaptive<T, false, true>(a, st) : launch_dadaptive<T, false, false>(a, st);
 }
 
+template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(relay_mix_kernel<T>, a.c, a, st);
+}
+// the received rows stay in registers: 4 of them for paths and binary trees, kRelayMaxDeg up to a star hub.  With at most
+// 4 neighbors and more than 4 gradient partials the step keeps 8 loads in flight, as kgt_step; the 16-slot variant keeps
+// 4 (the summation order is the same for any depth)
+template <typename T> cudaError_t launch_relay_step(const RelayArgs<T>& a, cudaStream_t st) {
+  if (a.c.dmax > kRelayMaxDeg) return cudaErrorInvalidValue;
+  if (a.c.dmax > 4) return launch_one_wave(relay_step_kernel<T, 4, kRelayMaxDeg>, a.c, a, st);
+  return launch_by_s(relay_step_kernel<T, 4, 4>, relay_step_kernel<T, 8, 4>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st) {
   if (cg_chunks(a.c) > a.pstride) return cudaErrorInvalidValue;
   return launch_one_wave(cg_dist_kernel<T>, a.c, a, st);
@@ -1953,6 +2054,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
+  template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_relay_step<T>(const RelayArgs<T>&, cudaStream_t);       \
   template cudaError_t launch_cg_dist<T>(const ClipArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_cg_mix<T>(const ClipArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_cg_step<T>(const ClipArgs<T>&, cudaStream_t);           \

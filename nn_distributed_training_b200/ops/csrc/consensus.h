@@ -189,6 +189,23 @@ struct DAdaptiveArgs {
   int adagrad, tracking;
 };
 
+// RelaySum (Vogels et al. 2021), optimizers/relaysum.py, on a fixed tree.  The published buffer has C = dmax channels:
+// channel e of node i is its message m_{i -> j_e} for its e-th neighbor.  The pointer table's channel-0 entry of edge
+// (i, e) names neighbor j_e's channel for i (its reverse slot), so a round pulls one row per edge, as DSGD's.  relay_mix
+// keeps the deg received rows in `rin` and writes x into theta; relay_step writes h into theta and publishes the deg
+// messages h + sum_{e' != e} r_e' into the other parity.  The step holds the received rows in registers, so a node
+// has at most kRelayMaxDeg neighbors (ops/engine.py: check_relay_plan).
+constexpr int kRelayMaxDeg = 16;
+
+template <typename T>
+struct RelayArgs {
+  Common<T> c;
+  const T* reach;                  // [L, diam + 1] R_i^k - 1 (exact in T), read at min(k, diam)
+  T* rin;                          // [L, dmax, n_pad] the messages received in the round's mix
+  int diam;
+  T n;                             // nodes of the tree
+};
+
 // ClippedGossip (He, Karimireddy, Jaggi 2022): DSGD's single published channel with a self-centred clipped mix, and
 // Byzantine nodes that publish an attack row instead of theta.  Round k: cg_dist reduces the squared
 // distances |theta_j^pub - theta_i|^2 of every neighbor, one partial per fixed chunk of the row, into dist_part; cg_mix
@@ -272,6 +289,8 @@ template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream
 template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_relay_step(const RelayArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st);

@@ -38,7 +38,7 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip"):
+    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT and dadaptive: a constant step
         alpha[:] = opt.alpha
@@ -93,6 +93,20 @@ def check_topk_capacity(alg: str, n_pad: int, itemsize: int, chans: int) -> None
                          f"{need} bytes per CTA against a limit of {TOPK_ROW_SMEM})")
 
 
+RELAY_MAX_DEG = 16     # consensus.h: kRelayMaxDeg
+
+
+def check_relay_plan(topos: List[Topology], dmax: int) -> None:
+    """RelaySum relays over one fixed tree, and its step holds a node's received messages in registers, for at most
+    ``RELAY_MAX_DEG`` neighbors."""
+    if len(topos) > 1:
+        raise ValueError(f"relaysum needs a fixed tree: the planned graph sequence of this problem has {len(topos)} "
+                         f"topologies (its messages relay over one fixed tree)")
+    if dmax > RELAY_MAX_DEG:
+        raise ValueError(f"relaysum handles at most {RELAY_MAX_DEG} neighbors per node on the fused kernels; the tree "
+                         f"has a node with {dmax}")
+
+
 class ConsensusEngine:
     def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
@@ -106,6 +120,10 @@ class ConsensusEngine:
         kgt_corr = opt.alg_name == "kgt" and opt.correction
         ad_track = opt.alg_name == "dadaptive" and opt.tracking
         self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") or kgt_corr or ad_track else 1
+        # RelaySum publishes one message per neighbor: channel e of node i is its message for neighbor j_e
+        self.relay = opt.alg_name == "relaysum"
+        if self.relay:
+            self.C = opt.dmax
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
         self.choco = opt.alg_name == "choco_sgd"
@@ -145,6 +163,8 @@ class ConsensusEngine:
             self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
         elif self.cg:                               # an attacker's published row is not its theta
             self.pub[k0 & 1, 0, :L].copy_(opt.pub)
+        elif self.relay:                            # the messages published at the end of round k0 - 1
+            self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
@@ -191,6 +211,10 @@ class ConsensusEngine:
                              f"{G} topologies (s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a "
                              "fixed W)")
         dmax = max(1, max(t.max_degree for t in topos))
+        if self.relay:
+            check_relay_plan(topos, dmax)
+            if topos[0].key != opt.topo.key:
+                raise ValueError("relaysum: the planned graph is not the tree the optimizer was built on")
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
         directed = any(t.directed for t in topos)
@@ -204,6 +228,7 @@ class ConsensusEngine:
         rdr_deg = np.zeros((G, L), dtype=np.int32) if directed else None
         rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
+            rslot = t.reverse_slots() if self.relay else None
             # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
             # push-sum weights, over the in-neighbors (as Push-DIGing)
             if push_sum:
@@ -220,6 +245,10 @@ class ConsensusEngine:
                     if r != ctx.rank:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
+                        if self.relay:      # channel 0 of the edge: j's message for this node (its reverse slot)
+                            row = (par * self.C + rslot[g][e]) * self.Lpub + lj
+                            nbr_ptr[gi, l, e, par, 0] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
+                            continue
                         for ch in range(self.C):
                             row = (par * self.C + ch) * self.Lpub + lj
                             nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
@@ -286,8 +315,10 @@ class ConsensusEngine:
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
         # (CHOCO-SGD, BEER, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
-        # numerators with a weight; so does ClippedGossip, which clips per edge; complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and not (self.choco or self.beer or self.cg)
+        # numerators with a weight; so do ClippedGossip, which clips per edge, and RelaySum, whose rows are per-edge
+        # messages (a 2-node complete graph is a tree); complete_graph_mode is ignored)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
+                         and not (self.choco or self.beer or self.cg or self.relay)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -383,6 +414,14 @@ class ConsensusEngine:
                      clip_delta=float(opt.delta), attack_scale=float(opt.scale), attack_z=float(opt.z),
                      attack=None if self.t_attack is None else self.t_attack.data_ptr(),
                      nbr_byz=self.t_nbr_byz.data_ptr())
+        self.t_reach = self.rin = None
+        if self.relay:
+            # R_i^k - 1 of the local nodes for k = 0 .. diam (exact in either dtype), and the received messages of the
+            # round, written by relay_mix and read by relay_step
+            self.t_reach = torch.as_tensor(
+                (opt.reach[pl.lo: pl.lo + L] - 1).astype(npdt), device=dev).contiguous()
+            self.rin = torch.zeros(L, dmax, n_pad, dtype=self.dtype, device=dev)
+            d.update(reach=self.t_reach.data_ptr(), rin=self.rin.data_ptr(), diam=opt.diam, relay_n=pr.N)
         if opt.alg_name == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
@@ -419,10 +458,12 @@ class ConsensusEngine:
         counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
         steps.  dadaptive with tracking publishes two rows (theta and u~), without it one.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
         for the mix (``clip: none`` once, as DSGD; an ALIE attacker also reads its honest neighbors' rows, not
-        counted)."""
+        counted).  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
+        neighbor wrote for it: the pulled bytes are DSGD's."""
         deg = int(self.t_deg[0].sum().item())
         reads = 2 if self.cg and self.opt.clip == "adaptive" else 1
-        return {"row": int(self.row_bytes) * self.C, "pulled": int(self.row_bytes) * self.C * deg * reads}
+        chans = 1 if self.relay else self.C
+        return {"row": int(self.row_bytes) * chans, "pulled": int(self.row_bytes) * chans * deg * reads}
 
     def consensus_metric(self, k: int):
         """Fused consensus-error metric (csrc/consensus.cu: consensus_metric_kernel) on the rows published

@@ -13,6 +13,7 @@ A round is a short, fixed kernel sequence
     K-GT:  kgt_mix, [fwd/bwd, kgt_step(p)] x local_steps       (local DSGD: dsgd_mix in place of kgt_mix)
     ClippedGossip:  cg_dist, cg_mix, fwd/bwd, cg_step           (clip: none: dsgd_mix, fwd/bwd, cg_step)
     decentralized AMSGrad / AdaGrad:  dadaptive_mix, fwd/bwd, dadaptive_step     (own second moment: dsgd_mix first)
+    RelaySum:  relay_mix, fwd/bwd, relay_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -100,6 +101,10 @@ def _round_ops_impl(opt, eng, grads):
             eng.op.dsgd_mix()
         grads(0)
         eng.op.dadaptive_step()
+    elif alg == "relaysum":
+        eng.op.relay_mix()
+        grads(0)
+        eng.op.relay_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -154,9 +159,10 @@ class RoundProgram:
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
         # publish codes, SGP and Push-DIGing numerators and ClippedGossip's attackers attack rows, so their metric reads
-        # the parameter rows (all_theta) at the evaluation points instead
+        # the parameter rows (all_theta) at the evaluation points instead, as does RelaySum, which publishes messages
         attacked = self.eng.cg and bool(opt.byzantine)
-        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked)
+        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
+                                      or self.eng.relay)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -327,8 +333,11 @@ class RoundProgram:
             opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip") and opt.k > 0:
+        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
+                            "relaysum") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
+        if opt.alg_name == "relaysum":          # the messages published for round k
+            opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
         if opt.alg_name == "clipped_gossip":
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
         if opt.alg_name == "choco_sgd":

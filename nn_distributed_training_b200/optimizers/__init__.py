@@ -9,11 +9,13 @@ from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
 from .kgt import KGT
 from .push_diging import PushDIGing
+from .relaysum import RelaySum
 from .sgp import SGP
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
-              "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive}
+              "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
+              "relaysum": RelaySum}
 
 
 def build_optimizer(problem, device, opt_conf):

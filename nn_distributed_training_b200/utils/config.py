@@ -20,7 +20,7 @@ from ..ops.consensus_ref import CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, TOPK_RATI
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive")
+        "clipped_gossip", "dadaptive", "relaysum")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -52,6 +52,7 @@ OPT_SCHEMA = {
     # beta2 (default DADAPTIVE_BETA2) is filled in for variant amsgrad only
     "dadaptive": {"alpha": REQUIRED, "variant": REQUIRED, "tracking": True, "beta1": 0.9, "eps": 1e-8,
                   "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
+    "relaysum": {"alpha0": REQUIRED, "mu": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -101,6 +102,21 @@ def _check_dadaptive(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.alpha must be > 0 (got {c['alpha']!r})")
 
 
+RELAYSUM_KEYS = ("alg_name", "alpha0", "mu", "outer_iterations", "profile")
+
+
+def _check_relaysum(c: Dict[str, Any], path: str) -> None:
+    """RelaySum: DSGD's step schedule and no other key (RelaySum/Grad and momentum are not implemented)."""
+    for key in c:
+        if key not in RELAYSUM_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: relaysum takes no key {key!r} (its keys are alpha0, mu and "
+                              f"outer_iterations)")
+    if not _real(c["alpha0"]) or not float(c["alpha0"]) > 0.0:
+        raise ConfigError(f"{path}.alpha0 must be > 0 (got {c['alpha0']!r})")
+    if not _real(c["mu"]) or not float(c["mu"]) >= 0.0:
+        raise ConfigError(f"{path}.mu must be >= 0 (got {c['mu']!r})")
+
+
 def _fill(d: Dict[str, Any], schema: Dict[str, Any], path: str, extra: Iterable[str] = ()) -> Dict[str, Any]:
     out = dict(d)
     for k, dflt in schema.items():
@@ -138,7 +154,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only "
                           f"(alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive")
+                "dadaptive", "relaysum")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -173,6 +189,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.correction must be true or false (got {c['correction']!r})")
     if alg == "dadaptive":
         _check_dadaptive(c, path)
+    if alg == "relaysum":
+        _check_relaysum(c, path)
     if alg == "clipped_gossip":
         if c["clip"] not in ("none", "adaptive"):
             raise ConfigError(f"{path}.clip must be one of none|adaptive (got {c['clip']!r})")

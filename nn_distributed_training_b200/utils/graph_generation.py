@@ -185,7 +185,8 @@ DIRECTED_TYPES = ("directed_cycle", "exponential", "random_directed")
 def generate_from_conf(graph_conf) -> Tuple[int, nx.Graph]:
     """Build a graph from a YAML ``graph:`` block (reference :69-104).
     Types: wheel | cycle | complete | random (+ ``p``, ``gen_attempts``), and —
-    new here — ``path``, ``star``, ``disk`` (``target_fied``) and the directed
+    new here — ``path``, ``star``, ``binary_tree`` (``nx.full_rary_tree(2, N)``:
+    node i's children are 2i+1 and 2i+2), ``disk`` (``target_fied``) and the directed
     ``directed_cycle`` (``i -> i+1``), ``exponential`` (``i -> i + 2^m mod N``
     for every ``2^m < N``) and ``random_directed`` (``p``, ``seed``,
     ``gen_attempts``: strongly connected).  Directed graphs (``DIRECTED_TYPES``)
@@ -225,6 +226,8 @@ def generate_from_conf(graph_conf) -> Tuple[int, nx.Graph]:
         graph = nx.path_graph(N)
     elif kind == "star":
         graph = nx.star_graph(N - 1)
+    elif kind == "binary_tree":
+        graph = nx.full_rary_tree(2, N)
     elif kind == "disk":
         graph = disk_with_fied(N, graph_conf.get("target_fied", 1.0))
     elif kind == "random":
@@ -329,6 +332,34 @@ class Topology:
 
     def is_complete(self) -> bool:
         return self.N > 1 and bool((self.deg == self.N - 1).all())
+
+    def reverse_slots(self) -> List[List[int]]:
+        """``rs[i][e]``: the position of i in ``neighbors_noself[j]`` for ``j = neighbors_noself[i][e]`` (undirected
+        graphs), the slot under which neighbor j keeps what it exchanges with i."""
+        pos = [{j: e for e, j in enumerate(nb)} for nb in self.neighbors_noself]
+        return [[pos[j][i] for j in nb] for i, nb in enumerate(self.neighbors_noself)]
+
+    def reach_table(self) -> np.ndarray:
+        """``R[i, k] = |{l : d(i, l) <= k}|`` (i itself included) for ``k = 0 .. diam``, by breadth-first search from
+        every node; ``diam`` is the largest finite hop distance, so ``R[:, -1]`` is each node's component size."""
+        dist = np.full((self.N, self.N), -1, dtype=np.int64)
+        for s in range(self.N):
+            dist[s, s] = 0
+            frontier = [s]
+            while frontier:
+                nxt = []
+                for u in frontier:
+                    for v in self.neighbors_noself[u]:
+                        if dist[s, v] < 0:
+                            dist[s, v] = dist[s, u] + 1
+                            nxt.append(v)
+                frontier = nxt
+        diam = int(dist.max()) if self.N else 0
+        return np.stack([((dist >= 0) & (dist <= k)).sum(1) for k in range(diam + 1)], axis=1)
+
+    def is_tree(self) -> bool:
+        """Undirected, connected and exactly ``N - 1`` edges."""
+        return not self.directed and self.is_connected() and int(self.adj.sum()) // 2 == self.N - 1
 
     def padded_table(self, dmax: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray, np.ndarray]:
         """(nbr_idx [N,dmax] int32 (-1 pad), nbr_w [N,dmax] f64, self_w [N] f64, deg [N] int32)."""
