@@ -501,6 +501,34 @@ def cg_publish_(pub: torch.Tensor, theta: torch.Tensor, pub_all: torch.Tensor, a
     pub.copy_(out)
 
 
+# ----------------------------------------------------------------- BRIDGE ----
+BRIDGE_SCREENS = ("trimmed_mean", "median")
+
+
+def bridge_mix_(theta: torch.Tensor, pub_all: torch.Tensor, nbrs, lo: int, screen: str, b: int = 0):
+    """Coordinate-wise screened mix of the local rows ``theta`` [L, n_pad] (bridge_mix_kernel): per element, the
+    neighbors' values of ``pub_all`` [N, n_pad] sorted (``torch.sort`` over the neighbor axis), then
+    ``trimmed_mean``: ``(theta_i + sorted positions [b, deg - b) in ascending order) / (1 + max(0, deg - 2b))``, or
+    ``median``: the median of theta_i and the deg values (``0.5 (lower + upper)`` of an even count), in fp64 and rounded
+    once to the row dtype.  ``nbrs[g]``: the neighbors of node g."""
+    out = theta.clone()
+    for l in range(theta.shape[0]):
+        nb = list(nbrs[lo + l])
+        x = theta[l].double()
+        s = torch.sort(pub_all[nb].double(), dim=0).values if nb else pub_all[:0].double()
+        deg = len(nb)
+        if screen == "median":
+            allv = torch.sort(torch.cat([x[None], s]), dim=0).values
+            y = allv[deg // 2] if deg % 2 == 0 else 0.5 * (allv[deg // 2] + allv[deg // 2 + 1])
+        else:
+            acc = x.clone()
+            for p in range(b, deg - b):
+                acc = acc + s[p]
+            y = acc / (1 + max(0, deg - 2 * b))
+        out[l] = y.to(theta.dtype)
+    theta.copy_(out)
+
+
 # ------------------------------------------------------------------ SGP ----
 # Push-sum (Stochastic Gradient Push): numerator rows x [L, n_pad] and float64 weights w [L].  The combine weights are
 # the column-stochastic A of Topology.push_weights, rounded to the arena dtype; w is mixed with those same rounded

@@ -129,11 +129,14 @@ struct ConsensusOp {
   consensus::RelayArgs<T> rs{};
   consensus::ClipArgs<T> cg{};
   int cg_adaptive = 0;
+  consensus::ScreenArgs<T> br{};
   consensus::SgpArgs<T> sg{};
   consensus::PushDigArgs<T> pd{};
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
-    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; sg.c = c; pd.c = c;
+    dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
+    pd.c = c;
+    br.b = geti(d, "screen_b", -1); br.median = geti(d, "screen_median", 0);
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
     pd.u = ptr<T>(d, "u"); pd.w = sg.w; pd.ysum = ptr<T>(d, "ysum"); pd.g_old = ptr<T>(d, "g_old");
@@ -273,6 +276,13 @@ struct ConsensusOp {
     cg_check("cg_step", false);
     check(consensus::launch_cg_step<T>(cg, cur_stream()), "cg_step");
   }
+  void bridge_mix() {
+    if (c.C != 1 || c.sum_mode || br.b < 0 || c.dmax > consensus::kBridgeMaxDeg)
+      throw std::runtime_error("bridge_mix needs one published channel, the pointer-table neighbors, the screen "
+                               "(`screen_b` >= 0, `screen_median`) and at most " +
+                               std::to_string(consensus::kBridgeMaxDeg) + " neighbors per node");
+    check(consensus::launch_bridge_mix<T>(br, cur_stream()), "bridge_mix");
+  }
   void sgp_check(const char* what) const {
     if (sg.x == nullptr || sg.w == nullptr || sg.row_stride <= 0)
       throw std::runtime_error(std::string(what) + " needs the SGP rows `x`, `w` and `row_stride`");
@@ -344,6 +354,7 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("cg_dist", &ConsensusOp<T>::cg_dist)
       .def("cg_mix", &ConsensusOp<T>::cg_mix)
       .def("cg_step", &ConsensusOp<T>::cg_step)
+      .def("bridge_mix", &ConsensusOp<T>::bridge_mix)
       .def("sgp_mix", &ConsensusOp<T>::sgp_mix)
       .def("sgp_step", &ConsensusOp<T>::sgp_step)
       .def("pdg_mix", &ConsensusOp<T>::pdg_mix)

@@ -16,6 +16,7 @@
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
 // ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
+// BRIDGE (no reference counterpart, optimizers/bridge.py)                  -> bridge_mix / cg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
@@ -1581,6 +1582,123 @@ __global__ void __launch_bounds__(THREADS) cg_step_kernel(const ClipArgs<T> a) {
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------------ BRIDGE ----
+// Round k (layout and rules in consensus.h): bridge_mix, fwd/bwd, cg_step.  Each thread screens the elements of its
+// 16-byte vector one component at a time: the D neighbor values (+inf in the slots past deg) go through Batcher's
+// odd-even merge network (5, 19 or 63 compare-exchanges for D = 4, 8, 16), then fully unrolled, predicated loops over
+// static positions sum the kept ones or pick the median, so nothing is indexed dynamically and no value leaves the
+// registers.  The median places the own value by its rank among the sorted neighbors instead of sorting D + 1 values.
+// Sorted values do not depend on the neighbor table order, so neither does the result (up to the sign of a zero).
+template <typename T>
+NNDT_DEVINL void cmp_swap(T& x, T& y) {
+  const T lo = y < x ? y : x, hi = y < x ? x : y;
+  x = lo;
+  y = hi;
+}
+
+// Batcher's network written as template recursion, so every index is a compile-time constant (the nested loop form
+// was not fully unrolled and put the values on the stack)
+template <int I, int END, int STEP, int R, int D, typename T>
+NNDT_DEVINL void oe_merge_cmp(T (&v)[D]) {
+  if constexpr (I < END) {
+    cmp_swap(v[I], v[I + R]);
+    oe_merge_cmp<I + STEP, END, STEP, R>(v);
+  }
+}
+
+// merge the two sorted halves of v[LO, LO + N) compared at distance R
+template <int LO, int N, int R, int D, typename T>
+NNDT_DEVINL void oe_merge(T (&v)[D]) {
+  if constexpr (2 * R < N) {
+    oe_merge<LO, N, 2 * R>(v);
+    oe_merge<LO + R, N, 2 * R>(v);
+    oe_merge_cmp<LO + R, LO + N - R, 2 * R, R>(v);
+  } else {
+    cmp_swap(v[LO], v[LO + R]);
+  }
+}
+
+template <int LO, int N, int D, typename T>
+NNDT_DEVINL void oe_sort(T (&v)[D]) {
+  if constexpr (N > 1) {
+    oe_sort<LO, N / 2>(v);
+    oe_sort<LO + N / 2, N / 2>(v);
+    oe_merge<LO, N, 1>(v);
+  }
+}
+
+template <int D, typename T>
+NNDT_DEVINL void odd_even_merge_sort(T (&v)[D]) {
+  static_assert((D & (D - 1)) == 0, "the network sorts a power of two");
+  oe_sort<0, D>(v);
+}
+
+// merged position q of the own value x (rank r among the sorted neighbors s) and s
+template <int D, typename T>
+NNDT_DEVINL T merged_at(const T (&s)[D], T x, int r, int q) {
+  T out = x;
+#pragma unroll
+  for (int p = 0; p < D; ++p) {
+    if (p < r && p == q) out = s[p];
+    if (p >= r && p + 1 == q) out = s[p];
+  }
+  return out;
+}
+
+// -Xptxas -v, no spills and no stack: 58 / 88 / 122 registers for fp64 with 4 / 8 / 16 slots, 66 / 86 / 136 for fp32.
+// Without the minimum of one CTA per SM ptxas held the fp32 16-slot variant to 128 registers and spilled.
+template <typename T, int D>
+__global__ void __launch_bounds__(THREADS, 1) bridge_mix_kernel(const ScreenArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const int lo = a.b, hi = deg - a.b;                        // trimmed mean: kept sorted positions [lo, hi)
+  const double kept = 1.0 + (double)max(0, hi - lo);
+  const int ql = deg / 2, qh = (deg + 1) / 2;                 // median: middle merged positions of deg + 1 values
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> th = ldv(c.theta + row + i);
+    Pack<T> q[D];
+#pragma unroll
+    for (int e = 0; e < D; ++e) {
+      if (e < deg) {
+        q[e] = ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i);
+      } else {
+#pragma unroll
+        for (int u = 0; u < N; ++u) q[e].v[u] = (T)INFINITY;
+      }
+    }
+    Pack<T> y;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      T s[D];
+#pragma unroll
+      for (int e = 0; e < D; ++e) s[e] = q[e].v[u];
+      odd_even_merge_sort<D>(s);
+      const T x = th.v[u];
+      if (a.median) {
+        int r = 0;
+#pragma unroll
+        for (int p = 0; p < D; ++p) r += s[p] < x ? 1 : 0;
+        const T vl = merged_at<D>(s, x, r, ql), vh = merged_at<D>(s, x, r, qh);
+        y.v[u] = ql == qh ? vl : (T)(0.5 * ((double)vl + (double)vh));
+      } else {
+        double acc = (double)x;
+#pragma unroll
+        for (int p = 0; p < D; ++p)
+          if (p >= lo && p < hi) acc += (double)s[p];
+        y.v[u] = (T)div_rn(acc, kept);
+      }
+    }
+    stv(c.theta + row + i, y);
+  }
+}
+
 // -------------------------------------------------------------------- SGP ----
 // Round k: sgp_mix pulls the in-neighbors' rows (x, w) of round k, x_i <- sum_j A_ij x_j, w_i <- sum_j A_ij w_j,
 // theta_i <- x_i / w_i; sgp_step takes x_i -= alpha_k g_i(theta_i), theta_i <- x_i / w_i and publishes (x_i, w_i).
@@ -2017,6 +2135,14 @@ template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStrea
   return launch_one_wave(cg_step_kernel<T, 4, true>, a.c, a, st);
 }
 
+// the fewest neighbor slots that hold the plan's largest degree
+template <typename T> cudaError_t launch_bridge_mix(const ScreenArgs<T>& a, cudaStream_t st) {
+  if (a.c.dmax > kBridgeMaxDeg) return cudaErrorInvalidValue;
+  if (a.c.dmax <= 4) return launch_one_wave(bridge_mix_kernel<T, 4>, a.c, a, st);
+  if (a.c.dmax <= 8) return launch_one_wave(bridge_mix_kernel<T, 8>, a.c, a, st);
+  return launch_one_wave(bridge_mix_kernel<T, kBridgeMaxDeg>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(sgp_mix_kernel<T>, a.c, a, st);
 }
@@ -2059,6 +2185,7 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_cg_dist<T>(const ClipArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_cg_mix<T>(const ClipArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_cg_step<T>(const ClipArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_bridge_mix<T>(const ScreenArgs<T>&, cudaStream_t);      \
   template cudaError_t launch_sgp_mix<T>(const SgpArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_sgp_step<T>(const SgpArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_pdg_mix<T>(const PushDigArgs<T>&, cudaStream_t);        \

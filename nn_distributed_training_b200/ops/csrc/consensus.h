@@ -231,6 +231,22 @@ struct ClipArgs {
   double scale, z;                 // sign-flip scale, ALIE's z
 };
 
+// BRIDGE (Fang, Yang, Bajwa 2022), optimizers/bridge.py: DSGD's single published channel with a coordinate-wise
+// screened mix, and ClippedGossip's step and attack rows (cg_step with a ClipArgs).  Per element, bridge_mix sorts the
+// deg neighbor values of round k and writes into theta
+//   trimmed mean: (theta_i + sorted positions [b, deg - b), ascending) / (1 + max(0, deg - 2b))
+//   median:       the median of theta_i and the deg values, 0.5 (lower + upper) of an even count
+// summed and averaged in fp64 and rounded once.  The neighbor values sit in registers: a node has at most
+// kBridgeMaxDeg neighbors (ops/engine.py: check_bridge_capacity).
+constexpr int kBridgeMaxDeg = 16;
+
+template <typename T>
+struct ScreenArgs {
+  Common<T> c;
+  int b;                           // values trimmed at each end (trimmed mean)
+  int median;                      // 1 = median screen, 0 = trimmed mean
+};
+
 // SGP, Stochastic Gradient Push (Assran et al. 2019): push-sum gossip over a column-stochastic A, on directed graphs.
 // The topology tables hold in-neighbors (nbr_ptr, deg, nbr_rank) and the weights of A (nbr_w = A_ij, self_w = A_ii).
 // A published row is [n_pad] T numerators x, then a 16-byte tail whose first 8 bytes are the float64 push-sum weight w:
@@ -294,6 +310,7 @@ template <typename T> cudaError_t launch_relay_step(const RelayArgs<T>& a, cudaS
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_bridge_mix(const ScreenArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_mix(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_sgp_step(const SgpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pdg_mix(const PushDigArgs<T>& a, cudaStream_t st);

@@ -38,7 +38,8 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum"):
+    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
+                          "bridge"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT and dadaptive: a constant step
         alpha[:] = opt.alpha
@@ -65,6 +66,17 @@ def check_clip_capacity(dmax: int) -> None:
     if dmax > CLIP_MAX_DEG:
         raise ValueError(f"clipped_gossip with clip: adaptive handles at most {CLIP_MAX_DEG} neighbors per node on the "
                          f"fused kernels; the planned graphs have a node with {dmax}")
+
+
+BRIDGE_MAX_DEG = 16     # consensus.h: kBridgeMaxDeg
+
+
+def check_bridge_capacity(dmax: int) -> None:
+    """BRIDGE's mix screens each element over the neighbor values held in registers, for at most ``BRIDGE_MAX_DEG``
+    neighbors per node."""
+    if dmax > BRIDGE_MAX_DEG:
+        raise ValueError(f"bridge handles at most {BRIDGE_MAX_DEG} neighbors per node on the fused kernels; the planned "
+                         f"graphs have a node with {dmax}")
 
 
 TOPK_CLUSTER = 8              # consensus.h: kTopkCluster
@@ -131,6 +143,7 @@ class ConsensusEngine:
         self.sgp = opt.alg_name == "sgp"
         self.pdg = opt.alg_name == "push_diging"
         self.cg = opt.alg_name == "clipped_gossip"
+        self.bridge = opt.alg_name == "bridge"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -161,7 +174,7 @@ class ConsensusEngine:
             self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.u)
             self.pub_weights(k0 & 1).copy_(opt.w)
             self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
-        elif self.cg:                               # an attacker's published row is not its theta
+        elif self.cg or self.bridge:                # an attacker's published row is not its theta
             self.pub[k0 & 1, 0, :L].copy_(opt.pub)
         elif self.relay:                            # the messages published at the end of round k0 - 1
             self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
@@ -211,6 +224,8 @@ class ConsensusEngine:
                              f"{G} topologies (s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a "
                              "fixed W)")
         dmax = max(1, max(t.max_degree for t in topos))
+        if self.bridge:
+            check_bridge_capacity(dmax)
         if self.relay:
             check_relay_plan(topos, dmax)
             if topos[0].key != opt.topo.key:
@@ -315,10 +330,11 @@ class ConsensusEngine:
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
         # (CHOCO-SGD, BEER, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
-        # numerators with a weight; so do ClippedGossip, which clips per edge, and RelaySum, whose rows are per-edge
-        # messages (a 2-node complete graph is a tree); complete_graph_mode is ignored)
+        # numerators with a weight; so do ClippedGossip, which clips per edge, BRIDGE, which screens the neighbor
+        # values, and RelaySum, whose rows are per-edge messages (a 2-node complete graph is a tree);
+        # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
-                         and not (self.choco or self.beer or self.cg or self.relay)
+                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -395,12 +411,17 @@ class ConsensusEngine:
                      vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if ad_track else None, beta1=opt.beta1,
                      beta2=opt.beta2, ad_eps=opt.eps, adagrad=int(opt.adagrad), tracking=int(ad_track))
         self.dist_part = self.t_attack = self.t_nbr_byz = None
-        if self.cg:
-            if opt.clip == "adaptive":
-                check_clip_capacity(dmax)
-            # fp64 partials of the squared neighbor distances: one per chunk of THREADS * (16 / itemsize) elements
-            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
-            self.dist_part = torch.zeros(L * dmax * pstride, dtype=torch.float64, device=dev)
+        if self.cg or self.bridge:         # BRIDGE's step is cg_step, with the same attack tables
+            if self.cg:
+                if opt.clip == "adaptive":
+                    check_clip_capacity(dmax)
+                # fp64 partials of the squared neighbor distances: one per chunk of THREADS * (16 / itemsize) elements
+                pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+                self.dist_part = torch.zeros(L * dmax * pstride, dtype=torch.float64, device=dev)
+                d.update(dist_part=self.dist_part.data_ptr(), pstride=pstride,
+                         clip_adaptive=int(opt.clip == "adaptive"), clip_delta=float(opt.delta))
+            else:
+                d.update(screen_b=opt.b, screen_median=int(opt.screen == "median"))
             byz = set(opt.byzantine)
             nbr_byz = np.zeros((G, L, dmax), dtype=np.int32)
             for gi, t in enumerate(topos):
@@ -410,8 +431,7 @@ class ConsensusEngine:
             self.t_nbr_byz = torch.as_tensor(nbr_byz, device=dev)
             if any(opt.attack):
                 self.t_attack = torch.as_tensor(np.asarray(opt.attack, dtype=np.int32), device=dev)
-            d.update(dist_part=self.dist_part.data_ptr(), pstride=pstride, clip_adaptive=int(opt.clip == "adaptive"),
-                     clip_delta=float(opt.delta), attack_scale=float(opt.scale), attack_z=float(opt.z),
+            d.update(attack_scale=float(opt.scale), attack_z=float(opt.z),
                      attack=None if self.t_attack is None else self.t_attack.data_ptr(),
                      nbr_byz=self.t_nbr_byz.data_ptr())
         self.t_reach = self.rin = None
@@ -458,7 +478,7 @@ class ConsensusEngine:
         counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
         steps.  dadaptive with tracking publishes two rows (theta and u~), without it one.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
         for the mix (``clip: none`` once, as DSGD; an ALIE attacker also reads its honest neighbors' rows, not
-        counted).  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
+        counted); BRIDGE reads each neighbor row once, as DSGD.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
         neighbor wrote for it: the pulled bytes are DSGD's."""
         deg = int(self.t_deg[0].sum().item())
         reads = 2 if self.cg and self.opt.clip == "adaptive" else 1

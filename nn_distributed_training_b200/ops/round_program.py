@@ -14,6 +14,7 @@ A round is a short, fixed kernel sequence
     ClippedGossip:  cg_dist, cg_mix, fwd/bwd, cg_step           (clip: none: dsgd_mix, fwd/bwd, cg_step)
     decentralized AMSGrad / AdaGrad:  dadaptive_mix, fwd/bwd, dadaptive_step     (own second moment: dsgd_mix first)
     RelaySum:  relay_mix, fwd/bwd, relay_step
+    BRIDGE (trimmed mean / median screening):  bridge_mix, fwd/bwd, cg_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -94,6 +95,10 @@ def _round_ops_impl(opt, eng, grads):
             eng.op.dsgd_mix()
         grads(0)
         eng.op.cg_step()
+    elif alg == "bridge":
+        eng.op.bridge_mix()
+        grads(0)
+        eng.op.cg_step()
     elif alg == "dadaptive":
         if opt.tracking:
             eng.op.dadaptive_mix()
@@ -158,9 +163,10 @@ class RoundProgram:
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
-        # publish codes, SGP and Push-DIGing numerators and ClippedGossip's attackers attack rows, so their metric reads
-        # the parameter rows (all_theta) at the evaluation points instead, as does RelaySum, which publishes messages
-        attacked = self.eng.cg and bool(opt.byzantine)
+        # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
+        # their metric reads the parameter rows (all_theta) at the evaluation points instead, as does RelaySum, which
+        # publishes messages
+        attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
                                       or self.eng.relay)
                              else (self.eng, lambda: opt.k))
@@ -334,11 +340,11 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum") and opt.k > 0:
+                            "relaysum", "bridge") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
-        if opt.alg_name == "clipped_gossip":
+        if opt.alg_name in ("clipped_gossip", "bridge"):
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
         if opt.alg_name == "choco_sgd":
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))

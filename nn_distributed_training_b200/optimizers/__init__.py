@@ -1,4 +1,5 @@
 from .beer import BEER
+from .bridge import Bridge
 from .clipped_gossip import ClippedGossip
 from .choco import ChocoSGD
 from .dadaptive import DAdaptive
@@ -15,7 +16,7 @@ from .sgp import SGP
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
-              "relaysum": RelaySum}
+              "relaysum": RelaySum, "bridge": Bridge}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -61,6 +61,20 @@ def check_byzantine(byz, N: int) -> List[int]:
     return sorted(nodes)
 
 
+def setup_attackers(opt, byz) -> None:
+    """The attacker fields of a Byzantine-robust optimizer (ClippedGossip, BRIDGE) from ``byzantine`` (or None):
+    ``byzantine`` (sorted node ids), ``attack_name``, ``scale``, ``z`` and ``attack``, the attack code of each local
+    node (cg_step's table)."""
+    attacked = byz is not None
+    opt.byzantine = check_byzantine(byz, opt.pr.N) if attacked else []
+    opt.attack_name = byz["attack"] if attacked else None
+    opt.scale = float(byz.get("scale", 1.0)) if attacked else 1.0
+    opt.z = float(byz.get("z", 1.0)) if attacked else 1.0
+    lo, L = opt.pr.placement.lo, opt.pr.placement.L
+    code = ref.ATTACK_CODE.get(opt.attack_name, 0)
+    opt.attack = [code if lo + l in opt.byzantine else 0 for l in range(L)]    # per local node
+
+
 class ClippedGossip(ConsensusOptimizer):
     alg_name = "clipped_gossip"
     STATE = ("pub",)
@@ -83,15 +97,7 @@ class ClippedGossip(ConsensusOptimizer):
         if self.clip == "adaptive" and not 0.0 <= self.delta < 1.0:
             raise ValueError(f"clipped_gossip delta must be in [0, 1) (got {conf['delta']!r})")
         self.refresh_graph = bool(conf.get("update_graph", True))
-        byz = conf.get("byzantine")
-        attacked = byz is not None
-        self.byzantine = check_byzantine(byz, self.pr.N) if attacked else []
-        self.attack_name = byz["attack"] if attacked else None
-        self.scale = float(byz.get("scale", 1.0)) if attacked else 1.0
-        self.z = float(byz.get("z", 1.0)) if attacked else 1.0
-        lo, L = self.pr.placement.lo, self.pr.placement.L
-        code = ref.ATTACK_CODE.get(self.attack_name, 0)
-        self.attack = [code if lo + l in self.byzantine else 0 for l in range(L)]    # per local node
+        setup_attackers(self, conf.get("byzantine"))
         self.pub = self.arena.theta.detach().clone()      # the rows the local nodes published last
 
     def alpha_table(self, n=None):

@@ -15,12 +15,14 @@ import yaml
 
 import math
 
-from ..ops.consensus_ref import CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, TOPK_RATIO_DEFAULT
+from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, TOPK_RATIO_DEFAULT
 
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge")
+# the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
+BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
 DIRECTED_GRAPH_TYPES = ("directed_cycle", "exponential", "random_directed")
 DIRECTED_ALGS = ("sgp", "push_diging")
@@ -53,6 +55,9 @@ OPT_SCHEMA = {
     "dadaptive": {"alpha": REQUIRED, "variant": REQUIRED, "tracking": True, "beta1": 0.9, "eps": 1e-8,
                   "outer_iterations": REQUIRED, "profile": False, "update_graph": True},
     "relaysum": {"alpha0": REQUIRED, "mu": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
+    # b is required with screen trimmed_mean and refused with median
+    "bridge": {"alpha0": REQUIRED, "mu": 0.0, "screen": REQUIRED, "outer_iterations": REQUIRED, "profile": False,
+               "update_graph": True},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -117,6 +122,21 @@ def _check_relaysum(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.mu must be >= 0 (got {c['mu']!r})")
 
 
+def _check_bridge(c: Dict[str, Any], path: str) -> None:
+    """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
+    if c["screen"] not in BRIDGE_SCREENS:
+        raise ConfigError(f"{path}.screen must be one of {'|'.join(BRIDGE_SCREENS)} (got {c['screen']!r})")
+    if c["screen"] == "median":
+        if "b" in c:
+            raise ConfigError(f"{path}.b applies to screen trimmed_mean only (screen is 'median')")
+        return
+    if "b" not in c:
+        raise ConfigError(f"missing required key {path}.b (screen: trimmed_mean)")
+    b = c["b"]
+    if isinstance(b, bool) or not isinstance(b, int) or b < 0:
+        raise ConfigError(f"{path}.b must be an integer >= 0 (got {b!r})")
+
+
 def _fill(d: Dict[str, Any], schema: Dict[str, Any], path: str, extra: Iterable[str] = ()) -> Dict[str, Any]:
     out = dict(d)
     for k, dflt in schema.items():
@@ -150,11 +170,11 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             raise ConfigError(f"{path}.lr_decay_type: {c['lr_decay_type']!r}")
         if c["primal_optimizer"] not in ("adam", "sgd", "adamw"):
             raise ConfigError(f"{path}.primal_optimizer: {c['primal_optimizer']!r}")
-    if "byzantine" in c and alg != "clipped_gossip":
-        raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only "
-                          f"(alg_name is {alg!r})")
+    if "byzantine" in c and alg not in BYZANTINE_ALGS:
+        raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
+                          f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum")
+                "dadaptive", "relaysum", "bridge")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -200,12 +220,14 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
             dl = c["delta"]
             if isinstance(dl, bool) or not isinstance(dl, (int, float)) or not 0.0 <= float(dl) < 1.0:
                 raise ConfigError(f"{path}.delta must be in [0, 1) (got {dl!r})")
-        if c.get("byzantine") is not None:
-            from ..optimizers.clipped_gossip import check_byzantine
-            try:
-                check_byzantine(c["byzantine"], None)
-            except ValueError as e:
-                raise ConfigError(f"{path}.{e}") from None
+    if alg == "bridge":
+        _check_bridge(c, path)
+    if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
+        from ..optimizers.clipped_gossip import check_byzantine
+        try:
+            check_byzantine(c["byzantine"], None)
+        except ValueError as e:
+            raise ConfigError(f"{path}.{e}") from None
     if int(c["outer_iterations"]) <= 0:
         raise ConfigError(f"{path}.outer_iterations must be positive")
     return c

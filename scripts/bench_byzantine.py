@@ -1,19 +1,21 @@
-"""ClippedGossip against Byzantine nodes on the setup of ``experiments/dist_mnist_byzantine.yaml`` (10-node complete graph
-through the neighbor pointer table, heterogeneous class split, MNISTConvNet(3, 5, 64), batch 64, nodes 0 and 1
-attacking, delta 0.2, on the fused sm_90a kernels).  Device time per round, bytes read per round, and the honest
+"""ClippedGossip and BRIDGE against Byzantine nodes on the setup of ``experiments/dist_mnist_byzantine.yaml`` (10-node
+complete graph through the neighbor pointer table, heterogeneous class split, MNISTConvNet(3, 5, 64), batch 64, nodes 0
+and 1 attacking, delta 0.2; the BRIDGE arms of ``experiments/dist_mnist_bridge.yaml``, trimmed mean with b 2 and
+median, on the same setup), on the fused sm_90a kernels.  Device time per round, bytes read per round, and the honest
 nodes' accuracy.
 
     python scripts/bench_byzantine.py [--dtypes fp64,fp32] [--rounds 400] [--warmup 40] [--repeats 3]
                                       [--accuracy-rounds 2000] [--accuracy-dtype fp32]
                                       [--data-source auto|mnist|synthetic|synthetic_hard] [--out FILE.json]
 
-  * speed: for each dtype the arms DSGD, ``clip: none`` and ``clip: adaptive`` (no attacker) alternate ``--repeats``
+  * speed: for each dtype the arms DSGD, ``clip: none``, ``clip: adaptive``, BRIDGE ``trimmed_mean`` (``bridge_tm``) and
+    BRIDGE ``median`` (no attacker) alternate ``--repeats``
     times; each builds its problem, runs ``--warmup`` rounds, captures the CUDA graphs of the next ``--rounds`` rounds
     and times their replay with CUDA events (ms per round, the median over repeats);
   * bytes: what this process's nodes read from their neighbors per round, from the engine (computed, not measured);
-  * accuracy: one run of ``--accuracy-rounds`` rounds per arm (DSGD without attack; ``clip: none`` and ``adaptive``
-    under ``sign_flip`` and ``alie``), arms alternated in this process; mean and worst top-1 over the honest nodes at
-    the last evaluation.
+  * accuracy: one run of ``--accuracy-rounds`` rounds per arm (DSGD without attack; ``clip: none``, ``adaptive`` and
+    the two BRIDGE screens under ``sign_flip`` and ``alie``), arms alternated in this process; mean and worst top-1
+    over the honest nodes at the last evaluation.
 The card's name and power limit are printed in the same run.  Prints one JSON line (and writes it to ``--out``).
 """
 from __future__ import annotations
@@ -42,7 +44,8 @@ from nn_distributed_training_b200.utils.config import load_experiment  # noqa: E
 
 DTYPES = {"fp64": torch.float64, "fp32": torch.float32}
 YAML = os.path.join(ROOT, "experiments", "dist_mnist_byzantine.yaml")
-SPEED = ["dsgd", "cg_none", "cg_adaptive"]
+BRIDGE_YAML = os.path.join(ROOT, "experiments", "dist_mnist_bridge.yaml")
+SPEED = ["dsgd", "cg_none", "cg_adaptive", "bridge_tm", "bridge_median"]
 
 
 def main(argv=None):
@@ -71,9 +74,12 @@ def main(argv=None):
     shards = split_hetero(train, N)
     print(f"MNIST source: {src} ({len(train)} train / {len(val)} val), {N} nodes, {exp['graph']['type']}", flush=True)
     problems = {pc["problem_name"]: pc for pc in conf["problem_configs"].values()}
-    for clip in ("none", "adaptive"):            # the speed arms: no attacker
-        pc = problems[f"cg_{clip}"] = copy.deepcopy(problems[f"cg_{clip}_sign_flip"])
-        pc["problem_name"] = f"cg_{clip}"
+    bridge = load_experiment(BRIDGE_YAML, "mnist")       # the same experiment block; its BRIDGE arms only
+    problems.update({pc["problem_name"]: pc for pc in bridge["problem_configs"].values()
+                     if pc["optimizer_config"]["alg_name"] == "bridge"})
+    for name in SPEED[1:]:                       # the speed arms: no attacker
+        pc = problems[name] = copy.deepcopy(problems[f"{name}_sign_flip"])
+        pc["problem_name"] = name
         del pc["optimizer_config"]["byzantine"]
 
     def build(name, dtype, rounds, eval_every):
