@@ -431,6 +431,136 @@ def relaysum_step_(theta: torch.Tensor, msg: torch.Tensor, r: torch.Tensor, live
         msg[:, e] = torch.where(live[:, e, None], m, torch.zeros((), dtype=m.dtype))
 
 
+# ------------------------------------------------------------- PowerGossip ----
+class PgLayout:
+    """The matrix table of PowerGossip, from a ``FlatLayout``: every parameter tensor with two or more dimensions is a
+    matrix ``(shape[0], prod(shape[1:]))``, the others (biases) are gossiped whole.  In slot order, ``segs`` holds one
+    ``(offset, m, n, poff, qoff)`` per tensor: for a matrix ``poff`` / ``qoff`` are its offsets in the row space
+    (``P = sum m``) and the column space (``Q = sum n``); for a 1-D tensor ``n = 0``, ``m`` is its length and ``poff``
+    its offset in the bias block (``B`` elements).  A phase-0 message is ``[the products h q (P) | biases (B)]``, a
+    phase-1 message ``[h^T p (Q) | biases (B)]``; ``width`` is the longer of the two, rounded up to 16 bytes in either
+    dtype (consensus.h: PgArgs)."""
+
+    def __init__(self, layout):
+        self.segs: List[Tuple[int, int, int, int, int]] = []
+        P = Q = B = 0
+        for s in layout.slots:
+            if len(s.shape) >= 2:
+                m = int(s.shape[0])
+                n = int(s.numel) // m
+                self.segs.append((int(s.offset), m, n, P, Q))
+                P += m
+                Q += n
+            else:
+                self.segs.append((int(s.offset), int(s.numel), 0, B, 0))
+                B += int(s.numel)
+        self.P, self.Q, self.B = P, Q, B
+        self.mats = [sg for sg in self.segs if sg[2] > 0]
+        self.vecs = [sg for sg in self.segs if sg[2] == 0]
+        self.width = -(-max(P + B, Q + B, 1) // 4) * 4
+
+    def msg_len(self, phase: int) -> int:
+        """Elements of a message of ``phase`` (unpadded)."""
+        return (self.Q if phase else self.P) + self.B
+
+
+def pg_start_vectors(lay: PgLayout, lo: int, hi: int, dtype: torch.dtype) -> torch.Tensor:
+    """``[P + Q]``: the unit vectors ``p_{e,l}`` (row space) then ``q_{e,l}`` (column space) of edge ``{lo, hi}``
+    (``lo < hi``), drawn for matrix l from ``np.random.default_rng((lo, hi, l))`` (p first), normalised in float64 and
+    rounded once to ``dtype``.  Both endpoints draw the same vectors."""
+    out = np.zeros(lay.P + lay.Q)
+    for l, (_, m, n, poff, qoff) in enumerate(lay.mats):
+        rng = np.random.default_rng((lo, hi, l))
+        p = rng.standard_normal(m)
+        q = rng.standard_normal(n)
+        out[poff: poff + m] = p / np.linalg.norm(p)
+        out[lay.P + qoff: lay.P + qoff + n] = q / np.linalg.norm(q)
+    return torch.as_tensor(out).to(dtype)
+
+
+def pg_sumsq(d: torch.Tensor) -> torch.Tensor:
+    """``sum d^2`` over the last dimension in float64, in the order of one warp of pg_mix_kernel: lane t sums the
+    elements t, t + 32, ... (each square rounded, then added), then the 32 lane sums are combined by xor butterflies
+    16, 8, 4, 2, 1.  Bit for bit the kernel's value, whatever the row's position in a batch."""
+    x = d.double()
+    n = x.shape[-1]
+    x = torch.nn.functional.pad(x, (0, (-n) % 32)).reshape(*x.shape[:-1], -1, 32)
+    s = torch.zeros(x.shape[:-2] + (32,), dtype=torch.float64, device=x.device)
+    for c in range(x.shape[-2]):
+        s = s + x[..., c, :] * x[..., c, :]
+    lane = torch.arange(32, device=x.device)
+    for o in (16, 8, 4, 2, 1):
+        s = s + s[..., lane ^ o]
+    return s[..., 0]
+
+
+def pg_messages(h: torch.Tensor, vec: torch.Tensor, live: torch.Tensor, lay: PgLayout, phase: int) -> torch.Tensor:
+    """The messages ``[L, dmax, width]`` node i publishes for its neighbor slots after its step: per matrix the product
+    ``h q_e`` (phase 0, length m) or ``h^T p_e`` (phase 1, length n), then h's 1-D tensors; zero past deg_i and past the
+    phase's length."""
+    L, dmax = live.shape
+    msg = torch.zeros(L, dmax, lay.width, dtype=h.dtype, device=h.device)
+    for off, m, n, poff, qoff in lay.mats:
+        H = h[:, off: off + m * n].reshape(L, 1, m, n)
+        if phase == 0:
+            q = vec[:, :, lay.P + qoff: lay.P + qoff + n]
+            msg[:, :, poff: poff + m] = (H @ q[..., None])[..., 0]
+        else:
+            p = vec[:, :, poff: poff + m]
+            msg[:, :, qoff: qoff + n] = (p[:, :, None, :] @ H)[:, :, 0]
+    base = lay.Q if phase else lay.P
+    for off, m, _, boff, _ in lay.vecs:
+        msg[:, :, base + boff: base + boff + m] = h[:, None, off: off + m]
+    return torch.where(live[:, :, None], msg, torch.zeros((), dtype=msg.dtype))
+
+
+def pg_mix_(theta: torch.Tensor, vec: torch.Tensor, own: torch.Tensor, nbr: torch.Tensor, sign: torch.Tensor,
+            w: torch.Tensor, live: torch.Tensor, gamma: float, lay: PgLayout, phase: int):
+    """The mix of round k (``phase = k & 1``) for the local rows ``theta`` (holding h).  ``own`` / ``nbr``
+    (``[L, dmax, width]``) are the messages node i and its neighbor j_e published for edge e; ``sign`` is +1 where
+    i < j_e, else -1.  Per edge, ``d = a_lo - a_hi`` (the same bits at both endpoints), ``U_e = d q^T`` (phase 0) or
+    ``p d^T`` (phase 1) per matrix and the whole difference for the 1-D tensors; then
+    ``x = h - gamma * sum_e (W_ie s_ie) U_e`` (e ascending) into ``theta``.  The next vectors ``p <- d / |d|``
+    (phase 0) or ``q <- d / |d|`` (phase 1) go into ``vec``, with ``|d|`` from ``pg_sumsq`` and one rounding; a zero
+    difference keeps the stored vector."""
+    L, dmax = live.shape
+    d = torch.where(sign[:, :, None] > 0, own - nbr, nbr - own)
+    coef = w * sign.to(w.dtype)
+    acc = torch.zeros_like(theta)
+    for off, m, n, poff, qoff in lay.mats:
+        a = torch.zeros(L, m, n, dtype=theta.dtype, device=theta.device)
+        for e in range(dmax):
+            if phase == 0:
+                U = d[:, e, poff: poff + m, None] * vec[:, e, None, lay.P + qoff: lay.P + qoff + n]
+            else:
+                U = vec[:, e, poff: poff + m, None] * d[:, e, None, qoff: qoff + n]
+            a = torch.where(live[:, e, None, None], a + coef[:, e, None, None] * U, a)
+        acc[:, off: off + m * n] = a.reshape(L, m * n)
+    base = lay.Q if phase else lay.P
+    for off, m, _, boff, _ in lay.vecs:
+        a = torch.zeros(L, m, dtype=theta.dtype, device=theta.device)
+        for e in range(dmax):
+            U = d[:, e, base + boff: base + boff + m]
+            a = torch.where(live[:, e, None], a + coef[:, e, None] * U, a)
+        acc[:, off: off + m] = a
+    theta.sub_(gamma * acc)
+    for off, m, n, poff, qoff in lay.mats:
+        lo, ln = (poff, m) if phase == 0 else (qoff, n)
+        out = poff if phase == 0 else lay.P + qoff
+        dl = d[:, :, lo: lo + ln]
+        ss = pg_sumsq(dl)
+        keep = (ss == 0) | ~live
+        nv = (dl.double() / ss.sqrt()[..., None]).to(vec.dtype)
+        vec[:, :, out: out + ln] = torch.where(keep[..., None], vec[:, :, out: out + ln], nv)
+
+
+def pg_step_(theta: torch.Tensor, msg: torch.Tensor, grad: torch.Tensor, alpha: float, vec: torch.Tensor,
+             live: torch.Tensor, lay: PgLayout, phase: int):
+    """``h = x - alpha g`` into ``theta``, and the messages of ``phase`` (that of round k + 1) into ``msg``."""
+    theta.add_(grad, alpha=-alpha)
+    msg.copy_(pg_messages(theta, vec, live, lay, phase))
+
+
 # ---------------------------------------------------------- ClippedGossip ----
 ATTACK_CODE = {"sign_flip": 1, "alie": 2}      # consensus.h: Attack (0 = honest)
 CLIP_SLACK = 1e-6      # consensus.h: kClipSlack, a prefix of (rounded) weights fits in delta up to this

@@ -127,6 +127,7 @@ struct ConsensusOp {
   consensus::KgtArgs<T> kg{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
+  consensus::PgArgs<T> pg{};
   consensus::ClipArgs<T> cg{};
   int cg_adaptive = 0;
   consensus::ScreenArgs<T> br{};
@@ -135,7 +136,10 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c;
+    pd.c = c; pg.c = c;
+    pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
+    pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
+    pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
     br.b = geti(d, "screen_b", -1); br.median = geti(d, "screen_median", 0);
     sg.x = ptr<T>(d, "x"); sg.w = ptr<double>(d, "w");
     sg.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
@@ -255,6 +259,22 @@ struct ConsensusOp {
     relay_check("relay_step");
     check(consensus::launch_relay_step<T>(rs, cur_stream()), "relay_step");
   }
+  void pg_check(const char* what) const {
+    if (pg.seg == nullptr || pg.sign == nullptr || pg.nseg < 1 || (pg.vec == nullptr && pg.P + pg.Q > 0) ||
+        pg.W < std::max(pg.P, pg.Q) + pg.B || c.sum_mode || c.C != c.dmax || c.dmax > consensus::kPgMaxDeg)
+      throw std::runtime_error(std::string(what) + " needs the segment table `pg_seg` (`pg_nseg`, `pg_P`, `pg_Q`, `pg_B`), "
+                               "the edge signs `pg_sign`, the vectors `pg_vec`, a message stride `pg_W` that holds both "
+                               "phases, the pointer-table neighbors and one published channel per neighbor slot (C = "
+                               "dmax <= " + std::to_string(consensus::kPgMaxDeg) + ")");
+  }
+  void pg_mix() {
+    pg_check("pg_mix");
+    check(consensus::launch_pg_mix<T>(pg, cur_stream()), "pg_mix");
+  }
+  void pg_step() {
+    pg_check("pg_step");
+    check(consensus::launch_pg_step<T>(pg, cur_stream()), "pg_step");
+  }
   void cg_check(const char* what, bool clip) const {
     if (c.C != 1 || c.sum_mode)
       throw std::runtime_error(std::string(what) + " needs one published channel and the pointer-table neighbors");
@@ -351,6 +371,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)
       .def("relay_step", &ConsensusOp<T>::relay_step)
+      .def("pg_mix", &ConsensusOp<T>::pg_mix)
+      .def("pg_step", &ConsensusOp<T>::pg_step)
       .def("cg_dist", &ConsensusOp<T>::cg_dist)
       .def("cg_mix", &ConsensusOp<T>::cg_mix)
       .def("cg_step", &ConsensusOp<T>::cg_step)

@@ -17,6 +17,7 @@
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
 // ClippedGossip (no reference counterpart, optimizers/clipped_gossip.py)   -> cg_dist + cg_mix or dsgd_mix / cg_step
 // BRIDGE (no reference counterpart, optimizers/bridge.py)                  -> bridge_mix / cg_step
+// PowerGossip (no reference counterpart, optimizers/powergossip.py)        -> pg_mix / pg_step
 // SGP (no reference counterpart, optimizers/sgp.py)                        -> sgp_mix / sgp_step
 // Push-DIGing (no reference counterpart, optimizers/push_diging.py)        -> pdg_mix / pdg_track
 //
@@ -1394,6 +1395,174 @@ __global__ void __launch_bounds__(THREADS, U <= 4 && D <= 4 ? 3 : 2) relay_step_
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------- PowerGossip ----
+// Layout in consensus.h.  Round k runs phase k & 1: pg_mix, fwd/bwd, pg_step.  Every neighbor read of the round is in
+// pg_mix, after begin_round; pg_step writes only the other parity.
+template <typename T>
+NNDT_DEVINL T* pg_row(const PgArgs<T>& a, int par, int chan, int l) {
+  const Common<T>& c = a.c;
+  return c.pub + ((size_t)(par * c.C + chan) * c.pub_L + l) * a.W;
+}
+
+// Each CTA of node l pulls the deg messages of round k (own channel e and the one neighbor j_e wrote for l, 4 elements
+// in flight per thread) into shared memory as d_e = a_lo - a_hi: the same bits at both endpoints.  CTA 0 then writes
+// the next vectors d / |d|, one warp per (edge, matrix): |d|^2 is summed in fp64 by the lanes in element order and
+// combined by xor butterflies, an order that depends on nothing but the difference (ops/consensus_ref.py: pg_sumsq), so
+// both endpoints store the same bits; a zero difference keeps the stored vector.  Phase 0 writes p and reads q, phase 1
+// writes q and reads p, so the other CTAs never read what CTA 0 writes.  Every CTA applies
+// x = h - gamma sum_e (W_ie s_ie) U_e to its grid-stride share of the row.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) pg_mix_kernel(const PgArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  extern __shared__ __align__(16) unsigned char pg_smem[];
+  T* d = reinterpret_cast<T*>(pg_smem);                 // [deg, W] canonical differences
+  __shared__ T coef[kPgMaxDeg];                         // W_ie s_ie
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const int ph = ri.par;
+  const int len = (ph ? a.Q : a.P) + a.B;
+  const int* sg = a.sign + l * c.dmax;
+  if ((int)threadIdx.x < deg) coef[threadIdx.x] = c.nbr_w[(ri.gid * c.L + l) * c.dmax + threadIdx.x] * (T)sg[threadIdx.x];
+  const int total = deg * len;
+  for (int b = threadIdx.x; b < total; b += 4 * THREADS) {
+    T own[4], nb[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = b + u * THREADS;
+      if (t < total) {
+        const int e = t / len, j = t - e * len;
+        own[u] = pg_row(a, ph, e, l)[j];
+        nb[u] = nbr_row(c, ri.gid, l, e, ph, 0)[j];
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int t = b + u * THREADS;
+      if (t < total) {
+        const int e = t / len, j = t - e * len;
+        d[e * a.W + j] = sg[e] > 0 ? own[u] - nb[u] : nb[u] - own[u];
+      }
+    }
+  }
+  __syncthreads();
+  const int PQ = a.P + a.Q;
+  T* vl = a.vec + (size_t)l * c.dmax * PQ;
+  if (blockIdx.x == 0) {
+    const int lane = threadIdx.x & 31;
+    for (int t = threadIdx.x >> 5; t < deg * a.nseg; t += THREADS / 32) {
+      const int e = t / a.nseg;
+      const int* sd = a.seg + 5 * (t - e * a.nseg);
+      if (sd[2] == 0) continue;                          // a 1-D tensor has no vectors
+      const int ln = ph ? sd[2] : sd[1];
+      const T* dv = d + e * a.W + (ph ? sd[4] : sd[3]);
+      double ss = 0.0;
+      for (int j = lane; j < ln; j += 32) {
+        const double x = (double)dv[j];
+        ss = __dadd_rn(ss, __dmul_rn(x, x));
+      }
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) ss = __dadd_rn(ss, __shfl_xor_sync(0xffffffffu, ss, o));
+      if (ss > 0.0) {
+        const double nrm = sqrt_rn(ss);
+        T* out = vl + (size_t)e * PQ + (ph ? a.P + sd[4] : sd[3]);
+        for (int j = lane; j < ln; j += 32) out[j] = (T)div_rn((double)dv[j], nrm);
+      }
+    }
+  }
+  T* th = c.theta + (size_t)l * c.n_pad;
+  const int gt = blockIdx.x * THREADS + threadIdx.x, gs = gridDim.x * THREADS;
+  const int base = ph ? a.Q : a.P;
+  for (int s = 0; s < a.nseg; ++s) {
+    const int* sd = a.seg + 5 * s;
+    const int off = sd[0], m = sd[1], n = sd[2], poff = sd[3], qoff = sd[4];
+    const int numel = n > 0 ? m * n : m;
+    for (int t = gt; t < numel; t += gs) {
+      T acc = (T)0;
+      if (n > 0) {
+        const int r = t / n, cc = t - r * n;
+        for (int e = 0; e < deg; ++e) {
+          const T* ve = vl + (size_t)e * PQ;
+          const T* de = d + e * a.W;
+          const T u = ph ? ve[poff + r] * de[qoff + cc] : de[poff + r] * ve[a.P + qoff + cc];
+          acc += coef[e] * u;
+        }
+      } else {
+        for (int e = 0; e < deg; ++e) acc += coef[e] * d[e * a.W + base + poff + t];
+      }
+      th[off + t] -= a.gamma * acc;
+    }
+  }
+}
+
+// h = x - alpha_k g into theta, and the deg messages of phase (k + 1) & 1 into the other parity.  One warp per unit: a
+// row of a matrix (phase 0: the products h q_e are row dot products), a column (phase 1: h^T p_e, column dot products) or
+// kPgVecChunk elements of a 1-D tensor (copied).  The warp steps the unit's elements, then sums each product in the
+// lanes' element order and xor butterflies, so a message does not depend on the grid.  Each lane reads back only the
+// elements it stepped.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) pg_step_kernel(const PgArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  const T alpha = c.alpha[ri.k];
+  const int ph = ri.par ^ 1;
+  const int lane = threadIdx.x & 31;
+  const int nw = gridDim.x * (THREADS / 32);
+  T* th = c.theta + (size_t)l * c.n_pad;
+  const T* gp = c.grad_part + (size_t)l * c.S * c.n_pad;
+  const int PQ = a.P + a.Q;
+  const T* vl = a.vec + (size_t)l * c.dmax * PQ;
+  const int base = ph ? a.Q : a.P;
+  for (int g = blockIdx.x * (THREADS / 32) + (threadIdx.x >> 5);; g += nw) {
+    int s = 0, u = g, nu = 0;
+    for (; s < a.nseg; ++s) {
+      const int* sd = a.seg + 5 * s;
+      nu = sd[2] > 0 ? (ph ? sd[2] : sd[1]) : (sd[1] + kPgVecChunk - 1) / kPgVecChunk;
+      if (u < nu) break;
+      u -= nu;
+    }
+    if (s == a.nseg) break;
+    const int* sd = a.seg + 5 * s;
+    const int off = sd[0], m = sd[1], n = sd[2], poff = sd[3], qoff = sd[4];
+    int i0, stride, len, vo = 0, mo;
+    if (n == 0) {
+      i0 = off + u * kPgVecChunk; stride = 1; len = min(kPgVecChunk, m - u * kPgVecChunk);
+      mo = base + poff + u * kPgVecChunk;
+    } else if (ph == 0) {
+      i0 = off + u * n; stride = 1; len = n; vo = a.P + qoff; mo = poff + u;
+    } else {
+      i0 = off + u; stride = n; len = m; vo = poff; mo = qoff + u;
+    }
+    for (int j = lane; j < len; j += 32) {
+      const size_t i = (size_t)i0 + (size_t)j * stride;
+      T gr = gp[i];
+      for (int q = 1; q < c.S; ++q) gr += gp[(size_t)q * c.n_pad + i];
+      th[i] -= alpha * gr;
+    }
+    for (int e = 0; e < deg; ++e) {
+      T* out = pg_row(a, ri.par ^ 1, e, l) + mo;
+      if (n == 0) {
+        for (int j = lane; j < len; j += 32) out[j] = th[i0 + j];
+        continue;
+      }
+      const T* ve = vl + (size_t)e * PQ + vo;
+      T acc = (T)0;
+      for (int j = lane; j < len; j += 32) acc += th[(size_t)i0 + (size_t)j * stride] * ve[j];
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+      if (lane == 0) *out = acc;
+    }
+  }
+  end_step(c, l, ri.k, true);
+}
+
 // ----------------------------------------------------------- ClippedGossip ----
 // Round k (layout and rules in consensus.h): cg_dist, cg_mix, fwd/bwd, cg_step; with `clip: none` dsgd_mix replaces
 // the first two.  A clipped edge needs its distance over the whole row before any element is mixed, and the row is
@@ -2119,6 +2288,39 @@ template <typename T> cudaError_t launch_relay_step(const RelayArgs<T>& a, cudaS
   return launch_by_s(relay_step_kernel<T, 4, 4>, relay_step_kernel<T, 8, 4>, a.c, a, st);
 }
 
+// PowerGossip: pg_mix holds the deg message differences in dynamic shared memory (the opt-in limit is checked by
+// ops/engine.py: check_powergossip_capacity); the grid is one wave at that footprint, or `grid_x` CTAs per node
+template <typename T, typename K>
+static cudaError_t launch_pg(K kernel, const PgArgs<T>& a, size_t smem, cudaStream_t st) {
+  const Common<T>& c = a.c;
+  if (c.dmax > kPgMaxDeg) return cudaErrorInvalidValue;
+  int dev = 0, sms = 0, occ = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  if (smem > 48 * 1024) {
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+  }
+  int gx = a.grid_x;
+  if (gx <= 0) {
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, THREADS, smem) != cudaSuccess || occ < 1) occ = 1;
+    const int per_block = THREADS * Vec<T>::N, slots = sms * occ;
+    gx = (c.n_pad + per_block - 1) / per_block;
+    if (gx * c.L > slots) {
+      const int iters = (gx * c.L + slots - 1) / slots;
+      gx = (gx + iters - 1) / iters;
+    }
+    gx = gx > 0 ? gx : 1;
+  }
+  return launch_pdl(kernel, dim3(gx, c.L), dim3(THREADS), smem, st, a);
+}
+template <typename T> cudaError_t launch_pg_mix(const PgArgs<T>& a, cudaStream_t st) {
+  return launch_pg(pg_mix_kernel<T>, a, (size_t)a.c.dmax * a.W * sizeof(T), st);
+}
+template <typename T> cudaError_t launch_pg_step(const PgArgs<T>& a, cudaStream_t st) {
+  return launch_pg(pg_step_kernel<T>, a, 0, st);
+}
+
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st) {
   if (cg_chunks(a.c) > a.pstride) return cudaErrorInvalidValue;
   return launch_one_wave(cg_dist_kernel<T>, a.c, a, st);
@@ -2182,6 +2384,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_relay_step<T>(const RelayArgs<T>&, cudaStream_t);       \
+  template cudaError_t launch_pg_mix<T>(const PgArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_pg_step<T>(const PgArgs<T>&, cudaStream_t);          \
   template cudaError_t launch_cg_dist<T>(const ClipArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_cg_mix<T>(const ClipArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_cg_step<T>(const ClipArgs<T>&, cudaStream_t);           \

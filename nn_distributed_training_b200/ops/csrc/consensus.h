@@ -206,6 +206,30 @@ struct RelayArgs {
   T n;                             // nodes of the tree
 };
 
+// PowerGossip (Vogels, Karimireddy, Jaggi 2020), optimizers/powergossip.py, on a fixed undirected graph.  Round k runs
+// phase k & 1.  The published buffer has C = dmax channels of message rows `W` elements long (not n_pad): channel e of
+// node i is its message for neighbor j_e, [per matrix the product h q (phase 0, m_l long) or h^T p (phase 1, n_l long) |
+// the 1-D tensors (B)], and the pointer table's channel-0 entry of edge (i, e) names j_e's channel for i, as RelaySum's.
+// pg_mix pulls the deg messages into shared memory as canonical differences d = a_lo - a_hi, writes
+// x = h - gamma sum_e W_ie s_ie U_e into theta and the next vectors d / |d| into `vec` (|d| in fp64, one fixed order);
+// pg_step writes h into theta and publishes the products of phase (k + 1) & 1 into the other parity.
+// Segment s of `seg` is one parameter tensor in slot order: {offset, m, n, poff, qoff}, n = 0 for a 1-D tensor (m its
+// length, poff its offset in the bias block).  A node has at most kPgMaxDeg neighbors, and its deg message differences
+// must fit the opt-in shared memory (ops/engine.py: check_powergossip_capacity).
+constexpr int kPgMaxDeg = 16;
+constexpr int kPgVecChunk = 256;   // elements of a 1-D tensor one warp of pg_step publishes per unit
+
+template <typename T>
+struct PgArgs {
+  Common<T> c;
+  T* vec;                          // [L, dmax, P + Q] every edge's p (row space) then q (column space)
+  const int* seg;                  // [nseg, 5]
+  const int* sign;                 // [L, dmax] +1 when this node is the edge's lower endpoint, else -1
+  int nseg, P, Q, B, W;            // segments, sum m, sum n, bias elements, message row stride (elements)
+  T gamma;
+  int grid_x;                      // CTAs per node, 0 = one wave (the messages do not depend on it)
+};
+
 // ClippedGossip (He, Karimireddy, Jaggi 2022): DSGD's single published channel with a self-centred clipped mix, and
 // Byzantine nodes that publish an attack row instead of theta.  Round k: cg_dist reduces the squared
 // distances |theta_j^pub - theta_i|^2 of every neighbor, one partial per fixed chunk of the row, into dist_part; cg_mix
@@ -307,6 +331,8 @@ template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_step(const RelayArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pg_mix(const PgArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pg_step(const PgArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_dist(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_mix(const ClipArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_cg_step(const ClipArgs<T>& a, cudaStream_t st);

@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge"):
+                          "bridge", "powergossip"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT and dadaptive: a constant step
         alpha[:] = opt.alpha
@@ -119,6 +119,28 @@ def check_relay_plan(topos: List[Topology], dmax: int) -> None:
                          f"has a node with {dmax}")
 
 
+PG_MAX_DEG = 16     # consensus.h: kPgMaxDeg
+
+
+def pg_mix_smem(dmax: int, width: int, itemsize: int) -> int:
+    """Dynamic shared memory of pg_mix: the message differences of ``dmax`` neighbor slots."""
+    return dmax * width * itemsize
+
+
+def check_powergossip_capacity(dmax: int, width: int, itemsize: int, optin: int) -> None:
+    """PowerGossip's mix keeps a node's message differences (``dmax`` slots of ``width`` elements) in the shared memory
+    of each of its CTAs, at most ``optin`` bytes (the device's opt-in limit per block), and its per-edge weights for at
+    most ``PG_MAX_DEG`` neighbors."""
+    if dmax > PG_MAX_DEG:
+        raise ValueError(f"powergossip handles at most {PG_MAX_DEG} neighbors per node on the fused kernels; the graph "
+                         f"has a node with {dmax}")
+    need = pg_mix_smem(dmax, width, itemsize)
+    if need > optin:
+        raise ValueError(f"powergossip's mix holds {dmax} message differences of {width} elements in shared memory: "
+                         f"{need} bytes per CTA against the device's opt-in limit of {optin} (a model with shorter "
+                         f"messages, a graph of lower degree or float32 fits)")
+
+
 class ConsensusEngine:
     def __init__(self, opt, graphs_per_round: List):
         self.opt = opt
@@ -135,6 +157,10 @@ class ConsensusEngine:
         # RelaySum publishes one message per neighbor: channel e of node i is its message for neighbor j_e
         self.relay = opt.alg_name == "relaysum"
         if self.relay:
+            self.C = opt.dmax
+        # PowerGossip likewise, with message rows of the layout's message width instead of n_pad
+        self.pg = opt.alg_name == "powergossip"
+        if self.pg:
             self.C = opt.dmax
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
@@ -154,6 +180,8 @@ class ConsensusEngine:
             self.row_bytes = opt.code_bytes
         elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
+        elif self.pg:
+            self.row_bytes = opt.lay.width * itemsize
         else:
             self.row_bytes = n_pad * itemsize
         Lmax = max(pl.counts)
@@ -177,6 +205,9 @@ class ConsensusEngine:
         elif self.cg or self.bridge:                # an attacker's published row is not its theta
             self.pub[k0 & 1, 0, :L].copy_(opt.pub)
         elif self.relay:                            # the messages published at the end of round k0 - 1
+            self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
+        elif self.pg:                               # the messages of round k0 (phase k0 & 1), zero past their length
+            self.pub.zero_()
             self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
@@ -230,6 +261,14 @@ class ConsensusEngine:
             check_relay_plan(topos, dmax)
             if topos[0].key != opt.topo.key:
                 raise ValueError("relaysum: the planned graph is not the tree the optimizer was built on")
+        if self.pg:
+            if G > 1 or topos[0].key != opt.topo.key:
+                raise ValueError("powergossip needs a fixed graph: the planned graph sequence of this problem is not "
+                                 "the one graph the optimizer was built on (both endpoints of an edge carry its "
+                                 "power-iteration vectors from round to round)")
+            props = torch.cuda.get_device_properties(dev)
+            check_powergossip_capacity(dmax, opt.lay.width, itemsize,
+                                       int(getattr(props, "shared_memory_per_block_optin", 227 * 1024)))
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
         directed = any(t.directed for t in topos)
@@ -243,7 +282,7 @@ class ConsensusEngine:
         rdr_deg = np.zeros((G, L), dtype=np.int32) if directed else None
         rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
-            rslot = t.reverse_slots() if self.relay else None
+            rslot = t.reverse_slots() if self.relay or self.pg else None
             # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
             # push-sum weights, over the in-neighbors (as Push-DIGing)
             if push_sum:
@@ -260,7 +299,7 @@ class ConsensusEngine:
                     if r != ctx.rank:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
-                        if self.relay:      # channel 0 of the edge: j's message for this node (its reverse slot)
+                        if rslot is not None:   # channel 0 of the edge: j's message for this node (its reverse slot)
                             row = (par * self.C + rslot[g][e]) * self.Lpub + lj
                             nbr_ptr[gi, l, e, par, 0] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
                             continue
@@ -334,7 +373,7 @@ class ConsensusEngine:
         # values, and RelaySum, whose rows are per-edge messages (a 2-node complete graph is a tree);
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
-                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay)
+                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -442,6 +481,15 @@ class ConsensusEngine:
                 (opt.reach[pl.lo: pl.lo + L] - 1).astype(npdt), device=dev).contiguous()
             self.rin = torch.zeros(L, dmax, n_pad, dtype=self.dtype, device=dev)
             d.update(reach=self.t_reach.data_ptr(), rin=self.rin.data_ptr(), diam=opt.diam, relay_n=pr.N)
+        self.t_pg_seg = None
+        if self.pg:
+            # the segment table {offset, m, n, poff, qoff} and the edge signs; the vectors are the optimizer's own rows,
+            # updated in place by pg_mix
+            lay = opt.lay
+            self.t_pg_seg = torch.as_tensor(np.asarray(lay.segs, dtype=np.int32).reshape(-1, 5), device=dev)
+            d.update(pg_vec=opt.vec.data_ptr() if opt.vec.numel() else None, pg_seg=self.t_pg_seg.data_ptr(),
+                     pg_sign=opt.sign.data_ptr(), pg_nseg=len(lay.segs), pg_P=lay.P, pg_Q=lay.Q, pg_B=lay.B,
+                     pg_W=lay.width, gamma=float(opt.gamma), pg_grid=int(getattr(opt, "pg_grid", 0)))
         if opt.alg_name == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
@@ -478,9 +526,15 @@ class ConsensusEngine:
         counted).  An SGP or Push-DIGing row includes its 16-byte tail.  A K-GT round takes ``local_steps`` gradient
         steps.  dadaptive with tracking publishes two rows (theta and u~), without it one.  ClippedGossip with ``clip: adaptive`` reads every neighbor row twice, once for the distances and once
         for the mix (``clip: none`` once, as DSGD; an ALIE attacker also reads its honest neighbors' rows, not
-        counted); BRIDGE reads each neighbor row once, as DSGD.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
+        counted); BRIDGE reads each neighbor row once, as DSGD.  A PowerGossip node pulls one message per neighbor, of
+        ``sum m + biases`` (phase 0) or ``sum n + biases`` (phase 1) elements (unpadded): ``pulled_phase0`` and
+        ``pulled_phase1`` report both, ``pulled`` their mean, and ``row`` is the padded message row.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
         neighbor wrote for it: the pulled bytes are DSGD's."""
         deg = int(self.t_deg[0].sum().item())
+        if self.pg:
+            lay, itemsize = self.opt.lay, self.pub.element_size()
+            p0, p1 = (deg * lay.msg_len(ph) * itemsize for ph in (0, 1))
+            return {"row": int(self.row_bytes), "pulled": (p0 + p1) // 2, "pulled_phase0": p0, "pulled_phase1": p1}
         reads = 2 if self.cg and self.opt.clip == "adaptive" else 1
         chans = 1 if self.relay else self.C
         return {"row": int(self.row_bytes) * chans, "pulled": int(self.row_bytes) * chans * deg * reads}

@@ -15,6 +15,7 @@ A round is a short, fixed kernel sequence
     decentralized AMSGrad / AdaGrad:  dadaptive_mix, fwd/bwd, dadaptive_step     (own second moment: dsgd_mix first)
     RelaySum:  relay_mix, fwd/bwd, relay_step
     BRIDGE (trimmed mean / median screening):  bridge_mix, fwd/bwd, cg_step
+    PowerGossip:  pg_mix, fwd/bwd, pg_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -110,6 +111,10 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.relay_mix()
         grads(0)
         eng.op.relay_step()
+    elif alg == "powergossip":
+        eng.op.pg_mix()
+        grads(0)
+        eng.op.pg_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -164,11 +169,11 @@ class RoundProgram:
         self.graph_plan = graphs
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
         # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
-        # their metric reads the parameter rows (all_theta) at the evaluation points instead, as does RelaySum, which
-        # publishes messages
+        # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
+        # PowerGossip, which publish messages
         attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
-                                      or self.eng.relay)
+                                      or self.eng.relay or self.eng.pg)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -340,9 +345,11 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge") and opt.k > 0:
+                            "relaysum", "bridge", "powergossip") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
+            opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
+        if opt.alg_name == "powergossip":       # the messages of round k; pg_mix updates the vectors (opt.vec) in place
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
         if opt.alg_name in ("clipped_gossip", "bridge"):
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])

@@ -9,6 +9,7 @@ from .dsgdm import DSGDm
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
 from .kgt import KGT
+from .powergossip import PowerGossip
 from .push_diging import PushDIGing
 from .relaysum import RelaySum
 from .sgp import SGP
@@ -16,7 +17,7 @@ from .sgp import SGP
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
-              "relaysum": RelaySum, "bridge": Bridge}
+              "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip}
 
 
 def build_optimizer(problem, device, opt_conf):

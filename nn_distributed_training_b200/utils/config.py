@@ -20,7 +20,7 @@ from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VAR
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -58,6 +58,7 @@ OPT_SCHEMA = {
     # b is required with screen trimmed_mean and refused with median
     "bridge": {"alpha0": REQUIRED, "mu": 0.0, "screen": REQUIRED, "outer_iterations": REQUIRED, "profile": False,
                "update_graph": True},
+    "powergossip": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -122,6 +123,25 @@ def _check_relaysum(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.mu must be >= 0 (got {c['mu']!r})")
 
 
+POWERGOSSIP_KEYS = ("alg_name", "alpha0", "mu", "gamma", "outer_iterations", "profile")
+
+
+def _check_powergossip(c: Dict[str, Any], path: str) -> None:
+    """PowerGossip: DSGD's step schedule, the consensus step ``gamma`` in (0, 1], and no other key (higher ranks are not
+    implemented)."""
+    for key in c:
+        if key not in POWERGOSSIP_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: powergossip takes no key {key!r} (its keys are alpha0, mu, gamma and "
+                              f"outer_iterations)")
+    if not _real(c["alpha0"]) or not (math.isfinite(float(c["alpha0"])) and float(c["alpha0"]) >= 0.0):
+        raise ConfigError(f"{path}.alpha0 must be finite and >= 0 (got {c['alpha0']!r})")
+    if not _real(c["mu"]) or not (math.isfinite(float(c["mu"])) and float(c["mu"]) >= 0.0):
+        raise ConfigError(f"{path}.mu must be finite and >= 0 (got {c['mu']!r})")
+    g = c["gamma"]
+    if not _real(g) or not (math.isfinite(float(g)) and 0.0 < float(g) <= 1.0):
+        raise ConfigError(f"{path}.gamma must be finite and in (0, 1] (got {g!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -174,7 +194,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge")
+                "dadaptive", "relaysum", "bridge", "powergossip")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -222,6 +242,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
                 raise ConfigError(f"{path}.delta must be in [0, 1) (got {dl!r})")
     if alg == "bridge":
         _check_bridge(c, path)
+    if alg == "powergossip":
+        _check_powergossip(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:

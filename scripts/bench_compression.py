@@ -1,11 +1,11 @@
-"""DSGD and CHOCO-SGD (compressor none / int8 / sign) on the PAPER MNIST setup: device time per round, bytes published
+"""DSGD, CHOCO-SGD (compressor none / int8 / sign) and optionally PowerGossip on the PAPER MNIST setup: device time per round, bytes published
 per row and pulled per round, and final accuracy.
 
     python scripts/bench_compression.py [--dtypes fp64,fp32] [--rounds 400] [--warmup 40] [--repeats 3]
                                         [--accuracy-rounds 2000] [--accuracy-dtypes fp32]
                                         [--sweep 0.1,0.3,0.5,0.8,1.0] [--sweep-rounds 500]
                                         [--data-source auto|mnist|synthetic|synthetic_hard] [--out FILE.json]
-                                        [--topk 0.01,0.05] [--step-launches 2000]
+                                        [--topk 0.01,0.05] [--step-launches 2000] [--powergossip 1.0]
 
 The problems are those of ``experiments/dist_mnist_choco.yaml`` (a 10-node cycle, the heterogeneous class split,
 MNISTConvNet(3, 5, 64), batch 64, on the fused sm_90a kernels), with ``choco_none`` added at the int8 problem's gamma.
@@ -19,7 +19,9 @@ MNISTConvNet(3, 5, 64), batch 64, on the fused sm_90a kernels), with ``choco_non
   * ``--topk``: a ``choco_topk<ratio>`` configuration per ratio (the int8 problem with compressor topk), measured with
     the others; ``--step-launches``: the step kernel alone, int8 against each top-k ratio, timed with CUDA events over
     that many back-to-back launches replayed from one CUDA graph (ms per launch, per dtype).
-Without ``--topk`` the output is that of the four configurations above.
+  * ``--powergossip``: a ``powergossip`` configuration (rank-one compressed edge differences, the int8 problem's step
+    schedule) at that gamma, measured with the others.
+Without ``--topk`` and ``--powergossip`` the output is that of the four configurations above.
 The card's name and power limit are printed in the same run.  Prints one JSON line (and writes it to ``--out``).
 """
 from __future__ import annotations
@@ -65,6 +67,7 @@ def main(argv=None):
     ap.add_argument("--out", default=None)
     ap.add_argument("--topk", default="")
     ap.add_argument("--step-launches", type=int, default=0)
+    ap.add_argument("--powergossip", type=float, default=None, help="add PowerGossip at this gamma")
     args = ap.parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("bench_compression.py measures the fused kernels and needs a CUDA device")
@@ -90,6 +93,12 @@ def main(argv=None):
         problems[f"choco_topk{r:g}"] = copy.deepcopy(problems["choco_int8"])
         problems[f"choco_topk{r:g}"]["optimizer_config"].update(compressor="topk", topk_ratio=r)
         names.append(f"choco_topk{r:g}")
+    if args.powergossip is not None:
+        pg = problems["powergossip"] = copy.deepcopy(problems["choco_int8"])
+        oc = pg["optimizer_config"]
+        pg["optimizer_config"] = {"alg_name": "powergossip", "gamma": args.powergossip, "alpha0": oc["alpha0"],
+                                  "mu": oc["mu"], "outer_iterations": oc["outer_iterations"], "profile": False}
+        names.append("powergossip")
 
     def build(name, dtype, rounds, eval_every, gamma=None):
         pc = copy.deepcopy(problems[name])
