@@ -94,6 +94,44 @@ def dsgt_track(y_all: torch.Tensor, w_rows: torch.Tensor, g_new: torch.Tensor, g
     return w_rows.to(y_all.dtype) @ y_all + g_new - g_old
 
 
+# ---------------------------------------------------------------- DeTAG ----
+def mixing_lambda(W: np.ndarray) -> float:
+    """``max |eig(W - 11^T / N)|`` of a symmetric mixing matrix, in float64 (0 for one node and the complete graph)."""
+    N = W.shape[0]
+    if N == 1:
+        return 0.0
+    return float(np.abs(np.linalg.eigvalsh(np.asarray(W, dtype=np.float64) - 1.0 / N)).max())
+
+
+def chebyshev_weights(lam: float, K: int, accelerate: bool = True) -> List[float]:
+    """The sub-step weights ``w_0 .. w_{K-1}`` of Chebyshev-accelerated gossip, in float64: ``w_0 = 1``,
+    ``w_1 = 2 / (2 - lam^2)``, ``w_s = 1 / (1 - lam^2 w_{s-1} / 4)``.  Every ``w_s = 1`` without acceleration (plain K-step
+    gossip) and when ``lam = 0``."""
+    out = [1.0] * K
+    if accelerate and lam > 0.0:
+        l2 = lam * lam
+        for s in range(1, K):
+            out[s] = 2.0 / (2.0 - l2) if s == 1 else 1.0 / (1.0 - l2 * out[s - 1] / 4.0)
+    return out
+
+
+def ag_gossip(x_all: torch.Tensor, x_prev: Optional[torch.Tensor], w_rows: torch.Tensor, omega: float) -> torch.Tensor:
+    """One gossip sub-step of the local rows: ``M = sum_j W_ij X_j`` and ``X_prev + omega (M - X_prev)`` (``omega == 1``:
+    ``M``, and ``x_prev`` is not read)."""
+    m = dsgd_mix(x_all, w_rows)
+    if omega == 1.0:
+        return m
+    return x_prev + omega * (m - x_prev)
+
+
+def detag_track_(y: torch.Tensor, g_old: torch.Tensor, ymix: torch.Tensor, grad: torch.Tensor, theta: torch.Tensor,
+                 alpha: float) -> torch.Tensor:
+    """``y <- Y_K + (g - g_old)``, ``g_old <- g``; returns the row to publish, ``z = theta - alpha y``."""
+    y.copy_(ymix + (grad - g_old))
+    g_old.copy_(grad)
+    return theta - alpha * y
+
+
 # ------------------------------------------------------ Exact Diffusion ----
 def ed_weights(W):
     """``A = (I + W) / 2`` of a float64 Metropolis matrix: the combine weights of Exact Diffusion."""

@@ -125,6 +125,7 @@ struct ConsensusOp {
   consensus::ChocoArgs<T> ch{};
   consensus::BeerArgs<T> be{};
   consensus::KgtArgs<T> kg{};
+  consensus::DetagArgs<T> dt{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -136,7 +137,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c;
+    pd.c = c; pg.c = c; dt.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -158,6 +159,8 @@ struct ConsensusOp {
     be.live = ch.live; be.gamma = ch.gamma; be.code = ch.code; be.code_stride = ch.code_stride; be.topk_k = ch.topk_k;
     kg.corr = ptr<T>(d, "corr"); kg.dacc = ptr<T>(d, "dacc");
     kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
+    dt.omega = ptr<const T>(d, "omega"); dt.ymix = ptr<T>(d, "ymix"); dt.g_old = ptr<T>(d, "g_old");
+    dt.K = geti(d, "gossip_steps", 0);
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -231,6 +234,22 @@ struct ConsensusOp {
       throw std::runtime_error("kgt_step with correction needs the K-GT rows `corr`, `dacc` and two published channels");
     kg.step = step;
     check(consensus::launch_kgt_step<T>(kg, cur_stream()), "kgt_step");
+  }
+  void detag_check(const char* what) const {
+    if (dt.omega == nullptr || dt.ymix == nullptr || dt.g_old == nullptr || dt.K < 1 || c.sum_mode || c.C != 2)
+      throw std::runtime_error(std::string(what) + " needs the sub-step weights `omega`, the rows `ymix` and `g_old`, "
+                               "`gossip_steps` >= 1, the pointer-table neighbors and two published channels");
+  }
+  void ag_gossip(int step) {
+    detag_check("ag_gossip");
+    if (step < 0 || step >= dt.K)
+      throw std::runtime_error("ag_gossip: sub-step " + std::to_string(step) + " outside 0.." + std::to_string(dt.K - 1));
+    dt.step = step;
+    check(consensus::launch_ag_gossip<T>(dt, cur_stream()), "ag_gossip");
+  }
+  void detag_track() {
+    detag_check("detag_track");
+    check(consensus::launch_detag_track<T>(dt, cur_stream()), "detag_track");
   }
   void dadaptive_mix() {
     if (!ad.tracking || ad.ut == nullptr || c.C != 2)
@@ -367,6 +386,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("beer_step", &ConsensusOp<T>::beer_step)
       .def("kgt_mix", &ConsensusOp<T>::kgt_mix)
       .def("kgt_step", &ConsensusOp<T>::kgt_step)
+      .def("ag_gossip", &ConsensusOp<T>::ag_gossip)
+      .def("detag_track", &ConsensusOp<T>::detag_track)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

@@ -12,6 +12,7 @@
 // BEER (no reference counterpart, optimizers/beer.py)                      -> beer_mix / beer_step
 //                                                          (top-k codes)   -> beer_topk_mix / beer_topk_step
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
+// DeTAG (no reference counterpart, optimizers/detag.py)                    -> K x ag_gossip / detag_track
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
@@ -1178,6 +1179,121 @@ __global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 2) kgt_step_kernel(const
   end_step(c, l, ri.k, last);
 }
 
+// ------------------------------------------------------------------- DeTAG ----
+// Channel 0 of the published buffer is z = theta - alpha y, channel 1 the tracker y.  Gradient round k is K protocol
+// rounds p = K k + s, one ag_gossip launch each, then fwd/bwd and detag_track in the last of them.  Sub-step s mixes
+// both channels, M_s = sum_j W_ij X_s,j (own term first, then neighbors in table order, as dsgd_mix), and takes
+// X_{s+1} = X_{s-1} + w_s (M_s - X_{s-1}); with w_s == 1 it is M_s and X_{s-1} is not read.  X_s is the parity p & 1
+// row.  X_{s-1} is the node's own row of parity (p + 1) & 1, which a non-last sub-step overwrites with X_{s+1}: each
+// thread reads its element before it writes it, and the round-start wait guarantees the neighbors have finished
+// reading it in round p - 1.  The round counter that names the parities was advanced by the previous sub-step, so
+// nothing is loaded before the dependency wait.  The last sub-step (LAST) writes theta = X_K and ymix = Y_K, publishes
+// nothing and leaves the round open.
+template <typename T, bool LAST>
+__global__ void __launch_bounds__(THREADS) ag_gossip_kernel(const DetagArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T om = a.omega[a.step];
+  const bool acc = om != (T)1;
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const T* xs = pub_row(c, ri.par, 0, l);
+  const T* ys = pub_row(c, ri.par, 1, l);
+  T* xo = pub_row(c, ri.par ^ 1, 0, l);
+  T* yo = pub_row(c, ri.par ^ 1, 1, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> mx = ldv(xs + i), my = ldv(ys + i), px, py;
+    if (acc) {
+      px = ldv(xo + i);
+      py = ldv(yo + i);
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      mx.v[u] *= ws;
+      my.v[u] *= ws;
+    }
+    // for_neighbors<2> written out, as in dsgt_mix: two channels of two neighbors in flight
+    for (int e0 = 0; e0 < deg; e0 += 2) {
+      Pack<T> qx[2], qy[2];
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          qx[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 0) + i);
+          qy[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 1) + i);
+        }
+#pragma unroll
+      for (int j = 0; j < 2; ++j)
+        if (e0 + j < deg) {
+          const T we = w[e0 + j];
+#pragma unroll
+          for (int u = 0; u < N; ++u) {
+            mx.v[u] += we * qx[j].v[u];
+            my.v[u] += we * qy[j].v[u];
+          }
+        }
+    }
+    if (acc) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        mx.v[u] = px.v[u] + om * (mx.v[u] - px.v[u]);
+        my.v[u] = py.v[u] + om * (my.v[u] - py.v[u]);
+      }
+    }
+    if (LAST) {
+      stv(c.theta + row + i, mx);
+      stv(a.ymix + row + i, my);
+    } else {
+      stv(xo + i, mx);
+      stv(yo + i, my);
+    }
+  }
+  if (!LAST) {
+    tag_published(c, l, ri.k);
+    finish_round(c, ri.k);
+  }
+}
+
+// Tracking step of gradient round k, in protocol round p = K k + K - 1: y = Y_K + (g - g_old), g_old = g, and publish
+// z = theta - alpha y and y into the other parity.  Y_K (ymix), theta and g_old were written two launches back or
+// earlier and are read before the dependency wait; only the gradient partials after it.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) detag_track_kernel(const DetagArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  T* zo = pub_row(c, ri.par ^ 1, 0, l);
+  T* yo = pub_row(c, ri.par ^ 1, 1, l);
+  bool waited = false;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> y = ldv(a.ymix + row + i);
+    const Pack<T> go = ldv(a.g_old + row + i);
+    const Pack<T> th = ldv(c.theta + row + i);
+    release_dependents_once(waited);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> z;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      y.v[u] += g.v[u] - go.v[u];
+      z.v[u] = th.v[u] - alpha * y.v[u];
+    }
+    stv(a.g_old + row + i, g);
+    stv(zo + i, z);
+    stv(yo + i, y);
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2262,6 +2378,13 @@ template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStrea
   return a.correction ? launch_kgt<T, true>(a, st) : launch_kgt<T, false>(a, st);
 }
 
+template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(a.step == a.K - 1 ? ag_gossip_kernel<T, true> : ag_gossip_kernel<T, false>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(detag_track_kernel<T, 4>, detag_track_kernel<T, 8>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
 }
@@ -2380,6 +2503,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_beer_step<T>(const BeerArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_kgt_mix<T>(const KgtArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
+  template cudaError_t launch_ag_gossip<T>(const DetagArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_detag_track<T>(const DetagArgs<T>&, cudaStream_t);      \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

@@ -174,6 +174,19 @@ struct KgtArgs {
   int step, K, correction;
 };
 
+// DeTAG (Lu, De Sa 2021): gradient tracking with K Chebyshev-accelerated gossip sub-steps per gradient step.  Channel 0
+// of the published buffer is z = theta - alpha y, channel 1 the tracker y.  Every sub-step is a protocol round of its
+// own: the device round counter counts sub-steps, p = K k + s, and `graph_id` / `alpha` hold K entries per gradient
+// round.  `step` is the sub-step index s of the launch; the last one writes theta and `ymix` instead of publishing.
+template <typename T>
+struct DetagArgs {
+  Common<T> c;
+  const T* omega;                  // [K] the sub-step weights w_s (w_0 = 1)
+  T* ymix;                         // [L, n_pad] Y_K of the last sub-step, read by detag_track (dead between rounds)
+  T* g_old;                        // [L, n_pad] the gradient of the previous round (zero at the start)
+  int step, K;
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -327,6 +340,8 @@ template <typename T> cudaError_t launch_beer_mix(const BeerArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_beer_step(const BeerArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

@@ -41,7 +41,7 @@ def schedule_tables(opt, H: int):
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
                           "bridge", "powergossip"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT and dadaptive: a constant step
+    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive and DeTAG: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -153,7 +153,7 @@ class ConsensusEngine:
         # dadaptive with its second-moment tracker u~ (tracking) or without it
         kgt_corr = opt.alg_name == "kgt" and opt.correction
         ad_track = opt.alg_name == "dadaptive" and opt.tracking
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer") or kgt_corr or ad_track else 1
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer", "detag") or kgt_corr or ad_track else 1
         # RelaySum publishes one message per neighbor: channel e of node i is its message for neighbor j_e
         self.relay = opt.alg_name == "relaysum"
         if self.relay:
@@ -170,6 +170,10 @@ class ConsensusEngine:
         self.pdg = opt.alg_name == "push_diging"
         self.cg = opt.alg_name == "clipped_gossip"
         self.bridge = opt.alg_name == "bridge"
+        # DeTAG: every gossip sub-step is a protocol round, p = K k + s, so the device round counter, the flags and the
+        # sequence tags count K per gradient round and the schedules hold K entries per gradient round
+        self.detag = opt.alg_name == "detag"
+        K = self.rounds_per_step = opt.gossip_steps if self.detag else 1
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -189,6 +193,7 @@ class ConsensusEngine:
         self.pub = self.pub_buf.local
         self.Lpub = Lmax
         k0 = opt.k
+        p0 = K * k0                 # the protocol round of gradient round k0
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
         if self.choco:
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
@@ -209,6 +214,9 @@ class ConsensusEngine:
         elif self.pg:                               # the messages of round k0 (phase k0 & 1), zero past their length
             self.pub.zero_()
             self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
+        elif self.detag:                            # z = theta - alpha y and y, published for protocol round p0
+            self.pub[p0 & 1, 0, :L].copy_(opt.z)
+            self.pub[p0 & 1, 1, :L].copy_(opt.y)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
@@ -218,7 +226,7 @@ class ConsensusEngine:
 
         # ---- schedules ----------------------------------------------------------
         H = self.horizon = schedule_horizon(opt)
-        rho, lr, alpha = schedule_tables(opt, H)
+        rho, lr, alpha = (np.repeat(t, K) for t in schedule_tables(opt, H))
         self.rho = torch.as_tensor(rho.astype(npdt), device=dev)
         self.lr = torch.as_tensor(lr.astype(npdt), device=dev)
         self.alpha = torch.as_tensor(alpha.astype(npdt), device=dev)
@@ -243,6 +251,7 @@ class ConsensusEngine:
                     topos.append(t)
                 gi = by_object[id(g)] = key_to_id[t.key]
             gid[k] = gi
+        gid = np.repeat(gid, K)
         self.topos = topos
         G = len(topos)
         if (self.choco or self.beer) and opt.compressor == "topk":
@@ -269,6 +278,10 @@ class ConsensusEngine:
             props = torch.cuda.get_device_properties(dev)
             check_powergossip_capacity(dmax, opt.lay.width, itemsize,
                                        int(getattr(props, "shared_memory_per_block_optin", 227 * 1024)))
+        if self.detag and (G > 1 or topos[0].key != opt.topo.key):
+            raise ValueError("detag needs a fixed graph: the planned graph sequence of this problem is not the one graph "
+                             "its Chebyshev weights were computed for (acceleration has no guarantee on a changing "
+                             "mixing matrix)")
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
         directed = any(t.directed for t in topos)
@@ -326,8 +339,8 @@ class ConsensusEngine:
         self.t_nbr_seq = None
         if opt.conf.get("debug_sequence_check", False) or os.environ.get("NNDT_SEQ_CHECK") == "1":
             self.seq_buf = SymmetricBuffer((2, Lmax), torch.int32, ctx)
-            self.seq_buf.local.fill_(k0 - 1)
-            self.seq_buf.local[k0 & 1].fill_(k0)
+            self.seq_buf.local.fill_(p0 - 1)
+            self.seq_buf.local[p0 & 1].fill_(p0)
             nbr_seq = np.zeros((G, L, dmax, 2), dtype=np.int64)
             for gi, t in enumerate(topos):
                 for l, g in enumerate(pl.local_nodes):
@@ -338,11 +351,11 @@ class ConsensusEngine:
             self.t_nbr_seq = torch.as_tensor(nbr_seq, device=dev)
 
         # ---- counters / flags -----------------------------------------------------
-        self.round_ctr = torch.full((1,), k0, dtype=torch.int32, device=dev)
+        self.round_ctr = torch.full((1,), p0, dtype=torch.int32, device=dev)
         self.done_ctr = torch.zeros(1, dtype=torch.int32, device=dev)
         self.err = torch.zeros(1, dtype=torch.int32, device=dev)
         self.flag_buf = SymmetricBuffer((max(ctx.world_size, 1),), torch.int32, ctx)
-        self.flag_buf.local.fill_(k0)
+        self.flag_buf.local.fill_(p0)
         peer_flag = np.zeros(max(ctx.world_size, 1), dtype=np.int64)
         for r in range(ctx.world_size):
             peer_flag[r] = self.flag_buf.peer_ptrs[r] + 4 * ctx.rank
@@ -373,7 +386,8 @@ class ConsensusEngine:
         # values, and RelaySum, whose rows are per-edge messages (a 2-node complete graph is a tree);
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
-                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg)
+                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
+                                  or self.detag)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -445,6 +459,13 @@ class ConsensusEngine:
         if opt.alg_name == "kgt":
             d.update(local_steps=opt.local_steps, correction=int(opt.correction),
                      corr=opt.c.data_ptr() if kgt_corr else None, dacc=opt.d.data_ptr() if kgt_corr else None)
+        self.omega = self.ymix = None
+        if self.detag:
+            # the sub-step weights in the arena dtype, and Y_K of the last sub-step (dead between rounds)
+            self.omega = torch.as_tensor(np.asarray(opt.omega, dtype=npdt), device=dev)
+            self.ymix = torch.zeros(L, n_pad, dtype=self.dtype, device=dev)
+            d.update(omega=self.omega.data_ptr(), ymix=self.ymix.data_ptr(), g_old=opt.g_old.data_ptr(),
+                     gossip_steps=K)
         if opt.alg_name == "dadaptive":
             d.update(ad_m=opt.m.data_ptr(), ad_v=None if opt.v is None else opt.v.data_ptr(),
                      vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if ad_track else None, beta1=opt.beta1,
@@ -529,7 +550,8 @@ class ConsensusEngine:
         counted); BRIDGE reads each neighbor row once, as DSGD.  A PowerGossip node pulls one message per neighbor, of
         ``sum m + biases`` (phase 0) or ``sum n + biases`` (phase 1) elements (unpadded): ``pulled_phase0`` and
         ``pulled_phase1`` report both, ``pulled`` their mean, and ``row`` is the padded message row.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
-        neighbor wrote for it: the pulled bytes are DSGD's."""
+        neighbor wrote for it: the pulled bytes are DSGD's.  A DeTAG round gossips ``gossip_steps`` times, each a DSGT
+        pull: ``pulled`` counts them all."""
         deg = int(self.t_deg[0].sum().item())
         if self.pg:
             lay, itemsize = self.opt.lay, self.pub.element_size()
@@ -537,7 +559,8 @@ class ConsensusEngine:
             return {"row": int(self.row_bytes), "pulled": (p0 + p1) // 2, "pulled_phase0": p0, "pulled_phase1": p1}
         reads = 2 if self.cg and self.opt.clip == "adaptive" else 1
         chans = 1 if self.relay else self.C
-        return {"row": int(self.row_bytes) * chans, "pulled": int(self.row_bytes) * chans * deg * reads}
+        return {"row": int(self.row_bytes) * chans,
+                "pulled": int(self.row_bytes) * chans * deg * reads * self.rounds_per_step}
 
     def consensus_metric(self, k: int):
         """Fused consensus-error metric (csrc/consensus.cu: consensus_metric_kernel) on the rows published

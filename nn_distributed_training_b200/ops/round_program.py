@@ -16,6 +16,7 @@ A round is a short, fixed kernel sequence
     RelaySum:  relay_mix, fwd/bwd, relay_step
     BRIDGE (trimmed mean / median screening):  bridge_mix, fwd/bwd, cg_step
     PowerGossip:  pg_mix, fwd/bwd, pg_step
+    DeTAG:  ag_gossip(s) x gossip_steps, fwd/bwd, detag_track      (every ag_gossip a protocol round)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -115,6 +116,11 @@ def _round_ops_impl(opt, eng, grads):
         eng.op.pg_mix()
         grads(0)
         eng.op.pg_step()
+    elif alg == "detag":
+        for s in range(opt.gossip_steps):
+            eng.op.ag_gossip(s)
+        grads(0)
+        eng.op.detag_track()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -170,10 +176,10 @@ class RoundProgram:
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
         # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
         # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
-        # PowerGossip, which publish messages
+        # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y
         attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
-                                      or self.eng.relay or self.eng.pg)
+                                      or self.eng.relay or self.eng.pg or self.eng.detag)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -209,6 +215,8 @@ class RoundProgram:
             return n + 2 * self.opt.pits
         if self.opt.alg_name == "clipped_gossip" and self.opt.clip == "adaptive":
             return n + 4
+        if self.opt.alg_name == "detag":
+            return n + self.opt.gossip_steps + 2
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
@@ -351,6 +359,10 @@ class RoundProgram:
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
         if opt.alg_name == "powergossip":       # the messages of round k; pg_mix updates the vectors (opt.vec) in place
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
+        if opt.alg_name == "detag":             # g_old is the optimizer's own row; the rows of protocol round K k
+            par = (opt.gossip_steps * opt.k) & 1
+            opt.z.copy_(eng.pub[par, 0, :L])
+            opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name in ("clipped_gossip", "bridge"):
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
         if opt.alg_name == "choco_sgd":

@@ -3,6 +3,7 @@ from .bridge import Bridge
 from .clipped_gossip import ClippedGossip
 from .choco import ChocoSGD
 from .dadaptive import DAdaptive
+from .detag import DeTAG
 from .dinno import DiNNO
 from .dsgd import DSGD
 from .dsgdm import DSGDm
@@ -17,7 +18,7 @@ from .sgp import SGP
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
-              "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip}
+              "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG}
 
 
 def build_optimizer(problem, device, opt_conf):

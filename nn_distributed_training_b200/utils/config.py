@@ -20,7 +20,7 @@ from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VAR
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -59,6 +59,8 @@ OPT_SCHEMA = {
     "bridge": {"alpha0": REQUIRED, "mu": 0.0, "screen": REQUIRED, "outer_iterations": REQUIRED, "profile": False,
                "update_graph": True},
     "powergossip": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
+    "detag": {"alpha": REQUIRED, "gossip_steps": REQUIRED, "accelerate": True, "outer_iterations": REQUIRED,
+              "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -142,6 +144,25 @@ def _check_powergossip(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.gamma must be finite and in (0, 1] (got {g!r})")
 
 
+DETAG_KEYS = ("alg_name", "alpha", "gossip_steps", "accelerate", "outer_iterations", "profile")
+
+
+def _check_detag(c: Dict[str, Any], path: str) -> None:
+    """DeTAG: the step ``alpha`` (finite, > 0), ``gossip_steps`` (an integer >= 1), ``accelerate`` (a bool) and no other
+    key."""
+    for key in c:
+        if key not in DETAG_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: detag takes no key {key!r} (its keys are alpha, gossip_steps, accelerate "
+                              f"and outer_iterations)")
+    if not _real(c["alpha"]) or not (math.isfinite(float(c["alpha"])) and float(c["alpha"]) > 0.0):
+        raise ConfigError(f"{path}.alpha must be finite and > 0 (got {c['alpha']!r})")
+    ks = c["gossip_steps"]
+    if isinstance(ks, bool) or not isinstance(ks, int) or ks < 1:
+        raise ConfigError(f"{path}.gossip_steps must be an integer >= 1 (got {ks!r})")
+    if not isinstance(c["accelerate"], bool):
+        raise ConfigError(f"{path}.accelerate must be true or false (got {c['accelerate']!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -194,7 +215,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge", "powergossip")
+                "dadaptive", "relaysum", "bridge", "powergossip", "detag")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -244,6 +265,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_bridge(c, path)
     if alg == "powergossip":
         _check_powergossip(c, path)
+    if alg == "detag":
+        _check_detag(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
