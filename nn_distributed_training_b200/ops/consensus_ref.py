@@ -132,6 +132,18 @@ def detag_track_(y: torch.Tensor, g_old: torch.Tensor, ymix: torch.Tensor, grad:
     return theta - alpha * y
 
 
+# -------------------------------------------------------------- GT-HSGD ----
+def hsgd_track_(y: torch.Tensor, v: torch.Tensor, theta_prev: torch.Tensor, y_all: torch.Tensor, w_rows: torch.Tensor,
+                grad: torch.Tensor, grad_prev: torch.Tensor, theta: torch.Tensor, omb: float, first: bool) -> None:
+    """The tracking step of GT-HSGD on the local rows: ``v' = g`` (``first``, round 0) or ``g + omb (v - gp)`` with
+    ``omb = 1 - beta``, then ``y <- sum_j W_ij y_j + v' - v`` (``dsgt_track`` with v in place of the gradient),
+    ``v <- v'`` and ``theta_prev <- theta``."""
+    vn = grad.clone() if first else grad + omb * (v - grad_prev)
+    y.copy_(dsgt_track(y_all, w_rows, vn, v))
+    v.copy_(vn)
+    theta_prev.copy_(theta)
+
+
 # ------------------------------------------------------ Exact Diffusion ----
 def ed_weights(W):
     """``A = (I + W) / 2`` of a float64 Metropolis matrix: the combine weights of Exact Diffusion."""

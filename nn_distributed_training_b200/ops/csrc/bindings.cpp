@@ -126,6 +126,7 @@ struct ConsensusOp {
   consensus::BeerArgs<T> be{};
   consensus::KgtArgs<T> kg{};
   consensus::DetagArgs<T> dt{};
+  consensus::HsgdArgs<T> hs{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -137,7 +138,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -161,6 +162,8 @@ struct ConsensusOp {
     kg.K = geti(d, "local_steps", 1); kg.correction = geti(d, "correction", 1);
     dt.omega = ptr<const T>(d, "omega"); dt.ymix = ptr<T>(d, "ymix"); dt.g_old = ptr<T>(d, "g_old");
     dt.K = geti(d, "gossip_steps", 0);
+    hs.grad_part_prev = ptr<const T>(d, "grad_part_prev"); hs.v = ptr<T>(d, "hsgd_v"); hs.theta_prev = ptr<T>(d, "theta_prev");
+    hs.omb = (T)getf(d, "omb", 0.0);
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -250,6 +253,12 @@ struct ConsensusOp {
   void detag_track() {
     detag_check("detag_track");
     check(consensus::launch_detag_track<T>(dt, cur_stream()), "detag_track");
+  }
+  void hsgd_track() {
+    if (hs.grad_part_prev == nullptr || hs.v == nullptr || hs.theta_prev == nullptr || c.C != 2)
+      throw std::runtime_error("hsgd_track needs the prev-point partials `grad_part_prev`, the rows `hsgd_v` and "
+                               "`theta_prev` and two published channels");
+    check(consensus::launch_hsgd_track<T>(hs, cur_stream()), "hsgd_track");
   }
   void dadaptive_mix() {
     if (!ad.tracking || ad.ut == nullptr || c.C != 2)
@@ -388,6 +397,7 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("kgt_step", &ConsensusOp<T>::kgt_step)
       .def("ag_gossip", &ConsensusOp<T>::ag_gossip)
       .def("detag_track", &ConsensusOp<T>::detag_track)
+      .def("hsgd_track", &ConsensusOp<T>::hsgd_track)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

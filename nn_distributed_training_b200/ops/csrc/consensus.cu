@@ -13,6 +13,7 @@
 //                                                          (top-k codes)   -> beer_topk_mix / beer_topk_step
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // DeTAG (no reference counterpart, optimizers/detag.py)                    -> K x ag_gossip / detag_track
+// GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
@@ -1294,6 +1295,98 @@ __global__ void __launch_bounds__(THREADS) detag_track_kernel(const DetagArgs<T>
   end_step(c, l, ri.k, true);
 }
 
+// ----------------------------------------------------------------- GT-HSGD ----
+// dsgt_track with the hybrid estimator in place of the gradient.  g and gp are the sums of the two partial sets (the
+// forward/backward at theta and the one at theta_prev, on the same minibatch):
+//   v' = g                        in round 0
+//      = g + (1 - beta) (v - gp)  otherwise
+//   y  = sum_j W_ij y_j + (v' - v);  v <- v';  theta_prev <- theta;  publish theta and y
+// Every store is after the pdl_wait.  That matters for theta_prev: the prev-point forward/backward, the launch
+// immediately before this one, reads it, and the wait is what orders this write after those reads (the PDL convention
+// of common.cuh).  The next round's prev-point launch is three launches later and sees the new row.
+template <int U, typename T>
+NNDT_DEVINL Pack<T> sum_prev_partials(const HsgdArgs<T>& a, int l, int i) {
+  // sum_partials over grad_part_prev: the same issue order and summation order s = 0, 1, 2, ...
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const T* gp = a.grad_part_prev + (size_t)l * c.S * c.n_pad + i;
+  Pack<T> q[U];
+#pragma unroll
+  for (int s = 0; s < U; ++s)
+    if (s < c.S) q[s] = ldv(gp + (size_t)s * c.n_pad);
+  Pack<T> g = q[0];
+#pragma unroll
+  for (int s = 1; s < U; ++s)
+    if (s < c.S) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) g.v[u] += q[s].v[u];
+    }
+  for (int s = U; s < c.S; ++s) {
+    const Pack<T> r = ldv(gp + (size_t)s * c.n_pad);
+#pragma unroll
+    for (int u = 0; u < N; ++u) g.v[u] += r.v[u];
+  }
+  return g;
+}
+
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) hsgd_track_kernel(const HsgdArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const bool first = ri.k == 0;
+  const T omb = a.omb;
+  const int deg = c.deg[ri.gid * c.L + l];
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const T* ys = pub_row(c, ri.par, 1, l);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> y;
+    if (c.sum_mode) {
+      const DPack<N> sy = network_sum(c, ri.par, 1, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) y.v[u] = (T)(sy.v[u] / (double)c.n_total);
+    } else {
+      y = ldv(ys + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) y.v[u] *= ws;
+      // for_neighbors<4> written out, as in dsgt_track
+      for (int e0 = 0; e0 < deg; e0 += 4) {
+        Pack<T> q[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (e0 + j < deg) q[j] = ldv(nbr_row(c, ri.gid, l, e0 + j, ri.par, 1) + i);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (e0 + j < deg) {
+            const T we = w[e0 + j];
+#pragma unroll
+            for (int u = 0; u < N; ++u) y.v[u] += we * q[j].v[u];
+          }
+      }
+    }
+    Pack<T> vn = sum_partials<U>(c, l, i);
+    const Pack<T> vo = ldv(a.v + row + i);
+    if (!first) {
+      const Pack<T> gp = sum_prev_partials<U>(a, l, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) vn.v[u] += omb * (vo.v[u] - gp.v[u]);
+    }
+#pragma unroll
+    for (int u = 0; u < N; ++u) y.v[u] += vn.v[u] - vo.v[u];
+    const Pack<T> th = ldv(c.theta + row + i);
+    stv(a.v + row + i, vn);
+    stv(a.theta_prev + row + i, th);
+    stv(pub_row(c, ri.par ^ 1, 1, l) + i, y);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+  }
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2384,6 +2477,10 @@ template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaSt
 template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st) {
   return launch_by_s(detag_track_kernel<T, 4>, detag_track_kernel<T, 8>, a.c, a, st);
 }
+template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaStream_t st) {
+  // 8-deep as detag_track (S > 8 runs the tail loop): with two partial sets the 16-deep fp32 variant spills
+  return launch_by_s(hsgd_track_kernel<T, 4>, hsgd_track_kernel<T, 8>, a.c, a, st);
+}
 
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
@@ -2505,6 +2602,7 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_kgt_step<T>(const KgtArgs<T>&, cudaStream_t);           \
   template cudaError_t launch_ag_gossip<T>(const DetagArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_detag_track<T>(const DetagArgs<T>&, cudaStream_t);      \
+  template cudaError_t launch_hsgd_track<T>(const HsgdArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

@@ -187,6 +187,19 @@ struct DetagArgs {
   int step, K;
 };
 
+// GT-HSGD (Xin, Khan, Kar 2021): gradient tracking with a hybrid variance-reduced estimator, optimizers/gt_hsgd.py.
+// The round is DSGT's (dsgt_mix first, channel 0 theta, channel 1 the tracker y) with a second forward/backward on
+// the same minibatch at theta_prev; hsgd_track sums both partial sets (`c.grad_part` at theta, `grad_part_prev` at
+// theta_prev, both with c.S rows per node), updates v and y, and stores theta_prev <- theta.
+template <typename T>
+struct HsgdArgs {
+  Common<T> c;
+  const T* grad_part_prev;         // [L, S, n_pad] partials of the forward/backward at theta_prev
+  T* v;                            // [L, n_pad] the estimator v of the previous round (zero at the start)
+  T* theta_prev;                   // [L, n_pad] the iterate of the previous round (theta^0 at the start)
+  T omb;                           // 1 - beta, rounded once to T
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -342,6 +355,7 @@ template <typename T> cudaError_t launch_kgt_mix(const KgtArgs<T>& a, cudaStream
 template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

@@ -41,7 +41,7 @@ def schedule_tables(opt, H: int):
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
                           "bridge", "powergossip"):
         alpha[:] = opt.alpha_table(H)
-    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive and DeTAG: a constant step
+    elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
@@ -153,7 +153,7 @@ class ConsensusEngine:
         # dadaptive with its second-moment tracker u~ (tracking) or without it
         kgt_corr = opt.alg_name == "kgt" and opt.correction
         ad_track = opt.alg_name == "dadaptive" and opt.tracking
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer", "detag") or kgt_corr or ad_track else 1
+        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer", "detag", "gt_hsgd") or kgt_corr or ad_track else 1
         # RelaySum publishes one message per neighbor: channel e of node i is its message for neighbor j_e
         self.relay = opt.alg_name == "relaysum"
         if self.relay:
@@ -174,6 +174,8 @@ class ConsensusEngine:
         # sequence tags count K per gradient round and the schedules hold K entries per gradient round
         self.detag = opt.alg_name == "detag"
         K = self.rounds_per_step = opt.gossip_steps if self.detag else 1
+        # GT-HSGD: DSGT's channels and mix, and a second set of gradient partials (theta_prev, the same minibatch)
+        self.hsgd = opt.alg_name == "gt_hsgd"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -219,7 +221,7 @@ class ConsensusEngine:
             self.pub[p0 & 1, 1, :L].copy_(opt.y)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
-        if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr:
+        if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr or self.hsgd:
             self.pub[k0 & 1, 1, :L].copy_(opt.y)
         if ad_track:
             self.pub[k0 & 1, 1, :L].copy_(opt.ut)
@@ -454,6 +456,12 @@ class ConsensusEngine:
         if opt.alg_name == "dsgt":
             d.update(g_old=opt.g.data_ptr(), own_tracker=int(bool(getattr(opt, "own_tracker_step", False))),
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
+        if self.hsgd:
+            # the prev-point partials: the fused problem's second op, or (autograd gradients) the optimizer's grad_prev,
+            # one row per node as a.grad
+            gpp = pr.fused.grad_part_prev if pr.fused is not None else opt.grad_prev
+            d.update(grad_part_prev=gpp.data_ptr(), hsgd_v=opt.v.data_ptr(), theta_prev=opt.theta_prev.data_ptr(),
+                     omb=opt.omb)
         if opt.alg_name == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
         if opt.alg_name == "kgt":
@@ -551,7 +559,7 @@ class ConsensusEngine:
         ``sum m + biases`` (phase 0) or ``sum n + biases`` (phase 1) elements (unpadded): ``pulled_phase0`` and
         ``pulled_phase1`` report both, ``pulled`` their mean, and ``row`` is the padded message row.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
         neighbor wrote for it: the pulled bytes are DSGD's.  A DeTAG round gossips ``gossip_steps`` times, each a DSGT
-        pull: ``pulled`` counts them all."""
+        pull: ``pulled`` counts them all.  A GT-HSGD round exchanges what a DSGT round does."""
         deg = int(self.t_deg[0].sum().item())
         if self.pg:
             lay, itemsize = self.opt.lay, self.pub.element_size()

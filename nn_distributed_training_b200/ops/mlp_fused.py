@@ -117,6 +117,20 @@ class FusedMLP:
         self.train_op = self.ext.MlpOp(d)
         self._fwd = MlpForward(a, self.spec, self.L, dev)
         self.host_feed = None
+        self.prev_op = None
+
+    def enable_prev_point(self, theta_prev: torch.Tensor):
+        """Build the prev-point op (GT-HSGD): the training kernel on ``theta_prev`` (``[L, n_pad]``, kept at this
+        address) with its own partials.  It reads the same draw counters ``calls`` as the training op, which the
+        consensus step advances after both launches, so it draws the same minibatch.  It leaves the loss EMA alone."""
+        assert theta_prev.shape == self.pr.arena.theta.shape and theta_prev.dtype == self.dtype
+        self.theta_prev = theta_prev
+        self.grad_part_prev = torch.zeros_like(self.grad_part)
+        self.loss_part_prev = torch.zeros_like(self.loss_part)
+        d = dict(self.base)
+        d.update(theta=theta_prev.data_ptr(), grad_part=self.grad_part_prev.data_ptr(),
+                 loss_part=self.loss_part_prev.data_ptr())
+        self.prev_op = self.ext.MlpOp(d)
 
     WIN_MAX = 64
 
@@ -154,9 +168,25 @@ class FusedMLP:
             # device-side EMA of the training loss (capturable: no host sync)
             self.pr._ema_update(self.pr.tloss_local, self.loss_part.sum(1))
 
-    def compute_grads(self) -> torch.Tensor:
-        pr = self.pr
+    def launch_prev(self):
+        """Enqueue the prev-point fwd+bwd on the batch of the last ``launch`` (graph-capturable)."""
+        self.prev_op.train()
+
+    def compute_grads_pair(self, theta_prev: torch.Tensor, grad_prev: torch.Tensor) -> torch.Tensor:
+        """Eager API of ``ConsensusProblem.compute_grads_pair``: both launches on one draw, then ``compute_grads``'s
+        bookkeeping once."""
+        assert self.prev_op is not None and theta_prev.data_ptr() == self.theta_prev.data_ptr()
         self.launch()
+        self.launch_prev()
+        torch.sum(self.grad_part_prev, dim=1, out=grad_prev)
+        return self._collect_grads()
+
+    def compute_grads(self) -> torch.Tensor:
+        self.launch()
+        return self._collect_grads()
+
+    def _collect_grads(self) -> torch.Tensor:
+        pr = self.pr
         torch.sum(self.grad_part, dim=1, out=pr.arena.grad)
         self.calls += 1
         pr.count_draws_all(1)

@@ -113,6 +113,56 @@ class FusedMnist:
         self.train_op = self.ext.MnistOp(self.base)
         self._setup_eval()
         self.host_feed = None
+        self.prev_op = None
+        self.direct_prev_ops = []
+
+    # ---- a second point on the same minibatch (GT-HSGD) ---------------------
+    def enable_prev_point(self, theta_prev: torch.Tensor):
+        """Build the prev-point op: the training kernel on ``theta_prev`` (``[L, n_pad]``, kept at this address) with
+        its own partials.  It draws the same minibatch as the training op because its draw counters (``calls_prev``,
+        ``arrive_prev``) are a twin that the kernel advances in lockstep and ``sync_calls_from_host`` sets from the same
+        host mirror.  It stores no loss into the host mirror."""
+        assert theta_prev.shape == self.pr.arena.theta.shape and theta_prev.dtype == self.dtype
+        self.theta_prev = theta_prev
+        self.calls_prev = torch.zeros_like(self.calls)
+        self.arrive_prev = torch.zeros_like(self.arrive)
+        self.grad_part_prev = torch.zeros_like(self.grad_part)
+        self.loss_part_prev = torch.zeros_like(self.loss_part)
+        d = dict(self.base)
+        d.pop("step_prof", None)
+        d.update(theta=theta_prev.data_ptr(), calls=self.calls_prev.data_ptr(), arrive=self.arrive_prev.data_ptr(),
+                 grad_part=self.grad_part_prev.data_ptr(), loss_part=self.loss_part_prev.data_ptr())
+        if self.tc:
+            a = self.pr.arena
+            off_w1 = self.base["off_w1"]
+            d.update(w1_map=self.ext.make_w1_tensor_map(theta_prev.data_ptr(), a.n_pad, self.L, off_w1))
+        self.base_prev = d
+        self.prev_op = self.ext.MnistOp(d)
+        self.sync_calls_from_host()
+        if self.host_feed is not None:
+            self._build_direct_prev_ops()
+
+    def _build_direct_prev_ops(self):
+        # the prev-point twins of the direct ops of step 0: the same stage slot, so the same staged minibatch
+        self.direct_prev_ops = []
+        for b in range(2):
+            d = dict(self.base_prev)
+            d.update(direct=1, x=self.x_stage[b, 0].data_ptr(), y=self.y_stage[b, 0].data_ptr(),
+                     direct_bs=self.bs_stage[b, 0].data_ptr())
+            self.direct_prev_ops.append(self.ext.MnistOp(d))
+
+    def launch_prev(self):
+        """Enqueue the prev-point fwd+bwd on the batch the last ``launch`` drew (graph-capturable)."""
+        self.prev_op.train()
+
+    def compute_grads_pair(self, theta_prev: torch.Tensor, grad_prev: torch.Tensor) -> torch.Tensor:
+        """Eager API of ``ConsensusProblem.compute_grads_pair``: ``arena.grad`` at theta and ``grad_prev`` at the
+        prev-point op's ``theta_prev``, on one draw."""
+        assert self.prev_op is not None and theta_prev.data_ptr() == self.theta_prev.data_ptr()
+        self.launch()
+        self.launch_prev()
+        torch.sum(self.grad_part_prev, dim=1, out=grad_prev)
+        return self._collect_grads()
 
     # ---- training ---------------------------------------------------------
     def launch(self):
@@ -122,8 +172,11 @@ class FusedMnist:
 
     def compute_grads(self) -> torch.Tensor:
         """Eager API: fills ``arena.grad`` and advances the counters itself."""
-        pr = self.pr
         self.launch()
+        return self._collect_grads()
+
+    def _collect_grads(self) -> torch.Tensor:
+        pr = self.pr
         torch.sum(self.grad_part, dim=1, out=pr.arena.grad)
         pr.count_draws_all(1)
         pr.last_losses = self.loss_part.sum(1).to(self.dtype)
@@ -132,6 +185,8 @@ class FusedMnist:
     def sync_calls_from_host(self):
         pl = self.pr.placement
         self.calls.copy_(torch.as_tensor(self.pr.calls[pl.lo: pl.lo + pl.L].astype(np.int32)))
+        if self.prev_op is not None:
+            self.calls_prev.copy_(self.calls)
 
     # ---- host-fed batches (end-to-end input pipeline) -----------------------
     def enable_host_feed(self, steps_per_round: int, source: str):
@@ -193,6 +248,8 @@ class FusedMnist:
         self.host_feed = dict(P=P, mode="gpu_pull", source=source,
                               h2d_bytes=P * L * B * (784 * xb + 8) if source == "host" else 0,
                               d2h_bytes=L * self.S * 4 if source == "host" else 0)
+        if self.prev_op is not None:
+            self._build_direct_prev_ops()
         return self.host_feed
 
     # ---- validation ---------------------------------------------------------

@@ -17,6 +17,7 @@ A round is a short, fixed kernel sequence
     BRIDGE (trimmed mean / median screening):  bridge_mix, fwd/bwd, cg_step
     PowerGossip:  pg_mix, fwd/bwd, pg_step
     DeTAG:  ag_gossip(s) x gossip_steps, fwd/bwd, detag_track      (every ag_gossip a protocol round)
+    GT-HSGD:  dsgt_mix, fwd/bwd, fwd/bwd at theta_prev, hsgd_track   (both fwd/bwd on the same minibatch)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -44,12 +45,12 @@ def _nvtx(name):
     return torch.cuda.nvtx.range(name)
 
 
-def _round_ops(opt, eng, grads):
+def _round_ops(opt, eng, grads, grads_prev):
     with _nvtx(f"consensus_round/{opt.alg_name}"):
-        _round_ops_impl(opt, eng, grads)
+        _round_ops_impl(opt, eng, grads, grads_prev)
 
 
-def _round_ops_impl(opt, eng, grads):
+def _round_ops_impl(opt, eng, grads, grads_prev):
     alg = opt.alg_name
     if eng.sum_mode:
         eng.op.local_sum()   # complete graph: per-rank partial sums feeding the NVLS reduction
@@ -121,6 +122,11 @@ def _round_ops_impl(opt, eng, grads):
             eng.op.ag_gossip(s)
         grads(0)
         eng.op.detag_track()
+    elif alg == "gt_hsgd":
+        eng.op.dsgt_mix()
+        grads(0)
+        grads_prev()
+        eng.op.hsgd_track()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -217,16 +223,32 @@ class RoundProgram:
             return n + 4
         if self.opt.alg_name == "detag":
             return n + self.opt.gossip_steps + 2
+        if self.opt.alg_name == "gt_hsgd":
+            return n + 4
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
         pr = self.pr
         if pr.fused is None:
-            pr.compute_grads()
+            if self.opt.alg_name == "gt_hsgd":     # autograd: both points in one call (grads_prev has nothing left)
+                pr.compute_grads_pair(self.opt.theta_prev, self.opt.grad_prev)
+            else:
+                pr.compute_grads()
         elif self.host_mode:
             pr.fused.direct_ops[self._stage_set][p].train()
         else:
             pr.fused.launch()
+
+    def grads_prev(self):
+        """GT-HSGD's second forward/backward, at theta_prev on the minibatch ``grads(0)`` just drew: the prev-point op,
+        or the direct one of the current stage set."""
+        pr = self.pr
+        if pr.fused is None:
+            return
+        if self.host_mode:
+            pr.fused.direct_prev_ops[self._stage_set].train()
+        else:
+            pr.fused.launch_prev()
 
     def _count(self, rounds: int):
         """Host mirror of the device-side draw counters."""
@@ -263,7 +285,7 @@ class RoundProgram:
                 with torch.cuda.stream(side):
                     fz.gather_ops[b ^ 1].launch()
                 self._stage_set = b
-                _round_ops(self.opt, self.eng, self.grads)
+                _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
                 main.wait_stream(side)     # round i+1 consumes what was just staged (also joins the fork)
         return g
 
@@ -297,7 +319,7 @@ class RoundProgram:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads)
+                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
             self._graphs[r] = g
         return g
 
@@ -333,7 +355,7 @@ class RoundProgram:
                 self._resident_graph(r).replay()
             else:
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads)
+                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
             self._count(r)
             left -= r
 
@@ -341,7 +363,7 @@ class RoundProgram:
         """Mirror device-resident optimizer state into the optimizer object."""
         opt, eng = self.opt, self.eng
         L = self.pr.placement.L
-        if opt.alg_name == "dsgt":
+        if opt.alg_name in ("dsgt", "gt_hsgd"):    # GT-HSGD's v and theta_prev are the optimizer's own rows
             par = opt.k & 1
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name == "kgt" and opt.correction:      # c is the optimizer's own row; d is dead between rounds

@@ -9,6 +9,7 @@ from .dsgd import DSGD
 from .dsgdm import DSGDm
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
+from .gt_hsgd import GTHSGD
 from .kgt import KGT
 from .powergossip import PowerGossip
 from .push_diging import PushDIGing
@@ -18,7 +19,8 @@ from .sgp import SGP
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
-              "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG}
+              "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
+              "gt_hsgd": GTHSGD}
 
 
 def build_optimizer(problem, device, opt_conf):

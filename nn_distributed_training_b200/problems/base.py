@@ -189,6 +189,36 @@ class ConsensusProblem:
                 self._count_draw(g)
         return self.last_losses
 
+    def compute_grads_pair(self, theta_prev: torch.Tensor, grad_prev: torch.Tensor) -> torch.Tensor:
+        """``compute_grads`` plus the gradient at a second point on the *same* minibatch: ``arena.grad`` at theta and
+        ``grad_prev`` at ``theta_prev`` (both ``[L, n_pad]``).  One draw per node: the draw counters, ``forward_cnt``
+        and the losses (of the current point) advance once, as for ``compute_grads``.  Returns the ``[L]`` losses at
+        theta."""
+        if self.fused is not None:
+            return self.fused.compute_grads_pair(theta_prev, grad_prev)
+        for l, g in enumerate(self.placement.local_nodes):
+            model = self.models[g]
+            x, y = self._batch(g)
+            loss = self._loss(model, x, y)
+            self._after_loss(g, loss)
+            self.arena.set_row_from_grads(l, torch.autograd.grad(loss, list(model.parameters())))
+            self.last_losses[l] = loss.detach()
+            # the same network at theta_prev on the same batch: leaves viewing the row, through functional_call; the
+            # loss hook (_after_loss) sees the current point only
+            prev = [p.detach().requires_grad_(True) for p in self.layout.views(theta_prev[l])]
+            params = {s.name: p for s, p in zip(self.layout.slots, prev)}
+
+            def at_prev(inp, model=model, params=params):
+                return torch.func.functional_call(model, params, (inp,))
+            at_prev.parameters = lambda prev=prev: iter(prev)     # what a loss hook may inspect on a NaN
+            loss_p = self._loss(at_prev, x, y)
+            for dst, t in zip(self.layout.views(grad_prev[l]), torch.autograd.grad(loss_p, prev)):
+                dst.copy_(t)
+        for g in range(self.N):
+            if not self.placement.is_local(g):
+                self._count_draw(g)
+        return self.last_losses
+
     # ------------------------------------------------------------------
     # graph
     # ------------------------------------------------------------------

@@ -20,7 +20,7 @@ from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VAR
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -61,6 +61,8 @@ OPT_SCHEMA = {
     "powergossip": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "outer_iterations": REQUIRED, "profile": False},
     "detag": {"alpha": REQUIRED, "gossip_steps": REQUIRED, "accelerate": True, "outer_iterations": REQUIRED,
               "profile": False},
+    "gt_hsgd": {"alpha": REQUIRED, "beta": REQUIRED, "outer_iterations": REQUIRED, "update_graph": True,
+                "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -163,6 +165,21 @@ def _check_detag(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.accelerate must be true or false (got {c['accelerate']!r})")
 
 
+GT_HSGD_KEYS = ("alg_name", "alpha", "beta", "outer_iterations", "update_graph", "profile")
+
+
+def _check_gt_hsgd(c: Dict[str, Any], path: str) -> None:
+    """GT-HSGD: the step ``alpha`` (finite, > 0), the mixing weight ``beta`` (finite, in (0, 1]) and no other key."""
+    for key in c:
+        if key not in GT_HSGD_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: gt_hsgd takes no key {key!r} (its keys are alpha, beta, outer_iterations "
+                              f"and update_graph)")
+    if not _real(c["alpha"]) or not (math.isfinite(float(c["alpha"])) and float(c["alpha"]) > 0.0):
+        raise ConfigError(f"{path}.alpha must be finite and > 0 (got {c['alpha']!r})")
+    if not _real(c["beta"]) or not (math.isfinite(float(c["beta"])) and 0.0 < float(c["beta"]) <= 1.0):
+        raise ConfigError(f"{path}.beta must be finite and in (0, 1] (got {c['beta']!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -215,7 +232,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge", "powergossip", "detag")
+                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -267,6 +284,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_powergossip(c, path)
     if alg == "detag":
         _check_detag(c, path)
+    if alg == "gt_hsgd":
+        _check_gt_hsgd(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
