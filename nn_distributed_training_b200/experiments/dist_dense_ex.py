@@ -73,7 +73,8 @@ def experiment(yaml_pth):
         if prob_conf["optimizer_config"]["alg_name"] not in ("dinno", "dsgt", "dsgd", "dsgdm", "exact_diffusion", "choco_sgd",
                                                              "beer", "sgp", "push_diging", "kgt",
                                                              "clipped_gossip", "dadaptive", "relaysum",
-                                                             "bridge", "powergossip", "detag", "gt_hsgd"):
+                                                             "bridge", "powergossip", "detag", "gt_hsgd",
+                                                             "gossip_pga"):
             raise NameError("Unknown distributed opt algorithm.")
         prob = DistDensityProblem(graph, base_model, base_loss, train_subsets, val_set, ctx.device, prob_conf,
                                   ctx=ctx, seed=int(exp_conf.get("seed", 0)))

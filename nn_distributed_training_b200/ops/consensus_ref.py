@@ -94,6 +94,17 @@ def dsgt_track(y_all: torch.Tensor, w_rows: torch.Tensor, g_new: torch.Tensor, g
     return w_rows.to(y_all.dtype) @ y_all + g_new - g_old
 
 
+# ----------------------------------------------------------- Gossip-PGA ----
+def pga_mean_(theta: torch.Tensor, theta_all: torch.Tensor) -> None:
+    """The global round's mix of Gossip-PGA: every local row of ``theta`` becomes the mean of all N rows of
+    ``theta_all``, accumulated in float64 in node order and cast once to the arena dtype (the fused ``pga_mix`` on one
+    GPU computes the same bits)."""
+    s = torch.zeros(theta_all.shape[1], dtype=torch.float64, device=theta_all.device)
+    for j in range(theta_all.shape[0]):
+        s += theta_all[j].double()
+    theta.copy_((s / theta_all.shape[0]).to(theta.dtype).expand_as(theta))
+
+
 # ---------------------------------------------------------------- DeTAG ----
 def mixing_lambda(W: np.ndarray) -> float:
     """``max |eig(W - 11^T / N)|`` of a symmetric mixing matrix, in float64 (0 for one node and the complete graph)."""

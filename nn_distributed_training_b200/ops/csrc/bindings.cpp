@@ -127,6 +127,7 @@ struct ConsensusOp {
   consensus::KgtArgs<T> kg{};
   consensus::DetagArgs<T> dt{};
   consensus::HsgdArgs<T> hs{};
+  consensus::PgaArgs<T> pa{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -138,7 +139,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -164,6 +165,7 @@ struct ConsensusOp {
     dt.K = geti(d, "gossip_steps", 0);
     hs.grad_part_prev = ptr<const T>(d, "grad_part_prev"); hs.v = ptr<T>(d, "hsgd_v"); hs.theta_prev = ptr<T>(d, "theta_prev");
     hs.omb = (T)getf(d, "omb", 0.0);
+    pa.period = geti(d, "period", 0); pa.gossip = geti(d, "gossip", 1);
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -259,6 +261,19 @@ struct ConsensusOp {
       throw std::runtime_error("hsgd_track needs the prev-point partials `grad_part_prev`, the rows `hsgd_v` and "
                                "`theta_prev` and two published channels");
     check(consensus::launch_hsgd_track<T>(hs, cur_stream()), "hsgd_track");
+  }
+  void pga_check(const char* what) const {
+    if (pa.period < 1 || c.sum_local == nullptr || c.sum_mode || c.C != 1 || c.n_total < 1)
+      throw std::runtime_error(std::string(what) + " needs `period` >= 1, the fp64 partial-sum buffer `sum_local`, "
+                               "`n_total`, the pointer-table neighbors and one published channel");
+  }
+  void pga_sum() {
+    pga_check("pga_sum");
+    check(consensus::launch_pga_sum<T>(pa, cur_stream()), "pga_sum");
+  }
+  void pga_mix() {
+    pga_check("pga_mix");
+    check(consensus::launch_pga_mix<T>(pa, cur_stream()), "pga_mix");
   }
   void dadaptive_mix() {
     if (!ad.tracking || ad.ut == nullptr || c.C != 2)
@@ -398,6 +413,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("ag_gossip", &ConsensusOp<T>::ag_gossip)
       .def("detag_track", &ConsensusOp<T>::detag_track)
       .def("hsgd_track", &ConsensusOp<T>::hsgd_track)
+      .def("pga_sum", &ConsensusOp<T>::pga_sum)
+      .def("pga_mix", &ConsensusOp<T>::pga_mix)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

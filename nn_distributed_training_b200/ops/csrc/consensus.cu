@@ -14,6 +14,7 @@
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // DeTAG (no reference counterpart, optimizers/detag.py)                    -> K x ag_gossip / detag_track
 // GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
+// Gossip-PGA / local SGD (no reference counterpart, optimizers/gossip_pga.py) -> pga_sum + pga_mix / dsgd_step
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
@@ -1387,6 +1388,92 @@ __global__ void __launch_bounds__(THREADS) hsgd_track_kernel(const HsgdArgs<T> a
   end_step(c, l, ri.k, true);
 }
 
+// ------------------------------------------------------------- Gossip-PGA ----
+// Round k: pga_sum, pga_mix, fwd/bwd, dsgd_step (DSGD's, unchanged).  Global round (k mod period == period - 1):
+// pga_sum reduces this rank's published rows of round k into its fp64 partial, as local_sum_kernel does, and posts the
+// sum flag k + 1; pga_mix waits for every rank's partial and writes the network mean into theta, as dsgd_mix_kernel's
+// complete-graph mode does.  Gossip round: pga_sum returns at once and pga_mix is dsgd_mix_kernel's pointer-table mix
+// (gossip) or leaves theta as it is (local SGD).
+// pga_sum's grid is one CTA per THREADS vectors of the row, far from filling the SMs, so it asks for one resident CTA
+// per SM: with the default bound the fp64 variant spilled 4 bytes (96 registers without the bound's pressure).
+template <typename T>
+__global__ void __launch_bounds__(THREADS, 1) pga_sum_kernel(const PgaArgs<T> a) {
+  const Common<T>& c = a.c;
+  pdl_wait();
+  pdl_launch_dependents();
+  const RoundInfo<T> ri = round_info(c);
+  const PgaPhase ph = pga_phase(ri.k, a.period);
+  if (!ph.global) return;
+  constexpr int N = Vec<T>::N;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    double s[N];
+#pragma unroll
+    for (int u = 0; u < N; ++u) s[u] = 0.0;
+    for (int l = 0; l < c.L; ++l) {
+      const Pack<T> q = ldv(pub_row(c, ri.par, 0, l) + i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) s[u] += (double)q.v[u];
+    }
+    double* dst = c.sum_local + (size_t)(ph.sum_par * c.C) * c.n_pad + i;
+#pragma unroll
+    for (int u = 0; u < N; u += 2) *reinterpret_cast<double2*>(dst + u) = make_double2(s[u], s[u + 1]);
+  }
+  // last block: tell every peer that this rank's partial sum of round k is ready
+  __shared__ bool is_last;
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) is_last = (atomicAdd(c.done_ctr, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (is_last) {
+    if (threadIdx.x == 0) *c.done_ctr = 0;
+    if (c.world > 1) {
+      __threadfence_system();
+      if ((int)threadIdx.x < c.world && (int)threadIdx.x != c.rank)
+        st_release_sys(reinterpret_cast<int*>(c.peer_sum_flag[threadIdx.x]), ri.k + 1);
+    }
+  }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(THREADS) pga_mix_kernel(const PgaArgs<T> a) {
+  const Common<T>& c = a.c;
+  pdl_wait();
+  pdl_launch_dependents();
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const size_t row = (size_t)l * c.n_pad;
+  const PgaPhase ph = pga_phase(ri.k, a.period);
+  if (ph.global) {     // theta_i <- the network mean of the rows published for round k
+    if (c.world > 1 && blockIdx.x == 0 && blockIdx.y == 0) announce_round(c, ri.k);
+    wait_all_sums(c, ri.k);
+    for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+      const DPack<N> sall = network_sum(c, ph.sum_par, 0, i);
+      Pack<T> th;
+#pragma unroll
+      for (int u = 0; u < N; ++u) th.v[u] = (T)(sall.v[u] / (double)c.n_total);
+      stv(c.theta + row + i, th);
+    }
+    return;
+  }
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);      // c.sum_mode is 0: the neighbor wait (none on the edgeless graph of local SGD)
+  if (!a.gossip) return;
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] *= ws;
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
+#pragma unroll
+                       for (int u = 0; u < N; ++u) th.v[u] += w[e] * q.v[u];
+                     });
+    stv(c.theta + row + i, th);
+  }
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2482,6 +2569,18 @@ template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaSt
   return launch_by_s(hsgd_track_kernel<T, 4>, hsgd_track_kernel<T, 8>, a.c, a, st);
 }
 
+// pga_sum covers the row once, one CTA per THREADS vectors, as local_sum; pga_mix is one wave, as dsgd_mix
+template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st) {
+  if (a.period < 1 || a.c.sum_local == nullptr || a.c.C != 1 || a.c.sum_mode) return cudaErrorInvalidValue;
+  const int per_block = THREADS * Vec<T>::N;
+  return launch_pdl(pga_sum_kernel<T>, dim3((a.c.n_pad + per_block - 1) / per_block), dim3(THREADS), 0, st, a);
+}
+template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st) {
+  if (a.period < 1 || a.c.sum_local == nullptr || a.c.C != 1 || a.c.sum_mode || a.c.n_total < 1)
+    return cudaErrorInvalidValue;
+  return launch_one_wave(pga_mix_kernel<T>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
 }
@@ -2603,6 +2702,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_ag_gossip<T>(const DetagArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_detag_track<T>(const DetagArgs<T>&, cudaStream_t);      \
   template cudaError_t launch_hsgd_track<T>(const HsgdArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_pga_sum<T>(const PgaArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_pga_mix<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

@@ -200,6 +200,20 @@ struct HsgdArgs {
   T omb;                           // 1 - beta, rounded once to T
 };
 
+// Gossip-PGA (Chen, Yuan, Zhang, Pan, Xu, Yin 2021), optimizers/gossip_pga.py: DSGD's single published channel, with
+// every `period`-th round (k mod period == period - 1) a global round that replaces the gossip mix with the exact
+// network mean.  The round is pga_sum, pga_mix, fwd/bwd, dsgd_step; the branch is taken on the device from the round
+// counter.  A global round reduces through the complete-graph fields of Common (sum_local, sum_mc, sum_flags,
+// peer_sum_flag, n_total) while c.sum_mode stays 0, so gossip rounds pull through the pointer table.  The partial-sum
+// buffer is indexed by the parity of the global round's count, (k / period) & 1 (consensus_device.cuh: pga_phase).
+// `gossip` = 0 is local SGD: a gossip round leaves theta as it is and pulls nothing.
+template <typename T>
+struct PgaArgs {
+  Common<T> c;
+  int period;                      // >= 1
+  int gossip;                      // 1 = Metropolis mix on gossip rounds, 0 = none (local SGD)
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -356,6 +370,8 @@ template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStrea
 template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

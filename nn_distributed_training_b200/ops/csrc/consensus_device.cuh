@@ -219,6 +219,23 @@ NNDT_DEVINL void wait_all_sums(const Common<T>& c, int k) {
   }
 }
 
+// ---- Gossip-PGA: round k is global when k mod period == period - 1 ----
+// `sum_par` is the parity of the partial-sum buffer of global round k: the parity of the global round's count
+// g = k / period, not of k.
+// Round parity is unsafe once global rounds are `period` apart: with an even period every global round lands on the
+// same parity, and a rank more than period - 1 gossip hops ahead could overwrite its partial of global round g + 1
+// while a far rank still reduces g (tests/test_protocol_model_pga.py finds that interleaving at period 2 on a 3-rank
+// path).  With the count's parity, a rank writes its partial of g + 2 into g's buffer only after its global round g + 1
+// waited for every rank's partial of g + 1, and each rank posts that partial only in round k_{g+1}, after every launch
+// of round k_g, which read g's buffer, has completed.  So no rank still reads g's buffer when it is overwritten: the
+// argument that makes the every-round complete-graph mode safe, applied to the global rounds alone.  The sum flags
+// carry k + 1 and only grow, so "flag >= k + 1" is the same test in both modes.
+struct PgaPhase { bool global; int sum_par; };
+NNDT_DEVINL PgaPhase pga_phase(int k, int period) {
+  const int g = k / period;
+  return {k - g * period == period - 1, g & 1};
+}
+
 template <int U, typename T>
 NNDT_DEVINL Pack<T> sum_partials(const Common<T>& c, int l, int i) {
   // all (up to U) partial loads are issued before the first add: one L2 round trip instead of S dependent ones;

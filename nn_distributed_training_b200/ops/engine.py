@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip"):
+                          "bridge", "powergossip", "gossip_pga"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
@@ -176,6 +176,12 @@ class ConsensusEngine:
         K = self.rounds_per_step = opt.gossip_steps if self.detag else 1
         # GT-HSGD: DSGT's channels and mix, and a second set of gradient partials (theta_prev, the same minibatch)
         self.hsgd = opt.alg_name == "gt_hsgd"
+        # Gossip-PGA: DSGD's channel and pointer-table mix on gossip rounds, and the fp64 partial sums of the
+        # complete-graph mode on global rounds (sum_mode stays 0).  Local SGD (gossip: false) plans the edgeless graph
+        self.pga = opt.alg_name == "gossip_pga"
+        if self.pga and not opt.gossip:
+            edgeless = opt.edgeless_graph()
+            graphs_per_round = [edgeless] * len(graphs_per_round)
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -389,23 +395,27 @@ class ConsensusEngine:
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
                          and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag)
+                                  or self.detag or self.pga)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
-        if self.sum_mode:
+        if self.sum_mode or self.pga:
             self.sum_buf = SymmetricBuffer((2, self.C, n_pad), torch.float64, ctx)   # fp64: S - N*theta cancels in fp32
             self.sum_flag_buf = SymmetricBuffer((max(ctx.world_size, 1),), torch.int32, ctx)
             self.sum_flag_buf.local.fill_(k0)
             if ctx.is_distributed:
                 if self.sum_buf.multicast_ptr:
                     sum_mc = self.sum_buf.multicast_ptr      # NVLS: one in-switch reduction per element
+                elif self.pga:
+                    raise ValueError("gossip_pga on more than one rank averages over NVLS (one in-switch reduction of "
+                                     "the fp64 partial sums per global round), and this fabric gives its symmetric "
+                                     "buffer no multicast mapping")
                 else:
                     self.sum_mode = False                    # no multicast mapping on this fabric: pointer table
                 torch.cuda.synchronize(dev)
                 ctx.barrier()
         peer_sum_flag = np.zeros(max(ctx.world_size, 1), dtype=np.int64)
-        if self.sum_mode:
+        if self.sum_mode or self.pga:
             for r in range(ctx.world_size):
                 peer_sum_flag[r] = self.sum_flag_buf.peer_ptrs[r] + 4 * ctx.rank
         self.t_peer_sum_flag = torch.as_tensor(peer_sum_flag, device=dev)
@@ -448,6 +458,10 @@ class ConsensusEngine:
         if self.sum_mode:
             d.update(sum_mode=1, n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
                      sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr())
+        if self.pga:
+            d.update(n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
+                     sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr(),
+                     period=opt.period, gossip=int(opt.gossip))
         if opt.alg_name == "dinno":
             d.update(dual=opt.duals.data_ptr(), delta=opt.delta.data_ptr(),
                      m=None if opt.m is None else opt.m.data_ptr(),
@@ -559,8 +573,14 @@ class ConsensusEngine:
         ``sum m + biases`` (phase 0) or ``sum n + biases`` (phase 1) elements (unpadded): ``pulled_phase0`` and
         ``pulled_phase1`` report both, ``pulled`` their mean, and ``row`` is the padded message row.  A RelaySum node publishes one message row per neighbor (``row`` counts one) and pulls the one its
         neighbor wrote for it: the pulled bytes are DSGD's.  A DeTAG round gossips ``gossip_steps`` times, each a DSGT
-        pull: ``pulled`` counts them all.  A GT-HSGD round exchanges what a DSGT round does."""
+        pull: ``pulled`` counts them all.  A GT-HSGD round exchanges what a DSGT round does.  A Gossip-PGA gossip round
+        pulls what a DSGD round does (nothing with ``gossip: false``: the edgeless graph); a global round pulls no row
+        and contributes one fp64 partial-sum row per rank (``global_row``, ``n_pad * 8`` bytes) to the NVLS
+        reduction, once every ``period`` rounds."""
         deg = int(self.t_deg[0].sum().item())
+        if self.pga:
+            return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,
+                    "global_row": int(self.pr.arena.n_pad) * 8, "period": int(self.opt.period)}
         if self.pg:
             lay, itemsize = self.opt.lay, self.pub.element_size()
             p0, p1 = (deg * lay.msg_len(ph) * itemsize for ph in (0, 1))

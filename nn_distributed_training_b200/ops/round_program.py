@@ -18,6 +18,7 @@ A round is a short, fixed kernel sequence
     PowerGossip:  pg_mix, fwd/bwd, pg_step
     DeTAG:  ag_gossip(s) x gossip_steps, fwd/bwd, detag_track      (every ag_gossip a protocol round)
     GT-HSGD:  dsgt_mix, fwd/bwd, fwd/bwd at theta_prev, hsgd_track   (both fwd/bwd on the same minibatch)
+    Gossip-PGA:  pga_sum, pga_mix, fwd/bwd, dsgd_step             (pga_sum returns at once on gossip rounds)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -127,6 +128,11 @@ def _round_ops_impl(opt, eng, grads, grads_prev):
         grads(0)
         grads_prev()
         eng.op.hsgd_track()
+    elif alg == "gossip_pga":
+        eng.op.pga_sum()
+        eng.op.pga_mix()
+        grads(0)
+        eng.op.dsgd_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -223,7 +229,7 @@ class RoundProgram:
             return n + 4
         if self.opt.alg_name == "detag":
             return n + self.opt.gossip_steps + 2
-        if self.opt.alg_name == "gt_hsgd":
+        if self.opt.alg_name in ("gt_hsgd", "gossip_pga"):
             return n + 4
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
@@ -375,7 +381,7 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge", "powergossip") and opt.k > 0:
+                            "relaysum", "bridge", "powergossip", "gossip_pga") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))

@@ -9,6 +9,7 @@ from .dsgd import DSGD
 from .dsgdm import DSGDm
 from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
+from .gossip_pga import GossipPGA
 from .gt_hsgd import GTHSGD
 from .kgt import KGT
 from .powergossip import PowerGossip
@@ -20,7 +21,7 @@ ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
-              "gt_hsgd": GTHSGD}
+              "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA}
 
 
 def build_optimizer(problem, device, opt_conf):

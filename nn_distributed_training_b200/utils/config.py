@@ -20,7 +20,7 @@ from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VAR
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -63,6 +63,8 @@ OPT_SCHEMA = {
               "profile": False},
     "gt_hsgd": {"alpha": REQUIRED, "beta": REQUIRED, "outer_iterations": REQUIRED, "update_graph": True,
                 "profile": False},
+    "gossip_pga": {"alpha0": REQUIRED, "mu": 0.0, "period": REQUIRED, "gossip": True, "outer_iterations": REQUIRED,
+                   "update_graph": True, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -180,6 +182,26 @@ def _check_gt_hsgd(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.beta must be finite and in (0, 1] (got {c['beta']!r})")
 
 
+GOSSIP_PGA_KEYS = ("alg_name", "alpha0", "mu", "period", "gossip", "outer_iterations", "update_graph", "profile")
+
+
+def _check_gossip_pga(c: Dict[str, Any], path: str) -> None:
+    """Gossip-PGA: DSGD's step schedule (``alpha0`` and ``mu`` finite, >= 0), ``period`` (an integer >= 1), ``gossip``
+    (a bool) and no other key."""
+    for key in c:
+        if key not in GOSSIP_PGA_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: gossip_pga takes no key {key!r} (its keys are alpha0, mu, period, gossip, "
+                              f"outer_iterations and update_graph)")
+    for key in ("alpha0", "mu"):
+        if not _real(c[key]) or not (math.isfinite(float(c[key])) and float(c[key]) >= 0.0):
+            raise ConfigError(f"{path}.{key} must be finite and >= 0 (got {c[key]!r})")
+    p = c["period"]
+    if isinstance(p, bool) or not isinstance(p, int) or p < 1:
+        raise ConfigError(f"{path}.period must be an integer >= 1 (got {p!r})")
+    if not isinstance(c["gossip"], bool):
+        raise ConfigError(f"{path}.gossip must be true or false (got {c['gossip']!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -232,7 +254,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd")
+                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -286,6 +308,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_detag(c, path)
     if alg == "gt_hsgd":
         _check_gt_hsgd(c, path)
+    if alg == "gossip_pga":
+        _check_gossip_pga(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
