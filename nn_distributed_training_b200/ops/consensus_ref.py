@@ -765,6 +765,108 @@ def pdg_track_(y: torch.Tensor, g_old: torch.Tensor, ysum: torch.Tensor, grad: t
     g_old.copy_(grad)
 
 
+# ---------------------------------------------------------------- DP-DSGD ----
+# The noise stream (consensus.h: DpArgs): Philox4x32-10, key (lo32(seed), hi32(seed) ^ DP_KEY_DOMAIN), counter
+# (element pair p, round k, a, b) with (a, b) = (i, DP_LOCAL) for node i's own stream and (min(i, j), max(i, j)) for
+# edge {i, j}.  One call gives the normals of elements 2p and 2p + 1 by Box-Muller in float64.
+DP_KEY_DOMAIN = 0x44505347          # "DPSG": the DP key never equals the problem seed's plain Philox key
+DP_LOCAL = 0xFFFFFFFF               # b of a node's own stream (no node id is 2^32 - 1)
+_PHILOX_M = (np.uint64(0xD2511F53), np.uint64(0xCD9E8D57))
+_PHILOX_W = (0x9E3779B9, 0xBB67AE85)
+_M32 = np.uint64(0xFFFFFFFF)
+
+
+def philox4x32_10(ctr, key) -> np.ndarray:
+    """Philox4x32-10 (Salmon, Moraes, Dror, Shaw, SC 2011; curand's ``curand_Philox4x32_10``) of the counters
+    ``ctr [..., 4]`` under ``key (k0, k1)``, vectorised over the leading axes: ``[..., 4]`` uint32."""
+    c = [np.asarray(x, dtype=np.uint64) & _M32 for x in np.moveaxis(np.asarray(ctr, dtype=np.uint64), -1, 0)]
+    k0, k1 = int(key[0]) & 0xFFFFFFFF, int(key[1]) & 0xFFFFFFFF
+    for r in range(10):
+        if r:
+            k0, k1 = (k0 + _PHILOX_W[0]) & 0xFFFFFFFF, (k1 + _PHILOX_W[1]) & 0xFFFFFFFF
+        p0, p1 = _PHILOX_M[0] * c[0], _PHILOX_M[1] * c[2]       # exact: 32 x 32 bits in uint64
+        c = [(p1 >> np.uint64(32)) ^ c[1] ^ np.uint64(k0), p1 & _M32, (p0 >> np.uint64(32)) ^ c[3] ^ np.uint64(k1),
+             p0 & _M32]
+    return np.stack(c, axis=-1).astype(np.uint32)
+
+
+def dp_key(seed: int) -> Tuple[int, int]:
+    """The 64-bit Philox key of the DP noise for ``noise_seed`` (any integer, taken mod 2^64)."""
+    s = int(seed) & 0xFFFFFFFFFFFFFFFF
+    return s & 0xFFFFFFFF, (s >> 32) ^ DP_KEY_DOMAIN
+
+
+def _cospi_sinpi(x: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+    """``(cos(pi x), sin(pi x))`` for x in [0, 2) a multiple of 2^-52: x = q / 2 + y exactly with |y| <= 1/4, so the
+    rounding of ``pi y`` stays below 1e-16 absolute."""
+    q = np.rint(2.0 * x)
+    y = x - 0.5 * q
+    c, s = np.cos(np.pi * y), np.sin(np.pi * y)
+    q = q.astype(np.int64) & 3
+    cs = np.select([q == 0, q == 1, q == 2], [c, -s, -c], s)
+    sn = np.select([q == 0, q == 1, q == 2], [s, c, -s], -c)
+    return cs, sn
+
+
+def dp_normals(key, k: int, a: int, b: int, n_pad: int) -> np.ndarray:
+    """The ``[n_pad]`` float64 standard normals of stream ``(a, b)`` in round k (before the live mask)."""
+    p = np.arange(n_pad // 2, dtype=np.uint64)
+    ctr = np.stack([p, np.full_like(p, k), np.full_like(p, a), np.full_like(p, b)], axis=-1)
+    x = philox4x32_10(ctr, key).astype(np.uint64)
+    u1 = (((x[:, 0] >> np.uint64(5)) << np.uint64(26)) + (x[:, 1] >> np.uint64(6)) + np.uint64(1)).astype(np.float64)
+    u2 = (((x[:, 2] >> np.uint64(5)) << np.uint64(26)) + (x[:, 3] >> np.uint64(6))).astype(np.float64)
+    u1 *= 2.0 ** -53
+    u2 *= 2.0 ** -53
+    r = np.sqrt(-2.0 * np.log(u1))
+    c, s = _cospi_sinpi(2.0 * u2)
+    out = np.empty(n_pad)
+    out[0::2], out[1::2] = r * c, r * s
+    return out
+
+
+def dp_noise(key, k: int, i: int, nbrs, n_pad: int, cz_dp: float, cz_pair: float, live: np.ndarray) -> np.ndarray:
+    """``v_i`` of round k in float64 (``[n_pad]``, 0 off the live elements): ``cz_dp xi_i + cz_pair sum_j s_ij xi_ij``
+    over the neighbors ``nbrs`` in table order, ``s_ij = +1`` if i < j else -1, with ``cz = C z`` rounded once.  The
+    kernel (dp_step_kernel) evaluates the same expression in the same order."""
+    v = np.zeros(n_pad)
+    if cz_dp != 0.0:
+        v = cz_dp * dp_normals(key, k, i, DP_LOCAL, n_pad)
+    if cz_pair != 0.0 and len(nbrs):
+        e = np.zeros(n_pad)
+        for j in nbrs:
+            xi = dp_normals(key, k, min(i, j), max(i, j), n_pad)
+            e = e + xi if i < j else e - xi
+        v = v + cz_pair * e
+    return np.where(live, v, 0.0)
+
+
+def dp_clip_factor(sumsq: float, clip: float) -> float:
+    """``min(1, C / ||g||)`` from ``||g||^2`` in float64 (1 when g = 0)."""
+    nrm = math.sqrt(sumsq)
+    return clip / nrm if nrm > clip else 1.0
+
+
+def dp_rho(W: np.ndarray, z_dp: float, z_pair: float) -> Tuple[np.ndarray, np.ndarray]:
+    """zCDP cost ``[N]`` of one round per node, (eavesdropper, any observer) (DESIGN §2.16): the noise of one coordinate
+    across nodes has covariance ``C^2 Sigma``, ``Sigma = z_dp^2 I + z_pair^2 Lap(G)``; replacing node i's shard moves
+    its row by at most ``2 C alpha``, so rho = 2 [Sigma^-1]_ii for an observer who sees every published row and knows no
+    pair secret, and 2 / z_dp^2 for one who knows them all.  ``W`` only gives the graph (its off-diagonal support)."""
+    N = W.shape[0]
+    if z_dp == 0.0:
+        inf = np.full(N, np.inf)
+        return inf, inf.copy()
+    A = ((W != 0) & ~np.eye(N, dtype=bool)).astype(np.float64)
+    lap = np.diag(A.sum(1)) - A
+    sigma = z_dp * z_dp * np.eye(N) + z_pair * z_pair * lap
+    return 2.0 * np.diag(np.linalg.inv(sigma)).copy(), np.full(N, 2.0 / (z_dp * z_dp))
+
+
+def dp_epsilon(rho, delta: float) -> float:
+    """(epsilon, delta)-DP of a rho-zCDP ledger, ``rho + 2 sqrt(rho ln(1/delta))``, the maximum over its nodes."""
+    rho = np.asarray(rho, dtype=np.float64)
+    return float(np.max(rho + 2.0 * np.sqrt(rho * math.log(1.0 / delta))))
+
+
 # ------------------------------------------------------------- metrics ----
 def consensus_error(theta_all: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Pairwise and to-mean distances of L2-normalised parameter rows

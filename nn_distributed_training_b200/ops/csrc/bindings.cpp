@@ -128,6 +128,7 @@ struct ConsensusOp {
   consensus::DetagArgs<T> dt{};
   consensus::HsgdArgs<T> hs{};
   consensus::PgaArgs<T> pa{};
+  consensus::DpArgs<T> dp{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -139,7 +140,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -166,6 +167,11 @@ struct ConsensusOp {
     hs.grad_part_prev = ptr<const T>(d, "grad_part_prev"); hs.v = ptr<T>(d, "hsgd_v"); hs.theta_prev = ptr<T>(d, "theta_prev");
     hs.omb = (T)getf(d, "omb", 0.0);
     pa.period = geti(d, "period", 0); pa.gossip = geti(d, "gossip", 1);
+    dp.norm_part = ptr<double>(d, "norm_part"); dp.pstride = geti(d, "pstride", 0);
+    dp.nbr_id = ptr<const int>(d, "nbr_id"); dp.live = ptr<const unsigned>(d, "live"); dp.node0 = geti(d, "node0", 0);
+    dp.clip = getf(d, "clip_norm", 0.0); dp.cz_dp = getf(d, "cz_dp", 0.0); dp.cz_pair = getf(d, "cz_pair", 0.0);
+    dp.key0 = d.contains("dp_key0") ? (unsigned)d["dp_key0"].cast<unsigned long long>() : 0u;
+    dp.key1 = d.contains("dp_key1") ? (unsigned)d["dp_key1"].cast<unsigned long long>() : 0u;
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -274,6 +280,21 @@ struct ConsensusOp {
   void pga_mix() {
     pga_check("pga_mix");
     check(consensus::launch_pga_mix<T>(pa, cur_stream()), "pga_mix");
+  }
+  void dp_check(const char* what) const {
+    if (dp.norm_part == nullptr || dp.pstride <= 0 || dp.nbr_id == nullptr || dp.live == nullptr || !(dp.clip > 0.0) ||
+        c.C != 1 || c.sum_mode)
+      throw std::runtime_error(std::string(what) + " needs the fp64 norm partials `norm_part` and `pstride`, the "
+                               "neighbor id table `nbr_id`, the `live` mask, `clip_norm` > 0, one published channel and "
+                               "the pointer-table neighbors");
+  }
+  void dp_norm() {
+    dp_check("dp_norm");
+    check(consensus::launch_dp_norm<T>(dp, cur_stream()), "dp_norm");
+  }
+  void dp_step() {
+    dp_check("dp_step");
+    check(consensus::launch_dp_step<T>(dp, cur_stream()), "dp_step");
   }
   void dadaptive_mix() {
     if (!ad.tracking || ad.ut == nullptr || c.C != 2)
@@ -415,6 +436,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("hsgd_track", &ConsensusOp<T>::hsgd_track)
       .def("pga_sum", &ConsensusOp<T>::pga_sum)
       .def("pga_mix", &ConsensusOp<T>::pga_mix)
+      .def("dp_norm", &ConsensusOp<T>::dp_norm)
+      .def("dp_step", &ConsensusOp<T>::dp_step)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

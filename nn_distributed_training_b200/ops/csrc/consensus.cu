@@ -15,6 +15,7 @@
 // DeTAG (no reference counterpart, optimizers/detag.py)                    -> K x ag_gossip / detag_track
 // GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
 // Gossip-PGA / local SGD (no reference counterpart, optimizers/gossip_pga.py) -> pga_sum + pga_mix / dsgd_step
+// DP-DSGD / DECOR (no reference counterpart, optimizers/dp_dsgd.py)        -> dsgd_mix / dp_norm + dp_step
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
@@ -1474,6 +1475,93 @@ __global__ void __launch_bounds__(THREADS) pga_mix_kernel(const PgaArgs<T> a) {
   }
 }
 
+// ---------------------------------------------------------------- DP-DSGD ----
+// Round k (stream and rules in consensus.h: DpArgs): dsgd_mix, fwd/bwd, dp_norm, dp_step.  The clip factor needs the
+// norm of the whole gradient row, which is spread over the CTAs of the node, so the norm takes a launch of its own:
+// dp_norm sums the partials as the step will and writes one fp64 partial of sum g^2 per fixed chunk of the row (the
+// partials do not depend on the one-wave grid, as cg_dist's), dp_step adds them in chunk order.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) dp_norm_kernel(const DpArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int nchunk = cg_chunks(c);
+  __shared__ double red[THREADS / 32];
+  for (int ch = blockIdx.x; ch < nchunk; ch += gridDim.x) {
+    const int i = (ch * THREADS + threadIdx.x) * N;
+    double s = 0.0;
+    if (i < c.n_pad) {
+      const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) s += (double)g.v[u] * (double)g.v[u];
+    }
+#pragma unroll
+    for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) red[warp] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      double t = red[0];
+#pragma unroll
+      for (int w = 1; w < THREADS / 32; ++w) t += red[w];
+      a.norm_part[(size_t)l * a.pstride + ch] = t;
+    }
+    __syncthreads();
+  }
+}
+
+// theta_i -= alpha_k (f_i g_i + v_i) and publish.  With no noise the step is f_i g_i rounded on its own, so f_i = 1 is
+// dsgd_step's arithmetic bit for bit.
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) dp_step_kernel(const DpArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const size_t row = (size_t)l * c.n_pad;
+  const int i0 = (blockIdx.x * THREADS + threadIdx.x) * N;
+  // theta was last written by dsgd_mix, three launches back: the first vector is loaded before the dependency wait
+  Pack<T> th0;
+  if (i0 < c.n_pad) th0 = ldv(c.theta + row + i0);
+  pdl_wait();
+  pdl_launch_dependents();
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  __shared__ double fsh;
+  if (threadIdx.x == 0) {
+    const double* np = a.norm_part + (size_t)l * a.pstride;
+    const int nchunk = cg_chunks(c);
+    double s = 0.0;
+    for (int ch = 0; ch < nchunk; ++ch) s += np[ch];
+    const double nrm = sqrt(s);
+    fsh = nrm > a.clip ? a.clip / nrm : 1.0;
+  }
+  __syncthreads();
+  const T f = (T)fsh;
+  const bool noisy = a.cz_dp != 0.0 || a.cz_pair != 0.0;
+  const int deg = c.deg[ri.gid * c.L + l];
+  const int* ids = a.nbr_id + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const unsigned me = (unsigned)(a.node0 + l);
+  for (int i = i0; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = i == i0 ? th0 : ldv(c.theta + row + i);
+    const Pack<T> g = sum_partials<U>(c, l, i);
+    Pack<T> u;
+#pragma unroll
+    for (int q = 0; q < N; ++q) u.v[q] = mul_rn(f, g.v[q]);
+    if (noisy) {
+      const Pack<T> v = dp_noise(a, ri.k, me, deg, ids, i);
+#pragma unroll
+      for (int q = 0; q < N; ++q) u.v[q] += v.v[q];
+    }
+#pragma unroll
+    for (int q = 0; q < N; ++q) th.v[q] -= alpha * u.v[q];
+    stv(c.theta + row + i, th);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+  }
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2581,6 +2669,20 @@ template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream
   return launch_one_wave(pga_mix_kernel<T>, a.c, a, st);
 }
 
+// dp_norm and dp_step: one wave each, the 8-deep partial sum beyond 4 partials (as sgp_step)
+template <typename T> static bool dp_ready(const DpArgs<T>& a) {
+  return a.norm_part != nullptr && a.pstride >= cg_chunks(a.c) && a.nbr_id != nullptr && a.live != nullptr &&
+         a.c.C == 1 && !a.c.sum_mode;
+}
+template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_t st) {
+  if (!dp_ready(a)) return cudaErrorInvalidValue;
+  return launch_by_s(dp_norm_kernel<T, 4>, dp_norm_kernel<T, 8>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_t st) {
+  if (!dp_ready(a)) return cudaErrorInvalidValue;
+  return launch_by_s(dp_step_kernel<T, 4>, dp_step_kernel<T, 8>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
 }
@@ -2704,6 +2806,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_hsgd_track<T>(const HsgdArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_pga_sum<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_pga_mix<T>(const PgaArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_dp_norm<T>(const DpArgs<T>&, cudaStream_t);             \
+  template cudaError_t launch_dp_step<T>(const DpArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

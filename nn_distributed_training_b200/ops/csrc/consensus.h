@@ -214,6 +214,29 @@ struct PgaArgs {
   int gossip;                      // 1 = Metropolis mix on gossip rounds, 0 = none (local SGD)
 };
 
+// DP-DSGD and DECOR (Allouah, Koloskova, El Mrini, Guerraoui, Jaggi 2024), optimizers/dp_dsgd.py: DSGD's single
+// published channel and mix (dsgd_mix_kernel through the pointer table), then the node-level clipped and noised step
+//   f_i = min(1, C / ||g_i||),  v_i = cz_dp xi_i + cz_pair sum_j s_ij xi_ij,  theta_i -= alpha_k (f_i g_i + v_i)
+// dp_norm writes one fp64 partial of sum g^2 per chunk of THREADS * (16 / sizeof(T)) elements (as cg_dist), dp_step
+// adds them in chunk order.  The normals come from Philox4x32-10 under `key` with the counter (element pair p, round k,
+// a, b): (a, b) = (node, kDpLocal) for the node's own stream and (min(i, j), max(i, j)) for edge {i, j}, so both ends
+// draw an edge's stream bit for bit; Box-Muller in fp64 gives elements 2p and 2p + 1 (ops/consensus_ref.py: dp_normals,
+// the host twin).  v is evaluated in fp64, 0 off the live elements, and rounded once to T.
+constexpr unsigned kDpLocal = 0xFFFFFFFFu;
+
+template <typename T>
+struct DpArgs {
+  Common<T> c;
+  double* norm_part;               // [L, pstride] partial sums of g^2, one per chunk
+  int pstride;                     // >= the chunk count of a row
+  const int* nbr_id;               // [G, L, dmax] global node id of each neighbor
+  const unsigned* live;            // [n_pad / 32] live-element bits
+  int node0;                       // global id of local node 0
+  double clip;                     // C
+  double cz_dp, cz_pair;           // C z_dp, C z_pair (both 0: no draw at all)
+  unsigned key0, key1;             // Philox key
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -372,6 +395,8 @@ template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cuda
 template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

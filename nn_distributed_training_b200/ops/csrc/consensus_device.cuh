@@ -1,5 +1,7 @@
 // Device-side helpers of the consensus kernels (consensus.cu).
 #pragma once
+#include <curand_philox4x32_x.h>
+
 #include "common.cuh"
 #include "consensus.h"
 
@@ -667,6 +669,53 @@ NNDT_DEVINL void topk_gather(const char* code, int k, int c0, int len, T* tile, 
 template <typename T>
 __host__ __device__ __forceinline__ int cg_chunks(const Common<T>& c) {
   return (c.n_pad + THREADS * Vec<T>::N - 1) / (THREADS * Vec<T>::N);
+}
+
+// ---- DP-DSGD (stream in consensus.h: DpArgs) ----
+// the standard normals of elements 2p and 2p + 1 of stream (a, b) in round k: u1 in (0, 1] and u2 in [0, 1) from 53
+// bits each, Box-Muller in fp64 (ops/consensus_ref.py: dp_normals)
+NNDT_DEVINL double2 dp_normal2(unsigned key0, unsigned key1, unsigned p, unsigned k, unsigned a, unsigned b) {
+  const uint4 x = curand_Philox4x32_10(make_uint4(p, k, a, b), make_uint2(key0, key1));
+  const double u1 = (double)(((unsigned long long)(x.x >> 5) << 26) + (x.y >> 6) + 1ull) * 0x1p-53;
+  const double u2 = (double)(((unsigned long long)(x.z >> 5) << 26) + (x.w >> 6)) * 0x1p-53;
+  const double r = sqrt(-2.0 * log(u1));
+  double s, c;
+  sincospi(2.0 * u2, &s, &c);
+  return make_double2(r * c, r * s);
+}
+
+// v of node `me` at the Vec<T>::N elements from i: cz_dp xi_me + cz_pair sum_e s_e xi_{me, ids[e]} in fp64, the
+// products rounded on their own as the host twin rounds them (ops/consensus_ref.py: dp_noise), 0 off the live elements,
+// rounded once to T
+template <typename T>
+NNDT_DEVINL Pack<T> dp_noise(const DpArgs<T>& a, int k, unsigned me, int deg, const int* ids, int i) {
+  constexpr int N = Vec<T>::N;
+  const unsigned lw = a.live[i >> 5];
+  Pack<T> out;
+#pragma unroll
+  for (int q = 0; q < N; q += 2) {
+    const unsigned p = (unsigned)(i >> 1) + (unsigned)(q >> 1);
+    double v0 = 0.0, v1 = 0.0;
+    if (a.cz_dp != 0.0) {
+      const double2 x = dp_normal2(a.key0, a.key1, p, (unsigned)k, me, kDpLocal);
+      v0 = __dmul_rn(a.cz_dp, x.x);
+      v1 = __dmul_rn(a.cz_dp, x.y);
+    }
+    if (a.cz_pair != 0.0 && deg > 0) {
+      double e0 = 0.0, e1 = 0.0;
+      for (int e = 0; e < deg; ++e) {
+        const unsigned j = (unsigned)ids[e];
+        const double2 x = dp_normal2(a.key0, a.key1, p, (unsigned)k, min(me, j), max(me, j));
+        if (me < j) { e0 += x.x; e1 += x.y; } else { e0 -= x.x; e1 -= x.y; }
+      }
+      v0 += __dmul_rn(a.cz_pair, e0);
+      v1 += __dmul_rn(a.cz_pair, e1);
+    }
+    const int b = (i & 31) + q;
+    out.v[q] = ((lw >> b) & 1u) ? (T)v0 : (T)0;
+    out.v[q + 1] = ((lw >> (b + 1)) & 1u) ? (T)v1 : (T)0;
+  }
+  return out;
 }
 
 // ---- SGP (layout in consensus.h) ----

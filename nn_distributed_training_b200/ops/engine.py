@@ -13,7 +13,7 @@ import numpy as np
 import torch
 
 from . import load_ext
-from .consensus_ref import CHOCO_CODE, choco_live_words, ed_weights
+from .consensus_ref import CHOCO_CODE, choco_live, choco_live_words, ed_weights
 from ..parallel.symm import SymmetricBuffer
 from ..utils.graph_generation import Topology
 
@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip", "gossip_pga"):
+                          "bridge", "powergossip", "gossip_pga", "dp_dsgd"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
@@ -182,6 +182,8 @@ class ConsensusEngine:
         if self.pga and not opt.gossip:
             edgeless = opt.edgeless_graph()
             graphs_per_round = [edgeless] * len(graphs_per_round)
+        # DP-DSGD: DSGD's channel and pointer-table mix, a clipped and noised step (dp_norm, dp_step)
+        self.dp = opt.alg_name == "dp_dsgd"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
@@ -260,6 +262,7 @@ class ConsensusEngine:
                 gi = by_object[id(g)] = key_to_id[t.key]
             gid[k] = gi
         gid = np.repeat(gid, K)
+        self.gid = gid
         self.topos = topos
         G = len(topos)
         if (self.choco or self.beer) and opt.compressor == "topk":
@@ -293,6 +296,9 @@ class ConsensusEngine:
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
         directed = any(t.directed for t in topos)
+        if self.dp and directed:
+            raise ValueError("dp_dsgd needs undirected graphs: a planned graph is directed (the pairwise noise of an edge "
+                             "cancels between its two ends)")
         rmax = max(1, max(t.max_readers for t in topos))
         check_wait_capacity(dmax, rmax if directed or G > 1 else 0)    # a static undirected graph has no second wait
         nbr_ptr = np.zeros((G, L, dmax, 2, self.C), dtype=np.int64)
@@ -395,7 +401,7 @@ class ConsensusEngine:
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
                          and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag or self.pga)
+                                  or self.detag or self.pga or self.dp)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -492,6 +498,7 @@ class ConsensusEngine:
             d.update(ad_m=opt.m.data_ptr(), ad_v=None if opt.v is None else opt.v.data_ptr(),
                      vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if ad_track else None, beta1=opt.beta1,
                      beta2=opt.beta2, ad_eps=opt.eps, adagrad=int(opt.adagrad), tracking=int(ad_track))
+        self.t_live = None
         self.dist_part = self.t_attack = self.t_nbr_byz = None
         if self.cg or self.bridge:         # BRIDGE's step is cg_step, with the same attack tables
             if self.cg:
@@ -533,10 +540,29 @@ class ConsensusEngine:
             d.update(pg_vec=opt.vec.data_ptr() if opt.vec.numel() else None, pg_seg=self.t_pg_seg.data_ptr(),
                      pg_sign=opt.sign.data_ptr(), pg_nseg=len(lay.segs), pg_P=lay.P, pg_Q=lay.Q, pg_B=lay.B,
                      pg_W=lay.width, gamma=float(opt.gamma), pg_grid=int(getattr(opt, "pg_grid", 0)))
+        self.norm_part = self.t_nbr_id = None
+        if self.dp:
+            # fp64 partials of sum g^2, one per chunk of THREADS * (16 / itemsize) elements (cg_dist's chunks); the
+            # global id of every neighbor slot (the edge streams); the live mask (no noise on padding and slot holes);
+            # and the zCDP cost of one round on each planned graph (the ledger of the fused path)
+            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+            self.norm_part = torch.zeros(L * pstride, dtype=torch.float64, device=dev)
+            nbr_id = np.zeros((G, L, dmax), dtype=np.int32)
+            for gi, t in enumerate(topos):
+                for l, g in enumerate(pl.local_nodes):
+                    for e, j in enumerate(t.neighbors_noself[g]):
+                        nbr_id[gi, l, e] = j
+            self.t_nbr_id = torch.as_tensor(nbr_id, device=dev)
+            live = choco_live(a.layout)
+            live = torch.cat([live, live.new_zeros(-n_pad % 32)])      # whole words: a row may be shorter than 32
+            self.t_live = choco_live_words(live).to(dev)
+            self.dp_rho = [opt.round_rho(t) for t in topos]
+            d.update(norm_part=self.norm_part.data_ptr(), pstride=pstride, nbr_id=self.t_nbr_id.data_ptr(),
+                     live=self.t_live.data_ptr(), node0=int(pl.lo), clip_norm=float(opt.clip), cz_dp=float(opt.cz_dp),
+                     cz_pair=float(opt.cz_pair), dp_key0=int(opt.key[0]), dp_key1=int(opt.key[1]))
         if opt.alg_name == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
-        self.t_live = None
         if self.choco:
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
@@ -576,7 +602,8 @@ class ConsensusEngine:
         pull: ``pulled`` counts them all.  A GT-HSGD round exchanges what a DSGT round does.  A Gossip-PGA gossip round
         pulls what a DSGD round does (nothing with ``gossip: false``: the edgeless graph); a global round pulls no row
         and contributes one fp64 partial-sum row per rank (``global_row``, ``n_pad * 8`` bytes) to the NVLS
-        reduction, once every ``period`` rounds."""
+        reduction, once every ``period`` rounds.  A DP-DSGD round pulls what a DSGD round does: the edge noise is
+        drawn on both ends, and the norm partials stay on the node."""
         deg = int(self.t_deg[0].sum().item())
         if self.pga:
             return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,

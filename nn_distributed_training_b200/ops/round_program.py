@@ -19,6 +19,7 @@ A round is a short, fixed kernel sequence
     DeTAG:  ag_gossip(s) x gossip_steps, fwd/bwd, detag_track      (every ag_gossip a protocol round)
     GT-HSGD:  dsgt_mix, fwd/bwd, fwd/bwd at theta_prev, hsgd_track   (both fwd/bwd on the same minibatch)
     Gossip-PGA:  pga_sum, pga_mix, fwd/bwd, dsgd_step             (pga_sum returns at once on gossip rounds)
+    DP-DSGD / DECOR:  dsgd_mix, fwd/bwd, dp_norm, dp_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -133,6 +134,11 @@ def _round_ops_impl(opt, eng, grads, grads_prev):
         eng.op.pga_mix()
         grads(0)
         eng.op.dsgd_step()
+    elif alg == "dp_dsgd":
+        eng.op.dsgd_mix()
+        grads(0)
+        eng.op.dp_norm()
+        eng.op.dp_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -229,7 +235,7 @@ class RoundProgram:
             return n + 4
         if self.opt.alg_name == "detag":
             return n + self.opt.gossip_steps + 2
-        if self.opt.alg_name in ("gt_hsgd", "gossip_pga"):
+        if self.opt.alg_name in ("gt_hsgd", "gossip_pga", "dp_dsgd"):
             return n + 4
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
@@ -352,6 +358,11 @@ class RoundProgram:
         if self.opt.k + rounds > self.eng.horizon:
             raise RuntimeError(f"rounds {self.opt.k}..{self.opt.k + rounds - 1} run past the schedule horizon of "
                                f"{self.eng.horizon} rounds")
+        if self.eng.dp:         # the privacy ledger follows the planned graph of every round run
+            for k in range(self.opt.k, self.opt.k + rounds):
+                eav, allo = self.eng.dp_rho[self.eng.gid[k]]
+                self.opt.rho_eav += eav
+                self.opt.rho_all += allo
         if self.host_mode:
             return self._run_pull_graphs(rounds)
         left = rounds
@@ -381,7 +392,7 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge", "powergossip", "gossip_pga") and opt.k > 0:
+                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))

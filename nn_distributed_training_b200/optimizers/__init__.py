@@ -5,6 +5,7 @@ from .choco import ChocoSGD
 from .dadaptive import DAdaptive
 from .detag import DeTAG
 from .dinno import DiNNO
+from .dp_dsgd import DPDSGD
 from .dsgd import DSGD
 from .dsgdm import DSGDm
 from .dsgt import DSGT
@@ -21,7 +22,7 @@ ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
-              "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA}
+              "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -115,6 +115,8 @@ class ConsensusOptimizer:
         if self.mixing_order == "reference" and self.pr.ctx.is_distributed:
             raise ValueError("reference (Gauss-Seidel) mixing order is a single-process oracle mode")
         self.checkpointer = None  # set by utils.checkpoint.attach
+        if isinstance(self.pr, ConsensusProblem):
+            self.pr.privacy_record = None   # a differentially private optimizer sets its own after this
 
     # -- helpers ---------------------------------------------------------
     @property

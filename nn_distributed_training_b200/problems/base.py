@@ -15,7 +15,7 @@ from __future__ import annotations
 
 import copy
 import os
-from typing import Dict, List, Optional, Sequence
+from typing import Callable, Dict, List, Optional, Sequence
 
 import networkx as nx
 import numpy as np
@@ -57,6 +57,9 @@ class ConsensusProblem:
 
     #: squeeze model output before the loss (density problems)
     squeeze_output = False
+    #: ``() -> dict`` of the optimizer training this problem when it is differentially private (optimizers/dp_dsgd.py),
+    #: written into the results file as ``privacy``; every optimizer resets it to None when it is built
+    privacy_record: Optional[Callable[[], dict]] = None
 
     def __init__(self, graph, base_model, base_loss, train_sets, val_set, device, conf,
                  ctx: Optional[DistContext] = None, backend: Optional[str] = None,
@@ -288,6 +291,8 @@ class ConsensusProblem:
         byz = self.conf.get("optimizer_config", {}).get("byzantine")
         if byz:
             out["byzantine_nodes"] = sorted(int(v) for v in byz["nodes"])   # summaries average the other nodes
+        if self.privacy_record is not None:
+            out["privacy"] = self.privacy_record()
         torch.save(out, path)
 
     def state_dicts(self) -> Dict[int, dict]:

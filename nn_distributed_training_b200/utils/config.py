@@ -20,7 +20,7 @@ from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VAR
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -65,6 +65,10 @@ OPT_SCHEMA = {
                 "profile": False},
     "gossip_pga": {"alpha0": REQUIRED, "mu": 0.0, "period": REQUIRED, "gossip": True, "outer_iterations": REQUIRED,
                    "update_graph": True, "profile": False},
+    # noise_seed defaults to the problem's seed (filled in by the optimizer, which knows it)
+    "dp_dsgd": {"alpha0": REQUIRED, "mu": 0.0, "clip_norm": REQUIRED, "noise_multiplier": REQUIRED,
+                "pair_noise_multiplier": 0.0, "target_delta": 1e-5, "outer_iterations": REQUIRED, "update_graph": True,
+                "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -202,6 +206,31 @@ def _check_gossip_pga(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.gossip must be true or false (got {c['gossip']!r})")
 
 
+DP_DSGD_KEYS = ("alg_name", "alpha0", "mu", "clip_norm", "noise_multiplier", "pair_noise_multiplier", "target_delta",
+                "noise_seed", "outer_iterations", "update_graph", "profile")
+
+
+def _check_dp_dsgd(c: Dict[str, Any], path: str) -> None:
+    """DP-DSGD: DSGD's step schedule (``alpha0`` and ``mu`` finite, >= 0), ``clip_norm`` (finite, > 0), the multipliers
+    (finite, >= 0), ``target_delta`` in (0, 1), an integer ``noise_seed`` and no other key.  ClippedGossip's ``clip`` and
+    ``delta`` mean something else and are refused here."""
+    for key in c:
+        if key not in DP_DSGD_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: dp_dsgd takes no key {key!r} (its keys are alpha0, mu, clip_norm, "
+                              f"noise_multiplier, pair_noise_multiplier, target_delta, noise_seed, outer_iterations and "
+                              f"update_graph)")
+    for key in ("alpha0", "mu", "noise_multiplier", "pair_noise_multiplier"):
+        if not _real(c[key]) or not (math.isfinite(float(c[key])) and float(c[key]) >= 0.0):
+            raise ConfigError(f"{path}.{key} must be finite and >= 0 (got {c[key]!r})")
+    if not _real(c["clip_norm"]) or not (math.isfinite(float(c["clip_norm"])) and float(c["clip_norm"]) > 0.0):
+        raise ConfigError(f"{path}.clip_norm must be finite and > 0 (got {c['clip_norm']!r})")
+    if not _real(c["target_delta"]) or not 0.0 < float(c["target_delta"]) < 1.0:
+        raise ConfigError(f"{path}.target_delta must be in (0, 1) (got {c['target_delta']!r})")
+    s = c.get("noise_seed", 0)
+    if isinstance(s, bool) or not isinstance(s, int):
+        raise ConfigError(f"{path}.noise_seed must be an integer (got {s!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -254,7 +283,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga")
+                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -310,6 +339,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_gt_hsgd(c, path)
     if alg == "gossip_pga":
         _check_gossip_pga(c, path)
+    if alg == "dp_dsgd":
+        _check_dp_dsgd(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
