@@ -48,7 +48,10 @@ class _FFNet(nn.Module):
             from ..ops import mlp_generic as mg
             acts = self._layer_acts()
             if mg.enabled() and mg.supported(self.shape, acts, x.dtype):
-                return mg.fused_mlp(x, [p for p in self.seq.parameters()], self.shape, acts)
+                params = list(self.seq.parameters())
+                if not mg.arguments_match(x, params, self.shape):
+                    return self.seq(x)          # a dtype, device or width mismatch: nn.Sequential's own error
+                return mg.fused_mlp(x, params, self.shape, acts)
             if not getattr(self, "_warned", False):
                 self._warned = True
                 print(f"[nndt] WARNING: {type(self).__name__}{self.shape} ({x.dtype}) runs nn.Sequential (cuBLAS) on CUDA: "

@@ -24,6 +24,14 @@ def supported(shape: Sequence[int], acts: Sequence[str], dtype) -> bool:
             and all(a in ACT for a in acts) and dtype in (torch.float32, torch.float64))
 
 
+def arguments_match(x: torch.Tensor, params: Sequence[torch.Tensor], shape: Sequence[int]) -> bool:
+    """The kernels read ``x`` and the parameters as raw ``x.dtype`` arrays on ``x``'s device, ``shape[0]`` values per
+    row: a parameter of another dtype or device, or a row of another width, would be read as garbage or out of bounds.
+    Callers run ``nn.Sequential`` instead, which raises its own error for the mismatch."""
+    return (x.shape[-1] == int(shape[0])
+            and all(p.dtype == x.dtype and p.device == x.device for p in params))
+
+
 def enabled() -> bool:
     return os.environ.get("NNDT_FUSED_MLP", "1") != "0"
 

@@ -5,7 +5,10 @@
 * ``convnet_fp64`` is ``MNISTConvNet`` in float64 autograd (``csrc/mnist_tc.cu`` and ``csrc/mnist_cl64.cu``); with
   ``tf32_fc1=True`` the operands of its three fc1-sized contractions are rounded to TF32 first, which is the error a
   1xTF32 kernel would make: the yardstick of the 3xTF32 kernel.  ``convnet_fp64_eval`` is the same forward per sample
-  (NLL and logits), the oracle of the evaluation kernels.
+  (NLL and logits), the oracle of the evaluation kernels.  ``convnet_tf32_point`` is the yardstick of the fp32
+  CUDA-core kernel: the oracle at the TF32 rounding of every parameter and of float rows.
+* ``mlp_fp64`` is the generic feed-forward net of ``csrc/mlp_generic.cu`` (forward, saved activations, backward) in
+  float64; its yardstick is the same function at the TF32 rounding of the parameters, the rows and dL/dout.
 * ``mlp_bf16_faithful`` is the density MLP of ``csrc/mlp_tc.cu`` written out by hand, rounding to bf16 exactly where
   the kernel rounds and nowhere else; ``rounding=False`` gives the exact math of the same network.
 * ``assert_close_to_oracle`` accepts a kernel when its error is a small fraction of a yardstick's error, per tensor and
@@ -90,6 +93,22 @@ def flatten(tensors, spec, n_pad: int) -> torch.Tensor:
     return out
 
 
+def poison_partials(fz, spec):
+    """NaN in every parameter slot of every slice's partial row of a ``FusedMnist`` and in every loss partial; the
+    arena padding between the slots stays as it is (zero: the training kernels never write it)."""
+    for o, s in slots(spec):
+        fz.grad_part[:, :, o: o + math.prod(s)] = float("nan")
+    fz.loss_part.fill_(float("nan"))
+
+
+def padding_mask(spec, n_pad, device):
+    """True on the arena padding of a row: the entries between (and after) the parameter slots."""
+    pad = torch.ones(n_pad, dtype=torch.bool, device=device)
+    for o, s in slots(spec):
+        pad[o: o + math.prod(s)] = False
+    return pad
+
+
 def batch_rows(shard_sizes, batch: int, seed: int, node: int, call: int, node0: int = 0) -> torch.Tensor:
     """Rows of the concatenated local shards that local node ``node`` draws at its ``call``-th draw: the Feistel
     schedule of ``data.sampler`` keyed by the global node id, plus the node's shard offset."""
@@ -169,6 +188,15 @@ def convnet_fp64(theta_row, spec, x, y, mean=0.0, std=1.0, tf32_fc1=False, dtype
     return loss.detach(), flatten([g.detach() for g in grads], spec, theta_row.shape[-1])
 
 
+def convnet_tf32_point(theta_row, spec, x, y, mean=0.0, std=1.0):
+    """Yardstick of the fp32 CUDA-core kernel ``convnet_generic_kernel<float, ...>``: ``convnet_fp64`` (with
+    ``pool_f32``) at the TF32 rounding of every parameter and of float rows.  ``tf32_fc1`` rounds only the fc1
+    contractions, so it leaves the fc2 and b2 gradients of a small net nearly exact (exact where every fc1 unit is
+    off), which no fp32 kernel can match; rounding every tensor perturbs every gradient."""
+    xr = x if x.dtype == torch.uint8 else round_tf32(x)
+    return convnet_fp64(round_tf32(theta_row), spec, xr, y, mean, std, pool_f32=True)
+
+
 def convnet_fp64_eval(theta_row, spec, x, y, mean=0.0, std=1.0, tf32_fc1=False, dtype=torch.float64):
     """Per-sample NLL ``[n]`` and logits ``[n, 10]`` of ``MNISTConvNet`` on rows ``x``, the forward of
     ``convnet_fp64``: what the evaluation kernels store per validation sample."""
@@ -245,14 +273,100 @@ def mlp_bf16_faithful(theta_row, spec, x, y, loss, rounding=True, accum=torch.fl
     return lrow.sum() / bs, flatten(grads, spec, theta_row.shape[-1]), p
 
 
+# ---- generic feed-forward net (FFReLUNet / FFTanhNet / FFSigmoidNet, csrc/mlp_generic.cu) -----------------------------
+def mlp_layout(shape):
+    """``[(w_off, b_off)]`` of every layer in the flat parameter vector of ``ops/mlp_generic.py``: W0, b0, W1, b1, ...
+    back to back in ``nn.Linear`` layout."""
+    out, off = [], 0
+    for l in range(len(shape) - 1):
+        out.append((off, off + shape[l + 1] * shape[l]))
+        off += shape[l + 1] * (shape[l] + 1)
+    return out
+
+
+def mlp_params(shape, seed=0):
+    """Flat float64 parameters of ``shape`` in the ``mlp_layout``, drawn like ``nn.Linear``'s defaults:
+    U(-1 / sqrt(d_in), 1 / sqrt(d_in))."""
+    g = torch.Generator().manual_seed(seed)
+    ps = []
+    for l in range(len(shape) - 1):
+        bound = shape[l] ** -0.5
+        ps += [(torch.rand(shape[l + 1] * (shape[l] + 1), generator=g, dtype=torch.float64) * 2 - 1) * bound]
+    return torch.cat(ps)
+
+
+def _act(z, a):
+    return {"none": lambda t: t, "relu": torch.relu, "tanh": torch.tanh, "sigmoid": torch.sigmoid}[a](z)
+
+
+def _act_deriv(y, a):
+    """The activation's derivative written through its output ``y``."""
+    if a == "relu":
+        return (y > 0).to(y.dtype)
+    if a == "tanh":
+        return 1 - y * y
+    if a == "sigmoid":
+        return y * (1 - y)
+    return torch.ones_like(y)
+
+
+def mlp_fp64(params, shape, acts, x, gout):
+    """Forward and backward of the feed-forward net ``shape`` with activations ``acts`` (one per layer) in float64,
+    written out by hand: the oracle of ``mlp_generic_forward_kernel`` / ``mlp_generic_backward_kernel``.
+
+    ``params`` is the flat vector of ``mlp_layout``, ``x`` is ``[M, shape[0]]`` and ``gout`` is ``dL/dout``
+    ``[M, shape[-1]]``.  Returns ``(out, [every layer's post-activation], flat parameter gradient, dx)``."""
+    shape = [int(s) for s in shape]
+    p = params.to(torch.float64)
+    h = [x.to(torch.float64)]
+    Ws, bs = [], []
+    for l, (wo, bo) in enumerate(mlp_layout(shape)):
+        Ws.append(p[wo: bo].reshape(shape[l + 1], shape[l]))
+        bs.append(p[bo: bo + shape[l + 1]])
+        h.append(_act(h[-1] @ Ws[-1].T + bs[-1], acts[l]))
+    g = torch.zeros_like(p)
+    d = gout.to(torch.float64) * _act_deriv(h[-1], acts[-1])
+    for l in reversed(range(len(Ws))):
+        wo, bo = mlp_layout(shape)[l]
+        g[wo: bo] = (d.T @ h[l]).reshape(-1)
+        g[bo: bo + shape[l + 1]] = d.sum(0)
+        d = d @ Ws[l]
+        if l > 0:
+            d = d * _act_deriv(h[l], acts[l - 1])
+    return h[-1], h[1:], g, d
+
+
+def mlp_named(shape, out, hs, g, dx=None):
+    """``{name: tensor}`` of what ``mlp_fp64`` returns (or a kernel computed), for ``assert_close_to_oracle``: the
+    output, every layer's post-activation ``a<l>``, every weight and bias gradient ``W<l>`` / ``b<l>`` and, unless
+    None, ``dx``; ``hs=None`` leaves the post-activations out."""
+    out_d = {"out": out.reshape(-1, int(shape[-1]))}
+    for l, (wo, bo) in enumerate(mlp_layout(shape)):
+        if hs is not None:
+            out_d[f"a{l}"] = hs[l].reshape(-1, int(shape[l + 1]))
+        out_d[f"W{l}"] = g[wo: bo].reshape(int(shape[l + 1]), int(shape[l]))
+        out_d[f"b{l}"] = g[bo: bo + int(shape[l + 1])]
+    if dx is not None:
+        out_d["dx"] = dx.reshape(-1, int(shape[0]))
+    return out_d
+
+
 # ---- acceptance ------------------------------------------------------------------------------------------------------
 # Fractions of the yardstick's error a kernel may make.  The 3xTF32 conv-net kernel measures at most 0.02 of the
 # 1xTF32 yardstick (H100, all three cluster instantiations).  The bf16 MLP training kernel measures at most 0.14 of
 # the faithful-vs-exact yardstick (per tensor and per block; H100): the SFU sine and exp and the fp32 tensor-core
 # accumulation move a small fraction of the bf16 roundings by one ulp.  A zeroed 16 x 8 tile, a missing 16-row
 # k-step or a stored-instead-of-added tile measures 9x or more (tests/test_kernel_oracles.py).
+#
+# The fp32 CUDA-core kernels (``convnet_generic_kernel<float, ...>``, ``mlp_generic_*_kernel<float>``) are held to
+# TF32_POINT_FRAC of the error the exact math makes at the TF32 rounding of its inputs (``convnet_tf32_point``, and
+# ``mlp_fp64`` at ``round_tf32`` of the parameters, the rows and dL/dout).  fp32 autograd measures at most 0.032
+# (conv net) and 0.009 (MLP) of it on CPU; a partial batch scaled by the wrong size, a dropped sample or a dropped
+# conv-gradient partition measure 200x or more, a 32-row CTA missing from a weight gradient 4.3x
+# (tests/test_kernel_oracles.py).
 CONVNET_FRAC = 0.1
 MLP_FRAC = 0.3
+TF32_POINT_FRAC = 0.1
 
 
 def _block_errors(d: torch.Tensor, block) -> torch.Tensor:

@@ -11,8 +11,6 @@ Both oracles take the max-pool argmax from the conv as an fp32 kernel evaluates 
 first batch of node 0 holds a pool window whose two largest conv outputs differ by 7e-8, less than fp32 resolves: the
 kernel, like fp32 autograd, routes that cell's gradient to the other position, and that alone puts the conv-weight
 gradient at 0.17x the yardstick's error when measured against the fp64 routing (tests/test_kernel_oracles.py)."""
-import math
-
 import networkx as nx
 import pytest
 import torch
@@ -47,31 +45,16 @@ def _problem(L, B, spb, float_rows):
     return pr
 
 
-def _poison_partials(fz, spec):
-    """NaN in every parameter slot of every slice's partial row and in every loss partial; the arena padding between
-    the slots stays as it is (zero: the kernel never writes it)."""
-    for o, s in ko.slots(spec):
-        fz.grad_part[:, :, o: o + math.prod(s)] = float("nan")
-    fz.loss_part.fill_(float("nan"))
-
-
-def _padding_mask(spec, n_pad):
-    pad = torch.ones(n_pad, dtype=torch.bool, device=DEV)
-    for o, s in ko.slots(spec):
-        pad[o: o + math.prod(s)] = False
-    return pad
-
-
 def _run_and_compare(L, B, spb, float_rows, steps=3):
     pr = _problem(L, B, spb, float_rows)
     fz, spec = pr.fused, pr.base_model.spec
     assert not fz.tc and not fz.generic and fz.spb == spb and fz.S == -(-B // spb)
     mean, std = pr.shards.norm if pr.shards.norm is not None else (0.0, 1.0)
-    pad = _padding_mask(spec, fz.n_pad)
+    pad = ko.padding_mask(spec, fz.n_pad, DEV)
     worst = {}
     for step in range(steps):               # full batch, partial batch, first batch of the next epoch
         calls = pr.calls.copy()
-        _poison_partials(fz, spec)
+        ko.poison_partials(fz, spec)
         loss = fz.compute_grads().clone()
         assert not fz.grad_part[:, :, pad].any(), "the kernel wrote the arena padding"
         assert torch.isfinite(fz.loss_part).all(), "a slice left its loss partial unwritten"

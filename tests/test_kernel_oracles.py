@@ -266,3 +266,235 @@ def test_fp32_references_turns_tf32_off_and_restores_it():
         assert torch.backends.cudnn.allow_tf32 and torch.backends.cuda.matmul.allow_tf32
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = saved
+
+
+# ---- the generic CUDA-core conv-net kernel: oracle, TF32-point yardstick, mutations ----------------------------------
+GENERIC_SHAPES = [(1, 3, 1), (1, 5, 10), (8, 5, 128), (2, 3, 33), (3, 5, 64)]
+
+
+@pytest.mark.parametrize("shape", [(1, 3, 1), (8, 5, 128)])
+def test_convnet_oracle_matches_module_autograd_at_generic_edges(shape):
+    torch.manual_seed(0)
+    model = MNISTConvNet(*shape, dtype=torch.float64)
+    sh = synthetic_mnist(37, seed=5)
+    x = (sh.x.double() / 255 - MNIST_MEAN) / MNIST_STD
+    out = torch.nn.NLLLoss()(model(x), sh.y)
+    ref = torch.autograd.grad(out, list(model.parameters()))
+    l, g = ko.convnet_fp64(_row(model), model.spec, sh.x, sh.y, MNIST_MEAN, MNIST_STD)
+    torch.testing.assert_close(l, out.detach(), rtol=1e-13, atol=0)
+    torch.testing.assert_close(g, _row_of_tensors(ref, model), rtol=1e-12, atol=1e-15)
+
+
+def _generic_conv_case(shape, B, float_rows=False, draw=0):
+    """One node of the generic-kernel GPU test on CPU: its rows for ``draw`` (0: a full batch, 1: the partial one),
+    the fp64 oracle, the TF32-point yardstick and fp32 autograd standing in for an fp32-exact kernel."""
+    torch.manual_seed(0)
+    model = MNISTConvNet(*shape)
+    M = B + B // 2 + 1
+    sh = synthetic_mnist(M, seed=100, classes=[0])
+    rows = ko.batch_rows([M], B, 7, 0, draw)
+    x, y = sh.x[rows], sh.y[rows]
+    mean, std = MNIST_MEAN, MNIST_STD
+    if float_rows:
+        x, mean, std = ((x.double() / 255 - MNIST_MEAN) / MNIST_STD).float(), 0.0, 1.0
+    row = _row(model)
+    o, (lw,) = ko.slots(model.spec)[3]
+    row[o: o + lw] = row[o: o + lw].abs() + 0.1           # b1 > 0: at linear width 1 a dead unit zeroes every gradient
+    args = (model.spec, x, y, mean, std)
+    ref = ko.convnet_fp64(row, *args, pool_f32=True)[1]
+    yard = ko.convnet_tf32_point(row, *args)[1]
+    fp32 = ko.convnet_fp64(row, *args, dtype=torch.float32)[1].double()
+    return model, row, args, ref, yard, fp32
+
+
+@pytest.mark.parametrize("float_rows", [False, True], ids=["u8", "f32"])
+@pytest.mark.parametrize("B", [8, 37])
+@pytest.mark.parametrize("shape", GENERIC_SHAPES)
+def test_fp32_autograd_passes_the_tf32_point_convnet_check(shape, B, float_rows):
+    for draw in (0, 1):
+        model, _, _, ref, yard, fp32 = _generic_conv_case(shape, B, float_rows, draw)
+        assert all(t.abs().max() > 0 for t in ko.unflatten(ref, model.spec))
+        rat = ko.assert_close_to_oracle(fp32, ref, yard, ko.TF32_POINT_FRAC, spec=model.spec)
+        print(f"\nRATIO {shape} B={B} draw {draw}: " + " ".join(f"{k}={max(v):.2e}" for k, v in rat.items()))
+
+
+def test_partial_batch_divided_by_the_batch_size_is_rejected():
+    """The partial batch (19 of 37 rows) scaled by 1 / 37 instead of 1 / 19, and by 1 / 20."""
+    model, _, args, ref, yard, fp32 = _generic_conv_case((2, 3, 33), 37, draw=1)
+    n = args[1].shape[0]
+    assert n == 19
+    for wrong in (37, n + 1):
+        _rejected(fp32 * n / wrong, ref, yard, model.spec, ko.TF32_POINT_FRAC)
+
+
+def test_dropped_sample_of_a_slice_is_rejected():
+    """A slice that skips its third sample but still divides by the batch size."""
+    model, row, (spec, x, y, mean, std), ref, yard, _ = _generic_conv_case((1, 5, 10), 37)
+    keep = torch.arange(x.shape[0]) != 2
+    bad = ko.convnet_fp64(row, spec, x[keep], y[keep], mean, std, dtype=torch.float32)[1].double()
+    _rejected(bad * (x.shape[0] - 1) / x.shape[0], ref, yard, spec, ko.TF32_POINT_FRAC)
+
+
+def _conv_partition_grads(row, spec, x, y, mean, std, q, npart):
+    """Conv weight and bias gradients routed through the pool cells of conv-gradient partition ``q`` of ``npart``
+    (cells ``q NP / npart .. (q + 1) NP / npart - 1`` of every filter, as ``generic_chunk`` splits them)."""
+    wc, bc, w1, b1, w2, b2 = params = [p.requires_grad_(True) for p in ko.unflatten(row, spec)]
+    xin = (x.double().reshape(-1, 1, 28, 28) / 255.0 - mean) / std
+    a = torch.nn.functional.max_pool2d(torch.relu(torch.nn.functional.conv2d(xin, wc, bc)), 2)
+    npos = a.shape[-1] ** 2
+    p = torch.arange(npos)
+    keep = ((p >= q * npos // npart) & (p < (q + 1) * npos // npart)).double().reshape(a.shape[-2:])
+    a.register_hook(lambda g: g * keep)
+    z = torch.relu(a.flatten(1) @ w1.T + b1) @ w2.T + b2
+    loss = torch.nn.functional.nll_loss(torch.log_softmax(z, 1), y)
+    return torch.autograd.grad(loss, [wc, bc])
+
+
+@pytest.mark.parametrize("shape,npart", [((8, 5, 128), 2), ((1, 3, 1), 51)])
+def test_dropped_conv_gradient_partition_is_rejected(shape, npart):
+    """``npart = 512 / (F KS^2 + F)`` partitions of the pool cells: a CTA that leaves one partition's partial out of
+    the conv weight and bias gradients."""
+    F_, KS = shape[:2]
+    assert max(1, 512 // (F_ * KS * KS + F_)) == npart
+    model, row, args, ref, yard, fp32 = _generic_conv_case(shape, 37)
+    gwc, gbc = _conv_partition_grads(row, *args, q=npart // 2, npart=npart)
+    (owc, swc), (obc, _) = ko.slots(model.spec)[:2]
+    bad = fp32.clone()
+    bad[owc: owc + gwc.numel()] -= gwc.reshape(-1)
+    bad[obc: obc + gbc.numel()] -= gbc
+    _rejected(bad, ref, yard, model.spec, ko.TF32_POINT_FRAC)
+
+
+# ---- the generic CUDA-core MLP kernels: oracle, TF32-point yardstick, mutations --------------------------------------
+ACT_MIXES = [([5, 7, 3], ["relu", "none"]), ([5, 7, 3], ["tanh", "tanh"]), ([5, 7, 3], ["sigmoid", "sigmoid"]),
+             ([4, 9, 6, 8, 2], ["none", "relu", "tanh", "sigmoid"]), ([3, 6, 6, 4], ["sigmoid", "none", "relu"]),
+             ([2, 5, 1], ["tanh", "relu"]), ([1, 1], ["none"])]
+ACT_MODULES = {"none": torch.nn.Identity, "relu": torch.nn.ReLU, "tanh": torch.nn.Tanh, "sigmoid": torch.nn.Sigmoid}
+
+
+@pytest.mark.parametrize("shape,acts", ACT_MIXES)
+def test_mlp_oracle_matches_sequential_autograd(shape, acts):
+    flat = ko.mlp_params(shape)
+    mods = []
+    for l, a in enumerate(acts):
+        lin = torch.nn.Linear(shape[l], shape[l + 1], dtype=torch.float64)
+        wo, bo = ko.mlp_layout(shape)[l]
+        with torch.no_grad():
+            lin.weight.copy_(flat[wo: bo].reshape(lin.weight.shape))
+            lin.bias.copy_(flat[bo: bo + shape[l + 1]])
+        mods += [lin, ACT_MODULES[a]()]
+    seq = torch.nn.Sequential(*mods)
+    g = torch.Generator().manual_seed(1)
+    x = torch.randn(50, shape[0], generator=g, dtype=torch.float64, requires_grad=True)
+    gout = torch.randn(50, shape[-1], generator=g, dtype=torch.float64)
+    out = seq(x)
+    grads = torch.autograd.grad((out * gout).sum(), [x, *seq.parameters()])
+    o, hs, gflat, dx = ko.mlp_fp64(flat, shape, acts, x.detach(), gout)
+    torch.testing.assert_close(o, out.detach(), rtol=1e-14, atol=1e-15)
+    h = x.detach()
+    for l in range(len(acts)):
+        h = seq[2 * l + 1](seq[2 * l](h))
+        torch.testing.assert_close(hs[l], h.detach(), rtol=1e-14, atol=1e-15)
+    torch.testing.assert_close(gflat, torch.cat([t.reshape(-1) for t in grads[1:]]), rtol=1e-12, atol=1e-14)
+    torch.testing.assert_close(dx, grads[0], rtol=1e-12, atol=1e-14)
+
+
+class _TanhFromPreactivation(torch.autograd.Function):
+    """tanh with the derivative a buggy kernel would take: 1 - z^2 of the pre-activation z instead of 1 - y^2."""
+
+    @staticmethod
+    def forward(ctx, z):
+        ctx.save_for_backward(z)
+        return torch.tanh(z)
+
+    @staticmethod
+    def backward(ctx, g):
+        z, = ctx.saved_tensors
+        return g * (1 - z * z)
+
+
+def _mlp_autograd(flat, shape, acts, x, gout, tanh=torch.tanh):
+    """``mlp_fp64``'s results from autograd in the dtype of the arguments."""
+    flat = flat.detach().requires_grad_(True)
+    x = x.detach().requires_grad_(True)
+    h, hs = x, []
+    for l, (wo, bo) in enumerate(ko.mlp_layout(shape)):
+        z = h @ flat[wo: bo].reshape(shape[l + 1], shape[l]).T + flat[bo: bo + shape[l + 1]]
+        h = tanh(z) if acts[l] == "tanh" else ko._act(z, acts[l])
+        hs.append(h)
+    gflat, dx = torch.autograd.grad((h * gout).sum(), [flat, x])
+    return h.detach(), [t.detach() for t in hs], gflat, dx
+
+
+MLP_CASES = [([12, 64, 64, 64, 5], ["relu"] * 3 + ["none"], 2400), ([12, 64, 64, 64, 1], ["relu"] * 3 + ["none"], 777),
+             ([2, 37, 129, 3], ["tanh"] * 3, 100), ([7, 256, 16, 8], ["sigmoid"] * 3, 65),
+             ([2, 200, 1], ["relu", "none"], 33), ([1, 1], ["none"], 31),
+             ([256, 9, 17, 33, 65, 129, 256, 8, 1], ["relu", "tanh", "sigmoid", "none", "relu", "tanh", "sigmoid", "none"],
+              300)]
+
+
+def _mlp_generic_case(shape, acts, M, seed=0):
+    g = torch.Generator().manual_seed(seed)
+    flat = ko.mlp_params(shape, seed).float()
+    x = torch.randn(M, shape[0], generator=g)
+    gout = torch.randn(M, shape[-1], generator=g)
+    ref = ko.mlp_named(shape, *ko.mlp_fp64(flat, shape, acts, x, gout))
+    yard = ko.mlp_named(shape, *ko.mlp_fp64(ko.round_tf32(flat), shape, acts, ko.round_tf32(x), ko.round_tf32(gout)))
+    return flat, x, gout, ref, yard
+
+
+@pytest.mark.parametrize("shape,acts,M", MLP_CASES)
+def test_fp32_autograd_passes_the_tf32_point_mlp_check(shape, acts, M):
+    flat, x, gout, ref, yard = _mlp_generic_case(shape, acts, M)
+    got = ko.mlp_named(shape, *_mlp_autograd(flat, shape, acts, x, gout))
+    rat = ko.assert_close_to_oracle(got, ref, yard, ko.TF32_POINT_FRAC)
+    assert 0 < max(max(v) for v in rat.values())
+
+
+def _mlp_rejected(got, ref, yard):
+    with pytest.raises(AssertionError, match=f"above {ko.TF32_POINT_FRAC}"):
+        ko.assert_close_to_oracle(got, ref, yard, ko.TF32_POINT_FRAC)
+
+
+def test_mlp_cta_missing_from_a_weight_gradient_is_rejected():
+    """The RL actor at M = 2400 (75 CTAs of 32 rows): CTA 40's rows left out of W0's gradient."""
+    shape, acts, M = MLP_CASES[0]
+    flat, x, gout, ref, yard = _mlp_generic_case(shape, acts, M)
+    got = ko.mlp_named(shape, *_mlp_autograd(flat, shape, acts, x, gout))
+    rows = slice(40 * 32, 41 * 32)
+    part = ko.mlp_named(shape, *ko.mlp_fp64(flat, shape, acts, x[rows], gout[rows]))
+    got["W0"] = got["W0"] - part["W0"].float()
+    _mlp_rejected(got, ref, yard)
+
+
+def test_mlp_skipped_k_chunk_is_rejected():
+    """A forward that skips the third 32-wide K chunk of the 256-wide layer 1 (``din > 32``)."""
+    shape, acts, M = MLP_CASES[3]
+    flat, x, gout, ref, yard = _mlp_generic_case(shape, acts, M)
+    wo, bo = ko.mlp_layout(shape)[1]
+    bad = flat.clone()
+    bad[wo: bo].view(shape[2], shape[1])[:, 64:96] = 0.0
+    got = ko.mlp_named(shape, *_mlp_autograd(bad, shape, acts, x, gout))
+    got = {k: got[k] for k in ("out", "a1", "a2")}
+    _mlp_rejected(got, {k: ref[k] for k in got}, {k: yard[k] for k in got})
+
+
+def test_tanh_derivative_of_the_preactivation_is_rejected():
+    shape, acts, M = MLP_CASES[2]
+    flat, x, gout, ref, yard = _mlp_generic_case(shape, acts, M)
+    got = ko.mlp_named(shape, *_mlp_autograd(flat, shape, acts, x, gout, tanh=_TanhFromPreactivation.apply))
+    _mlp_rejected(got, ref, yard)
+
+
+# ---- the fused MLP runs only on arguments it can read ----------------------------------------------------------------
+def test_fused_mlp_arguments_must_match_dtype_device_and_width():
+    from nn_distributed_training_b200.ops.mlp_generic import arguments_match
+    shape = [12, 64, 5]
+    params = [torch.zeros(64, 12), torch.zeros(64), torch.zeros(5, 64), torch.zeros(5)]
+    assert arguments_match(torch.zeros(30, 12), params, shape)
+    assert arguments_match(torch.zeros(4, 30, 12), params, shape)             # leading dims are rows
+    assert not arguments_match(torch.zeros(30, 12, dtype=torch.float64), params, shape)
+    assert not arguments_match(torch.zeros(30, 12), params[:3] + [torch.zeros(5, dtype=torch.float64)], shape)
+    assert not arguments_match(torch.zeros(30, 11), params, shape)
+    assert not arguments_match(torch.zeros(30, 13), params, shape)
+    assert not arguments_match(torch.zeros(30, 12), params[:1] + [torch.zeros(64, device="meta")] + params[2:], shape)
