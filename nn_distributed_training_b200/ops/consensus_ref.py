@@ -867,6 +867,138 @@ def dp_epsilon(rho, delta: float) -> float:
     return float(np.max(rho + 2.0 * np.sqrt(rho * math.log(1.0 / delta))))
 
 
+# ---------------------------------------------------------------- Moniqua ----
+# Code rows (the layout of csrc/consensus.h: MoniquaArgs, the only other place it is written): b-bit codes of the
+# parameters modulo the range B, element e at bit (e b) % 32 of 32-bit word (e b) / 32, little-end first, so a row
+# is n_pad b / 8 bytes.  With L = 2^b and delta = 1 / L, all in float64:
+#   encode  t = frac(x / B) L;  c = (floor(t) + (u < t - floor(t))) mod L     u from the rounding stream
+#   decode  v = y / B - c / L;  n = rint(v);  xhat = B (c / L + n);  margin offset v - n   (y: the reader's own value)
+# The rounding stream is Philox4x32-10 under mq_key(rounding_seed) with the counter (e / 4, k, node, MQ_TAG): output
+# word e % 4 gives u = r 2^-32 for element e of the code that `node` publishes for round k (read in round k).  Padding
+# and slot holes get code 0.  Every division and product is a single IEEE operation, so the kernels write the same bits.
+MQ_BITS = (2, 4, 8)
+MQ_BASES = ("dsgd", "exact_diffusion")
+MQ_KEY_DOMAIN = 0x4D4E5155          # "MNQU": the rounding key never equals the problem seed's plain Philox key
+MQ_TAG = 0x4D515244                 # "MQRD": the fourth counter word of the rounding stream
+
+
+def mq_key(seed: int) -> Tuple[int, int]:
+    """The 64-bit Philox key of the rounding stream for ``rounding_seed`` (any integer, taken mod 2^64)."""
+    s = int(seed) & 0xFFFFFFFFFFFFFFFF
+    return s & 0xFFFFFFFF, (s >> 32) ^ MQ_KEY_DOMAIN
+
+
+def mq_range(theta_bound: float, bits: int) -> float:
+    """``B = 2 theta_bound / (1 - 2 delta)``, ``delta = 2^-bits``: the modulus that makes every decode exact while the
+    reader is within ``theta_bound`` of the value behind the code (DESIGN §2.17)."""
+    return 2.0 * float(theta_bound) / (1.0 - 2.0 * 2.0 ** -int(bits))
+
+
+def mq_code_bytes(n_pad: int, bits: int) -> int:
+    """Bytes of one code row; rows must be padded to a multiple of 128 elements, so rows stay 16-byte aligned."""
+    if n_pad % 128 != 0:
+        raise ValueError(f"moniqua needs rows padded to a multiple of 128 elements (n_pad = {n_pad})")
+    return n_pad * int(bits) // 8
+
+
+def mq_uniforms(key, k: int, node: int, n_pad: int) -> np.ndarray:
+    """The ``[n_pad]`` float64 uniforms ``r 2^-32`` that round the code ``node`` publishes for round ``k``."""
+    p = np.arange(n_pad // 4, dtype=np.uint64)
+    ctr = np.stack([p, np.full_like(p, k), np.full_like(p, node), np.full_like(p, MQ_TAG)], axis=-1)
+    return philox4x32_10(ctr, key).reshape(-1).astype(np.float64) * 2.0 ** -32
+
+
+def mq_codes(x: torch.Tensor, B: float, bits: int, u: torch.Tensor, live: torch.Tensor) -> torch.Tensor:
+    """The codes ``[R, n_pad]`` (int64, in ``[0, 2^bits)``) of the rows ``x`` with the uniforms ``u`` (same shape)."""
+    L = 1 << bits
+    z = x.double() / B
+    t = (z - torch.floor(z)) * L
+    fl = torch.floor(t)
+    c = (fl.to(torch.int64) + (u.to(t.device) < t - fl).to(torch.int64)) % L
+    return torch.where(live.to(c.device), c, torch.zeros_like(c))
+
+
+def mq_pack(codes: torch.Tensor, bits: int) -> torch.Tensor:
+    """Code rows ``[R, n_pad b / 8]`` (uint8) of the codes ``[R, n_pad]``."""
+    R, n_pad = codes.shape
+    per = 32 // bits
+    shifts = torch.arange(per, device=codes.device, dtype=torch.int64) * bits
+    words = (codes.reshape(R, n_pad // per, per) << shifts).sum(-1)
+    return torch.stack([(words >> (8 * q)) & 255 for q in range(4)], dim=-1).to(torch.uint8).reshape(R, -1)
+
+
+def mq_unpack(rows: torch.Tensor, bits: int) -> torch.Tensor:
+    """The codes ``[R, n_pad]`` (int64) of code rows ``[R, n_pad b / 8]`` (uint8)."""
+    R = rows.shape[0]
+    wb = rows.to(torch.int64).reshape(R, -1, 4)
+    words = wb[..., 0] | (wb[..., 1] << 8) | (wb[..., 2] << 16) | (wb[..., 3] << 24)
+    per = 32 // bits
+    shifts = torch.arange(per, device=rows.device, dtype=torch.int64) * bits
+    return ((words.unsqueeze(-1) >> shifts) & ((1 << bits) - 1)).reshape(R, -1)
+
+
+def mq_encode(x: torch.Tensor, B: float, bits: int, key, k: int, nodes, live: torch.Tensor) -> torch.Tensor:
+    """Code rows ``[R, n_pad b / 8]`` (uint8) that the nodes ``nodes`` (global ids, one per row of ``x``) publish for
+    round ``k``."""
+    u = torch.as_tensor(np.stack([mq_uniforms(key, k, int(g), x.shape[1]) for g in nodes]), device=x.device)
+    return mq_pack(mq_codes(x, B, bits, u, live), bits)
+
+
+def mq_decode(codes: torch.Tensor, y: torch.Tensor, B: float, bits: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``(xhat, v - n)`` in float64 of the codes ``codes`` (int64) decoded against the side information ``y``."""
+    cl = codes.double() * 2.0 ** -bits
+    v = y.double() / B - cl
+    n = torch.round(v)                     # half to even, as rint
+    return B * (cl + n), v - n
+
+
+def mq_margin_hits(off: torch.Tensor, bits: int) -> torch.Tensor:
+    """Margin hits: elements whose decode offset is past ``1/2 - delta`` (at or near the wrap boundary)."""
+    return off.abs() > 0.5 - 2.0 ** -bits
+
+
+def mq_mix_(theta: torch.Tensor, codes_all: torch.Tensor, w_rows: torch.Tensor, nbrs, lo: int, B: float, bits: int,
+            margin: torch.Tensor) -> None:
+    """The combine of the local rows: ``theta_i += sum_{j != i} w_ij (xhat_j - xhat_i)``, every code decoded against
+    ``y = theta_i``, the sum in float64 over the neighbors ``nbrs[l]`` (global ids) in table order with the weights of
+    ``w_rows [L, N]`` (in the arena dtype), rounded once.  ``codes_all [N, n_pad]`` are every node's pending codes;
+    each neighbor element past the margin adds one to ``margin[l]``."""
+    for l in range(theta.shape[0]):
+        y = theta[l].double()
+        xi, _ = mq_decode(codes_all[lo + l], y, B, bits)
+        acc = torch.zeros_like(y)
+        hits = 0
+        for j in nbrs[l]:
+            xj, off = mq_decode(codes_all[j], y, B, bits)
+            acc = acc + float(w_rows[l, j]) * (xj - xi)
+            hits += int(mq_margin_hits(off, bits).sum())
+        theta[l] = (y + acc).to(theta.dtype)
+        margin[l] += hits
+
+
+def mq_step_(theta: torch.Tensor, psi: Optional[torch.Tensor], grad: torch.Tensor, alpha: float, first: bool, B: float,
+             bits: int, key, k: int, nodes, live: torch.Tensor) -> torch.Tensor:
+    """The step of round ``k`` on the mixed rows, DSGD's (``psi`` None) or Exact Diffusion's (``ed_step_``, with
+    ``psi <- theta`` first in round 0); returns the code rows published for round ``k + 1``."""
+    if psi is None:
+        dsgd_step_(theta, grad, alpha)
+    else:
+        if first:
+            psi.copy_(theta)
+        ed_step_(theta, psi, grad, alpha)
+    return mq_encode(theta, B, bits, key, k + 1, nodes, live)
+
+
+def mq_edge_gap(theta_all: torch.Tensor, edges, theta_bound: float) -> float:
+    """``max over edges {i, j} of |theta_j - theta_i|_inf / theta_bound`` (0 without an edge): above 1 the run has left
+    the decode guarantee."""
+    gap = 0.0
+    for i, j in edges:
+        if i != j:
+            gap = max(gap, float((theta_all[j].double() - theta_all[i].double()).abs().max()))
+    return gap / float(theta_bound)
+
+
 # ------------------------------------------------------------- metrics ----
 def consensus_error(theta_all: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
     """Pairwise and to-mean distances of L2-normalised parameter rows

@@ -129,6 +129,7 @@ struct ConsensusOp {
   consensus::HsgdArgs<T> hs{};
   consensus::PgaArgs<T> pa{};
   consensus::DpArgs<T> dp{};
+  consensus::MoniquaArgs<T> mq{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -140,7 +141,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -172,6 +173,11 @@ struct ConsensusOp {
     dp.clip = getf(d, "clip_norm", 0.0); dp.cz_dp = getf(d, "cz_dp", 0.0); dp.cz_pair = getf(d, "cz_pair", 0.0);
     dp.key0 = d.contains("dp_key0") ? (unsigned)d["dp_key0"].cast<unsigned long long>() : 0u;
     dp.key1 = d.contains("dp_key1") ? (unsigned)d["dp_key1"].cast<unsigned long long>() : 0u;
+    mq.psi = ptr<T>(d, "psi"); mq.live = ptr<const unsigned>(d, "live"); mq.B = getf(d, "mq_B", 0.0);
+    mq.bits = geti(d, "mq_bits", 0); mq.node0 = geti(d, "node0", 0); mq.margin = ptr<unsigned long long>(d, "mq_margin");
+    mq.key0 = d.contains("mq_key0") ? (unsigned)d["mq_key0"].cast<unsigned long long>() : 0u;
+    mq.key1 = d.contains("mq_key1") ? (unsigned)d["mq_key1"].cast<unsigned long long>() : 0u;
+    mq.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -295,6 +301,21 @@ struct ConsensusOp {
   void dp_step() {
     dp_check("dp_step");
     check(consensus::launch_dp_step<T>(dp, cur_stream()), "dp_step");
+  }
+  void mq_check(const char* what) const {
+    if (!(mq.bits == 2 || mq.bits == 4 || mq.bits == 8) || mq.live == nullptr || mq.margin == nullptr || !(mq.B > 0.0) ||
+        c.n_pad % 128 != 0 || mq.code_stride != (long long)c.n_pad * mq.bits / 8 || c.C != 1 || c.sum_mode)
+      throw std::runtime_error(std::string(what) + " needs `mq_bits` in {2, 4, 8}, the `live` mask, the `mq_margin` "
+                               "counters, `mq_B` > 0, rows padded to a multiple of 128, `code_stride` = n_pad * bits / 8, "
+                               "one published channel and the pointer-table neighbors");
+  }
+  void mq_mix() {
+    mq_check("mq_mix");
+    check(consensus::launch_mq_mix<T>(mq, cur_stream()), "mq_mix");
+  }
+  void mq_step() {
+    mq_check("mq_step");
+    check(consensus::launch_mq_step<T>(mq, cur_stream()), "mq_step");
   }
   void dadaptive_mix() {
     if (!ad.tracking || ad.ut == nullptr || c.C != 2)
@@ -438,6 +459,8 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("pga_mix", &ConsensusOp<T>::pga_mix)
       .def("dp_norm", &ConsensusOp<T>::dp_norm)
       .def("dp_step", &ConsensusOp<T>::dp_step)
+      .def("mq_mix", &ConsensusOp<T>::mq_mix)
+      .def("mq_step", &ConsensusOp<T>::mq_step)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

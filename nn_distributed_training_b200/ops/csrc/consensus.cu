@@ -16,6 +16,7 @@
 // GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
 // Gossip-PGA / local SGD (no reference counterpart, optimizers/gossip_pga.py) -> pga_sum + pga_mix / dsgd_step
 // DP-DSGD / DECOR (no reference counterpart, optimizers/dp_dsgd.py)        -> dsgd_mix / dp_norm + dp_step
+// Moniqua (no reference counterpart, optimizers/moniqua.py)                -> mq_mix / mq_step
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
 //                                  optimizers/dadaptive.py)                -> dadaptive_mix or dsgd_mix / dadaptive_step
 // RelaySum (no reference counterpart, optimizers/relaysum.py)             -> relay_mix / relay_step
@@ -1562,6 +1563,126 @@ __global__ void __launch_bounds__(THREADS) dp_step_kernel(const DpArgs<T> a) {
   end_step(c, l, ri.k, true);
 }
 
+// ---------------------------------------------------------------- Moniqua ----
+// Round k (layout, stream and rules in consensus.h: MoniquaArgs): mq_mix, fwd/bwd, mq_step.  mq_mix pulls one 32-bit
+// code word per neighbor and thread (the codes of its Vec<T>::N elements), decodes in registers against y = theta_i
+// (y / B once per element) and accumulates sum_{j != i} w_ij (xhat_j - xhat_i) in fp64 in neighbor order, each product
+// rounded on its own, so the host twin computes the same bits.  The margin hits of a warp go out in one atomic.
+template <typename T, int BITS>
+__global__ void __launch_bounds__(THREADS) mq_mix_kernel(const MoniquaArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  constexpr unsigned MASK = (1u << BITS) - 1u;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const unsigned* own = mq_code_row(a, ri.par, l);
+  const double lim = 0.5 - 1.0 / (1 << BITS);
+  unsigned hits = 0u;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    Pack<T> th = ldv(c.theta + row + i);
+    const unsigned cw = mq_word<T, BITS>(own, i);
+    double yb[N], xi[N], acc[N];
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      double off;
+      yb[u] = __ddiv_rn((double)th.v[u], a.B);
+      xi[u] = mq_decode<BITS>((cw >> (u * BITS)) & MASK, yb[u], a.B, off);
+      acc[u] = 0.0;
+    }
+    for_neighbors<4>(deg, [&](int e) { return mq_word<T, BITS>(reinterpret_cast<const unsigned*>(nbr_row(c, ri.gid, l, e, ri.par, 0)), i); },
+                     [&](int e, unsigned q) {
+                       const double we = (double)w[e];
+#pragma unroll
+                       for (int u = 0; u < N; ++u) {
+                         double off;
+                         const double xj = mq_decode<BITS>((q >> (u * BITS)) & MASK, yb[u], a.B, off);
+                         acc[u] = __dadd_rn(acc[u], __dmul_rn(we, __dsub_rn(xj, xi[u])));
+                         hits += fabs(off) > lim ? 1u : 0u;
+                       }
+                     });
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] = (T)__dadd_rn((double)th.v[u], acc[u]);
+    stv(c.theta + row + i, th);
+  }
+  hits = __reduce_add_sync(0xffffffffu, hits);
+  if ((threadIdx.x & 31) == 0 && hits != 0u) atomicAdd(a.margin + l, (unsigned long long)hits);
+}
+
+// DSGD's step (ED = false) or ed_step's adapt / correct (ED: psi <- theta in round 0), then the code of the new theta
+// for round k + 1.  The loop runs per warp, as choco_step: the G lanes holding one code word OR their bits together with
+// xor shuffles and the first of them stores the word; a lane past the end of the row takes part and stores nothing.
+template <typename T, int U, int BITS, bool ED>
+__global__ void __launch_bounds__(THREADS) mq_step_kernel(const MoniquaArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  constexpr int G = 32 / BITS / N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const bool init = ri.k == 0;
+  const size_t row = (size_t)l * c.n_pad;
+  unsigned* out = mq_code_row(a, ri.par ^ 1, l);
+  const unsigned me = (unsigned)(a.node0 + l);
+  const int lane = threadIdx.x & 31;
+  // theta (written by the mix two launches back) and psi (the previous round's step) are read before the
+  // programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int w0 = (blockIdx.x * THREADS + (threadIdx.x & ~31)) * N; w0 < c.n_pad; w0 += gridDim.x * THREADS * N) {
+    const int i = w0 + lane * N;
+    const bool in = i < c.n_pad;
+    Pack<T> th, dc;
+#pragma unroll
+    for (int u = 0; u < N; ++u) { th.v[u] = (T)0; dc.v[u] = (T)0; }
+    if (in) {
+      th = ldv(c.theta + row + i);
+      if (ED && !init) {
+        const Pack<T> ps = ldv(a.psi + row + i);
+#pragma unroll
+        for (int u = 0; u < N; ++u) dc.v[u] = th.v[u] - ps.v[u];
+      }
+    }
+    release_dependents_once(waited);
+    unsigned bits = 0u;
+    if (in) {
+      const Pack<T> g = sum_partials<U>(c, l, i);
+      if (ED) {
+        Pack<T> pn;
+#pragma unroll
+        for (int u = 0; u < N; ++u) {
+          pn.v[u] = th.v[u] - alpha * g.v[u];
+          th.v[u] = pn.v[u] + dc.v[u];
+        }
+        stv(a.psi + row + i, pn);
+      } else {
+#pragma unroll
+        for (int u = 0; u < N; ++u) th.v[u] -= alpha * g.v[u];
+      }
+      stv(c.theta + row + i, th);
+      const uint4 r = curand_Philox4x32_10(make_uint4((unsigned)(i >> 2), (unsigned)(ri.k + 1), me, kMqTag),
+                                           make_uint2(a.key0, a.key1));
+      const unsigned lw = a.live[i >> 5];
+#pragma unroll
+      for (int u = 0; u < N; ++u) {
+        const int q = (i & 3) + u;
+        const unsigned rr = q == 0 ? r.x : q == 1 ? r.y : q == 2 ? r.z : r.w;
+        const unsigned code = ((lw >> ((i & 31) + u)) & 1u) ? mq_code<BITS>((double)th.v[u], a.B, rr) : 0u;
+        bits |= code << (((i + u) * BITS) & 31);
+      }
+    }
+#pragma unroll
+    for (int o = G / 2; o >= 1; o >>= 1) bits |= __shfl_xor_sync(0xffffffffu, bits, o);
+    if (in && (lane & (G - 1)) == 0) out[(i * BITS) >> 5] = bits;
+  }
+  release_dependents_once(waited);
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2683,6 +2804,28 @@ template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_
   return launch_by_s(dp_step_kernel<T, 4>, dp_step_kernel<T, 8>, a.c, a, st);
 }
 
+// mq_mix and mq_step: the bit width and the base are template parameters; beyond 4 gradient partials the step keeps 8
+// loads in flight (as choco_step)
+template <typename T> static bool mq_ready(const MoniquaArgs<T>& a) {
+  return (a.bits == 2 || a.bits == 4 || a.bits == 8) && a.live != nullptr && a.margin != nullptr && a.B > 0.0 &&
+         a.c.n_pad % 128 == 0 && a.code_stride == (long long)a.c.n_pad * a.bits / 8 && a.c.C == 1 && !a.c.sum_mode;
+}
+template <typename T, int BITS> static cudaError_t launch_mq_bits(const MoniquaArgs<T>& a, bool step, cudaStream_t st) {
+  if (!step) return launch_one_wave(mq_mix_kernel<T, BITS>, a.c, a, st);
+  if (a.psi != nullptr) return launch_by_s(mq_step_kernel<T, 4, BITS, true>, mq_step_kernel<T, 8, BITS, true>, a.c, a, st);
+  return launch_by_s(mq_step_kernel<T, 4, BITS, false>, mq_step_kernel<T, 8, BITS, false>, a.c, a, st);
+}
+template <typename T> static cudaError_t launch_mq(const MoniquaArgs<T>& a, bool step, cudaStream_t st) {
+  if (!mq_ready(a)) return cudaErrorInvalidValue;
+  switch (a.bits) {
+    case 2: return launch_mq_bits<T, 2>(a, step, st);
+    case 4: return launch_mq_bits<T, 4>(a, step, st);
+    default: return launch_mq_bits<T, 8>(a, step, st);
+  }
+}
+template <typename T> cudaError_t launch_mq_mix(const MoniquaArgs<T>& a, cudaStream_t st) { return launch_mq(a, false, st); }
+template <typename T> cudaError_t launch_mq_step(const MoniquaArgs<T>& a, cudaStream_t st) { return launch_mq(a, true, st); }
+
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
 }
@@ -2808,6 +2951,8 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_pga_mix<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_dp_norm<T>(const DpArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_dp_step<T>(const DpArgs<T>&, cudaStream_t);             \
+  template cudaError_t launch_mq_mix<T>(const MoniquaArgs<T>&, cudaStream_t);         \
+  template cudaError_t launch_mq_step<T>(const MoniquaArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

@@ -237,6 +237,33 @@ struct DpArgs {
   unsigned key0, key1;             // Philox key
 };
 
+// Moniqua (Lu, De Sa 2020), optimizers/moniqua.py: modulo-quantized gossip on DSGD or Exact Diffusion.  The published
+// buffer holds one code row per node of `code_stride` = n_pad * bits / 8 bytes: the bits-bit code of element e at bit
+// (e * bits) % 32 of 32-bit word (e * bits) / 32.  With L = 2^bits and delta = 1 / L, in fp64:
+//   encode  t = frac(x / B) L,  c = (floor(t) + (u < t - floor(t))) mod L,  u = r 2^-32
+//   decode  v = y / B - c / L,  n = rint(v),  xhat = B (c / L + n)          y: the reader's own theta
+// r is word e % 4 of Philox4x32-10 under `key` with the counter (e / 4, k, node, kMqTag): the code a node publishes for
+// round k (written by the step of round k - 1), so a code depends on (seed, round, node, element, x) only.  Padding and
+// slot holes (clear in `live`) get code 0.  Round k: mq_mix decodes the node's own code and its neighbors' against theta_i,
+// theta_i += sum_{j != i} w_ij (xhat_j - xhat_i) in fp64 with the topology weights (W, or A = (I + W) / 2 for the Exact
+// Diffusion base), rounded once; a neighbor element with |v - n| > 1/2 - delta is a margin hit, counted per node.
+// mq_step takes DSGD's step (psi == nullptr) or ed_step's, encodes theta and publishes the code row
+// (ops/consensus_ref.py: mq_mix_, mq_step_, the host twin).
+constexpr unsigned kMqTag = 0x4D515244u;
+
+template <typename T>
+struct MoniquaArgs {
+  Common<T> c;
+  T* psi;                          // [L, n_pad] Exact Diffusion base: the adapt step of the previous round; nullptr = DSGD
+  const unsigned* live;            // [n_pad / 32] live-element bits
+  double B;                        // the modulus 2 theta_bound / (1 - 2 delta)
+  int bits;                        // 2, 4 or 8
+  unsigned key0, key1;             // Philox key
+  int node0;                       // global id of local node 0
+  unsigned long long* margin;      // [L] margin hits per local node
+  long long code_stride;           // bytes per code row of the published buffer
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -397,6 +424,8 @@ template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream
 template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_mq_mix(const MoniquaArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_mq_step(const MoniquaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

@@ -718,6 +718,38 @@ NNDT_DEVINL Pack<T> dp_noise(const DpArgs<T>& a, int k, unsigned me, int deg, co
   return out;
 }
 
+// ---- Moniqua (layout and stream in consensus.h: MoniquaArgs) ----
+template <typename T>
+NNDT_DEVINL unsigned* mq_code_row(const MoniquaArgs<T>& a, int par, int l) {
+  return reinterpret_cast<unsigned*>(reinterpret_cast<char*>(a.c.pub) + ((size_t)par * a.c.pub_L + l) * (size_t)a.code_stride);
+}
+
+// the codes of the Vec<T>::N elements from i in the low bits of the result (element i + u at bits u * BITS)
+template <typename T, int BITS>
+NNDT_DEVINL unsigned mq_word(const unsigned* row, int i) {
+  return row[(i * BITS) >> 5] >> ((i * BITS) & 31);
+}
+
+// the code of x (fp64) rounded with the 32 random bits r; every operation a single IEEE one, as mq_codes
+template <int BITS>
+NNDT_DEVINL unsigned mq_code(double x, double B, unsigned r) {
+  const double z = __ddiv_rn(x, B);
+  const double t = __dmul_rn(__dsub_rn(z, floor(z)), (double)(1 << BITS));
+  const double fl = floor(t);
+  const double u = __dmul_rn((double)r, 0x1p-32);
+  return ((unsigned)fl + (u < __dsub_rn(t, fl) ? 1u : 0u)) & ((1u << BITS) - 1u);
+}
+
+// xhat of code c from yb = y / B, and the margin offset v - n
+template <int BITS>
+NNDT_DEVINL double mq_decode(unsigned c, double yb, double B, double& off) {
+  const double cl = (double)c * (1.0 / (1 << BITS));       // exact
+  const double v = __dsub_rn(yb, cl);
+  const double n = rint(v);
+  off = __dsub_rn(v, n);
+  return __dmul_rn(B, __dadd_rn(cl, n));
+}
+
 // ---- SGP (layout in consensus.h) ----
 template <typename T>
 NNDT_DEVINL T* sgp_row(const SgpArgs<T>& a, int par, int l) {

@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip", "gossip_pga", "dp_dsgd"):
+                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
@@ -184,13 +184,16 @@ class ConsensusEngine:
             graphs_per_round = [edgeless] * len(graphs_per_round)
         # DP-DSGD: DSGD's channel and pointer-table mix, a clipped and noised step (dp_norm, dp_step)
         self.dp = opt.alg_name == "dp_dsgd"
+        # Moniqua: one channel of modulo-quantized code rows, pulled through the pointer table (mq_mix, mq_step)
+        self.mq = opt.alg_name == "moniqua"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
         # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
         # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w (Push-DIGing: both
         # channels, u with w in the tail and y, have that stride).  BEER publishes two channels of CHOCO code rows.
-        if self.choco or self.beer:
+        # Moniqua publishes code rows of n_pad * bits / 8 bytes.
+        if self.choco or self.beer or self.mq:
             self.row_bytes = opt.code_bytes
         elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
@@ -206,6 +209,10 @@ class ConsensusEngine:
         p0 = K * k0                 # the protocol round of gradient round k0
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
         if self.choco:
+            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
+        elif self.mq:                               # round 0 reads the codes of theta^0
+            if k0 == 0:
+                opt.encode_initial()
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
         elif self.beer:
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code_h)
@@ -299,6 +306,9 @@ class ConsensusEngine:
         if self.dp and directed:
             raise ValueError("dp_dsgd needs undirected graphs: a planned graph is directed (the pairwise noise of an edge "
                              "cancels between its two ends)")
+        if self.mq and directed:
+            raise ValueError("moniqua needs undirected graphs: a planned graph is directed (its mix conserves the network "
+                             "sum only with symmetric weights)")
         rmax = max(1, max(t.max_readers for t in topos))
         check_wait_capacity(dmax, rmax if directed or G > 1 else 0)    # a static undirected graph has no second wait
         nbr_ptr = np.zeros((G, L, dmax, 2, self.C), dtype=np.int64)
@@ -315,7 +325,8 @@ class ConsensusEngine:
             if push_sum:
                 Wt = t.push_weights
             else:
-                Wt = ed_weights(t.W) if opt.alg_name == "exact_diffusion" else t.W
+                ed = opt.alg_name == "exact_diffusion" or (self.mq and opt.base == "exact_diffusion")
+                Wt = ed_weights(t.W) if ed else t.W
             for l, g in enumerate(pl.local_nodes):
                 nb = t.neighbors_noself[g]
                 deg[gi, l] = len(nb)
@@ -401,7 +412,7 @@ class ConsensusEngine:
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
                          and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag or self.pga or self.dp)
+                                  or self.detag or self.pga or self.dp or self.mq)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -573,6 +584,11 @@ class ConsensusEngine:
                      s_g=opt.s_g.data_ptr(), m_old=opt.m_old.data_ptr(), live=self.t_live.data_ptr(),
                      gamma=float(opt.gamma), code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes),
                      topk_k=int(opt.topk_k or 0))
+        if self.mq:
+            self.t_live = choco_live_words(opt.live).to(dev)
+            d.update(psi=None if opt.psi is None else opt.psi.data_ptr(), live=self.t_live.data_ptr(), mq_B=float(opt.B),
+                     mq_bits=int(opt.bits), mq_key0=int(opt.key[0]), mq_key1=int(opt.key[1]), node0=int(pl.lo),
+                     mq_margin=opt.margin.data_ptr(), code_stride=int(self.row_bytes))
         if self.sgp:
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
         if self.pdg:
@@ -603,7 +619,8 @@ class ConsensusEngine:
         pulls what a DSGD round does (nothing with ``gossip: false``: the edgeless graph); a global round pulls no row
         and contributes one fp64 partial-sum row per rank (``global_row``, ``n_pad * 8`` bytes) to the NVLS
         reduction, once every ``period`` rounds.  A DP-DSGD round pulls what a DSGD round does: the edge noise is
-        drawn on both ends, and the norm partials stay on the node."""
+        drawn on both ends, and the norm partials stay on the node.  A Moniqua row is the node's code row,
+        ``n_pad * bits / 8`` bytes, one per neighbor edge as DSGD's rows; the margin counters stay on the node."""
         deg = int(self.t_deg[0].sum().item())
         if self.pga:
             return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,

@@ -20,6 +20,7 @@ A round is a short, fixed kernel sequence
     GT-HSGD:  dsgt_mix, fwd/bwd, fwd/bwd at theta_prev, hsgd_track   (both fwd/bwd on the same minibatch)
     Gossip-PGA:  pga_sum, pga_mix, fwd/bwd, dsgd_step             (pga_sum returns at once on gossip rounds)
     DP-DSGD / DECOR:  dsgd_mix, fwd/bwd, dp_norm, dp_step
+    Moniqua:  mq_mix, fwd/bwd, mq_step
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -139,6 +140,10 @@ def _round_ops_impl(opt, eng, grads, grads_prev):
         grads(0)
         eng.op.dp_norm()
         eng.op.dp_step()
+    elif alg == "moniqua":
+        eng.op.mq_mix()
+        grads(0)
+        eng.op.mq_step()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -194,10 +199,11 @@ class RoundProgram:
         # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
         # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
         # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
-        # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y
+        # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y; Moniqua publishes
+        # codes too
         attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
-                                      or self.eng.relay or self.eng.pg or self.eng.detag)
+                                      or self.eng.relay or self.eng.pg or self.eng.detag or self.eng.mq)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -392,7 +398,7 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd") and opt.k > 0:
+                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
@@ -404,7 +410,7 @@ class RoundProgram:
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name in ("clipped_gossip", "bridge"):
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
-        if opt.alg_name == "choco_sgd":
+        if opt.alg_name in ("choco_sgd", "moniqua"):     # Moniqua's psi and margin counters are its own rows
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
         if opt.alg_name == "beer":              # h, s_h, v, g, s_g and m_old are the optimizer's own rows
             opt.code_h.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))

@@ -12,6 +12,7 @@ from .dsgt import DSGT
 from .exact_diffusion import ExactDiffusion
 from .gossip_pga import GossipPGA
 from .gt_hsgd import GTHSGD
+from .moniqua import Moniqua
 from .kgt import KGT
 from .powergossip import PowerGossip
 from .push_diging import PushDIGing
@@ -22,7 +23,8 @@ ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
-              "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD}
+              "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD,
+              "moniqua": Moniqua}
 
 
 def build_optimizer(problem, device, opt_conf):

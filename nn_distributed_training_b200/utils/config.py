@@ -15,12 +15,14 @@ import yaml
 
 import math
 
-from ..ops.consensus_ref import BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, TOPK_RATIO_DEFAULT
+from ..ops.consensus_ref import (BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, MQ_BASES, MQ_BITS,
+                                 TOPK_RATIO_DEFAULT)
 
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
-        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd")
+        "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
+        "moniqua")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -69,6 +71,9 @@ OPT_SCHEMA = {
     "dp_dsgd": {"alpha0": REQUIRED, "mu": 0.0, "clip_norm": REQUIRED, "noise_multiplier": REQUIRED,
                 "pair_noise_multiplier": 0.0, "target_delta": 1e-5, "outer_iterations": REQUIRED, "update_graph": True,
                 "profile": False},
+    # rounding_seed defaults to the problem's seed (filled in by the optimizer, which knows it)
+    "moniqua": {"alpha0": REQUIRED, "mu": 0.0, "bits": REQUIRED, "theta_bound": REQUIRED, "base": "dsgd",
+                "outer_iterations": REQUIRED, "update_graph": True, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -231,6 +236,33 @@ def _check_dp_dsgd(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.noise_seed must be an integer (got {s!r})")
 
 
+MONIQUA_KEYS = ("alg_name", "alpha0", "mu", "bits", "theta_bound", "base", "rounding_seed", "outer_iterations",
+                "update_graph", "profile")
+
+
+def _check_moniqua(c: Dict[str, Any], path: str) -> None:
+    """Moniqua: DSGD's step schedule (``alpha0`` and ``mu`` finite, >= 0), ``bits`` (2, 4 or 8, not a bool),
+    ``theta_bound`` (finite, > 0), the ``base``, an integer ``rounding_seed`` and no other key."""
+    for key in c:
+        if key not in MONIQUA_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: moniqua takes no key {key!r} (its keys are alpha0, mu, bits, theta_bound, "
+                              f"base, rounding_seed, outer_iterations and update_graph)")
+    for key in ("alpha0", "mu"):
+        if not _real(c[key]) or not (math.isfinite(float(c[key])) and float(c[key]) >= 0.0):
+            raise ConfigError(f"{path}.{key} must be finite and >= 0 (got {c[key]!r})")
+    b = c["bits"]
+    if isinstance(b, bool) or not isinstance(b, int) or b not in MQ_BITS:
+        raise ConfigError(f"{path}.bits must be one of {'|'.join(map(str, MQ_BITS))} (got {b!r})")
+    tb = c["theta_bound"]
+    if not _real(tb) or not (math.isfinite(float(tb)) and float(tb) > 0.0):
+        raise ConfigError(f"{path}.theta_bound must be finite and > 0 (got {tb!r})")
+    if c["base"] not in MQ_BASES:
+        raise ConfigError(f"{path}.base must be one of {'|'.join(MQ_BASES)} (got {c['base']!r})")
+    s = c.get("rounding_seed", 0)
+    if isinstance(s, bool) or not isinstance(s, int):
+        raise ConfigError(f"{path}.rounding_seed must be an integer (got {s!r})")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -283,7 +315,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         raise ConfigError(f"{path}.byzantine: Byzantine attackers are modelled by alg_name clipped_gossip only, or "
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
-                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd")
+                "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
+                "moniqua")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -341,6 +374,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_gossip_pga(c, path)
     if alg == "dp_dsgd":
         _check_dp_dsgd(c, path)
+    if alg == "moniqua":
+        _check_moniqua(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
