@@ -369,6 +369,70 @@ def choco_step_(theta: torch.Tensor, x_hat: torch.Tensor, grad: torch.Tensor, al
     return codes
 
 
+# ------------------------------------------------------------ SPARQ-SGD ----
+# A SPARQ row is a CHOCO code row (choco_encode's bytes) followed by a 16-byte tail: uint32 trig, uint32 0, float64 e
+# (csrc/consensus.h: SparqArgs).  A node whose tail says 0 is not pulled past its tail.
+SPARQ_COMPRESSORS = ("none", "int8", "sign")
+SPARQ_TAIL = 16
+
+
+def sparq_row_bytes(code_bytes: int) -> int:
+    """Bytes of one published SPARQ row: the code row and the tail, rounded up to 16."""
+    return -(-(int(code_bytes) + SPARQ_TAIL) // 16) * 16
+
+
+def sparq_threshold(threshold: float, growth: float, alphas) -> np.ndarray:
+    """``thr_k = threshold (k + 1)^growth alpha_k^2`` in float64 for the given ``alpha_k`` of rounds 0, 1, ..."""
+    a = np.asarray(alphas, dtype=np.float64)
+    k1 = np.arange(1, a.size + 1, dtype=np.float64)
+    return float(threshold) * k1 ** float(growth) * (a * a)
+
+
+def sparq_tails(trig: torch.Tensor, e: torch.Tensor) -> torch.Tensor:
+    """``[L, 16]`` uint8 tails of trigger bits ``trig [L]`` and errors ``e [L]`` (float64)."""
+    L = trig.shape[0]
+    head = torch.stack([trig.to(torch.int32), torch.zeros_like(trig, dtype=torch.int32)], dim=1).contiguous()
+    return torch.cat([head.view(torch.uint8).reshape(L, 8),
+                      e.to(torch.float64).reshape(L, 1).contiguous().view(torch.uint8).reshape(L, 8)], dim=1)
+
+
+def sparq_tail_read(rows: torch.Tensor, code_bytes: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The trigger bits (bool ``[R]``) and errors (float64 ``[R]``) in the tails of published rows ``[R, row_bytes]``."""
+    t = rows[:, code_bytes: code_bytes + SPARQ_TAIL].contiguous()
+    return t[:, :4].view(torch.int32)[:, 0] != 0, t[:, 8:].view(torch.float64)[:, 0]
+
+
+def sparq_mix_(theta: torch.Tensor, x_hat: torch.Tensor, s: torch.Tensor, rows_all: torch.Tensor, w_rows: torch.Tensor,
+               gamma: float, compressor: str, live: torch.Tensor, code_bytes: int) -> None:
+    """``s_i += sum_j W_ij dec(q_j)`` over the nodes whose pending tail says triggered (own term included), then
+    ``theta_i += gamma (s_i - x_hat_i)``.  A non-triggered row's body is not decoded into the sum (it may be stale)."""
+    trig, _ = sparq_tail_read(rows_all, code_bytes)
+    dec = choco_decode(rows_all[:, :code_bytes], compressor, theta.shape[1], theta.dtype, live)
+    dec = torch.where(trig.to(dec.device)[:, None], dec, torch.zeros((), dtype=dec.dtype, device=dec.device))
+    choco_mix_(theta, x_hat, s, dec, w_rows, gamma)
+
+
+def sparq_step_(theta: torch.Tensor, grad: torch.Tensor, alpha: float) -> None:
+    """One local step ``theta -= alpha g`` (DSGD's)."""
+    theta.add_(grad, alpha=-alpha)
+
+
+def sparq_publish_(theta: torch.Tensor, x_hat: torch.Tensor, code: torch.Tensor, thr: float, compressor: str,
+                   live: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """``e_i = ||theta_i - x_hat_i||^2`` (float64), ``trig_i = e_i > thr``.  A triggered node writes ``Q(theta_i -
+    x_hat_i)`` into the body of its row ``code [L, row_bytes]`` and takes ``x_hat_i += dec``; every node writes its tail.
+    Returns ``(trig, e)``."""
+    v = theta - x_hat
+    e = (v.to(torch.float64) ** 2).sum(1)
+    trig = e > float(thr)
+    codes, dec = choco_encode(v, compressor, live)
+    cb = codes.shape[1]
+    code[:, :cb] = torch.where(trig[:, None], codes, code[:, :cb])
+    x_hat.copy_(torch.where(trig[:, None], x_hat + dec, x_hat))
+    code[:, cb: cb + SPARQ_TAIL] = sparq_tails(trig, e)
+    return trig, e
+
+
 # ----------------------------------------------------------------- BEER ----
 # Gradient tracking with both channels gossiped as CHOCO codes: channel 0 codes theta - h, channel 1 codes v - g, with
 # CHOCO's encoder, decoder and byte layout.

@@ -130,6 +130,7 @@ struct ConsensusOp {
   consensus::PgaArgs<T> pa{};
   consensus::DpArgs<T> dp{};
   consensus::MoniquaArgs<T> mq{};
+  consensus::SparqArgs<T> sq{};
   consensus::DAdaptiveArgs<T> ad{};
   consensus::RelayArgs<T> rs{};
   consensus::PgArgs<T> pg{};
@@ -141,7 +142,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c; sq.c = c;
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -178,6 +179,12 @@ struct ConsensusOp {
     mq.key0 = d.contains("mq_key0") ? (unsigned)d["mq_key0"].cast<unsigned long long>() : 0u;
     mq.key1 = d.contains("mq_key1") ? (unsigned)d["mq_key1"].cast<unsigned long long>() : 0u;
     mq.code_stride = d.contains("code_stride") ? d["code_stride"].cast<long long>() : 0;
+    sq.x_hat = ptr<T>(d, "x_hat"); sq.s = ptr<T>(d, "s"); sq.live = ptr<const unsigned>(d, "live");
+    sq.thr = ptr<const double>(d, "sparq_thr"); sq.norm_part = ptr<double>(d, "norm_part"); sq.pstride = geti(d, "pstride", 0);
+    sq.triggers = ptr<long long>(d, "sparq_triggers"); sq.gamma = (T)getf(d, "gamma", 1.0); sq.code = geti(d, "code", 0);
+    sq.code_bytes = d.contains("sparq_code_bytes") ? d["sparq_code_bytes"].cast<long long>() : 0;
+    sq.row_stride = d.contains("row_stride") ? d["row_stride"].cast<long long>() : 0;
+    sq.H = geti(d, "local_steps", 1);
     ad.m = ptr<T>(d, "ad_m"); ad.v = ptr<T>(d, "ad_v"); ad.vhat = ptr<T>(d, "vhat"); ad.ut = ptr<T>(d, "ut");
     ad.beta1 = (T)getf(d, "beta1", 0.9); ad.beta2 = (T)getf(d, "beta2", 0.999); ad.eps = (T)getf(d, "ad_eps", 1e-8);
     ad.adagrad = geti(d, "adagrad", 0); ad.tracking = geti(d, "tracking", 1);
@@ -308,6 +315,32 @@ struct ConsensusOp {
       throw std::runtime_error(std::string(what) + " needs `mq_bits` in {2, 4, 8}, the `live` mask, the `mq_margin` "
                                "counters, `mq_B` > 0, rows padded to a multiple of 128, `code_stride` = n_pad * bits / 8, "
                                "one published channel and the pointer-table neighbors");
+  }
+  void sparq_check(const char* what) const {
+    if (sq.x_hat == nullptr || sq.s == nullptr || sq.live == nullptr || sq.thr == nullptr || sq.norm_part == nullptr ||
+        sq.triggers == nullptr || sq.pstride <= 0 || sq.H < 1 || sq.code_bytes <= 0 || sq.code_bytes % 16 != 0 ||
+        sq.row_stride != sq.code_bytes + 16 || c.n_pad % 128 != 0 || c.dmax > 256 || c.C != 1 || c.sum_mode ||
+        !(sq.code == 0 || sq.code == 1 || sq.code == 2))
+      throw std::runtime_error(std::string(what) + " needs the SPARQ rows `x_hat`, `s`, the `live` mask, the threshold "
+                               "schedule `sparq_thr`, the fp64 partials `norm_part` and `pstride`, the `sparq_triggers` "
+                               "counters, `local_steps` >= 1, a code of none / int8 / sign with `sparq_code_bytes` (a "
+                               "multiple of 16) and `row_stride` = sparq_code_bytes + 16, rows padded to a multiple of "
+                               "128, at most 256 neighbors, one published channel and the pointer-table neighbors");
+  }
+  void sparq_mix() {
+    sparq_check("sparq_mix");
+    check(consensus::launch_sparq_mix<T>(sq, cur_stream()), "sparq_mix");
+  }
+  void sparq_step(int step) {
+    sparq_check("sparq_step");
+    if (step < 0 || step >= sq.H)
+      throw std::runtime_error("sparq_step: step " + std::to_string(step) + " outside 0.." + std::to_string(sq.H - 1));
+    sq.step = step;
+    check(consensus::launch_sparq_step<T>(sq, cur_stream()), "sparq_step");
+  }
+  void sparq_publish() {
+    sparq_check("sparq_publish");
+    check(consensus::launch_sparq_publish<T>(sq, cur_stream()), "sparq_publish");
   }
   void mq_mix() {
     mq_check("mq_mix");
@@ -461,6 +494,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("dp_step", &ConsensusOp<T>::dp_step)
       .def("mq_mix", &ConsensusOp<T>::mq_mix)
       .def("mq_step", &ConsensusOp<T>::mq_step)
+      .def("sparq_mix", &ConsensusOp<T>::sparq_mix)
+      .def("sparq_step", &ConsensusOp<T>::sparq_step)
+      .def("sparq_publish", &ConsensusOp<T>::sparq_publish)
       .def("dadaptive_mix", &ConsensusOp<T>::dadaptive_mix)
       .def("dadaptive_step", &ConsensusOp<T>::dadaptive_step)
       .def("relay_mix", &ConsensusOp<T>::relay_mix)

@@ -1683,6 +1683,195 @@ __global__ void __launch_bounds__(THREADS) mq_step_kernel(const MoniquaArgs<T> a
   end_step(c, l, ri.k, true);
 }
 
+// ---------------------------------------------------------------- SPARQ-SGD ----
+// Round k (layout and rules in consensus.h: SparqArgs): sparq_mix, H x [fwd/bwd, sparq_step(p)], sparq_publish.
+// sparq_mix reads the tails of the node's own row and of its neighbors' rows of parity k & 1 after the round-start wait,
+// lists the triggered neighbor slots in table order (one warp ballot per 32 slots; a node has at most THREADS
+// neighbors, ops/engine.py: check_wait_capacity) and runs choco_mix's arithmetic over the own row, when triggered, and
+// the listed slots only: a row whose tail says 0 is never read past its tail.  With a zero code choco_mix would add
+// W_ij * 0 for it, so with every code of a non-triggered node zero (threshold 0) the mix is choco_mix bit for bit.
+template <typename T, int Q>
+__global__ void __launch_bounds__(THREADS) sparq_mix_kernel(const SparqArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  __shared__ int slot[THREADS];
+  __shared__ unsigned wmask[THREADS / 32];
+  __shared__ int own_trig;
+  const char* own = sparq_row(a, ri.par, l);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int e = threadIdx.x;
+  const bool f = e < deg && sparq_trig(reinterpret_cast<const char*>(nbr_row(c, ri.gid, l, e, ri.par, 0)), a.code_bytes);
+  const unsigned m = __ballot_sync(0xffffffffu, f);
+  if (lane == 0) wmask[warp] = m;
+  if (threadIdx.x == 0) own_trig = sparq_trig(own, a.code_bytes);
+  __syncthreads();
+  int before = 0, nsel = 0;
+#pragma unroll
+  for (int q = 0; q < THREADS / 32; ++q) {
+    const int cnt = __popc(wmask[q]);
+    before += q < warp ? cnt : 0;
+    nsel += cnt;
+  }
+  if (f) slot[before + __popc(m & ((1u << lane) - 1u))] = e;
+  __syncthreads();
+  const bool ot = own_trig != 0;
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const unsigned lw = Q == kCodeSign ? a.live[i >> 5] : 0u;
+    Pack<T> t;
+    if (ot) {
+      t = choco_decode<T, Q>(own, c.n_pad, i, lw);
+#pragma unroll
+      for (int u = 0; u < N; ++u) t.v[u] *= ws;
+    } else {
+#pragma unroll
+      for (int u = 0; u < N; ++u) t.v[u] = (T)0;
+    }
+    for_neighbors<4>(nsel, [&](int j) {
+                       return choco_decode<T, Q>(reinterpret_cast<const char*>(nbr_row(c, ri.gid, l, slot[j], ri.par, 0)),
+                                                 c.n_pad, i, lw);
+                     },
+                     [&](int j, const Pack<T>& q) {
+                       const T we = w[slot[j]];
+#pragma unroll
+                       for (int u = 0; u < N; ++u) t.v[u] += we * q.v[u];
+                     });
+    Pack<T> s = ldv(a.s + row + i);
+    const Pack<T> xh = ldv(a.x_hat + row + i);
+    Pack<T> th = ldv(c.theta + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      s.v[u] += t.v[u];
+      th.v[u] += a.gamma * (s.v[u] - xh.v[u]);
+    }
+    stv(a.s + row + i, s);
+    stv(c.theta + row + i, th);
+  }
+}
+
+// Local step p of H: theta -= alpha_k g (dsgd_step's expression).  The loop walks dp_norm's chunks (chunk ch is the
+// grid-stride iteration that covers it), so the last step writes one fp64 partial of sum (theta - x_hat)^2 per chunk,
+// reduced as dp_norm reduces: in element order per thread, xor shuffles per warp, warps in order.  The partials do not
+// depend on the grid, the local node count or the launch order.  Steps p < H - 1 end as K-GT's do; the last one leaves
+// the draw counter and the round to sparq_publish, which ends the round without drawing again (H draws per round).
+// As kgt_step, the 4-deep variant is held to 64 registers and the 8-deep one to 128: left to the compiler, the 8-deep
+// steps spilled at 64.
+template <typename T, int U, bool LAST>
+__global__ void __launch_bounds__(THREADS, U <= 4 ? 4 : 2) sparq_step_kernel(const SparqArgs<T> a) {
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const T alpha = c.alpha[ri.k];
+  const size_t row = (size_t)l * c.n_pad;
+  const int nchunk = cg_chunks(c);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __shared__ double red[THREADS / 32];
+  // theta (the mix or the previous step, two launches back) and x_hat (the previous round's publish) are read before
+  // the programmatic-dependency wait; only the gradient partials of the forward/backward kernel after it
+  bool waited = false;
+  for (int ch = blockIdx.x; ch < nchunk; ch += gridDim.x) {
+    const int i = (ch * THREADS + threadIdx.x) * N;
+    double sq = 0.0;
+    if (i < c.n_pad) {
+      Pack<T> th = ldv(c.theta + row + i);
+      Pack<T> xh;
+      if (LAST) xh = ldv(a.x_hat + row + i);
+      release_dependents_once(waited);
+      const Pack<T> g = sum_partials<U>(c, l, i);
+#pragma unroll
+      for (int u = 0; u < N; ++u) th.v[u] -= alpha * g.v[u];
+      stv(c.theta + row + i, th);
+      if (LAST) {
+#pragma unroll
+        for (int u = 0; u < N; ++u) {
+          const T d = th.v[u] - xh.v[u];
+          sq += (double)d * (double)d;
+        }
+      }
+    }
+    if (LAST) {
+#pragma unroll
+      for (int o = 16; o >= 1; o >>= 1) sq += __shfl_xor_sync(0xffffffffu, sq, o);
+      if (lane == 0) red[warp] = sq;
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        double t = red[0];
+#pragma unroll
+        for (int q = 1; q < THREADS / 32; ++q) t += red[q];
+        a.norm_part[(size_t)l * a.pstride + ch] = t;
+      }
+      __syncthreads();
+    }
+  }
+  release_dependents_once(waited);
+  if (!LAST) end_step(c, l, ri.k, false);
+}
+
+// e_i = the partials in chunk order (thread 0, into shared memory: every CTA of the node takes the same decision) and
+// trig = e_i > thr[k].  On a trigger the code of v = theta - x_hat goes into parity (k+1) & 1 with choco_encode and
+// x_hat += dec; a non-triggered node writes no code byte.  CTA 0 of the node writes the tail and counts the trigger.
+template <typename T, int Q>
+__global__ void __launch_bounds__(THREADS) sparq_publish_kernel(const SparqArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  __shared__ double esh;
+  if (threadIdx.x == 0) {
+    const double* np = a.norm_part + (size_t)l * a.pstride;
+    const int nchunk = cg_chunks(c);
+    double s = 0.0;
+    for (int ch = 0; ch < nchunk; ++ch) s += np[ch];
+    esh = s;
+  }
+  __syncthreads();
+  const double e = esh;
+  const bool trig = e > a.thr[ri.k];
+  char* out = sparq_row(a, ri.par ^ 1, l);
+  const size_t row = (size_t)l * c.n_pad;
+  const int lane = threadIdx.x & 31;
+  if (trig) {
+    for (int w0 = (blockIdx.x * THREADS + (threadIdx.x & ~31)) * N; w0 < c.n_pad; w0 += gridDim.x * THREADS * N) {
+      const int i = w0 + lane * N;
+      const bool in = i < c.n_pad;
+      Pack<T> th, xh, v;
+#pragma unroll
+      for (int u = 0; u < N; ++u) { th.v[u] = (T)0; xh.v[u] = (T)0; }
+      if (in) {
+        th = ldv(c.theta + row + i);
+        xh = ldv(a.x_hat + row + i);
+      }
+#pragma unroll
+      for (int u = 0; u < N; ++u) v.v[u] = th.v[u] - xh.v[u];
+      const Pack<T> d = choco_encode<T, Q>(v, out, c.n_pad, i, in, lane, a.live);
+      if (in) {
+#pragma unroll
+        for (int u = 0; u < N; ++u) xh.v[u] += d.v[u];
+        stv(a.x_hat + row + i, xh);
+      }
+    }
+  }
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    unsigned* tail = reinterpret_cast<unsigned*>(out + a.code_bytes);
+    tail[0] = trig ? 1u : 0u;
+    tail[1] = 0u;
+    *reinterpret_cast<double*>(out + a.code_bytes + 8) = e;
+    a.triggers[l] += trig ? 1 : 0;
+  }
+  end_step(c, l, ri.k, true);
+}
+
 // ------------------------------------------------- decentralized AMSGrad / AdaGrad ----
 // Channel 0 of the published buffer is theta, channel 1 the second-moment tracker u~ (tracking).  Round k:
 // dadaptive_mix pulls the rows published at the end of round k-1, x_i = sum_j W_ij theta_j into theta and
@@ -2826,6 +3015,33 @@ template <typename T> static cudaError_t launch_mq(const MoniquaArgs<T>& a, bool
 template <typename T> cudaError_t launch_mq_mix(const MoniquaArgs<T>& a, cudaStream_t st) { return launch_mq(a, false, st); }
 template <typename T> cudaError_t launch_mq_step(const MoniquaArgs<T>& a, cudaStream_t st) { return launch_mq(a, true, st); }
 
+// sparq_mix and sparq_publish: the compressor is a template parameter, one wave each (as choco_mix); sparq_step keeps 8
+// gradient loads in flight beyond 4 partials (as kgt_step), and the last step is a variant of its own
+template <typename T> static bool sparq_ready(const SparqArgs<T>& a) {
+  return a.x_hat != nullptr && a.s != nullptr && a.live != nullptr && a.thr != nullptr && a.norm_part != nullptr &&
+         a.triggers != nullptr && a.pstride >= cg_chunks(a.c) && a.H >= 1 && a.code_bytes > 0 && a.code_bytes % 16 == 0 &&
+         a.row_stride == a.code_bytes + 16 && a.c.n_pad % 128 == 0 && a.c.dmax <= THREADS && a.c.C == 1 &&
+         !a.c.sum_mode && (a.code == kCodeNone || a.code == kCodeInt8 || a.code == kCodeSign);
+}
+template <typename T, int Q> static cudaError_t launch_sparq_q(const SparqArgs<T>& a, bool publish, cudaStream_t st) {
+  return launch_one_wave(publish ? sparq_publish_kernel<T, Q> : sparq_mix_kernel<T, Q>, a.c, a, st);
+}
+template <typename T> static cudaError_t launch_sparq(const SparqArgs<T>& a, bool publish, cudaStream_t st) {
+  if (!sparq_ready(a)) return cudaErrorInvalidValue;
+  switch (a.code) {
+    case kCodeNone: return launch_sparq_q<T, kCodeNone>(a, publish, st);
+    case kCodeInt8: return launch_sparq_q<T, kCodeInt8>(a, publish, st);
+    default: return launch_sparq_q<T, kCodeSign>(a, publish, st);
+  }
+}
+template <typename T> cudaError_t launch_sparq_mix(const SparqArgs<T>& a, cudaStream_t st) { return launch_sparq(a, false, st); }
+template <typename T> cudaError_t launch_sparq_publish(const SparqArgs<T>& a, cudaStream_t st) { return launch_sparq(a, true, st); }
+template <typename T> cudaError_t launch_sparq_step(const SparqArgs<T>& a, cudaStream_t st) {
+  if (!sparq_ready(a) || a.step < 0 || a.step >= a.H) return cudaErrorInvalidValue;
+  if (a.step == a.H - 1) return launch_by_s(sparq_step_kernel<T, 4, true>, sparq_step_kernel<T, 8, true>, a.c, a, st);
+  return launch_by_s(sparq_step_kernel<T, 4, false>, sparq_step_kernel<T, 8, false>, a.c, a, st);
+}
+
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st) {
   return launch_one_wave(dadaptive_mix_kernel<T>, a.c, a, st);
 }
@@ -2953,6 +3169,9 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_dp_step<T>(const DpArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_mq_mix<T>(const MoniquaArgs<T>&, cudaStream_t);         \
   template cudaError_t launch_mq_step<T>(const MoniquaArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_sparq_mix<T>(const SparqArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_sparq_step<T>(const SparqArgs<T>&, cudaStream_t);       \
+  template cudaError_t launch_sparq_publish<T>(const SparqArgs<T>&, cudaStream_t);    \
   template cudaError_t launch_dadaptive_mix<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_dadaptive_step<T>(const DAdaptiveArgs<T>&, cudaStream_t); \
   template cudaError_t launch_relay_mix<T>(const RelayArgs<T>&, cudaStream_t);        \

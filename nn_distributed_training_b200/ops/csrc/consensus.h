@@ -264,6 +264,35 @@ struct MoniquaArgs {
   long long code_stride;           // bytes per code row of the published buffer
 };
 
+// SPARQ-SGD (Singh, Data, George, Diggavi 2021), optimizers/sparq.py: CHOCO-SGD's compressed gossip with an event
+// trigger and H local steps, on a fixed undirected graph.  A published row is a CHOCO code row (code_bytes, layout
+// above, int8 / sign / none) followed by a 16-byte tail {uint32 trig, uint32 0, float64 e}: `row_stride` = code_bytes
+// + 16.  Round k of node i:
+//   sparq_mix:       s_i += sum over {i} u N_i with trig_j^{k-1} = 1 of W_ij dec(q_j), table order, own term first (a
+//                    row whose tail says 0 is not read past its tail); theta_i += gamma (s_i - x_hat_i)
+//   sparq_step(p):   theta_i -= alpha_k g_i, p = 0 .. H-1; the last step also writes the fp64 partials of
+//                    (theta_i - x_hat_i)^2, one per chunk of THREADS * (16 / sizeof(T)) elements (dp_norm's chunks)
+//   sparq_publish:   e_i = the partials summed in chunk order; trig = e_i > thr[k].  On a trigger q_i = Q(theta_i -
+//                    x_hat_i) into parity (k+1) & 1 and x_hat_i += dec(q_i); either way the tail {trig, 0, e_i} and
+//                    triggers[i] += trig
+// (ops/consensus_ref.py: sparq_mix_, sparq_step_, sparq_publish_, the host twin).
+template <typename T>
+struct SparqArgs {
+  Common<T> c;
+  T* x_hat;                        // [L, n_pad] public estimate: the sum of the node's decoded codes
+  T* s;                            // [L, n_pad] sum_j W_ij x_hat_j (own term included)
+  const unsigned* live;            // [n_pad / 32] live-element bits
+  const double* thr;               // [oits] trigger thresholds
+  double* norm_part;               // [L, pstride] partial sums of (theta - x_hat)^2, one per chunk
+  int pstride;                     // >= the chunk count of a row
+  long long* triggers;             // [L] rounds each local node triggered in
+  T gamma;                         // consensus step
+  int code;                        // Code (none, int8, sign)
+  long long code_bytes;            // bytes of the code part of a row
+  long long row_stride;            // code_bytes + 16
+  int step, H;                     // local step index of sparq_step, local steps per round
+};
+
 // Decentralized AMSGrad / AdaGrad (Chen, Karimi, Zhao, Li 2022), optimizers/dadaptive.py.  With `tracking` two published
 // channels, theta and the second-moment tracker u~; the mix (dadaptive_mix_kernel) writes x into theta and
 // z = sum_j W_ij u~_j into `ut`, the step turns z into the new u~ and publishes it without storing it back.  Without
@@ -426,6 +455,9 @@ template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_
 template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_mq_mix(const MoniquaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_mq_step(const MoniquaArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_sparq_mix(const SparqArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_sparq_step(const SparqArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_sparq_publish(const SparqArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_mix(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dadaptive_step(const DAdaptiveArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_relay_mix(const RelayArgs<T>& a, cudaStream_t st);

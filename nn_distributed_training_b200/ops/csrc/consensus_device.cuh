@@ -750,6 +750,16 @@ NNDT_DEVINL double mq_decode(unsigned c, double yb, double B, double& off) {
   return __dmul_rn(B, __dadd_rn(cl, n));
 }
 
+// ---- SPARQ-SGD (layout in consensus.h: SparqArgs) ----
+template <typename T>
+NNDT_DEVINL char* sparq_row(const SparqArgs<T>& a, int par, int l) {
+  return reinterpret_cast<char*>(a.c.pub) + ((size_t)par * a.c.pub_L + l) * (size_t)a.row_stride;
+}
+// the trigger bit in the tail of a published row
+NNDT_DEVINL bool sparq_trig(const char* row, long long code_bytes) {
+  return *reinterpret_cast<const unsigned*>(row + code_bytes) != 0u;
+}
+
 // ---- SGP (layout in consensus.h) ----
 template <typename T>
 NNDT_DEVINL T* sgp_row(const SgpArgs<T>& a, int par, int l) {

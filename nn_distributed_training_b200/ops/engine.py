@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua"):
+                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua", "sparq_sgd"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
@@ -186,15 +186,19 @@ class ConsensusEngine:
         self.dp = opt.alg_name == "dp_dsgd"
         # Moniqua: one channel of modulo-quantized code rows, pulled through the pointer table (mq_mix, mq_step)
         self.mq = opt.alg_name == "moniqua"
+        # SPARQ-SGD: one channel of CHOCO code rows with a 16-byte trigger tail, pulled through the pointer table
+        self.sparq = opt.alg_name == "sparq_sgd"
         push_sum = self.sgp or self.pdg
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
         # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
         # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w (Push-DIGing: both
         # channels, u with w in the tail and y, have that stride).  BEER publishes two channels of CHOCO code rows.
-        # Moniqua publishes code rows of n_pad * bits / 8 bytes.
+        # Moniqua publishes code rows of n_pad * bits / 8 bytes, SPARQ-SGD code rows followed by their trigger tail.
         if self.choco or self.beer or self.mq:
             self.row_bytes = opt.code_bytes
+        elif self.sparq:
+            self.row_bytes = opt.row_bytes
         elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
         elif self.pg:
@@ -208,7 +212,7 @@ class ConsensusEngine:
         k0 = opt.k
         p0 = K * k0                 # the protocol round of gradient round k0
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
-        if self.choco:
+        if self.choco or self.sparq:
             self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
         elif self.mq:                               # round 0 reads the codes of theta^0
             if k0 == 0:
@@ -277,6 +281,9 @@ class ConsensusEngine:
         if self.choco and G > 1:
             raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
                              f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
+        if self.sparq and G > 1:
+            raise ValueError("sparq_sgd needs a fixed graph: the planned graph sequence of this problem has "
+                             f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
         if self.beer and G > 1:
             raise ValueError("beer needs a fixed graph: the planned graph sequence of this problem has "
                              f"{G} topologies (s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a "
@@ -306,6 +313,9 @@ class ConsensusEngine:
         if self.dp and directed:
             raise ValueError("dp_dsgd needs undirected graphs: a planned graph is directed (the pairwise noise of an edge "
                              "cancels between its two ends)")
+        if self.sparq and directed:
+            raise ValueError("sparq_sgd needs undirected graphs: a planned graph is directed (its mix conserves the "
+                             "network sum only with symmetric weights)")
         if self.mq and directed:
             raise ValueError("moniqua needs undirected graphs: a planned graph is directed (its mix conserves the network "
                              "sum only with symmetric weights)")
@@ -412,7 +422,7 @@ class ConsensusEngine:
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
                          and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag or self.pga or self.dp or self.mq)
+                                  or self.detag or self.pga or self.dp or self.mq or self.sparq)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -589,6 +599,19 @@ class ConsensusEngine:
             d.update(psi=None if opt.psi is None else opt.psi.data_ptr(), live=self.t_live.data_ptr(), mq_B=float(opt.B),
                      mq_bits=int(opt.bits), mq_key0=int(opt.key[0]), mq_key1=int(opt.key[1]), node0=int(pl.lo),
                      mq_margin=opt.margin.data_ptr(), code_stride=int(self.row_bytes))
+        self.sparq_thr = None
+        if self.sparq:
+            # the trigger thresholds (float64 in either dtype), fp64 partials of sum (theta - x_hat)^2 per chunk of
+            # THREADS * (16 / itemsize) elements (dp_norm's chunks) and the optimizer's trigger counters
+            self.t_live = choco_live_words(opt.live).to(dev)
+            self.sparq_thr = torch.as_tensor(opt.threshold_table(H), dtype=torch.float64, device=dev)
+            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+            self.norm_part = torch.zeros(L * pstride, dtype=torch.float64, device=dev)
+            d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
+                     code=CHOCO_CODE[opt.compressor], sparq_code_bytes=int(opt.code_bytes),
+                     row_stride=int(self.row_bytes), sparq_thr=self.sparq_thr.data_ptr(),
+                     norm_part=self.norm_part.data_ptr(), pstride=pstride, sparq_triggers=opt.triggers.data_ptr(),
+                     local_steps=int(opt.local_steps))
         if self.sgp:
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
         if self.pdg:
@@ -620,8 +643,13 @@ class ConsensusEngine:
         and contributes one fp64 partial-sum row per rank (``global_row``, ``n_pad * 8`` bytes) to the NVLS
         reduction, once every ``period`` rounds.  A DP-DSGD round pulls what a DSGD round does: the edge noise is
         drawn on both ends, and the norm partials stay on the node.  A Moniqua row is the node's code row,
-        ``n_pad * bits / 8`` bytes, one per neighbor edge as DSGD's rows; the margin counters stay on the node."""
+        ``n_pad * bits / 8`` bytes, one per neighbor edge as DSGD's rows; the margin counters stay on the node.  A
+        SPARQ-SGD row is the code row and its 16-byte tail (``row``); every neighbor edge pulls the tail each round
+        (``tail``) and the code body only when its source triggered: ``pulled_max`` is the round where every neighbor
+        triggered, and ``pulled_bytes()`` gives what the mixes actually pulled."""
         deg = int(self.t_deg[0].sum().item())
+        if self.sparq:
+            return {"row": int(self.row_bytes), "tail": 16, "pulled_max": int(self.row_bytes) * deg}
         if self.pga:
             return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,
                     "global_row": int(self.pr.arena.n_pad) * 8, "period": int(self.opt.period)}
@@ -633,6 +661,11 @@ class ConsensusEngine:
         chans = 1 if self.relay else self.C
         return {"row": int(self.row_bytes) * chans,
                 "pulled": int(self.row_bytes) * chans * deg * reads * self.rounds_per_step}
+
+    def pulled_bytes(self) -> int:
+        """SPARQ-SGD: the bytes the mixes of the rounds run so far pulled over the whole network, exact, from the
+        trigger counters and the fixed degrees (optimizers/sparq.py: pulled_bytes)."""
+        return self.opt.pulled_bytes()
 
     def consensus_metric(self, k: int):
         """Fused consensus-error metric (csrc/consensus.cu: consensus_metric_kernel) on the rows published

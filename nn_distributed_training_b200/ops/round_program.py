@@ -21,6 +21,7 @@ A round is a short, fixed kernel sequence
     Gossip-PGA:  pga_sum, pga_mix, fwd/bwd, dsgd_step             (pga_sum returns at once on gossip rounds)
     DP-DSGD / DECOR:  dsgd_mix, fwd/bwd, dp_norm, dp_step
     Moniqua:  mq_mix, fwd/bwd, mq_step
+    SPARQ-SGD:  sparq_mix, [fwd/bwd, sparq_step(p)] x local_steps, sparq_publish
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -144,6 +145,12 @@ def _round_ops_impl(opt, eng, grads, grads_prev):
         eng.op.mq_mix()
         grads(0)
         eng.op.mq_step()
+    elif alg == "sparq_sgd":
+        eng.op.sparq_mix()
+        for p in range(opt.local_steps):
+            grads(p)
+            eng.op.sparq_step(p)
+        eng.op.sparq_publish()
     elif alg == "sgp":
         eng.op.sgp_mix()
         grads(0)
@@ -166,7 +173,7 @@ def _collect_before_capture():
 def draws_per_round(opt) -> int:
     if opt.alg_name == "dinno":
         return opt.pits
-    return opt.local_steps if opt.alg_name == "kgt" else 1
+    return opt.local_steps if opt.alg_name in ("kgt", "sparq_sgd") else 1
 
 
 class RoundProgram:
@@ -200,10 +207,11 @@ class RoundProgram:
         # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
         # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
         # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y; Moniqua publishes
-        # codes too
+        # codes too, and SPARQ-SGD code rows with a trigger tail
         attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
-                                      or self.eng.relay or self.eng.pg or self.eng.detag or self.eng.mq)
+                                      or self.eng.relay or self.eng.pg or self.eng.detag or self.eng.mq
+                                      or self.eng.sparq)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -243,6 +251,8 @@ class RoundProgram:
             return n + self.opt.gossip_steps + 2
         if self.opt.alg_name in ("gt_hsgd", "gossip_pga", "dp_dsgd"):
             return n + 4
+        if self.opt.alg_name == "sparq_sgd":
+            return n + 2 + 2 * self.opt.local_steps
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
@@ -398,7 +408,8 @@ class RoundProgram:
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua") and opt.k > 0:
+                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua",
+                            "sparq_sgd") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
@@ -410,7 +421,8 @@ class RoundProgram:
             opt.y.copy_(eng.pub[par, 1, :L])
         if opt.alg_name in ("clipped_gossip", "bridge"):
             opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
-        if opt.alg_name in ("choco_sgd", "moniqua"):     # Moniqua's psi and margin counters are its own rows
+        # Moniqua's psi and margin counters and SPARQ-SGD's x_hat, s and trigger counters are their own rows
+        if opt.alg_name in ("choco_sgd", "moniqua", "sparq_sgd"):
             opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
         if opt.alg_name == "beer":              # h, s_h, v, g, s_g and m_old are the optimizer's own rows
             opt.code_h.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))

@@ -18,13 +18,14 @@ from .powergossip import PowerGossip
 from .push_diging import PushDIGing
 from .relaysum import RelaySum
 from .sgp import SGP
+from .sparq import SparqSGD
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
               "choco_sgd": ChocoSGD, "beer": BEER, "sgp": SGP,
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
               "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD,
-              "moniqua": Moniqua}
+              "moniqua": Moniqua, "sparq_sgd": SparqSGD}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -16,13 +16,13 @@ import yaml
 import math
 
 from ..ops.consensus_ref import (BRIDGE_SCREENS, CHOCO_COMPRESSORS, DADAPTIVE_VARIANTS, MQ_BASES, MQ_BITS,
-                                 TOPK_RATIO_DEFAULT)
+                                 SPARQ_COMPRESSORS, TOPK_RATIO_DEFAULT)
 
 REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
         "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-        "moniqua")
+        "moniqua", "sparq_sgd")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -74,6 +74,8 @@ OPT_SCHEMA = {
     # rounding_seed defaults to the problem's seed (filled in by the optimizer, which knows it)
     "moniqua": {"alpha0": REQUIRED, "mu": 0.0, "bits": REQUIRED, "theta_bound": REQUIRED, "base": "dsgd",
                 "outer_iterations": REQUIRED, "update_graph": True, "profile": False},
+    "sparq_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED, "threshold": REQUIRED,
+                  "local_steps": 1, "threshold_growth": 0.0, "outer_iterations": REQUIRED, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -263,6 +265,41 @@ def _check_moniqua(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.rounding_seed must be an integer (got {s!r})")
 
 
+SPARQ_KEYS = ("alg_name", "alpha0", "mu", "gamma", "compressor", "threshold", "local_steps", "threshold_growth",
+              "outer_iterations", "update_graph", "profile")
+
+
+def _check_sparq(c: Dict[str, Any], path: str) -> None:
+    """SPARQ-SGD: DSGD's step schedule (``alpha0`` and ``mu`` finite, >= 0), ``gamma`` in (0, 1], a compressor of none,
+    int8 or sign, ``threshold`` (finite, >= 0), ``threshold_growth`` in [0, 1), ``local_steps`` (an integer >= 1), a
+    fixed graph and no other key."""
+    for key in c:
+        if key not in SPARQ_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: sparq_sgd takes no key {key!r} (its keys are alpha0, mu, gamma, "
+                              f"compressor, threshold, threshold_growth, local_steps and outer_iterations)")
+    for key in ("alpha0", "mu", "threshold"):
+        if not _real(c[key]) or not (math.isfinite(float(c[key])) and float(c[key]) >= 0.0):
+            raise ConfigError(f"{path}.{key} must be finite and >= 0 (got {c[key]!r})")
+    g = c["gamma"]
+    if not _real(g) or not (math.isfinite(float(g)) and 0.0 < float(g) <= 1.0):
+        raise ConfigError(f"{path}.gamma must be finite and in (0, 1] (got {g!r})")
+    if c["compressor"] == "topk":
+        raise ConfigError(f"{path}.compressor: sparq_sgd has no topk compressor (the top-k code is selected by a "
+                          f"cluster kernel that has no trigger); use none|int8|sign")
+    if c["compressor"] not in SPARQ_COMPRESSORS:
+        raise ConfigError(f"{path}.compressor must be one of {'|'.join(SPARQ_COMPRESSORS)} (got {c['compressor']!r})")
+    tg = c["threshold_growth"]
+    if not _real(tg) or not 0.0 <= float(tg) < 1.0:
+        raise ConfigError(f"{path}.threshold_growth must be in [0, 1) (got {tg!r})")
+    h = c["local_steps"]
+    if isinstance(h, bool) or not isinstance(h, int) or h < 1:
+        raise ConfigError(f"{path}.local_steps must be an integer >= 1 (got {h!r})")
+    # s = sum_j W_ij x_hat_j is only valid for a fixed W: the graph is never refreshed
+    if c.setdefault("update_graph", False):
+        raise ConfigError(f"{path}.update_graph: sparq_sgd needs a fixed graph (its sum of the neighbors' estimates "
+                          f"is only valid for a fixed mixing matrix)")
+
+
 def _check_bridge(c: Dict[str, Any], path: str) -> None:
     """BRIDGE: the screen, and ``b`` (an integer >= 0) with ``trimmed_mean`` only."""
     if c["screen"] not in BRIDGE_SCREENS:
@@ -316,7 +353,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
                 "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-                "moniqua")
+                "moniqua", "sparq_sgd")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -376,6 +413,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_dp_dsgd(c, path)
     if alg == "moniqua":
         _check_moniqua(c, path)
+    if alg == "sparq_sgd":
+        _check_sparq(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
