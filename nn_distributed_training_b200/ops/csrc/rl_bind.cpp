@@ -107,14 +107,36 @@ void bind_rl(py::module& m) {
     const cudaError_t e = tag::launch(a, at::cuda::getCurrentCUDAStream().stream());
     if (e != cudaSuccess) throw std::runtime_error(std::string("tag_rollout: ") + cudaGetErrorString(e));
   });
+  // The plan tag_rollout would launch with on the current device: (worlds per CTA, actors staged, RW, shared memory).
+  // Only the shapes of the description are read; its buffers may be absent.
+  m.def("tag_rollout_plan", [](const py::dict& d) {
+    const tag::Plan p = tag::plan(tag_args(d));
+    return py::make_tuple(p.wpb, p.stage, p.rw, p.smem);
+  });
+  // The plan of ppo_grads (backward) or ppo_advantages on the current device: (rows per tile, chunks per network,
+  // dynamic shared memory, workspace bytes of ppo_grads).  Only the shapes of the description are read.
+  m.def("ppo_plan", [](const py::dict& d, bool backward) {
+    const ppo::Args a = ppo_args(d);
+    if (backward && a.nl[ppo::kActor] < 1) throw std::runtime_error("ppo_plan: the gradient pass needs an actor");
+    const ppo::Plan p = ppo::plan(a, backward);
+    if (p.err != cudaSuccess) throw std::runtime_error(std::string("ppo_plan: ") + cudaGetErrorString(p.err));
+    return py::make_tuple(p.tm, p.chunks, p.smem, p.work_bytes);
+  });
   m.def("ppo_grads", [](const py::dict& d) {
     const ppo::Args a = ppo_args(d);
     if (const char* why = ppo::check(a, true)) throw std::runtime_error(std::string("ppo_grads: ") + why);
     const ppo::Plan p = ppo::plan(a, true);
     if (p.err != cudaSuccess) throw std::runtime_error(std::string("ppo_grads: ") + cudaGetErrorString(p.err));
-    // partial slots from the caching allocator, on the current device and stream
-    at::Tensor work = at::empty({(int64_t)p.work_bytes}, at::TensorOptions().dtype(at::kByte).device(at::kCUDA));
-    const cudaError_t e = ppo::grads(a, p, work.data_ptr(), at::cuda::getCurrentCUDAStream().stream());
+    // partial slots: the caller's workspace, or one from the caching allocator on the current device and stream
+    void* wp = mptr(d, "work");
+    at::Tensor work;
+    if (wp) {
+      if (d["work_bytes"].cast<uint64_t>() < p.work_bytes) throw std::runtime_error("ppo_grads: workspace too small");
+    } else {
+      work = at::empty({(int64_t)p.work_bytes}, at::TensorOptions().dtype(at::kByte).device(at::kCUDA));
+      wp = work.data_ptr();
+    }
+    const cudaError_t e = ppo::grads(a, p, wp, at::cuda::getCurrentCUDAStream().stream());
     if (e != cudaSuccess) throw std::runtime_error(std::string("ppo_grads: ") + cudaGetErrorString(e));
   });
   m.def("ppo_advantages", [](const py::dict& d) {

@@ -394,14 +394,14 @@ Plan plan(const Args& a) {
   auto bytes = [&](int w, int s) { return layout(a, w, s).total * es; };
   int stage = bytes(wpb, 1) <= (size_t)optin;
   while (!stage && wpb > 1 && bytes(wpb, 0) > (size_t)optin) wpb = wpb > 4 ? wpb - 4 : wpb - 1;
-  return Plan{wpb, stage, bytes(wpb, stage)};
+  return Plan{wpb, stage, wpb % 4 == 0 ? 4 : 1, bytes(wpb, stage)};
 }
 
 cudaError_t launch(const Args& a, cudaStream_t st) {
   if (check(a)) return cudaErrorInvalidValue;
   const Plan p = plan(a);
-  if (a.dtype64) return p.wpb % 4 == 0 ? launch_t<double, 4>(a, p, st) : launch_t<double, 1>(a, p, st);
-  return p.wpb % 4 == 0 ? launch_t<float, 4>(a, p, st) : launch_t<float, 1>(a, p, st);
+  if (a.dtype64) return p.rw == 4 ? launch_t<double, 4>(a, p, st) : launch_t<double, 1>(a, p, st);
+  return p.rw == 4 ? launch_t<float, 4>(a, p, st) : launch_t<float, 1>(a, p, st);
 }
 
 }  // namespace tag

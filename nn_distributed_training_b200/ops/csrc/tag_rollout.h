@@ -42,9 +42,10 @@ struct Args {
   void* pos_trace;         // optional [n_ep, T, E, A, 2], positions after each cycle
 };
 
-// Worlds per CTA, shared memory per CTA and whether the actors are staged in shared memory for this launch.
+// Worlds per CTA, whether the actors are staged in shared memory, worlds per register block (the kernel's RW: 4 when
+// wpb is a multiple of 4, else 1) and shared memory per CTA for this launch.
 struct Plan {
-  int wpb, stage;
+  int wpb, stage, rw;
   size_t smem;
 };
 

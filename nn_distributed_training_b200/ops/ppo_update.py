@@ -81,15 +81,18 @@ def require(actors, critics) -> None:
         raise ValueError(f"update backend 'cuda' does not support this configuration: {why}")
 
 
-def _desc(actors, critics, dtype, N, R):
-    """Kernel description of N (actor, critic) pairs; ``actors=None`` describes the critics only."""
+def _desc(actors, critics, dtype, dev, N, R):
+    """Kernel description of N (actor, critic) pairs whose parameters are on ``dev``; ``actors=None`` describes the
+    critics only."""
     crits = _as_list(critics)
     acts = _as_list(actors) if actors is not None else []
     if len(crits) != N or (actors is not None and len(acts) != N):
         raise ValueError(f"{len(acts)} actors and {len(crits)} critics for a batch of {N} nodes")
     for m in acts + crits:
         for p in m.parameters():
-            if p.dtype != dtype or p.device.type != "cuda" or not p.is_contiguous():
+            if p.device != dev:
+                raise ValueError(f"network parameter on {p.device}, batch on {dev}")
+            if p.dtype != dtype or not p.is_contiguous():
                 raise ValueError(f"network parameters must be contiguous CUDA tensors of the batch dtype {dtype}")
     lins = [[_linears(a) if actors is not None else [], _linears(c)] for a, c in zip(acts or [None] * N, crits)]
     dims = [[ln[0].in_features] + [m.out_features for m in ln] if ln else [] for ln in lins[0]]
@@ -98,9 +101,15 @@ def _desc(actors, critics, dtype, N, R):
                 b=[[[m.bias.data_ptr() for m in ln] for ln in node] for node in lins], clip=0.0, cov_var=1.0, lp_const=0.0)
 
 
+def _described(t) -> str:
+    """``t``'s shape, dtype and device as an error message shows them (a device inside a tuple would print as
+    ``device(type='cuda', index=1)``)."""
+    return f"{tuple(t.shape)} {t.dtype} on {t.device}" if torch.is_tensor(t) else type(t).__name__
+
+
 def _batch(name, t, shape, dtype, dev):
     if not torch.is_tensor(t) or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != dev:
-        got = (tuple(t.shape), t.dtype, t.device) if torch.is_tensor(t) else type(t).__name__
+        got = _described(t)
         raise ValueError(f"{name}: expected {tuple(shape)} {dtype} on {dev}, got {got}")
     return t.contiguous()
 
@@ -116,20 +125,38 @@ def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor, out: Optional[tor
         raise ValueError(f"rtgs: expected [N, R], got {tuple(rtgs.shape)}")
     N, R = rtgs.shape
     dev, dt = rtgs.device, rtgs.dtype
-    d = _desc(None, crits, dt, N, R)
+    d = _desc(None, crits, dt, dev, N, R)
     obs = _batch("obs", obs, (N, R, d["dims"][1][0]), dt, dev)
     rtgs = rtgs.contiguous()
     adv = torch.empty(N, R, device=dev, dtype=dt) if out is None else _out("out", out, (N, R), dt, dev)
     d.update(obs=obs.data_ptr(), rtgs=rtgs.data_ptr(), adv=adv.data_ptr())
-    ext.ppo_advantages(d)
+    with torch.cuda.device(dev):
+        ext.ppo_advantages(d)
     return adv
+
+
+def launch_plan(actors, critics, R: int, backward: bool = True) -> Dict[str, int]:
+    """The launch plan of ``grads`` (``backward=True``) or of ``advantages`` (``backward=False``, ``actors`` unused)
+    for these per-node networks and ``R`` samples per node on the networks' device, without launching: ``tm`` rows per
+    tile, ``chunks`` CTAs per node and network (each walks ``per = ceil(ceil(R / chunks) / tm) * tm`` rows),
+    ``smem`` bytes of dynamic shared memory per CTA and ``work_bytes`` of workspace (the partial-sum slots of
+    ``grads``; 0 for ``advantages``)."""
+    crits = _as_list(critics)
+    acts = _as_list(actors) if backward else None
+    require(acts, crits)
+    ext = load_ext(required=True)
+    p = next(crits[0].parameters())
+    d = _desc(acts, crits, p.dtype, p.device, len(crits), int(R))
+    with torch.cuda.device(p.device):
+        tm, chunks, smem, work_bytes = ext.ppo_plan(d, bool(backward))
+    return dict(tm=tm, chunks=chunks, smem=smem, work_bytes=work_bytes)
 
 
 def _out(name, t, shape, dtype, dev):
     """An output tensor the kernel writes in place: exactly ``shape``, ``dtype``, ``dev`` and contiguous."""
     if not torch.is_tensor(t) or tuple(t.shape) != tuple(shape) or t.dtype != dtype or t.device != dev \
             or not t.is_contiguous():
-        got = (tuple(t.shape), t.dtype, t.device) if torch.is_tensor(t) else type(t).__name__
+        got = _described(t)
         raise ValueError(f"{name}: expected a contiguous {tuple(shape)} {dtype} tensor on {dev}, got {got}")
     return t
 
@@ -148,7 +175,7 @@ def _grads_desc(acts_l, crits, grad_out, N, R, dt, dev):
     if d is not None:
         return d
     require(acts_l, crits)
-    d = _desc(acts_l, crits, dt, N, R)
+    d = _desc(acts_l, crits, dt, dev, N, R)
     gW, gb = [], []
     for i in range(N):
         g = list(grad_out[i])
@@ -156,7 +183,8 @@ def _grads_desc(acts_l, crits, grad_out, N, R, dt, dev):
             raise ValueError(f"grad_out[{i}]: {len(g)} tensors for {len(params[i])} parameters")
         for p, t in zip(params[i], g):
             if t.shape != p.shape or t.dtype != dt or t.device != dev or not t.is_contiguous():
-                raise ValueError(f"grad_out[{i}]: expected contiguous {tuple(p.shape)} {dt} tensors on {dev}")
+                raise ValueError(f"grad_out[{i}]: expected contiguous {tuple(p.shape)} {dt} tensors on {dev}, "
+                                 f"got {_described(t)}")
         na = len(list(acts_l[i].parameters()))
         gW.append([[t.data_ptr() for t in g[:na:2]], [t.data_ptr() for t in g[na::2]]])
         gb.append([[t.data_ptr() for t in g[1:na:2]], [t.data_ptr() for t in g[na + 1::2]]])
@@ -169,13 +197,15 @@ def _grads_desc(acts_l, crits, grad_out, N, R, dt, dev):
 
 def grads(actors, critics, obs: torch.Tensor, acts: torch.Tensor, old_lp: torch.Tensor, rtgs: torch.Tensor,
           adv: torch.Tensor, clip: float, cov_var: float, grad_out: Sequence[Sequence[torch.Tensor]],
-          nonfinite: Optional[torch.Tensor] = None, losses_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+          nonfinite: Optional[torch.Tensor] = None, losses_out: Optional[torch.Tensor] = None,
+          workspace: Optional[torch.Tensor] = None) -> torch.Tensor:
     """One primal step of every node: writes the gradients of node ``i``'s PPO-clip actor loss and critic MSE into
     ``grad_out[i]`` — one tensor per parameter, in ``parameters()`` order of the actor then the critic (arena-row views
     or ``p.grad``) — and returns ``losses [N, 2]`` (actor, critic), written into ``losses_out`` when given (a
     contiguous ``[N, 2]`` tensor of the batch dtype, for example a row of a buffer a CUDA graph replays into).
-    ``nonfinite``, an int32 CUDA tensor, is set to 1 if an actor mean is not finite; it is never cleared here.  Nothing
-    is synchronised."""
+    ``nonfinite``, an int32 CUDA tensor, is set to 1 if an actor mean is not finite; it is never cleared here.
+    ``workspace``: a contiguous, 16-byte aligned uint8 tensor on the batch's device of at least ``launch_plan(...)["work_bytes"]``
+    bytes for the per-CTA partial sums (default: one from the caching allocator per call).  Nothing is synchronised."""
     acts_l, crits = _as_list(actors), _as_list(critics)
     ext = load_ext(required=True)
     if rtgs.dim() != 2:
@@ -199,5 +229,12 @@ def grads(actors, critics, obs: torch.Tensor, acts: torch.Tensor, old_lp: torch.
              adv=adv.data_ptr(), clip=float(clip), cov_var=float(cov_var),
              lp_const=0.5 * ACT_DIM * math.log(2 * math.pi * cov_var), losses=losses.data_ptr(),
              nonfinite=nonfinite.data_ptr())
-    ext.ppo_grads(d)
+    if workspace is not None:
+        if workspace.dtype != torch.uint8 or workspace.device != dev or not workspace.is_contiguous() \
+                or workspace.data_ptr() % 16:
+            raise ValueError(f"workspace: expected a contiguous, 16-byte aligned uint8 tensor on {dev}, "
+                             f"got {_described(workspace)}")
+        d.update(work=workspace.data_ptr(), work_bytes=workspace.numel())
+    with torch.cuda.device(dev):
+        ext.ppo_grads(d)
     return losses

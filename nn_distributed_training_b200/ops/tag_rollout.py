@@ -107,39 +107,30 @@ def reset_positions(env, n_ep: int) -> torch.Tensor:
     return torch.stack(out)
 
 
-def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_scale: float = 1.0, key: int = 0,
-            index: int = 0, pos0: Optional[torch.Tensor] = None, debug: bool = False,
-            out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
-    """Run ``n_ep`` episodes of ``T`` cycles in ``env.E`` worlds each.  ``actors``: one module shared by every predator,
-    or one per predator.  ``pos0`` defaults to ``reset_positions(env, n_ep)``.  ``debug`` adds the standard-normal
-    draws ``eps [N, R, 5]`` and the positions after every cycle ``pos [n_ep, T, E, A, 2]``.  ``out``: contiguous
-    ``obs`` / ``acts`` / ``log_probs`` / ``rtgs`` tensors of the batch's shapes to write into (persistent buffers);
-    the returned dict holds them.  Afterwards ``env`` holds the last episode's final state, as after the torch loop."""
-    require(env, actors)
-    ext = load_ext(required=True)
-    dev, dt = env.device, env.dtype
-    N, E, A = env.n_adv, env.E, env.A
-    T, n_ep = int(T), int(n_ep)
-    if T < 1 or n_ep < 1:
-        raise ValueError("T and n_ep must be >= 1")
-    if pos0 is None:
-        pos0 = reset_positions(env, n_ep)
-    pos0 = pos0.to(device=dev, dtype=dt).contiguous()
-    if tuple(pos0.shape) != (n_ep, E, A, 2):
-        raise ValueError(f"pos0 has shape {tuple(pos0.shape)}, expected {(n_ep, E, A, 2)}")
-    acts_in = _actor_list(env, actors)
+def _distinct(env, actors):
+    """The distinct actor modules and, per predator, the index of its actor among them."""
     distinct: List[nn.Module] = []
     actor_of = []
-    for a in acts_in:
+    for a in _actor_list(env, actors):
         k = next((j for j, d in enumerate(distinct) if d is a), None)
         if k is None:
             distinct.append(a)
             k = len(distinct) - 1
         actor_of.append(k)
-    keep = []                                            # contiguous copies stay alive until the launch returns
+    return distinct, actor_of
+
+
+def describe(env, actors, T: int, n_ep: int, gamma: float = 1.0, cov_var: float = 1.0, noise_scale: float = 1.0,
+             key: int = 0, index: int = 0, keep: Optional[list] = None) -> dict:
+    """Kernel description of the actors, the environment and the episode shape, without the start positions and the
+    output buffers.  Every actor parameter must be on the environment's device; non-contiguous ones are copied, and
+    the copies are appended to ``keep``, which must outlive the launch."""
+    require(env, actors)
+    dev = env.size.device
+    keep = [] if keep is None else keep
 
     def ptr(t):
-        if t.device.type != "cuda":
+        if t.device != dev:
             raise ValueError(f"actor parameter on {t.device}, environment on {dev}")
         t = t.detach()
         if not t.is_contiguous():
@@ -147,34 +138,72 @@ def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_
             keep.append(t)
         return t.data_ptr()
 
+    distinct, actor_of = _distinct(env, actors)
     lins = [_linears(a) for a in distinct]
     dims = [lins[0][0].in_features] + [m.out_features for m in lins[0]]
+    return dict(dtype64=int(env.dtype == torch.float64), dims=dims, actor_of=actor_of,
+                W=[[ptr(m.weight) for m in lin] for lin in lins], b=[[ptr(m.bias) for m in lin] for lin in lins],
+                N=env.n_adv, n_good=env.n_good, A=env.A, n_obst=env.n_obs,
+                size=env.size.data_ptr(), accel=env.accel.data_ptr(), max_speed=env.max_speed.data_ptr(),
+                obst=env.obst.data_ptr() if env.n_obs else None,
+                E=env.E, n_ep=int(n_ep), T=int(T), gamma=float(gamma), cov_var=float(cov_var),
+                noise_std=float(noise_scale) * math.sqrt(cov_var),
+                lp_const=0.5 * ACT_DIM * math.log(2 * math.pi * cov_var), key=int(key) & (2 ** 64 - 1),
+                index=int(index) & 0xFFFFFFFF)
+
+
+def launch_plan(env, actors, T: int, n_ep: int) -> Dict[str, int]:
+    """The launch plan ``rollout`` would use for this environment, these actors and this episode shape on the
+    environment's device, without launching: ``wpb`` worlds per CTA, ``stage`` (1: the actors are copied into shared
+    memory, 0: read in place), ``rw`` worlds per register block and ``smem`` bytes of shared memory per CTA."""
+    ext = load_ext(required=True)
+    keep: list = []
+    d = describe(env, actors, T, n_ep, keep=keep)
+    with torch.cuda.device(env.size.device):
+        wpb, stage, rw, smem = ext.tag_rollout_plan(d)
+    return dict(wpb=wpb, stage=stage, rw=rw, smem=smem)
+
+
+def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_scale: float = 1.0, key: int = 0,
+            index: int = 0, pos0: Optional[torch.Tensor] = None, debug: bool = False,
+            out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+    """Run ``n_ep`` episodes of ``T`` cycles in ``env.E`` worlds each.  ``actors``: one module shared by every predator,
+    or one per predator.  ``pos0`` defaults to ``reset_positions(env, n_ep)``.  Returns ``obs``, ``acts``,
+    ``log_probs``, ``rtgs``, ``ep_returns`` and every world's final ``final_pos`` / ``final_vel [n_ep, E, A, 2]``;
+    ``debug`` adds the standard-normal draws ``eps [N, R, 5]`` and the positions after every cycle
+    ``pos [n_ep, T, E, A, 2]``.  ``out``: contiguous tensors of the batch's shapes, dtype and device to write any of
+    these into (persistent buffers); the returned dict holds them.  Afterwards ``env`` holds the last episode's final
+    state, as after the torch loop (a copy, when ``out`` holds ``final_pos`` / ``final_vel``)."""
+    T, n_ep = int(T), int(n_ep)
+    if T < 1 or n_ep < 1:
+        raise ValueError("T and n_ep must be >= 1")
+    keep = []                                            # contiguous copies stay alive until the launch returns
+    d = describe(env, actors, T, n_ep, gamma, cov_var, noise_scale, key, index, keep)
+    ext = load_ext(required=True)
+    dev, dt = env.size.device, env.dtype
+    N, E, A = env.n_adv, env.E, env.A
+    if pos0 is None:
+        pos0 = reset_positions(env, n_ep)
+    pos0 = pos0.to(device=dev, dtype=dt).contiguous()
+    if tuple(pos0.shape) != (n_ep, E, A, 2):
+        raise ValueError(f"pos0 has shape {tuple(pos0.shape)}, expected {(n_ep, E, A, 2)}")
     R = n_ep * T * E
-    kw = dict(device=dev, dtype=dt)
-    shapes = dict(obs=(N, R, dims[0]), acts=(N, R, ACT_DIM), log_probs=(N, R), rtgs=(N, R))
+    shapes = dict(obs=(N, R, d["dims"][0]), acts=(N, R, ACT_DIM), log_probs=(N, R), rtgs=(N, R), ep_returns=(n_ep * E,),
+                  final_pos=(n_ep, E, A, 2), final_vel=(n_ep, E, A, 2))
+    if debug:
+        shapes.update(eps=(N, R, ACT_DIM), pos=(n_ep, T, E, A, 2))
     given = out or {}
     for k, t in given.items():
         if k not in shapes or not torch.is_tensor(t) or tuple(t.shape) != shapes[k] or t.dtype != dt \
-                or t.device.type != torch.device(dev).type or not t.is_contiguous():
+                or t.device != dev or not t.is_contiguous():
             raise ValueError(f"out[{k!r}]: expected a contiguous {shapes.get(k)} {dt} tensor on {dev}")
-    out = {k: given[k] if k in given else torch.empty(*shp, **kw) for k, shp in shapes.items()}
-    out["ep_returns"] = torch.empty(n_ep * E, **kw)
-    final_pos = torch.empty(n_ep, E, A, 2, **kw)
-    final_vel = torch.empty(n_ep, E, A, 2, **kw)
-    if debug:
-        out["eps"] = torch.empty(N, R, ACT_DIM, **kw)
-        out["pos"] = torch.empty(n_ep, T, E, A, 2, **kw)
-    d = dict(dtype64=int(dt == torch.float64), dims=dims, actor_of=actor_of,
-             W=[[ptr(m.weight) for m in lin] for lin in lins], b=[[ptr(m.bias) for m in lin] for lin in lins],
-             N=N, n_good=env.n_good, A=A, n_obst=env.n_obs,
-             size=env.size.data_ptr(), accel=env.accel.data_ptr(), max_speed=env.max_speed.data_ptr(),
-             obst=env.obst.data_ptr() if env.n_obs else None,
-             E=E, n_ep=n_ep, T=T, pos0=pos0.data_ptr(), gamma=float(gamma), cov_var=float(cov_var),
-             noise_std=float(noise_scale) * math.sqrt(cov_var),
-             lp_const=0.5 * ACT_DIM * math.log(2 * math.pi * cov_var), key=int(key) & (2 ** 64 - 1),
-             index=int(index) & 0xFFFFFFFF, final_pos=final_pos.data_ptr(), final_vel=final_vel.data_ptr(),
-             eps=out["eps"].data_ptr() if debug else None, pos_trace=out["pos"].data_ptr() if debug else None,
+    out = {k: given[k] if k in given else torch.empty(*shp, device=dev, dtype=dt) for k, shp in shapes.items()}
+    d.update(pos0=pos0.data_ptr(), eps=out["eps"].data_ptr() if debug else None,
+             pos_trace=out["pos"].data_ptr() if debug else None,
              **{k: v.data_ptr() for k, v in out.items() if k not in ("eps", "pos")})
-    ext.tag_rollout(d)
-    env.pos, env.vel, env.cycle = final_pos[-1], final_vel[-1], T
+    with torch.cuda.device(dev):
+        ext.tag_rollout(d)
+    # the environment keeps its own copy of a caller's persistent buffer, which the next rollout into it overwrites
+    final = {k: out[k][-1].clone() if k in given else out[k][-1] for k in ("final_pos", "final_vel")}
+    env.pos, env.vel, env.cycle = final["final_pos"], final["final_vel"], T
     return out

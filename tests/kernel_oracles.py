@@ -11,6 +11,8 @@
   float64; its yardstick is the same function at the TF32 rounding of the parameters, the rows and dL/dout.
 * ``mlp_bf16_faithful`` is the density MLP of ``csrc/mlp_tc.cu`` written out by hand, rounding to bf16 exactly where
   the kernel rounds and nowhere else; ``rounding=False`` gives the exact math of the same network.
+* ``Guarded`` packs a kernel's output tensors, poisoned with NaN, between guard values in one buffer, so a skipped
+  or an out-of-range write shows.
 * ``assert_close_to_oracle`` accepts a kernel when its error is a small fraction of a yardstick's error, per tensor and
   per 16 x 8 block, so one bad MMA tile cannot hide inside a good norm.
 """
@@ -349,6 +351,26 @@ def mlp_named(shape, out, hs, g, dx=None):
     if dx is not None:
         out_d["dx"] = dx.reshape(-1, int(shape[0]))
     return out_d
+
+
+# ---- poisoned outputs -----------------------------------------------------------------------------------------------
+class Guarded:
+    """Tensors of the given shapes, each filled with NaN, packed in one buffer with ``gap`` guard values before,
+    between and after them (contiguous views, as arena rows are)."""
+    GUARD = 1234.5
+
+    def __init__(self, shapes, dtype, device, gap=7):
+        sizes = [math.prod(s) for s in shapes]
+        self.buf = torch.full((sum(sizes) + gap * (len(shapes) + 1),), self.GUARD, dtype=dtype, device=device)
+        self.guard = torch.ones(self.buf.shape, dtype=torch.bool, device=device)
+        self.views, off = [], gap
+        for s, n in zip(shapes, sizes):
+            self.views.append(self.buf[off: off + n].view(s).fill_(float("nan")))
+            self.guard[off: off + n] = False
+            off += n + gap
+
+    def assert_guards(self, what=""):
+        assert (self.buf[self.guard] == self.GUARD).all(), (what, "a write outside the outputs")
 
 
 # ---- acceptance ------------------------------------------------------------------------------------------------------

@@ -17,7 +17,8 @@ import torch
 
 import consensus_oracle as co
 from test_gpu_consensus_kernels import C, NPDT, ROUNDS, Harness, KernelProblem, _snap
-from test_gpu_ppo_update import F32_FLOOR, _batch, _copy_params, _load, _problem, _rel
+from ppo_oracle import F32_FLOOR, rel as _rel
+from test_gpu_ppo_update import _batch, _copy_params, _load, _problem
 from nn_distributed_training_b200.ops.round_program import RoundProgram
 from nn_distributed_training_b200.optimizers import DSGT
 from nn_distributed_training_b200.rl import DSGDPPO, DSGTPPO, DiNNOPPO

@@ -11,24 +11,17 @@ gradient summed over R samples by about 1/sqrt(R) (3e-4 at 204,800).  So the rec
 pre-activation and every ratio a margin away from the jumps (``_batch``); the yardstick then measures rounding, not
 which side of a kink a sample happened to land on.
 """
-import math
-
 import networkx as nx
 import pytest
 import torch
 
 from nn_distributed_training_b200.ops import ppo_update
 from nn_distributed_training_b200.rl import DSGDPPO, DSGTPPO, DiNNOPPO, PPO, DistPPOProblem, FFReLUNet, SimpleTagEnv
+from ppo_oracle import F32_FLOOR, KINK_MARGIN, make_batch, rel
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 COV, CLIP = 0.5, 0.2
-F32_FLOOR = 8 * torch.finfo(torch.float32).eps
-KINK_MARGIN = 1e-4   # far above the fp32 error of a pre-activation (~1e-6 of the sum of its absolute terms)
-
-
-def _rel(x, ref):
-    return float((x.double() - ref.double()).norm() / ref.double().norm().clamp_min(1e-300))
 
 
 def _problem(N, hidden, dtype, n_good=1, seed=0, **kw):
@@ -46,47 +39,11 @@ def _problem(N, hidden, dtype, n_good=1, seed=0, **kw):
     return pr
 
 
-def near_kinks(pr, obs, margin=KINK_MARGIN):
-    """[N, R] bool: rows where a hidden pre-activation of node i's actor or critic lies within ``margin`` of the ReLU kink,
-    relative to the sum of the absolute values of its terms, in float64."""
-    near = torch.zeros(obs.shape[:2], dtype=torch.bool, device=DEV)
-    with torch.no_grad():
-        for i in range(pr.N):
-            for net in (pr.models[i].actor, pr.models[i].critic):
-                h = obs[i].double()
-                for m in [m for m in net.seq if isinstance(m, torch.nn.Linear)][:-1]:
-                    W, b = m.weight.double(), m.bias.double()
-                    z = h @ W.T + b
-                    near[i] |= (z.abs() < margin * (h.abs() @ W.abs().T + b.abs())).any(-1)
-                    h = z.clamp_min(0)
-    return near
-
-
 def _batch(pr, R, seed=1, spread=0.3, kink_margin=KINK_MARGIN):
-    """A recorded batch [N, R, ...]: acts around the current actor means, so the ratios spread around 1 and some clip.
-    Observations that put a hidden pre-activation within ``kink_margin`` of a ReLU kink are redrawn."""
-    g = torch.Generator(device=DEV).manual_seed(seed)
-    N, dt = pr.N, next(pr.models[0].parameters()).dtype
-    d0 = pr.obs_dim
-    obs = torch.randn(N, R, d0, device=DEV, dtype=dt, generator=g)
-    for _ in range(100 if kink_margin else 0):
-        near = near_kinks(pr, obs, kink_margin)
-        if not near.any():
-            break
-        obs = torch.where(near[..., None], torch.randn(N, R, d0, device=DEV, dtype=dt, generator=g), obs)
-    else:
-        assert not kink_margin or not near_kinks(pr, obs, kink_margin).any()
-    with torch.no_grad():
-        mean = torch.stack([pr.models[i].actor(obs[i]) for i in range(N)])
-    acts = mean + math.sqrt(COV) * torch.randn(N, R, 5, device=DEV, dtype=dt, generator=g)
-    lp = pr._log_prob(mean, acts)
-    old_lp = lp + spread * torch.randn(N, R, device=DEV, dtype=dt, generator=g)
-    # the clip edges r = 1 +- clip: keep every ratio 1e-3 away from both (multiplying a near one by e^0.01)
-    r = torch.exp(lp - old_lp)
-    near = ((r - (1 - CLIP)).abs() < 1e-3) | ((r - (1 + CLIP)).abs() < 1e-3)
-    old_lp = torch.where(near, old_lp - 0.01, old_lp)
-    rtgs = 3.0 * torch.randn(N, R, device=DEV, dtype=dt, generator=g) - 1.0
-    return dict(obs=obs, acts=acts, log_probs=old_lp, rtgs=rtgs)
+    """A recorded batch [N, R, ...] from ``ppo_oracle.make_batch``: acts around the current actor means, so the ratios
+    spread around 1 and some clip; no hidden pre-activation within ``kink_margin`` of a ReLU kink."""
+    return make_batch([pr.models[i].actor for i in range(pr.N)], [pr.models[i].critic for i in range(pr.N)], R, CLIP,
+                      COV, seed=seed, spread=spread, kink_margin=kink_margin)
 
 
 def _load(pr, batch):
@@ -142,15 +99,15 @@ def test_fp64_against_autograd(N, hidden, n_good, R):
         if R == 1:   # unbiased std of one sample
             assert torch.isnan(pr.A_k[i]).all() and torch.isnan(ref.A_k[i]).all()
         else:
-            assert _rel(pr.A_k[i], ref.A_k[i]) < 1e-12
+            assert rel(pr.A_k[i], ref.A_k[i]) < 1e-12
     adv = pr._adv if R > 1 else torch.randn(N, R, device=DEV, dtype=torch.float64)
     if R == 1:
         ref.A_k = {i: adv[i] for i in range(N)}
     losses, grads = _kernel(pr, adv)
     for i, (l_ref, g_ref) in enumerate(_autograd(ref)):
-        assert _rel(losses[i], l_ref) < 1e-12, (i, losses[i], l_ref)
+        assert rel(losses[i], l_ref) < 1e-12, (i, losses[i], l_ref)
         for k, (g, gr) in enumerate(zip(grads[i], g_ref)):
-            assert _rel(g, gr) < 1e-9, (i, k, _rel(g, gr))
+            assert rel(g, gr) < 1e-9, (i, k, rel(g, gr))
 
 
 @pytest.mark.parametrize("N,hidden,n_good,R", [c for c in CASES if c[3] > 1])
@@ -165,7 +122,7 @@ def test_fp32_against_the_torch_fp32_yardstick(N, hidden, n_good, R):
         _load(pr, batch)
         pr.update_advantage()
     for i in range(N):
-        e_t, e_k = _rel(t32.A_k[i], ref.A_k[i]), _rel(k32.A_k[i], ref.A_k[i])
+        e_t, e_k = rel(t32.A_k[i], ref.A_k[i]), rel(k32.A_k[i], ref.A_k[i])
         assert e_k <= 4 * max(e_t, F32_FLOOR), ("adv", i, e_k, e_t)
     adv = k32._adv.double()   # one advantage for all three, so the gradients compare the update alone
     ref.A_k = {i: adv[i] for i in range(N)}
@@ -173,10 +130,10 @@ def test_fp32_against_the_torch_fp32_yardstick(N, hidden, n_good, R):
     losses, grads = _kernel(k32, adv.float())
     for i, ((l_ref, g_ref), (l_t, g_t)) in enumerate(zip(_autograd(ref), _autograd(t32))):
         for n in range(2):
-            e_t, e_k = _rel(l_t[n], l_ref[n]), _rel(losses[i, n], l_ref[n])
+            e_t, e_k = rel(l_t[n], l_ref[n]), rel(losses[i, n], l_ref[n])
             assert e_k <= 4 * max(e_t, F32_FLOOR), ("loss", i, n, e_k, e_t)
         for k, (g, gt, gr) in enumerate(zip(grads[i], g_t, g_ref)):
-            e_t, e_k = _rel(gt, gr), _rel(g, gr)
+            e_t, e_k = rel(gt, gr), rel(g, gr)
             assert e_k <= 4 * max(e_t, F32_FLOOR), ("grad", i, k, e_k, e_t)
 
 
@@ -198,9 +155,9 @@ def test_clip_semantics_against_autograd():
     ref.A_k = {i: adv[i] for i in range(3)}
     losses, grads = _kernel(pr, adv)
     for i, (l_ref, g_ref) in enumerate(_autograd(ref)):
-        assert _rel(losses[i], l_ref) < 1e-12
+        assert rel(losses[i], l_ref) < 1e-12
         for g, gr in zip(grads[i], g_ref):
-            assert _rel(g, gr) < 1e-12
+            assert rel(g, gr) < 1e-12
 
 
 @pytest.mark.parametrize("dtype", [torch.float32, torch.float64])
@@ -253,7 +210,7 @@ def test_whole_runs_match_the_torch_update(cls, conf):
             pr.check_update()
         out.append(torch.cat([torch.nn.utils.parameters_to_vector(pr.models[i].parameters()) for i in range(3)]))
         assert not torch.equal(out[-1], start)
-    assert _rel(out[1], out[0]) < 1e-8
+    assert rel(out[1], out[0]) < 1e-8
 
 
 def test_end_to_end_dinno_ppo_with_both_kernels(tmp_path):

@@ -1,10 +1,5 @@
 """The fused predator-prey rollout kernel (ops/csrc/tag_rollout.cu) against the float64 replay oracle, its noise, and
-the RL entry points that run it.
-
-Contacts are stiff, so rounding differences grow along a trajectory.  The fp64 kernel is therefore held to a
-yardstick: the oracle's own divergence when ``pos0`` moves by one ulp (running max over the cycles so far, taken over
-all worlds); the kernel's error must stay within 10x of it, with a floor of 1e-12 of the quantity's scale.  The fp32
-kernel is held to 4x the error of the torch fp32 path against the same fp64 oracle, with a floor of a few fp32 ulps.
+the RL entry points that run it.  The yardsticks (``check_fp64``, ``fp32_ratio``) are those of tests/tag_rollout_oracle.py.
 """
 import os
 
@@ -16,18 +11,13 @@ import torch
 from nn_distributed_training_b200.ops import tag_rollout
 from nn_distributed_training_b200.rl import DSGDPPO, DSGTPPO, DiNNOPPO, PPO, DistPPOProblem, FFReLUNet, SimpleTagEnv
 from nn_distributed_training_b200.rl.eval_policy import load_distributed_actors, rollout as eval_rollout
-from tag_rollout_oracle import replay_tag_rollout
+from tag_rollout_oracle import COV, GAMMA, check_fp64 as _check_fp64, fp32_ratio as _fp32_ratio, on as _on, \
+    run_kernel as _run_kernel, tag_env as _env
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TRAINED = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "nn_distributed_training_b200", "rl",
                        "trained")
-GAMMA, COV = 0.99, 0.5
-
-
-def _env(E=16, n_adv=3, n_good=1, n_obst=8, max_cycles=200, dtype=torch.float64, device=DEV, seed=0):
-    return SimpleTagEnv(num_envs=E, num_good=n_good, num_adversaries=n_adv, num_obstacles=n_obst, max_cycles=max_cycles,
-                        device=device, dtype=dtype, seed=seed)
 
 
 def _actors(env, dtype, hidden=(64, 64, 64), seed=1, shipped=False):
@@ -40,68 +30,6 @@ def _actors(env, dtype, hidden=(64, 64, 64), seed=1, shipped=False):
     return [FFReLUNet([d0, *hidden, 5], dtype=dtype) for _ in range(env.n_adv)]
 
 
-def _on(actors, device):
-    import copy
-    return [copy.deepcopy(a).to(device) for a in actors]
-
-
-def _per_cycle(x, n_ep, T, E):
-    """[N, R, ...] -> [T, everything else] (max over worlds is taken per cycle)."""
-    N = x.shape[0]
-    return x.reshape(N, n_ep, T, E, -1).permute(2, 0, 1, 3, 4).reshape(T, -1)
-
-
-def _cycles(out, n_ep, T, E):
-    q = {k: _per_cycle(out[k].double().cpu(), n_ep, T, E) for k in ("obs", "acts", "log_probs", "rtgs")}
-    q["pos"] = out["pos"].double().cpu().permute(1, 0, 2, 3, 4).reshape(T, -1)
-    return q
-
-
-def _err(a, b):
-    return {k: (a[k] - b[k]).abs().amax(dim=1) for k in a}            # [T] per quantity
-
-
-def _envelope(e):
-    return torch.cummax(e, dim=0).values
-
-
-def _run_kernel(env, actors, pos0, T, key=7, index=0, noise=1.0):
-    n_ep = pos0.shape[0]
-    out = tag_rollout.rollout(env, actors, T=T, n_ep=n_ep, gamma=GAMMA, cov_var=COV, noise_scale=noise, key=key,
-                              index=index, pos0=pos0, debug=True)
-    torch.cuda.synchronize()
-    return out
-
-
-def _oracle(actors, pos0, eps, T, cfg, dtype=torch.float64):
-    env = _env(**dict(cfg, dtype=dtype, device="cpu"))
-    acts = [a.to("cpu", dtype) for a in _on(actors, "cpu")]
-    return replay_tag_rollout(env, acts, pos0.to("cpu", dtype), eps.to("cpu", dtype), T, GAMMA, COV)
-
-
-def _check_fp64(cfg, actors, n_ep, T):
-    env = _env(**cfg)
-    pos0 = tag_rollout.reset_positions(env, n_ep)
-    out = _run_kernel(env, actors, pos0, T)
-    E = env.E
-    ref = _oracle(actors, pos0, out["eps"], T, cfg)
-    yard = _oracle(actors, torch.nextafter(pos0.cpu(), torch.tensor(float("inf"), dtype=torch.float64)), out["eps"], T, cfg)
-    k, o, y = _cycles(out, n_ep, T, E), _cycles(ref, n_ep, T, E), _cycles(yard, n_ep, T, E)
-    ek, ey = _err(k, o), _err(y, o)
-    worst = 0.0
-    for q in k:
-        scale = o[q].abs().max().item()
-        bound = torch.clamp(10 * _envelope(ey[q]), min=1e-12 * scale)
-        assert (ek[q] <= bound).all(), (q, ek[q].tolist(), bound.tolist())
-        if q != "rtgs":                                   # an early reward-to-go sums the whole episode
-            assert (ek[q][:2] <= 1e-12 * max(scale, 1.0)).all(), (q, ek[q][:2].tolist())
-        worst = max(worst, (ek[q] / bound).max().item())
-    rk, ro, ry = out["ep_returns"].cpu(), ref["ep_returns"], yard["ep_returns"]
-    assert (rk - ro).abs().max() <= max(10 * (ry - ro).abs().max().item(), 1e-12 * ro.abs().max().item())
-    print(f"fp64 kernel error / bound, worst over quantities and cycles: {worst:.3g}")
-    return out
-
-
 def test_fp64_kernel_matches_replay_oracle_distinct_actors():
     cfg = dict(E=16, n_obst=8, max_cycles=200)
     _check_fp64(cfg, _on(_actors(_env(**cfg), torch.float64), DEV), n_ep=2, T=50)
@@ -110,7 +38,7 @@ def test_fp64_kernel_matches_replay_oracle_distinct_actors():
 def test_fp64_kernel_matches_replay_oracle_shipped_actors():
     """The trained DiNNO predators keep catching the prey, so contacts are exercised."""
     cfg = dict(E=16, n_obst=8, max_cycles=200)
-    out = _check_fp64(cfg, _on(_actors(None, torch.float64, shipped=True), DEV), n_ep=2, T=50)
+    out, _ = _check_fp64(cfg, _on(_actors(None, torch.float64, shipped=True), DEV), n_ep=2, T=50)
     assert out["ep_returns"].mean().item() > 0
 
 
@@ -135,34 +63,6 @@ def test_fp32_kernel_many_worlds_per_cta():
     """600 worlds: 4 worlds per CTA with the three fp32 actors staged in shared memory."""
     cfg = dict(E=600, n_obst=8, max_cycles=200)
     _fp32_ratio(cfg, _on(_actors(_env(**cfg), torch.float32), DEV), T=50, n_ep=1)
-
-
-def _fp32_ratio(cfg, actors32, T, n_ep, noise=1.0, perturbed_yardstick=False):
-    """``perturbed_yardstick``: the torch fp32 error is the larger of the runs from pos0 and from pos0 moved by one fp32
-    ulp.  The deterministic trained policy keeps the predators in stiff contact, so when the trajectories first
-    amplify a rounding difference depends on where that difference lands; one torch run is then too narrow a sample."""
-    env = _env(**dict(cfg, dtype=torch.float32))
-    pos0 = tag_rollout.reset_positions(env, n_ep)
-    out = _run_kernel(env, actors32, pos0, T, noise=noise)
-    E = env.E
-    eps = out["eps"] * noise
-    ref = _oracle(actors32, pos0, eps, T, cfg)                                         # fp64 oracle, fp32 inputs
-    t32 = _oracle(actors32, pos0, eps, T, cfg, dtype=torch.float32)                    # the torch fp32 path
-    k, o, t = _cycles(out, n_ep, T, E), _cycles(ref, n_ep, T, E), _cycles(t32, n_ep, T, E)
-    ek, et = _err(k, o), _err(t, o)
-    if perturbed_yardstick:
-        up = torch.nextafter(pos0.cpu(), torch.tensor(float("inf")))
-        t2 = _cycles(_oracle(actors32, up, eps, T, cfg, dtype=torch.float32), n_ep, T, E)
-        et = {q: torch.maximum(et[q], v) for q, v in _err(t2, o).items()}
-    worst = 0.0
-    for q in k:
-        scale = o[q].abs().max().item()
-        floor = 4 * 2.0 ** -23 * scale
-        bound = torch.clamp(4 * _envelope(et[q]), min=floor)
-        assert (ek[q] <= bound).all(), (q, ek[q].tolist(), bound.tolist())
-        worst = max(worst, (ek[q] / torch.clamp(_envelope(et[q]), min=floor)).max().item())
-    print(f"fp32 kernel error / torch fp32 error, worst over quantities and cycles: {worst:.3g}")
-    return out, worst
 
 
 def test_fp32_kernel_against_fp64_oracle_within_4x_torch_fp32():

@@ -59,6 +59,15 @@ def test_require_needs_cuda_and_names_the_reason():
         ppo_update.advantages(c, torch.zeros(1, 4, 12), torch.zeros(1, 4))
 
 
+def test_shape_errors_name_the_tensors_device():
+    """A wrongly placed batch, output or workspace tensor is named with its device as ``cuda:1`` / ``cpu`` reads,
+    not as the ``device(type=...)`` a tuple would print."""
+    dev = torch.device("cuda", 0)
+    for check in (ppo_update._out, ppo_update._batch):
+        with pytest.raises(ValueError, match=r"out: expected .* on cuda:0, got \(8, 40\) torch.float64 on cpu$"):
+            check("out", torch.zeros(8, 40, dtype=torch.float64), (8, 40), torch.float64, dev)
+
+
 def _problem(**kw):
     env = SimpleTagEnv(num_envs=2, num_good=1, num_adversaries=3, num_obstacles=8, max_cycles=5)
     return DistPPOProblem(FFReLUNet([12, 16, 5]), FFReLUNet([12, 16, 1]), nx.wheel_graph(3), env,
