@@ -155,6 +155,51 @@ def hsgd_track_(y: torch.Tensor, v: torch.Tensor, theta_prev: torch.Tensor, y_al
     theta_prev.copy_(theta)
 
 
+# ------------------------------------------------------- cross-gradient ----
+def xg_coefs(W: np.ndarray, neighbors, lam: float, lo: int, L: int, dmax: int) -> Tuple[np.ndarray, np.ndarray]:
+    """float64 weights of the aggregated direction of local nodes ``lo .. lo + L - 1``: ``coef0[l] = (1 - lam) + lam
+    W_ii`` and ``coef[l, e] = lam W_{i j_e}`` in table order (``neighbors[i]``), 0 past deg_i."""
+    coef0 = np.zeros(L)
+    coef = np.zeros((L, dmax))
+    for l in range(L):
+        i = lo + l
+        coef0[l] = (1.0 - lam) + lam * W[i, i]
+        for e, j in enumerate(neighbors[i]):
+            coef[l, e] = lam * W[i, j]
+    return coef0, coef
+
+
+def xg_cross_points(theta_all: torch.Tensor, src_node: torch.Tensor, live: torch.Tensor, lo: int) -> torch.Tensor:
+    """``[dmax, L, n_pad]``: slot e of local node l is neighbor j_e's row (``src_node[l, e]``) of ``theta_all``, or the
+    node's own row past deg_l (``live`` false)."""
+    L, dmax = src_node.shape
+    own = theta_all[lo: lo + L]
+    return torch.stack([torch.where(live[:, e, None], theta_all[src_node[:, e]], own) for e in range(dmax)])
+
+
+def xg_received(grad_x_all: torch.Tensor, src_node: torch.Tensor, src_slot: torch.Tensor,
+                live: torch.Tensor) -> torch.Tensor:
+    """``[L, dmax, n_pad]``: ``g_{j_e -> i}``, the gradient neighbor j_e took at this node's row, picked from every
+    node's cross gradients ``grad_x_all`` (``[dmax, N, n_pad]``) at ``[src_slot, src_node]`` (its reverse slot); zero
+    past deg_i."""
+    r = grad_x_all[src_slot, src_node]
+    return torch.where(live[:, :, None], r, torch.zeros((), dtype=r.dtype))
+
+
+def xg_step_(theta: torch.Tensor, xmix: torch.Tensor, grad: torch.Tensor, recv: torch.Tensor, coef0: torch.Tensor,
+             coef: torch.Tensor, alpha: float) -> torch.Tensor:
+    """``d = coef0 g + sum_e coef_e g_{j_e -> i}`` in float64 (own term first, then table order), rounded once to the
+    arena dtype; then ``theta = xmix - alpha d`` (dsgd_step_).  ``coef0`` ``[L]`` and ``coef`` ``[L, dmax]`` are
+    float64; ``recv`` ``[L, dmax, n_pad]``.  Returns d."""
+    d = coef0[:, None] * grad.double()
+    for e in range(recv.shape[1]):
+        d = d + coef[:, e, None] * recv[:, e].double()
+    d = d.to(theta.dtype)
+    theta.copy_(xmix)
+    dsgd_step_(theta, d, alpha)
+    return d
+
+
 # ------------------------------------------------------ Exact Diffusion ----
 def ed_weights(W):
     """``A = (I + W) / 2`` of a float64 Metropolis matrix: the combine weights of Exact Diffusion."""

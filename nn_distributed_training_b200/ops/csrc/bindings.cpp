@@ -127,6 +127,7 @@ struct ConsensusOp {
   consensus::KgtArgs<T> kg{};
   consensus::DetagArgs<T> dt{};
   consensus::HsgdArgs<T> hs{};
+  consensus::XgArgs<T> xg{};
   consensus::PgaArgs<T> pa{};
   consensus::DpArgs<T> dp{};
   consensus::MoniquaArgs<T> mq{};
@@ -142,7 +143,9 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c; sq.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c; sq.c = c; xg.c = c;
+    xg.xmix = ptr<T>(d, "xmix"); xg.theta_x = ptr<T>(d, "theta_x"); xg.grad_part_x = ptr<const T>(d, "grad_part_x");
+    xg.g = ptr<T>(d, "xg_g"); xg.coef0 = ptr<const double>(d, "xg_coef0"); xg.coef = ptr<const double>(d, "xg_coef");
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
     pg.nseg = geti(d, "pg_nseg", 0); pg.P = geti(d, "pg_P", 0); pg.Q = geti(d, "pg_Q", 0); pg.B = geti(d, "pg_B", 0);
     pg.W = geti(d, "pg_W", 0); pg.gamma = (T)getf(d, "gamma", 1.0); pg.grid_x = geti(d, "pg_grid", 0);
@@ -363,6 +366,25 @@ struct ConsensusOp {
                                "and two published channels (one without)");
     check(consensus::launch_dadaptive_step<T>(ad, cur_stream()), "dadaptive_step");
   }
+  void xg_check(const char* what) const {
+    if (xg.xmix == nullptr || xg.theta_x == nullptr || xg.grad_part_x == nullptr || xg.g == nullptr ||
+        xg.coef0 == nullptr || xg.coef == nullptr || c.sum_mode || c.C != 1 + c.dmax)
+      throw std::runtime_error(std::string(what) + " needs the rows `xmix`, `theta_x`, `xg_g`, the cross partials "
+                               "`grad_part_x`, the weights `xg_coef0` and `xg_coef`, the pointer-table neighbors and "
+                               "one published channel per neighbor slot after the theta channel (C = 1 + dmax)");
+  }
+  void xg_pull() {
+    xg_check("xg_pull");
+    check(consensus::launch_xg_pull<T>(xg, cur_stream()), "xg_pull");
+  }
+  void xg_publish() {
+    xg_check("xg_publish");
+    check(consensus::launch_xg_publish<T>(xg, cur_stream()), "xg_publish");
+  }
+  void xg_step() {
+    xg_check("xg_step");
+    check(consensus::launch_xg_step<T>(xg, cur_stream()), "xg_step");
+  }
   void relay_check(const char* what) const {
     if (rs.reach == nullptr || rs.rin == nullptr || rs.n < (T)1 || rs.diam < 0 || c.sum_mode || c.C != c.dmax)
       throw std::runtime_error(std::string(what) + " needs the reach table `reach`, the received rows `rin`, the node "
@@ -488,6 +510,9 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("ag_gossip", &ConsensusOp<T>::ag_gossip)
       .def("detag_track", &ConsensusOp<T>::detag_track)
       .def("hsgd_track", &ConsensusOp<T>::hsgd_track)
+      .def("xg_pull", &ConsensusOp<T>::xg_pull)
+      .def("xg_publish", &ConsensusOp<T>::xg_publish)
+      .def("xg_step", &ConsensusOp<T>::xg_step)
       .def("pga_sum", &ConsensusOp<T>::pga_sum)
       .def("pga_mix", &ConsensusOp<T>::pga_mix)
       .def("dp_norm", &ConsensusOp<T>::dp_norm)

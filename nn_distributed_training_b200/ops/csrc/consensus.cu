@@ -14,6 +14,7 @@
 // K-GT / local DSGD (no reference counterpart, optimizers/kgt.py)          -> kgt_mix or dsgd_mix / K x kgt_step
 // DeTAG (no reference counterpart, optimizers/detag.py)                    -> K x ag_gossip / detag_track
 // GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
+// cross-gradient (no reference counterpart, optimizers/cross_gradient.py)  -> xg_pull / xg_publish, xg_step
 // Gossip-PGA / local SGD (no reference counterpart, optimizers/gossip_pga.py) -> pga_sum + pga_mix / dsgd_step
 // DP-DSGD / DECOR (no reference counterpart, optimizers/dp_dsgd.py)        -> dsgd_mix / dp_norm + dp_step
 // Moniqua (no reference counterpart, optimizers/moniqua.py)                -> mq_mix / mq_step
@@ -1385,6 +1386,104 @@ __global__ void __launch_bounds__(THREADS) hsgd_track_kernel(const HsgdArgs<T> a
     stv(a.v + row + i, vn);
     stv(a.theta_prev + row + i, th);
     stv(pub_row(c, ri.par ^ 1, 1, l) + i, y);
+    stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
+  }
+  end_step(c, l, ri.k, true);
+}
+
+// --------------------------------------------------------- cross-gradient ----
+// Layout and round in consensus.h (XgArgs).  Every neighbor read of protocol round 2k is in xg_pull, after begin_round;
+// xg_publish writes only the other parity and ends the protocol round.  Protocol round 2k + 1 is all of xg_step: its
+// begin_round waits for the cross-gradients addressed to this node, it pulls them and writes only the other parity.
+// Each kernel stores after its pdl_wait: theta_x and xmix are read by the launches of the previous round.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) xg_pull_kernel(const XgArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T ws = c.self_w[ri.gid * c.L + l];
+  const T* w = c.nbr_w + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  const size_t slot = (size_t)c.L * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> own = ldv(c.theta + row + i);
+    Pack<T> x = own;
+#pragma unroll
+    for (int u = 0; u < N; ++u) x.v[u] *= ws;
+    // dsgd_mix's accumulation; the same loads are the cross points
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 0) + i); },
+                     [&](int e, const Pack<T>& q) {
+                       stv(a.theta_x + e * slot + row + i, q);
+#pragma unroll
+                       for (int u = 0; u < N; ++u) x.v[u] += w[e] * q.v[u];
+                     });
+    // an idle slot computes a finite gradient at the own row, never published
+    for (int e = deg; e < c.dmax; ++e) stv(a.theta_x + e * slot + row + i, own);
+    stv(a.xmix + row + i, x);
+  }
+}
+
+// the own gradient into g, and slot e's gradient into channel 1 + e of the other parity for e < deg; every sum in the
+// order s = 0, 1, 2, ... (sum_partials, as hsgd_track sums both of its sets)
+template <typename T, int U>
+__global__ void __launch_bounds__(THREADS) xg_publish_kernel(const XgArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  const size_t row = (size_t)l * c.n_pad;
+  const size_t slot = (size_t)c.L * c.S * c.n_pad;
+  const T* gx = a.grad_part_x + (size_t)l * c.S * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    for (int e = 0; e < deg; ++e)
+      stv(pub_row(c, ri.par ^ 1, 1 + e, l) + i, sum_partial_rows<U>(gx + e * slot + i, c.S, c.n_pad));
+    stv(a.g + row + i, sum_partials<U>(c, l, i));
+  }
+  tag_published(c, l, ri.k);
+  finish_round(c, ri.k);
+}
+
+// d = coef0 g + sum_e coef_e g_{j_e -> i} in fp64, own term first and then table order, rounded once to T; then
+// dsgd_step's arithmetic on (xmix, d)
+template <typename T>
+__global__ void __launch_bounds__(THREADS) xg_step_kernel(const XgArgs<T> a) {
+  pdl_wait();
+  pdl_launch_dependents();
+  const Common<T>& c = a.c;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const RoundInfo<T> ri = round_info(c);
+  const int deg = c.deg[ri.gid * c.L + l];
+  begin_round(c, ri.gid, l, ri.k);
+  const T alpha = c.alpha[ri.k];
+  const double c0 = a.coef0[ri.gid * c.L + l];
+  const double* ce = a.coef + (size_t)(ri.gid * c.L + l) * c.dmax;
+  const size_t row = (size_t)l * c.n_pad;
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> g = ldv(a.g + row + i);
+    DPack<N> d;
+#pragma unroll
+    for (int u = 0; u < N; ++u) d.v[u] = c0 * (double)g.v[u];
+    for_neighbors<4>(deg, [&](int e) { return ldv(nbr_row(c, ri.gid, l, e, ri.par, 1 + e) + i); },
+                     [&](int e, const Pack<T>& q) {
+                       const double we = ce[e];
+#pragma unroll
+                       for (int u = 0; u < N; ++u) d.v[u] += we * (double)q.v[u];
+                     });
+    Pack<T> dt, th = ldv(a.xmix + row + i);
+#pragma unroll
+    for (int u = 0; u < N; ++u) dt.v[u] = (T)d.v[u];
+#pragma unroll
+    for (int u = 0; u < N; ++u) th.v[u] -= alpha * dt.v[u];
+    stv(c.theta + row + i, th);
     stv(pub_row(c, ri.par ^ 1, 0, l) + i, th);
   }
   end_step(c, l, ri.k, true);
@@ -2966,6 +3065,15 @@ template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaSt
   // 8-deep as detag_track (S > 8 runs the tail loop): with two partial sets the 16-deep fp32 variant spills
   return launch_by_s(hsgd_track_kernel<T, 4>, hsgd_track_kernel<T, 8>, a.c, a, st);
 }
+template <typename T> cudaError_t launch_xg_pull(const XgArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(xg_pull_kernel<T>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_xg_publish(const XgArgs<T>& a, cudaStream_t st) {
+  return launch_by_s(xg_publish_kernel<T, 4>, xg_publish_kernel<T, 8>, a.c, a, st);
+}
+template <typename T> cudaError_t launch_xg_step(const XgArgs<T>& a, cudaStream_t st) {
+  return launch_one_wave(xg_step_kernel<T>, a.c, a, st);
+}
 
 // pga_sum covers the row once, one CTA per THREADS vectors, as local_sum; pga_mix is one wave, as dsgd_mix
 template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st) {
@@ -3163,6 +3271,9 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_ag_gossip<T>(const DetagArgs<T>&, cudaStream_t);        \
   template cudaError_t launch_detag_track<T>(const DetagArgs<T>&, cudaStream_t);      \
   template cudaError_t launch_hsgd_track<T>(const HsgdArgs<T>&, cudaStream_t);        \
+  template cudaError_t launch_xg_pull<T>(const XgArgs<T>&, cudaStream_t);             \
+  template cudaError_t launch_xg_publish<T>(const XgArgs<T>&, cudaStream_t);          \
+  template cudaError_t launch_xg_step<T>(const XgArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_pga_sum<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_pga_mix<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_dp_norm<T>(const DpArgs<T>&, cudaStream_t);             \

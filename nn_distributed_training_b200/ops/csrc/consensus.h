@@ -200,6 +200,27 @@ struct HsgdArgs {
   T omb;                           // 1 - beta, rounded once to T
 };
 
+// Cross-gradient gossip (CGA / NGC), optimizers/cross_gradient.py.  Gradient round k is two protocol rounds,
+// p = 2k and p = 2k + 1, and the published buffer has C = 1 + dmax channels: channel 0 is the theta row, channel 1 + e
+// node i's gradient at neighbor j_e's row.  The pointer-table entry of edge (i, e) for channel 1 + e names j_e's channel
+// for i (its reverse slot), so the step pulls g_{j_e -> i}, the gradient node j_e took at theta_i.
+//   xg_pull    (p = 2k):      xmix = sum_j W_ij theta_j and theta_x[e] = theta_{j_e} (the own row for e >= deg_i)
+//   fwd/bwd at theta and at every theta_x[e], on one draw
+//   xg_publish (p = 2k):      g = sum of the own partials; channel 1 + e of parity (p + 1) & 1 = sum of slot e's
+//                             partials, e < deg_i; ends protocol round p
+//   xg_step    (p = 2k + 1):  d = coef0 g + sum_e coef_e g_{j_e -> i} in fp64 (own term first, then table order),
+//                             rounded once; theta = xmix - alpha d; publish theta into channel 0 of parity (p + 1) & 1
+template <typename T>
+struct XgArgs {
+  Common<T> c;
+  T* xmix;                         // [L, n_pad] the mixed row of the round (dead between rounds)
+  T* theta_x;                      // [dmax, L, n_pad] the cross points of the round
+  const T* grad_part_x;            // [dmax, L, S, n_pad] partials of the forward/backward at each cross point
+  T* g;                            // [L, n_pad] the own gradient of the round
+  const double* coef0;             // [G, L] (1 - lam) + lam W_ii
+  const double* coef;              // [G, L, dmax] lam W_{i j_e}, 0 past deg_i
+};
+
 // Gossip-PGA (Chen, Yuan, Zhang, Pan, Xu, Yin 2021), optimizers/gossip_pga.py: DSGD's single published channel, with
 // every `period`-th round (k mod period == period - 1) a global round that replaces the gossip mix with the exact
 // network mean.  The round is pga_sum, pga_mix, fwd/bwd, dsgd_step; the branch is taken on the device from the round
@@ -449,6 +470,9 @@ template <typename T> cudaError_t launch_kgt_step(const KgtArgs<T>& a, cudaStrea
 template <typename T> cudaError_t launch_ag_gossip(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_detag_track(const DetagArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_hsgd_track(const HsgdArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_xg_pull(const XgArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_xg_publish(const XgArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_xg_step(const XgArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_t st);

@@ -264,6 +264,30 @@ NNDT_DEVINL Pack<T> sum_partials(const Common<T>& c, int l, int i) {
   return g;
 }
 
+// sum_partials over any partial set: `gp` is the node's first partial row at element i, S rows n_pad apart; the same
+// issue order and summation order s = 0, 1, 2, ...
+template <int U, typename T>
+NNDT_DEVINL Pack<T> sum_partial_rows(const T* gp, int S, int n_pad) {
+  constexpr int N = Vec<T>::N;
+  Pack<T> q[U];
+#pragma unroll
+  for (int s = 0; s < U; ++s)
+    if (s < S) q[s] = ldv(gp + (size_t)s * n_pad);
+  Pack<T> g = q[0];
+#pragma unroll
+  for (int s = 1; s < U; ++s)
+    if (s < S) {
+#pragma unroll
+      for (int u = 0; u < N; ++u) g.v[u] += q[s].v[u];
+    }
+  for (int s = U; s < S; ++s) {
+    const Pack<T> r = ldv(gp + (size_t)s * n_pad);
+#pragma unroll
+    for (int u = 0; u < N; ++u) g.v[u] += r.v[u];
+  }
+  return g;
+}
+
 // step bookkeeping done by one thread per node in the kernel that consumes a gradient: advance the sampler's
 // draw counter and fold the step's training loss into the moving average (problems/dist_online_dense_problem.py:129-137)
 template <typename T>

@@ -39,7 +39,7 @@ def schedule_tables(opt, H: int):
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
     elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua", "sparq_sgd"):
+                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua", "sparq_sgd", "cross_gradient"):
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
@@ -173,7 +173,12 @@ class ConsensusEngine:
         # DeTAG: every gossip sub-step is a protocol round, p = K k + s, so the device round counter, the flags and the
         # sequence tags count K per gradient round and the schedules hold K entries per gradient round
         self.detag = opt.alg_name == "detag"
-        K = self.rounds_per_step = opt.gossip_steps if self.detag else 1
+        # cross-gradient: gradient round k is protocol rounds 2k (xg_pull .. xg_publish) and 2k + 1 (xg_step).  Channel 0
+        # is theta, channel 1 + e the node's gradient at neighbor j_e's row
+        self.xg = opt.alg_name == "cross_gradient"
+        if self.xg:
+            self.C = 1 + opt.dmax
+        K = self.rounds_per_step = opt.gossip_steps if self.detag else 2 if self.xg else 1
         # GT-HSGD: DSGT's channels and mix, and a second set of gradient partials (theta_prev, the same minibatch)
         self.hsgd = opt.alg_name == "gt_hsgd"
         # Gossip-PGA: DSGD's channel and pointer-table mix on gossip rounds, and the fp64 partial sums of the
@@ -238,6 +243,8 @@ class ConsensusEngine:
         elif self.detag:                            # z = theta - alpha y and y, published for protocol round p0
             self.pub[p0 & 1, 0, :L].copy_(opt.z)
             self.pub[p0 & 1, 1, :L].copy_(opt.y)
+        elif self.xg:                               # theta, published for protocol round p0 = 2 k0
+            self.pub[p0 & 1, 0, :L].copy_(a.theta)
         else:
             self.pub[k0 & 1, 0, :L].copy_(a.theta)
         if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr or self.hsgd:
@@ -303,6 +310,10 @@ class ConsensusEngine:
             props = torch.cuda.get_device_properties(dev)
             check_powergossip_capacity(dmax, opt.lay.width, itemsize,
                                        int(getattr(props, "shared_memory_per_block_optin", 227 * 1024)))
+        if self.xg and (G > 1 or topos[0].key != opt.topo.key):
+            raise ValueError("cross_gradient needs a fixed graph: the planned graph sequence of this problem is not the "
+                             "one graph the optimizer was built on (its cross-gradients travel back over the edges of "
+                             "one fixed graph)")
         if self.detag and (G > 1 or topos[0].key != opt.topo.key):
             raise ValueError("detag needs a fixed graph: the planned graph sequence of this problem is not the one graph "
                              "its Chebyshev weights were computed for (acceleration has no guarantee on a changing "
@@ -329,7 +340,7 @@ class ConsensusEngine:
         rdr_deg = np.zeros((G, L), dtype=np.int32) if directed else None
         rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
-            rslot = t.reverse_slots() if self.relay or self.pg else None
+            rslot = t.reverse_slots() if self.relay or self.pg or self.xg else None
             # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
             # push-sum weights, over the in-neighbors (as Push-DIGing)
             if push_sum:
@@ -347,6 +358,11 @@ class ConsensusEngine:
                     if r != ctx.rank:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
+                        if self.xg:     # theta, and channel 1 + e of the edge: j's gradient at this node's row
+                            for ch, jch in ((0, 0), (1 + e, 1 + rslot[g][e])):
+                                row = (par * self.C + jch) * self.Lpub + lj
+                                nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
+                            continue
                         if rslot is not None:   # channel 0 of the edge: j's message for this node (its reverse slot)
                             row = (par * self.C + rslot[g][e]) * self.Lpub + lj
                             nbr_ptr[gi, l, e, par, 0] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
@@ -422,7 +438,7 @@ class ConsensusEngine:
         # complete_graph_mode is ignored)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
                          and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag or self.pga or self.dp or self.mq or self.sparq)
+                                  or self.detag or self.pga or self.dp or self.mq or self.sparq or self.xg)
                          and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
@@ -503,6 +519,17 @@ class ConsensusEngine:
             gpp = pr.fused.grad_part_prev if pr.fused is not None else opt.grad_prev
             d.update(grad_part_prev=gpp.data_ptr(), hsgd_v=opt.v.data_ptr(), theta_prev=opt.theta_prev.data_ptr(),
                      omb=opt.omb)
+        self.xmix = self.xg_g = self.t_xg_coef0 = self.t_xg_coef = None
+        if self.xg:
+            # the round's mixed row and own gradient (dead between rounds); the cross partials: the fused problem's extra
+            # ops, or (autograd gradients) the optimizer's grad_x, one row per node and slot; the float64 weights of d
+            gx = pr.fused.grad_part_x if pr.fused is not None else opt.grad_x
+            self.xmix = torch.zeros(L, n_pad, dtype=self.dtype, device=dev)
+            self.xg_g = torch.zeros(L, n_pad, dtype=self.dtype, device=dev)
+            self.t_xg_coef0 = opt.coef0.reshape(1, L).contiguous()
+            self.t_xg_coef = opt.coef.reshape(1, L, dmax).contiguous()
+            d.update(xmix=self.xmix.data_ptr(), theta_x=opt.theta_x.data_ptr(), grad_part_x=gx.data_ptr(),
+                     xg_g=self.xg_g.data_ptr(), xg_coef0=self.t_xg_coef0.data_ptr(), xg_coef=self.t_xg_coef.data_ptr())
         if opt.alg_name == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
         if opt.alg_name == "kgt":
@@ -646,8 +673,13 @@ class ConsensusEngine:
         ``n_pad * bits / 8`` bytes, one per neighbor edge as DSGD's rows; the margin counters stay on the node.  A
         SPARQ-SGD row is the code row and its 16-byte tail (``row``); every neighbor edge pulls the tail each round
         (``tail``) and the code body only when its source triggered: ``pulled_max`` is the round where every neighbor
-        triggered, and ``pulled_bytes()`` gives what the mixes actually pulled."""
+        triggered, and ``pulled_bytes()`` gives what the mixes actually pulled.  A cross-gradient node pulls each
+        neighbor's theta row (``pulled_theta``) and the gradient that neighbor took at its own row (``pulled_cross``), one
+        row each per neighbor edge; ``pulled`` is both.  ``grad_evals()`` gives the round's gradient evaluations."""
         deg = int(self.t_deg[0].sum().item())
+        if self.xg:
+            return {"row": int(self.row_bytes), "pulled": 2 * int(self.row_bytes) * deg,
+                    "pulled_theta": int(self.row_bytes) * deg, "pulled_cross": int(self.row_bytes) * deg}
         if self.sparq:
             return {"row": int(self.row_bytes), "tail": 16, "pulled_max": int(self.row_bytes) * deg}
         if self.pga:
@@ -661,6 +693,17 @@ class ConsensusEngine:
         chans = 1 if self.relay else self.C
         return {"row": int(self.row_bytes) * chans,
                 "pulled": int(self.row_bytes) * chans * deg * reads * self.rounds_per_step}
+
+    def grad_evals(self) -> Dict[str, int]:
+        """Forward/backward passes per round over the network: ``useful`` counts the own gradients and one per directed
+        edge, ``N + 2|E|``; ``launched`` also the idle slots of nodes below the largest degree, ``N (1 + dmax)``.  Every
+        other optimizer evaluates ``draws_per_round`` gradients per node."""
+        if self.xg:
+            useful, launched = self.opt.grad_evals()
+            return {"useful": useful, "launched": launched}
+        from .round_program import draws_per_round
+        n = self.pr.N * draws_per_round(self.opt)
+        return {"useful": n, "launched": n}
 
     def pulled_bytes(self) -> int:
         """SPARQ-SGD: the bytes the mixes of the rounds run so far pulled over the whole network, exact, from the

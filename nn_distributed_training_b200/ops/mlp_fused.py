@@ -118,19 +118,32 @@ class FusedMLP:
         self._fwd = MlpForward(a, self.spec, self.L, dev)
         self.host_feed = None
         self.prev_op = None
+        self.cross = []
+
+    def _point_op(self, theta_pt: torch.Tensor, grad_part: torch.Tensor):
+        """The training kernel on another parameter buffer ``theta_pt`` (``[L, n_pad]``, kept at this address) with its
+        own partials ``grad_part``.  It reads the same draw counters ``calls`` as the training op, which the consensus
+        step advances after every launch of the round, so it draws the same minibatch.  It leaves the loss EMA alone."""
+        assert theta_pt.shape == self.pr.arena.theta.shape and theta_pt.dtype == self.dtype
+        loss_part = torch.zeros_like(self.loss_part)
+        d = dict(self.base)
+        d.update(theta=theta_pt.data_ptr(), grad_part=grad_part.data_ptr(), loss_part=loss_part.data_ptr())
+        return self.ext.MlpOp(d), loss_part
 
     def enable_prev_point(self, theta_prev: torch.Tensor):
-        """Build the prev-point op (GT-HSGD): the training kernel on ``theta_prev`` (``[L, n_pad]``, kept at this
-        address) with its own partials.  It reads the same draw counters ``calls`` as the training op, which the
-        consensus step advances after both launches, so it draws the same minibatch.  It leaves the loss EMA alone."""
-        assert theta_prev.shape == self.pr.arena.theta.shape and theta_prev.dtype == self.dtype
+        """Build the prev-point op (GT-HSGD) on ``theta_prev``: ``_point_op``."""
         self.theta_prev = theta_prev
         self.grad_part_prev = torch.zeros_like(self.grad_part)
-        self.loss_part_prev = torch.zeros_like(self.loss_part)
-        d = dict(self.base)
-        d.update(theta=theta_prev.data_ptr(), grad_part=self.grad_part_prev.data_ptr(),
-                 loss_part=self.loss_part_prev.data_ptr())
-        self.prev_op = self.ext.MlpOp(d)
+        self.prev_op, self.loss_part_prev = self._point_op(theta_prev, self.grad_part_prev)
+
+    def enable_cross_points(self, theta_x: torch.Tensor):
+        """Build one training op per slot of ``theta_x`` (``[P, L, n_pad]``, kept at this address), each a
+        ``_point_op``; their partials are the slots of ``grad_part_x`` (``[P, L, S, n_pad]``)."""
+        assert theta_x.dim() == 3 and theta_x.is_contiguous()
+        self.theta_x = theta_x
+        self.grad_part_x = torch.zeros((theta_x.shape[0],) + tuple(self.grad_part.shape), dtype=self.dtype,
+                                       device=self.grad_part.device)
+        self.cross = [self._point_op(theta_x[e], self.grad_part_x[e]) for e in range(theta_x.shape[0])]
 
     WIN_MAX = 64
 
@@ -179,6 +192,19 @@ class FusedMLP:
         self.launch()
         self.launch_prev()
         torch.sum(self.grad_part_prev, dim=1, out=grad_prev)
+        return self._collect_grads()
+
+    def launch_cross(self, e: int):
+        """Enqueue the fwd+bwd at cross point ``e`` on the batch of the last ``launch`` (graph-capturable)."""
+        self.cross[e][0].train()
+
+    def compute_grads_multi(self, points: torch.Tensor, grads: torch.Tensor) -> torch.Tensor:
+        """Eager API of ``ConsensusProblem.compute_grads_multi`` on the cross-point ops' ``theta_x``."""
+        assert self.cross and points.data_ptr() == self.theta_x.data_ptr()
+        self.launch()
+        for e in range(len(self.cross)):
+            self.launch_cross(e)
+        torch.sum(self.grad_part_x, dim=2, out=grads)
         return self._collect_grads()
 
     def compute_grads(self) -> torch.Tensor:

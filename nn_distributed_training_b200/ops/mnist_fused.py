@@ -114,46 +114,71 @@ class FusedMnist:
         self._setup_eval()
         self.host_feed = None
         self.prev_op = None
-        self.direct_prev_ops = []
+        self._prev = None
+        self._points = []       # every extra-point op (_point_op), in build order
+        self.cross = []
 
-    # ---- a second point on the same minibatch (GT-HSGD) ---------------------
-    def enable_prev_point(self, theta_prev: torch.Tensor):
-        """Build the prev-point op: the training kernel on ``theta_prev`` (``[L, n_pad]``, kept at this address) with
-        its own partials.  It draws the same minibatch as the training op because its draw counters (``calls_prev``,
-        ``arrive_prev``) are a twin that the kernel advances in lockstep and ``sync_calls_from_host`` sets from the same
-        host mirror.  It stores no loss into the host mirror."""
-        assert theta_prev.shape == self.pr.arena.theta.shape and theta_prev.dtype == self.dtype
-        self.theta_prev = theta_prev
-        self.calls_prev = torch.zeros_like(self.calls)
-        self.arrive_prev = torch.zeros_like(self.arrive)
-        self.grad_part_prev = torch.zeros_like(self.grad_part)
-        self.loss_part_prev = torch.zeros_like(self.loss_part)
+    # ---- more points on the same minibatch (GT-HSGD, cross-gradient) --------
+    def _point_op(self, theta_pt: torch.Tensor, grad_part: torch.Tensor) -> dict:
+        """The training kernel on another parameter buffer ``theta_pt`` (``[L, n_pad]``, kept at this address) with its
+        own partials ``grad_part``.  It draws the same minibatch as the training op because its draw counters
+        (``calls``, ``arrive``) are a twin that the kernel advances in lockstep and ``sync_calls_from_host`` sets from
+        the same host mirror; the fp32 cluster kernel gets its own W1 tensor map.  It stores no loss into the host
+        mirror."""
+        assert theta_pt.shape == self.pr.arena.theta.shape and theta_pt.dtype == self.dtype
+        pt = dict(theta=theta_pt, calls=torch.zeros_like(self.calls), arrive=torch.zeros_like(self.arrive),
+                  grad_part=grad_part, loss_part=torch.zeros_like(self.loss_part), direct=[])
         d = dict(self.base)
         d.pop("step_prof", None)
-        d.update(theta=theta_prev.data_ptr(), calls=self.calls_prev.data_ptr(), arrive=self.arrive_prev.data_ptr(),
-                 grad_part=self.grad_part_prev.data_ptr(), loss_part=self.loss_part_prev.data_ptr())
+        d.update(theta=theta_pt.data_ptr(), calls=pt["calls"].data_ptr(), arrive=pt["arrive"].data_ptr(),
+                 grad_part=grad_part.data_ptr(), loss_part=pt["loss_part"].data_ptr())
         if self.tc:
             a = self.pr.arena
             off_w1 = self.base["off_w1"]
-            d.update(w1_map=self.ext.make_w1_tensor_map(theta_prev.data_ptr(), a.n_pad, self.L, off_w1))
-        self.base_prev = d
-        self.prev_op = self.ext.MnistOp(d)
+            d.update(w1_map=self.ext.make_w1_tensor_map(theta_pt.data_ptr(), a.n_pad, self.L, off_w1))
+        pt.update(base=d, op=self.ext.MnistOp(d))
+        self._points.append(pt)
         self.sync_calls_from_host()
         if self.host_feed is not None:
-            self._build_direct_prev_ops()
+            self._build_direct_point_ops(pt)
+        return pt
 
-    def _build_direct_prev_ops(self):
-        # the prev-point twins of the direct ops of step 0: the same stage slot, so the same staged minibatch
-        self.direct_prev_ops = []
+    def _build_direct_point_ops(self, pt: dict):
+        # the point's twins of the direct ops of step 0: the same stage slot, so the same staged minibatch
+        pt["direct"] = []
         for b in range(2):
-            d = dict(self.base_prev)
+            d = dict(pt["base"])
             d.update(direct=1, x=self.x_stage[b, 0].data_ptr(), y=self.y_stage[b, 0].data_ptr(),
                      direct_bs=self.bs_stage[b, 0].data_ptr())
-            self.direct_prev_ops.append(self.ext.MnistOp(d))
+            pt["direct"].append(self.ext.MnistOp(d))
+
+    def enable_prev_point(self, theta_prev: torch.Tensor):
+        """Build the prev-point op (GT-HSGD) on ``theta_prev``: ``_point_op``."""
+        pt = self._prev = self._point_op(theta_prev, torch.zeros_like(self.grad_part))
+        self.theta_prev, self.prev_op = theta_prev, pt["op"]
+        self.calls_prev, self.arrive_prev = pt["calls"], pt["arrive"]
+        self.grad_part_prev, self.loss_part_prev = pt["grad_part"], pt["loss_part"]
+
+    @property
+    def direct_prev_ops(self):
+        return self._prev["direct"] if self._prev is not None else []
+
+    def enable_cross_points(self, theta_x: torch.Tensor):
+        """Build one training op per slot of ``theta_x`` (``[P, L, n_pad]``, kept at this address), each a
+        ``_point_op``; their partials are the slots of ``grad_part_x`` (``[P, L, S, n_pad]``)."""
+        assert theta_x.dim() == 3 and theta_x.is_contiguous()
+        self.theta_x = theta_x
+        self.grad_part_x = torch.zeros((theta_x.shape[0],) + tuple(self.grad_part.shape), dtype=self.dtype,
+                                       device=self.grad_part.device)
+        self.cross = [self._point_op(theta_x[e], self.grad_part_x[e]) for e in range(theta_x.shape[0])]
 
     def launch_prev(self):
         """Enqueue the prev-point fwd+bwd on the batch the last ``launch`` drew (graph-capturable)."""
         self.prev_op.train()
+
+    def launch_cross(self, e: int):
+        """Enqueue the fwd+bwd at cross point ``e`` on the batch the last ``launch`` drew (graph-capturable)."""
+        self.cross[e]["op"].train()
 
     def compute_grads_pair(self, theta_prev: torch.Tensor, grad_prev: torch.Tensor) -> torch.Tensor:
         """Eager API of ``ConsensusProblem.compute_grads_pair``: ``arena.grad`` at theta and ``grad_prev`` at the
@@ -162,6 +187,15 @@ class FusedMnist:
         self.launch()
         self.launch_prev()
         torch.sum(self.grad_part_prev, dim=1, out=grad_prev)
+        return self._collect_grads()
+
+    def compute_grads_multi(self, points: torch.Tensor, grads: torch.Tensor) -> torch.Tensor:
+        """Eager API of ``ConsensusProblem.compute_grads_multi`` on the cross-point ops' ``theta_x``."""
+        assert self.cross and points.data_ptr() == self.theta_x.data_ptr()
+        self.launch()
+        for e in range(len(self.cross)):
+            self.launch_cross(e)
+        torch.sum(self.grad_part_x, dim=2, out=grads)
         return self._collect_grads()
 
     # ---- training ---------------------------------------------------------
@@ -185,8 +219,8 @@ class FusedMnist:
     def sync_calls_from_host(self):
         pl = self.pr.placement
         self.calls.copy_(torch.as_tensor(self.pr.calls[pl.lo: pl.lo + pl.L].astype(np.int32)))
-        if self.prev_op is not None:
-            self.calls_prev.copy_(self.calls)
+        for pt in self._points:
+            pt["calls"].copy_(self.calls)
 
     # ---- host-fed batches (end-to-end input pipeline) -----------------------
     def enable_host_feed(self, steps_per_round: int, source: str):
@@ -248,8 +282,8 @@ class FusedMnist:
         self.host_feed = dict(P=P, mode="gpu_pull", source=source,
                               h2d_bytes=P * L * B * (784 * xb + 8) if source == "host" else 0,
                               d2h_bytes=L * self.S * 4 if source == "host" else 0)
-        if self.prev_op is not None:
-            self._build_direct_prev_ops()
+        for pt in self._points:
+            self._build_direct_point_ops(pt)
         return self.host_feed
 
     # ---- validation ---------------------------------------------------------

@@ -22,6 +22,7 @@ A round is a short, fixed kernel sequence
     DP-DSGD / DECOR:  dsgd_mix, fwd/bwd, dp_norm, dp_step
     Moniqua:  mq_mix, fwd/bwd, mq_step
     SPARQ-SGD:  sparq_mix, [fwd/bwd, sparq_step(p)] x local_steps, sparq_publish
+    cross-gradient:  xg_pull, fwd/bwd, fwd/bwd at theta_x[e] x dmax, xg_publish, xg_step   (two protocol rounds)
 whose per-round scalars come from device schedules indexed by a device round
 counter, so ``R`` consecutive rounds are captured once as a CUDA graph and
 replayed between evaluation points with no host work (the reference issues
@@ -49,12 +50,12 @@ def _nvtx(name):
     return torch.cuda.nvtx.range(name)
 
 
-def _round_ops(opt, eng, grads, grads_prev):
+def _round_ops(opt, eng, grads, grads_prev, grads_cross):
     with _nvtx(f"consensus_round/{opt.alg_name}"):
-        _round_ops_impl(opt, eng, grads, grads_prev)
+        _round_ops_impl(opt, eng, grads, grads_prev, grads_cross)
 
 
-def _round_ops_impl(opt, eng, grads, grads_prev):
+def _round_ops_impl(opt, eng, grads, grads_prev, grads_cross):
     alg = opt.alg_name
     if eng.sum_mode:
         eng.op.local_sum()   # complete graph: per-rank partial sums feeding the NVLS reduction
@@ -131,6 +132,13 @@ def _round_ops_impl(opt, eng, grads, grads_prev):
         grads(0)
         grads_prev()
         eng.op.hsgd_track()
+    elif alg == "cross_gradient":
+        eng.op.xg_pull()
+        grads(0)
+        for e in range(opt.dmax):
+            grads_cross(e)
+        eng.op.xg_publish()
+        eng.op.xg_step()
     elif alg == "gossip_pga":
         eng.op.pga_sum()
         eng.op.pga_mix()
@@ -207,11 +215,11 @@ class RoundProgram:
         # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
         # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
         # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y; Moniqua publishes
-        # codes too, and SPARQ-SGD code rows with a trigger tail
+        # codes too, and SPARQ-SGD code rows with a trigger tail; the cross-gradient channels are gradients
         attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
         pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
                                       or self.eng.relay or self.eng.pg or self.eng.detag or self.eng.mq
-                                      or self.eng.sparq)
+                                      or self.eng.sparq or self.eng.xg)
                              else (self.eng, lambda: opt.k))
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
@@ -253,6 +261,8 @@ class RoundProgram:
             return n + 4
         if self.opt.alg_name == "sparq_sgd":
             return n + 2 + 2 * self.opt.local_steps
+        if self.opt.alg_name == "cross_gradient":
+            return n + 4 + self.opt.dmax
         return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
 
     def grads(self, p: int = 0):
@@ -260,6 +270,8 @@ class RoundProgram:
         if pr.fused is None:
             if self.opt.alg_name == "gt_hsgd":     # autograd: both points in one call (grads_prev has nothing left)
                 pr.compute_grads_pair(self.opt.theta_prev, self.opt.grad_prev)
+            elif self.opt.alg_name == "cross_gradient":     # autograd: every point in one call (as gt_hsgd)
+                pr.compute_grads_multi(self.opt.theta_x, self.opt.grad_x)
             else:
                 pr.compute_grads()
         elif self.host_mode:
@@ -277,6 +289,17 @@ class RoundProgram:
             pr.fused.direct_prev_ops[self._stage_set].train()
         else:
             pr.fused.launch_prev()
+
+    def grads_cross(self, e: int):
+        """The cross-gradient forward/backward at ``theta_x[e]`` on the minibatch ``grads(0)`` just drew: cross-point op
+        ``e``, or its direct op of the current stage set."""
+        pr = self.pr
+        if pr.fused is None:
+            return
+        if self.host_mode:
+            pr.fused.cross[e]["direct"][self._stage_set].train()
+        else:
+            pr.fused.launch_cross(e)
 
     def _count(self, rounds: int):
         """Host mirror of the device-side draw counters."""
@@ -313,7 +336,7 @@ class RoundProgram:
                 with torch.cuda.stream(side):
                     fz.gather_ops[b ^ 1].launch()
                 self._stage_set = b
-                _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
+                _round_ops(self.opt, self.eng, self.grads, self.grads_prev, self.grads_cross)
                 main.wait_stream(side)     # round i+1 consumes what was just staged (also joins the fork)
         return g
 
@@ -347,7 +370,7 @@ class RoundProgram:
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
+                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev, self.grads_cross)
             self._graphs[r] = g
         return g
 
@@ -388,7 +411,7 @@ class RoundProgram:
                 self._resident_graph(r).replay()
             else:
                 for _ in range(r):
-                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev)
+                    _round_ops(self.opt, self.eng, self.grads, self.grads_prev, self.grads_cross)
             self._count(r)
             left -= r
 
@@ -409,7 +432,7 @@ class RoundProgram:
             opt.rho = opt.rho_at(opt.k - 1)
         if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
                             "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua",
-                            "sparq_sgd") and opt.k > 0:
+                            "sparq_sgd", "cross_gradient") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
         if opt.alg_name == "relaysum":          # the messages published for round k
             opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))

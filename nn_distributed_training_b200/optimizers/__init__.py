@@ -2,6 +2,7 @@ from .beer import BEER
 from .bridge import Bridge
 from .clipped_gossip import ClippedGossip
 from .choco import ChocoSGD
+from .cross_gradient import CrossGradient
 from .dadaptive import DAdaptive
 from .detag import DeTAG
 from .dinno import DiNNO
@@ -25,7 +26,7 @@ ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
               "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD,
-              "moniqua": Moniqua, "sparq_sgd": SparqSGD}
+              "moniqua": Moniqua, "sparq_sgd": SparqSGD, "cross_gradient": CrossGradient}
 
 
 def build_optimizer(problem, device, opt_conf):

@@ -117,6 +117,7 @@ class ConsensusOptimizer:
         self.checkpointer = None  # set by utils.checkpoint.attach
         if isinstance(self.pr, ConsensusProblem):
             self.pr.privacy_record = None   # a differentially private optimizer sets its own after this
+            self.pr.xg_grad_evals = None    # so does the cross-gradient optimizer, with its gradient evaluations
 
     # -- helpers ---------------------------------------------------------
     @property

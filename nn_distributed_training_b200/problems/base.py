@@ -199,6 +199,15 @@ class ConsensusProblem:
         theta."""
         if self.fused is not None:
             return self.fused.compute_grads_pair(theta_prev, grad_prev)
+        return self.compute_grads_multi(theta_prev.unsqueeze(0), grad_prev.unsqueeze(0))
+
+    def compute_grads_multi(self, points: torch.Tensor, grads: torch.Tensor) -> torch.Tensor:
+        """``compute_grads`` plus the gradient at ``P`` more points on the *same* minibatch: ``arena.grad`` at theta and
+        ``grads[p]`` at ``points[p]`` (both ``[P, L, n_pad]``).  One draw per node: the draw counters, ``forward_cnt``
+        and the losses (of theta) advance once, as for ``compute_grads``.  On the fused kernels the points are the
+        buffers the extra training ops were built on (``enable_cross_points``).  Returns the ``[L]`` losses at theta."""
+        if self.fused is not None:
+            return self.fused.compute_grads_multi(points, grads)
         for l, g in enumerate(self.placement.local_nodes):
             model = self.models[g]
             x, y = self._batch(g)
@@ -206,17 +215,18 @@ class ConsensusProblem:
             self._after_loss(g, loss)
             self.arena.set_row_from_grads(l, torch.autograd.grad(loss, list(model.parameters())))
             self.last_losses[l] = loss.detach()
-            # the same network at theta_prev on the same batch: leaves viewing the row, through functional_call; the
-            # loss hook (_after_loss) sees the current point only
-            prev = [p.detach().requires_grad_(True) for p in self.layout.views(theta_prev[l])]
-            params = {s.name: p for s, p in zip(self.layout.slots, prev)}
+            # the same network at each point on the same batch: leaves viewing the row, through functional_call; the
+            # loss hook (_after_loss) sees theta only
+            for p in range(points.shape[0]):
+                prev = [t.detach().requires_grad_(True) for t in self.layout.views(points[p, l])]
+                params = {s.name: t for s, t in zip(self.layout.slots, prev)}
 
-            def at_prev(inp, model=model, params=params):
-                return torch.func.functional_call(model, params, (inp,))
-            at_prev.parameters = lambda prev=prev: iter(prev)     # what a loss hook may inspect on a NaN
-            loss_p = self._loss(at_prev, x, y)
-            for dst, t in zip(self.layout.views(grad_prev[l]), torch.autograd.grad(loss_p, prev)):
-                dst.copy_(t)
+                def at_prev(inp, model=model, params=params):
+                    return torch.func.functional_call(model, params, (inp,))
+                at_prev.parameters = lambda prev=prev: iter(prev)     # what a loss hook may inspect on a NaN
+                loss_p = self._loss(at_prev, x, y)
+                for dst, t in zip(self.layout.views(grads[p, l]), torch.autograd.grad(loss_p, prev)):
+                    dst.copy_(t)
         for g in range(self.N):
             if not self.placement.is_local(g):
                 self._count_draw(g)
@@ -293,6 +303,8 @@ class ConsensusProblem:
             out["byzantine_nodes"] = sorted(int(v) for v in byz["nodes"])   # summaries average the other nodes
         if self.privacy_record is not None:
             out["privacy"] = self.privacy_record()
+        if getattr(self, "xg_grad_evals", None) is not None:
+            out["xg_grad_evals"] = self.xg_grad_evals
         torch.save(out, path)
 
     def state_dicts(self) -> Dict[int, dict]:

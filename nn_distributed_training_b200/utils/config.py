@@ -22,7 +22,7 @@ REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
         "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-        "moniqua", "sparq_sgd")
+        "moniqua", "sparq_sgd", "cross_gradient")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -76,6 +76,8 @@ OPT_SCHEMA = {
                 "outer_iterations": REQUIRED, "update_graph": True, "profile": False},
     "sparq_sgd": {"alpha0": REQUIRED, "mu": 0.0, "gamma": REQUIRED, "compressor": REQUIRED, "threshold": REQUIRED,
                   "local_steps": 1, "threshold_growth": 0.0, "outer_iterations": REQUIRED, "profile": False},
+    "cross_gradient": {"alpha0": REQUIRED, "mu": 0.0, "cross_weight": REQUIRED, "outer_iterations": REQUIRED,
+                       "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -211,6 +213,37 @@ def _check_gossip_pga(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.period must be an integer >= 1 (got {p!r})")
     if not isinstance(c["gossip"], bool):
         raise ConfigError(f"{path}.gossip must be true or false (got {c['gossip']!r})")
+
+
+CROSS_GRADIENT_KEYS = ("alg_name", "alpha0", "mu", "cross_weight", "outer_iterations", "profile")
+
+
+def _check_cross_gradient(c: Dict[str, Any], path: str) -> None:
+    """Cross-gradient gossip: DSGD's step schedule (``alpha0`` and ``mu`` finite, >= 0), ``cross_weight`` (finite, in
+    [0, 1]) and no other key."""
+    for key in c:
+        if key not in CROSS_GRADIENT_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: cross_gradient takes no key {key!r} (its keys are alpha0, mu, cross_weight "
+                              f"and outer_iterations)")
+    for key in ("alpha0", "mu"):
+        if not _real(c[key]) or not (math.isfinite(float(c[key])) and float(c[key]) >= 0.0):
+            raise ConfigError(f"{path}.{key} must be finite and >= 0 (got {c[key]!r})")
+    w = c["cross_weight"]
+    if not _real(w) or not (math.isfinite(float(w)) and 0.0 <= float(w) <= 1.0):
+        raise ConfigError(f"{path}.cross_weight must be finite and in [0, 1] (got {w!r})")
+
+
+def _check_fixed_graph(c: Dict[str, Any], path: str, kind: str) -> None:
+    """Cross-gradient gossip sends each gradient back over the edge it came from, on one fixed graph: link drops and the
+    online-density runner's moving graph are refused."""
+    if c["optimizer_config"]["alg_name"] != "cross_gradient":
+        return
+    if c.get("fault_injection"):
+        raise ConfigError(f"{path}.fault_injection: cross_gradient needs a fixed graph (link drops change it during the "
+                          f"run)")
+    if kind == "online_density":
+        raise ConfigError(f"{path}.optimizer_config.alg_name: cross_gradient needs a fixed graph, and the online-density "
+                          f"runner moves the graph with the agents (the offline density runner is supported)")
 
 
 DP_DSGD_KEYS = ("alg_name", "alpha0", "mu", "clip_norm", "noise_multiplier", "pair_noise_multiplier", "target_delta",
@@ -353,7 +386,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
                 "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-                "moniqua", "sparq_sgd")
+                "moniqua", "sparq_sgd", "cross_gradient")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -415,6 +448,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_moniqua(c, path)
     if alg == "sparq_sgd":
         _check_sparq(c, path)
+    if alg == "cross_gradient":
+        _check_cross_gradient(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:
@@ -464,6 +499,7 @@ def validate_problem(conf: Dict[str, Any], path: str, kind: str) -> Dict[str, An
         c = _fill(c, {"comm_radius": REQUIRED, "dynamic_graph": True, "save_models": False}, path)
     c["metrics_config"] = mc
     c["optimizer_config"] = validate_optimizer(c["optimizer_config"], path + ".optimizer_config")
+    _check_fixed_graph(c, path, kind)
     return c
 
 
