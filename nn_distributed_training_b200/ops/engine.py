@@ -14,6 +14,8 @@ import torch
 
 from . import load_ext
 from .consensus_ref import CHOCO_CODE, choco_live, choco_live_words, ed_weights
+from ..optimizers.beer import FIXED_W as BEER_FIXED_W
+from ..optimizers.sparq import FIXED_W as SPARQ_FIXED_W
 from ..parallel.symm import SymmetricBuffer
 from ..utils.graph_generation import Topology
 
@@ -38,15 +40,59 @@ def schedule_tables(opt, H: int):
     if opt.alg_name == "dinno":
         rho[:] = [opt.rho_at(k) for k in range(H)]
         lr[:] = [opt.lr_at(k) for k in range(H)]
-    elif opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip", "relaysum",
-                          "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua", "sparq_sgd", "cross_gradient"):
+    elif hasattr(opt, "alpha_table"):        # a decaying step
         alpha[:] = opt.alpha_table(H)
     elif not torch.is_tensor(opt.alpha):     # DSGT, BEER, Push-DIGing, K-GT, dadaptive, DeTAG, GT-HSGD: a constant step
         alpha[:] = opt.alpha
     return rho, lr, alpha
 
 
+# Algorithms whose mix has the complete-graph sum mode: channel 0 is theta and every aggregate of the mix is a function
+# of the network sum.  The others pull through the pointer table: their rows are codes, numerators with a weight or
+# per-edge messages, or a mix clips, screens, noises or averages globally per edge or per round
+SUM_MODE_ALGS = frozenset({"dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "kgt", "dadaptive", "gt_hsgd"})
+# Algorithms whose published channel 0 is theta, so the fused consensus metric can read it (not while Byzantine nodes
+# publish attack rows there)
+THETA_ROW_ALGS = SUM_MODE_ALGS | {"gossip_pga", "dp_dsgd", "clipped_gossip", "bridge"}
+
+# Why an algorithm needs the planned graph sequence to be one fixed graph (and the one in ``opt.topo`` when it holds one)
+FIXED_GRAPH = {
+    "choco_sgd": "s = sum_j W_ij x_hat_j is only valid for a fixed W",
+    "beer": BEER_FIXED_W,
+    "sparq_sgd": SPARQ_FIXED_W,
+    "relaysum": "its messages relay over one fixed tree",
+    "powergossip": "both endpoints of an edge carry its power-iteration vectors from round to round",
+    "cross_gradient": "its cross-gradients travel back over the edges of one fixed graph",
+    "detag": "Chebyshev acceleration has no guarantee on a changing mixing matrix",
+}
+# Why an algorithm needs undirected planned graphs
+UNDIRECTED = {
+    "dp_dsgd": "the pairwise noise of an edge cancels between its two ends",
+    "sparq_sgd": "its mix conserves the network sum only with symmetric weights",
+    "moniqua": "its mix conserves the network sum only with symmetric weights",
+}
+
+
+def check_plan_graphs(opt, topos: List[Topology]) -> None:
+    """The planned topologies of a ``FIXED_GRAPH`` algorithm are one, the graph the optimizer was built on when it holds
+    one; those of an ``UNDIRECTED`` algorithm are undirected."""
+    alg, topo = opt.alg_name, getattr(opt, "topo", None)
+    if alg in FIXED_GRAPH and (len(topos) > 1 or (topo is not None and topos[0].key != topo.key)):
+        shape = "tree" if alg == "relaysum" else "graph"
+        plan = f"has {len(topos)} topologies" if len(topos) > 1 else f"is not the {shape} the optimizer was built on"
+        raise ValueError(f"{alg} needs a fixed {shape}: the planned graph sequence of this problem {plan} "
+                         f"({FIXED_GRAPH[alg]})")
+    if alg in UNDIRECTED and any(t.directed for t in topos):
+        raise ValueError(f"{alg} needs undirected graphs: a planned graph is directed ({UNDIRECTED[alg]})")
+
+
 WAIT_THREADS = 256     # consensus_device.cuh: THREADS
+
+
+def partials_stride(n_pad: int, itemsize: int) -> int:
+    """fp64 partial sums per row of the norm and distance kernels: one per chunk of ``WAIT_THREADS * (16 / itemsize)``
+    elements (a 16-byte vector per thread)."""
+    return max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
 
 
 def check_wait_capacity(dmax: int, rmax: int) -> None:
@@ -108,12 +154,9 @@ def check_topk_capacity(alg: str, n_pad: int, itemsize: int, chans: int) -> None
 RELAY_MAX_DEG = 16     # consensus.h: kRelayMaxDeg
 
 
-def check_relay_plan(topos: List[Topology], dmax: int) -> None:
-    """RelaySum relays over one fixed tree, and its step holds a node's received messages in registers, for at most
-    ``RELAY_MAX_DEG`` neighbors."""
-    if len(topos) > 1:
-        raise ValueError(f"relaysum needs a fixed tree: the planned graph sequence of this problem has {len(topos)} "
-                         f"topologies (its messages relay over one fixed tree)")
+def check_relay_plan(dmax: int) -> None:
+    """RelaySum's step holds a node's received messages in registers, for at most ``RELAY_MAX_DEG`` neighbors (its one
+    fixed tree is ``check_plan_graphs``'s)."""
     if dmax > RELAY_MAX_DEG:
         raise ValueError(f"relaysum handles at most {RELAY_MAX_DEG} neighbors per node on the fused kernels; the tree "
                          f"has a node with {dmax}")
@@ -149,64 +192,43 @@ class ConsensusEngine:
         dev, a, pl, ctx = pr.device, pr.arena, pr.placement, pr.ctx
         self.dtype = a.dtype
         npdt = np.float32 if self.dtype == torch.float32 else np.float64
-        # K-GT publishes its tracker y in channel 1; local DSGD (kgt without correction) publishes theta only.  So does
-        # dadaptive with its second-moment tracker u~ (tracking) or without it
-        kgt_corr = opt.alg_name == "kgt" and opt.correction
-        ad_track = opt.alg_name == "dadaptive" and opt.tracking
-        self.C = 2 if opt.alg_name in ("dsgt", "push_diging", "beer", "detag", "gt_hsgd") or kgt_corr or ad_track else 1
-        # RelaySum publishes one message per neighbor: channel e of node i is its message for neighbor j_e
-        self.relay = opt.alg_name == "relaysum"
-        if self.relay:
+        alg = opt.alg_name
+        # published channels: channel 0, and channel 1 for a second published row (the tracker y of DSGT, Push-DIGing,
+        # DeTAG, GT-HSGD and K-GT with correction, dadaptive's u~ with tracking, BEER's g codes).  RelaySum and
+        # PowerGossip publish one message per neighbor: channel e of node i is its message for neighbor j_e.
+        # Cross-gradient: channel 0 is theta, channel 1 + e the node's gradient at neighbor j_e's row
+        if hasattr(opt, "msg"):
             self.C = opt.dmax
-        # PowerGossip likewise, with message rows of the layout's message width instead of n_pad
-        self.pg = opt.alg_name == "powergossip"
-        if self.pg:
-            self.C = opt.dmax
+        elif alg == "cross_gradient":
+            self.C = 1 + opt.dmax
+        else:
+            self.C = 2 if (alg == "beer" or getattr(opt, "y", None) is not None
+                           or getattr(opt, "ut", None) is not None) else 1
         L, n_pad, oits = pl.L, a.n_pad, opt.oits
         itemsize = a.theta.element_size()
-        self.choco = opt.alg_name == "choco_sgd"
-        self.beer = opt.alg_name == "beer"
-        self.sgp = opt.alg_name == "sgp"
-        self.pdg = opt.alg_name == "push_diging"
-        self.cg = opt.alg_name == "clipped_gossip"
-        self.bridge = opt.alg_name == "bridge"
         # DeTAG: every gossip sub-step is a protocol round, p = K k + s, so the device round counter, the flags and the
-        # sequence tags count K per gradient round and the schedules hold K entries per gradient round
-        self.detag = opt.alg_name == "detag"
-        # cross-gradient: gradient round k is protocol rounds 2k (xg_pull .. xg_publish) and 2k + 1 (xg_step).  Channel 0
-        # is theta, channel 1 + e the node's gradient at neighbor j_e's row
-        self.xg = opt.alg_name == "cross_gradient"
-        if self.xg:
-            self.C = 1 + opt.dmax
-        K = self.rounds_per_step = opt.gossip_steps if self.detag else 2 if self.xg else 1
-        # GT-HSGD: DSGT's channels and mix, and a second set of gradient partials (theta_prev, the same minibatch)
-        self.hsgd = opt.alg_name == "gt_hsgd"
-        # Gossip-PGA: DSGD's channel and pointer-table mix on gossip rounds, and the fp64 partial sums of the
-        # complete-graph mode on global rounds (sum_mode stays 0).  Local SGD (gossip: false) plans the edgeless graph
-        self.pga = opt.alg_name == "gossip_pga"
-        if self.pga and not opt.gossip:
+        # sequence tags count K per gradient round and the schedules hold K entries per gradient round.
+        # Cross-gradient: gradient round k is protocol rounds 2k (xg_pull .. xg_publish) and 2k + 1 (xg_step)
+        K = self.rounds_per_step = opt.gossip_steps if alg == "detag" else 2 if alg == "cross_gradient" else 1
+        # Gossip-PGA's local SGD (gossip: false) plans the edgeless graph
+        if alg == "gossip_pga" and not opt.gossip:
             edgeless = opt.edgeless_graph()
             graphs_per_round = [edgeless] * len(graphs_per_round)
-        # DP-DSGD: DSGD's channel and pointer-table mix, a clipped and noised step (dp_norm, dp_step)
-        self.dp = opt.alg_name == "dp_dsgd"
-        # Moniqua: one channel of modulo-quantized code rows, pulled through the pointer table (mq_mix, mq_step)
-        self.mq = opt.alg_name == "moniqua"
-        # SPARQ-SGD: one channel of CHOCO code rows with a 16-byte trigger tail, pulled through the pointer table
-        self.sparq = opt.alg_name == "sparq_sgd"
-        push_sum = self.sgp or self.pdg
+        # SGP and Push-DIGing mix with the column-stochastic push-sum weights and publish the node's weight w
+        push_sum = hasattr(opt, "w")
 
         # ---- published rows (double buffered, peer mapped when multi-GPU) -----
-        # CHOCO-SGD publishes code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter rows; SGP
-        # publishes its numerators x followed by a 16-byte tail holding the float64 push-sum weight w (Push-DIGing: both
-        # channels, u with w in the tail and y, have that stride).  BEER publishes two channels of CHOCO code rows.
-        # Moniqua publishes code rows of n_pad * bits / 8 bytes, SPARQ-SGD code rows followed by their trigger tail.
-        if self.choco or self.beer or self.mq:
-            self.row_bytes = opt.code_bytes
-        elif self.sparq:
+        # CHOCO-SGD, BEER and Moniqua publish code rows of opt.code_bytes bytes (a multiple of 16) instead of parameter
+        # rows, SPARQ-SGD code rows followed by their 16-byte trigger tail (opt.row_bytes); SGP and Push-DIGing rows
+        # (both channels) are followed by a 16-byte tail holding the float64 push-sum weight w; PowerGossip's message
+        # rows are of the layout's message width
+        if hasattr(opt, "row_bytes"):
             self.row_bytes = opt.row_bytes
+        elif hasattr(opt, "code_bytes"):
+            self.row_bytes = opt.code_bytes
         elif push_sum:
             self.row_bytes = n_pad * itemsize + 16
-        elif self.pg:
+        elif alg == "powergossip":
             self.row_bytes = opt.lay.width * itemsize
         else:
             self.row_bytes = n_pad * itemsize
@@ -217,40 +239,12 @@ class ConsensusEngine:
         k0 = opt.k
         p0 = K * k0                 # the protocol round of gradient round k0
         # round k0 (0, or the round a checkpoint resumed at) is "published" in the parity it will be read from
-        if self.choco or self.sparq:
-            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
-        elif self.mq:                               # round 0 reads the codes of theta^0
-            if k0 == 0:
-                opt.encode_initial()
-            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code)
-        elif self.beer:
-            self.pub[k0 & 1, 0, :L].view(torch.uint8).copy_(opt.code_h)
-            self.pub[k0 & 1, 1, :L].view(torch.uint8).copy_(opt.code_g)
-        elif self.sgp:
-            self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.x)
-            self.pub_weights(k0 & 1).copy_(opt.w)
-        elif self.pdg:
-            self.pub[k0 & 1, 0, :L, :n_pad].copy_(opt.u)
-            self.pub_weights(k0 & 1).copy_(opt.w)
-            self.pub[k0 & 1, 1, :L, :n_pad].copy_(opt.y)
-        elif self.cg or self.bridge:                # an attacker's published row is not its theta
-            self.pub[k0 & 1, 0, :L].copy_(opt.pub)
-        elif self.relay:                            # the messages published at the end of round k0 - 1
-            self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
-        elif self.pg:                               # the messages of round k0 (phase k0 & 1), zero past their length
-            self.pub.zero_()
-            self.pub[k0 & 1, :, :L].copy_(opt.msg.transpose(0, 1))
-        elif self.detag:                            # z = theta - alpha y and y, published for protocol round p0
-            self.pub[p0 & 1, 0, :L].copy_(opt.z)
-            self.pub[p0 & 1, 1, :L].copy_(opt.y)
-        elif self.xg:                               # theta, published for protocol round p0 = 2 k0
-            self.pub[p0 & 1, 0, :L].copy_(a.theta)
-        else:
-            self.pub[k0 & 1, 0, :L].copy_(a.theta)
-        if (opt.alg_name == "dsgt" and getattr(opt, "_initialised", False)) or kgt_corr or self.hsgd:
-            self.pub[k0 & 1, 1, :L].copy_(opt.y)
-        if ad_track:
-            self.pub[k0 & 1, 1, :L].copy_(opt.ut)
+        if alg == "moniqua" and k0 == 0:
+            opt.encode_initial()                    # round 0 reads the codes of theta^0
+        if alg == "powergossip":
+            self.pub.zero_()                        # messages are zero past their length
+        for row, src, _ in self.published_rows(k0):
+            row.copy_(src)
 
         # ---- schedules ----------------------------------------------------------
         H = self.horizon = schedule_horizon(opt)
@@ -260,7 +254,7 @@ class ConsensusEngine:
         self.alpha = torch.as_tensor(alpha.astype(npdt), device=dev)
         # DSGT with a per-coordinate step: the [n_pad] row replaces the alpha_k schedule in dsgt_mix
         self.alpha_row = None
-        if opt.alg_name == "dsgt" and torch.is_tensor(opt.alpha):
+        if alg == "dsgt" and torch.is_tensor(opt.alpha):
             self.alpha_row = opt.alpha.detach().to(device=dev, dtype=self.dtype).reshape(-1).contiguous()
             if self.alpha_row.numel() != n_pad:
                 raise ValueError(f"per-coordinate alpha has {self.alpha_row.numel()} entries for rows of {n_pad}")
@@ -283,53 +277,21 @@ class ConsensusEngine:
         self.gid = gid
         self.topos = topos
         G = len(topos)
-        if (self.choco or self.beer) and opt.compressor == "topk":
-            check_topk_capacity(opt.alg_name, n_pad, itemsize, self.C)
-        if self.choco and G > 1:
-            raise ValueError("choco_sgd needs a fixed graph: the planned graph sequence of this problem has "
-                             f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
-        if self.sparq and G > 1:
-            raise ValueError("sparq_sgd needs a fixed graph: the planned graph sequence of this problem has "
-                             f"{G} topologies (s = sum_j W_ij x_hat_j is only valid for a fixed W)")
-        if self.beer and G > 1:
-            raise ValueError("beer needs a fixed graph: the planned graph sequence of this problem has "
-                             f"{G} topologies (s_h = sum_j W_ij h_j and s_g = sum_j W_ij g_j are only valid for a "
-                             "fixed W)")
+        if getattr(opt, "compressor", None) == "topk":
+            check_topk_capacity(alg, n_pad, itemsize, self.C)
+        check_plan_graphs(opt, topos)
         dmax = max(1, max(t.max_degree for t in topos))
-        if self.bridge:
+        if alg == "bridge":
             check_bridge_capacity(dmax)
-        if self.relay:
-            check_relay_plan(topos, dmax)
-            if topos[0].key != opt.topo.key:
-                raise ValueError("relaysum: the planned graph is not the tree the optimizer was built on")
-        if self.pg:
-            if G > 1 or topos[0].key != opt.topo.key:
-                raise ValueError("powergossip needs a fixed graph: the planned graph sequence of this problem is not "
-                                 "the one graph the optimizer was built on (both endpoints of an edge carry its "
-                                 "power-iteration vectors from round to round)")
+        if alg == "relaysum":
+            check_relay_plan(dmax)
+        if alg == "powergossip":
             props = torch.cuda.get_device_properties(dev)
             check_powergossip_capacity(dmax, opt.lay.width, itemsize,
                                        int(getattr(props, "shared_memory_per_block_optin", 227 * 1024)))
-        if self.xg and (G > 1 or topos[0].key != opt.topo.key):
-            raise ValueError("cross_gradient needs a fixed graph: the planned graph sequence of this problem is not the "
-                             "one graph the optimizer was built on (its cross-gradients travel back over the edges of "
-                             "one fixed graph)")
-        if self.detag and (G > 1 or topos[0].key != opt.topo.key):
-            raise ValueError("detag needs a fixed graph: the planned graph sequence of this problem is not the one graph "
-                             "its Chebyshev weights were computed for (acceleration has no guarantee on a changing "
-                             "mixing matrix)")
         # reader tables (the out-neighbors the round-start wait also covers) only when a planned graph is directed:
         # on undirected graphs the readers are the neighbors and the kernels take them from deg / nbr_rank
         directed = any(t.directed for t in topos)
-        if self.dp and directed:
-            raise ValueError("dp_dsgd needs undirected graphs: a planned graph is directed (the pairwise noise of an edge "
-                             "cancels between its two ends)")
-        if self.sparq and directed:
-            raise ValueError("sparq_sgd needs undirected graphs: a planned graph is directed (its mix conserves the "
-                             "network sum only with symmetric weights)")
-        if self.mq and directed:
-            raise ValueError("moniqua needs undirected graphs: a planned graph is directed (its mix conserves the network "
-                             "sum only with symmetric weights)")
         rmax = max(1, max(t.max_readers for t in topos))
         check_wait_capacity(dmax, rmax if directed or G > 1 else 0)    # a static undirected graph has no second wait
         nbr_ptr = np.zeros((G, L, dmax, 2, self.C), dtype=np.int64)
@@ -340,13 +302,13 @@ class ConsensusEngine:
         rdr_deg = np.zeros((G, L), dtype=np.int32) if directed else None
         rdr_rank = -np.ones((G, L, rmax), dtype=np.int32) if directed else None
         for gi, t in enumerate(topos):
-            rslot = t.reverse_slots() if self.relay or self.pg or self.xg else None
-            # Exact Diffusion combines with A = (I + W) / 2 through the same mix kernel; SGP with the column-stochastic
-            # push-sum weights, over the in-neighbors (as Push-DIGing)
+            rslot = t.reverse_slots() if hasattr(opt, "msg") or alg == "cross_gradient" else None
+            # Exact Diffusion (and Moniqua on its base) combines with A = (I + W) / 2 through the same mix kernel; SGP
+            # and Push-DIGing with the column-stochastic push-sum weights, over the in-neighbors
             if push_sum:
                 Wt = t.push_weights
             else:
-                ed = opt.alg_name == "exact_diffusion" or (self.mq and opt.base == "exact_diffusion")
+                ed = alg == "exact_diffusion" or (alg == "moniqua" and opt.base == "exact_diffusion")
                 Wt = ed_weights(t.W) if ed else t.W
             for l, g in enumerate(pl.local_nodes):
                 nb = t.neighbors_noself[g]
@@ -358,7 +320,7 @@ class ConsensusEngine:
                     if r != ctx.rank:
                         nbr_rank[gi, l, e] = r
                     for par in range(2):
-                        if self.xg:     # theta, and channel 1 + e of the edge: j's gradient at this node's row
+                        if alg == "cross_gradient":     # theta, and channel 1 + e of the edge: j's gradient here
                             for ch, jch in ((0, 0), (1 + e, 1 + rslot[g][e])):
                                 row = (par * self.C + jch) * self.Lpub + lj
                                 nbr_ptr[gi, l, e, par, ch] = self.pub_buf.peer_ptrs[r] + row * self.row_bytes
@@ -432,24 +394,20 @@ class ConsensusEngine:
             ctx.barrier()
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
-        # (CHOCO-SGD, BEER, SGP and Push-DIGing always pull through the pointer table: their published rows are codes /
-        # numerators with a weight; so do ClippedGossip, which clips per edge, BRIDGE, which screens the neighbor
-        # values, and RelaySum, whose rows are per-edge messages (a 2-node complete graph is a tree);
-        # complete_graph_mode is ignored)
-        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1
-                         and not (self.choco or self.beer or self.cg or self.bridge or self.relay or self.pg
-                                  or self.detag or self.pga or self.dp or self.mq or self.sparq or self.xg)
-                         and not push_sum and opt.conf.get("complete_graph_mode", "sum") == "sum")
+        # (the algorithms outside SUM_MODE_ALGS always pull through the pointer table; complete_graph_mode is ignored.
+        # Gossip-PGA's global rounds average through the same fp64 partial sums, with sum_mode 0)
+        self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and alg in SUM_MODE_ALGS
+                         and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
-        if self.sum_mode or self.pga:
+        if self.sum_mode or alg == "gossip_pga":
             self.sum_buf = SymmetricBuffer((2, self.C, n_pad), torch.float64, ctx)   # fp64: S - N*theta cancels in fp32
             self.sum_flag_buf = SymmetricBuffer((max(ctx.world_size, 1),), torch.int32, ctx)
             self.sum_flag_buf.local.fill_(k0)
             if ctx.is_distributed:
                 if self.sum_buf.multicast_ptr:
                     sum_mc = self.sum_buf.multicast_ptr      # NVLS: one in-switch reduction per element
-                elif self.pga:
+                elif alg == "gossip_pga":
                     raise ValueError("gossip_pga on more than one rank averages over NVLS (one in-switch reduction of "
                                      "the fp64 partial sums per global round), and this fabric gives its symmetric "
                                      "buffer no multicast mapping")
@@ -458,7 +416,7 @@ class ConsensusEngine:
                 torch.cuda.synchronize(dev)
                 ctx.barrier()
         peer_sum_flag = np.zeros(max(ctx.world_size, 1), dtype=np.int64)
-        if self.sum_mode or self.pga:
+        if self.sum_mode or alg == "gossip_pga":
             for r in range(ctx.world_size):
                 peer_sum_flag[r] = self.sum_flag_buf.peer_ptrs[r] + 4 * ctx.rank
         self.t_peer_sum_flag = torch.as_tensor(peer_sum_flag, device=dev)
@@ -501,26 +459,26 @@ class ConsensusEngine:
         if self.sum_mode:
             d.update(sum_mode=1, n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
                      sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr())
-        if self.pga:
+        if alg == "gossip_pga":
             d.update(n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
                      sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr(),
                      period=opt.period, gossip=int(opt.gossip))
-        if opt.alg_name == "dinno":
+        if alg == "dinno":
             d.update(dual=opt.duals.data_ptr(), delta=opt.delta.data_ptr(),
                      m=None if opt.m is None else opt.m.data_ptr(),
                      v=None if opt.v is None else opt.v.data_ptr(),
                      pits=opt.pits, opt=OPT_CODE[opt.opt_kind], persistent=int(opt.persistent))
-        if opt.alg_name == "dsgt":
+        if alg == "dsgt":
             d.update(g_old=opt.g.data_ptr(), own_tracker=int(bool(getattr(opt, "own_tracker_step", False))),
                      alpha_row=None if self.alpha_row is None else self.alpha_row.data_ptr())
-        if self.hsgd:
+        if alg == "gt_hsgd":
             # the prev-point partials: the fused problem's second op, or (autograd gradients) the optimizer's grad_prev,
             # one row per node as a.grad
             gpp = pr.fused.grad_part_prev if pr.fused is not None else opt.grad_prev
             d.update(grad_part_prev=gpp.data_ptr(), hsgd_v=opt.v.data_ptr(), theta_prev=opt.theta_prev.data_ptr(),
                      omb=opt.omb)
         self.xmix = self.xg_g = self.t_xg_coef0 = self.t_xg_coef = None
-        if self.xg:
+        if alg == "cross_gradient":
             # the round's mixed row and own gradient (dead between rounds); the cross partials: the fused problem's extra
             # ops, or (autograd gradients) the optimizer's grad_x, one row per node and slot; the float64 weights of d
             gx = pr.fused.grad_part_x if pr.fused is not None else opt.grad_x
@@ -530,30 +488,31 @@ class ConsensusEngine:
             self.t_xg_coef = opt.coef.reshape(1, L, dmax).contiguous()
             d.update(xmix=self.xmix.data_ptr(), theta_x=opt.theta_x.data_ptr(), grad_part_x=gx.data_ptr(),
                      xg_g=self.xg_g.data_ptr(), xg_coef0=self.t_xg_coef0.data_ptr(), xg_coef=self.t_xg_coef.data_ptr())
-        if opt.alg_name == "exact_diffusion":
+        if alg == "exact_diffusion":
             d.update(psi=opt.psi.data_ptr())
-        if opt.alg_name == "kgt":
+        if alg == "kgt":
             d.update(local_steps=opt.local_steps, correction=int(opt.correction),
-                     corr=opt.c.data_ptr() if kgt_corr else None, dacc=opt.d.data_ptr() if kgt_corr else None)
+                     corr=opt.c.data_ptr() if opt.correction else None,
+                     dacc=opt.d.data_ptr() if opt.correction else None)
         self.omega = self.ymix = None
-        if self.detag:
+        if alg == "detag":
             # the sub-step weights in the arena dtype, and Y_K of the last sub-step (dead between rounds)
             self.omega = torch.as_tensor(np.asarray(opt.omega, dtype=npdt), device=dev)
             self.ymix = torch.zeros(L, n_pad, dtype=self.dtype, device=dev)
             d.update(omega=self.omega.data_ptr(), ymix=self.ymix.data_ptr(), g_old=opt.g_old.data_ptr(),
                      gossip_steps=K)
-        if opt.alg_name == "dadaptive":
+        if alg == "dadaptive":
             d.update(ad_m=opt.m.data_ptr(), ad_v=None if opt.v is None else opt.v.data_ptr(),
-                     vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if ad_track else None, beta1=opt.beta1,
-                     beta2=opt.beta2, ad_eps=opt.eps, adagrad=int(opt.adagrad), tracking=int(ad_track))
+                     vhat=opt.vhat.data_ptr(), ut=opt.ut.data_ptr() if opt.tracking else None, beta1=opt.beta1,
+                     beta2=opt.beta2, ad_eps=opt.eps, adagrad=int(opt.adagrad), tracking=int(opt.tracking))
         self.t_live = None
         self.dist_part = self.t_attack = self.t_nbr_byz = None
-        if self.cg or self.bridge:         # BRIDGE's step is cg_step, with the same attack tables
-            if self.cg:
+        if hasattr(opt, "byzantine"):     # ClippedGossip, BRIDGE: BRIDGE's step is cg_step, with the same attack tables
+            if alg == "clipped_gossip":
                 if opt.clip == "adaptive":
                     check_clip_capacity(dmax)
                 # fp64 partials of the squared neighbor distances: one per chunk of THREADS * (16 / itemsize) elements
-                pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+                pstride = partials_stride(n_pad, itemsize)
                 self.dist_part = torch.zeros(L * dmax * pstride, dtype=torch.float64, device=dev)
                 d.update(dist_part=self.dist_part.data_ptr(), pstride=pstride,
                          clip_adaptive=int(opt.clip == "adaptive"), clip_delta=float(opt.delta))
@@ -572,7 +531,7 @@ class ConsensusEngine:
                      attack=None if self.t_attack is None else self.t_attack.data_ptr(),
                      nbr_byz=self.t_nbr_byz.data_ptr())
         self.t_reach = self.rin = None
-        if self.relay:
+        if alg == "relaysum":
             # R_i^k - 1 of the local nodes for k = 0 .. diam (exact in either dtype), and the received messages of the
             # round, written by relay_mix and read by relay_step
             self.t_reach = torch.as_tensor(
@@ -580,7 +539,7 @@ class ConsensusEngine:
             self.rin = torch.zeros(L, dmax, n_pad, dtype=self.dtype, device=dev)
             d.update(reach=self.t_reach.data_ptr(), rin=self.rin.data_ptr(), diam=opt.diam, relay_n=pr.N)
         self.t_pg_seg = None
-        if self.pg:
+        if alg == "powergossip":
             # the segment table {offset, m, n, poff, qoff} and the edge signs; the vectors are the optimizer's own rows,
             # updated in place by pg_mix
             lay = opt.lay
@@ -588,12 +547,13 @@ class ConsensusEngine:
             d.update(pg_vec=opt.vec.data_ptr() if opt.vec.numel() else None, pg_seg=self.t_pg_seg.data_ptr(),
                      pg_sign=opt.sign.data_ptr(), pg_nseg=len(lay.segs), pg_P=lay.P, pg_Q=lay.Q, pg_B=lay.B,
                      pg_W=lay.width, gamma=float(opt.gamma), pg_grid=int(getattr(opt, "pg_grid", 0)))
-        self.norm_part = self.t_nbr_id = None
-        if self.dp:
+        # DP-DSGD: ``dp`` is the privacy ledger of the fused path, the zCDP cost of one round on each planned graph
+        # (None for the other algorithms)
+        self.norm_part = self.t_nbr_id = self.dp = None
+        if alg == "dp_dsgd":
             # fp64 partials of sum g^2, one per chunk of THREADS * (16 / itemsize) elements (cg_dist's chunks); the
-            # global id of every neighbor slot (the edge streams); the live mask (no noise on padding and slot holes);
-            # and the zCDP cost of one round on each planned graph (the ledger of the fused path)
-            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+            # global id of every neighbor slot (the edge streams); the live mask (no noise on padding and slot holes)
+            pstride = partials_stride(n_pad, itemsize)
             self.norm_part = torch.zeros(L * pstride, dtype=torch.float64, device=dev)
             nbr_id = np.zeros((G, L, dmax), dtype=np.int32)
             for gi, t in enumerate(topos):
@@ -604,44 +564,48 @@ class ConsensusEngine:
             live = choco_live(a.layout)
             live = torch.cat([live, live.new_zeros(-n_pad % 32)])      # whole words: a row may be shorter than 32
             self.t_live = choco_live_words(live).to(dev)
-            self.dp_rho = [opt.round_rho(t) for t in topos]
+            self.dp = [opt.round_rho(t) for t in topos]
             d.update(norm_part=self.norm_part.data_ptr(), pstride=pstride, nbr_id=self.t_nbr_id.data_ptr(),
                      live=self.t_live.data_ptr(), node0=int(pl.lo), clip_norm=float(opt.clip), cz_dp=float(opt.cz_dp),
                      cz_pair=float(opt.cz_pair), dp_key0=int(opt.key[0]), dp_key1=int(opt.key[1]))
-        if opt.alg_name == "dsgdm":
+        if alg == "dsgdm":
             d.update(m=opt.m.data_ptr(), x_prev=None if opt.x_prev is None else opt.x_prev.data_ptr(), beta=opt.beta,
                      quasi_global=int(opt.quasi_global), nesterov=int(opt.nesterov))
-        if self.choco:
+        if alg == "choco_sgd":
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
                      code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes), topk_k=int(opt.topk_k or 0))
-        if self.beer:
+        if alg == "beer":
             self.t_live = choco_live_words(opt.live).to(dev)
             d.update(h=opt.h.data_ptr(), s_h=opt.s_h.data_ptr(), v=opt.v.data_ptr(), g=opt.g.data_ptr(),
                      s_g=opt.s_g.data_ptr(), m_old=opt.m_old.data_ptr(), live=self.t_live.data_ptr(),
                      gamma=float(opt.gamma), code=CHOCO_CODE[opt.compressor], code_stride=int(self.row_bytes),
                      topk_k=int(opt.topk_k or 0))
-        if self.mq:
+        # Moniqua: ``mq`` holds the kernels' arguments of the modulo code the published rows carry (range, bit width,
+        # rounding keys, margin counters, code row stride; None for the other algorithms)
+        self.mq = None
+        if alg == "moniqua":
             self.t_live = choco_live_words(opt.live).to(dev)
-            d.update(psi=None if opt.psi is None else opt.psi.data_ptr(), live=self.t_live.data_ptr(), mq_B=float(opt.B),
-                     mq_bits=int(opt.bits), mq_key0=int(opt.key[0]), mq_key1=int(opt.key[1]), node0=int(pl.lo),
-                     mq_margin=opt.margin.data_ptr(), code_stride=int(self.row_bytes))
+            self.mq = dict(mq_B=float(opt.B), mq_bits=int(opt.bits), mq_key0=int(opt.key[0]), mq_key1=int(opt.key[1]),
+                           mq_margin=opt.margin.data_ptr(), code_stride=int(self.row_bytes))
+            d.update(self.mq, psi=None if opt.psi is None else opt.psi.data_ptr(), live=self.t_live.data_ptr(),
+                     node0=int(pl.lo))
         self.sparq_thr = None
-        if self.sparq:
+        if alg == "sparq_sgd":
             # the trigger thresholds (float64 in either dtype), fp64 partials of sum (theta - x_hat)^2 per chunk of
             # THREADS * (16 / itemsize) elements (dp_norm's chunks) and the optimizer's trigger counters
             self.t_live = choco_live_words(opt.live).to(dev)
             self.sparq_thr = torch.as_tensor(opt.threshold_table(H), dtype=torch.float64, device=dev)
-            pstride = max(1, -(-n_pad // (WAIT_THREADS * (16 // itemsize))))
+            pstride = partials_stride(n_pad, itemsize)
             self.norm_part = torch.zeros(L * pstride, dtype=torch.float64, device=dev)
             d.update(x_hat=opt.x_hat.data_ptr(), s=opt.s.data_ptr(), live=self.t_live.data_ptr(), gamma=float(opt.gamma),
                      code=CHOCO_CODE[opt.compressor], sparq_code_bytes=int(opt.code_bytes),
                      row_stride=int(self.row_bytes), sparq_thr=self.sparq_thr.data_ptr(),
                      norm_part=self.norm_part.data_ptr(), pstride=pstride, sparq_triggers=opt.triggers.data_ptr(),
                      local_steps=int(opt.local_steps))
-        if self.sgp:
+        if alg == "sgp":
             d.update(x=opt.x.data_ptr(), w=opt.w.data_ptr(), row_stride=int(self.row_bytes))
-        if self.pdg:
+        if alg == "push_diging":
             d.update(u=opt.u.data_ptr(), w=opt.w.data_ptr(), ysum=opt.ysum.data_ptr(), g_old=opt.g.data_ptr(),
                      row_stride=int(self.row_bytes))
         cls = self.ext.ConsensusOpF32 if self.dtype == torch.float32 else self.ext.ConsensusOpF64
@@ -654,6 +618,35 @@ class ConsensusEngine:
         tail = self.pr.arena.n_pad * self.pub.element_size()
         rows = self.pub[par, 0, :self.pr.placement.L].view(torch.uint8)
         return rows[:, tail: tail + 8].view(torch.float64)[:, 0]
+
+    def published_rows(self, k: int):
+        """The rows published for round ``k`` that hold optimizer state, as ``(view into pub, optimizer tensor, only)``.
+        ``only`` marks a published copy that is the only live one: the kernels update it and not the tensor, so
+        ``RoundProgram.sync_back`` copies it back.  ``__init__`` publishes round ``k0`` by copying every tensor in."""
+        opt, alg, n_pad = self.opt, self.opt.alg_name, self.pr.arena.n_pad
+        par = (self.rounds_per_step * k) & 1        # DeTAG, cross-gradient: the parity of protocol round K k
+        pub = self.pub[par, :, :self.pr.placement.L]
+        if alg == "beer":
+            return [(pub[0].view(torch.uint8), opt.code_h, True), (pub[1].view(torch.uint8), opt.code_g, True)]
+        if hasattr(opt, "code"):       # CHOCO-SGD, Moniqua, SPARQ-SGD
+            return [(pub[0].view(torch.uint8), opt.code, True)]
+        if alg == "sgp":               # the numerators x, and w in the row tail
+            return [(pub[0, :, :n_pad], opt.x, False), (self.pub_weights(par), opt.w, False)]
+        if alg == "push_diging":       # u with w in its row tail, and y in channel 1
+            return [(pub[0, :, :n_pad], opt.u, False), (self.pub_weights(par), opt.w, False),
+                    (pub[1, :, :n_pad], opt.y, True)]
+        if hasattr(opt, "msg"):        # RelaySum, PowerGossip: the messages, published at the end of round k - 1
+            return [(pub.transpose(0, 1), opt.msg, True)]
+        if alg == "detag":             # z = theta - alpha y and y
+            return [(pub[0], opt.z, True), (pub[1], opt.y, True)]
+        if hasattr(opt, "pub"):        # ClippedGossip, BRIDGE: an attacker's published row is not its theta
+            return [(pub[0], opt.pub, True)]
+        rows = [(pub[0], self.pr.arena.theta, False)]
+        if getattr(opt, "y", None) is not None and (alg != "dsgt" or opt._initialised):
+            rows.append((pub[1], opt.y, True))        # DSGT once initialised, K-GT with correction, GT-HSGD
+        if getattr(opt, "ut", None) is not None:
+            rows.append((pub[1], opt.ut, True))       # dadaptive with tracking (its ut row holds the mix's z)
+        return rows
 
     def bytes_per_round(self) -> Dict[str, int]:
         """Bytes one node publishes per round (``row``: one published row) and bytes this rank's nodes pull from their
@@ -677,20 +670,21 @@ class ConsensusEngine:
         neighbor's theta row (``pulled_theta``) and the gradient that neighbor took at its own row (``pulled_cross``), one
         row each per neighbor edge; ``pulled`` is both.  ``grad_evals()`` gives the round's gradient evaluations."""
         deg = int(self.t_deg[0].sum().item())
-        if self.xg:
+        alg = self.opt.alg_name
+        if alg == "cross_gradient":
             return {"row": int(self.row_bytes), "pulled": 2 * int(self.row_bytes) * deg,
                     "pulled_theta": int(self.row_bytes) * deg, "pulled_cross": int(self.row_bytes) * deg}
-        if self.sparq:
+        if alg == "sparq_sgd":
             return {"row": int(self.row_bytes), "tail": 16, "pulled_max": int(self.row_bytes) * deg}
-        if self.pga:
+        if alg == "gossip_pga":
             return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,
                     "global_row": int(self.pr.arena.n_pad) * 8, "period": int(self.opt.period)}
-        if self.pg:
+        if alg == "powergossip":
             lay, itemsize = self.opt.lay, self.pub.element_size()
             p0, p1 = (deg * lay.msg_len(ph) * itemsize for ph in (0, 1))
             return {"row": int(self.row_bytes), "pulled": (p0 + p1) // 2, "pulled_phase0": p0, "pulled_phase1": p1}
-        reads = 2 if self.cg and self.opt.clip == "adaptive" else 1
-        chans = 1 if self.relay else self.C
+        reads = 2 if alg == "clipped_gossip" and self.opt.clip == "adaptive" else 1
+        chans = 1 if alg == "relaysum" else self.C
         return {"row": int(self.row_bytes) * chans,
                 "pulled": int(self.row_bytes) * chans * deg * reads * self.rounds_per_step}
 
@@ -698,7 +692,7 @@ class ConsensusEngine:
         """Forward/backward passes per round over the network: ``useful`` counts the own gradients and one per directed
         edge, ``N + 2|E|``; ``launched`` also the idle slots of nodes below the largest degree, ``N (1 + dmax)``.  Every
         other optimizer evaluates ``draws_per_round`` gradients per node."""
-        if self.xg:
+        if self.opt.alg_name == "cross_gradient":
             useful, launched = self.opt.grad_evals()
             return {"useful": useful, "launched": launched}
         from .round_program import draws_per_round

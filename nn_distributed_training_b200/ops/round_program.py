@@ -38,7 +38,7 @@ from typing import Dict
 
 import torch
 
-from .engine import ConsensusEngine, schedule_horizon
+from .engine import THETA_ROW_ALGS, ConsensusEngine, schedule_horizon
 
 MAX_ROUNDS_PER_GRAPH = 64
 PULL_ROUNDS_PER_GRAPH = 64     # host-fed / staged rounds captured per graph (staging kernel forked inside the graph); a
@@ -178,10 +178,32 @@ def _collect_before_capture():
     gc.collect()
 
 
+class _RoundCount:
+    """Runs ``_round_ops_impl`` once without a device, as the engine and the gradient callbacks, and counts the round's
+    calls: ``ops`` on ``eng.op``, ``draws`` of ``grads(p)`` and ``extra`` of ``grads_prev`` and ``grads_cross``."""
+
+    def __init__(self, opt, sum_mode: bool = False):
+        self.sum_mode = sum_mode
+        self.op = self
+        self.ops = self.draws = self.extra = 0
+        _round_ops_impl(opt, self, self._draw, self._extra, self._extra)
+
+    def __getattr__(self, name):       # a kernel of eng.op
+        return self._op
+
+    def _op(self, *args):
+        self.ops += 1
+
+    def _draw(self, p: int = 0):
+        self.draws += 1
+
+    def _extra(self, *args):
+        self.extra += 1
+
+
 def draws_per_round(opt) -> int:
-    if opt.alg_name == "dinno":
-        return opt.pits
-    return opt.local_steps if opt.alg_name in ("kgt", "sparq_sgd") else 1
+    """Minibatch draws (``grads(p)`` calls) of one round."""
+    return _RoundCount(opt).draws
 
 
 class RoundProgram:
@@ -211,16 +233,10 @@ class RoundProgram:
                 pipeline = "resident"
         self.eng = ConsensusEngine(opt, graphs)
         self.graph_plan = graphs
-        # evaluation between rounds can use the fused consensus-metric kernel on the published rows; CHOCO-SGD and BEER
-        # publish codes, SGP and Push-DIGing numerators and the attackers of ClippedGossip and BRIDGE attack rows, so
-        # their metric reads the parameter rows (all_theta) at the evaluation points instead, as do RelaySum and
-        # PowerGossip, which publish messages, and DeTAG, whose channel 0 holds z = theta - alpha y; Moniqua publishes
-        # codes too, and SPARQ-SGD code rows with a trigger tail; the cross-gradient channels are gradients
-        attacked = (self.eng.cg or self.eng.bridge) and bool(opt.byzantine)
-        pr._metric_engine = (None if (self.eng.choco or self.eng.beer or self.eng.sgp or self.eng.pdg or attacked
-                                      or self.eng.relay or self.eng.pg or self.eng.detag or self.eng.mq
-                                      or self.eng.sparq or self.eng.xg)
-                             else (self.eng, lambda: opt.k))
+        # evaluation between rounds can use the fused consensus-metric kernel on the published rows where channel 0 holds
+        # theta; the others' metric reads the parameter rows (all_theta) at the evaluation points instead
+        theta_rows = opt.alg_name in THETA_ROW_ALGS and not getattr(opt, "byzantine", None)
+        pr._metric_engine = (self.eng, lambda: opt.k) if theta_rows else None
         self._graphs: Dict[int, torch.cuda.CUDAGraph] = {}
         self.host_mode = False
         self.pipeline = "resident"
@@ -248,22 +264,8 @@ class RoundProgram:
     def launches_per_round(self) -> int:
         """Kernel launches of one communication round (the staging kernel of the host-fed / staged pipelines
         included)."""
-        n = 1 if self.eng.sum_mode else 0
-        if self.host_mode:
-            n += 1
-        if self.opt.alg_name == "dinno":
-            return n + 2 * self.opt.pits
-        if self.opt.alg_name == "clipped_gossip" and self.opt.clip == "adaptive":
-            return n + 4
-        if self.opt.alg_name == "detag":
-            return n + self.opt.gossip_steps + 2
-        if self.opt.alg_name in ("gt_hsgd", "gossip_pga", "dp_dsgd"):
-            return n + 4
-        if self.opt.alg_name == "sparq_sgd":
-            return n + 2 + 2 * self.opt.local_steps
-        if self.opt.alg_name == "cross_gradient":
-            return n + 4 + self.opt.dmax
-        return n + (1 + 2 * self.opt.local_steps if self.opt.alg_name == "kgt" else 3)
+        c = _RoundCount(self.opt, self.eng.sum_mode)
+        return c.ops + c.draws + c.extra + (1 if self.host_mode else 0)
 
     def grads(self, p: int = 0):
         pr = self.pr
@@ -399,7 +401,7 @@ class RoundProgram:
                                f"{self.eng.horizon} rounds")
         if self.eng.dp:         # the privacy ledger follows the planned graph of every round run
             for k in range(self.opt.k, self.opt.k + rounds):
-                eav, allo = self.eng.dp_rho[self.eng.gid[k]]
+                eav, allo = self.eng.dp[self.eng.gid[k]]
                 self.opt.rho_eav += eav
                 self.opt.rho_all += allo
         if self.host_mode:
@@ -416,51 +418,21 @@ class RoundProgram:
             left -= r
 
     def sync_back(self):
-        """Mirror device-resident optimizer state into the optimizer object."""
-        opt, eng = self.opt, self.eng
-        L = self.pr.placement.L
-        if opt.alg_name in ("dsgt", "gt_hsgd"):    # GT-HSGD's v and theta_prev are the optimizer's own rows
-            par = opt.k & 1
-            opt.y.copy_(eng.pub[par, 1, :L])
-        if opt.alg_name == "kgt" and opt.correction:      # c is the optimizer's own row; d is dead between rounds
-            opt.y.copy_(eng.pub[opt.k & 1, 1, :L])
-        if opt.alg_name == "dadaptive" and opt.tracking:  # the fused ut row holds the mix's z; u~ is the published row
-            opt.ut.copy_(eng.pub[opt.k & 1, 1, :L])
-        if opt.alg_name == "push_diging":       # y is the first n_pad elements of channel 1 (u and w are shared)
-            opt.y.copy_(eng.pub[opt.k & 1, 1, :L, :self.pr.arena.n_pad])
+        """Mirror device-resident optimizer state into the optimizer object: the published rows that are the only live
+        copy (``ConsensusEngine.published_rows``) and the host scalars of round k."""
+        opt = self.opt
+        for row, dst, only in self.eng.published_rows(opt.k):
+            if only:
+                dst.copy_(row)
         if opt.alg_name == "dinno" and opt.k > 0:
             opt.rho = opt.rho_at(opt.k - 1)
-        if opt.alg_name in ("dsgd", "dsgdm", "exact_diffusion", "choco_sgd", "sgp", "clipped_gossip",
-                            "relaysum", "bridge", "powergossip", "gossip_pga", "dp_dsgd", "moniqua",
-                            "sparq_sgd", "cross_gradient") and opt.k > 0:
+        if hasattr(opt, "alpha_table") and opt.k > 0:
             opt.alph = opt.alpha_table(opt.k)[opt.k - 1]
-        if opt.alg_name == "relaysum":          # the messages published for round k
-            opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
-        if opt.alg_name == "powergossip":       # the messages of round k; pg_mix updates the vectors (opt.vec) in place
-            opt.msg.copy_(eng.pub[opt.k & 1, :, :L].transpose(0, 1))
-        if opt.alg_name == "detag":             # g_old is the optimizer's own row; the rows of protocol round K k
-            par = (opt.gossip_steps * opt.k) & 1
-            opt.z.copy_(eng.pub[par, 0, :L])
-            opt.y.copy_(eng.pub[par, 1, :L])
-        if opt.alg_name in ("clipped_gossip", "bridge"):
-            opt.pub.copy_(eng.pub[opt.k & 1, 0, :L])
-        # Moniqua's psi and margin counters and SPARQ-SGD's x_hat, s and trigger counters are their own rows
-        if opt.alg_name in ("choco_sgd", "moniqua", "sparq_sgd"):
-            opt.code.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
-        if opt.alg_name == "beer":              # h, s_h, v, g, s_g and m_old are the optimizer's own rows
-            opt.code_h.copy_(eng.pub[opt.k & 1, 0, :L].view(torch.uint8))
-            opt.code_g.copy_(eng.pub[opt.k & 1, 1, :L].view(torch.uint8))
 
 
 def run_fused_training(opt, profiler=None):
     pr = opt.pr
-    prog = getattr(opt, "_program", None)
-    if prog is None:
-        prog = opt._program = RoundProgram(opt)
-    if opt.alg_name == "dsgt" and opt.init_grads and not opt._initialised:
-        prog.dsgt_init()
-    if opt.alg_name == "dsgt":
-        opt._initialised = True
+    prog = opt.fused_program()
     every = opt._eval_every()
     oits = opt.oits
     while opt.k < oits:

@@ -167,15 +167,7 @@ class ConsensusOptimizer:
         if n <= 0:
             return
         if self._use_engine():
-            from ..ops.round_program import RoundProgram
-            prog = getattr(self, "_program", None)
-            if prog is None:
-                prog = self._program = RoundProgram(self)
-                if self.alg_name == "dsgt":
-                    if self.init_grads and not self._initialised:
-                        prog.dsgt_init()
-                    self._initialised = True
-            prog.run(n)
+            self.fused_program().run(n)
             self.k += n
         else:
             self._before_training()
@@ -189,15 +181,20 @@ class ConsensusOptimizer:
         n = min(int(n), self.oits - self.k)
         if n <= 0 or not self._use_engine():
             return
-        from ..ops.round_program import RoundProgram
+        self.fused_program().prepare(n)
+
+    def fused_program(self):
+        """The ``RoundProgram`` of the fused consensus kernels, built on first use (DSGT's initial gradient, with
+        ``init_grads``, runs then)."""
         prog = getattr(self, "_program", None)
         if prog is None:
+            from ..ops.round_program import RoundProgram
             prog = self._program = RoundProgram(self)
             if self.alg_name == "dsgt":
                 if self.init_grads and not self._initialised:
                     prog.dsgt_init()
                 self._initialised = True
-        prog.prepare(n)
+        return prog
 
     def _use_engine(self) -> bool:
         """Fused sm_90a consensus kernels.  ``consensus_backend``: ``torch`` never; ``auto`` (default) for any arena
