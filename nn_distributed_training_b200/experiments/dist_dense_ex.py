@@ -74,7 +74,8 @@ def experiment(yaml_pth):
                                                              "beer", "sgp", "push_diging", "kgt",
                                                              "clipped_gossip", "dadaptive", "relaysum",
                                                              "bridge", "powergossip", "detag", "gt_hsgd",
-                                                             "gossip_pga", "dp_dsgd", "moniqua", "cross_gradient"):
+                                                             "gossip_pga", "dp_dsgd", "moniqua", "cross_gradient",
+                                                             "slowmo"):
             raise NameError("Unknown distributed opt algorithm.")
         prob = DistDensityProblem(graph, base_model, base_loss, train_subsets, val_set, ctx.device, prob_conf,
                                   ctx=ctx, seed=int(exp_conf.get("seed", 0)))

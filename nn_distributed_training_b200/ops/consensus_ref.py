@@ -105,6 +105,24 @@ def pga_mean_(theta: torch.Tensor, theta_all: torch.Tensor) -> None:
     theta.copy_((s / theta_all.shape[0]).to(theta.dtype).expand_as(theta))
 
 
+# ---------------------------------------------------------------- SlowMo ----
+def slowmo_outer_(theta: torch.Tensor, anchor: torch.Tensor, u: torch.Tensor, m: Optional[torch.Tensor], gamma: float,
+                  slow_lr: float, slow_momentum: float) -> None:
+    """SlowMo's outer update on a global round, with ``theta`` holding the mean ``xbar`` (``pga_mean_``):
+    ``u <- slow_momentum u + (anchor - xbar) / gamma``, ``anchor <- anchor - (slow_lr gamma) u``, ``theta <- anchor``
+    and ``m <- 0`` (when given).  Evaluated in float64 from the stored rows, every operation rounded on its own, and
+    each stored row rounded once; ``gamma`` is taken in the arena dtype first, as the fused kernel reads it from the
+    schedule (csrc/consensus.cu: slowmo_outer_kernel computes the same bits)."""
+    gamma = float(torch.tensor(gamma, dtype=theta.dtype))
+    a = anchor.double()
+    un = u.double() * slow_momentum + (a - theta.double()) / gamma
+    u.copy_(un)
+    anchor.copy_(a - (slow_lr * gamma) * un)
+    theta.copy_(anchor)
+    if m is not None:
+        m.zero_()
+
+
 # ---------------------------------------------------------------- DeTAG ----
 def mixing_lambda(W: np.ndarray) -> float:
     """``max |eig(W - 11^T / N)|`` of a symmetric mixing matrix, in float64 (0 for one node and the complete graph)."""

@@ -129,6 +129,7 @@ struct ConsensusOp {
   consensus::HsgdArgs<T> hs{};
   consensus::XgArgs<T> xg{};
   consensus::PgaArgs<T> pa{};
+  consensus::SlowmoArgs<T> sm{};
   consensus::DpArgs<T> dp{};
   consensus::MoniquaArgs<T> mq{};
   consensus::SparqArgs<T> sq{};
@@ -143,7 +144,7 @@ struct ConsensusOp {
   explicit ConsensusOp(const py::dict& d) {
     c = common_from<T>(d);
     dn.c = c; gt.c = c; ed.c = c; mo.c = c; ch.c = c; be.c = c; kg.c = c; ad.c = c; rs.c = c; cg.c = c; br.c = c; sg.c = c;
-    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c; sq.c = c; xg.c = c;
+    pd.c = c; pg.c = c; dt.c = c; hs.c = c; pa.c = c; dp.c = c; mq.c = c; sq.c = c; xg.c = c; sm.c = c;
     xg.xmix = ptr<T>(d, "xmix"); xg.theta_x = ptr<T>(d, "theta_x"); xg.grad_part_x = ptr<const T>(d, "grad_part_x");
     xg.g = ptr<T>(d, "xg_g"); xg.coef0 = ptr<const double>(d, "xg_coef0"); xg.coef = ptr<const double>(d, "xg_coef");
     pg.vec = ptr<T>(d, "pg_vec"); pg.seg = ptr<const int>(d, "pg_seg"); pg.sign = ptr<const int>(d, "pg_sign");
@@ -172,6 +173,9 @@ struct ConsensusOp {
     hs.grad_part_prev = ptr<const T>(d, "grad_part_prev"); hs.v = ptr<T>(d, "hsgd_v"); hs.theta_prev = ptr<T>(d, "theta_prev");
     hs.omb = (T)getf(d, "omb", 0.0);
     pa.period = geti(d, "period", 0); pa.gossip = geti(d, "gossip", 1);
+    sm.anchor = ptr<T>(d, "anchor"); sm.u = ptr<T>(d, "slow_u"); sm.m = ptr<T>(d, "m"); sm.period = pa.period;
+    sm.alpha0 = (T)getf(d, "alpha0", 0.0); sm.slow_lr = getf(d, "slow_lr", 1.0);
+    sm.slow_momentum = getf(d, "slow_momentum", 0.0);
     dp.norm_part = ptr<double>(d, "norm_part"); dp.pstride = geti(d, "pstride", 0);
     dp.nbr_id = ptr<const int>(d, "nbr_id"); dp.live = ptr<const unsigned>(d, "live"); dp.node0 = geti(d, "node0", 0);
     dp.clip = getf(d, "clip_norm", 0.0); dp.cz_dp = getf(d, "cz_dp", 0.0); dp.cz_pair = getf(d, "cz_pair", 0.0);
@@ -296,6 +300,12 @@ struct ConsensusOp {
   void pga_mix() {
     pga_check("pga_mix");
     check(consensus::launch_pga_mix<T>(pa, cur_stream()), "pga_mix");
+  }
+  void slowmo_outer() {
+    if (sm.period < 1 || sm.anchor == nullptr || sm.u == nullptr || c.C != 1)
+      throw std::runtime_error("slowmo_outer needs `period` >= 1, the SlowMo rows `anchor` and `slow_u` and one "
+                               "published channel");
+    check(consensus::launch_slowmo_outer<T>(sm, cur_stream()), "slowmo_outer");
   }
   void dp_check(const char* what) const {
     if (dp.norm_part == nullptr || dp.pstride <= 0 || dp.nbr_id == nullptr || dp.live == nullptr || !(dp.clip > 0.0) ||
@@ -515,6 +525,7 @@ static void bind_consensus(py::module& m, const char* name) {
       .def("xg_step", &ConsensusOp<T>::xg_step)
       .def("pga_sum", &ConsensusOp<T>::pga_sum)
       .def("pga_mix", &ConsensusOp<T>::pga_mix)
+      .def("slowmo_outer", &ConsensusOp<T>::slowmo_outer)
       .def("dp_norm", &ConsensusOp<T>::dp_norm)
       .def("dp_step", &ConsensusOp<T>::dp_step)
       .def("mq_mix", &ConsensusOp<T>::mq_mix)

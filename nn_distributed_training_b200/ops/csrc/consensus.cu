@@ -16,6 +16,7 @@
 // GT-HSGD (no reference counterpart, optimizers/gt_hsgd.py)                -> dsgt_mix / hsgd_track
 // cross-gradient (no reference counterpart, optimizers/cross_gradient.py)  -> xg_pull / xg_publish, xg_step
 // Gossip-PGA / local SGD (no reference counterpart, optimizers/gossip_pga.py) -> pga_sum + pga_mix / dsgd_step
+// SlowMo (no reference counterpart, optimizers/slowmo.py)  -> pga_sum + pga_mix + slowmo_outer / dsgd_step or dsgdm_step
 // DP-DSGD / DECOR (no reference counterpart, optimizers/dp_dsgd.py)        -> dsgd_mix / dp_norm + dp_step
 // Moniqua (no reference counterpart, optimizers/moniqua.py)                -> mq_mix / mq_step
 // decentralized AMSGrad / AdaGrad (no reference counterpart,
@@ -1575,6 +1576,47 @@ __global__ void __launch_bounds__(THREADS) pga_mix_kernel(const PgaArgs<T> a) {
   }
 }
 
+// ----------------------------------------------------------------- SlowMo ----
+// Round k: pga_sum, pga_mix, slowmo_outer, fwd/bwd, dsgd_step or dsgdm_step (both unchanged).  A separate launch keeps
+// pga_mix as Gossip-PGA has it.  On a global round, after pga_mix wrote xbar into theta (consensus.h: SlowmoArgs):
+//   u <- beta_s u + (a - xbar) / gamma;  a <- a - (alpha_s gamma) u;  theta <- a;  m <- 0
+// in fp64 from the stored rows, every operation rounded on its own (no contraction, as the PyTorch path computes it),
+// each stored row rounded once.  A zeroed m makes the next dsgdm_step take its round-0 step.  Every store is after the
+// pdl_wait: theta is pga_mix's, m the previous round's step's.
+template <typename T>
+__global__ void __launch_bounds__(THREADS) slowmo_outer_kernel(const SlowmoArgs<T> a) {
+  const Common<T>& c = a.c;
+  pdl_wait();
+  pdl_launch_dependents();
+  const RoundInfo<T> ri = round_info(c);
+  if (!pga_phase(ri.k, a.period).global) return;
+  constexpr int N = Vec<T>::N;
+  const int l = node_of_block(c);
+  const size_t row = (size_t)l * c.n_pad;
+  const double gamma = ri.k == 0 ? (double)a.alpha0 : (double)c.alpha[ri.k - 1];
+  const double step = __dmul_rn(a.slow_lr, gamma);
+  for (int i = (blockIdx.x * THREADS + threadIdx.x) * N; i < c.n_pad; i += gridDim.x * THREADS * N) {
+    const Pack<T> x = ldv(c.theta + row + i);
+    Pack<T> an = ldv(a.anchor + row + i), uu = ldv(a.u + row + i);
+#pragma unroll
+    for (int v = 0; v < N; ++v) {
+      const double un = __dadd_rn(__dmul_rn(a.slow_momentum, (double)uu.v[v]),
+                                  div_rn(__dsub_rn((double)an.v[v], (double)x.v[v]), gamma));
+      uu.v[v] = (T)un;
+      an.v[v] = (T)__dsub_rn((double)an.v[v], __dmul_rn(step, un));
+    }
+    stv(a.u + row + i, uu);
+    stv(a.anchor + row + i, an);
+    stv(c.theta + row + i, an);
+    if (a.m != nullptr) {
+      Pack<T> z;
+#pragma unroll
+      for (int v = 0; v < N; ++v) z.v[v] = (T)0;
+      stv(a.m + row + i, z);
+    }
+  }
+}
+
 // ---------------------------------------------------------------- DP-DSGD ----
 // Round k (stream and rules in consensus.h: DpArgs): dsgd_mix, fwd/bwd, dp_norm, dp_step.  The clip factor needs the
 // norm of the whole gradient row, which is spread over the CTAs of the node, so the norm takes a launch of its own:
@@ -3086,6 +3128,11 @@ template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream
     return cudaErrorInvalidValue;
   return launch_one_wave(pga_mix_kernel<T>, a.c, a, st);
 }
+// one wave over the local rows, as dsgd_step
+template <typename T> cudaError_t launch_slowmo_outer(const SlowmoArgs<T>& a, cudaStream_t st) {
+  if (a.period < 1 || a.anchor == nullptr || a.u == nullptr || a.c.C != 1) return cudaErrorInvalidValue;
+  return launch_one_wave(slowmo_outer_kernel<T>, a.c, a, st);
+}
 
 // dp_norm and dp_step: one wave each, the 8-deep partial sum beyond 4 partials (as sgp_step)
 template <typename T> static bool dp_ready(const DpArgs<T>& a) {
@@ -3276,6 +3323,7 @@ template <typename T> cudaError_t launch_pdg_track(const PushDigArgs<T>& a, cuda
   template cudaError_t launch_xg_step<T>(const XgArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_pga_sum<T>(const PgaArgs<T>&, cudaStream_t);            \
   template cudaError_t launch_pga_mix<T>(const PgaArgs<T>&, cudaStream_t);            \
+  template cudaError_t launch_slowmo_outer<T>(const SlowmoArgs<T>&, cudaStream_t);    \
   template cudaError_t launch_dp_norm<T>(const DpArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_dp_step<T>(const DpArgs<T>&, cudaStream_t);             \
   template cudaError_t launch_mq_mix<T>(const MoniquaArgs<T>&, cudaStream_t);         \

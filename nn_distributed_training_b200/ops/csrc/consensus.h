@@ -235,6 +235,23 @@ struct PgaArgs {
   int gossip;                      // 1 = Metropolis mix on gossip rounds, 0 = none (local SGD)
 };
 
+// SlowMo (Wang, Tantia, Ballas, Rabbat 2020), optimizers/slowmo.py: Gossip-PGA's round with an outer update after the
+// global mix.  The round is pga_sum, pga_mix, slowmo_outer, fwd/bwd, then dsgd_step or (base momentum) dsgdm_step in
+// local mode.  On a global round slowmo_outer takes xbar from theta (pga_mix wrote the mean there) and, in fp64 with
+// gamma = alpha[k - 1] (alpha0 at k = 0),
+//   u <- slow_momentum u + (anchor - xbar) / gamma;  anchor <- anchor - slow_lr gamma u;  theta <- anchor;  m <- 0
+// rounding each stored row once; on a gossip round it returns at once.  It adds no cross-node traffic.
+template <typename T>
+struct SlowmoArgs {
+  Common<T> c;
+  T* anchor;                       // [L, n_pad] the point the last global round stepped to (theta^0 before it)
+  T* u;                            // [L, n_pad] the slow momentum
+  T* m;                            // [L, n_pad] the base momentum row zeroed on global rounds; nullptr = no base momentum
+  int period;                      // >= 1, Gossip-PGA's
+  T alpha0;                        // gamma of round 0
+  double slow_lr, slow_momentum;
+};
+
 // DP-DSGD and DECOR (Allouah, Koloskova, El Mrini, Guerraoui, Jaggi 2024), optimizers/dp_dsgd.py: DSGD's single
 // published channel and mix (dsgd_mix_kernel through the pointer table), then the node-level clipped and noised step
 //   f_i = min(1, C / ||g_i||),  v_i = cz_dp xi_i + cz_pair sum_j s_ij xi_ij,  theta_i -= alpha_k (f_i g_i + v_i)
@@ -475,6 +492,7 @@ template <typename T> cudaError_t launch_xg_publish(const XgArgs<T>& a, cudaStre
 template <typename T> cudaError_t launch_xg_step(const XgArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_sum(const PgaArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_pga_mix(const PgaArgs<T>& a, cudaStream_t st);
+template <typename T> cudaError_t launch_slowmo_outer(const SlowmoArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dp_norm(const DpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_dp_step(const DpArgs<T>& a, cudaStream_t st);
 template <typename T> cudaError_t launch_mq_mix(const MoniquaArgs<T>& a, cudaStream_t st);

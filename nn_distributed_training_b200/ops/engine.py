@@ -51,9 +51,13 @@ def schedule_tables(opt, H: int):
 # of the network sum.  The others pull through the pointer table: their rows are codes, numerators with a weight or
 # per-edge messages, or a mix clips, screens, noises or averages globally per edge or per round
 SUM_MODE_ALGS = frozenset({"dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "kgt", "dadaptive", "gt_hsgd"})
+# Algorithms that average the whole network every ``period``-th round (Gossip-PGA's global round: pga_sum, pga_mix): they
+# own the fp64 partial sums and sum flags on any graph, need NVLS across ranks, plan the edgeless graph with
+# ``gossip: false`` and pull Gossip-PGA's bytes
+GLOBAL_AVG_ALGS = frozenset({"gossip_pga", "slowmo"})
 # Algorithms whose published channel 0 is theta, so the fused consensus metric can read it (not while Byzantine nodes
 # publish attack rows there)
-THETA_ROW_ALGS = SUM_MODE_ALGS | {"gossip_pga", "dp_dsgd", "clipped_gossip", "bridge"}
+THETA_ROW_ALGS = SUM_MODE_ALGS | GLOBAL_AVG_ALGS | {"dp_dsgd", "clipped_gossip", "bridge"}
 
 # Why an algorithm needs the planned graph sequence to be one fixed graph (and the one in ``opt.topo`` when it holds one)
 FIXED_GRAPH = {
@@ -210,8 +214,8 @@ class ConsensusEngine:
         # sequence tags count K per gradient round and the schedules hold K entries per gradient round.
         # Cross-gradient: gradient round k is protocol rounds 2k (xg_pull .. xg_publish) and 2k + 1 (xg_step)
         K = self.rounds_per_step = opt.gossip_steps if alg == "detag" else 2 if alg == "cross_gradient" else 1
-        # Gossip-PGA's local SGD (gossip: false) plans the edgeless graph
-        if alg == "gossip_pga" and not opt.gossip:
+        # Gossip-PGA's and SlowMo's local SGD (gossip: false) plans the edgeless graph
+        if alg in GLOBAL_AVG_ALGS and not opt.gossip:
             edgeless = opt.edgeless_graph()
             graphs_per_round = [edgeless] * len(graphs_per_round)
         # SGP and Push-DIGing mix with the column-stochastic push-sum weights and publish the node's weight w
@@ -395,28 +399,28 @@ class ConsensusEngine:
 
         # ---- complete graph: uniform Metropolis weights -> aggregates are functions of the network sum ----
         # (the algorithms outside SUM_MODE_ALGS always pull through the pointer table; complete_graph_mode is ignored.
-        # Gossip-PGA's global rounds average through the same fp64 partial sums, with sum_mode 0)
+        # the global rounds of GLOBAL_AVG_ALGS average through the same fp64 partial sums, with sum_mode 0)
         self.sum_mode = (G == 1 and topos[0].is_complete() and pr.N > 1 and alg in SUM_MODE_ALGS
                          and opt.conf.get("complete_graph_mode", "sum") == "sum")
         self.sum_buf = self.sum_flag_buf = None
         sum_mc = None
-        if self.sum_mode or alg == "gossip_pga":
+        if self.sum_mode or alg in GLOBAL_AVG_ALGS:
             self.sum_buf = SymmetricBuffer((2, self.C, n_pad), torch.float64, ctx)   # fp64: S - N*theta cancels in fp32
             self.sum_flag_buf = SymmetricBuffer((max(ctx.world_size, 1),), torch.int32, ctx)
             self.sum_flag_buf.local.fill_(k0)
             if ctx.is_distributed:
                 if self.sum_buf.multicast_ptr:
                     sum_mc = self.sum_buf.multicast_ptr      # NVLS: one in-switch reduction per element
-                elif alg == "gossip_pga":
-                    raise ValueError("gossip_pga on more than one rank averages over NVLS (one in-switch reduction of "
-                                     "the fp64 partial sums per global round), and this fabric gives its symmetric "
-                                     "buffer no multicast mapping")
+                elif alg in GLOBAL_AVG_ALGS:
+                    raise ValueError(f"{alg} on more than one rank averages over NVLS (one in-switch reduction of "
+                                     f"the fp64 partial sums per global round), and this fabric gives its symmetric "
+                                     f"buffer no multicast mapping")
                 else:
                     self.sum_mode = False                    # no multicast mapping on this fabric: pointer table
                 torch.cuda.synchronize(dev)
                 ctx.barrier()
         peer_sum_flag = np.zeros(max(ctx.world_size, 1), dtype=np.int64)
-        if self.sum_mode or alg == "gossip_pga":
+        if self.sum_mode or alg in GLOBAL_AVG_ALGS:
             for r in range(ctx.world_size):
                 peer_sum_flag[r] = self.sum_flag_buf.peer_ptrs[r] + 4 * ctx.rank
         self.t_peer_sum_flag = torch.as_tensor(peer_sum_flag, device=dev)
@@ -459,10 +463,15 @@ class ConsensusEngine:
         if self.sum_mode:
             d.update(sum_mode=1, n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
                      sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr())
-        if alg == "gossip_pga":
+        if alg in GLOBAL_AVG_ALGS:
             d.update(n_total=pr.N, sum_local=self.sum_buf.local.data_ptr(), sum_mc=sum_mc,
                      sum_flags=self.sum_flag_buf.local.data_ptr(), peer_sum_flag=self.t_peer_sum_flag.data_ptr(),
                      period=opt.period, gossip=int(opt.gossip))
+        if alg == "slowmo":
+            # the outer update's rows, and the base momentum row with its local-mode dsgdm_step arguments
+            d.update(anchor=opt.anchor.data_ptr(), slow_u=opt.u.data_ptr(), alpha0=opt.alph0, slow_lr=opt.slow_lr,
+                     slow_momentum=opt.slow_momentum, m=None if opt.m is None else opt.m.data_ptr(),
+                     beta=opt.base_momentum, quasi_global=0, nesterov=int(opt.nesterov))
         if alg == "dinno":
             d.update(dual=opt.duals.data_ptr(), delta=opt.delta.data_ptr(),
                      m=None if opt.m is None else opt.m.data_ptr(),
@@ -661,8 +670,8 @@ class ConsensusEngine:
         pull: ``pulled`` counts them all.  A GT-HSGD round exchanges what a DSGT round does.  A Gossip-PGA gossip round
         pulls what a DSGD round does (nothing with ``gossip: false``: the edgeless graph); a global round pulls no row
         and contributes one fp64 partial-sum row per rank (``global_row``, ``n_pad * 8`` bytes) to the NVLS
-        reduction, once every ``period`` rounds.  A DP-DSGD round pulls what a DSGD round does: the edge noise is
-        drawn on both ends, and the norm partials stay on the node.  A Moniqua row is the node's code row,
+        reduction, once every ``period`` rounds; SlowMo's outer update adds no traffic, so it pulls Gossip-PGA's
+        bytes.  A DP-DSGD round pulls what a DSGD round does: the edge noise is drawn on both ends, and the norm partials stay on the node.  A Moniqua row is the node's code row,
         ``n_pad * bits / 8`` bytes, one per neighbor edge as DSGD's rows; the margin counters stay on the node.  A
         SPARQ-SGD row is the code row and its 16-byte tail (``row``); every neighbor edge pulls the tail each round
         (``tail``) and the code body only when its source triggered: ``pulled_max`` is the round where every neighbor
@@ -676,7 +685,7 @@ class ConsensusEngine:
                     "pulled_theta": int(self.row_bytes) * deg, "pulled_cross": int(self.row_bytes) * deg}
         if alg == "sparq_sgd":
             return {"row": int(self.row_bytes), "tail": 16, "pulled_max": int(self.row_bytes) * deg}
-        if alg == "gossip_pga":
+        if alg in GLOBAL_AVG_ALGS:
             return {"row": int(self.row_bytes), "pulled": int(self.row_bytes) * deg,
                     "global_row": int(self.pr.arena.n_pad) * 8, "period": int(self.opt.period)}
         if alg == "powergossip":

@@ -19,6 +19,8 @@ A round is a short, fixed kernel sequence
     DeTAG:  ag_gossip(s) x gossip_steps, fwd/bwd, detag_track      (every ag_gossip a protocol round)
     GT-HSGD:  dsgt_mix, fwd/bwd, fwd/bwd at theta_prev, hsgd_track   (both fwd/bwd on the same minibatch)
     Gossip-PGA:  pga_sum, pga_mix, fwd/bwd, dsgd_step             (pga_sum returns at once on gossip rounds)
+    SlowMo:  pga_sum, pga_mix, slowmo_outer, fwd/bwd, dsgd_step   (base momentum: dsgdm_step; slowmo_outer returns at once
+             on gossip rounds)
     DP-DSGD / DECOR:  dsgd_mix, fwd/bwd, dp_norm, dp_step
     Moniqua:  mq_mix, fwd/bwd, mq_step
     SPARQ-SGD:  sparq_mix, [fwd/bwd, sparq_step(p)] x local_steps, sparq_publish
@@ -144,6 +146,15 @@ def _round_ops_impl(opt, eng, grads, grads_prev, grads_cross):
         eng.op.pga_mix()
         grads(0)
         eng.op.dsgd_step()
+    elif alg == "slowmo":
+        eng.op.pga_sum()
+        eng.op.pga_mix()
+        eng.op.slowmo_outer()
+        grads(0)
+        if opt.m is None:
+            eng.op.dsgd_step()
+        else:
+            eng.op.dsgdm_step()
     elif alg == "dp_dsgd":
         eng.op.dsgd_mix()
         grads(0)

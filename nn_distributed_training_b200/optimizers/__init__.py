@@ -19,6 +19,7 @@ from .powergossip import PowerGossip
 from .push_diging import PushDIGing
 from .relaysum import RelaySum
 from .sgp import SGP
+from .slowmo import SlowMo
 from .sparq import SparqSGD
 
 ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact_diffusion": ExactDiffusion,
@@ -26,7 +27,8 @@ ALGORITHMS = {"dinno": DiNNO, "dsgd": DSGD, "dsgdm": DSGDm, "dsgt": DSGT, "exact
               "push_diging": PushDIGing, "kgt": KGT, "clipped_gossip": ClippedGossip, "dadaptive": DAdaptive,
               "relaysum": RelaySum, "bridge": Bridge, "powergossip": PowerGossip, "detag": DeTAG,
               "gt_hsgd": GTHSGD, "gossip_pga": GossipPGA, "dp_dsgd": DPDSGD,
-              "moniqua": Moniqua, "sparq_sgd": SparqSGD, "cross_gradient": CrossGradient}
+              "moniqua": Moniqua, "sparq_sgd": SparqSGD, "cross_gradient": CrossGradient,
+              "slowmo": SlowMo}
 
 
 def build_optimizer(problem, device, opt_conf):

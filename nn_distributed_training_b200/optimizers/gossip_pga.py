@@ -33,10 +33,10 @@ from .base import ConsensusOptimizer
 from ..ops import consensus_ref as ref
 
 
-def check_period(v) -> int:
+def check_period(v, alg: str = "gossip_pga") -> int:
     """``period`` must be an integer >= 1 (a bool or a float is refused)."""
     if isinstance(v, bool) or not isinstance(v, numbers.Integral) or int(v) < 1:
-        raise ValueError(f"gossip_pga period must be an integer >= 1 (got {v!r})")
+        raise ValueError(f"{alg} period must be an integer >= 1 (got {v!r})")
     return int(v)
 
 
@@ -46,21 +46,21 @@ class GossipPGA(ConsensusOptimizer):
 
     def __init__(self, ddl_problem, device, conf):
         if conf.get("mixing_order", "jacobi") != "jacobi":
-            raise ValueError("gossip_pga runs the synchronous (jacobi) mixing order only")
+            raise ValueError(f"{self.alg_name} runs the synchronous (jacobi) mixing order only")
         super().__init__(ddl_problem, device, conf)
         graph = getattr(self.pr, "graph", None)
         if graph is not None and graph.is_directed():
-            raise ValueError("gossip_pga needs an undirected graph (a doubly stochastic Metropolis matrix)")
+            raise ValueError(f"{self.alg_name} needs an undirected graph (a doubly stochastic Metropolis matrix)")
         if conf.get("byzantine") is not None:
-            raise ValueError("gossip_pga does not model Byzantine attackers (clipped_gossip and bridge do)")
+            raise ValueError(f"{self.alg_name} does not model Byzantine attackers (clipped_gossip and bridge do)")
         self.alph0 = float(conf["alpha0"])
         if not (math.isfinite(self.alph0) and self.alph0 >= 0.0):
-            raise ValueError(f"gossip_pga alpha0 must be finite and >= 0 (got {conf['alpha0']!r})")
+            raise ValueError(f"{self.alg_name} alpha0 must be finite and >= 0 (got {conf['alpha0']!r})")
         self.mu = float(conf.get("mu", 0.0))
-        self.period = check_period(conf["period"])
+        self.period = check_period(conf["period"], self.alg_name)
         self.gossip = conf.get("gossip", True)
         if not isinstance(self.gossip, bool):
-            raise ValueError(f"gossip_pga gossip must be true or false (got {self.gossip!r})")
+            raise ValueError(f"{self.alg_name} gossip must be true or false (got {self.gossip!r})")
         self.alph = self.alph0
         self.refresh_graph = bool(conf.get("update_graph", True))
 

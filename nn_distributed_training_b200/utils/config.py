@@ -22,7 +22,7 @@ REQUIRED = object()
 
 ALGS = ("dinno", "dsgd", "dsgdm", "dsgt", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt",
         "clipped_gossip", "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-        "moniqua", "sparq_sgd", "cross_gradient")
+        "moniqua", "sparq_sgd", "cross_gradient", "slowmo")
 # the algorithms that model Byzantine attackers (byzantine: {nodes, attack, scale, z})
 BYZANTINE_ALGS = ("clipped_gossip", "bridge")
 # graph types that generate an nx.DiGraph (utils/graph_generation.py); only the push-sum algorithms run on them
@@ -78,6 +78,9 @@ OPT_SCHEMA = {
                   "local_steps": 1, "threshold_growth": 0.0, "outer_iterations": REQUIRED, "profile": False},
     "cross_gradient": {"alpha0": REQUIRED, "mu": 0.0, "cross_weight": REQUIRED, "outer_iterations": REQUIRED,
                        "profile": False},
+    "slowmo": {"alpha0": REQUIRED, "mu": 0.0, "period": REQUIRED, "gossip": True, "slow_momentum": REQUIRED,
+               "slow_lr": 1.0, "base_momentum": 0.0, "nesterov": False, "outer_iterations": REQUIRED,
+               "update_graph": True, "profile": False},
 }
 DADAPTIVE_BETA2 = 0.999
 # framework extensions accepted in every optimizer_config
@@ -213,6 +216,35 @@ def _check_gossip_pga(c: Dict[str, Any], path: str) -> None:
         raise ConfigError(f"{path}.period must be an integer >= 1 (got {p!r})")
     if not isinstance(c["gossip"], bool):
         raise ConfigError(f"{path}.gossip must be true or false (got {c['gossip']!r})")
+
+
+SLOWMO_KEYS = ("alg_name", "alpha0", "mu", "period", "gossip", "slow_momentum", "slow_lr", "base_momentum", "nesterov",
+               "outer_iterations", "update_graph", "profile")
+
+
+def _check_slowmo(c: Dict[str, Any], path: str) -> None:
+    """SlowMo: Gossip-PGA's keys with ``alpha0`` > 0 (the slow step divides by the step size), ``slow_momentum`` and
+    ``base_momentum`` in [0, 1), ``slow_lr`` (finite, > 0), ``nesterov`` (a bool) and no other key.  A schedule that
+    reaches a step <= 0 is refused when the optimizer is built."""
+    for key in c:
+        if key not in SLOWMO_KEYS and key not in OPT_EXTRA and key != "debug_sequence_check":
+            raise ConfigError(f"{path}.{key}: slowmo takes no key {key!r} (its keys are alpha0, mu, period, gossip, "
+                              f"slow_momentum, slow_lr, base_momentum, nesterov, outer_iterations and update_graph)")
+    if not _real(c["alpha0"]) or not (math.isfinite(float(c["alpha0"])) and float(c["alpha0"]) > 0.0):
+        raise ConfigError(f"{path}.alpha0 must be finite and > 0 (got {c['alpha0']!r})")
+    if not _real(c["mu"]) or not (math.isfinite(float(c["mu"])) and float(c["mu"]) >= 0.0):
+        raise ConfigError(f"{path}.mu must be finite and >= 0 (got {c['mu']!r})")
+    p = c["period"]
+    if isinstance(p, bool) or not isinstance(p, int) or p < 1:
+        raise ConfigError(f"{path}.period must be an integer >= 1 (got {p!r})")
+    for key in ("slow_momentum", "base_momentum"):
+        if not _real(c[key]) or not 0.0 <= float(c[key]) < 1.0:
+            raise ConfigError(f"{path}.{key} must be in [0, 1) (got {c[key]!r})")
+    if not _real(c["slow_lr"]) or not (math.isfinite(float(c["slow_lr"])) and float(c["slow_lr"]) > 0.0):
+        raise ConfigError(f"{path}.slow_lr must be finite and > 0 (got {c['slow_lr']!r})")
+    for key in ("gossip", "nesterov"):
+        if not isinstance(c[key], bool):
+            raise ConfigError(f"{path}.{key} must be true or false (got {c[key]!r})")
 
 
 CROSS_GRADIENT_KEYS = ("alg_name", "alpha0", "mu", "cross_weight", "outer_iterations", "profile")
@@ -386,7 +418,7 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
                           f"bridge (alg_name is {alg!r})")
     if (alg in ("dsgdm", "exact_diffusion", "choco_sgd", "beer", "sgp", "push_diging", "kgt", "clipped_gossip",
                 "dadaptive", "relaysum", "bridge", "powergossip", "detag", "gt_hsgd", "gossip_pga", "dp_dsgd",
-                "moniqua", "sparq_sgd", "cross_gradient")
+                "moniqua", "sparq_sgd", "cross_gradient", "slowmo")
             and c.get("mixing_order", "jacobi") != "jacobi"):
         raise ConfigError(f"{path}.mixing_order: {alg} runs the synchronous 'jacobi' order only "
                           f"(got {c['mixing_order']!r})")
@@ -450,6 +482,8 @@ def validate_optimizer(conf: Dict[str, Any], path: str = "optimizer_config") -> 
         _check_sparq(c, path)
     if alg == "cross_gradient":
         _check_cross_gradient(c, path)
+    if alg == "slowmo":
+        _check_slowmo(c, path)
     if alg in BYZANTINE_ALGS and c.get("byzantine") is not None:
         from ..optimizers.clipped_gossip import check_byzantine
         try:

@@ -26,7 +26,8 @@ ALG_COLORS = {"dinno": (255, 140, 0), "cadmm": (255, 140, 0), "dsgt": (50, 205, 
               "relaysum": (210, 105, 30), "bridge": (112, 128, 144),
               "powergossip": (0, 139, 139), "detag": (178, 34, 34),
               "gt_hsgd": (72, 61, 139), "gossip_pga": (218, 165, 32),
-              "dp_dsgd": (199, 21, 133), "moniqua": (46, 139, 87), "cross_gradient": (0, 0, 205)}
+              "dp_dsgd": (199, 21, 133), "moniqua": (46, 139, 87), "cross_gradient": (0, 0, 205),
+              "slowmo": (255, 99, 71)}
 FALLBACK = [(31, 119, 180), (214, 39, 40), (44, 160, 44), (148, 103, 189), (140, 86, 75), (23, 190, 207)]
 
 
