@@ -170,3 +170,29 @@ class OnlineWindowSchedule:
             d += take
             left -= take
         return torch.cat(out)
+
+
+WIN_MAX = 64   # windows per period the in-kernel sampler holds (kWinMax in ops/csrc/sampler.cuh)
+
+
+def window_table(schedules: List[OnlineWindowSchedule], K: int = WIN_MAX) -> np.ndarray:
+    """Per-node tables of one period of each sliding-window stream, the layout ``stream_row`` of
+    ops/csrc/sampler.cuh decodes: row ``l`` is ``[n_windows, period, cum[0..K], lb[K], ub[K]]`` for
+    ``schedules[l]``, where ``cum`` are the window start offsets in the period.  The period ends at
+    the first recurrence of window 0."""
+    tab = np.zeros((len(schedules), 2 + (K + 1) + 2 * K), dtype=np.int64)
+    for l, sch in enumerate(schedules):
+        wins = [sch.window(0)]
+        while True:
+            w = sch.window(len(wins))
+            if w == wins[0]:
+                break
+            wins.append(w)
+            if len(wins) > K:
+                raise RuntimeError(f"online window stream has more than {K} windows per period")
+        cum = np.concatenate([[0], np.cumsum([ub - lb for lb, ub, _ in wins])])
+        tab[l, 0], tab[l, 1] = len(wins), cum[-1]
+        tab[l, 2: 2 + len(cum)] = cum
+        tab[l, 2 + K + 1: 2 + K + 1 + len(wins)] = [w[0] for w in wins]
+        tab[l, 2 + 2 * K + 1: 2 + 2 * K + 1 + len(wins)] = [w[1] for w in wins]
+    return tab

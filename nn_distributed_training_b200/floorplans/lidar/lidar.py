@@ -89,20 +89,23 @@ class Lidar2D(_LidarBase):
             self._tables = (key, t(tx), t(ty), t(c))
         return self._tables[1:]
 
+    def cuda_args(self, device):
+        """Spline tables and beam parameters of ops/csrc/lidar.cu's ``lidar_scan`` / ``lidar_density``, without the
+        poses and the output."""
+        tx, ty, c = self._spline_tables(device)
+        return dict(tx=tx.data_ptr(), ty=ty.data_ptr(), coef=c.data_ptr(), ntx=tx.numel(), nty=ty.numel(),
+                    num_beams=self.num_beams, beam_samps=self.beam_samps, collision_samps=self.collision_samps,
+                    fine_samps=self.fine_samps, beam_len=float(self.beam_len), samp_df=float(self.samp_df))
+
     def scan_batch_cuda(self, pos, device="cuda"):
         """GPU twin of ``scan_batch`` (one thread per pose x beam; fp64)."""
         from ...ops import load_ext
         ext = load_ext(required=True)
         pos = np.asarray(pos, dtype=float).reshape(-1, 2)
         self._check_free(pos)
-        tx, ty, c = self._spline_tables(device)
         poses = torch.as_tensor(pos, dtype=torch.float64, device=device).contiguous()
         out = torch.empty(pos.shape[0], self.num_beams * self.beam_samps, 3, dtype=torch.float64, device=device)
-        ext.lidar_scan(dict(tx=tx.data_ptr(), ty=ty.data_ptr(), coef=c.data_ptr(), ntx=tx.numel(), nty=ty.numel(),
-                            poses=poses.data_ptr(), n_poses=pos.shape[0], num_beams=self.num_beams,
-                            beam_samps=self.beam_samps, collision_samps=self.collision_samps,
-                            fine_samps=self.fine_samps, beam_len=float(self.beam_len), samp_df=float(self.samp_df),
-                            out=out.data_ptr()))
+        ext.lidar_scan(dict(self.cuda_args(device), poses=poses.data_ptr(), n_poses=pos.shape[0], out=out.data_ptr()))
         return out
 
     def scan_batch(self, pos, chunk=512, device=None):

@@ -42,6 +42,9 @@ __device__ __forceinline__ void basis(const double* t, int i, double x, double (
   }
 }
 
+// spacing of n samples over [0, 1], as np.linspace(0, 1, n): a single sample sits at t = 0
+__device__ __forceinline__ double unit_step(int n) { return n > 1 ? 1.0 / (double)(n - 1) : 0.0; }
+
 __device__ __forceinline__ double density(const Spline& s, double x, double y) {
   x = fmin(fmax(x, s.tx[3]), s.tx[s.ntx - 4]);
   y = fmin(fmax(y, s.ty[3]), s.ty[s.nty - 4]);
@@ -69,7 +72,7 @@ __global__ void __launch_bounds__(128) scan_kernel(const Args a) {
   const double bx = a.beam_len * cos(ang), by = a.beam_len * sin(ang);
   const double thr = 0.5;
   // coarse march: first sample at or above the threshold (index 0 == the pose itself == "no hit")
-  const double cstep = 1.0 / (double)(a.collision_samps - 1);
+  const double cstep = unit_step(a.collision_samps);
   int hit = 0;
   for (int i = 0; i < a.collision_samps; ++i) {
     const double t = (double)i * cstep;
@@ -80,7 +83,7 @@ __global__ void __launch_bounds__(128) scan_kernel(const Args a) {
   if (collided) {
     const double t1 = (double)hit * cstep, t0 = (double)(hit - 1) * cstep;
     const double cx = px + t1 * bx, cy = py + t1 * by, lx = px + t0 * bx, ly = py + t0 * by;
-    const double fstep = 1.0 / (double)(a.fine_samps - 1);
+    const double fstep = unit_step(a.fine_samps);
     int fh = 0;
     for (int i = 0; i < a.fine_samps; ++i) {
       const double t = (double)i * fstep;
@@ -89,7 +92,7 @@ __global__ void __launch_bounds__(128) scan_kernel(const Args a) {
     const double tf = (double)fh * fstep;
     ex = lx + tf * (cx - lx); ey = ly + tf * (cy - ly);
   }
-  const double sstep = 1.0 / (double)(a.beam_samps - 1);
+  const double sstep = unit_step(a.beam_samps);
   double* out = a.out + ((size_t)p * a.num_beams + b) * a.beam_samps * 3;
   for (int i = 0; i < a.beam_samps; ++i) {
     double t = (double)i * sstep;
@@ -106,10 +109,12 @@ __global__ void density_kernel(const Args a, const double* xy, int n, double* ou
 
 cudaError_t launch_scan(const Args& a, cudaStream_t st) {
   const int n = a.n_poses * a.num_beams;
+  if (n <= 0) return cudaSuccess;        // no poses: nothing to scan (an empty grid is not a valid launch)
   scan_kernel<<<(n + 127) / 128, 128, 0, st>>>(a);
   return cudaGetLastError();
 }
 cudaError_t launch_density(const Args& a, const double* xy, int n, double* out, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
   density_kernel<<<(n + 255) / 256, 256, 0, st>>>(a, xy, n, out);
   return cudaGetLastError();
 }

@@ -6,6 +6,7 @@ import numpy as np
 import torch
 
 from . import load_ext
+from ..data.sampler import WIN_MAX, window_table
 from ..models.spec import MLPSpec
 
 FIRST = {"relu": 0, "sin_relu": 1}
@@ -145,7 +146,7 @@ class FusedMLP:
                                        device=self.grad_part.device)
         self.cross = [self._point_op(theta_x[e], self.grad_part_x[e]) for e in range(theta_x.shape[0])]
 
-    WIN_MAX = 64
+    WIN_MAX = WIN_MAX
 
     def _window_table(self):
         """Online problems: per-node tables of one period of the sliding-window stream
@@ -154,23 +155,7 @@ class FusedMLP:
         dsets = getattr(pr, "_datasets", None)
         if dsets is None or not hasattr(dsets[0], "schedule"):
             return None
-        K = self.WIN_MAX
-        tab = np.zeros((self.L, 2 + (K + 1) + 2 * K), dtype=np.int64)
-        for l, g in enumerate(pr.placement.local_nodes):
-            sch = dsets[g].schedule
-            wins = [sch.window(0)]
-            while True:
-                w = sch.window(len(wins))
-                if w == wins[0]:
-                    break
-                wins.append(w)
-                if len(wins) > K:
-                    raise RuntimeError("online window stream has more than 64 windows per period")
-            cum = np.concatenate([[0], np.cumsum([ub - lb for lb, ub, _ in wins])])
-            tab[l, 0], tab[l, 1] = len(wins), cum[-1]
-            tab[l, 2: 2 + len(cum)] = cum
-            tab[l, 2 + K + 1: 2 + K + 1 + len(wins)] = [w[0] for w in wins]
-            tab[l, 2 + 2 * K + 1: 2 + 2 * K + 1 + len(wins)] = [w[1] for w in wins]
+        tab = window_table([dsets[g].schedule for g in pr.placement.local_nodes], self.WIN_MAX)
         return torch.as_tensor(tab, device=pr.device)
 
     ema_in_kernel = False   # set by the consensus engine when its kernels maintain the loss EMA

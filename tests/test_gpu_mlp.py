@@ -153,23 +153,6 @@ def test_online_density_fused_training_tracks_torch_path(tmp_path):
     assert fused.forward_cnt == ref.forward_cnt
 
 
-def test_gpu_lidar_matches_cpu_scans(tmp_path):
-    """ops/csrc/lidar.cu (bicubic B-spline density + beam marching, fp64) vs the NumPy/scipy path."""
-    import os
-    import numpy as np
-    from nn_distributed_training_b200.floorplans.lidar import Lidar2D, interpolate_waypoints
-    from nn_distributed_training_b200.floorplans.synthetic import write_dataset
-    d = str(tmp_path)
-    write_dataset(d, n_paths=2, seed=1)
-    lidar = Lidar2D(os.path.join(d, "floor_img.png"), 20, 0.2, 25, 1.3, 50, 3, border_width=8)
-    wp = np.load(os.path.join(d, "tight_paths", "1.npy"))
-    traj = interpolate_waypoints(wp[:, 0], wp[:, 1], 6) * np.array([lidar.nx * 0.5, lidar.ny * 0.5])
-    cpu = lidar.scan_batch(traj)
-    gpu = lidar.scan_batch(traj, device=DEV)
-    assert gpu.shape == cpu.shape
-    np.testing.assert_allclose(gpu, cpu, rtol=0, atol=1e-7)
-
-
 # ---- generic CUDA-core MLP kernels (csrc/mlp_generic.cu): any widths <= 256, ReLU / Tanh / Sigmoid, fp32 / fp64 ---------
 @pytest.mark.parametrize("cls_name,shape,dtype,M", [
     ("FFReLUNet", [12, 64, 64, 64, 5], torch.float32, 2400),        # RL actor (reference RL/dist_rl/model.py)
