@@ -61,6 +61,12 @@ __host__ __device__ inline Layout layout(const int* dims, int nl, int tm, bool b
   return L;
 }
 
+NNDT_DEVINL float add_rn(float x, float y) { return __fadd_rn(x, y); }
+NNDT_DEVINL double add_rn(double x, double y) { return __dadd_rn(x, y); }
+NNDT_DEVINL float sub_rn(float x, float y) { return __fsub_rn(x, y); }
+NNDT_DEVINL double sub_rn(double x, double y) { return __dsub_rn(x, y); }
+NNDT_DEVINL float mul_rn(float x, float y) { return __fmul_rn(x, y); }
+NNDT_DEVINL double mul_rn(double x, double y) { return __dmul_rn(x, y); }
 template <typename T> NNDT_DEVINL T div_rn(T x, T y);
 template <> NNDT_DEVINL float div_rn(float x, float y) { return __fdiv_rn(x, y); }
 template <> NNDT_DEVINL double div_rn(double x, double y) { return __ddiv_rn(x, y); }
@@ -72,7 +78,7 @@ NNDT_DEVINL void zero_acc(T (&c)[2][4]) {
 }
 
 // One CTA = (chunk, network net0 + blockIdx.y, node blockIdx.z).  BWD = false is the advantage pass: critic forward
-// only, writing A = rtgs - V.
+// only, writing A = rtgs - V, or V itself for gae_kernel when GAE is requested.
 template <typename T, bool BWD>
 __global__ void __launch_bounds__(NT, 1) ppo_grad_kernel(const Args a, const int tm, const int chunks, const int net0,
                                                       const size_t gmax, double* gpart, double* lpart) {
@@ -175,7 +181,7 @@ __global__ void __launch_bounds__(NT, 1) ppo_grad_kernel(const Args a, const int
           const double e = (double)O[0] - (double)rtg;
           loss = e * e;
           if (BWD) O[0] = (T)(2.0 * e / (double)R);
-          else reinterpret_cast<T*>(a.adv)[r] = rtg - O[0];
+          else reinterpret_cast<T*>(a.adv)[r] = a.gae ? O[0] : rtg - O[0];
         }
       } else if (BWD) {
         for (int k = 0; k < L.P[nl]; ++k) O[k] = (T)0;   // rows past the chunk contribute nothing
@@ -315,6 +321,35 @@ __global__ void __launch_bounds__(NT) adv_norm_kernel(T* adv, const int R) {
   for (int r = threadIdx.x; r < R; r += NT) A[r] = div_rn<T>(A[r] - mt, den);
 }
 
+// GAE(lambda), one thread per (node, episode block, world): a backward scan over the block's T cycles,
+//   delta_c = r_c + gamma V_{c+1} - V_c,  A_c = delta_c + (gamma lam) A_{c+1},  G_c = A_c + V_c,  V_T = A_T = 0,
+// with V read from adv (the critic pass's output) and overwritten by A, and copied to `values` when given.  Every product and sum is rounded on its own
+// (no FMA contraction), in the order written, as the rewards-to-go scan of the rollout kernel is: the torch path's
+// elementwise ops give the same bits.  gl = gamma * lam is rounded in double, then to T, as torch rounds a Python
+// scalar.
+template <typename T>
+__global__ void __launch_bounds__(NT) gae_kernel(const T* rews, T* adv, T* returns, T* values, const int R,
+                                                 const int steps, const int E, const double gamma, const double gl,
+                                                 const int lanes) {
+  const int q = blockIdx.x * NT + threadIdx.x;   // (node, block, world) of the N * (R / (T * E)) * E scans
+  if (q >= lanes) return;
+  const int per = R / steps;                     // scans per node: (R / (T * E)) * E
+  const int node = q / per, k = q - node * per, blk = k / E, e = k - blk * E;
+  const size_t base = (size_t)node * R + (size_t)blk * steps * E + e;
+  const T g = (T)gamma, l = (T)gl;
+  T A = (T)0, vn = (T)0;
+  for (int c = steps - 1; c >= 0; --c) {
+    const size_t r = base + (size_t)c * E;
+    const T v = adv[r];
+    const T delta = sub_rn(add_rn(rews[r], mul_rn(g, vn)), v);
+    A = add_rn(delta, mul_rn(l, A));
+    adv[r] = A;
+    returns[r] = add_rn(A, v);
+    if (values) values[r] = v;
+    vn = v;
+  }
+}
+
 template <typename T>
 size_t gmax_of(const Args& a, int tm) {
   size_t gmax = 0;
@@ -388,6 +423,15 @@ cudaError_t advantages_t(const Args& a, const Plan& p, cudaStream_t st) {
   ppo_grad_kernel<T, false><<<dim3(p.chunks, 1, a.N), NT, p.smem, st>>>(a, p.tm, p.chunks, kCritic, 0, nullptr, nullptr);
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return e;
+  if (a.gae) {
+    const int lanes = a.N * (a.R / a.T);
+    gae_kernel<T><<<(lanes + NT - 1) / NT, NT, 0, st>>>(reinterpret_cast<const T*>(a.rews), reinterpret_cast<T*>(a.adv),
+                                                        reinterpret_cast<T*>(a.returns),
+                                                        reinterpret_cast<T*>(a.values), a.R, a.T, a.E, a.gamma,
+                                                        a.gamma * a.lam, lanes);
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return e;
+  }
   adv_norm_kernel<T><<<a.N, NT, 0, st>>>(reinterpret_cast<T*>(a.adv), a.R);
   return cudaGetLastError();
 }
@@ -407,6 +451,11 @@ const char* check(const Args& a, bool with_actor) {
   }
   if (a.dims[kCritic][a.nl[kCritic]] != 1) return "critic output width != 1";
   if (!a.obs || !a.rtgs || !a.adv) return "missing buffer";
+  if (a.gae) {
+    if (!a.rews || !a.returns) return "missing buffer";
+    if (a.T < 1 || a.E < 1 || a.R % a.T || (a.R / a.T) % a.E) return "GAE needs T * E to divide R";
+    if (!(a.gamma >= 0.0 && a.gamma <= 1.0) || !(a.lam >= 0.0 && a.lam <= 1.0)) return "GAE needs gamma and lam in [0, 1]";
+  }
   if (!with_actor) return nullptr;
   if (a.dims[kActor][0] != a.dims[kCritic][0]) return "actor and critic input widths differ";
   if (a.dims[kActor][a.nl[kActor]] != kActDim) return "actor output width != 5";

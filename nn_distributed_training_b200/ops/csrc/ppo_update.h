@@ -34,6 +34,14 @@ struct Args {
   double clip, cov_var, lp_const;  // lp = -0.5 |act - mean|^2 / cov_var - lp_const
   void* losses;                    // [N, 2]: actor, critic loss
   int* nonfinite;                  // set to 1 if an actor mean is not finite; never cleared
+  // GAE(lambda) of advantages() (gae != 0): per-cycle rewards rews [N, R] in the rollout's row order
+  // r = (blk * T + c) * E + e, with T * E dividing R; the lambda-returns A + V go to returns [N, R], raw A to adv
+  // before the normalisation.  gae == 0: none of these is read, and adv = normalised (rtgs - V).
+  int gae, T, E;
+  double gamma, lam;
+  const void* rews;
+  void* returns;
+  void* values;                    // optional [N, R]: the critic's V
 };
 
 // Rows per tile, chunks per node (CTAs per network), dynamic shared memory, accumulator slot size (doubles) and
@@ -51,7 +59,8 @@ const char* check(const Args& a, bool with_actor);
 Plan plan(const Args& a, bool backward);
 // grads(): losses and every gradient with p = plan(a, true); `work` holds p.work_bytes.
 cudaError_t grads(const Args& a, const Plan& p, void* work, cudaStream_t st);
-// advantages(): adv = normalised (rtgs - critic(obs)) per node.
+// advantages(): adv = normalised (rtgs - critic(obs)) per node; with a.gae, adv = normalised GAE(lambda) advantages
+// and returns = their lambda-returns.
 cudaError_t advantages(const Args& a, cudaStream_t st);
 
 }  // namespace ppo

@@ -51,7 +51,7 @@ tag::Args tag_args(const py::dict& d) {
   a.key = d["key"].cast<uint64_t>(); a.index = d["index"].cast<uint32_t>();
   a.obs = mptr(d, "obs"); a.acts = mptr(d, "acts"); a.log_probs = mptr(d, "log_probs"); a.rtgs = mptr(d, "rtgs");
   a.ep_returns = mptr(d, "ep_returns"); a.final_pos = mptr(d, "final_pos"); a.final_vel = mptr(d, "final_vel");
-  a.eps = mptr(d, "eps"); a.pos_trace = mptr(d, "pos_trace");
+  a.eps = mptr(d, "eps"); a.pos_trace = mptr(d, "pos_trace"); a.rews = mptr(d, "rews");
   return a;
 }
 
@@ -96,6 +96,12 @@ ppo::Args ppo_args(const py::dict& d) {
   a.clip = d["clip"].cast<double>(); a.cov_var = d["cov_var"].cast<double>(); a.lp_const = d["lp_const"].cast<double>();
   a.losses = mptr(d, "losses");
   a.nonfinite = reinterpret_cast<int*>(mptr(d, "nonfinite"));
+  if (d.contains("gae") && d["gae"].cast<bool>()) {   // GAE(lambda) of the advantage pass
+    a.gae = 1;
+    a.T = d["T"].cast<int>(); a.E = d["E"].cast<int>();
+    a.gamma = d["gamma"].cast<double>(); a.lam = d["lam"].cast<double>();
+    a.rews = cptr(d, "rews"); a.returns = mptr(d, "returns"); a.values = mptr(d, "values");
+  }
   return a;
 }
 }  // namespace

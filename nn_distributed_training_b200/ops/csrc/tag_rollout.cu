@@ -1,6 +1,6 @@
 // One launch = one whole multi-agent PPO rollout on the predator-prey environment (rl/simple_tag.py, rl/dist_ppo.py):
 // every episode of a batch, every cycle, every predator's actor MLP and Gaussian action, the heuristic prey, the contact
-// physics, the shared predator reward and finally the rewards-to-go.
+// physics, the shared predator reward (optionally stored per cycle for GAE) and finally the rewards-to-go.
 //
 // Decomposition: worlds (episode, env) are independent, so a CTA owns `wpb` of them for their whole life; the host picks
 // wpb so that even a 16-world batch spreads over 16 SMs.  Each distinct actor is staged once per CTA in shared memory,
@@ -321,7 +321,10 @@ __global__ void __launch_bounds__(NT) tag_rollout_kernel(const Args a, const int
       const T r = add_rn(mul_rn((T)-0.1, sum), mul_rn((T)10, (T)hits));
       ret_sum = add_rn(ret_sum, r);
       const int g = g0 + tid, ep = g / E, e = g - ep * E;
-      rtgs[((size_t)ep * T_ + c) * E + e] = r;   // predator 0's row holds the rewards until the episode ends
+      const size_t row = ((size_t)ep * T_ + c) * E + e;
+      rtgs[row] = r;   // predator 0's row holds the rewards until the episode ends
+      if (a.rews)   // read from the parameter bank here: a pointer kept live across the cycle loop spills
+        for (int i = 0; i < N; ++i) reinterpret_cast<T*>(a.rews)[(size_t)i * R + row] = r;
     }
   }
 

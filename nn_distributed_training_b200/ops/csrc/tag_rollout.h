@@ -40,6 +40,7 @@ struct Args {
   void* final_vel;         // [n_ep, E, A, 2]
   void* eps;               // optional [N, R, 5]
   void* pos_trace;         // optional [n_ep, T, E, A, 2], positions after each cycle
+  void* rews;              // optional [N, R], the shared predator reward of each cycle (before the rewards-to-go)
 };
 
 // Worlds per CTA, whether the actors are staged in shared memory, worlds per register block (the kernel's RW: 4 when

@@ -4,7 +4,9 @@ The torch path (``DistPPOProblem.evaluate`` / ``ev_ppo_loss`` and autograd, ``PP
 one host synchronisation per node per primal step.  Here
 
 * ``advantages(critics, obs, rtgs)`` is the critic forward over every node's samples and the per-node normalisation
-  ``(A - mean) / (std + 1e-10)`` of ``A = rtgs - V`` (two launches), and
+  ``(A - mean) / (std + 1e-10)`` of ``A = rtgs - V`` (two launches); with ``gae=GAE(...)`` ``A`` is the GAE(lambda)
+  advantage of the per-cycle rewards and the lambda-returns ``A + V`` come back as the critic's target (three
+  launches), and
 * ``grads(...)`` is one primal step of every node: forward, PPO-clip actor loss, critic MSE and both backward passes,
   written straight into the caller's gradient tensors (two launches, no synchronisation).
 
@@ -14,7 +16,8 @@ The batch layout is the rollout kernel's: node ``i``'s samples are row ``i`` of 
 from __future__ import annotations
 
 import math
-from typing import Dict, List, Optional, Sequence
+from dataclasses import dataclass
+from typing import Dict, List, Optional, Sequence, Tuple, Union
 
 import torch
 from torch import nn
@@ -114,10 +117,32 @@ def _batch(name, t, shape, dtype, dev):
     return t.contiguous()
 
 
-def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+@dataclass
+class GAE:
+    """Generalized advantage estimation for ``advantages``: ``rews [N, R]`` the per-cycle rewards in the batch's row
+    order ``r = (blk * T + c) * E + e`` (``T`` cycles of ``E`` worlds per block, ``T * E`` dividing ``R``; each block
+    ends in a terminal step), discount ``gamma`` and ``lam`` in [0, 1].  ``returns``: an optional contiguous
+    ``[N, R]`` output for the lambda-returns; ``values``: an optional one the critic's ``V`` is copied into (the
+    baseline the advantages subtract, for diagnostics such as the explained variance)."""
+    rews: torch.Tensor
+    gamma: float
+    lam: float
+    T: int
+    E: int
+    returns: Optional[torch.Tensor] = None
+    values: Optional[torch.Tensor] = None
+
+
+def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor, out: Optional[torch.Tensor] = None, *,
+               gae: Optional[Union[GAE, dict]] = None) -> Union[torch.Tensor, Tuple[torch.Tensor, torch.Tensor]]:
     """``[N, R]`` normalised advantages ``(A - mean) / (std + 1e-10)`` of ``A = rtgs - critic_i(obs[i])``, with node
     ``i``'s mean and unbiased std (so NaN for R = 1, as torch's ``std``).  ``critics``: one per node.  ``out``: a
-    contiguous ``[N, R]`` tensor of the batch dtype to write them into (returned)."""
+    contiguous ``[N, R]`` tensor of the batch dtype to write them into (returned).
+
+    ``gae``: a ``GAE`` (or a dict of its fields).  Then ``A`` is the GAE(lambda) advantage of ``gae.rews`` within each
+    (episode block, world), ``delta_c = r_c + gamma V_{c+1} - V_c`` and ``A_c = delta_c + gamma lam A_{c+1}`` with
+    ``V_T = A_T = 0``, and the call returns ``(adv, returns)``: ``returns = A + V`` is the critic's target, written into
+    ``gae.returns`` when given.  ``rtgs`` then does not enter the result."""
     crits = _as_list(critics)
     require(None, crits)
     ext = load_ext(required=True)
@@ -130,9 +155,21 @@ def advantages(critics, obs: torch.Tensor, rtgs: torch.Tensor, out: Optional[tor
     rtgs = rtgs.contiguous()
     adv = torch.empty(N, R, device=dev, dtype=dt) if out is None else _out("out", out, (N, R), dt, dev)
     d.update(obs=obs.data_ptr(), rtgs=rtgs.data_ptr(), adv=adv.data_ptr())
+    if gae is not None:
+        g = GAE(**gae) if isinstance(gae, dict) else gae
+        T, E, gamma, lam = int(g.T), int(g.E), float(g.gamma), float(g.lam)
+        if T < 1 or E < 1 or R % (T * E):
+            raise ValueError(f"gae: T * E = {T} * {E} must divide R = {R}")
+        if not (0.0 <= gamma <= 1.0 and 0.0 <= lam <= 1.0):
+            raise ValueError(f"gae: gamma {gamma} and lam {lam} must lie in [0, 1]")
+        rews = _batch("gae.rews", g.rews, (N, R), dt, dev)
+        ret = torch.empty(N, R, device=dev, dtype=dt) if g.returns is None \
+            else _out("gae.returns", g.returns, (N, R), dt, dev)
+        vals = None if g.values is None else _out("gae.values", g.values, (N, R), dt, dev).data_ptr()
+        d.update(gae=True, T=T, E=E, gamma=gamma, lam=lam, rews=rews.data_ptr(), returns=ret.data_ptr(), values=vals)
     with torch.cuda.device(dev):
         ext.ppo_advantages(d)
-    return adv
+    return adv if gae is None else (adv, ret)
 
 
 def launch_plan(actors, critics, R: int, backward: bool = True) -> Dict[str, int]:

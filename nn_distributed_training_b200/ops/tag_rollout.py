@@ -166,12 +166,13 @@ def launch_plan(env, actors, T: int, n_ep: int) -> Dict[str, int]:
 
 def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_scale: float = 1.0, key: int = 0,
             index: int = 0, pos0: Optional[torch.Tensor] = None, debug: bool = False,
-            out: Optional[Dict[str, torch.Tensor]] = None) -> Dict[str, torch.Tensor]:
+            out: Optional[Dict[str, torch.Tensor]] = None, rews: bool = False) -> Dict[str, torch.Tensor]:
     """Run ``n_ep`` episodes of ``T`` cycles in ``env.E`` worlds each.  ``actors``: one module shared by every predator,
     or one per predator.  ``pos0`` defaults to ``reset_positions(env, n_ep)``.  Returns ``obs``, ``acts``,
     ``log_probs``, ``rtgs``, ``ep_returns`` and every world's final ``final_pos`` / ``final_vel [n_ep, E, A, 2]``;
     ``debug`` adds the standard-normal draws ``eps [N, R, 5]`` and the positions after every cycle
-    ``pos [n_ep, T, E, A, 2]``.  ``out``: contiguous tensors of the batch's shapes, dtype and device to write any of
+    ``pos [n_ep, T, E, A, 2]``.  ``rews`` adds the shared predator reward of every cycle, ``rews [N, R]`` in the batch
+    layout (what generalized advantage estimation needs); ``rtgs`` is its rewards-to-go.  ``out``: contiguous tensors of the batch's shapes, dtype and device to write any of
     these into (persistent buffers); the returned dict holds them.  Afterwards ``env`` holds the last episode's final
     state, as after the torch loop (a copy, when ``out`` holds ``final_pos`` / ``final_vel``)."""
     T, n_ep = int(T), int(n_ep)
@@ -192,6 +193,8 @@ def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_
                   final_pos=(n_ep, E, A, 2), final_vel=(n_ep, E, A, 2))
     if debug:
         shapes.update(eps=(N, R, ACT_DIM), pos=(n_ep, T, E, A, 2))
+    if rews:
+        shapes.update(rews=(N, R))
     given = out or {}
     for k, t in given.items():
         if k not in shapes or not torch.is_tensor(t) or tuple(t.shape) != shapes[k] or t.dtype != dt \
@@ -199,8 +202,8 @@ def rollout(env, actors, T: int, n_ep: int, gamma: float, cov_var: float, noise_
             raise ValueError(f"out[{k!r}]: expected a contiguous {shapes.get(k)} {dt} tensor on {dev}")
     out = {k: given[k] if k in given else torch.empty(*shp, device=dev, dtype=dt) for k, shp in shapes.items()}
     d.update(pos0=pos0.data_ptr(), eps=out["eps"].data_ptr() if debug else None,
-             pos_trace=out["pos"].data_ptr() if debug else None,
-             **{k: v.data_ptr() for k, v in out.items() if k not in ("eps", "pos")})
+             pos_trace=out["pos"].data_ptr() if debug else None, rews=out["rews"].data_ptr() if rews else None,
+             **{k: v.data_ptr() for k, v in out.items() if k not in ("eps", "pos", "rews")})
     with torch.cuda.device(dev):
         ext.tag_rollout(d)
     # the environment keeps its own copy of a caller's persistent buffer, which the next rollout into it overwrites

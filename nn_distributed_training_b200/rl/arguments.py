@@ -17,4 +17,5 @@ def get_args(argv=None):
     p.add_argument("--ID", type=int, default=0)
     p.add_argument("--save_freq", type=int, default=10)
     p.add_argument("--seed", type=int, default=None)
+    p.add_argument("--gae_lambda", type=float, default=None)  # GAE(lambda) advantages, lambda in [0, 1]
     return p.parse_args(argv)

@@ -18,11 +18,13 @@ import numpy as np
 import torch
 from torch import nn
 
+from .gae import check_gae_lambda, gae
 from .model import ActorCritic
 from .simple_tag import SimpleTagEnv, heuristic_prey_action
 
 
 BATCH_KEYS = ("obs", "acts", "log_probs", "rtgs")
+GAE_KEYS = BATCH_KEYS + ("rews",)   # the batch under gae_lambda: the per-cycle rewards too
 
 
 class DistPPOProblem:
@@ -31,15 +33,18 @@ class DistPPOProblem:
     # update_backend "cuda": advantages and every node's gradients per primal step are fused kernels (ops/ppo_update.py);
     # a non-finite actor mean then raises from check_update(), which the trainers call at the end of every iteration,
     # and at the latest from the next update_advantage() -- not inside the primal step as on the torch path
+    # gae_lambda: None keeps the Monte-Carlo advantages rtgs - V and the critic target rtgs; a float in [0, 1] makes
+    # them GAE(lambda) advantages and lambda-returns (rl/gae.py), on both update backends
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
                     lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
-                    rollout_backend="torch", update_backend="torch")
+                    rollout_backend="torch", update_backend="torch", gae_lambda=None)
 
     def __init__(self, base_actor, base_critic, graph, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
             if k not in self.DEFAULTS:
                 raise TypeError(f"unknown PPO hyper-parameter {k!r}")
             setattr(self, k, v)
+        self.gae_lambda = check_gae_lambda(self.gae_lambda)
         if self.seed is not None:
             assert isinstance(self.seed, int)
             torch.manual_seed(self.seed)
@@ -90,9 +95,14 @@ class DistPPOProblem:
         the consensus rounds around it can be captured in a CUDA graph and replayed (``ReferenceProblemAdapter``)."""
         return self.fixed_batch and self.batched_grads is not None
 
+    @property
+    def batch_keys(self):
+        return BATCH_KEYS if self.gae_lambda is None else GAE_KEYS
+
     def use_fixed_batch(self, steps_per_iteration: int):
         """Fused-consensus mode of the trainers: from the next batch on, ``obs`` / ``acts`` / ``log_probs`` / ``rtgs``
-        and the advantages live in persistent ``[N, R, ...]`` buffers (reallocated, with ``batch_version`` bumped, only
+        (and, under ``gae_lambda``, ``rews`` and the lambda-returns) and the advantages live in persistent
+        ``[N, R, ...]`` buffers (reallocated, with ``batch_version`` bumped, only
         when R changes) and each primal step's ``[N, 2]`` losses go to row ``s`` of ``step_losses [steps_per_iteration,
         N, 2]``, s counted from ``begin_steps()``; ``end_steps()`` then logs them.  ``curr_*[i]`` / ``A_k[i]`` stay views of
         row i."""
@@ -105,12 +115,14 @@ class DistPPOProblem:
             self.step_losses = torch.zeros(int(steps_per_iteration), self.N, 2, device=p.device, dtype=p.dtype)
 
     def _into_buffers(self, out):
-        b = self._bufs
-        if b is None or any(b[k].shape != out[k].shape or b[k].dtype != out[k].dtype for k in BATCH_KEYS):
-            b = self._bufs = {k: torch.empty(out[k].shape, dtype=out[k].dtype, device=out[k].device) for k in BATCH_KEYS}
+        b, keys = self._bufs, self.batch_keys
+        if b is None or any(b[k].shape != out[k].shape or b[k].dtype != out[k].dtype for k in keys):
+            b = self._bufs = {k: torch.empty(out[k].shape, dtype=out[k].dtype, device=out[k].device) for k in keys}
             b["adv"] = torch.empty(out["rtgs"].shape, dtype=out["rtgs"].dtype, device=out["rtgs"].device)
+            if self.gae_lambda is not None:
+                b["returns"] = torch.empty_like(b["adv"])
             self.batch_version += 1
-        for k in BATCH_KEYS:
+        for k in keys:
             if out[k] is not b[k]:
                 b[k].copy_(out[k])
         return b
@@ -165,7 +177,7 @@ class DistPPOProblem:
         env, N = self.env, self.N
         cycles = max(1, self.max_timesteps_per_episode // env.num_agents)
         obs_b = [[] for _ in range(N)]; act_b = [[] for _ in range(N)]
-        lp_b = [[] for _ in range(N)]; rtg_b = [[] for _ in range(N)]
+        lp_b = [[] for _ in range(N)]; rtg_b = [[] for _ in range(N)]; rew_b = [[] for _ in range(N)]
         ep_returns, ep_lens, t = [], [], 0
         while t < self.timesteps_per_batch:
             obs_adv, obs_good = env.reset()
@@ -191,6 +203,7 @@ class DistPPOProblem:
                 rtg[s] = run
             for i in range(N):
                 rtg_b[i].append(rtg[:, :, i])
+                rew_b[i].append(R[:, :, i])
             ep_returns.extend(R.sum(0).sum(-1).tolist())            # joint predator return per world
             ep_lens.extend([R.shape[0] * env.num_agents] * env.E)
         flat = lambda xs: torch.cat([x.reshape(-1, *x.shape[2:]) if x.dim() > 2 else x.reshape(-1) for x in xs])
@@ -198,11 +211,15 @@ class DistPPOProblem:
         self.curr_acts = {i: torch.cat(act_b[i]) for i in range(N)}
         self.curr_log_probs = {i: torch.cat(lp_b[i]) for i in range(N)}
         self.curr_rtgs = {i: torch.cat([r.reshape(-1) for r in rtg_b[i]]) for i in range(N)}
+        if self.gae_lambda is not None:
+            self.curr_rews = {i: torch.cat([r.reshape(-1) for r in rew_b[i]]) for i in range(N)}
+            lens = {r.shape[0] for r in rew_b[0]}
+            if len(lens) != 1:   # every episode runs min(cycles, max_cycles) cycles from a reset
+                raise RuntimeError(f"GAE needs episodes of one length, got {sorted(lens)}")
+            self._episode_T = lens.pop()
         if self.update_backend == "cuda":
-            self._stack_batch(dict(obs=torch.stack([self.curr_obs[i] for i in range(N)]),
-                                   acts=torch.stack([self.curr_acts[i] for i in range(N)]),
-                                   log_probs=torch.stack([self.curr_log_probs[i] for i in range(N)]),
-                                   rtgs=torch.stack([self.curr_rtgs[i] for i in range(N)])))
+            self._stack_batch({k: torch.stack([getattr(self, "curr_" + k)[i] for i in range(N)])
+                               for k in self.batch_keys})
         self.logger["batch_rews"] = ep_returns
         self.logger["batch_lens"] = ep_lens
         self.logger["t_so_far"] += int(np.sum(ep_lens))
@@ -217,10 +234,13 @@ class DistPPOProblem:
         if self._rollout_key is None:
             self._rollout_key = tag_rollout.draw_key()
         b, R = getattr(self, "_bufs", None), n_ep * T * env.E
-        into = {k: b[k] for k in BATCH_KEYS} if self.fixed_batch and b is not None and b["rtgs"].shape == (N, R) else None
+        into = {k: b[k] for k in self.batch_keys} if self.fixed_batch and b is not None and b["rtgs"].shape == (N, R) \
+            else None
         out = tag_rollout.rollout(env, self.actors, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
-                                  key=self._rollout_key, index=self._rollout_index, out=into)
+                                  key=self._rollout_key, index=self._rollout_index, out=into,
+                                  rews=self.gae_lambda is not None)
         self._rollout_index += 1
+        self._episode_T = T
         self._stack_batch(out)
         ep_lens = [T * env.num_agents] * (n_ep * env.E)
         self.logger["batch_rews"] = out["ep_returns"].tolist()
@@ -232,11 +252,13 @@ class DistPPOProblem:
         """Keep the batch as ``[N, R, ...]`` tensors (the update kernels' layout); ``curr_*[i]`` are views of row i."""
         if self.fixed_batch:
             out = self._into_buffers(out)
-        self._batch = {k: out[k] for k in BATCH_KEYS}
+        self._batch = {k: out[k] for k in self.batch_keys}
         self.curr_obs = {i: out["obs"][i] for i in range(self.N)}
         self.curr_acts = {i: out["acts"][i] for i in range(self.N)}
         self.curr_log_probs = {i: out["log_probs"][i] for i in range(self.N)}
         self.curr_rtgs = {i: out["rtgs"][i] for i in range(self.N)}
+        if self.gae_lambda is not None:
+            self.curr_rews = {i: out["rews"][i] for i in range(self.N)}
 
     def compute_rtgs(self, batch_rews):
         out = []
@@ -248,19 +270,39 @@ class DistPPOProblem:
         return torch.tensor(out, dtype=torch.float)
 
     def update_advantage(self):
+        """Per-node normalised advantages ``A_k`` of the critics at the start of the iteration, and the critic targets:
+        ``rtgs - V`` and ``rtgs``, or under ``gae_lambda`` the GAE(lambda) advantages and lambda-returns of each
+        episode of the batch (``curr_returns``)."""
         if self.update_backend == "cuda":
             from ..ops import ppo_update
             self.check_update()   # the previous iteration's steps, if the driver did not check them
-            self._adv = ppo_update.advantages(self.critics, self._batch["obs"], self._batch["rtgs"],
-                                              out=self._bufs["adv"] if self.fixed_batch else None)
+            b, bufs = self._batch, self._bufs if self.fixed_batch else None
+            out = bufs["adv"] if bufs is not None else None
+            if self.gae_lambda is None:
+                self._adv = ppo_update.advantages(self.critics, b["obs"], b["rtgs"], out=out)
+            else:
+                g = ppo_update.GAE(rews=b["rews"], gamma=self.gamma, lam=self.gae_lambda, T=self._episode_T,
+                                   E=self.env.E, returns=bufs["returns"] if bufs is not None else None)
+                self._adv, self._returns = ppo_update.advantages(self.critics, b["obs"], b["rtgs"], out=out, gae=g)
+                self.curr_returns = {i: self._returns[i] for i in range(self.N)}
             self.A_k = {i: self._adv[i] for i in range(self.N)}
             return
         self.A_k = {}
+        if self.gae_lambda is not None:
+            self.curr_returns = {}
         with torch.no_grad():
             for i in range(self.N):
                 V, _ = self.evaluate(i)
-                A = self.curr_rtgs[i] - V                             # ALG STEP 5
+                if self.gae_lambda is None:
+                    A = self.curr_rtgs[i] - V                         # ALG STEP 5
+                else:
+                    A, self.curr_returns[i] = gae(self.curr_rews[i], V, self.gamma, self.gae_lambda,
+                                                  self._episode_T, self.env.E)
                 self.A_k[i] = (A - A.mean()) / (A.std() + 1e-10)
+
+    def critic_target(self, i):
+        """Node i's critic target: the rewards-to-go, or the lambda-returns under ``gae_lambda``."""
+        return self.curr_rtgs[i] if self.gae_lambda is None else self.curr_returns[i]
 
     # ---- losses ---------------------------------------------------------------------------
     def ev_ppo_loss(self, i):
@@ -269,7 +311,7 @@ class DistPPOProblem:
         surr1 = ratios * self.A_k[i]
         surr2 = torch.clamp(ratios, 1 - self.clip, 1 + self.clip) * self.A_k[i]
         actor_loss = (-torch.min(surr1, surr2)).mean()
-        critic_loss = nn.functional.mse_loss(V, self.curr_rtgs[i])
+        critic_loss = nn.functional.mse_loss(V, self.critic_target(i))
         self.logger["actor_losses"].append(actor_loss.detach())
         return actor_loss, critic_loss
 
@@ -284,18 +326,19 @@ class DistPPOProblem:
         tensor per parameter of models[i]) and returns the per-node losses ``[N, 2]`` without a host synchronisation."""
         from ..ops import ppo_update
         b = self._batch
+        target = b["rtgs"] if self.gae_lambda is None else self._returns   # a persistent buffer under fixed_batch
         if self.fixed_batch:     # fused consensus: replayable, the trainer logs step_losses after the iteration
             slot = self._loss_step % self.step_losses.shape[0]
             self._loss_step += 1
-            losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], b["rtgs"],
+            losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], target,
                                       self._adv, self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite,
                                       losses_out=self.step_losses[slot])
             self._checked = False
             if not self._in_steps:   # a step outside the trainer's iteration (DSGT's init_grads): logged as it runs
                 self.logger["actor_losses"].extend(losses.clone()[:, 0])
             return losses
-        losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], b["rtgs"], self._adv,
-                                  self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite)
+        losses = ppo_update.grads(self.actors, self.critics, b["obs"], b["acts"], b["log_probs"], target,
+                                  self._adv, self.clip, self.cov_var, grad_out, nonfinite=self._nonfinite)
         self.logger["actor_losses"].extend(losses[i, 0] for i in range(self.N))
         self._checked = False
         return losses

@@ -47,7 +47,7 @@ def main(argv=None):
     hyper = {"timesteps_per_batch": 2000, "max_timesteps_per_episode": 200, "gamma": 0.99,
              "n_updates_per_iteration": 10, "lr": 3e-4, "clip": 0.2, "out_dir": args.out_dir, "ID": args.ID,
              "save_freq": args.save_freq, "seed": args.seed, "rollout_backend": args.rollout,
-             "update_backend": args.update}
+             "update_backend": args.update, "gae_lambda": args.gae_lambda}
     env = make_env(args.num_envs, 200, args.device)
     if args.mode == "train":
         train(env, hyper, args.actor_model, args.critic_model, args.total_timesteps)

@@ -11,19 +11,24 @@ import torch
 from torch import nn
 from torch.optim import Adam
 
+from .gae import check_gae_lambda, gae
 from .simple_tag import SimpleTagEnv, heuristic_prey_action
 
 
 class PPO:
+    # gae_lambda: None keeps the Monte-Carlo advantages rtgs - V and the critic target rtgs; a float in [0, 1] makes
+    # them GAE(lambda) advantages and lambda-returns (rl/gae.py), on both update backends.  A batch's samples are
+    # rows ((ep * T + c) * E + e) * n_adv + i, so each episode is T cycles of E * n_adv (world, predator) columns.
     DEFAULTS = dict(timesteps_per_batch=4800, max_timesteps_per_episode=1600, n_updates_per_iteration=5,
                     lr=0.005, gamma=0.95, clip=0.2, render=False, render_every_i=10, save_freq=10, seed=None,
-                    ID=0, out_dir="./trained", rollout_backend="torch", update_backend="torch")
+                    ID=0, out_dir="./trained", rollout_backend="torch", update_backend="torch", gae_lambda=None)
 
     def __init__(self, policy_class, env: SimpleTagEnv, **hyperparameters):
         for k, v in {**self.DEFAULTS, **hyperparameters}.items():
             if k not in self.DEFAULTS:
                 raise TypeError(f"unknown PPO hyper-parameter {k!r}")
             setattr(self, k, v)
+        self.gae_lambda = check_gae_lambda(self.gae_lambda)
         if self.seed is not None:
             torch.manual_seed(self.seed)
         self.env = env
@@ -63,11 +68,14 @@ class PPO:
         return self.critic(obs).squeeze(-1), self._log_prob(self.actor(obs), acts)
 
     def rollout(self):
+        """One batch: ``(obs, acts, log_probs, rtgs, episode lengths)``, one row per (cycle, world, predator).  Under
+        ``gae_lambda`` the per-cycle rewards of those rows and the episodes' cycle count are kept as ``self.rews`` and
+        ``self.episode_T`` for the update."""
         if self.rollout_backend == "cuda":
             return self._rollout_cuda()
         env = self.env
         cycles = max(1, self.max_timesteps_per_episode // env.num_agents)
-        obs_b, act_b, lp_b, rtg_b, ep_ret, ep_len, t = [], [], [], [], [], [], 0
+        obs_b, act_b, lp_b, rtg_b, rew_b, ep_ret, ep_len, t = [], [], [], [], [], [], [], 0
         while t < self.timesteps_per_batch:
             obs_adv, obs_good = env.reset()
             rews = []
@@ -90,8 +98,14 @@ class PPO:
                 run = R[s] + self.gamma * run
                 rtg[s] = run
             rtg_b.append(rtg.reshape(-1))
+            rew_b.append(R)
             ep_ret.extend(R.sum(0).sum(-1).tolist()); ep_len.extend([R.shape[0] * env.num_agents] * env.E)
         self.logger["batch_rews"], self.logger["batch_lens"] = ep_ret, ep_len
+        if self.gae_lambda is not None:
+            lens = {r.shape[0] for r in rew_b}
+            if len(lens) != 1:   # every episode runs min(cycles, max_cycles) cycles from a reset
+                raise RuntimeError(f"GAE needs episodes of one length, got {sorted(lens)}")
+            self.rews, self.episode_T = torch.cat([r.reshape(-1) for r in rew_b]), lens.pop()
         return torch.cat(obs_b), torch.cat(act_b), torch.cat(lp_b), torch.cat(rtg_b), ep_len
 
     def _rollout_cuda(self):
@@ -104,9 +118,11 @@ class PPO:
         if self._rollout_key is None:
             self._rollout_key = tag_rollout.draw_key()
         out = tag_rollout.rollout(env, self.actor, T=T, n_ep=n_ep, gamma=self.gamma, cov_var=self.cov_var,
-                                  key=self._rollout_key, index=self._rollout_index)
+                                  key=self._rollout_key, index=self._rollout_index, rews=self.gae_lambda is not None)
         self._rollout_index += 1
         flat = lambda x: x.transpose(0, 1).reshape(-1, *x.shape[2:])      # [N, R, ...] -> [R * N, ...]
+        if self.gae_lambda is not None:
+            self.rews, self.episode_T = flat(out["rews"]), T
         ep_len = [T * env.num_agents] * (n_ep * env.E)
         self.logger["batch_rews"], self.logger["batch_lens"] = out["ep_returns"].tolist(), ep_len
         return flat(out["obs"]), flat(out["acts"]), flat(out["log_probs"]), flat(out["rtgs"]), ep_len
@@ -131,11 +147,19 @@ class PPO:
             if self.render and i_so_far % self.render_every_i == 0:
                 self.render_episode(i_so_far)
 
-    def _update_torch(self, obs, acts, lps, rtgs):
+    def _advantages_torch(self, obs, acts, rtgs):
+        """Normalised advantages and the critic target of one batch on the torch update path: ``rtgs - V`` and
+        ``rtgs``, or under ``gae_lambda`` the GAE(lambda) advantages and lambda-returns."""
         with torch.no_grad():
             V, _ = self.evaluate(obs, acts)
-        A = rtgs - V
-        A = (A - A.mean()) / (A.std() + 1e-10)
+        if self.gae_lambda is None:
+            A = rtgs - V
+        else:
+            A, rtgs = gae(self.rews, V, self.gamma, self.gae_lambda, self.episode_T, self.env.E * self.env.n_adv)
+        return (A - A.mean()) / (A.std() + 1e-10), rtgs
+
+    def _update_torch(self, obs, acts, lps, rtgs):
+        A, rtgs = self._advantages_torch(obs, acts, rtgs)
         for _ in range(self.n_updates_per_iteration):
             V, cur = self.evaluate(obs, acts)
             ratios = torch.exp(cur - lps)
@@ -150,7 +174,12 @@ class PPO:
         layout; each step's gradients land in p.grad and the two Adam steps run as on the torch path."""
         from ..ops import ppo_update
         obs, acts, lps, rtgs = obs.unsqueeze(0), acts.unsqueeze(0), lps.unsqueeze(0), rtgs.unsqueeze(0)
-        A = ppo_update.advantages(self.critic, obs, rtgs)
+        if self.gae_lambda is None:
+            A = ppo_update.advantages(self.critic, obs, rtgs)
+        else:   # the critic's target becomes the lambda-return
+            g = ppo_update.GAE(rews=self.rews.unsqueeze(0), gamma=self.gamma, lam=self.gae_lambda, T=self.episode_T,
+                               E=self.env.E * self.env.n_adv)
+            A, rtgs = ppo_update.advantages(self.critic, obs, rtgs, gae=g)
         params = list(self.actor.parameters()) + list(self.critic.parameters())
         for _ in range(self.n_updates_per_iteration):
             for p in params:

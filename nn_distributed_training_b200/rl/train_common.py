@@ -30,6 +30,9 @@ def parse_args(argv=None, default_id=0):
     ap.add_argument("--render", action="store_true", help="write an episode GIF every --render_every_i iterations")
     ap.add_argument("--render_every_i", type=int, default=10)
     ap.add_argument("--seed", type=int, default=None)
+    ap.add_argument("--gae_lambda", type=float, default=None,
+                    help="GAE(lambda) advantages and lambda-return critic targets, lambda in [0, 1] (default: "
+                         "Monte-Carlo rewards-to-go)")
     ap.add_argument("--no_writeout", action="store_true")
     return ap.parse_args(argv)
 
@@ -42,7 +45,7 @@ def make_problem(args):
     hyper = {"timesteps_per_batch": 2000, "max_timesteps_per_episode": STEPS_PER_EPISODE, "gamma": 0.99,
              "n_updates_per_iteration": 5, "lr": 3e-4, "clip": 0.2, "render": bool(args.render),
              "render_every_i": args.render_every_i, "save_freq": args.save_freq, "seed": args.seed,
-             "rollout_backend": args.rollout, "update_backend": args.update}
+             "rollout_backend": args.rollout, "update_backend": args.update, "gae_lambda": args.gae_lambda}
     obs_dim = env.observation_spaces["adversary_0"].shape[0]
     act_dim = env.action_spaces["adversary_0"].shape[0]
     base_actor = FFReLUNet([obs_dim, 64, 64, 64, act_dim])
